@@ -6,7 +6,9 @@ A step = one pass of the reference's timed region ("Batch-Time": after EncryptLa
 conv 5x5/2 (845 outputs) -> square -> dense 845->100 -> square -> dense 100->10, P plaintext moduli (default 2, the
 reference's configuration, `CryptoNets.cs:17`).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--plain-moduli 1|2]      B200 arm (one process per GPU under torchrun)
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--plain-moduli 1|2]      GPU arm (one process per GPU under torchrun)
+        [--dump-outputs DIR]: after the timed steps, write what the last one computed (decrypted scores and a fixed sample of the score
+        ciphertext words) as DIR/*.npy, so that two builds can be compared output for output on identical, seeded inputs.
   python bench.py --impl reference ...                                          CPU arm: the in-repo C++ oracle (the
         reference's C#/SEAL path cannot be built here) on all host cores, each step a bounded sample of the same workload.
 
@@ -20,6 +22,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -37,11 +40,11 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0}, "fallback"
+        return {"hbm_gbs": 3350.0}, "data-sheet (H100 SXM HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks and throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks and throttle reasons during the timed region."""
 
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -67,11 +70,36 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait()
         sm = [float(r[0]) for r in self.rows if r and r[0].replace(".", "").isdigit()]
         mx = [float(r[1]) for r in self.rows if len(r) > 1 and r[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = sorted({names[i] for r in self.rows if len(r) >= 6 for i in range(4) if r[2 + i].lower().startswith("active")})
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons, "samples": len(sm)}
+
+
+def device_info(index):
+    """Name, power limit and maximum SM clock of the GPU the numbers were measured on: they are part of every absolute number."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+        return {"name": out[0], "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except Exception:
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "sm_max_mhz": None}
+
+
+def dump_outputs(directory, eng, out_matrix):
+    """What the timed path returned in its last step: the score ciphertexts, decrypted (float64 [10][8192]: one row per class, one column
+    per image), and a fixed, seeded sample of their words (8192 words per ciphertext and plaintext modulus, each word split into its high
+    and low 32 bits so that float64 holds it exactly)."""
+    os.makedirs(directory, exist_ok=True)
+    vecs = [v.vec for v in out_matrix.vectors]
+    np.save(os.path.join(directory, "scores.npy"), eng.decrypt_many(vecs).astype(np.float64))
+    idx = np.sort(np.random.default_rng(0).choice(eng.ct_words, 8192, replace=False))
+    words = np.stack([np.stack([v.export_raw(ch, 0)[idx] for ch in range(eng.P)]) for v in vecs])  # [10][P][8192] uint64
+    np.save(os.path.join(directory, "score_ciphertext_words_hi32.npy"), (words >> np.uint64(32)).astype(np.float64))
+    np.save(os.path.join(directory, "score_ciphertext_words_lo32.npy"), (words & np.uint64(0xFFFFFFFF)).astype(np.float64))
 
 
 # --------------------------------------------------------------------------------------------------------- CPU arm
@@ -241,16 +269,15 @@ def run_reference(args):
 
 
 def quiesce_python_gc():
-    """The cyclic collector's generation-2 pass walks the whole heap that torch, numpy and the network leave behind: 30-35 ms on the GPU
-    box, about once every nine CryptoNets batches -- longer than a batch of device time, so the GPU ran dry behind it
-    (profiles/r02_e2e_gc.txt).  Everything allocated during set-up is parked in the permanent generation; what the steps allocate is
-    still collected (young generations), a full pass now has almost nothing to walk."""
+    """The cyclic collector's generation-2 pass walks the whole heap that torch, numpy and the network leave behind, and can take longer
+    than a batch of device time, so the GPU would run dry behind it.  Everything allocated during set-up is parked in the permanent
+    generation; what the steps allocate is still collected (young generations), a full pass now has almost nothing to walk."""
     gc.collect()
     gc.freeze()
     return "gc.freeze() after set-up"
 
 
-# --------------------------------------------------------------------------------------------------------- B200 arm
+# --------------------------------------------------------------------------------------------------------- GPU arm
 def build_network(factory):
     """The CryptoNets-MNIST layer chain without its reader/encrypt layers (those sit before the timer)."""
     from cryptonets_b200.layers import PoolLayer, SquareActivation
@@ -351,6 +378,8 @@ def run_b200(args):
     ms = eng.timer_stop_ms()
     gatherer.finish()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, last)
     prof = eng.prof_collect()
     eng.prof_enable(False)
     launches = eng.launch_count() - launches0
@@ -433,16 +462,11 @@ def run_b200(args):
         fam = prof["ntt_forward"]
         # dominant family: forward NTT (incl. the digit-decomposing variant of relinearisation)
         achieved = fam["bytes"] / (fam["ms"] * 1e-3) / 1e9 if fam["ms"] > 0 else 0.0
-        # the forward transform is limited by FP64 issue (8 DP instructions per butterfly: 100 % of the pipe = 0.85 of this HBM figure), not by
-        # HBM itself; it is reported against the measured HBM copy bandwidth because that is the roofline SURVEY.md 8d prescribes
-        roof = {"bound": "hbm", "limited_by": "fp64-issue (ncu: 63 % of the FP64 pipe busy, math_pipe_throttle the top stall; 100 % of the pipe would be 0.85 of this HBM figure)", "kernel": "k_ntt_forward_fp / k_ntt_forward_digits_fp (N=8192), 16*N algorithmic bytes per transform", "achieved": achieved,
+        # the forward transform does 8 FP64 instructions per butterfly, so it may be limited by FP64 issue rather than by HBM itself; it is
+        # reported against the HBM bandwidth because that is the roofline SURVEY.md 8d prescribes
+        roof = {"bound": "hbm", "limited_by": "not profiled", "kernel": "k_ntt_forward_fp / k_ntt_forward_digits_fp (N=8192), 16*N algorithmic bytes per transform", "achieved": achieved,
                 "peak": peaks["hbm_gbs"],
-                "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"], "peak_source": peak_kind + " copy bandwidth (MEASURED_PEAKS.json)",
-                # ncu (profiles/r02_top_kernels_ncu.txt, same figures as round 1's capture): one k_ntt_forward_digits_fp launch of 16000 transforms moved 42.4 MB + 994.7 MB of
-                # DRAM traffic against 2097.2 MB algorithmic (16N per transform; the digit source is shared by 125 transforms through
-                # L2) -- ratio 0.495, applied to this run's mean launch (waves are larger than the captured one)
-                "traffic": 0.495 * fam["bytes"] / max(1, fam["launches"]),
-                "traffic_source": "ncu dram bytes / algorithmic bytes = 0.495 for k_ntt_forward_digits_fp<13,1> (profiles/r02_top_kernels_ncu.txt), scaled to this run's mean launch",
+                "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"], "peak_source": peak_kind + " bandwidth",
                 "launches_timed": fam["launches"], "algorithmic_bytes_per_launch": fam["bytes"] / max(1, fam["launches"]),
                 "avg_launch_ms": fam["ms"] / max(1, fam["launches"]), "share_of_step": fam["ms"] / ms if ms else None,
                 "families_ms_per_step": {k: v["ms"] / args.steps for k, v in prof.items()}}
@@ -456,7 +480,7 @@ def run_b200(args):
             "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u64",
             "data": "synthetic MNIST-shaped uint8 images (80% zeros), shipped CryptoNets weights, device-generated keys",
             "config": cpu_line_config(len(primes), world),
-            "clocks": clocks, "gpu_launches": int(launches), "numa": {k_: v for k_, v in numa.items() if k_ != "previous_cpus"}, "host_gc": host_gc,
+            "device": device_info(local), "clocks": clocks, "gpu_launches": int(launches), "numa": {k_: v for k_, v in numa.items() if k_ != "previous_cpus"}, "host_gc": host_gc,
             "collective": {"op": "all_gather_into_tensor (NCCL) of the score ciphertexts, every step, inside both timed regions",
                            "bytes_per_rank_per_step": int(eng.P * 10 * eng.ct_words * 8)},
             "e2e": {"value": e2e_value, "unit": "images/s", "h2d_bytes_per_step": int(host_in.numel() * 8), "d2h_bytes_per_step": int(host_out.numel() * 8)},
@@ -568,11 +592,8 @@ def run_lola(args):
     images_per_step = 1 if shard else world
     value = args.steps * images_per_step / (ms * 1e-3)
     if rank == 0:  # per-inference evaluator-operation counts: the CPU arm (`--impl reference --workload ...`) scales its per-op timings by them
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_opcounts_%s.json" % args.workload), "w") as fo:
-                json.dump(counts, fo)
-        except OSError:
-            pass
+        with open(opcounts_path(args.workload), "w") as fo:
+            json.dump(counts, fo)
 
     # ---- e2e: the image's ciphertexts come from pinned host memory every step, the score ciphertexts go back to the host
     vecs = xm.vectors
@@ -621,12 +642,12 @@ def run_lola(args):
             "config": {"workload": desc, "plain_moduli": len(primes),
                        "parallelism": ("rows of the 5488-row dense layer sharded x%d (one image)" % world) if shard else "replica-per-gpu x%d" % world,
                        "l2": "key-switching keys (%d Galois elements) and digit waves larger than L2" % eng.n_galois},
-            "clocks": clocks, "gpu_launches": int(launches), "operations_per_inference": counts,
+            "device": device_info(local), "clocks": clocks, "gpu_launches": int(launches), "operations_per_inference": counts,
             "e2e": {"value": args.steps * images_per_step / e2e_s, "unit": "images/s", "h2d_bytes_per_step": int(host_in.numel() * 8),
                     "d2h_bytes_per_step": int(host_out.numel() * 8)},
-            "roofline": {"bound": "hbm", "limited_by": "fp64-issue (ncu: 63 % of the FP64 pipe busy, math_pipe_throttle the top stall; 100 % of the pipe would be 0.85 of this HBM figure)", "kernel": "forward NTT family (digit transforms of the Galois / relinearisation key switch), 16*N algorithmic bytes per transform",
+            "roofline": {"bound": "hbm", "limited_by": "not profiled", "kernel": "forward NTT family (digit transforms of the Galois / relinearisation key switch), 16*N algorithmic bytes per transform",
                          "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-                         "peak_source": peak_kind + " copy bandwidth (MEASURED_PEAKS.json)", "traffic": None, "launches_timed": fam["launches"],
+                         "peak_source": peak_kind + " bandwidth", "traffic": None, "launches_timed": fam["launches"],
                          "share_of_step": fam["ms"] / ms if ms else None, "families_ms_per_step": {k_: v["ms"] / args.steps for k_, v in prof.items()}},
             "cpu_baseline": cpu,
         }
@@ -678,10 +699,17 @@ def lola_cpu_estimate(workload, counts, threads=None):
             "single_thread_seconds_per_image": one_thread, "per_op_seconds": per_op, "host": host_info()}
 
 
+def opcounts_path(workload):
+    """Where the GPU arm of a LoLa workload leaves its per-inference operation counts (the temporary directory: the tree may be read-only)."""
+    return os.path.join(tempfile.gettempdir(), "cnhe_opcounts_%s.json" % workload)
+
+
 def run_reference_lola(args):
-    """CPU arm of a LoLa workload: needs the per-inference operation counts, which come from a recorded GPU run (profiles/) or, when none is
-    present, from the counts written next to this file by the B200 arm."""
-    path = os.path.join(ROOT, "profiles", "r02_opcounts_%s.json" % args.workload)
+    """CPU arm of a LoLa workload: needs the per-inference operation counts, which come from the GPU arm's last run on this host or, when
+    there is none, from the counts stored in profiles/ (they depend on the network only, not on the GPU)."""
+    path = opcounts_path(args.workload)
+    if not os.path.exists(path):
+        path = os.path.join(ROOT, "profiles", "opcounts_%s.json" % args.workload)
     counts = json.load(open(path))
     threads = host_threads()
     cpu = lola_cpu_estimate(args.workload, counts, threads)
@@ -701,7 +729,7 @@ def run_microbench(args):
     coefficient moduli (prefixes of SEAL's default tables).  One JSON line per case."""
     from cryptonets_b200.engine import Engine
     from oracle.oracle_py import Oracle
-    PEAK = 6580.3
+    PEAK = 3350.0  # H100 SXM HBM3, data sheet
     try:
         PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
     except Exception:
@@ -766,12 +794,14 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="b200", choices=["b200", "reference"], help="b200 = the CUDA library (the name is historical)")
     ap.add_argument("--plain-moduli", type=int, default=2, choices=[1, 2])
     ap.add_argument("--workload", default="cryptonets", choices=["cryptonets", "lola_small", "lola_cifar", "microbench"],
                     help="cryptonets = BASELINE config 2 (the headline metric); lola_small / lola_cifar = configs 3 / 4 (one image per inference); "
                          "microbench = config 5 (one JSON line per case)")
     ap.add_argument("--microbench", action="store_true", help="same as --workload microbench")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="cryptonets: write the last timed step's outputs (decrypted scores, sampled score-ciphertext words) as DIR/*.npy")
     ap.add_argument("--shard-rows", action="store_true", help="lola_cifar on several GPUs: one image, the big dense layer's rows split over the ranks")
     args = ap.parse_args()
     if args.microbench or args.workload == "microbench":

@@ -1,4 +1,4 @@
-// K5/K6 element-wise stages of the BFV ciphertext x ciphertext multiply and of key switching (sm_100a).
+// K5/K6 element-wise stages of the BFV ciphertext x ciphertext multiply and of key switching (sm_90a).
 //
 // Replaces, stage by stage, SEAL 3.2 Evaluator::bfv_multiply and util::BaseConverter::{fastbconv_mtilde, mont_rq,
 // fast_floor, fastbconv_sk}, the 128-bit lazy inner product of Evaluator::relinearize_one_step / apply_galois, and the

@@ -2,7 +2,7 @@
 //
 // Same functions, same canonical outputs, different pipe: every modular product here is by a constant or of two residues
 // below 2^50, so it runs as the 6-instruction error-free FP64 product of fparith.cuh instead of a Barrett reduction of a
-// 128-bit integer product (4 mul.hi.u64 + 6 mul.lo.u64, the slowest instructions on the B200 integer pipe).  Wherever SEAL's
+// 128-bit integer product (4 mul.hi.u64 + 6 mul.lo.u64, the slowest instructions on the integer pipe).  Wherever SEAL's
 // algorithm depends on the *representative* of a residue (the fast base conversions sum [x c]_p * c' over the integers),
 // the canonical representative in [0,p) is formed first, exactly as in behz.cu.
 #include <cstdlib>

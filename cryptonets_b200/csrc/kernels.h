@@ -183,7 +183,7 @@ enum SampleKind { SAMPLE_TERNARY = 0, SAMPLE_NOISE = 1, SAMPLE_UNIFORM = 2 };
 // limbs = ceil(bits(q)/8); needs K*254*255 < 2^31
 cudaError_t launch_mac_dense_imma(const u64 *const *in_ptrs, const void *wfrag, const void *wfrag2, const u64 *bias, int K, int M, int limbs,
                                   u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
-// Scalar-MAC layers on tcgen05 (mac_umma.cu).  The layer's inputs are rows of one slab (input i at slab + i * slab_stride_words); a
+// Scalar-MAC layers on wgmma (mac_umma.cu).  The layer's inputs are rows of one slab (input i at slab + i * slab_stride_words); a
 // BUNDLE is up to 128 outputs whose taps lie in a window of consecutive inputs: chunk j of the bundle multiplies the 32 inputs that start
 // at row chunk_rows[chunk0 + j] (bit 30 set: a row of the scratch slab that holds the W2 taps) with the 128 x 32 weight block at
 // wpack + a_off + j * 4096.  Outputs and constant biases are listed in bundle order (out0 = first entry of the bundle).

@@ -1,4 +1,4 @@
-// Dense scalar-MAC layer on the integer tensor cores (sm_100a, mma.sync m16n8k32 s8 x u8 -> s32).
+// Dense scalar-MAC layer on the integer tensor cores (sm_90a, mma.sync m16n8k32 s8 x u8 -> s32).
 //
 // A dense layer over per-pixel ciphertexts (PoolLayer with one window covering the whole input: CryptoNets' 845 -> 100 and
 // 100 -> 10 layers, NeuralNetworks/PoolLayer.cs:196-227) IS a matrix product: out[m][c] = sum_k W[m][k] * x[k][c] mod q_l, with c

@@ -1,28 +1,26 @@
-// Scalar-MAC layers (dense and convolution) on the 5th-generation tensor cores: tcgen05.mma kind::i8, accumulators in tensor memory.
+// Scalar-MAC layers (dense and convolution) on the Hopper tensor cores: wgmma.mma_async s8 x u8 -> s32, operands in shared memory,
+// accumulators in registers.
 //
 // Same arithmetic as mac_imma.cu (the layer IS a matrix product over 8-bit limbs of the ciphertext words:
 //     x = sum_a 2^(8a) x_a,  P_a[m][c] = sum_k W[m][k] x_a[k][c],  out = sum_a 2^(8a) P_a mod q_l,
 // NeuralNetworks/PoolLayer.cs:196-227), generalised from "one window covers the whole input" to BUNDLES: a bundle is a set of at most
 // 128 outputs whose taps lie in a window of consecutive inputs (a dense layer is one bundle; a strided convolution is one bundle per
-// output row, and all interior rows share one weight matrix because the window slides with them).  Re-designed around what limited the
-// mma.sync kernel
-// (profiles/r01_mac_layers_ncu.txt: 232 registers per thread for the 96 accumulators, one 8-warp CTA per SM, 12 % of HBM,
-// long-scoreboard + barrier stalls -- latency bound, not tensor bound):
-//   * accumulators live in TMEM (two 256-column buffers: the epilogue of one tile runs under the MMAs of the next), no thread
-//     holds them;
+// output row, and all interior rows share one weight matrix because the window slides with them).  What the mma.sync kernel is limited
+// by -- every warp loads and shuffles its own operands, so loads, address arithmetic and accumulators all compete for registers -- is
+// moved off the consumers:
 //   * the ciphertext words arrive by TMA into a six-stage ring, two cp.async.bulk.tensor requests per stage (a 2-D map over the
-//     slab the layer's inputs sit in: 32 taps x 16 words each, SWIZZLE_128B): no registers, no address arithmetic in the consumers,
-//     as many bytes in flight as HBM latency needs.  (Issuing one 256-byte cp.async.bulk per tap cost ~60 cycles each: 94 % of the
-//     first version's time.)  The few taps whose weights exceed a signed byte (W = W1 + W2) are gathered into a scratch slab by the
-//     host call and appear a second time, as extra chunks with W2 as their weights, through a second map;
-//   * eight "cutter" warps turn a raw stage into the B operand -- limb a of word n is row a*32 + n of a K-major, unswizzled
-//     UMMA tile (8-row x 16-byte core matrices) -- three byte permutes per limb, conflict-free 32-bit stores;
-//   * one thread issues ONE tcgen05.mma (M = 128 outputs, N = 32 * limbs, K = 32 taps) per stage against the weight chunk that
-//     has been resident in shared memory since the CTA started (A operand, packed by the host in core-matrix order), and
-//     tcgen05.commit hands the B stage back;
+//     slab the layer's inputs sit in: 32 taps x 16 words each, SWIZZLE_128B), issued by one producer warp that only waits on
+//     mbarriers.  The few taps whose weights exceed a signed byte (W = W1 + W2) are gathered into a scratch slab by the host call and
+//     appear a second time, as extra chunks with W2 as their weights, through a second map;
+//   * the weights of the whole layer stay resident in shared memory from the start of the CTA (A operand, packed by the host in
+//     core-matrix order: 8-row x 16-byte core matrices, K-major, no swizzle);
+//   * the 256 consumer threads (two warpgroups) turn a raw stage into the B operand -- limb a of word n is row a*32 + n of a K-major
+//     unswizzled tile -- with three byte permutes per limb and conflict-free 32-bit stores, then each warpgroup issues one
+//     m64n32k32 wgmma per limb for its 64 output rows.  The wgmma runs asynchronously under the cutting of the next stage;
+//   * the epilogue reads the accumulators straight from registers: a thread holds 8 words of 2 output rows for every limb, so the
+//     limbs combine without any exchange;
 //   * persistent CTAs (one per SM) walk the 32-word tiles of the ciphertext, and inside a tile the bundles of the layer.
-// Warp roles: 0-3 and 8-11 epilogue (TMEM lanes 32 (w % 4).. = output rows; each thread writes its row's 32 words straight to HBM, 64
-// bytes at a time; one group per accumulator buffer), 4 TMA producer, 5 MMA issuer, 6-7 and 12-17 cutters.
+// Warp roles: 0-7 consumers (warpgroup 0 = output rows 0-63 of a bundle, warpgroup 1 = rows 64-127), 8 TMA producer.
 // Output words are bit-identical to k_mac_dense_imma / k_mac_layer_fp and to the oracle (tests/test_gpu_kernels.py:
 // test_dense_layer_on_tensor_cores, test_convolution_on_tensor_cores, test_tensor_core_layers_randomised).
 #include <cstdio>
@@ -37,15 +35,13 @@ namespace cnhe {
 namespace {
 
 constexpr int UM_TN = 32;                            // ciphertext words per tile
-constexpr int UM_M = 128;                            // MMA rows (outputs, zero padded)
-constexpr int UM_CHUNK = 32;                         // taps per MMA (K of kind::i8)
+constexpr int UM_M = 128;                            // MMA rows (outputs, zero padded): two warpgroups of 64
+constexpr int UM_CHUNK = 32;                         // taps per MMA (K of the 8-bit wgmma)
 constexpr int UM_RAW_STAGES = 6, UM_B_STAGES = 4;
 constexpr int UM_RAW_BYTES = UM_CHUNK * UM_TN * 8;   // 8192: two halves of 32 taps x 16 words (128-byte rows, hardware swizzle)
 constexpr int UM_A_CHUNK = UM_M * UM_CHUNK;          // 4096 bytes of weights per chunk
-constexpr int UM_THREADS = 576;                      // warps 0-3 and 8-11 epilogue (one group per accumulator buffer), 4 producer, 5 MMA issuer,
-                                                     // 6-7 and 12-17 cutters
-constexpr int UM_ACC_COLS = 256;                     // TMEM columns per accumulator buffer (two buffers = all 512)
-constexpr int UM_CUTTERS = 256, UM_EPI = 128;
+constexpr int UM_CONSUMERS = 256;                    // warps 0-7
+constexpr int UM_THREADS = UM_CONSUMERS + 32;        // + warp 8, the producer
 
 __device__ __forceinline__ unsigned sptr(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mb_init(unsigned long long *bar, unsigned count) {
@@ -58,8 +54,7 @@ __device__ __forceinline__ void mb_arrive(unsigned long long *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(sptr(bar)) : "memory");
 }
 // bounded wait: a protocol error traps (the launch fails with an error) instead of hanging the GPU.  The try_wait carries a suspend-time
-// hint, so a waiting warp sleeps in hardware instead of spinning: in the first version the spin loops (TRYWAIT / ISETP / BRA / YIELD)
-// were 40 % of all executed instructions and took issue slots from the working warps of the same scheduler (ncu source view)
+// hint, so a waiting warp sleeps in hardware instead of spinning and taking issue slots from the working warps of its scheduler
 __device__ __forceinline__ void mb_wait(unsigned long long *bar, unsigned parity) {
     const unsigned a = sptr(bar);
     unsigned done = 0;
@@ -82,36 +77,35 @@ __device__ __forceinline__ void tma_g2s_2d(void *dst, const void *tmap, int c0, 
                  : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(unsigned long long *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(sptr(bar)) : "memory");
-}
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(UM_CONSUMERS) : "memory"); }
 // K-major operand without swizzle: 8-row x 16-byte core matrices; lbo = distance between the two 16-byte K halves, sbo = distance
-// between 8-row groups (bytes); descriptor version 1 (sm_100)
-__device__ __forceinline__ u64 umma_desc(unsigned saddr, unsigned lbo, unsigned sbo) {
-    return (u64)((saddr & 0x3FFFFu) >> 4) | ((u64)(lbo >> 4) << 16) | ((u64)(sbo >> 4) << 32) | (1ULL << 46);
+// between 8-row groups (bytes); layout type 0 (no swizzle) in bits 62-63
+__device__ __forceinline__ u64 wgmma_desc(unsigned saddr, unsigned lbo, unsigned sbo) {
+    return (u64)((saddr & 0x3FFFFu) >> 4) | ((u64)(lbo >> 4) << 16) | ((u64)(sbo >> 4) << 32);
 }
-__device__ __forceinline__ void umma_i8(unsigned tmem_d, u64 adesc, u64 bdesc, unsigned idesc, unsigned accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads or writes across an asynchronous wgmma
+__device__ __forceinline__ void acc_fence(int (&d)[16]) {
+#pragma unroll
+    for (int i = 0; i < 16; i++) asm volatile("" : "+r"(d[i])::"memory");
+}
+// D[64 x 32] (+)= A[64 x 32 signed bytes] * B[32 x 32 unsigned bytes]^T; fragment: d[i] is row 16 * warp + lane / 4 + 8 * ((i >> 1) & 1),
+// column 8 * (i >> 2) + 2 * (lane & 3) + (i & 1)
+__device__ __forceinline__ void wgmma_i8(int (&d)[16], u64 adesc, u64 bdesc, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.u8 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]),
+                   "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate)
                  : "memory");
 }
-__device__ __forceinline__ void tmem_ld8(unsigned taddr, int (&v)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr));
-}
-// the registers of a TMEM load are valid only after tcgen05.wait::ld; this empty volatile asm (ordered after the wait) "rewrites" them, so
-// no use of them can be scheduled above the wait
-template <int W>
-__device__ __forceinline__ void tmem_regs_ready(int (&v)[W], int o) { asm volatile("" : "+r"(v[o]), "+r"(v[o + 1]), "+r"(v[o + 2]), "+r"(v[o + 3])); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 // exact double of a signed integer |x| < 2^51: one integer add, one FP64 add (inverse of d2i)
 __device__ __forceinline__ double i2d(long long x) { return __dsub_rn(__longlong_as_double(x + 0x4338000000000000LL), FP_MAGIC); }
-__device__ __forceinline__ void stg256(u64 *p, u64 a, u64 b, u64 c, u64 d) {
-    asm volatile("st.global.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(p), "l"(a), "l"(b), "l"(c), "l"(d) : "memory");
-}
+__device__ __forceinline__ void stg128(u64 *p, u64 a, u64 b) { asm volatile("st.global.v2.b64 [%0], {%1,%2};" ::"l"(p), "l"(a), "l"(b) : "memory"); }
 
 struct UmSmem { // offsets into the dynamic shared memory block (bytes), after the 1024-byte alignment pad
     int w, raw, b, dst, bun, rows, mod, bars, total;
@@ -145,8 +139,7 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
     long long t_a = 0, t_b = 0, t_c = 0, t0 = 0;
 #define UM_T0() if (profiling) t0 = clock64()
 #define UM_ACC(x) if (profiling) { const long long t1_ = clock64(); x += t1_ - t0; t0 = t1_; }
-    constexpr int NB = LIMBS * UM_TN;            // MMA N: rows of the B operand / accumulator columns
-    constexpr int B_BYTES = NB * UM_CHUNK;
+    constexpr int B_BYTES = LIMBS * UM_TN * UM_CHUNK;
     const UmSmem L = um_layout(a_bytes, total_chunks, n_out_total, n_bundles, LIMBS);
     unsigned char *sw = smem + L.w, *sraw = smem + L.raw, *sb = smem + L.b;
     u64 **sdst = reinterpret_cast<u64 **>(smem + L.dst);
@@ -154,23 +147,18 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
     int *srows = reinterpret_cast<int *>(smem + L.rows);
     double *smod = reinterpret_cast<double *>(smem + L.mod);
     unsigned long long *bars = reinterpret_cast<unsigned long long *>(smem + L.bars);
-    unsigned long long *raw_full = bars, *raw_empty = raw_full + UM_RAW_STAGES, *b_full = raw_empty + UM_RAW_STAGES, *b_empty = b_full + UM_B_STAGES,
-                       *acc_full = b_empty + UM_B_STAGES, *acc_empty = acc_full + 2, *w_full = acc_empty + 2;
-    unsigned *tmem_slot = reinterpret_cast<unsigned *>(w_full + 1);
-    static_assert((2 * UM_RAW_STAGES + 2 * UM_B_STAGES + 6) * 8 <= 256, "barrier block");
+    unsigned long long *raw_full = bars, *raw_empty = raw_full + UM_RAW_STAGES, *w_full = raw_empty + UM_RAW_STAGES;
+    static_assert((2 * UM_RAW_STAGES + 1) * 8 <= 256, "barrier block");
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int N = 1 << logn;
     const int n_tiles = (int)(((size_t)2 * k << logn) / UM_TN);
 
     if (tid == 0) {
-        for (int i = 0; i < UM_RAW_STAGES; i++) { mb_init(raw_full + i, 1); mb_init(raw_empty + i, UM_CUTTERS); }
-        for (int i = 0; i < UM_B_STAGES; i++) { mb_init(b_full + i, UM_CUTTERS); mb_init(b_empty + i, 1); }
-        for (int i = 0; i < 2; i++) { mb_init(acc_full + i, 1); mb_init(acc_empty + i, UM_EPI); }
+        for (int i = 0; i < UM_RAW_STAGES; i++) { mb_init(raw_full + i, 1); mb_init(raw_empty + i, UM_CONSUMERS); }
         mb_init(w_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    // tables and modulus constants: fetched once, so that no role touches global memory for them again (a dependent pointer load per
-    // stage cost the first version's producer ~0.6 us per chunk)
+    // tables and modulus constants: fetched once, so that no role touches global memory for them again
     for (int i = tid; i < n_out_total; i += UM_THREADS) sdst[i] = out_ptrs[i];
     for (int i = tid; i < n_bundles; i += UM_THREADS) sbun[i] = bundles[i];
     for (int i = tid; i < total_chunks; i += UM_THREADS) srows[i] = chunk_rows[i];
@@ -180,16 +168,9 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
         smod[tid * 8 + 1] = pinv;
         for (int a = 3; a < 8; a++) smod[tid * 8 + a - 1] = frecenter((double)(1ULL << (8 * a)), p, pinv); // slots 2..6 = a 3..7
     }
-    if (warp == 0) { // the allocating warp also frees
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sptr(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
 
-    if (warp == 4) {
+    if (warp == UM_CONSUMERS / 32) {
         // ---- producer (one thread): the weight matrices once, then two tensor-map requests per stage
         if (lane == 0) {
             mb_expect_tx(w_full, (unsigned)a_bytes);
@@ -216,61 +197,40 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
             }
             if (profiling) { prof[0] = t_a; prof[1] = t_b; }
         }
-        __syncwarp();
-    } else if (warp == 5) {
-        // ---- MMA issuer: one thread
-        if (lane == 0) {
-            // instruction descriptor: D = s32 (2 << 4), A = signed 8 bit (1 << 7), B = unsigned 8 bit (0 << 10), both K-major,
-            // N >> 3 at bit 17, M >> 4 at bit 24
-            const unsigned idesc = (2u << 4) | (1u << 7) | ((unsigned)(NB >> 3) << 17) | ((unsigned)(UM_M >> 4) << 24);
-            mb_wait(w_full, 0);
-            unsigned it = 0, ti = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                for (int b = 0; b < n_bundles; b++, ti++) {
-                    const UmBundle bn = sbun[b];
-                    const unsigned as = ti & 1;
-                    UM_T0();
-                    mb_wait(acc_empty + as, ((ti >> 1) & 1) ^ 1);
-                    UM_ACC(t_a);
-                    tc_fence_after();
-                    for (int c = 0; c < bn.n_chunks; c++, it++) {
-                        const unsigned s = it % UM_B_STAGES, ph = (it / UM_B_STAGES) & 1;
-                        UM_T0();
-                        mb_wait(b_full + s, ph);
-                        UM_ACC(t_b);
-                        tc_fence_after();
-                        umma_i8(tmem_base + as * UM_ACC_COLS, umma_desc(sptr(sw + bn.a_off + c * UM_A_CHUNK), 128, 256), umma_desc(sptr(sb + s * B_BYTES), 128, 256),
-                                idesc, c > 0);
-                        tc_commit(b_empty + s); // the stage is free once this MMA (and everything before it) has read it
-                        UM_ACC(t_c);
-                    }
-                    tc_commit(acc_full + as);
-                }
-            }
-            if (profiling) { prof[4] = t_a; prof[5] = t_b; prof[6] = t_c; }
-        }
-        __syncwarp();
-    } else if (warp == 6 || warp == 7 || warp >= 12) {
-        // ---- cutters: raw words -> limb bytes in UMMA order.  Thread (q = tap quad 0..7, n = word 0..31) packs limb a of taps 4q..4q+3
-        // into one 32-bit store at row a*32+n, bytes 4q..4q+3.  Lane = (q & 3) + 4 * (n & 7): the 32 stores of a warp fill one 8-row core
-        // matrix half (512 contiguous bytes, conflict free); the 64-bit loads touch 8 consecutive words of 4 tap rows 4 apart, which
-        // the hardware swizzle (16-byte chunk index XOR row & 7) spreads over both halves of the banks (2 wavefronts)
-        const int cw = warp < 8 ? warp - 6 : warp - 10; // cutter warp 0..7: (n >> 3) + 4 * (q >> 2)
-        const int ct = cw * 32 + lane;
-        const int n = (cw & 3) * 8 + (lane >> 2), qh = cw >> 2, q = qh * 4 + (lane & 3);
-        const int half_off = (n >> 4) * (UM_RAW_BYTES / 2), j16 = (n & 15) >> 1, sub = (n & 1) * 8;
-        unsigned it = 0;
-        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            for (int c = 0; c < total_chunks; c++, it++) {
+        return;
+    }
+
+    // ---- consumers.  Cutting: thread (q = tap quad 0..7, n = word 0..31) packs limb a of taps 4q..4q+3 into one 32-bit store at B row
+    // a*32+n, bytes 4q..4q+3.  Lane = (q & 3) + 4 * (n & 7): the 32 stores of a warp fill one 8-row core matrix half (512 contiguous
+    // bytes, conflict free); the 64-bit loads touch 8 consecutive words of 4 tap rows 4 apart, which the hardware swizzle (16-byte chunk
+    // index XOR row & 7) spreads over both halves of the banks.
+    const int wg = warp >> 2;
+    const int n = (warp & 3) * 8 + (lane >> 2), qh = warp >> 2, q = qh * 4 + (lane & 3);
+    const int half_off = (n >> 4) * (UM_RAW_BYTES / 2), j16 = (n & 15) >> 1, sub = (n & 1) * 8;
+    // accumulator fragment of this thread: output rows r0 and r0 + 8 of the bundle, words 8j + 2 (lane & 3) + {0, 1} of the tile
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    int acc[LIMBS][16];
+    mb_wait(w_full, 0);
+    unsigned it = 0;
+    long long t_d = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const size_t col0 = (size_t)tile * UM_TN;
+        const int l = (int)((col0 >> logn) % k);
+        const double p = smod[l * 8], pinv = smod[l * 8 + 1];
+        const double c24 = smod[l * 8 + 2], c48 = smod[l * 8 + 5]; // 2^24, 2^48 mod p
+        const bool bias_tile = bias && col0 < (size_t)k * N && (col0 & (size_t)(N - 1)) == 0; // coefficient 0 of a c0 polynomial
+        for (int b = 0; b < n_bundles; b++) {
+            const UmBundle bn = sbun[b];
+            const bool active = wg * 64 < bn.n_out; // a warpgroup whose 64 rows are all padding issues no MMA (uniform per warpgroup)
+            for (int c = 0; c < bn.n_chunks; c++, it++) {
                 const unsigned rs = it % UM_RAW_STAGES, rph = (it / UM_RAW_STAGES) & 1;
-                const unsigned bs = it % UM_B_STAGES, bph = (it / UM_B_STAGES) & 1;
+                // B stage it % 4 was last read by the MMAs of chunk it - 4: every consumer has waited for those of chunk it - 3 (the
+                // wait_group below, at chunk it - 2) before the barrier of chunk it - 1, which this thread has passed
+                unsigned char *bst = sb + (it % UM_B_STAGES) * B_BYTES;
                 UM_T0();
                 mb_wait(raw_full + rs, rph);
                 UM_ACC(t_a);
-                mb_wait(b_empty + bs, bph ^ 1);
-                UM_ACC(t_b);
                 const unsigned char *raw = sraw + rs * UM_RAW_BYTES + half_off + sub;
-                unsigned char *bst = sb + bs * B_BYTES;
                 unsigned lo[4], hi[4];
 #pragma unroll
                 for (int j = 0; j < 4; j++) {
@@ -279,6 +239,7 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
                     lo[j] = t.x;
                     hi[j] = t.y;
                 }
+                mb_arrive(raw_empty + rs);
 #pragma unroll
                 for (int a = 0; a < LIMBS; a++) { // byte a of the four words -> one 32-bit word, three byte permutes
                     const unsigned sel = (a & 3) | (((a & 3) + 4) << 4);
@@ -289,89 +250,67 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
                     *reinterpret_cast<unsigned *>(bst + (row >> 3) * 256 + qh * 128 + (row & 7) * 16 + (lane & 3) * 4) = w;
                 }
                 fence_async_smem(); // generic-proxy stores -> visible to the tensor core's (async proxy) reads
-                mb_arrive(b_full + bs);
-                mb_arrive(raw_empty + rs);
+                consumers_sync();
+                UM_ACC(t_b);
+                if (active) {
+#pragma unroll
+                    for (int a = 0; a < LIMBS; a++) acc_fence(acc[a]);
+                    wgmma_fence();
+                    const u64 adesc = wgmma_desc(sptr(sw + bn.a_off + c * UM_A_CHUNK + wg * (UM_A_CHUNK / 2)), 128, 256);
+#pragma unroll
+                    for (int a = 0; a < LIMBS; a++) wgmma_i8(acc[a], adesc, wgmma_desc(sptr(bst + a * (UM_TN * UM_CHUNK)), 128, 256), c > 0);
+                    wgmma_commit();
+#pragma unroll
+                    for (int a = 0; a < LIMBS; a++) acc_fence(acc[a]);
+                }
+                wgmma_wait<1>();
                 UM_ACC(t_c);
             }
-        }
-        if (profiling && ct == 0) { prof[8] = t_a; prof[9] = t_b; prof[10] = t_c; }
-    } else {
-        // ---- epilogue (warps 0-3): thread = output row m of the bundle.  out = sum_a 2^(8a) P_a mod q_l, exact in FP64 for p < 2^50: the
-        // three low limbs combine below 2^48 without reduction, every higher limb is a modular product with 2^(8a) mod p
-        // two groups of four warps (0-3, 8-11: a warp may only touch the TMEM lanes 32 * (warp % 4) ..), one per accumulator buffer: the
-        // per-unit cost of the epilogue is latency (TMEM load -> dependent FP64 chain -> store), so two units are drained at a time
-        const int grp = warp >> 3, m = (warp & 3) * 32 + lane;
-        unsigned ti = 0;
-        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const size_t col0 = (size_t)tile * UM_TN;
-            const int l = (int)((col0 >> logn) % k);
-            const double p = smod[l * 8], pinv = smod[l * 8 + 1];
-            const double c24 = smod[l * 8 + 2], c48 = smod[l * 8 + 5]; // 2^24, 2^48 mod p
-            const bool bias_tile = bias && col0 < (size_t)k * N && (col0 & (size_t)(N - 1)) == 0; // coefficient 0 of a c0 polynomial
-            for (int b = 0; b < n_bundles; b++, ti++) {
-                const unsigned as = ti & 1;
-                if ((int)as != grp) continue; // the other group's buffer
-                const UmBundle bn = sbun[b];
-                UM_T0();
-                mb_wait(acc_full + as, (ti >> 1) & 1);
-                UM_ACC(t_a);
-                tc_fence_after();
-                const unsigned tbase = tmem_base + ((unsigned)((warp & 3) * 32) << 16) + as * UM_ACC_COLS;
-                if ((warp & 3) * 32 < bn.n_out) { // warps whose 32 rows are all padding skip the arithmetic (uniform per warp)
-                    u64 *orow = m < bn.n_out ? sdst[bn.out0 + m] + col0 : nullptr;
-                    // eight words per step: the epilogue is a latency chain (TMEM load -> integer combine -> FP64 modular product -> canonical
-                    // word -> store) at ~0.25 instructions per cycle and warp, so what counts is independent words in flight.  (Four words
-                    // with the next four prefetched from TMEM measured 14 % slower: the TMEM load is not what the chain waits for.)
+            // ---- epilogue: out = sum_a 2^(8a) P_a mod q_l, exact in FP64 for p < 2^50: the three low limbs combine below 2^48 without
+            // reduction, every higher limb is a modular product with 2^(8a) mod p
+            wgmma_wait<0>();
 #pragma unroll
-                    for (int n0 = 0; n0 < UM_TN; n0 += 8) {
-                        int acc[LIMBS][8];
+            for (int a = 0; a < LIMBS; a++) acc_fence(acc[a]);
+            if (active && (warp & 3) * 16 + wg * 64 < bn.n_out) { // warps whose 16 rows are all padding skip the arithmetic (uniform per warp)
 #pragma unroll
-                        for (int a = 0; a < LIMBS; a++) tmem_ld8(tbase + a * UM_TN + n0, acc[a]);
-                        tmem_ld_wait();
+                for (int h = 0; h < 2; h++) {
+                    const int m = r0 + 8 * h;
+                    if (m >= bn.n_out) continue;
+                    u64 *orow = sdst[bn.out0 + m] + col0;
+                    u64 res[8];
 #pragma unroll
-                        for (int a = 0; a < LIMBS; a++) { tmem_regs_ready(acc[a], 0); tmem_regs_ready(acc[a], 4); }
-                        u64 res[8];
+                    for (int j = 0; j < 4; j++)
 #pragma unroll
-                        for (int e = 0; e < 8; e++) {
+                        for (int e = 0; e < 2; e++) {
+                            const int i = 4 * j + 2 * h + e;
                             // limbs 0..2 and 3..5 combine exactly on the integer pipe (each sum below 2^48); one modular product joins them
-                            const long long lo = (long long)acc[0][e] + ((long long)acc[1][e] << 8) + ((long long)acc[2][e] << 16);
-                            long long hi = (long long)acc[3][e] + ((long long)acc[4][e] << 8);
-                            if constexpr (LIMBS >= 6) hi += (long long)acc[5][e] << 16;
+                            const long long lo = (long long)acc[0][i] + ((long long)acc[1][i] << 8) + ((long long)acc[2][i] << 16);
+                            long long hi = (long long)acc[3][i] + ((long long)acc[4][i] << 8);
+                            if constexpr (LIMBS >= 6) hi += (long long)acc[5][i] << 16;
                             double rr = __dadd_rn(i2d(lo), fmodmul(i2d(hi), c24, p, pinv));
-                            if constexpr (LIMBS == 7) rr = __dadd_rn(rr, fmodmul((double)acc[6][e], c48, p, pinv));
-                            res[e] = fcanon_u(rr, p, pinv);
+                            if constexpr (LIMBS == 7) rr = __dadd_rn(rr, fmodmul((double)acc[6][i], c48, p, pinv));
+                            res[2 * j + e] = fcanon_u(rr, p, pinv);
                         }
-                        if (n0 == 0 && bias_tile && orow) { // constant-plaintext bias: Delta*b on coefficient 0 of c0 (add_plain)
-                            const u64 bv = bias[bn.out0 + m];
-                            const DMod q = bc->q[l];
-                            if (bv) res[0] = addmod(res[0], scale_plain(bv, l, q, pc), q.p);
-                        }
-                        if (orow) { // 64 contiguous bytes of this thread's output row: two full-sector 32-byte stores
-                            stg256(orow + n0, res[0], res[1], res[2], res[3]);
-                            stg256(orow + n0 + 4, res[4], res[5], res[6], res[7]);
-                        }
+                    if (bias_tile && c0 == 0) { // constant-plaintext bias: Delta*b on coefficient 0 of c0 (add_plain)
+                        const u64 bv = bias[bn.out0 + m];
+                        const DMod qm = bc->q[l];
+                        if (bv) res[0] = addmod(res[0], scale_plain(bv, l, qm, pc), qm.p);
                     }
+#pragma unroll
+                    for (int j = 0; j < 4; j++) stg128(orow + 8 * j + c0, res[2 * j], res[2 * j + 1]);
                 }
-                tc_fence_before();
-                mb_arrive(acc_empty + as); // the accumulator buffer may be overwritten
-                UM_ACC(t_b);
             }
+            UM_ACC(t_d);
         }
-        if (profiling && tid == 0) { prof[12] = t_a; prof[13] = t_b; }
     }
+    if (profiling && tid == 0) { prof[8] = t_a; prof[9] = t_b; prof[10] = t_c; prof[12] = t_d; }
 #undef UM_T0
 #undef UM_ACC
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    }
 }
 
 int sm_count_cached() {
     static int n = [] {
-        int dev = 0, v = 148;
+        int dev = 0, v = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
         return v;
@@ -400,9 +339,9 @@ cudaError_t umma_go(const CUtensorMap &map0, const CUtensorMap &map1, const Umma
         unsigned long long h[16];
         cudaMemcpyAsync(h, prof, sizeof(h), cudaMemcpyDeviceToHost, s);
         cudaStreamSynchronize(s);
-        fprintf(stderr, "[umma bundles=%d chunks/tile=%d outputs=%d weights=%d KB tiles/cta=%.1f] producer: wait_empty %llu issue %llu | mma: wait_acc %llu wait_b %llu issue %llu | "
-                        "cutters: wait_raw %llu wait_b %llu work %llu | epilogue group 0: wait_acc %llu drain %llu (cycles, CTA 0)\n",
-                a.n_bundles, a.total_chunks, a.n_out_total, a.a_bytes / 1024, (double)n_tiles / grid, h[0], h[1], h[4], h[5], h[6], h[8], h[9], h[10], h[12], h[13]);
+        fprintf(stderr, "[umma bundles=%d chunks/tile=%d outputs=%d weights=%d KB tiles/cta=%.1f] producer: wait_empty %llu issue %llu | "
+                        "consumers: wait_raw %llu cut %llu mma %llu epilogue %llu (cycles, CTA 0)\n",
+                a.n_bundles, a.total_chunks, a.n_out_total, a.a_bytes / 1024, (double)n_tiles / grid, h[0], h[1], h[8], h[9], h[10], h[12]);
     }
     return cudaGetLastError();
 }

@@ -1,4 +1,4 @@
-// Device-side 64-bit modular arithmetic for the BFV hot path (sm_100a).
+// Device-side 64-bit modular arithmetic for the BFV hot path (sm_90a).
 // Integer pipes only: 64x64->128 products are IMAD.WIDE chains; there is no tensor-core formulation of a
 // modular 64-bit butterfly.  All routines return canonical residues unless the name says "lazy".
 #pragma once

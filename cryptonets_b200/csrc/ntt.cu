@@ -1,4 +1,4 @@
-// K1/K2: batched negacyclic NTT / inverse NTT over one residue polynomial per CTA  (sm_100a).
+// K1/K2: batched negacyclic NTT / inverse NTT over one residue polynomial per CTA  (sm_90a).
 //
 // Replaces SEAL 3.2 util::ntt_negacyclic_harvey(_lazy) / inverse_ntt_negacyclic_harvey(_lazy), reached from every
 // Evaluator.Multiply / Relinearize / Rotate* / dense MultiplyPlain call site of
@@ -300,9 +300,8 @@ k_ntt_inverse(const u64 *src, const u64 *base_add, int base_group, size_t base_s
 }
 
 // ================================================================ FP64 butterfly path (p < 2^50)
-// On B200 a 64x64->128-bit integer product costs ~9 IMAD-pipe slots (IMAD.WIDE issues at 0.77 and mul.hi.u64 at 0.23
-// warp-instr/clk/SM, measured: profiles/r01_pipe_issue_rates.txt) while DFMA/DADD issue at 1.94 and overlap with the integer
-// ALU.  For moduli below 2^50 -- all of SEAL's default coefficient primes and the 48-bit auxiliary base -- the butterfly
+// A 64x64->128-bit integer product costs ~9 IMAD-pipe slots (IMAD.WIDE and above all mul.hi.u64 issue well below the DFMA/DADD
+// rate: tools/pipe_bench.cu) while DFMA/DADD overlap with the integer ALU.  For moduli below 2^50 -- all of SEAL's default coefficient primes and the 48-bit auxiliary base -- the butterfly
 // is therefore done in double precision with error-free transformations:
 //     h = a*w, l = fma(a,w,-h) (exact product h+l),  q = rint(h/p),  r = fma(-q,p,h) + l  ==  a*w - q*p  exactly,
 // 6 DP ops for the modular product + 2 for the butterfly, no integer corrections at all: values stay centred and small
@@ -313,12 +312,12 @@ constexpr int TWC = 512;
 __device__ __forceinline__ void load_twiddle_cache(double *twc, const double *tw, int tid, int nthreads) {
     for (int i = tid; i < TWC; i += nthreads) twc[i] = __ldg(tw + i);
 }
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): a thread moves its 16 consecutive words as four full 32-byte sectors
+// a thread moves 4 consecutive words (one full 32-byte sector) as two adjacent 128-bit accesses, the widest global access sm_90 has
 __device__ __forceinline__ void ldg256(const u64 *p, u64 &a, u64 &b, u64 &c, u64 &d) {
-    asm volatile("ld.global.v4.b64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+    asm volatile("ld.global.v2.b64 {%0,%1}, [%4];\n\tld.global.v2.b64 {%2,%3}, [%4+16];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
 }
 __device__ __forceinline__ void stg256(u64 *p, u64 a, u64 b, u64 c, u64 d) {
-    asm volatile("st.global.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(p), "l"(a), "l"(b), "l"(c), "l"(d) : "memory");
+    asm volatile("st.global.v2.b64 [%0], {%1,%2};\n\tst.global.v2.b64 [%0+16], {%3,%4};" ::"l"(p), "l"(a), "l"(b), "l"(c), "l"(d) : "memory");
 }
 
 // Shared-memory round trips are what keeps the FP64 pipe idle (tools/dp_pass_bench.cu: 96 % utilisation on registers, ~62 %
@@ -548,7 +547,7 @@ __host__ __device__ constexpr int fp_min_blocks(int logn) { return logn >= 14 ? 
 template <int LOGN>
 __device__ __forceinline__ void prefetch_next_poly(const u64 *src_base, int b, int n_polys, int tid) {
     constexpr int N = 1 << LOGN, TR = fp_threads(LOGN);
-    const int ahead = b + 148 * fp_min_blocks(LOGN);
+    const int ahead = b + 132 * fp_min_blocks(LOGN); // 132 SMs on an H100 SXM
     if (ahead < n_polys) {
         const char *p = reinterpret_cast<const char *>(src_base + (size_t)ahead * N);
         for (int i = tid * 128; i < N * 8; i += TR * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + i));
@@ -1451,9 +1450,8 @@ static bool ws_flag(const char *name, bool dflt) {
     if (all) return atoi(all) != 0;
     return dflt;
 }
-// Measured on B200 (profiles/r02_ntt_ws_ab.txt): the persistent inverse transform is 20-25 % faster than one CTA per polynomial
-// (0.53-0.60 of the HBM roofline against 0.43-0.49); the persistent forward transform only draws level (0.50 against 0.52, and 12 % slower
-// in its digit-cutting form), so the forward direction keeps the per-polynomial kernel unless CNHE_NTT_WS_FWD=1 asks for the staged one.
+// Defaults: the persistent inverse transform, and the per-polynomial forward transform unless CNHE_NTT_WS_FWD=1 asks for the staged one
+// (the staged forward transform gains nothing over the per-polynomial one, and its digit-cutting form is slower).
 static bool ws_enabled_fwd() { return ws_flag("CNHE_NTT_WS_FWD", false); } // read per launch: tests flip it inside one process
 static bool ws_enabled_inv() { return ws_flag("CNHE_NTT_WS_INV", true); }
 // N = 8192 forward transforms with three CTAs per SM (CNHE_NTT_FWD_BLOCKS=3) or two (=2); read per launch
@@ -1473,7 +1471,7 @@ static cudaError_t split_prep(K kern) {
 }
 static int sm_count() {
     static int n = [] {
-        int dev = 0, v = 148;
+        int dev = 0, v = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
         return v;

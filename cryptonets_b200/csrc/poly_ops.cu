@@ -1,4 +1,4 @@
-// K3/K4/K7/K8/K9/K10 element-wise kernels of the BFV hot path (sm_100a): ciphertext add/sub/negate/add-many, plain add,
+// K3/K4/K7/K8/K9/K10 element-wise kernels of the BFV hot path (sm_90a): ciphertext add/sub/negate/add-many, plain add,
 // constant-plaintext scaling, dyadic products, the Galois coefficient permutation, the scalar multiply-accumulate layer
 // (CryptoNets conv/dense), sampling, BatchEncoder scatter/gather.
 //
@@ -183,7 +183,7 @@ __global__ void __launch_bounds__(128) k_mac_layer(const u64 *const *__restrict_
 
 // FP64 variant for small weights (|w| < 2^17, K*|w|*2^26 < 2^52 checked on the host): every ciphertext word is split into two
 // 26-bit halves and w*x is accumulated exactly in doubles -- 2 DFMA per multiply-accumulate instead of a 64x64->128 integer
-// product (mul.hi.u64 issues at 0.23 warp-instr/clk/SM on B200, DFMA at 1.94: profiles/r01_pipe_issue_rates.txt).
+// product (mul.hi.u64 issues at a fraction of the DFMA rate: tools/pipe_bench.cu).
 // The result sum_k w_k x_k is then reduced once, so the output is the same canonical residue as the integer path.
 __device__ __forceinline__ double mac_u2d(u64 x) { return __dsub_rn(__longlong_as_double((long long)(x | 0x4330000000000000ULL)), 4503599627370496.0); }
 __device__ __forceinline__ u64 mac_signed_reduce(double lo, double hi, const DMod &q) { // value = lo + hi * 2^26, both exact integers

@@ -74,13 +74,20 @@ DevBuf::DevBuf(size_t w, cudaStream_t s) : words(w), stream(s) {
     CNHE_CUDA(cudaMallocAsync((void **)&p, w * sizeof(u64), s));
 }
 constexpr size_t RECYCLE_MIN_WORDS = (size_t)1 << 19;        // 4 MB
-constexpr size_t RECYCLE_CAP_WORDS = (size_t)40 << 27;       // 40 GB parked at most
+constexpr size_t RECYCLE_CAP_WORDS = (size_t)16 << 27;       // 16 GiB parked at most (a fifth of an 80 GB H100)
 DevBuf::DevBuf(size_t w, cudaStream_t s, Context *ctx) : words(w), stream(s), owner(ctx) {
     if (!w) return;
     if (ctx && w >= RECYCLE_MIN_WORDS) {
         size_t got = 0;
         p = ctx->take_recycled(w, s, got);
         if (p) { words = got; return; }
+    }
+    if (ctx && !ctx->recycle.empty()) { // parked blocks of other sizes or streams are the first memory to give back when the device is full
+        if (cudaMallocAsync((void **)&p, w * sizeof(u64), s) == cudaSuccess) return;
+        p = nullptr;
+        (void)cudaGetLastError();
+        ctx->drop_recycled();
+        CNHE_CUDA(cudaDeviceSynchronize()); // the frees complete, so that the pool can hand their memory to this stream
     }
     DevBuf fresh(w, s); // traced allocation path
     p = fresh.p;
@@ -387,7 +394,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     if (dbc_relin < 1 || dbc_relin > 60 || dbc_galois < 1 || dbc_galois > 60) throw Error(-1, "decomposition bit count must be in [1,60]");
     int ndev = 0;
     cudaError_t de = cudaGetDeviceCount(&ndev);
-    if (de != cudaSuccess || ndev == 0) throw Error(-2, "libcnhe needs a CUDA device (B200); none is visible -- there is no CPU fallback");
+    if (de != cudaSuccess || ndev == 0) throw Error(-2, "libcnhe needs a CUDA device (H100); none is visible -- there is no CPU fallback");
     if (device < 0 || device >= ndev) throw Error(-1, "bad device ordinal");
     std::unique_ptr<Context> cp(new Context());
     Context &c = *cp;

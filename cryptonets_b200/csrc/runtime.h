@@ -163,7 +163,7 @@ struct Context {
     void drop_recycled();
     void launched(int n = 1) { launches += n; }
     void check(cudaError_t e, const char *what) { cuda_check(e, what); launched(); if (trace_ms > 0) trace_gap(what); }
-    std::unordered_map<u64, std::shared_ptr<void>> umma_plans; // tcgen05 layer plans (vec.cu), keyed by a hash of the layer's weights and gather table
+    std::unordered_map<u64, std::shared_ptr<void>> umma_plans; // wgmma layer plans (vec.cu), keyed by a hash of the layer's weights and gather table
     double trace_ms = 0; // CNHE_TRACE_SLOW: report host-side gaps between consecutive launches longer than this
     void trace_gap(const char *what);
     void sync();

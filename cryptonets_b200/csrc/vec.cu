@@ -21,7 +21,7 @@ int set_err(int code, const std::string &m) {
     return code;
 }
 extern "C" const char *cnhe_last_error(void) { return g_err.c_str(); }
-extern "C" const char *cnhe_version(void) { return "cnhe-b200 0.2 (sm_100a)"; }
+extern "C" const char *cnhe_version(void) { return "cnhe-b200 0.3 (sm_90a)"; }
 
 // ---------------------------------------------------------------------------------------------------- context & keys
 extern "C" int cnhe_context_create_custom(const uint64_t *plain_primes, int P, uint32_t N, const uint64_t *coeff, int k, int dbc_relin,
@@ -1188,7 +1188,7 @@ struct RowHash {
         return hsh;
     }
 };
-// ---- plan of a scalar-MAC layer for the tcgen05 kernel (mac_umma.cu): bundles of consecutive distinct gather rows
+// ---- plan of a scalar-MAC layer for the wgmma kernel (mac_umma.cu): bundles of consecutive distinct gather rows
 struct UmmaPlan {
     bool ok = false;
     std::vector<UmBundle> bundles;
@@ -1450,7 +1450,7 @@ static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int
         const bool imma = order_rows == 1 && wmax <= 254.0 && K >= 32 && M >= 8 && limbs >= 5 && limbs <= 7 && (double)K * 254.0 * 255.0 < 2147483648.0 &&
                           !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
         // ... or, for any layer whose inputs are evenly spaced rows of one slab (the previous layer's output, an imported batch) and whose
-        // weights stay within +-254: tcgen05 (mac_umma.cu), dense and convolution alike
+        // weights stay within +-254: wgmma (mac_umma.cu), dense and convolution alike
         std::shared_ptr<UmmaPlan> plan;
         long long tap_stride = 0;
         {

@@ -1,11 +1,11 @@
 /*
- * cnhe.h -- C ABI of libcnhe.so, the B200-native BFV engine behind the CryptoNets plugin API.
+ * cnhe.h -- C ABI of libcnhe.so, the H100-native BFV engine behind the CryptoNets plugin API.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these entry points
  * with [DllImport("cnhe")] (stub in INTEGRATION.md); the Python mirror in cryptonets_b200/ binds them with ctypes.
  * One cnhe_vec is one reference `EncryptedSealBfvVector` ("HE Wrapper/EncryptedSealBfvVector.cs:150-573"): P
  * plaintext-modulus channels, each an `AtomicSealBfvEncryptedVector` ("HE Wrapper/AtomicSealBfvVector.cs:303-1476")
- * whose SEAL Ciphertext[] / Plaintext[] live in B200 HBM.  Every call is batched over blocks and channels;
+ * whose SEAL Ciphertext[] / Plaintext[] live in GPU HBM.  Every call is batched over blocks and channels;
  * nothing here computes on the CPU and the library fails at load/first call when no CUDA device is present.
  *
  * Conventions: every function returns 0 (CNHE_OK) or a negative error code; cnhe_last_error() gives the message of

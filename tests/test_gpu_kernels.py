@@ -269,9 +269,9 @@ def test_dense_layer_on_tensor_cores(pair, shape, capfd):
     """Dense layer (all outputs read the same K inputs): the exact 8-bit-limb integer GEMM must give the same ciphertext words as the
     oracle's 128-bit multiply-accumulate -- odd M and K (padding inside the tiles), zero weights, extreme weights and maximal residues,
     bias on coefficient 0 of c0.  "gather": inputs scattered in memory, permuted, one padded tap -> mma.sync (mac_imma.cu).  "slab": the
-    inputs are consecutive ciphertexts of one allocation read in order, as a dense layer is fed by the layer before it -> tcgen05.mma with
-    TMEM accumulators and TMA loads (mac_umma.cu), up to 128 outputs, several 32-tap chunks, and ("wide", |w| <= 254) the W2 columns as
-    extra taps.  Every case is repeated with the tcgen05 path off and with both tensor-core paths off (FP64 scalar MAC)."""
+    inputs are consecutive ciphertexts of one allocation read in order, as a dense layer is fed by the layer before it -> wgmma with
+    register accumulators and TMA loads (mac_umma.cu), up to 128 outputs, several 32-tap chunks, and ("wide", |w| <= 254) the W2 columns as
+    extra taps.  Every case is repeated with the wgmma path off and with both tensor-core paths off (FP64 scalar MAC)."""
     import os
     from cryptonets_b200.engine import DENSE, SPARSE
     eng, orc, name = pair
@@ -280,8 +280,6 @@ def test_dense_layer_on_tensor_cores(pair, shape, capfd):
     feed, kind, dims = shape.split("-")
     wide = kind == "wide"
     M, K = [int(x) for x in dims.split("x")]
-    if M > 21 and name != "default4096":
-        pytest.skip("the larger shapes run on the smallest ring (oracle time)")
     n_in = K + 2
     vals, cts = _fresh_cts(orc, n_in, 12, nonce0=900)
     q = np.array(orc.q, dtype=np.uint64)
@@ -310,8 +308,8 @@ def test_dense_layer_on_tensor_cores(pair, shape, capfd):
     t = orc.t
     wres = np.where(w < 0, w + t, w).astype(np.uint64)
     bres = np.where(bias * 4 < 0, bias * 4 + t, bias * 4).astype(np.uint64)
-    want = orc.mac_layer(cts, gather, wres, bres, M, K, threads=4).reshape(M, -1)
-    os.environ["CNHE_UMMA_PROF"] = "1"  # the tcgen05 launcher then reports itself on stderr
+    want = orc.mac_layer(cts, gather, wres, bres, M, K, threads=max(4, os.cpu_count() or 1)).reshape(M, -1)
+    os.environ["CNHE_UMMA_PROF"] = "1"  # the wgmma launcher then reports itself on stderr
     capfd.readouterr()
     try:
         outs = eng.layer_conv_dense(ins, gather, wv, bv, M, K)
@@ -371,10 +369,9 @@ def test_cta_pair_and_whole_polynomial_transforms_agree(pair, split, monkeypatch
     """N = 16384 runs on CTA pairs by default (two 8192-point halves, the cross-half stage on the way in / through distributed shared
     memory on the way out); CNHE_NTT_SPLIT=0 keeps the one-CTA-per-polynomial kernels.  Both must give the oracle's words: plain
     transforms out of place and IN PLACE (the pair reads both halves before either writes), the digit-cutting forward and the lazy
-    variants inside multiply + relinearise."""
+    variants inside multiply + relinearise.  On the other rings, which have no CTA-pair kernels, either setting of the flag must leave
+    the same transforms exact."""
     eng, orc, name = pair
-    if eng.N != 16384:
-        pytest.skip("CTA pairs serve N = 16384 only")
     monkeypatch.setenv("CNHE_NTT_SPLIT", split)
     rng = np.random.default_rng(12)
     N, k, kt = eng.N, eng.k, eng.k + eng.kb
@@ -408,7 +405,7 @@ def test_cta_pair_and_whole_polynomial_transforms_agree(pair, split, monkeypatch
 
 @pytest.mark.parametrize("wide", [False, True])
 def test_convolution_on_tensor_cores(pair, wide, capfd):
-    """A strided, padded convolution over a slab of per-pixel ciphertexts (PoolLayer.cs:68-80, 196-227) on the tcgen05 path: the host
+    """A strided, padded convolution over a slab of per-pixel ciphertexts (PoolLayer.cs:68-80, 196-227) on the wgmma path: the host
     plan bundles the outputs of one output row (their taps lie in a window of consecutive inputs), interior rows share one weight matrix,
     padded taps carry no weight, and weights beyond a signed byte ("wide") ride on extra taps gathered into a scratch slab.  Same words as
     the oracle's 128-bit multiply-accumulate, and as the FP64 scalar-MAC kernel."""
@@ -457,7 +454,7 @@ def test_convolution_on_tensor_cores(pair, wide, capfd):
     finally:
         del os.environ["CNHE_UMMA_PROF"]
     err = capfd.readouterr().err
-    assert "[umma bundles=" in err, "the tcgen05 kernel did not serve the convolution"
+    assert "[umma bundles=" in err, "the wgmma kernel did not serve the convolution"
     for i in range(M):
         assert np.array_equal(outs[i].export_raw(0, 0), want[i]), i
     os.environ["CNHE_MAC_NO_UMMA"] = "1"
@@ -471,7 +468,7 @@ def test_convolution_on_tensor_cores(pair, wide, capfd):
 
 def test_tensor_core_layers_randomised():
     """Random dense shapes and random strided / padded convolutions (weights up to +-254, random biases, maximal words) through the
-    tcgen05 kernel and through the FP64 scalar-MAC kernel: two independent GPU implementations, bit-identical outputs
+    wgmma kernel and through the FP64 scalar-MAC kernel: two independent GPU implementations, bit-identical outputs
     (tools/umma_stress.py; the oracle-checked cases are test_dense_layer_on_tensor_cores / test_convolution_on_tensor_cores)."""
     import importlib.util
     import os
@@ -488,8 +485,6 @@ def test_key_switch_mac_full_waves(pair, monkeypatch):
     ciphertexts per CTA share the key words); smaller calls and CNHE_KSMAC_TMA=0 use the register kernels.  70 ciphertexts (a ragged last
     group of two): multiply + relinearise must match the oracle on sampled ciphertexts and the register kernel on all of them."""
     eng, orc, name = pair
-    if eng.N > 8192:
-        pytest.skip("oracle time")
     N, k = eng.N, eng.k
     m = 70
     _, few = _fresh_cts(orc, 6, 21, nonce0=3000)

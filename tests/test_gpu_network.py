@@ -1,4 +1,4 @@
-"""End-to-end parity of the reference networks on the B200 backend.
+"""End-to-end parity of the reference networks on the GPU backend.
 
 (i)  decrypted scores == the Raw (plaintext) backend exactly -- what the reference itself pins (SURVEY 8c);
 (ii) ciphertexts of sampled layer outputs == the CPU oracle run on the same input ciphertexts and keys, bit for bit."""

@@ -1,4 +1,4 @@
-"""The reference's own known-answer tests, restated on the B200 backend: `HE Wrapper Tests/BasicOperations.cs` (default factory:
+"""The reference's own known-answer tests, restated on the GPU backend: `HE Wrapper Tests/BasicOperations.cs` (default factory:
 N=4096, primes {40961,65537,114689,147457,188417}, IFactory.cs:247-253) and the BasicExample of README.md:61-73.
 Decrypted results must equal the plain results exactly, as in the reference (`Compare`, BasicOperations.cs:41-55)."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""Host-side planner of the tcgen05 scalar-MAC kernel (csrc/vec.cu: umma_try / umma_search), through the library's planner probe -- no GPU
+"""Host-side planner of the wgmma scalar-MAC kernel (csrc/vec.cu: umma_try / umma_search), through the library's planner probe -- no GPU
 needed.  A bundle is at most 128 outputs whose taps lie in a window of consecutive inputs; the planner tries every bundle size and keeps
 the plan with the fewest 32-tap chunks per tile that fits in shared memory; identical weight matrices are stored once."""
 import ctypes as C

@@ -1,4 +1,4 @@
-"""Exploratory: LoLa / LoLa-Dense on the B200 backend vs the Raw backend, with per-layer timings and remaining noise budget."""
+"""Exploratory: LoLa / LoLa-Dense on the GPU backend vs the Raw backend, with per-layer timings and remaining noise budget."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

@@ -119,7 +119,7 @@ class Model:
 
 def render(recs, out):
     w = out.write
-    w("# Per-operation noise budgets at the reference's parameters: measured (B200) vs the analytic BFV model\n\n")
+    w("# Per-operation noise budgets at the reference's parameters: measured by the GPU library (bit-exact, so independent of the GPU model) vs the analytic BFV model\n\n")
     w("Generated by `tools/noise_model.py` from the trace `tools/noise_trace.py` wrote on the GPU box (library option `trace_noise`:\n"
       "after every evaluator-level operation the invariant noise budget of its first output ciphertext is measured with the secret key,\n"
       "next to the budgets its inputs had).  `pred` is the model's output budget computed from the MEASURED input budgets of that one\n"

@@ -1,5 +1,5 @@
-// Issue-rate micro-benchmark for the pipes the modular butterflies use on B200: IMAD.WIDE, IMAD (lo), IADD3, DFMA, DADD, LOP3.
-// Reports warp-instructions per clock per SM.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipe_bench pipe_bench.cu
+// Issue-rate micro-benchmark for the pipes the modular butterflies use: IMAD.WIDE, IMAD (lo), IADD3, DFMA, DADD, LOP3.
+// Reports warp-instructions per clock per SM.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipe_bench pipe_bench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 typedef unsigned long long u64;

@@ -1,4 +1,4 @@
-"""Randomised cross-check of the tcgen05 scalar-MAC kernel against the FP64 scalar-MAC kernel (both on the GPU, bit-exact expected):
+"""Randomised cross-check of the wgmma scalar-MAC kernel against the FP64 scalar-MAC kernel (both on the GPU, bit-exact expected):
 random dense shapes and random strided/padded convolutions over a slab of ciphertexts, weights up to +-254, random biases.
 usage: python tools/umma_stress.py [cases] [seed]"""
 import os, sys
