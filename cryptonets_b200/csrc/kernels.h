@@ -24,7 +24,12 @@ struct NttTab {
     // N = 16384 runs as two half-size transforms on a CTA pair (ntt.cu, "split"): wd_hi / iwd_hi then hold the two halves' twiddle
     // tables ([half][8192], indexed like wd / iwd of an 8192-point transform) and this is the forward schedule of the passes 1+5 | 4 | 4
     unsigned fwd_recenter_split;
-    int fwd_out_rc;                     // lazy forward output must be re-centred (its bound squared would overflow the consumer's product)
+    // N = 4096 / 8192: the two halves' forward twiddle tables ([half][N/2]) of the fused key switch, which runs the same split form
+    // (fwd_recenter_split is then its schedule: passes 1+(logN-9) | 4 | 4); split_ok = 1 when that schedule is exact, split_out_rc is
+    // fwd_out_rc for its output
+    const double *wd_split;
+    int split_ok, split_out_rc;
+    int fwd_out_rc;                    // lazy forward output must be re-centred (its bound squared would overflow the consumer's product)
     double fwd_out_bound;               // |forward lazy output| <= fwd_out_bound * p
 };
 
@@ -53,6 +58,11 @@ cudaError_t launch_ntt_inverse(const u64 *src, u64 *dst, int n_polys, int logn, 
 // ciphertext c's k-residue target polynomial starts at target + c * ct_stride (words)
 cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *dst, int n_ct, int k, const DigitMap &dm, int logn,
                                       const NttTab *tabs, int fp, cudaStream_t s);
+// Fused key-switch inner product (N = 4096 / 8192, FP64 path, lazy output): acc[c][p][l] = sum_d NTT_l(digit d of target[c]) * key[d][p][l],
+// key [D][2][k][N] canonical NTT form, acc [n_ct][2][k][N] lazy doubles (|x| <= 0.51 p) -- what launch_ntt_forward_digits followed by
+// launch_ks_mac_fp(lazy) compute, with no digit buffer
+cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, u64 *acc, int n_ct, int k, const DigitMap &dm, int logn,
+                                    const NttTab *tabs, cudaStream_t s);
 // dst[b] = INTT(src[b]) + base[(b / base_group) * base_stride + (b % base_group) * N]  (mod p)
 cudaError_t launch_ntt_inverse_add(const u64 *src, const u64 *base, int base_group, size_t base_stride, u64 *dst, int n_polys, int logn,
                                    const NttTab *tabs, int mod_base, int mod_count, int fp, cudaStream_t s);

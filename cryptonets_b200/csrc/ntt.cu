@@ -1022,6 +1022,152 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
     inv_split_last<OUT_F>(sm, twc, d, ba, tb, tid, half);
 }
 
+// ================================================================ fused key switch, N = 4096 / 8192
+// acc[c][p][l] = sum_d NTT_l(digit_d(target_c)) * key[d][p][l]  without the digit transforms ever reaching HBM.  The digit path
+// (k_ntt_forward_digits_fp + k_ks_mac_tma) writes every digit transform as lazy doubles and reads it back once: 2 x 64 KiB per transform at
+// N = 8192, 31 GB per CryptoNets step, more than the FP64 work of the transforms costs on an H100.  Here a CTA owns one half of the
+// transform of one (ciphertext c, residue l) and walks all D digits: after the first stage the two halves of an N-point transform are
+// independent N/2-point transforms (the split form of the N = 16384 kernels), so CTA h folds stage 0 into its loads (it reads both halves
+// of the source residue, an L2 hit: the partner and the other residues' CTAs read the same lines at about the same time), runs the
+// N/2-point passes in shared memory and, in the last pass, multiplies its 16 coefficients per thread by the matching key words and
+// accumulates them in shared memory ([key poly][coefficient pair][thread]: every thread touches only its own slots, no extra barrier).
+// The twiddle cache is filled once per CTA instead of once per transform, and the next digit's source words are in flight while the CTA
+// waits at the barrier that ends the current digit.  Same arithmetic as the MAC kernels (fmodmul + dadd, re-centred every 8 digits and
+// at the end), so the accumulator leaves with |x| <= 0.51 p in the layout launch_ntt_inverse_add consumes.
+template <int HLOGN>
+__host__ __device__ constexpr int ks_fused_threads() { return (1 << HLOGN) / 16; }
+template <int HLOGN>
+__host__ __device__ constexpr int ks_fused_smem() { return (1 << HLOGN) * 8 * 3 + TWC * 8; } // work buffer, two accumulators, twiddle cache
+template <int HLOGN>
+__global__ void __launch_bounds__(ks_fused_threads<HLOGN>(), HLOGN == 12 ? 2 : 4)
+k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *__restrict__ key, u64 *__restrict__ acc, const NttTab *__restrict__ tabs,
+                   int k, DigitMap dm) {
+    constexpr int H = 1 << HLOGN, TR = ks_fused_threads<HLOGN>(), N = 2 * H;
+    constexpr int R1 = HLOGN - 8, E1 = 1 << R1, LG1 = HLOGN - R1; // first pass: stage 0 on the loads, then R1 stages; then 4 + 4
+    extern __shared__ __align__(16) u64 ks_raw[];
+    double *sm = reinterpret_cast<double *>(ks_raw);
+    double *twc = sm + H;
+    double2 *accv = reinterpret_cast<double2 *>(twc + TWC); // [p][e/2][TR]
+    const int half = blockIdx.x & 1, l = (blockIdx.x >> 1) % k, c = (blockIdx.x >> 1) / k, tid = threadIdx.x;
+    NttTab tb = tabs[l];
+    const double w0 = __ldg(tb.wd + 1);
+    tb.wd = tb.wd_split + half * H;
+    tb.fwd_recenter = tb.fwd_recenter_split;
+    const double p = tb.pd, pinv = tb.pinv;
+    const bool need_reduce = dm.mask >= tb.mod.p;
+    const u64 *src_c = target + (size_t)c * ct_stride;
+    const size_t kpoly = (size_t)k * N, kstride = 2 * kpoly;
+    const u64 *key_l = key + (size_t)l * N + half * H + 16 * tid;
+    load_twiddle_cache(twc, tb.wd, tid, TR);
+#pragma unroll
+    for (int i = 0; i < 16; i++) accv[i * TR + tid] = make_double2(0.0, 0.0);
+    auto cut = [&](u64 v, int shift) { // digit of a canonical word: exact below 2^50
+        const double x = u2d((v >> shift) & dm.mask);
+        return need_reduce ? frecenter(x, p, pinv) : x;
+    };
+#pragma unroll 1
+    for (int d = 0; d < dm.D; d++) {
+        const u64 *src = src_c + (size_t)dm.src[d] * N;
+        const int shift = dm.shift[d];
+        constexpr int VT1 = (H >> R1) / TR; // first-pass virtual threads per thread
+        double xs[VT1][E1]; // stage 0 of the N-point transform, computed while other warps finish the previous digit
+#pragma unroll
+        for (int v = 0; v < VT1; v++)
+#pragma unroll
+            for (int e = 0; e < E1; e++) {
+                const int idx = tid + v * TR + (e << LG1);
+                const double a = cut(src[idx], shift), t = fmodmul(cut(src[idx + H], shift), w0, p, pinv);
+                xs[v][e] = half ? __dsub_rn(a, t) : __dadd_rn(a, t);
+            }
+        __syncthreads(); // the previous digit's last pass is done with the work buffer (d = 0: the twiddle cache is filled)
+#pragma unroll
+        for (int v = 0; v < VT1; v++) {
+            const int vt = tid + v * TR;
+            double (&x)[E1] = xs[v];
+#pragma unroll
+            for (int u = 0; u < R1; u++) {
+                const int h = E1 >> (u + 1);
+#pragma unroll
+                for (int e = 0; e < E1; e++) {
+                    if (e & h) continue;
+                    const double w = twc[(1 << u) + (e >> (R1 - u))];
+                    const double t = fmodmul(x[e + h], w, p, pinv);
+                    const double a = x[e];
+                    x[e] = __dadd_rn(a, t);
+                    x[e + h] = __dsub_rn(a, t);
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < E1; e++) sm[swz(vt + (e << LG1))] = x[e];
+        }
+        __syncthreads();
+        {
+            FwdSrc unused;
+            unused.src = nullptr; unused.digit = false; unused.need_reduce = false; unused.shift = 0; unused.mask = 0;
+            fwd_pass_fp<HLOGN, R1, 4, false, 1, false>(sm, twc, unused, tb, tid);
+        }
+        __syncthreads();
+        // last pass (stages HLOGN-4 .. HLOGN-1 on 16 consecutive coefficients), then the key product
+        constexpr int S0 = HLOGN - 4;
+        const int j = tid, xr = j & 7;
+        const double2 *smv = reinterpret_cast<const double2 *>(sm);
+        double x[16];
+#pragma unroll
+        for (int ch = 0; ch < 8; ch++) {
+            const double2 v = smv[j * 8 + (ch ^ xr)];
+            x[2 * ch] = v.x;
+            x[2 * ch + 1] = v.y;
+        }
+        if ((tb.fwd_recenter >> 2) & 1) {
+#pragma unroll
+            for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
+        }
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int h = 8 >> u;
+#pragma unroll
+            for (int e = 0; e < 16; e++) {
+                if (e & h) continue;
+                const double w = __ldg(tb.wd + (1 << (S0 + u)) + (j << u) + (e >> (4 - u)));
+                const double t = fmodmul(x[e + h], w, p, pinv);
+                const double a = x[e];
+                x[e] = __dadd_rn(a, t);
+                x[e + h] = __dsub_rn(a, t);
+            }
+        }
+        if (tb.split_out_rc) {
+#pragma unroll
+            for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
+        }
+        const bool rc = (d & 7) == 7 || d == dm.D - 1;
+#pragma unroll
+        for (int kp = 0; kp < 2; kp++) {
+            const u64 *kw = key_l + (size_t)d * kstride + kp * kpoly;
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const ulonglong2 w = __ldg(reinterpret_cast<const ulonglong2 *>(kw) + i);
+                double2 a = accv[(kp * 8 + i) * TR + tid];
+                a.x = __dadd_rn(a.x, fmodmul(x[2 * i], u2d(w.x), p, pinv));
+                a.y = __dadd_rn(a.y, fmodmul(x[2 * i + 1], u2d(w.y), p, pinv));
+                if (rc) { // sums of 8 fresh products stay below 4.1 p; re-centre before they could leave the exact range (and at the end)
+                    a.x = frecenter(a.x, p, pinv);
+                    a.y = frecenter(a.y, p, pinv);
+                }
+                accv[(kp * 8 + i) * TR + tid] = a;
+            }
+        }
+    }
+#pragma unroll
+    for (int kp = 0; kp < 2; kp++) {
+        u64 *o = acc + ((size_t)(c * 2 + kp) * k + l) * N + half * H + 16 * tid;
+#pragma unroll
+        for (int g = 0; g < 4; g++) {
+            const double2 a = accv[(kp * 8 + 2 * g) * TR + tid], b = accv[(kp * 8 + 2 * g + 1) * TR + tid];
+            stg256(o + 4 * g, lazy_bits(a.x), lazy_bits(a.y), lazy_bits(b.x), lazy_bits(b.y));
+        }
+    }
+}
+
 // ================================================================ persistent TMA-staged transforms, N = 4096 / 8192
 // One persistent CTA per SM.  Each CTA is pinned to ONE modulus (CTA c serves the polynomials whose table index is c mod #moduli), so
 // the twiddles it needs never change: the 15N/16 twiddles of the four unit-stride stages -- the ones that used to be fetched from L2 by
@@ -1656,6 +1802,21 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
         k_ntt_forward_digits<L><<<n_ct * dm.D * k, (1 << L) / 16, ntt_kernel_smem_bytes(L), s>>>(target, ct_stride, dst, tabs, k, dm);
     });
     return cudaGetLastError();
+}
+template <int HL>
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, u64 *acc, int n_ct, int k, const DigitMap &dm, const NttTab *tabs,
+                                   cudaStream_t s) {
+    cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
+    if (e != cudaSuccess) return e;
+    k_key_switch_fused<HL><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, key, acc, tabs, k, dm);
+    return cudaGetLastError();
+}
+cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, u64 *acc, int n_ct, int k, const DigitMap &dm, int logn,
+                                    const NttTab *tabs, cudaStream_t s) {
+    if (n_ct <= 0) return cudaSuccess;
+    if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, acc, n_ct, k, dm, tabs, s);
+    if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, acc, n_ct, k, dm, tabs, s);
+    return cudaErrorInvalidValue;
 }
 template <int L, bool IN_F, bool OUT_F>
 static cudaError_t launch_inv_fp(const u64 *src, const u64 *base, int base_group, size_t base_stride, u64 *dst, int n_polys, const NttTab *tabs,

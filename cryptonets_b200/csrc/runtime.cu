@@ -344,15 +344,22 @@ static void fp_schedule(NttTab &tb, int logN, bool force_int) {
     double A;
     if (!forward(rad, np, tb.fwd_recenter, A)) return;
     tb.fwd_recenter_split = 0;
-    if (logN == 14) { // CTA-pair form: stage 0 rides on the first pass' loads
-        const int split[3] = {6, 4, 4};
-        double As;
-        if (!forward(split, 3, tb.fwd_recenter_split, As)) return;
-        A = std::max(A, As);
-    }
+    tb.split_ok = tb.split_out_rc = 0;
     // lazy forward output (|x| <= A p) feeds products of two such values (tensor) or of one with a canonical key word: both operands
     // of a modular product may be lazy only while A*A*p stays below 2^51
-    tb.fwd_out_rc = A * A * (double)p >= 0.9 * 2251799813685248.0;
+    auto out_rc = [&](double a) { return a * a * (double)p >= 0.9 * 2251799813685248.0; };
+    if (logN >= 12) { // split form (CTA pairs at N = 16384, the fused key switch at 4096 / 8192): stage 0 rides on the first pass' loads
+        const int split[3] = {logN - 8, 4, 4};
+        double As;
+        tb.split_ok = forward(split, 3, tb.fwd_recenter_split, As);
+        if (logN == 14) {
+            if (!tb.split_ok) return;
+            A = std::max(A, As);
+        } else if (tb.split_ok) {
+            tb.split_out_rc = out_rc(As);
+        }
+    }
+    tb.fwd_out_rc = out_rc(A);
     tb.fwd_out_bound = tb.fwd_out_rc ? 0.51 : A;
     // inverse: canonical or lazy input (tensor output: sum of two fresh products, <= 1.25 p); sums double every stage; bit v
     // re-centres the sums produced by stage v
@@ -474,14 +481,15 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     for (u64 p : c.q) moduli.push_back(p);
     for (u64 p : c.bsk) moduli.push_back(p);
     for (u64 p : c.t) moduli.push_back(p);
-    std::vector<u64> host((size_t)n_mod * 8 * N, 0);
+    constexpr size_t TAB_WORDS = 9; // N-word tables per modulus: w, ws, iw, iws, wd, iwd, wd_hi, iwd_hi, wd_split
+    std::vector<u64> host((size_t)n_mod * TAB_WORDS * N, 0);
     CNHE_CUDA(cudaMalloc((void **)&c.d_table_mem, host.size() * sizeof(u64)));
     c.h_tabs.resize(n_mod);
     for (int m = 0; m < n_mod; m++) {
         const u64 p = moduli[m];
         const u64 psi = hm::minimal_primitive_root(2ULL * N, p), ipsi = hm::inv(psi, p);
-        u64 *w = &host[((size_t)m * 8 + 0) * N], *ws = w + N, *iw = ws + N, *iws = iw + N;
-        double *wd = reinterpret_cast<double *>(iws + N), *iwd = wd + N, *wd_hi = iwd + N, *iwd_hi = wd_hi + N;
+        u64 *w = &host[(size_t)m * TAB_WORDS * N], *ws = w + N, *iw = ws + N, *iws = iw + N;
+        double *wd = reinterpret_cast<double *>(iws + N), *iwd = wd + N, *wd_hi = iwd + N, *iwd_hi = wd_hi + N, *wd_split = iwd_hi + N;
         u64 a = 1, b = 1;
         for (u64 i = 0; i < N; i++) {
             const u64 r = hm::bit_reverse(i, logN);
@@ -512,14 +520,22 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
                 for (int i = 0; i < 2; i++) iwd_hi[(u64)(12 + i) * T + j] = iwd[(N >> 3) + (j << 1) + i];
                 iwd_hi[(u64)14 * T + j] = iwd[(N >> 4) + j];
             }
+            const u64 H = N / 2; // the halves' forward tables of the fused key switch, laid out as wd_hi is at N = 16384
+            for (u64 h = 0; h < 2; h++)
+                for (u64 i = 1; i < H; i++) {
+                    u64 m2 = 1;
+                    while (2 * m2 <= i) m2 *= 2;
+                    wd_split[h * H + i] = wd[i + m2 + h * m2];
+                }
         }
         NttTab &tb = c.h_tabs[m];
-        u64 *base = c.d_table_mem + (size_t)m * 8 * N;
+        u64 *base = c.d_table_mem + (size_t)m * TAB_WORDS * N;
         tb.w = base; tb.ws = base + N; tb.iw = base + 2 * (size_t)N; tb.iws = base + 3 * (size_t)N;
         tb.wd = reinterpret_cast<const double *>(base + 4 * (size_t)N);
         tb.iwd = reinterpret_cast<const double *>(base + 5 * (size_t)N);
         tb.wd_hi = reinterpret_cast<const double *>(base + 6 * (size_t)N);
         tb.iwd_hi = reinterpret_cast<const double *>(base + 7 * (size_t)N);
+        tb.wd_split = reinterpret_cast<const double *>(base + 8 * (size_t)N);
         tb.inv_n = hm::inv(N % p, p);
         tb.inv_n_s = hm::shoup(tb.inv_n, p);
         tb.mod = make_dmod(p);
@@ -744,6 +760,22 @@ void op_ntt(Context &c, const u64 *src, u64 *dst, int n_polys, int mod_base, int
             "ntt");
 }
 
+// Key switches of at least this many ciphertexts run fused (digit transforms and key product in one kernel, ntt.cu): the fused grid has
+// 2k CTAs per ciphertext, each walking all D digits, so small calls leave most of the GPU idle where the digit path spreads n*D*k
+// transforms over it.  tools/keyswitch_bench.py on one H100 SXM (700 W), N = 8192, k = 5, D = 25: fused / digit path 0.53 / 0.52 ms at
+// 32 ciphertexts, 0.87 / 0.99 ms at 64, 11.9 / 14.1 ms at 945
+constexpr int KS_FUSED_MIN = 64;
+// whether a key switch of n ciphertexts takes the fused path: N = 4096 / 8192 on the lazy FP64 path, n >= KS_FUSED_MIN.
+// CNHE_KS_FUSED=0 / =1 forces the digit path / the fused path wherever it is built (read per call: tests compare both in one process)
+static bool ks_fused(const Context &c, int n) {
+    if (c.logN != 12 && c.logN != 13) return false;
+    if (!(c.lazy && c.fp_elementwise && fp_range(c, 0, c.k))) return false;
+    for (int i = 0; i < c.k; i++)
+        if (!c.h_tabs[i].split_ok) return false;
+    const char *v = getenv("CNHE_KS_FUSED");
+    if (v) return atoi(v) != 0;
+    return n >= KS_FUSED_MIN;
+}
 // out[i] = (base_i + sum_d NTT^-1(NTT(digit_d(target_i)) * key_d)): ciphertext i's target polynomial (k residues) is at
 // target + i * target_stride, its base (2 polynomials) at base + i * base_stride; out is packed [n][2][k][N]
 void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, const u64 *key, const DigitMap &dm, const u64 *base,
@@ -752,19 +784,25 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
     const size_t N = c.N;
     const int fpq = fp_range(c, 0, k);
     const bool lazy = c.lazy && fpq;
-    const int wave = c.wave(((size_t)dm.D * k + 2 * k) * N);
+    const bool fused = ks_fused(c, n);
+    const int wave = c.wave(((fused ? 0 : (size_t)dm.D * k) + 2 * k) * N);
     for (int c0 = 0; c0 < n; c0 += wave) {
         WsScope scope(c);
         const int m = std::min(wave, n - c0);
-        u64 *digits = c.ws_alloc((size_t)m * dm.D * k * N);
         u64 *acc = c.ws_alloc((size_t)m * 2 * k * N);
-        {
-            PROF(0, 16.0 * N * (double)m * dm.D * k); // SURVEY 8d: 16N bytes per transform (8N digit source read + 8N written)
-            c.check(launch_ntt_forward_digits(target + (size_t)c0 * target_stride, target_stride, digits, m, k, dm, c.logN, c.d_tabs,
-                                              fpq | (lazy ? NTT_OUT_F : 0), c.stream),
-                    "ntt_forward_digits");
-        }
-        {
+        if (fused) {
+            // HBM: the target residues once (the pair and the other residues' CTAs share them through L2), the keys once, the accumulator
+            PROF(3, 8.0 * N * ((double)m * k + (double)dm.D * 2 * k + (double)m * 2 * k));
+            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, key, acc, m, k, dm, c.logN, c.d_tabs, c.stream),
+                    "key_switch_fused");
+        } else {
+            u64 *digits = c.ws_alloc((size_t)m * dm.D * k * N);
+            {
+                PROF(0, 16.0 * N * (double)m * dm.D * k); // SURVEY 8d: 16N bytes per transform (8N digit source read + 8N written)
+                c.check(launch_ntt_forward_digits(target + (size_t)c0 * target_stride, target_stride, digits, m, k, dm, c.logN, c.d_tabs,
+                                                  fpq | (lazy ? NTT_OUT_F : 0), c.stream),
+                        "ntt_forward_digits");
+            }
             PROF(3, 8.0 * N * ((double)m * dm.D * k + (double)dm.D * 2 * k + (double)m * 2 * k));
             if (c.fp_elementwise) c.check(launch_ks_mac_fp(digits, key, acc, m, dm.D, k, c.logN, &c.h_bf, lazy, c.stream), "ks_mac_fp");
             else c.check(launch_ks_mac(digits, key, acc, m, dm.D, k, c.logN, c.d_bc, c.stream), "ks_mac");
@@ -842,7 +880,7 @@ void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, co
     if (!c.ch[ch].have_rlk) throw Error(-3, "relinearization keys are missing");
     const int n = (int)a.size(), k = c.k;
     const size_t N = c.N;
-    const int wave = c.wave(((size_t)c.dm_relin.D * k + 7 * (k + c.kb) + 5 * k) * N);
+    const int wave = c.wave(((ks_fused(c, n) ? 0 : (size_t)c.dm_relin.D * k) + 7 * (k + c.kb) + 5 * k) * N);
     for (int c0 = 0; c0 < n; c0 += wave) {
         WsScope scope(c); // stream-ordered frees: the next wave reuses the memory once these kernels are done
         const int m = std::min(wave, n - c0);

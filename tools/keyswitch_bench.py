@@ -1,0 +1,65 @@
+"""Key-switch micro-benchmark: relinearisation of n size-3 ciphertexts through the raw ABI (N=8192, SEAL default q, dbc=10, one
+stream), per-family device times and the HBM bytes the two key-switch forms need, computed from the shapes.
+
+    python tools/keyswitch_bench.py [n ...] [--iters I] [--path auto|fused|digits]
+
+During a relinearise-only call family 0 (ntt_forward) is the digit transforms alone, family 3 (keyswitch_mac) the key product -- or,
+on the fused path, digit transforms and key product together -- and family 1 (ntt_inverse) the inverse transforms with the base
+addition.  `--path` sets CNHE_KS_FUSED for the run (auto: the library's own choice by n).  One JSON line per n."""
+import argparse, json, os, sys
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np
+
+ap = argparse.ArgumentParser()
+ap.add_argument("n", type=int, nargs="*", default=[1, 8, 32, 64, 128, 945])
+ap.add_argument("--iters", type=int, default=5)
+ap.add_argument("--path", choices=["auto", "fused", "digits"], default="auto")
+args = ap.parse_args()
+if args.path != "auto":
+    os.environ["CNHE_KS_FUSED"] = "1" if args.path == "fused" else "0"
+
+from cryptonets_b200.engine import Engine
+
+eng = Engine([549764251649], 8192, 10, 20)
+eng.keygen(1)
+eng.set_option("multi_stream", 0)
+k, N = eng.k, 8192
+D = sum((int(q).bit_length() + 9) // 10 for q in eng.q)  # base-2^10 digits of every residue
+q = np.array(eng.q, dtype=np.uint64)
+rng = np.random.default_rng(0)
+# FP64 warp instructions per (ciphertext, residue, half) and digit of the fused kernel at N = 8192 (4096-point halves, 256 threads, 16
+# coefficients each): stage 0 folded into the loads (16 modular products + 16 adds), 12 radix-2 stages of 8 butterflies (6 + 2), the key
+# product (32 modular products + 32 adds), digit conversions (32 u2d) and key conversions (32 u2d)
+FMODMUL, BFLY = 6, 8
+DP_PER_THREAD = 16 * (FMODMUL + 1) + 12 * 8 * BFLY + 32 * (FMODMUL + 1) + 32 + 32
+DP_WARP_INSTR_PER_CT = DP_PER_THREAD * (256 // 32) * 2 * k * D
+for n in args.n:
+    host = (rng.integers(0, 1 << 62, (n, 3, k, N), dtype=np.uint64) % q[None, None, :, None]).astype(np.uint64)
+    a = eng.dev_from(host)
+    out = eng.dev_alloc(n * 2 * k * N)
+    for _ in range(2):
+        eng.raw_relinearize(0, a, n, out)
+    eng.sync()
+    eng.prof_enable(True)
+    eng.timer_start()
+    for _ in range(args.iters):
+        eng.raw_relinearize(0, a, n, out)
+    ms = eng.timer_stop_ms() / args.iters
+    prof = eng.prof_collect()
+    eng.prof_enable(False)
+    fam = {k_: round(v["ms"] / args.iters, 3) for k_, v in prof.items() if v["ms"] > 0}
+    fused = prof["ntt_forward"]["launches"] == 0
+    w = 8.0 * N
+    bytes_digits = w * (n * k * D * 2 + n * k * D + D * 2 * k + n * 2 * k)  # digit source + digits written, digits + keys read, acc written
+    bytes_fused = w * (n * k + D * 2 * k + n * 2 * k)  # target residues, keys, acc
+    bytes_inverse = w * (n * 2 * k * 3)  # acc read, base read, out written
+    rec = {"n": n, "path": "fused" if fused else "digits", "ms": round(ms, 3), "us_per_ct": round(ms * 1e3 / n, 2), "families_ms": fam,
+           "hbm_bytes": {"digits_path": bytes_digits + bytes_inverse, "fused_path": bytes_fused + bytes_inverse}}
+    if fused and fam.get("keyswitch_mac"):
+        rate = DP_WARP_INSTR_PER_CT * n / (fam["keyswitch_mac"] * 1e-3)
+        rec["fused_fp64_warp_instr_per_s"] = float("%.4g" % rate)
+        rec["fused_fp64_issue_share"] = round(rate / 522.7e9, 3)  # 132 SMs x 2 FP64 warp instructions / clock x 1.98 GHz
+    print(json.dumps(rec), flush=True)
+    eng.dev_free(a)
+    eng.dev_free(out)
+eng.close()
