@@ -58,6 +58,8 @@ _SIGS = {
     "cnhe_vecs_export_raw": [C.c_void_p, C.POINTER(VECP), i32, U64P, sz],
     "cnhe_vecs_export_raw_async": [C.c_void_p, C.POINTER(VECP), i32, U64P, sz, C.POINTER(i32)],
     "cnhe_export_wait": [C.c_void_p, i32],
+    "cnhe_vecs_encrypt_compact": [C.c_void_p, DBLP, i32, u64, C.c_double, C.c_void_p, sz, C.POINTER(sz)],
+    "cnhe_vecs_import_compact": [C.c_void_p, C.c_void_p, sz, C.POINTER(VECP), i32, C.POINTER(i32)],
     "cnhe_dev_copy": [C.c_void_p, u64, u64, sz],
     "cnhe_prof_enable": [C.c_void_p, i32],
     "cnhe_prof_collect": [C.c_void_p, i32, DBLP, U64P, DBLP],

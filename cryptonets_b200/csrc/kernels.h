@@ -234,6 +234,27 @@ cudaError_t launch_decode_gather(const u64 *plain_ntt, u64 *values, int n, const
 // ct[i] (already u*pk, coefficient form) += (e0 + Delta*m_i, e1)
 cudaError_t launch_encrypt_finish(u64 *ct, const u64 *plain, size_t plain_stride, int n, int coeffs, const RngKey &seed, u64 nonce0, int k, int logn,
                                   const BehzConst *bc, PlainConst pc, cudaStream_t s);
+// secret-key variant: ct[i] part 0 = -as[i] + e + Delta*m_i, part 1 (a) untouched; as [n][k][N] = a*s in coefficient form
+cudaError_t launch_encrypt_finish_sk(u64 *ct, const u64 *as, const u64 *plain, size_t plain_stride, int n, int coeffs, const RngKey &seed, u64 nonce0,
+                                     int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
+
+// ---- compact ciphertext upload (compact.cu; format in its header comment)
+// stream-id purposes no other sampler call uses: the expanded c1, the noise e of a secret-key encryption, a test-seeded expansion key
+constexpr u64 PURPOSE_COMPACT_A = 11, PURPOSE_COMPACT_E = 12, PURPOSE_COMPACT_KEY = 13;
+struct CompactKey {
+    u32 w[8]; // ChaCha20 key K_c (the 32 header bytes as little-endian words)
+};
+struct CompactShape {
+    int k, logn;
+    int bits[KMAX];      // b_l = bitlen(q_l)
+    u64 off[KMAX + 1];   // word offset of residue l inside one packed ciphertext; off[k] = words per ciphertext
+};
+// ct[j] = (c0 unpacked from packed[j] and made canonical, c1 expanded from key under ciphertext index j0 + j), j < n; packed == null:
+// only c1 is written
+cudaError_t launch_compact_expand(u64 *ct, const u64 *packed, const CompactKey &key, u64 j0, int n, const CompactShape &sh, const BehzConst *bc,
+                                  cudaStream_t s);
+// packed[j] = bit-packed c0 of ct[j] (canonical residues), j < n
+cudaError_t launch_pack_residues(const u64 *ct, u64 *packed, int n, const CompactShape &sh, cudaStream_t s);
 // x[n][k][N] = c0 + c1*s (coefficient form) -> plain[n][N]
 cudaError_t launch_decrypt_round(const u64 *x, u64 *plain, int n, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
 cudaError_t launch_fill_zero(u64 *p, size_t words, cudaStream_t s);

@@ -344,6 +344,25 @@ __global__ void __launch_bounds__(256) k_encrypt_finish(u64 *ct, const u64 *__re
     }
     ct[i] = v;
 }
+// secret-key encryption: part 0 = -(a s) + e + Delta*m (the same Delta and upper-half handling as above), part 1 = a stays as written
+__global__ void __launch_bounds__(256) k_encrypt_finish_sk(u64 *ct, const u64 *__restrict__ as, const u64 *__restrict__ plain, size_t plain_stride,
+                                                          int n, int coeffs, RngKey seed, u64 nonce0, int k, int logn, const BehzConst *__restrict__ bc,
+                                                          PlainConst pc) {
+    const int N = 1 << logn;
+    const size_t kN = (size_t)k * N;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)n * kN) return;
+    const size_t c = i / kN, r = i % kN;
+    const int l = (int)(r >> logn), x = (int)(r & (N - 1));
+    const DMod q = bc->q[l];
+    const u64 sid = stream_id(PURPOSE_COMPACT_E, nonce0 + c, 0);
+    u64 v = addmod(negmod(as[i], q.p), lift_small(draw_noise(rng64(seed, sid, x)), q.p), q.p);
+    if (x < coeffs) {
+        const u64 m = plain[c * plain_stride + x];
+        if (m) v = addmod(v, scale_plain(m, l, q, pc), q.p);
+    }
+    ct[c * 2 * kN + r] = v;
+}
 __global__ void __launch_bounds__(256) k_fill_zero(u64 *p, size_t words) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < words) p[i] = 0;
@@ -456,6 +475,12 @@ cudaError_t launch_encrypt_finish(u64 *ct, const u64 *plain, size_t plain_stride
                                   const BehzConst *bc, PlainConst pc, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     k_encrypt_finish<<<blocks_for(((size_t)n * 2 * k) << logn), 256, 0, s>>>(ct, plain, plain_stride, n, coeffs, seed, nonce0, k, logn, bc, pc);
+    return cudaGetLastError();
+}
+cudaError_t launch_encrypt_finish_sk(u64 *ct, const u64 *as, const u64 *plain, size_t plain_stride, int n, int coeffs, const RngKey &seed, u64 nonce0,
+                                     int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    k_encrypt_finish_sk<<<blocks_for(((size_t)n * k) << logn), 256, 0, s>>>(ct, as, plain, plain_stride, n, coeffs, seed, nonce0, k, logn, bc, pc);
     return cudaGetLastError();
 }
 cudaError_t launch_fill_zero(u64 *p, size_t words, cudaStream_t s) {

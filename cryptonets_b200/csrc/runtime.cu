@@ -1105,6 +1105,65 @@ void op_encrypt(Context &c, int chi, const u64 *plain, size_t plain_stride, int 
     }
     c.note(Context::OP_ENCRYPT, chi, n, ct);
 }
+CompactShape compact_shape(const Context &c) {
+    CompactShape sh;
+    memset(&sh, 0, sizeof(sh));
+    sh.k = c.k;
+    sh.logn = c.logN;
+    for (int l = 0; l < c.k; l++) {
+        sh.bits[l] = 64 - __builtin_clzll(c.q[l]);
+        sh.off[l + 1] = sh.off[l] + ((u64)c.N * sh.bits[l]) / 64; // N >= 64: every residue fills whole words
+    }
+    return sh;
+}
+CompactKey compact_key(Context &c, int chi, u64 nonce0) {
+    const Channel &ch = c.ch[chi];
+    CompactKey key;
+    if (ch.rng.secure) {
+        RngKey fresh;
+        rng_from_os(fresh);
+        memcpy(key.w, fresh.key, sizeof(key.w));
+    } else {
+        for (int i = 0; i < 4; i++) {
+            const u64 w = rng64(ch.rng, stream_id(PURPOSE_COMPACT_KEY, nonce0, 0), (u64)i);
+            key.w[2 * i] = (u32)w;
+            key.w[2 * i + 1] = (u32)(w >> 32);
+        }
+    }
+    return key;
+}
+// (c0, c1) = (-(a s) + e + Delta m, a): a from the expansion key (the server regenerates it), e fresh per ciphertext from the channel's sampler
+void op_encrypt_compact(Context &c, int chi, const u64 *plain, int n, u64 nonce0, const CompactKey &key, u64 *packed) {
+    Channel &ch = c.ch[chi];
+    if (!ch.have_sk) throw Error(-3, "secret key is missing");
+    const int k = c.k;
+    const size_t N = c.N, kN = (size_t)k * N;
+    const CompactShape sh = compact_shape(c);
+    for (int c0 = 0; c0 < n; c0 += 4 * c.chunk) {
+        WsScope scope(c);
+        const int m = std::min(4 * c.chunk, n - c0);
+        u64 *ct = c.ws_alloc((size_t)m * 2 * kN), *as = c.ws_alloc((size_t)m * kN);
+        c.check(launch_compact_expand(ct, nullptr, key, (u64)c0, m, sh, c.d_bc, c.stream), "compact_expand(a)");
+        CNHE_CUDA(cudaMemcpy2DAsync(as, kN * 8, ct + kN, 2 * kN * 8, kN * 8, m, cudaMemcpyDeviceToDevice, c.stream));
+        c.check(launch_ntt_forward(as, as, m * k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_forward");
+        c.check(launch_dyadic_bcast(as, ch.sk->p, as, m, 1, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic");
+        c.check(launch_ntt_inverse(as, as, m * k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_inverse");
+        c.check(launch_encrypt_finish_sk(ct, as, plain + (size_t)c0 * N, N, m, (int)N, ch.rng, nonce0 + c0, k, c.logN, c.d_bc, ch.pc, c.stream),
+                "encrypt_finish_sk");
+        c.check(launch_pack_residues(ct, packed + (size_t)c0 * sh.off[k], m, sh, c.stream), "pack_residues");
+        if (c0 == 0) c.note(Context::OP_ENCRYPT, chi, n, ct); // the first ciphertext is alive only in this wave
+    }
+}
+void op_compact_expand(Context &c, const u64 *packed, const CompactKey &key, int n, u64 *ct, cudaStream_t s) {
+    const CompactShape sh = compact_shape(c);
+    cudaStream_t keep = c.stream;
+    c.stream = s; // the profiling events go on the stream the kernel runs on
+    {
+        ProfScope ps(c, 5, (double)n * (sh.off[c.k] + c.ct_words()) * 8);
+        c.check(launch_compact_expand(ct, packed, key, 0, n, sh, c.d_bc, s), "compact_expand");
+    }
+    c.stream = keep;
+}
 static void dot_with_secret(Context &c, int chi, const u64 *ct, int n, u64 *x) {
     Channel &ch = c.ch[chi];
     if (!ch.have_sk) throw Error(-3, "secret key is missing");

@@ -223,6 +223,14 @@ void op_encode_onehot(Context &c, int ch, int n, int first_col, u64 *plain);
 u64 take_nonces(Context &c, int ch, u64 n);
 void op_encrypt(Context &c, int ch, const u64 *plain, size_t plain_stride, int n, int coeffs, u64 nonce0, u64 *ct);
 void op_decrypt(Context &c, int ch, const u64 *ct, int n, u64 *plain);
+// ---- compact ciphertext upload (format: compact.cu)
+CompactShape compact_shape(const Context &c); // bit lengths of the q_l and the packed word offsets of one ciphertext
+// expansion key K_c of one blob: a fresh OS draw on a secure channel; four words of the seeded sampler on a test channel (reproducible)
+CompactKey compact_key(Context &c, int ch, u64 nonce0);
+// seeded secret-key encryption of plain [n][N] (coefficient form) under nonces nonce0.. and key K_c -> packed c0 [n][off[k]] (device)
+void op_encrypt_compact(Context &c, int ch, const u64 *plain, int n, u64 nonce0, const CompactKey &key, u64 *packed);
+// packed [n][off[k]] + K_c -> ct [n][2kN] on stream s (timed as family 5 when profiling)
+void op_compact_expand(Context &c, const u64 *packed, const CompactKey &key, int n, u64 *ct, cudaStream_t s);
 int op_noise_budget(Context &c, int ch, const u64 *ct);
 
 } // namespace cnhe

@@ -677,6 +677,124 @@ extern "C" int cnhe_vecs_import_raw(cnhe_ctx *h, const uint64_t *src, int n, int
     }
     API_END
 }
+// ---------------------------------------------------------------------------------------- compact upload (format: csrc/compact.cu)
+static size_t compact_header_bytes(int k, int P) { return 44 + 8 * (size_t)k + 40 * (size_t)P; }
+struct CompactHeader {
+    uint32_t n = 0, B = 0;
+    uint64_t dim = 0;
+    double scale = 1;
+    std::vector<CompactKey> keys;
+    size_t header_bytes = 0, channel_words = 0; // packed words per channel
+};
+// the blob's header checked against the context; any mismatch is CNHE_ERR_INVALID
+static CompactHeader parse_compact(const Context &c, const uint8_t *src, size_t len) {
+    auto rd32 = [&](size_t off) { uint32_t v; memcpy(&v, src + off, 4); return v; };
+    auto rd64 = [&](size_t off) { uint64_t v; memcpy(&v, src + off, 8); return v; };
+    if (len < 44) fail("compact blob: truncated header");
+    if (memcmp(src, "CNHC", 4) != 0) fail("compact blob: bad magic");
+    if (rd32(4) != 1) fail("compact blob: unsupported version");
+    const uint32_t N = rd32(8), k = rd32(12), P = rd32(16);
+    if (N != c.N) fail("compact blob: ring dimension differs from the context's");
+    if ((int)k != c.k) fail("compact blob: coefficient modulus count differs from the context's");
+    if ((int)P != c.P) fail("compact blob: plaintext modulus count differs from the context's");
+    CompactHeader hd;
+    hd.header_bytes = compact_header_bytes(c.k, c.P);
+    if (len < hd.header_bytes) fail("compact blob: truncated header");
+    hd.n = rd32(20);
+    hd.B = rd32(24);
+    hd.dim = rd64(28);
+    memcpy(&hd.scale, src + 36, 8);
+    for (int l = 0; l < c.k; l++)
+        if (rd64(44 + 8 * (size_t)l) != c.q[l]) fail("compact blob: coefficient modulus differs from the context's");
+    for (int ch = 0; ch < c.P; ch++)
+        if (rd64(44 + 8 * (size_t)c.k + 8 * (size_t)ch) != c.t[ch]) fail("compact blob: plaintext modulus differs from the context's");
+    if (hd.n < 1 || hd.B < 1) fail("compact blob: empty");
+    if ((uint64_t)hd.n * hd.B >= (1ULL << 32) || hd.n > (uint32_t)INT_MAX) fail("compact blob: too many ciphertexts");
+    if (hd.dim < 1 || (hd.dim + c.N - 1) / c.N != hd.B) fail("compact blob: dimension does not match the block count");
+    if (!std::isfinite(hd.scale) || hd.scale == 0) fail("compact blob: bad scale");
+    hd.keys.resize(c.P);
+    for (int ch = 0; ch < c.P; ch++) memcpy(hd.keys[ch].w, src + 44 + 8 * (size_t)(c.k + c.P) + 32 * (size_t)ch, 32);
+    hd.channel_words = (size_t)hd.n * hd.B * compact_shape(c).off[c.k];
+    if (len != hd.header_bytes + (size_t)c.P * hd.channel_words * 8) fail("compact blob: length does not match the header");
+    return hd;
+}
+extern "C" int cnhe_vecs_encrypt_compact(cnhe_ctx *h, const double *v, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap, size_t *needed) {
+    API_BEGIN(h)
+    if (n < 1 || dim < 1 || !v || (!dst && !needed)) fail("bad arguments");
+    if (scale == 0) scale = 1;
+    const size_t N = c.N;
+    const uint64_t bl = (dim + N - 1) / N, nct = (uint64_t)n * bl;
+    if (nct >= (1ULL << 32)) fail("too many ciphertexts in one blob");
+    const CompactShape sh = compact_shape(c);
+    const size_t hdr = compact_header_bytes(c.k, c.P), per_ch = (size_t)nct * sh.off[c.k] * 8, total = hdr + (size_t)c.P * per_ch;
+    if (needed) *needed = total;
+    if (!dst) return CNHE_OK;
+    if (cap < total) fail("destination too small");
+    for (int ch = 0; ch < c.P; ch++)
+        if (!c.ch[ch].have_sk) throw Error(CNHE_ERR_STATE, "secret key is missing");
+    std::vector<std::vector<u64>> split;
+    split_values(c, v, (uint64_t)n * dim, scale, split);
+    std::vector<CompactKey> keys(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        std::vector<u64> padded((size_t)nct * N, 0);
+        for (int i = 0; i < n; i++) memcpy(&padded[(size_t)i * bl * N], &split[ch][(size_t)i * dim], dim * 8);
+        u64 *dvals = c.ws_alloc(padded.size()), *plain = c.ws_alloc(padded.size()), *packed = c.ws_alloc((size_t)nct * sh.off[c.k]);
+        CNHE_CUDA(cudaMemcpyAsync(dvals, padded.data(), padded.size() * 8, cudaMemcpyHostToDevice, c.stream));
+        op_encode(c, ch, dvals, (int)nct, (int)N, plain);
+        const u64 nonce0 = take_nonces(c, ch, nct);
+        keys[ch] = compact_key(c, ch, nonce0);
+        op_encrypt_compact(c, ch, plain, (int)nct, nonce0, keys[ch], packed);
+        CNHE_CUDA(cudaMemcpyAsync(dst + hdr + ch * per_ch, packed, per_ch, cudaMemcpyDeviceToHost, c.stream));
+        c.sync();
+    }
+    auto wr32 = [&](size_t off, uint32_t x) { memcpy(dst + off, &x, 4); };
+    auto wr64 = [&](size_t off, uint64_t x) { memcpy(dst + off, &x, 8); };
+    memcpy(dst, "CNHC", 4);
+    wr32(4, 1);
+    wr32(8, c.N);
+    wr32(12, (uint32_t)c.k);
+    wr32(16, (uint32_t)c.P);
+    wr32(20, (uint32_t)n);
+    wr32(24, (uint32_t)bl);
+    wr64(28, dim);
+    memcpy(dst + 36, &scale, 8);
+    for (int l = 0; l < c.k; l++) wr64(44 + 8 * (size_t)l, c.q[l]);
+    for (int ch = 0; ch < c.P; ch++) wr64(44 + 8 * (size_t)c.k + 8 * (size_t)ch, c.t[ch]);
+    for (int ch = 0; ch < c.P; ch++) memcpy(dst + 44 + 8 * (size_t)(c.k + c.P) + 32 * (size_t)ch, keys[ch].w, 32);
+    API_END
+}
+// Like cnhe_vecs_import_raw: the packed bytes go to a staging upload slot on the upload stream, k_compact_expand writes the ciphertexts
+// into a persistent upload slot on the same stream, and the channel's stream waits for it -- the call returns at once.
+extern "C" int cnhe_vecs_import_compact(cnhe_ctx *h, const uint8_t *src, size_t len, cnhe_vec **out, int cap, int *n) {
+    API_BEGIN(h)
+    if (!src || !out || !n) fail("bad arguments");
+    const CompactHeader hd = parse_compact(c, src, len);
+    *n = (int)hd.n;
+    if (cap < (int)hd.n) fail("output array too small for the blob's vectors");
+    const int nct = (int)(hd.n * hd.B);
+    const size_t per = (size_t)hd.B * c.ct_words();
+    std::vector<BufRef> big(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        BufRef stage = c.alloc_upload(hd.channel_words, c.copy_stream); // released behind the expansion on the upload stream
+        CNHE_CUDA(cudaMemcpyAsync(stage->p, src + hd.header_bytes + (size_t)ch * hd.channel_words * 8, hd.channel_words * 8, cudaMemcpyHostToDevice,
+                                  c.copy_stream));
+        big[ch] = c.alloc_upload((size_t)nct * c.ct_words(), c.stream);
+        op_compact_expand(c, stage->p, hd.keys[ch], nct, big[ch]->p, c.copy_stream);
+        CNHE_CUDA(cudaEventRecord(c.ev_copy, c.copy_stream));
+        CNHE_CUDA(cudaStreamWaitEvent(c.stream, c.ev_copy, 0));
+    }
+    for (uint32_t i = 0; i < hd.n; i++) {
+        cnhe_vec *o = new_vec(c, hd.dim, hd.scale, CNHE_DENSE, true, (int)hd.B);
+        for (int ch = 0; ch < c.P; ch++) {
+            o->buf[ch] = big[ch];
+            o->off[ch] = (size_t)i * per;
+        }
+        out[i] = o;
+    }
+    API_END
+}
 extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap) {
     API_BEGIN(h)
     if (n < 1 || !dst) fail("bad arguments");

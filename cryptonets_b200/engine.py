@@ -317,6 +317,37 @@ class Engine:
         check(self.L.cnhe_vecs_import_raw(self.h, src, n, blocks, int(dim), float(scale), fmt, out))
         return self._wrap_many(out, n)
 
+    def encrypt_compact(self, rows, scale=1.0):
+        """Seeded secret-key encryption of n dense vectors (rows [n][dim]) into one compact blob (bytes): bit-packed c0 plus one ChaCha20
+        key per plaintext modulus from which import_compact regenerates c1 on the GPU.  Needs the secret key."""
+        a = np.ascontiguousarray(rows, dtype=np.float64)
+        n, dim = a.shape
+        need = C.c_size_t()
+        check(self.L.cnhe_vecs_encrypt_compact(self.h, a.ctypes.data_as(DBLP), n, dim, float(scale), None, 0, C.byref(need)))
+        buf = (C.c_ubyte * need.value)()
+        check(self.L.cnhe_vecs_encrypt_compact(self.h, a.ctypes.data_as(DBLP), n, dim, float(scale), buf, need.value, C.byref(need)))
+        return bytes(buf)
+
+    def import_compact(self, buf_or_ptr, length=None):
+        """The vectors of a compact blob (bytes-like, or a host address with `length`, e.g. a pinned torch tensor's data_ptr()) as ordinary
+        encrypted dense vectors; asynchronous like import_raw_many.  Pinned memory must stay unchanged until the vectors are consumed."""
+        if isinstance(buf_or_ptr, int):
+            if length is None:
+                raise ValueError("length is required with a host address")
+            src, size = C.c_void_p(buf_or_ptr), int(length)
+            head = C.string_at(buf_or_ptr, min(size, 24))
+        else:
+            mv = memoryview(buf_or_ptr).cast("B")
+            size = mv.nbytes if length is None else int(length)
+            arr = np.frombuffer(mv, dtype=np.uint8)
+            src = C.c_void_p(arr.ctypes.data)
+            head = bytes(mv[:24])
+        cap = int.from_bytes(head[20:24], "little") if len(head) >= 24 else 0
+        out = (VECP * max(cap, 1))()
+        n = C.c_int()
+        check(self.L.cnhe_vecs_import_compact(self.h, src, size, out, cap, C.byref(n)))
+        return self._wrap_many(out, n.value)
+
     def export_raw_many(self, vecs, host_ptr=None):
         n, blocks = len(vecs), vecs[0].blocks
         words = self.P * n * blocks * self.ct_words

@@ -314,6 +314,16 @@ class B200BfvFactory:
         vecs = [B200BfvVector(self, v) for v in self.engine.encrypt_many(rows, scale)]
         return B200BfvMatrix(self, vecs, fmt, CopyVectors=False)
 
+    def GetEncryptedMatrixCompact(self, m, fmt, scale):
+        """The same encryption as GetEncryptedMatrix as one compact blob (bytes) for a server: bit-packed c0 and per-channel ChaCha20 keys
+        for c1 (include/cnhe.h, cnhe_vecs_encrypt_compact).  Needs the secret key; the matrix format travels out of band."""
+        return self.engine.encrypt_compact(np.ascontiguousarray(self._rows(m, fmt)), scale)
+
+    def LoadCompactMatrix(self, data, fmt):
+        """The matrix of a compact blob (GetEncryptedMatrixCompact), expanded on the GPU; `fmt` is the format it was made with."""
+        vecs = [B200BfvVector(self, v) for v in self.engine.import_compact(data)]
+        return B200BfvMatrix(self, vecs, fmt, CopyVectors=False)
+
     def GetMatrix(self, vectors, fmt, CopyVectors=True):
         return B200BfvMatrix(self, vectors, fmt, CopyVectors=CopyVectors)
 

@@ -153,6 +153,23 @@ int cnhe_vecs_export_raw(cnhe_ctx *, const cnhe_vec *const *vecs, int n, uint64_
  * (pinned host memory), without waiting for work queued afterwards.  Up to 8 tickets may be outstanding. */
 int cnhe_vecs_export_raw_async(cnhe_ctx *, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap_words, int *ticket);
 int cnhe_export_wait(cnhe_ctx *, int ticket);
+/* Compact upload (format version 1, this library's own; csrc/compact.cu has every field).  A secret-key encryption is
+ * (c0, c1) = (-(a s) + e + Delta m, a) with a uniform, so the data owner (who holds the secret key) sends c0 bit-packed at bitlen(q_l)
+ * bits per residue plus one 32-byte ChaCha20 key K_c per plaintext modulus from which the server regenerates a on the GPU: 2.6-2.9x
+ * fewer bytes than cnhe_vecs_import_raw's ciphertexts.  Blob: "CNHC" | u32 version = 1 | u32 N, k, P, n, B | u64 dim | f64 scale |
+ * k x u64 q_l | P x u64 t_c | P x 32-byte K_c | payload [P][n][B][k] packed c0 residues (N bitlen(q_l) / 64 words each); c1 of
+ * ciphertext j = i B + b, residue l, coefficient x is floor(q_l R / 2^128) with R = w[2x+1] 2^64 + w[2x], w[m] = 64-bit word m of the
+ * ChaCha20 keystream under K_c and stream id (11 << 48) | (j << 16) | l (block counter m >> 3, word m & 7).
+ * cnhe_vecs_encrypt_compact: seeded secret-key encryption of n dense vectors v[n][dim] (scale, CRT split and encoding as
+ * cnhe_vecs_encrypt) into one blob; dst == NULL queries the size in *needed.  Needs the secret key (CNHE_ERR_STATE otherwise).  A secure
+ * context draws a fresh K_c from the OS per call and channel; a context seeded by cnhe_keys_generate(seed) derives it from the seed.
+ * Counted as Encryption.
+ * cnhe_vecs_import_compact: the blob's vectors as ordinary encrypted dense vectors, asynchronous like cnhe_vecs_import_raw; out has room
+ * for cap vectors, *n receives the count.  Every header field is checked against the context (CNHE_ERR_INVALID, no vector created).
+ * Lifetime of src: pageable memory may be reused when the call returns; pinned memory (cudaHostAlloc / torch pin_memory) is read by an
+ * asynchronous copy and must stay unchanged until the imported vectors have been consumed (e.g. their outputs exported). */
+int cnhe_vecs_encrypt_compact(cnhe_ctx *, const double *v, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap, size_t *needed);
+int cnhe_vecs_import_compact(cnhe_ctx *, const uint8_t *src, size_t len, cnhe_vec **out, int cap, int *n);
 /* device pointer of a channel's ciphertext blocks (for NCCL gathers through torch; plumbing only) */
 int cnhe_vec_device_ptr(const cnhe_vec *, int channel, uint64_t *dptr, size_t *words);
 int cnhe_noise_budget(cnhe_ctx *, const cnhe_vec *, int channel, int block, int *bits); /* CryptoTracker.cs:41-52 */

@@ -66,6 +66,8 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_export_raw(IntPtr a0, IntPtr[] vecs, int n, IntPtr dst, UIntPtr cap_words);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_export_raw_async(IntPtr a0, IntPtr[] vecs, int n, IntPtr dst, UIntPtr cap_words, out int ticket);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_export_wait(IntPtr a0, int ticket);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_encrypt_compact(IntPtr a0, double[] v, int n, ulong dim, double scale, byte[] dst, UIntPtr cap, out UIntPtr needed);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_import_compact(IntPtr a0, byte[] src, UIntPtr len, IntPtr[] @out, int cap, out int n);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_device_ptr(IntPtr a0, int channel, out ulong dptr, out UIntPtr words);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_noise_budget(IntPtr a0, IntPtr a1, int channel, int block, out int bits);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_add(IntPtr a0, IntPtr a, IntPtr b, out IntPtr @out);
@@ -419,6 +421,25 @@ namespace HEWrapper
             var hs = new IntPtr[rows.Length];
             Cnhe.Check(Cnhe.cnhe_vecs_encrypt(Ctx, flat, rows.Length, dim, scale, hs));
             return new B200BfvMatrix(this, hs.Select(h => (IVector)new B200BfvVector(this, h)).ToArray(), format, false) { DataDisposedExternaly = false };
+        }
+        // the same encryption as one compact blob (bit-packed c0, per-channel ChaCha20 keys for c1; include/cnhe.h); needs the secret key
+        public byte[] GetEncryptedMatrixCompact(Matrix<double> m, EMatrixFormat format, double scale)
+        {
+            var rows = (format == EMatrixFormat.ColumnMajor ? m.EnumerateColumns() : m.EnumerateRows()).ToArray();
+            ulong dim = (ulong)rows[0].Count;
+            var flat = rows.SelectMany(r => r.ToArray()).ToArray();
+            Cnhe.Check(Cnhe.cnhe_vecs_encrypt_compact(Ctx, flat, rows.Length, dim, scale, null, UIntPtr.Zero, out UIntPtr needed));
+            var blob = new byte[(long)needed.ToUInt64()];
+            Cnhe.Check(Cnhe.cnhe_vecs_encrypt_compact(Ctx, flat, rows.Length, dim, scale, blob, needed, out needed));
+            return blob;
+        }
+        // the matrix of a compact blob, expanded on the GPU; the format travels out of band (as with raw import)
+        public IMatrix LoadCompactMatrix(byte[] data, EMatrixFormat format)
+        {
+            int cap = BitConverter.ToInt32(data, 20); // header field n
+            var hs = new IntPtr[Math.Max(cap, 1)];
+            Cnhe.Check(Cnhe.cnhe_vecs_import_compact(Ctx, data, (UIntPtr)(ulong)data.Length, hs, cap, out int n));
+            return new B200BfvMatrix(this, hs.Take(n).Select(h => (IVector)new B200BfvVector(this, h)).ToArray(), format, false) { DataDisposedExternaly = false };
         }
         public IMatrix GetMatrix(IVector[] vectors, EMatrixFormat format, bool CopyVectors = true) => new B200BfvMatrix(this, vectors, format, CopyVectors);
 
