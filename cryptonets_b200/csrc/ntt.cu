@@ -1034,14 +1034,43 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
 // The twiddle cache is filled once per CTA instead of once per transform, and the next digit's source words are in flight while the CTA
 // waits at the barrier that ends the current digit.  Same arithmetic as the MAC kernels (fmodmul + dadd, re-centred every 8 digits and
 // at the end), so the accumulator leaves with |x| <= 0.51 p in the layout launch_ntt_inverse_add consumes.
+// Keys: with PK the kernel reads the 48-bit packed copy of launch_pack_keys48 instead of the canonical u64 keys.  The key loads are the
+// kernel's costliest memory traffic (keys replaced by register values: -35 % kernel time at N = 8192, source words: -3.5 %, DESIGN
+// §4.4): a thread's 16 u64 words are 128 contiguous bytes, so each 16-byte load of a warp touches 32 cache lines and the lines are
+// fetched from L2 again before the thread's next load uses their second half.  The packed copy holds the same words in 6 bytes each,
+// laid out [D][2][k][half][6][TR] in 16-byte groups: group g of thread j is its bytes 16g..16g+15, so a warp's load is 512 contiguous
+// bytes and a thread reads 96 B instead of 128.
 template <int HLOGN>
 __host__ __device__ constexpr int ks_fused_threads() { return (1 << HLOGN) / 16; }
 template <int HLOGN>
 __host__ __device__ constexpr int ks_fused_smem() { return (1 << HLOGN) * 8 * 3 + TWC * 8; } // work buffer, two accumulators, twiddle cache
+// a word below 2^48 given as its low 32 bits and bits 32..47, as an exact double (u2d of the same word)
+__device__ __forceinline__ double u48d(unsigned lo, unsigned hi16) { return __dsub_rn(__hiloint2double((int)(hi16 | 0x43300000u), (int)lo), FP_TWO52); }
+// packed copy: the 16 key words of (polynomial b, half, thread j), 48 bits each, little-endian in 24 u32: word 2m in u32 3m and the low
+// half of 3m+1, word 2m+1 in the high half of 3m+1 and in 3m+2
 template <int HLOGN>
+__global__ void __launch_bounds__(256) k_pack_keys48(const u64 *__restrict__ key, uint4 *__restrict__ out, int n_polys) {
+    constexpr int H = 1 << HLOGN, TR = ks_fused_threads<HLOGN>();
+    const int gt = blockIdx.x * blockDim.x + threadIdx.x;
+    if (gt >= n_polys * 2 * TR) return;
+    const int j = gt % TR, bh = gt / TR; // bh = polynomial * 2 + half
+    const u64 *w = key + (size_t)bh * H + 16 * j;
+    unsigned u[24];
+#pragma unroll
+    for (int m = 0; m < 8; m++) {
+        const u64 a = w[2 * m], b = w[2 * m + 1];
+        u[3 * m] = (unsigned)a;
+        u[3 * m + 1] = (unsigned)(a >> 32 & 0xffff) | (unsigned)b << 16;
+        u[3 * m + 2] = (unsigned)(b >> 16);
+    }
+    uint4 *o = out + (size_t)bh * 6 * TR + j;
+#pragma unroll
+    for (int g = 0; g < 6; g++) o[g * TR] = make_uint4(u[4 * g], u[4 * g + 1], u[4 * g + 2], u[4 * g + 3]);
+}
+template <int HLOGN, bool PK>
 __global__ void __launch_bounds__(ks_fused_threads<HLOGN>(), HLOGN == 12 ? 2 : 4)
-k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *__restrict__ key, u64 *__restrict__ acc, const NttTab *__restrict__ tabs,
-                   int k, DigitMap dm) {
+k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *__restrict__ key, const uint4 *__restrict__ keyp, u64 *__restrict__ acc,
+                   const NttTab *__restrict__ tabs, int k, DigitMap dm) {
     constexpr int H = 1 << HLOGN, TR = ks_fused_threads<HLOGN>(), N = 2 * H;
     constexpr int R1 = HLOGN - 8, E1 = 1 << R1, LG1 = HLOGN - R1; // first pass: stage 0 on the loads, then R1 stages; then 4 + 4
     extern __shared__ __align__(16) u64 ks_raw[];
@@ -1142,13 +1171,34 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
         const bool rc = (d & 7) == 7 || d == dm.D - 1;
 #pragma unroll
         for (int kp = 0; kp < 2; kp++) {
-            const u64 *kw = key_l + (size_t)d * kstride + kp * kpoly;
+            double kd[16];
+            if constexpr (PK) {
+                const uint4 *kw = keyp + ((((size_t)d * 2 + kp) * k + l) * 2 + half) * 6 * TR + tid;
+                unsigned u[24];
+#pragma unroll
+                for (int g = 0; g < 6; g++) {
+                    const uint4 v = __ldg(kw + g * TR);
+                    u[4 * g] = v.x; u[4 * g + 1] = v.y; u[4 * g + 2] = v.z; u[4 * g + 3] = v.w;
+                }
+#pragma unroll
+                for (int m = 0; m < 8; m++) {
+                    kd[2 * m] = u48d(u[3 * m], u[3 * m + 1] & 0xffff);
+                    kd[2 * m + 1] = u48d(__funnelshift_r(u[3 * m + 1], u[3 * m + 2], 16), u[3 * m + 2] >> 16);
+                }
+            } else {
+                const u64 *kw = key_l + (size_t)d * kstride + kp * kpoly;
+#pragma unroll
+                for (int i = 0; i < 8; i++) {
+                    const ulonglong2 w = __ldg(reinterpret_cast<const ulonglong2 *>(kw) + i);
+                    kd[2 * i] = u2d(w.x);
+                    kd[2 * i + 1] = u2d(w.y);
+                }
+            }
 #pragma unroll
             for (int i = 0; i < 8; i++) {
-                const ulonglong2 w = __ldg(reinterpret_cast<const ulonglong2 *>(kw) + i);
                 double2 a = accv[(kp * 8 + i) * TR + tid];
-                a.x = __dadd_rn(a.x, fmodmul(x[2 * i], u2d(w.x), p, pinv));
-                a.y = __dadd_rn(a.y, fmodmul(x[2 * i + 1], u2d(w.y), p, pinv));
+                a.x = __dadd_rn(a.x, fmodmul(x[2 * i], kd[2 * i], p, pinv));
+                a.y = __dadd_rn(a.y, fmodmul(x[2 * i + 1], kd[2 * i + 1], p, pinv));
                 if (rc) { // sums of 8 fresh products stay below 4.1 p; re-centre before they could leave the exact range (and at the end)
                     a.x = frecenter(a.x, p, pinv);
                     a.y = frecenter(a.y, p, pinv);
@@ -1803,19 +1853,37 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
     });
     return cudaGetLastError();
 }
-template <int HL>
-static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, u64 *acc, int n_ct, int k, const DigitMap &dm, const NttTab *tabs,
-                                   cudaStream_t s) {
-    cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
+template <int HL, bool PK>
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, u64 *acc, int n_ct, int k, const DigitMap &dm,
+                                   const NttTab *tabs, cudaStream_t s) {
+    cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL, PK>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
     if (e != cudaSuccess) return e;
-    k_key_switch_fused<HL><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, key, acc, tabs, k, dm);
+    k_key_switch_fused<HL, PK><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, key, keyp, acc, tabs, k, dm);
     return cudaGetLastError();
 }
-cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, u64 *acc, int n_ct, int k, const DigitMap &dm, int logn,
-                                    const NttTab *tabs, cudaStream_t s) {
+template <int HL>
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, u64 *acc, int n_ct, int k, const DigitMap &dm,
+                                   const NttTab *tabs, cudaStream_t s) {
+    return keyp ? launch_ks_fused<HL, true>(target, ct_stride, key, keyp, acc, n_ct, k, dm, tabs, s)
+                : launch_ks_fused<HL, false>(target, ct_stride, key, keyp, acc, n_ct, k, dm, tabs, s);
+}
+cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, u64 *acc, int n_ct, int k,
+                                    const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s) {
     if (n_ct <= 0) return cudaSuccess;
-    if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, acc, n_ct, k, dm, tabs, s);
-    if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, acc, n_ct, k, dm, tabs, s);
+    if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, key_packed, acc, n_ct, k, dm, tabs, s);
+    if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, key_packed, acc, n_ct, k, dm, tabs, s);
+    return cudaErrorInvalidValue;
+}
+template <int HL>
+static cudaError_t launch_pk48(const u64 *key, uint4 *out, int n_polys, cudaStream_t s) {
+    const int threads = n_polys * 2 * ks_fused_threads<HL>();
+    k_pack_keys48<HL><<<(threads + 255) / 256, 256, 0, s>>>(key, out, n_polys);
+    return cudaGetLastError();
+}
+cudaError_t launch_pack_keys48(const u64 *key, uint4 *out, int n_polys, int logn, cudaStream_t s) {
+    if (n_polys <= 0) return cudaSuccess;
+    if (logn == 13) return launch_pk48<12>(key, out, n_polys, s);
+    if (logn == 12) return launch_pk48<11>(key, out, n_polys, s);
     return cudaErrorInvalidValue;
 }
 template <int L, bool IN_F, bool OUT_F>

@@ -763,15 +763,20 @@ void op_ntt(Context &c, const u64 *src, u64 *dst, int n_polys, int mod_base, int
 // Key switches of at least this many ciphertexts run fused (digit transforms and key product in one kernel, ntt.cu): the fused grid has
 // 2k CTAs per ciphertext, each walking all D digits, so small calls leave most of the GPU idle where the digit path spreads n*D*k
 // transforms over it.  tools/keyswitch_bench.py on one H100 SXM (700 W), N = 8192, k = 5, D = 25: fused / digit path 0.53 / 0.52 ms at
-// 32 ciphertexts, 0.87 / 0.99 ms at 64, 11.9 / 14.1 ms at 945
+// 32 ciphertexts, 0.87 / 0.99 ms at 64, 11.9 / 14.1 ms at 945.  With the packed relinearisation keys (H100 SXM at 400 W) relinearisation
+// crosses over lower, fused / digit path 0.41 / 0.52 ms at 32; Galois calls still read u64 keys and tie at 32, so the threshold stays
 constexpr int KS_FUSED_MIN = 64;
 // whether a key switch of n ciphertexts takes the fused path: N = 4096 / 8192 on the lazy FP64 path, n >= KS_FUSED_MIN.
 // CNHE_KS_FUSED=0 / =1 forces the digit path / the fused path wherever it is built (read per call: tests compare both in one process)
-static bool ks_fused(const Context &c, int n) {
+static bool ks_fused_built(const Context &c) {
     if (c.logN != 12 && c.logN != 13) return false;
     if (!(c.lazy && c.fp_elementwise && fp_range(c, 0, c.k))) return false;
     for (int i = 0; i < c.k; i++)
         if (!c.h_tabs[i].split_ok) return false;
+    return true;
+}
+static bool ks_fused(const Context &c, int n) {
+    if (!ks_fused_built(c)) return false;
     const char *v = getenv("CNHE_KS_FUSED");
     if (v) return atoi(v) != 0;
     return n >= KS_FUSED_MIN;
@@ -779,7 +784,7 @@ static bool ks_fused(const Context &c, int n) {
 // out[i] = (base_i + sum_d NTT^-1(NTT(digit_d(target_i)) * key_d)): ciphertext i's target polynomial (k residues) is at
 // target + i * target_stride, its base (2 polynomials) at base + i * base_stride; out is packed [n][2][k][N]
 void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, const u64 *key, const DigitMap &dm, const u64 *base,
-                   size_t base_stride, u64 *out) {
+                   size_t base_stride, u64 *out, const u64 *key_packed) {
     const int k = c.k;
     const size_t N = c.N;
     const int fpq = fp_range(c, 0, k);
@@ -792,8 +797,9 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
         u64 *acc = c.ws_alloc((size_t)m * 2 * k * N);
         if (fused) {
             // HBM: the target residues once (the pair and the other residues' CTAs share them through L2), the keys once, the accumulator
-            PROF(3, 8.0 * N * ((double)m * k + (double)dm.D * 2 * k + (double)m * 2 * k));
-            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, key, acc, m, k, dm, c.logN, c.d_tabs, c.stream),
+            PROF(3, 8.0 * N * ((double)m * k + (double)m * 2 * k) + (key_packed ? 6.0 : 8.0) * N * dm.D * 2 * k);
+            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, key, reinterpret_cast<const uint4 *>(key_packed), acc,
+                                            m, k, dm, c.logN, c.d_tabs, c.stream),
                     "key_switch_fused");
         } else {
             u64 *digits = c.ws_alloc((size_t)m * dm.D * k * N);
@@ -873,7 +879,8 @@ void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2) {
     const size_t N = c.N;
     // the size-3 layout [c0 c1 c2] is consumed in place: c2 is the key-switch target, (c0, c1) the base it is added to
     const size_t s3 = (size_t)3 * k * N;
-    op_key_switch(c, in3 + (size_t)2 * k * N, s3, n, c.ch[ch].rlk->p, c.dm_relin, in3, s3, out2);
+    const BufRef &pk = c.ch[ch].rlk_packed;
+    op_key_switch(c, in3 + (size_t)2 * k * N, s3, n, c.ch[ch].rlk->p, c.dm_relin, in3, s3, out2, pk ? pk->p : nullptr);
     c.note(Context::OP_RELINEARIZE, ch, n, out2);
 }
 void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2) {
@@ -887,7 +894,8 @@ void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, co
         u64 *ct3 = c.ws_alloc((size_t)m * 3 * k * N);
         multiply_chunk(c, ch, a, b, c0, m, ct3);
         const size_t s3 = (size_t)3 * k * N;
-        op_key_switch(c, ct3 + (size_t)2 * k * N, s3, m, c.ch[ch].rlk->p, c.dm_relin, ct3, s3, out2 + (size_t)c0 * 2 * k * N);
+        const BufRef &pk = c.ch[ch].rlk_packed;
+        op_key_switch(c, ct3 + (size_t)2 * k * N, s3, m, c.ch[ch].rlk->p, c.dm_relin, ct3, s3, out2 + (size_t)c0 * 2 * k * N, pk ? pk->p : nullptr);
     }
     c.op_count[Context::OP_MULTIPLY] += (uint64_t)n;
     c.note(Context::OP_RELINEARIZE, ch, n, out2, a[0], b[0]);
@@ -1291,6 +1299,19 @@ BufRef &key_slot(Context &c, int channel, int what, u64 arg, size_t &words, bool
     if (!*slot) throw Error(-3, "key is missing");
     return *slot;
 }
+void rlk_ready(Context &c, int channel) {
+    Channel &ch = c.ch[channel];
+    ch.have_rlk = true;
+    ch.rlk_packed.reset();
+    bool small = true;
+    for (u64 q : c.q) small = small && q < (1ULL << 48);
+    if (!ch.rlk || !small || !ks_fused_built(c)) return;
+    const size_t polys = (size_t)c.dm_relin.D * 2 * c.k;
+    ch.rlk_packed = c.alloc(polys * c.N * 6 / 8);
+    c.check(launch_pack_keys48(ch.rlk->p, reinterpret_cast<uint4 *>(ch.rlk_packed->p), (int)polys, c.logN, c.stream), "pack_keys48");
+    // the channel's key switches may run on another stream than this one: the copy is complete before any stream reads it
+    CNHE_CUDA(cudaStreamSynchronize(c.stream));
+}
 // key-switching keys for `target` (k*N, NTT form): key (i,j) = (-(a s + e) + [residue i] 2^{jw} target, a)
 static void make_kskeys(Context &c, Channel &ch, const u64 *target_ntt, const DigitMap &dm, int w, u64 purpose_a, u64 purpose_e, u64 key_tag, u64 *out) {
     const int k = c.k, D = dm.D;
@@ -1345,7 +1366,7 @@ static void keys_generate_impl(Context &c, bool secure, u64 seed) {
         u64 *s2 = c.ws_alloc(kN);
         c.check(launch_dyadic_bcast(sk->p, sk->p, s2, 1, 1, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic");
         make_kskeys(c, ch, s2, c.dm_relin, c.dbc_relin, 4, 5, 0, rlk->p);
-        ch.have_rlk = true;
+        rlk_ready(c, ci);
         // Galois keys: s(x^elt) in NTT form
         for (size_t gi = 0; gi < c.galois_elts.size(); gi++) {
             const u64 elt = c.galois_elts[gi], m2 = 2ULL * N;

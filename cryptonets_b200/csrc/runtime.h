@@ -43,6 +43,7 @@ struct Channel { // one plaintext modulus (one AtomicSealBfvEncryptedEnvironment
     int mod_id = 0; // NTT table id of t
     bool have_sk = false, have_pk = false, have_rlk = false;
     BufRef sk, pk, rlk;
+    BufRef rlk_packed; // rlk with 48-bit words for the fused key switch (set by rlk_ready when that kernel can run and every q_l < 2^48)
     std::map<u64, BufRef> glk;
     RngKey rng;    // secure (ChaCha20 keyed from the OS) unless a deterministic test seed was requested explicitly
     u64 nonce = 1; // running encryption counter (32 bits enter the stream id; a secure channel re-keys before it wraps)
@@ -186,6 +187,9 @@ void keys_generate_secure(Context &c);    // fresh OS entropy per channel
 void rng_from_os(RngKey &rk);
 const char *op_kind_name(int kind);
 BufRef &key_slot(Context &c, int channel, int what, u64 arg, size_t &words, bool create);
+// marks a channel's relinearisation keys present once they are written to its rlk slot (generated or loaded), and rebuilds the packed
+// copy the fused key switch reads; returns once that copy is complete
+void rlk_ready(Context &c, int channel);
 
 // ---- ciphertext-array operations (all asynchronous on c.stream; device pointers)
 // upload a host array of device pointers into workspace memory
@@ -197,8 +201,9 @@ void op_ntt(Context &c, const u64 *src, u64 *dst, int n_polys, int mod_base, int
 void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3);
 void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2);
 void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2);
+// key_packed: the channel's rlk_packed for relinearisation (nullptr: the fused kernel reads the u64 keys)
 void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, const u64 *key, const DigitMap &dm, const u64 *base,
-                   size_t base_stride, u64 *out);
+                   size_t base_stride, u64 *out, const u64 *key_packed = nullptr);
 void op_apply_galois(Context &c, int ch, const u64 *in, int n, u64 elt, u64 *out, bool add_back = false);
 bool op_rotate_add(Context &c, int ch, const u64 *in, int n, int steps, bool columns, u64 *out); // out = in + rotate(in) in one pass, if possible
 void op_rotate_rows(Context &c, int ch, const u64 *in, int n, int steps, u64 *out); // steps == 0 copies

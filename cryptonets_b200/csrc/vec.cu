@@ -190,7 +190,7 @@ extern "C" int cnhe_keys_import(cnhe_ctx *h, int channel, int what, uint64_t arg
     Channel &ch = c.ch[channel];
     if (what == 0) ch.have_sk = true;
     if (what == 1) ch.have_pk = true;
-    if (what == 2) ch.have_rlk = true;
+    if (what == 2) rlk_ready(c, channel);
     API_END
 }
 

@@ -472,7 +472,7 @@ extern "C" int cnhe_context_load(const uint8_t *archive, size_t len, int device,
                     }
                 };
                 read_kswitch(2, c.dm_relin.D, 1);
-                ch.have_rlk = true;
+                rlk_ready(c, ci);
                 read_kswitch(3, c.dm_galois.D, N);
                 ParmsId spid;
                 r.raw(spid, 32);

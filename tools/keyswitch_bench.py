@@ -5,7 +5,12 @@ stream), per-family device times and the HBM bytes the two key-switch forms need
 
 During a relinearise-only call family 0 (ntt_forward) is the digit transforms alone, family 3 (keyswitch_mac) the key product -- or,
 on the fused path, digit transforms and key product together -- and family 1 (ntt_inverse) the inverse transforms with the base
-addition.  `--path` sets CNHE_KS_FUSED for the run (auto: the library's own choice by n).  One JSON line per n."""
+addition.  `--path` sets CNHE_KS_FUSED for the run (auto: the library's own choice by n).  One JSON line per n.
+
+The fused kernel's operands come from L2: every (ciphertext, residue, half) CTA reads both halves of the source residue (8N bytes) and
+its half of the two key polynomials (8N bytes as u64 words, 6N in the 48-bit packed copy the library uses while every q_l < 2^48) per
+digit.  The line reports those bytes for both key forms and the achieved rate against --l2-tbs, the L2 read bandwidth tools/l2_bench
+measures (7.4 TB/s on one H100 80GB HBM3 at 700 W, 32 MiB buffer)."""
 import argparse, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -14,6 +19,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("n", type=int, nargs="*", default=[1, 8, 32, 64, 128, 945])
 ap.add_argument("--iters", type=int, default=5)
 ap.add_argument("--path", choices=["auto", "fused", "digits"], default="auto")
+ap.add_argument("--l2-tbs", type=float, default=7.4, help="L2 read bandwidth to compare the fused kernel's rate with (tools/l2_bench)")
 args = ap.parse_args()
 if args.path != "auto":
     os.environ["CNHE_KS_FUSED"] = "1" if args.path == "fused" else "0"
@@ -26,6 +32,7 @@ eng.set_option("multi_stream", 0)
 k, N = eng.k, 8192
 D = sum((int(q).bit_length() + 9) // 10 for q in eng.q)  # base-2^10 digits of every residue
 q = np.array(eng.q, dtype=np.uint64)
+packed = max(eng.q) < 1 << 48
 rng = np.random.default_rng(0)
 # FP64 warp instructions per (ciphertext, residue, half) and digit of the fused kernel at N = 8192 (4096-point halves, 256 threads, 16
 # coefficients each): stage 0 folded into the loads (16 modular products + 16 adds), 12 radix-2 stages of 8 butterflies (6 + 2), the key
@@ -51,14 +58,21 @@ for n in args.n:
     fused = prof["ntt_forward"]["launches"] == 0
     w = 8.0 * N
     bytes_digits = w * (n * k * D * 2 + n * k * D + D * 2 * k + n * 2 * k)  # digit source + digits written, digits + keys read, acc written
-    bytes_fused = w * (n * k + D * 2 * k + n * 2 * k)  # target residues, keys, acc
+    key_word = 6.0 if packed else 8.0  # bytes per key word the fused kernel reads (packed copy while every q_l < 2^48)
+    bytes_fused = w * (n * k + n * 2 * k) + key_word * N * D * 2 * k  # target residues, acc, keys
     bytes_inverse = w * (n * 2 * k * 3)  # acc read, base read, out written
+    cta_digits = n * 2 * k * D
+    l2_u64, l2_packed = cta_digits * (8.0 * N + 8.0 * N), cta_digits * (8.0 * N + 6.0 * N)  # source + keys, per key form
     rec = {"n": n, "path": "fused" if fused else "digits", "ms": round(ms, 3), "us_per_ct": round(ms * 1e3 / n, 2), "families_ms": fam,
            "hbm_bytes": {"digits_path": bytes_digits + bytes_inverse, "fused_path": bytes_fused + bytes_inverse}}
     if fused and fam.get("keyswitch_mac"):
         rate = DP_WARP_INSTR_PER_CT * n / (fam["keyswitch_mac"] * 1e-3)
         rec["fused_fp64_warp_instr_per_s"] = float("%.4g" % rate)
         rec["fused_fp64_issue_share"] = round(rate / 522.7e9, 3)  # 132 SMs x 2 FP64 warp instructions / clock x 1.98 GHz
+        l2 = l2_packed if packed else l2_u64
+        rec["fused_l2_bytes"] = {"u64_keys": l2_u64, "packed_keys": l2_packed}
+        rec["fused_l2_tb_s"] = round(l2 / (fam["keyswitch_mac"] * 1e-3) / 1e12, 2)
+        rec["fused_l2_share"] = round(rec["fused_l2_tb_s"] / args.l2_tbs, 3)
     print(json.dumps(rec), flush=True)
     eng.dev_free(a)
     eng.dev_free(out)
