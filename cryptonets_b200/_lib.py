@@ -30,6 +30,8 @@ _SIGS = {
     "cnhe_keys_generate": [C.c_void_p, u64],
     "cnhe_keys_save": [C.c_void_p, i32, C.c_void_p, sz, C.POINTER(sz)],
     "cnhe_context_load": [C.c_void_p, sz, i32, C.POINTER(C.c_void_p)],
+    "cnhe_keys_save_compact": [C.c_void_p, i32, U64P, i32, C.c_void_p, sz, C.POINTER(sz)],
+    "cnhe_context_load_compact": [C.c_void_p, sz, i32, C.POINTER(C.c_void_p)],
     "cnhe_vec_write": [C.c_void_p, VECP, C.c_void_p, sz, C.POINTER(sz)],
     "cnhe_vec_read": [C.c_void_p, C.c_char_p, sz, C.POINTER(VECP), C.POINTER(sz)],
     "cnhe_keys_generate_secure": [C.c_void_p],

@@ -13,6 +13,19 @@
 // A secret-key encryption is (c0, c1) = (-(a s) + e + Delta m, a) with a uniform: the client derives a from K_c and sends only c0 and K_c,
 // 2.6-2.9x fewer bytes than the ciphertexts.  The server regenerates a here (k_compact_expand); every later operation sees ordinary
 // ciphertexts in SEAL's layout [poly][residue][coeff].
+//
+// Compact evaluation keys, format version 1 (the same expansion; one blob per key set, made with cnhe_keys_save_compact):
+//   header   "CNHK" | u32 version = 1 | u32 N | u32 k | u32 P | u32 dbc_relin | u32 dbc_galois | u32 sets (bit 0 public key, bit 1
+//            relinearisation keys) | u32 G | k x u64 q_l | P x u64 t_c | G x u64 Galois elements (strictly increasing, each one of the
+//            context's standard elements) | P x 32-byte expansion keys K_c
+//   payload  for channel c, key pair kappa, residue l: the N words of part 0 (b) as the same bit stream as c0 above
+//   pairs    kappa in blob order: the public key (if present), the D_r relinearisation digits, then for each listed element the D_g digits
+//            of its Galois key (digit order of the decomposition map: residue-major, low bits first)
+//   part 1   (a) of pair kappa, residue l, word x: floor(q_l R / 2^128) as above under stream id stream_id(PURPOSE_KEYS_A, kappa, l); a is
+//            uniform in the NTT domain as well, so it is the key's NTT-form a directly
+// A key pair is (b, a) = (-(a s + e) + 2^{shift_d} [target]_{src_d}, a) in NTT form -- target s^2 for relinearisation, s(x^g) for Galois
+// element g, none for the public key -- with e the channel's noise sampler under stream_id(PURPOSE_KEYS_E, nonce0 + kappa, 0).  The
+// server writes (b, a) straight into its key slots with k_compact_expand.
 #include "kernels.h"
 
 namespace cnhe {
@@ -61,8 +74,8 @@ __device__ __forceinline__ u64 shape_off(const CompactShape &sh, int l) {
 
 // One thread per (ciphertext j, residue l, ChaCha20 block g): coefficients 4g..4g+3 of c1 from the block, and the same coefficients of c0
 // unpacked from the payload (packed == null: c0 is left alone -- the client's draw of a).  ct [n][2][k][N]; packed [n][sum_l N b_l / 64].
-__global__ void __launch_bounds__(256) k_compact_expand(u64 *__restrict__ ct, const u64 *__restrict__ packed, CompactKey key, u64 j0, int n,
-                                                       CompactShape sh, const BehzConst *__restrict__ bc) {
+__global__ void __launch_bounds__(256) k_compact_expand(u64 *__restrict__ ct, const u64 *__restrict__ packed, CompactKey key, u64 purpose, u64 j0,
+                                                       int n, CompactShape sh, const BehzConst *__restrict__ bc) {
     const int k = sh.k, logn = sh.logn;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= ((size_t)n * k) << (logn - 2)) return;
@@ -72,7 +85,7 @@ __global__ void __launch_bounds__(256) k_compact_expand(u64 *__restrict__ ct, co
     const size_t j = jl / k;
     const u64 q = bc->q[l].p;
     u32 x[16];
-    chacha20_block(key, g, stream_id(PURPOSE_COMPACT_A, j0 + j, (u64)l), x);
+    chacha20_block(key, g, stream_id(purpose, j0 + j, (u64)l), x);
     const size_t kN = (size_t)k << logn;
     u64 *c1 = ct + (2 * j + 1) * kN + ((size_t)l << logn) + 4 * (size_t)g;
     u64 v[4];
@@ -122,11 +135,11 @@ __global__ void __launch_bounds__(256) k_pack_residues(const u64 *__restrict__ c
     packed[i] = out;
 }
 
-cudaError_t launch_compact_expand(u64 *ct, const u64 *packed, const CompactKey &key, u64 j0, int n, const CompactShape &sh, const BehzConst *bc,
-                                  cudaStream_t s) {
+cudaError_t launch_compact_expand(u64 *ct, const u64 *packed, const CompactKey &key, u64 purpose, u64 j0, int n, const CompactShape &sh,
+                                  const BehzConst *bc, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     const size_t threads = ((size_t)n * sh.k) << (sh.logn - 2);
-    k_compact_expand<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(ct, packed, key, j0, n, sh, bc);
+    k_compact_expand<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(ct, packed, key, purpose, j0, n, sh, bc);
     return cudaGetLastError();
 }
 cudaError_t launch_pack_residues(const u64 *ct, u64 *packed, int n, const CompactShape &sh, cudaStream_t s) {

@@ -242,8 +242,9 @@ cudaError_t launch_encrypt_finish_sk(u64 *ct, const u64 *as, const u64 *plain, s
                                      int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
 
 // ---- compact ciphertext upload (compact.cu; format in its header comment)
-// stream-id purposes no other sampler call uses: the expanded c1, the noise e of a secret-key encryption, a test-seeded expansion key
-constexpr u64 PURPOSE_COMPACT_A = 11, PURPOSE_COMPACT_E = 12, PURPOSE_COMPACT_KEY = 13;
+// stream-id purposes no other sampler call uses: the expanded c1, the noise e of a secret-key encryption, a test-seeded expansion key;
+// the expanded a and the noise e of a compact key set's pairs
+constexpr u64 PURPOSE_COMPACT_A = 11, PURPOSE_COMPACT_E = 12, PURPOSE_COMPACT_KEY = 13, PURPOSE_KEYS_A = 14, PURPOSE_KEYS_E = 15;
 struct CompactKey {
     u32 w[8]; // ChaCha20 key K_c (the 32 header bytes as little-endian words)
 };
@@ -252,10 +253,10 @@ struct CompactShape {
     int bits[KMAX];      // b_l = bitlen(q_l)
     u64 off[KMAX + 1];   // word offset of residue l inside one packed ciphertext; off[k] = words per ciphertext
 };
-// ct[j] = (c0 unpacked from packed[j] and made canonical, c1 expanded from key under ciphertext index j0 + j), j < n; packed == null:
-// only c1 is written
-cudaError_t launch_compact_expand(u64 *ct, const u64 *packed, const CompactKey &key, u64 j0, int n, const CompactShape &sh, const BehzConst *bc,
-                                  cudaStream_t s);
+// ct[j] = (c0 unpacked from packed[j] and made canonical, c1 expanded from key under stream_id(purpose, j0 + j, l)), j < n; packed == null:
+// only c1 is written.  purpose: PURPOSE_COMPACT_A for ciphertexts, PURPOSE_KEYS_A for key pairs (ct is then [D][2][k][N] keys)
+cudaError_t launch_compact_expand(u64 *ct, const u64 *packed, const CompactKey &key, u64 purpose, u64 j0, int n, const CompactShape &sh,
+                                  const BehzConst *bc, cudaStream_t s);
 // packed[j] = bit-packed c0 of ct[j] (canonical residues), j < n
 cudaError_t launch_pack_residues(const u64 *ct, u64 *packed, int n, const CompactShape &sh, cudaStream_t s);
 // x[n][k][N] = c0 + c1*s (coefficient form) -> plain[n][N]

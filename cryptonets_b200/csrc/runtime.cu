@@ -392,6 +392,25 @@ static DigitMap make_digit_map(const std::vector<u64> &q, int w) {
     return dm;
 }
 
+// Galois elements of KeyGenerator::galois_keys(dbc): 2N-1, then 3^(2^i), 3^-(2^i) for i < logN-1
+std::vector<u64> standard_galois_elts(uint32_t N) {
+    std::vector<u64> out;
+    const u64 m2 = 2ULL * N;
+    int logN = 0;
+    while ((1u << logN) < N) logN++;
+    out.push_back(m2 - 1);
+    u64 p3 = 3, n3 = 0;
+    for (u64 x = 1; x < m2; x += 2)
+        if (((x * 3) & (m2 - 1)) == 1) { n3 = x; break; }
+    for (int i = 0; i < logN - 1; i++) {
+        out.push_back(p3);
+        p3 = (p3 * p3) & (m2 - 1);
+        out.push_back(n3);
+        n3 = (n3 * n3) & (m2 - 1);
+    }
+    return out;
+}
+
 Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *coeff, int k, int dbc_relin, int dbc_galois, int device) {
     if (P < 1 || P > 16) throw Error(-1, "need 1..16 plaintext primes");
     int logN = 0;
@@ -703,20 +722,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     }
     c.dm_relin = make_digit_map(c.q, dbc_relin);
     c.dm_galois = make_digit_map(c.q, dbc_galois);
-    // Galois elements of KeyGenerator::galois_keys(dbc): 2N-1, then 3^(2^i), 3^-(2^i) for i < logN-1
-    {
-        const u64 m2 = 2ULL * N;
-        c.galois_elts.push_back(m2 - 1);
-        u64 p3 = 3, n3 = 0;
-        for (u64 x = 1; x < m2; x += 2)
-            if (((x * 3) & (m2 - 1)) == 1) { n3 = x; break; }
-        for (int i = 0; i < logN - 1; i++) {
-            c.galois_elts.push_back(p3);
-            p3 = (p3 * p3) & (m2 - 1);
-            c.galois_elts.push_back(n3);
-            n3 = (n3 * n3) & (m2 - 1);
-        }
-    }
+    c.galois_elts = standard_galois_elts(N);
     // ---- wrapper CRT data (EncryptedSealBfvEnvironment.PreCompute, "EncryptedSealBfvVector.cs:79-90")
     {
         unsigned __int128 big = 1;
@@ -1151,7 +1157,7 @@ void op_encrypt_compact(Context &c, int chi, const u64 *plain, int n, u64 nonce0
         WsScope scope(c);
         const int m = std::min(4 * c.chunk, n - c0);
         u64 *ct = c.ws_alloc((size_t)m * 2 * kN), *as = c.ws_alloc((size_t)m * kN);
-        c.check(launch_compact_expand(ct, nullptr, key, (u64)c0, m, sh, c.d_bc, c.stream), "compact_expand(a)");
+        c.check(launch_compact_expand(ct, nullptr, key, PURPOSE_COMPACT_A, (u64)c0, m, sh, c.d_bc, c.stream), "compact_expand(a)");
         CNHE_CUDA(cudaMemcpy2DAsync(as, kN * 8, ct + kN, 2 * kN * 8, kN * 8, m, cudaMemcpyDeviceToDevice, c.stream));
         c.check(launch_ntt_forward(as, as, m * k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_forward");
         c.check(launch_dyadic_bcast(as, ch.sk->p, as, m, 1, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic");
@@ -1168,7 +1174,7 @@ void op_compact_expand(Context &c, const u64 *packed, const CompactKey &key, int
     c.stream = s; // the profiling events go on the stream the kernel runs on
     {
         ProfScope ps(c, 5, (double)n * (sh.off[c.k] + c.ct_words()) * 8);
-        c.check(launch_compact_expand(ct, packed, key, 0, n, sh, c.d_bc, s), "compact_expand");
+        c.check(launch_compact_expand(ct, packed, key, PURPOSE_COMPACT_A, 0, n, sh, c.d_bc, s), "compact_expand");
     }
     c.stream = keep;
 }
@@ -1312,14 +1318,26 @@ void rlk_ready(Context &c, int channel) {
     // the channel's key switches may run on another stream than this one: the copy is complete before any stream reads it
     CNHE_CUDA(cudaStreamSynchronize(c.stream));
 }
-// key-switching keys for `target` (k*N, NTT form): key (i,j) = (-(a s + e) + [residue i] 2^{jw} target, a)
-static void make_kskeys(Context &c, Channel &ch, const u64 *target_ntt, const DigitMap &dm, int w, u64 purpose_a, u64 purpose_e, u64 key_tag, u64 *out) {
-    const int k = c.k, D = dm.D;
+// Randomness of D consecutive key pairs: pair d draws a from the channel's uniform sampler under stream a_stream0 + (d << 16), or -- with
+// a_key set -- expands it from that key under stream_id(PURPOSE_KEYS_A, a_pair0 + d, l) (compact key sets); e under e_stream0 + (d << 16)
+struct KeyRandom {
+    const CompactKey *a_key = nullptr;
+    u64 a_stream0 = 0, a_pair0 = 0, e_stream0 = 0;
+};
+// key-switching keys for `target` (k*N, NTT form): key (i,j) = (-(a s + e) + [residue i] 2^{jw} target, a) -> out [D][2][k][N];
+// target == null: D = 1 and out = the public key (-(a s + e), a)
+static void make_kskeys(Context &c, Channel &ch, const u64 *target_ntt, const DigitMap *dm, const KeyRandom &r, u64 *out) {
+    const int k = c.k, D = target_ntt ? dm->D : 1;
     const size_t N = c.N, kN = (size_t)k * N;
     // c1 = a (uniform), written in place: key d part 1
     u64 *e = c.ws_alloc((size_t)D * kN), *as = c.ws_alloc((size_t)D * kN), *a = c.ws_alloc((size_t)D * kN);
-    c.check(launch_sample(a, D, SAMPLE_UNIFORM, ch.rng, stream_id(purpose_a, key_tag * 256, 0), 1ULL << 16, k, c.logN, c.d_bc, c.stream), "sample");
-    c.check(launch_sample(e, D, SAMPLE_NOISE, ch.rng, stream_id(purpose_e, key_tag * 256, 0), 1ULL << 16, k, c.logN, c.d_bc, c.stream), "sample");
+    if (r.a_key) {
+        c.check(launch_compact_expand(out, nullptr, *r.a_key, PURPOSE_KEYS_A, r.a_pair0, D, compact_shape(c), c.d_bc, c.stream), "compact_expand(a)");
+        CNHE_CUDA(cudaMemcpy2DAsync(a, kN * 8, out + kN, 2 * kN * 8, kN * 8, D, cudaMemcpyDeviceToDevice, c.stream));
+    } else {
+        c.check(launch_sample(a, D, SAMPLE_UNIFORM, ch.rng, r.a_stream0, 1ULL << 16, k, c.logN, c.d_bc, c.stream), "sample");
+    }
+    c.check(launch_sample(e, D, SAMPLE_NOISE, ch.rng, r.e_stream0, 1ULL << 16, k, c.logN, c.d_bc, c.stream), "sample");
     c.check(launch_ntt_forward(e, e, D * k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_forward");
     c.check(launch_dyadic_bcast(a, ch.sk->p, as, D, 1, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic");
     c.check(launch_ct_add(as, e, as, (size_t)D * kN, k, c.logN, c.d_bc, 0, c.stream), "ct_add");
@@ -1327,13 +1345,33 @@ static void make_kskeys(Context &c, Channel &ch, const u64 *target_ntt, const Di
     // interleave into [D][2][k][N]
     CNHE_CUDA(cudaMemcpy2DAsync(out, 2 * kN * 8, as, kN * 8, kN * 8, D, cudaMemcpyDeviceToDevice, c.stream));
     CNHE_CUDA(cudaMemcpy2DAsync(out + kN, 2 * kN * 8, a, kN * 8, kN * 8, D, cudaMemcpyDeviceToDevice, c.stream));
+    if (!target_ntt) return;
     // add 2^{jw} * target on residue src[d] of c0 of key d
     std::vector<u64> factors(D);
-    for (int d = 0; d < D; d++) factors[d] = hm::pw(2, (u64)dm.shift[d], c.q[dm.src[d]]);
-    (void)w;
+    for (int d = 0; d < D; d++) factors[d] = hm::pw(2, (u64)dm->shift[d], c.q[dm->src[d]]);
     u64 *dfac = c.ws_alloc(D);
     c.h2d(dfac, factors.data(), D * 8);
-    c.check(launch_key_add_scaled(out, target_ntt, dfac, dm, k, c.logN, c.d_bc, c.stream), "key_add_scaled");
+    c.check(launch_key_add_scaled(out, target_ntt, dfac, *dm, k, c.logN, c.d_bc, c.stream), "key_add_scaled");
+}
+static KeyRandom sampled(u64 purpose_a, u64 purpose_e, u64 key_tag) {
+    KeyRandom r;
+    r.a_stream0 = stream_id(purpose_a, key_tag * 256, 0);
+    r.e_stream0 = stream_id(purpose_e, key_tag * 256, 0);
+    return r;
+}
+// rs = NTT(s(x^elt)) from the coefficient-form secret key: the ciphertext Galois kernel on (sk_coeff, sk_coeff), whose perm_c1 output
+// receives the permuted second part
+static void galois_secret(Context &c, const u64 *sk_coeff, u64 elt, u64 *rs) {
+    const size_t kN = (size_t)c.k * c.N;
+    const u64 m2 = 2ULL * c.N;
+    u64 einv = 0;
+    for (u64 x = 1; x < m2; x += 2)
+        if (((x * elt) & (m2 - 1)) == 1) { einv = x; break; }
+    u64 *pair = c.ws_alloc(2 * kN), *base = c.ws_alloc(2 * kN);
+    CNHE_CUDA(cudaMemcpyAsync(pair, sk_coeff, kN * 8, cudaMemcpyDeviceToDevice, c.stream));
+    CNHE_CUDA(cudaMemcpyAsync(pair + kN, sk_coeff, kN * 8, cudaMemcpyDeviceToDevice, c.stream));
+    c.check(launch_galois(pair, base, rs, 1, einv, c.k, c.logN, c.d_bc, c.stream), "galois");
+    c.check(launch_ntt_forward(rs, rs, c.k, c.logN, c.d_tabs, 0, c.k, fp_range(c, 0, c.k), c.stream), "ntt_forward");
 }
 static void keys_generate_impl(Context &c, bool secure, u64 seed) {
     const int k = c.k;
@@ -1365,26 +1403,75 @@ static void keys_generate_impl(Context &c, bool secure, u64 seed) {
         BufRef &rlk = key_slot(c, ci, 2, 0, words, true);
         u64 *s2 = c.ws_alloc(kN);
         c.check(launch_dyadic_bcast(sk->p, sk->p, s2, 1, 1, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic");
-        make_kskeys(c, ch, s2, c.dm_relin, c.dbc_relin, 4, 5, 0, rlk->p);
+        make_kskeys(c, ch, s2, &c.dm_relin, sampled(4, 5, 0), rlk->p);
         rlk_ready(c, ci);
         // Galois keys: s(x^elt) in NTT form
         for (size_t gi = 0; gi < c.galois_elts.size(); gi++) {
-            const u64 elt = c.galois_elts[gi], m2 = 2ULL * N;
-            u64 einv = 0;
-            for (u64 x = 1; x < m2; x += 2)
-                if (((x * elt) & (m2 - 1)) == 1) { einv = x; break; }
-            // reuse the ciphertext Galois kernel on (sk_coeff, sk_coeff): perm_c1 receives the permuted second part
-            u64 *pair = c.ws_alloc(2 * kN), *base = c.ws_alloc(2 * kN), *rs = c.ws_alloc(kN);
-            CNHE_CUDA(cudaMemcpyAsync(pair, sk_coeff, kN * 8, cudaMemcpyDeviceToDevice, c.stream));
-            CNHE_CUDA(cudaMemcpyAsync(pair + kN, sk_coeff, kN * 8, cudaMemcpyDeviceToDevice, c.stream));
-            c.check(launch_galois(pair, base, rs, 1, einv, k, c.logN, c.d_bc, c.stream), "galois");
-            c.check(launch_ntt_forward(rs, rs, k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_forward");
+            const u64 elt = c.galois_elts[gi];
+            u64 *rs = c.ws_alloc(kN);
+            galois_secret(c, sk_coeff, elt, rs);
             BufRef &gk = key_slot(c, ci, 3, elt, words, true);
-            make_kskeys(c, ch, rs, c.dm_galois, c.dbc_galois, 6, 7, gi + 1, gk->p);
+            make_kskeys(c, ch, rs, &c.dm_galois, sampled(6, 7, gi + 1), gk->p);
         }
         c.sync();
         ws_release_all(c);
     }
+}
+
+// ---------------------------------------------------------------- compact key sets (format: compact.cu)
+size_t compact_key_pairs(const Context &c, int sets, size_t n_galois) {
+    return ((sets & 1) ? 1 : 0) + ((sets & 2) ? (size_t)c.dm_relin.D : 0) + n_galois * c.dm_galois.D;
+}
+void op_keys_save_compact(Context &c, int chi, int sets, const std::vector<u64> &elts, u64 nonce0, const CompactKey &key, u64 *packed) {
+    Channel &ch = c.ch[chi];
+    if (!ch.have_sk) throw Error(-3, "secret key is missing");
+    const int k = c.k;
+    const size_t kN = (size_t)k * c.N;
+    const CompactShape sh = compact_shape(c);
+    u64 *sk_coeff = c.ws_alloc(kN);
+    c.check(launch_ntt_inverse(ch.sk->p, sk_coeff, k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_inverse");
+    u64 kappa = 0;
+    // one key set: D pairs from kappa on, generated into scratch and packed into their place in the channel's payload
+    auto emit = [&](const u64 *target, const DigitMap *dm) {
+        WsScope scope(c);
+        const int D = target ? dm->D : 1;
+        KeyRandom r;
+        r.a_key = &key;
+        r.a_pair0 = kappa;
+        r.e_stream0 = stream_id(PURPOSE_KEYS_E, nonce0 + kappa, 0);
+        u64 *keys = c.ws_alloc((size_t)D * 2 * kN);
+        make_kskeys(c, ch, target, dm, r, keys);
+        c.check(launch_pack_residues(keys, packed + kappa * sh.off[k], D, sh, c.stream), "pack_residues");
+        kappa += D;
+    };
+    if (sets & 1) emit(nullptr, nullptr);
+    if (sets & 2) {
+        WsScope scope(c);
+        u64 *s2 = c.ws_alloc(kN);
+        c.check(launch_dyadic_bcast(ch.sk->p, ch.sk->p, s2, 1, 1, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic");
+        emit(s2, &c.dm_relin);
+    }
+    for (u64 elt : elts) {
+        WsScope scope(c);
+        u64 *rs = c.ws_alloc(kN);
+        galois_secret(c, sk_coeff, elt, rs);
+        emit(rs, &c.dm_galois);
+    }
+}
+void op_keys_load_compact(Context &c, int chi, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key) {
+    const CompactShape sh = compact_shape(c);
+    u64 kappa = 0;
+    auto expand = [&](int what, u64 arg) {
+        size_t words;
+        BufRef &slot = key_slot(c, chi, what, arg, words, true);
+        const int D = (int)(words / c.ct_words());
+        c.check(launch_compact_expand(slot->p, packed + kappa * sh.off[c.k], key, PURPOSE_KEYS_A, kappa, D, sh, c.d_bc, c.stream), "compact_expand");
+        kappa += D;
+    };
+    if (sets & 1) { expand(1, 0); c.ch[chi].have_pk = true; }
+    if (sets & 2) expand(2, 0);
+    for (u64 elt : elts) expand(3, elt);
+    if (sets & 2) rlk_ready(c, chi); // synchronises the channel's stream
 }
 
 void keys_generate(Context &c, u64 seed) { keys_generate_impl(c, false, seed); }

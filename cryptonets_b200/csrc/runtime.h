@@ -236,6 +236,14 @@ CompactKey compact_key(Context &c, int ch, u64 nonce0);
 void op_encrypt_compact(Context &c, int ch, const u64 *plain, int n, u64 nonce0, const CompactKey &key, u64 *packed);
 // packed [n][off[k]] + K_c -> ct [n][2kN] on stream s (timed as family 5 when profiling)
 void op_compact_expand(Context &c, const u64 *packed, const CompactKey &key, int n, u64 *ct, cudaStream_t s);
+// ---- compact key sets (format: compact.cu).  sets: bit 0 public key, bit 1 relinearisation keys; elts: Galois elements in blob order
+std::vector<u64> standard_galois_elts(uint32_t N); // KeyGenerator::galois_keys(dbc)'s elements, in the context's order
+size_t compact_key_pairs(const Context &c, int sets, size_t n_galois);
+// a fresh key set under the channel's secret key (its own keys are untouched): pair kappa's a expanded from K_c, e under nonce0 + kappa
+// -> packed b [pairs][off[k]] (device)
+void op_keys_save_compact(Context &c, int ch, int sets, const std::vector<u64> &elts, u64 nonce0, const CompactKey &key, u64 *packed);
+// packed b [pairs][off[k]] (device) + K_c -> the channel's key slots; returns once the keys are complete
+void op_keys_load_compact(Context &c, int ch, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key);
 int op_noise_budget(Context &c, int ch, const u64 *ct);
 
 } // namespace cnhe

@@ -795,6 +795,148 @@ extern "C" int cnhe_vecs_import_compact(cnhe_ctx *h, const uint8_t *src, size_t 
     }
     API_END
 }
+// ---------------------------------------------------------------------------------------- compact key sets (format: csrc/compact.cu)
+static size_t key_header_bytes(int k, int P, size_t G) { return 36 + 8 * (size_t)k + 40 * (size_t)P + 8 * G; }
+// the caller's element selection in blob order (increasing); -1: every standard element.  The standard list names 3^(N/4) twice (it is
+// its own inverse), so "every element" is the distinct ones.
+static std::vector<u64> select_galois(const Context &c, const uint64_t *elts, int n) {
+    std::vector<u64> std_elts = c.galois_elts;
+    std::sort(std_elts.begin(), std_elts.end());
+    std_elts.erase(std::unique(std_elts.begin(), std_elts.end()), std_elts.end());
+    if (n == -1) return std_elts;
+    if (n < 0 || (n > 0 && !elts)) fail("bad Galois element list");
+    std::vector<u64> out(elts, elts + n);
+    std::sort(out.begin(), out.end());
+    for (size_t i = 0; i < out.size(); i++) {
+        if (i && out[i] == out[i - 1]) fail("duplicate Galois element");
+        if (!std::binary_search(std_elts.begin(), std_elts.end(), out[i])) fail("not one of the context's Galois elements");
+    }
+    return out;
+}
+extern "C" int cnhe_keys_save_compact(cnhe_ctx *h, int sets, const uint64_t *galois_elts, int n_galois, uint8_t *dst, size_t cap, size_t *needed) {
+    API_BEGIN(h)
+    if (!dst && !needed) fail("bad arguments");
+    if (sets & ~3) fail("unknown key sets (bit 0 public key, bit 1 relinearization keys)");
+    const std::vector<u64> elts = select_galois(c, galois_elts, n_galois);
+    const CompactShape sh = compact_shape(c);
+    const size_t pairs = compact_key_pairs(c, sets, elts.size()), hdr = key_header_bytes(c.k, c.P, elts.size());
+    const size_t per_ch = pairs * sh.off[c.k] * 8, total = hdr + (size_t)c.P * per_ch;
+    if (needed) *needed = total;
+    if (!dst) return CNHE_OK;
+    if (cap < total) fail("destination too small");
+    for (int ch = 0; ch < c.P; ch++)
+        if (!c.ch[ch].have_sk) throw Error(CNHE_ERR_STATE, "secret key is missing");
+    std::vector<CompactKey> keys(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        const u64 nonce0 = take_nonces(c, ch, std::max<size_t>(pairs, 1)); // one noise nonce per pair; K_c stays unique even for no pairs
+        keys[ch] = compact_key(c, ch, nonce0);
+        if (pairs) {
+            u64 *packed = c.ws_alloc(pairs * sh.off[c.k]);
+            op_keys_save_compact(c, ch, sets, elts, nonce0, keys[ch], packed);
+            CNHE_CUDA(cudaMemcpyAsync(dst + hdr + ch * per_ch, packed, per_ch, cudaMemcpyDeviceToHost, c.stream));
+        }
+        c.sync();
+        ws_release_all(c);
+    }
+    auto wr32 = [&](size_t off, uint32_t x) { memcpy(dst + off, &x, 4); };
+    auto wr64 = [&](size_t off, uint64_t x) { memcpy(dst + off, &x, 8); };
+    memcpy(dst, "CNHK", 4);
+    wr32(4, 1);
+    wr32(8, c.N);
+    wr32(12, (uint32_t)c.k);
+    wr32(16, (uint32_t)c.P);
+    wr32(20, (uint32_t)c.dbc_relin);
+    wr32(24, (uint32_t)c.dbc_galois);
+    wr32(28, (uint32_t)sets);
+    wr32(32, (uint32_t)elts.size());
+    size_t o = 36;
+    for (int l = 0; l < c.k; l++, o += 8) wr64(o, c.q[l]);
+    for (int ch = 0; ch < c.P; ch++, o += 8) wr64(o, c.t[ch]);
+    for (u64 e : elts) { wr64(o, e); o += 8; }
+    for (int ch = 0; ch < c.P; ch++, o += 32) memcpy(dst + o, keys[ch].w, 32);
+    API_END
+}
+struct KeyBlob {
+    uint32_t N = 0, k = 0, P = 0, dbc_relin = 0, dbc_galois = 0, sets = 0;
+    std::vector<u64> q, t, elts;
+    std::vector<CompactKey> keys;
+    size_t header_bytes = 0, channel_words = 0; // packed words per channel
+};
+// every header field and the exact length, on the host; any defect is CNHE_ERR_INVALID
+static KeyBlob parse_compact_keys(const uint8_t *src, size_t len) {
+    auto rd32 = [&](size_t off) { uint32_t v; memcpy(&v, src + off, 4); return v; };
+    auto rd64 = [&](size_t off) { uint64_t v; memcpy(&v, src + off, 8); return v; };
+    if (len < 36) fail("compact key blob: truncated header");
+    if (memcmp(src, "CNHK", 4) != 0) fail("compact key blob: bad magic");
+    if (rd32(4) != 1) fail("compact key blob: unsupported version");
+    KeyBlob kb;
+    kb.N = rd32(8);
+    kb.k = rd32(12);
+    kb.P = rd32(16);
+    kb.dbc_relin = rd32(20);
+    kb.dbc_galois = rd32(24);
+    kb.sets = rd32(28);
+    const uint32_t G = rd32(32);
+    if (kb.sets & ~3u) fail("compact key blob: unknown key sets");
+    if (kb.N < 1024 || kb.N > 16384 || (kb.N & (kb.N - 1))) fail("compact key blob: PolyModulusDegree must be a power of two in [1024, 16384]");
+    if (kb.k < 1 || kb.k > (uint32_t)KMAX) fail("compact key blob: need 1..9 coefficient primes");
+    if (kb.P < 1 || kb.P > 16) fail("compact key blob: need 1..16 plaintext primes");
+    if (kb.dbc_relin < 1 || kb.dbc_relin > 60 || kb.dbc_galois < 1 || kb.dbc_galois > 60) fail("compact key blob: bad decomposition bit count");
+    const std::vector<u64> std_elts = standard_galois_elts(kb.N);
+    if (G >= std_elts.size()) fail("compact key blob: more Galois elements than the context has"); // one standard element is listed twice
+    kb.header_bytes = key_header_bytes((int)kb.k, (int)kb.P, G);
+    if (len < kb.header_bytes) fail("compact key blob: truncated header");
+    size_t o = 36;
+    for (uint32_t l = 0; l < kb.k; l++, o += 8) kb.q.push_back(rd64(o));
+    for (uint32_t ch = 0; ch < kb.P; ch++, o += 8) kb.t.push_back(rd64(o));
+    for (uint32_t g = 0; g < G; g++, o += 8) kb.elts.push_back(rd64(o));
+    kb.keys.resize(kb.P);
+    for (uint32_t ch = 0; ch < kb.P; ch++, o += 32) memcpy(kb.keys[ch].w, src + o, 32);
+    for (uint32_t g = 0; g < G; g++) {
+        if (g && kb.elts[g] <= kb.elts[g - 1]) fail("compact key blob: Galois elements must be strictly increasing");
+        if (std::find(std_elts.begin(), std_elts.end(), kb.elts[g]) == std_elts.end()) fail("compact key blob: not a standard Galois element");
+    }
+    size_t words = 0, d_relin = 0, d_galois = 0; // packed words per pair; digits per key (make_digit_map: ceil(bitlen(q_l) / w) each)
+    for (u64 q : kb.q) {
+        if (q < 2) fail("compact key blob: bad coefficient modulus");
+        const size_t b = 64 - __builtin_clzll(q);
+        words += kb.N * b / 64;
+        d_relin += (b + kb.dbc_relin - 1) / kb.dbc_relin;
+        d_galois += (b + kb.dbc_galois - 1) / kb.dbc_galois;
+    }
+    const size_t pairs = ((kb.sets & 1) ? 1 : 0) + ((kb.sets & 2) ? d_relin : 0) + (size_t)G * d_galois;
+    kb.channel_words = pairs * words;
+    if (len != kb.header_bytes + (size_t)kb.P * kb.channel_words * 8) fail("compact key blob: length does not match the header");
+    return kb;
+}
+extern "C" int cnhe_context_load_compact(const uint8_t *blob, size_t len, int device, cnhe_ctx **out) {
+    try {
+        if (!blob || !out) fail("null argument");
+        const KeyBlob kb = parse_compact_keys(blob, len);
+        std::unique_ptr<cnhe_ctx> ctx(new cnhe_ctx{nullptr});
+        ctx->c = context_create(kb.t.data(), (int)kb.P, kb.N, kb.q.data(), (int)kb.k, (int)kb.dbc_relin, (int)kb.dbc_galois, device);
+        Context &c = *ctx->c;
+        std::unique_ptr<Context> guard(ctx->c);
+        {
+            std::lock_guard<std::recursive_mutex> lock(c.mu);
+            if (compact_key_pairs(c, (int)kb.sets, kb.elts.size()) * compact_shape(c).off[c.k] != kb.channel_words)
+                fail("compact key blob: key sizes do not match the context");
+            for (int ci = 0; ci < c.P && kb.channel_words; ci++) {
+                c.set_channel(ci);
+                u64 *stage = c.ws_alloc(kb.channel_words); // the channel's packed payload in one copy
+                CNHE_CUDA(cudaMemcpyAsync(stage, blob + kb.header_bytes + (size_t)ci * kb.channel_words * 8, kb.channel_words * 8,
+                                          cudaMemcpyHostToDevice, c.stream));
+                op_keys_load_compact(c, ci, (int)kb.sets, kb.elts, stage, kb.keys[ci]);
+                c.sync();
+                ws_release_all(c);
+            }
+        }
+        guard.release();
+        *out = ctx.release();
+    } catch (const Error &e) { return set_err(e.code, e.what()); } catch (const std::exception &e) { return set_err(CNHE_ERR_INVALID, e.what()); }
+    return CNHE_OK;
+}
 extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap) {
     API_BEGIN(h)
     if (n < 1 || !dst) fail("bad arguments");

@@ -90,14 +90,21 @@ class Vec:
 class Engine:
     """One cnhe_ctx: parameters, device tables and keys for P plaintext moduli (== EncryptedSealBfvFactory)."""
 
-    def __init__(self, plain_primes, N=0, dbc_relin=10, dbc_galois=20, small_modulus_count=-1, device=0, coeff_moduli=None, archive=None):
-        """archive: bytes of a key archive (cnhe_keys_save / EncryptedSealBfvEnvironment.Save): parameters and keys come from it."""
+    def __init__(self, plain_primes, N=0, dbc_relin=10, dbc_galois=20, small_modulus_count=-1, device=0, coeff_moduli=None, archive=None,
+                 compact_keys=None):
+        """archive: bytes of a key archive (cnhe_keys_save / EncryptedSealBfvEnvironment.Save): parameters and keys come from it.
+        compact_keys: bytes of a compact key blob (save_compact_keys): parameters from its header, keys expanded on the GPU."""
         self.L = _lib.lib()
         self._live = weakref.WeakSet()
         h = C.c_void_p()
-        if archive is not None:
-            buf = (C.c_ubyte * len(archive)).from_buffer_copy(archive)
-            check(self.L.cnhe_context_load(buf, len(archive), device, C.byref(h)))
+        if archive is not None and compact_keys is not None:
+            raise ValueError("give either archive or compact_keys")
+        loaded = archive is not None or compact_keys is not None
+        if loaded:
+            blob = archive if archive is not None else compact_keys
+            load = self.L.cnhe_context_load if archive is not None else self.L.cnhe_context_load_compact
+            buf = (C.c_ubyte * len(blob)).from_buffer_copy(blob)
+            check(load(buf, len(blob), device, C.byref(h)))
             self.h = h
             P = C.c_int()
             check(self.L.cnhe_context_info(self.h, None, None, C.byref(P), None, None, None))
@@ -105,7 +112,7 @@ class Engine:
             check(self.L.cnhe_context_plain_moduli(self.h, _p(pp)))
         else:
             pp = _u64(plain_primes)
-        if archive is not None:
+        if loaded:
             pass
         elif coeff_moduli is None:
             check(self.L.cnhe_context_create(_p(pp), len(pp), N, dbc_relin, dbc_galois, small_modulus_count, device, C.byref(h)))
@@ -200,6 +207,22 @@ class Engine:
         check(self.L.cnhe_keys_save(self.h, int(with_private_keys), None, 0, C.byref(n)))
         buf = (C.c_ubyte * n.value)()
         check(self.L.cnhe_keys_save(self.h, int(with_private_keys), buf, n.value, C.byref(n)))
+        return bytes(buf)
+
+    def save_compact_keys(self, public=True, relin=True, galois=None):
+        """A freshly generated evaluation-key set as one compact blob (bytes) for a server (cnhe_keys_save_compact): a per-channel ChaCha20
+        key for every a and bit-packed b.  galois: None = every standard element, [] = none, else a list of elements.  Needs the secret key;
+        this engine's own keys are unchanged."""
+        sets = (1 if public else 0) | (2 if relin else 0)
+        if galois is None:
+            elts, n = None, -1
+        else:
+            arr = _u64(list(galois))
+            elts, n = (_p(arr) if arr.size else None), int(arr.size)
+        need = C.c_size_t()
+        check(self.L.cnhe_keys_save_compact(self.h, sets, elts, n, None, 0, C.byref(need)))
+        buf = (C.c_ubyte * need.value)()
+        check(self.L.cnhe_keys_save_compact(self.h, sets, elts, n, buf, need.value, C.byref(need)))
         return bytes(buf)
 
     def write_vector(self, vec):

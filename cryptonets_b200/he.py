@@ -260,7 +260,10 @@ class B200BfvFactory:
         An integer seed selects the deterministic sampler shared with the CPU oracle: parity tests only."""
         if isinstance(primes, (str, bytes, bytearray)):  # EncryptedSealBfvFactory(fileName) (IFactory.cs:262-265): parameters and keys from a key archive
             data = open(primes, "rb").read() if isinstance(primes, str) else bytes(primes)
-            self.engine = Engine(None, archive=data, device=device)
+            if data[:4] == b"CNHK":  # a compact key blob (SaveCompactKeys): keys expanded on the GPU, no secret key
+                self.engine = Engine(None, compact_keys=data, device=device)
+            else:
+                self.engine = Engine(None, archive=data, device=device)
             primes = self.engine.primes
         else:
             if primes is None:
@@ -331,6 +334,21 @@ class B200BfvFactory:
     def Save(self, target, withPrivateKeys=False):
         """IFactory.Save(stream | fileName, withPrivateKeys): the ZIP key archive."""
         data = self.engine.save_keys(withPrivateKeys)
+        if isinstance(target, str):
+            with open(target, "wb") as f:
+                f.write(data)
+        else:
+            target.write(data)
+        return target
+
+    def SaveCompactKeys(self, target=None, public=True, relin=True, galois=None):
+        """The evaluation keys a server needs as one compact blob (include/cnhe.h, cnhe_keys_save_compact): a freshly generated key set under
+        this factory's secret key, `a` of every key regenerated on the server's GPU from a per-channel ChaCha20 key, `b` bit-packed.
+        galois: None = every standard element, [] = none (CryptoNets never rotates), else the elements the network rotates by.  Returns the
+        bytes, or writes them to `target` (file name or binary stream); B200BfvFactory(blob or file name) is the server side."""
+        data = self.engine.save_compact_keys(public, relin, galois)
+        if target is None:
+            return data
         if isinstance(target, str):
             with open(target, "wb") as f:
                 f.write(data)

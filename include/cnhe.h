@@ -113,6 +113,26 @@ int cnhe_trace_read(cnhe_ctx *, int32_t *out, size_t cap_records, size_t *n_reco
  *   IFactory.LoadVector / LoadMatrix parse ("IFactory.cs:474-483"; a matrix is the reference's three header lines around its vectors). */
 int cnhe_keys_save(cnhe_ctx *, int with_private_keys, uint8_t *dst, size_t cap, size_t *needed);
 int cnhe_context_load(const uint8_t *archive, size_t len, int device, cnhe_ctx **out);
+/* Compact evaluation keys (format version 1, this library's own; csrc/compact.cu has every field).  Half of every key pair is the uniform
+ * polynomial a, which the server regenerates on the GPU from one 32-byte ChaCha20 key K_c per plaintext modulus (the ciphertext blob's
+ * expansion); the other half, b, travels bit-packed at bitlen(q_l) bits per word: 2.6-2.9x smaller than the archive's key words, and
+ * Galois elements the network never rotates by can be left out.  Blob: "CNHK" | u32 version = 1 | u32 N, k, P, dbc_relin, dbc_galois |
+ * u32 sets (bit 0 public key, bit 1 relinearisation keys) | u32 G | k x u64 q_l | P x u64 t_c | G x u64 Galois elements (strictly
+ * increasing) | P x 32-byte K_c | payload [P][pairs][k] packed b residues.  Pairs: public key, the relinearisation digits, then the Galois
+ * digits of each listed element; a of pair kappa, residue l, word x is floor(q_l R / 2^128) with R = w[2x+1] 2^64 + w[2x], w the ChaCha20
+ * keystream under K_c and stream id (14 << 48) | (kappa << 16) | l.
+ * cnhe_keys_save_compact: the client side; needs the secret key (CNHE_ERR_STATE otherwise).  sets as above (other bits: CNHE_ERR_INVALID);
+ * n_galois = -1 selects every element of cnhe_context_galois_elts, 0 none, otherwise galois_elts lists n_galois of them (any order;
+ * duplicates and other elements: CNHE_ERR_INVALID).  The blob carries a FRESHLY generated key set under the context's secret key -- the
+ * context's own keys are left untouched -- with one encryption nonce per pair for its noise.  K_c is a fresh OS draw per call and channel,
+ * or seed-derived on a context seeded by cnhe_keys_generate(seed) (tests only).  dst == NULL queries the size in *needed, which depends on
+ * the parameters and the selection only.  Counts no evaluator operation.
+ * cnhe_context_load_compact: the server side, like cnhe_context_load: parameters come from the header, the keys are expanded on the GPU
+ * straight into the key slots.  The context has no secret key and exactly the key sets the blob lists (missing ones refuse with
+ * CNHE_ERR_STATE as usual).  Every header field, the element list and the exact length are checked on the host before anything is
+ * allocated (CNHE_ERR_INVALID, no context).  Returns once the keys are complete. */
+int cnhe_keys_save_compact(cnhe_ctx *, int sets, const uint64_t *galois_elts, int n_galois, uint8_t *dst, size_t cap, size_t *needed);
+int cnhe_context_load_compact(const uint8_t *blob, size_t len, int device, cnhe_ctx **out);
 int cnhe_vec_write(cnhe_ctx *, const cnhe_vec *, char *dst, size_t cap, size_t *needed);
 int cnhe_vec_read(cnhe_ctx *, const char *text, size_t len, cnhe_vec **out, size_t *consumed);
 

@@ -47,6 +47,8 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_trace_read(IntPtr a0, int[] @out, UIntPtr cap_records, out UIntPtr n_records, int clear);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_keys_save(IntPtr a0, int with_private_keys, byte[] dst, UIntPtr cap, out UIntPtr needed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_load(byte[] archive, UIntPtr len, int device, out IntPtr @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_keys_save_compact(IntPtr a0, int sets, ulong[] galois_elts, int n_galois, byte[] dst, UIntPtr cap, out UIntPtr needed);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_load_compact(byte[] blob, UIntPtr len, int device, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_write(IntPtr a0, IntPtr a1, byte[] dst, UIntPtr cap, out UIntPtr needed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_read(IntPtr a0, byte[] text, UIntPtr len, out IntPtr @out, out UIntPtr consumed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_encrypt(IntPtr a0, double[] v, ulong dim, double scale, int format, out IntPtr @out);
@@ -349,9 +351,12 @@ namespace HEWrapper
         }
         /// EncryptedSealBfvFactory(string fileName) (IFactory.cs:262-271): parameters and keys from a key archive written by Save
         public B200BfvFactory(string fileName, int device = 0) : this(File.ReadAllBytes(fileName), device) { }
+        /// a compact key blob (SaveCompactKeys, magic "CNHK") is recognised too: its keys are expanded on the GPU, there is no secret key
         public B200BfvFactory(byte[] archive, int device = 0)
         {
-            Cnhe.Check(Cnhe.cnhe_context_load(archive, (UIntPtr)archive.Length, device, out Ctx));
+            bool compact = archive.Length >= 4 && archive[0] == (byte)'C' && archive[1] == (byte)'N' && archive[2] == (byte)'H' && archive[3] == (byte)'K';
+            if (compact) Cnhe.Check(Cnhe.cnhe_context_load_compact(archive, (UIntPtr)archive.Length, device, out Ctx));
+            else Cnhe.Check(Cnhe.cnhe_context_load(archive, (UIntPtr)archive.Length, device, out Ctx));
             Cnhe.Check(Cnhe.cnhe_context_info(Ctx, out _, out _, out int P, out _, out _, out _));
             var primes = new ulong[P];
             Cnhe.Check(Cnhe.cnhe_context_plain_moduli(Ctx, primes));
@@ -480,6 +485,16 @@ namespace HEWrapper
         public void Save(string FileName, bool withPrivateKeys = false)
         {
             using (var f = new FileStream(FileName, FileMode.Create)) { Save(f, withPrivateKeys); f.Flush(); }
+        }
+        /// the evaluation keys a server needs as one compact blob (include/cnhe.h, cnhe_keys_save_compact): a fresh key set under this
+        /// factory's secret key; galois null = every standard element, empty = none, else the elements the network rotates by
+        public byte[] SaveCompactKeys(bool publicKey = true, bool relin = true, ulong[] galois = null)
+        {
+            int sets = (publicKey ? 1 : 0) | (relin ? 2 : 0), n = galois == null ? -1 : galois.Length;
+            Cnhe.Check(Cnhe.cnhe_keys_save_compact(Ctx, sets, galois, n, null, UIntPtr.Zero, out var needed));
+            var buf = new byte[(long)needed];
+            Cnhe.Check(Cnhe.cnhe_keys_save_compact(Ctx, sets, galois, n, buf, needed, out needed));
+            return buf;
         }
 
         /// fused PoolLayer.Apply (NeuralNetworks/PoolLayer.cs:149-229): one device call for the whole layer instead of the per-output fan-out
