@@ -15,8 +15,9 @@ namespace cnhe {
 // unrolled every constant is an immediate c[bank][offset] operand of its DFMA -- no shared-memory copy, no LDS per product.
 static_assert(sizeof(BehzConstF) % 8 == 0 && sizeof(BehzConstF) <= 3584, "BehzConstF must fit the kernel parameter space");
 
-// LAZY (all kernels below): buffers exchanged with the NTT kernels hold lazy doubles (fparith.cuh) instead of canonical words
-template <bool LAZY>
+// LAZY (all kernels below): buffers exchanged with the NTT kernels hold lazy doubles (fparith.cuh) instead of canonical words.
+// BSK_ONLY: only the Bsk residues are written, out [n_polys][kb][N] (the fused square reads the q residues from the ciphertext itself)
+template <bool LAZY, bool BSK_ONLY = false>
 __global__ void __launch_bounds__(256) k_behz_lift_fp(const u64 *const *__restrict__ ct_ptrs, u64 *__restrict__ out, int n_polys, int logn,
                                                      const __grid_constant__ BehzConstF F) {
     const int N = 1 << logn, k = F.k, kb = F.kb, kt = k + kb;
@@ -24,7 +25,7 @@ __global__ void __launch_bounds__(256) k_behz_lift_fp(const u64 *const *__restri
     if (gid >= (size_t)n_polys << logn) return;
     const int x = (int)(gid & (N - 1)), poly = (int)(gid >> logn);
     const u64 *src = ct_ptrs[poly >> 1] + (size_t)(poly & 1) * k * N + x;
-    u64 *dst = out + (size_t)poly * kt * N + x;
+    u64 *dst = out + (size_t)poly * kt * N + x, *dst_b = BSK_ONLY ? out + (size_t)poly * kb * N + x : dst + (size_t)k * N;
     double tmp[KMAX];
     u64 sm = 0;
 #pragma unroll
@@ -32,7 +33,7 @@ __global__ void __launch_bounds__(256) k_behz_lift_fp(const u64 *const *__restri
         if (i < k) {
             const u64 v = src[(size_t)i * N];
             const double vd = u2d(v);
-            dst[(size_t)i * N] = LAZY ? lazy_bits(vd) : v;
+            if (!BSK_ONLY) dst[(size_t)i * N] = LAZY ? lazy_bits(vd) : v;
             tmp[i] = fcanon(fmodmul(vd, F.mtilde_inv_qhat_mod_q[i], F.qd[i], F.qinv[i]), F.qd[i], F.qinv[i]);
             sm += d2u(tmp[i]) * F.qhat_mod_mtilde[i];
         }
@@ -49,7 +50,7 @@ __global__ void __launch_bounds__(256) k_behz_lift_fp(const u64 *const *__restri
         for (int i = 0; i < KMAX; i++)
             if (i < k) acc = __dadd_rn(acc, fmodmul(tmp[i], F.qhat_mod_bsk[j][i], p, pinv));
         const double r = fmodmul(acc, F.inv_mtilde_mod_bsk[j], p, pinv); // fresh product: |r| <= 0.51 p
-        dst[(size_t)(k + j) * N] = LAZY ? lazy_bits(r) : fsmall_u(r, F.b_u[j]);
+        dst_b[(size_t)j * N] = LAZY ? lazy_bits(r) : fsmall_u(r, F.b_u[j]);
     }
 }
 
@@ -395,6 +396,11 @@ cudaError_t launch_behz_lift_fp(const u64 *const *ct_ptrs, u64 *out, int n, int 
     if (n <= 0) return cudaSuccess;
     if (lazy) k_behz_lift_fp<true><<<blocks_for((size_t)n * 2 << logn), 256, 0, s>>>(ct_ptrs, out, n * 2, logn, *f);
     else k_behz_lift_fp<false><<<blocks_for((size_t)n * 2 << logn), 256, 0, s>>>(ct_ptrs, out, n * 2, logn, *f);
+    return cudaGetLastError();
+}
+cudaError_t launch_behz_lift_bsk_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    k_behz_lift_fp<true, true><<<blocks_for((size_t)n * 2 << logn), 256, 0, s>>>(ct_ptrs, out, n * 2, logn, *f);
     return cudaGetLastError();
 }
 cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConstF *f, int lazy, cudaStream_t s) {

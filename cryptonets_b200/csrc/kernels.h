@@ -29,6 +29,7 @@ struct NttTab {
     // fwd_out_rc for its output
     const double *wd_split;
     int split_ok, split_out_rc;
+    const double *iwd_split; // N = 4096 / 8192: the two halves' inverse twiddle tables of the fused square ([half][N/2], like iwd_hi at 16384)
     int fwd_out_rc;                    // lazy forward output must be re-centred (its bound squared would overflow the consumer's product)
     double fwd_out_bound;               // |forward lazy output| <= fwd_out_bound * p
 };
@@ -178,6 +179,13 @@ cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, c
 // lazy = 1: the buffers exchanged with the NTT kernels (lift output, tensor input/output, floor input, digit input, accumulator
 // output) hold lazy doubles (fparith.cuh) -- pair with NTT_IN_F / NTT_OUT_F on the transforms in between
 cudaError_t launch_behz_lift_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
+// lazy Bsk residues only, out [n][2][kb][N]: the source of the fused square's residues l >= k
+cudaError_t launch_behz_lift_bsk_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, cudaStream_t s);
+// Fused square (N = 4096 / 8192, ntt.cu): d [n][3][kt][N] lazy doubles, coefficient form, from ciphertexts ct_ptrs[c] ([2][k][N]) and
+// their lifted Bsk residues lift_bsk ([n][2][kb][N], launch_behz_lift_bsk_fp) -- what forward transforms, the square tensor and inverse
+// transforms compute on the output of launch_behz_lift_fp(lazy); needs split_ok on all kt moduli
+cudaError_t launch_behz_square_fused(const u64 *const *ct_ptrs, const u64 *lift_bsk, u64 *d, int n_ct, int k, int kt, int logn, const NttTab *tabs,
+                                     cudaStream_t s);
 cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
 cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
 // folded constants + software-pipelined loads (lazy input only)

@@ -474,21 +474,29 @@ __device__ __forceinline__ void fwd_first_compute(double *sm, const double *twc,
     for (int e = 0; e < E; e++) sm[swz(vt + (e << LG))] = x[e];
 }
 
-// Last forward pass: stages [LOGN-4, LOGN) on 16 consecutive words; canonical result goes straight to HBM.
-template <int LOGN, int PASS, bool OUT_F>
-__device__ __forceinline__ void fwd_last_fp(const double *sm, u64 *dst, const NttTab &tb, int j) {
-    constexpr int S0 = LOGN - 4;
-    const double p = tb.pd, pinv = tb.pinv;
-    const bool rc = (tb.fwd_recenter >> PASS) & 1;
+// words 16j .. 16j+15 of a swizzled shared-memory polynomial (16-byte accesses, conflict free)
+__device__ __forceinline__ void ld_group16(const double *sm, int j, double (&x)[16]) {
     const double2 *smv = reinterpret_cast<const double2 *>(sm);
     const int xr = j & 7;
-    double x[16];
 #pragma unroll
     for (int ch = 0; ch < 8; ch++) {
-        double2 v = smv[j * 8 + (ch ^ xr)];
+        const double2 v = smv[j * 8 + (ch ^ xr)];
         x[2 * ch] = v.x;
         x[2 * ch + 1] = v.y;
     }
+}
+__device__ __forceinline__ void st_group16(double *sm, int j, const double (&x)[16]) {
+    double2 *smv = reinterpret_cast<double2 *>(sm);
+    const int xr = j & 7;
+#pragma unroll
+    for (int ch = 0; ch < 8; ch++) smv[j * 8 + (ch ^ xr)] = make_double2(x[2 * ch], x[2 * ch + 1]);
+}
+// stages [LOGN-4, LOGN) of the forward transform on the 16 consecutive coefficients of group j (pass PASS of the schedule)
+template <int LOGN, int PASS>
+__device__ __forceinline__ void fwd_last_stages(double (&x)[16], const NttTab &tb, int j) {
+    constexpr int S0 = LOGN - 4;
+    const double p = tb.pd, pinv = tb.pinv;
+    const bool rc = (tb.fwd_recenter >> PASS) & 1;
     if (rc) {
 #pragma unroll
         for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
@@ -523,6 +531,14 @@ __device__ __forceinline__ void fwd_last_fp(const double *sm, u64 *dst, const Nt
             x[e + h] = __dsub_rn(a, t);
         }
     }
+}
+// Last forward pass: stages [LOGN-4, LOGN) on 16 consecutive words; canonical result goes straight to HBM.
+template <int LOGN, int PASS, bool OUT_F>
+__device__ __forceinline__ void fwd_last_fp(const double *sm, u64 *dst, const NttTab &tb, int j) {
+    const double p = tb.pd, pinv = tb.pinv;
+    double x[16];
+    ld_group16(sm, j, x);
+    fwd_last_stages<LOGN, PASS>(x, tb, j);
     u64 *o = dst + 16 * j;
     if constexpr (OUT_F) { // lazy doubles: |x| <= fwd bound * p; re-centred only where the consumer's product could overflow (host flag)
         if (tb.fwd_out_rc) {
@@ -624,30 +640,11 @@ k_ntt_forward_digits_fp(const u64 *target, size_t ct_stride, u64 *dst, const Ntt
     fwd_body_fp<LOGN, false, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (((size_t)c * k + l) * dm.D + d) * N, tb, tid); // [c][l][d]
 }
 
-// ---- inverse, FP64: first pass reads 16 consecutive words per virtual thread straight from HBM (256-bit loads)
-template <int LOGN, bool IN_F>
-__device__ __forceinline__ void inv_first_fp(double *sm, const u64 *src, const NttTab &tb, int j) {
+// ---- inverse, FP64: stages 0..3 on the 16 consecutive coefficients of group j
+template <int LOGN>
+__device__ __forceinline__ void inv_first_stages(double (&x)[16], const NttTab &tb, int j) {
     constexpr int N = 1 << LOGN;
     const double p = tb.pd, pinv = tb.pinv;
-    double2 *smv = reinterpret_cast<double2 *>(sm);
-    const int xr = j & 7;
-    double x[16];
-#pragma unroll
-    for (int g = 0; g < 4; g++) {
-        u64 v0, v1, v2, v3;
-        ldg256(src + 16 * j + 4 * g, v0, v1, v2, v3);
-        if constexpr (IN_F) {
-            x[4 * g] = __longlong_as_double((long long)v0);
-            x[4 * g + 1] = __longlong_as_double((long long)v1);
-            x[4 * g + 2] = __longlong_as_double((long long)v2);
-            x[4 * g + 3] = __longlong_as_double((long long)v3);
-        } else {
-            x[4 * g] = u2d(v0);
-            x[4 * g + 1] = u2d(v1);
-            x[4 * g + 2] = u2d(v2);
-            x[4 * g + 3] = u2d(v3);
-        }
-    }
     // stage u uses 8 >> u consecutive inverse twiddles: 8 + 4 + 2 + 1 doubles per thread, 16-byte loads
     double tw[15];
 #pragma unroll
@@ -683,8 +680,29 @@ __device__ __forceinline__ void inv_first_fp(double *sm, const u64 *src, const N
                 if (!(e & h)) x[e] = frecenter(x[e], p, pinv);
         }
     }
+}
+// first pass reads 16 consecutive words per virtual thread straight from HBM (256-bit loads)
+template <int LOGN, bool IN_F>
+__device__ __forceinline__ void inv_first_fp(double *sm, const u64 *src, const NttTab &tb, int j) {
+    double x[16];
 #pragma unroll
-    for (int ch = 0; ch < 8; ch++) smv[j * 8 + (ch ^ xr)] = make_double2(x[2 * ch], x[2 * ch + 1]);
+    for (int g = 0; g < 4; g++) {
+        u64 v0, v1, v2, v3;
+        ldg256(src + 16 * j + 4 * g, v0, v1, v2, v3);
+        if constexpr (IN_F) {
+            x[4 * g] = __longlong_as_double((long long)v0);
+            x[4 * g + 1] = __longlong_as_double((long long)v1);
+            x[4 * g + 2] = __longlong_as_double((long long)v2);
+            x[4 * g + 3] = __longlong_as_double((long long)v3);
+        } else {
+            x[4 * g] = u2d(v0);
+            x[4 * g + 1] = u2d(v1);
+            x[4 * g + 2] = u2d(v2);
+            x[4 * g + 3] = u2d(v3);
+        }
+    }
+    inv_first_stages<LOGN>(x, tb, j);
+    st_group16(sm, j, x);
 }
 // The last stage (one twiddle, iw[1]) carries N^-1: sums are multiplied by N^-1, differences by iw[1]*N^-1, so every output is a
 // fresh modular product in (-0.51p, 0.51p): written as is (OUT_F, lazy double) or sign-fixed on the integer pipe (canonical).
@@ -873,16 +891,17 @@ __device__ __forceinline__ double ld_dsmem(unsigned addr) {
     asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(addr) : "memory");
     return v;
 }
-// first pass of half `upper`: stage 0 of the 16384-point transform folded into the loads, then 5 stages (j = 0: low twiddles only)
-template <bool IN_F>
+// first pass of half `upper` of a 2^(HLOGN+1)-point transform: its stage 0 folded into the loads, then HLOGN - 8 stages (j = 0: low
+// twiddles only), so that two 4-stage passes finish the half
+template <int HLOGN, bool IN_F>
 __device__ __forceinline__ void fwd_split_first(double *sm, const double *twc, const FwdSrc &src, const NttTab &tb, int vt, double w0, bool upper) {
-    constexpr int R = 5, E = 1 << R, LG = SPLIT_LOGN - R;
+    constexpr int R = HLOGN - 8, E = 1 << R, LG = HLOGN - R;
     const double p = tb.pd, pinv = tb.pinv;
     double x[E];
 #pragma unroll
     for (int e = 0; e < E; e++) {
         const int idx = vt + (e << LG);
-        const double a = fwd_load_fp<IN_F>(src, idx, p, pinv), c = fwd_load_fp<IN_F>(src, idx + SPLIT_H, p, pinv);
+        const double a = fwd_load_fp<IN_F>(src, idx, p, pinv), c = fwd_load_fp<IN_F>(src, idx + (1 << HLOGN), p, pinv);
         const double t = fmodmul(c, w0, p, pinv);
         x[e] = upper ? __dsub_rn(a, t) : __dadd_rn(a, t);
     }
@@ -911,7 +930,7 @@ __device__ __forceinline__ void fwd_split_body(double *sm, const FwdSrc &src, u6
     tb.fwd_recenter = tb.fwd_recenter_split;
     load_twiddle_cache(twc, tb.wd, tid, TR);
     __syncthreads();
-    fwd_split_first<IN_F>(sm, twc, src, tb, tid, w0, half != 0);
+    fwd_split_first<SPLIT_LOGN, IN_F>(sm, twc, src, tb, tid, w0, half != 0);
     cluster_arrive(); // this CTA has read everything it needs from the source polynomial
     __syncthreads();
     CNHE_VTN(SPLIT_H / 16, (fwd_pass_fp<SPLIT_LOGN, 5, 4, false, 1, false>(sm, twc, src, tb, vt))); __syncthreads();
@@ -944,53 +963,70 @@ k_ntt_forward_digits_split(const u64 *target, size_t ct_stride, u64 *dst, const 
     fs.need_reduce = dm.mask >= tb.mod.p;
     fwd_split_body<false, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (((size_t)c * k + l) * dm.D + d) * (2 * SPLIT_H) + half * SPLIT_H, tb, half, tid);
 }
-// last in-half pass (stages 8..12) and the cross-half butterfly: own results go to shared memory for the partner, the partner's come
-// back through DSMEM; half 0 keeps the sums (times N^-1), half 1 the differences (times iw[1] N^-1)
-template <bool OUT_F>
-__device__ __forceinline__ void inv_split_last(double *sm, const double *twc, u64 *dst, const u64 *base_add, const NttTab &tb, int vt, int half) {
-    constexpr int V0 = 8, R = 5, E = 1 << R, N = SPLIT_H;
+// last in-half pass (stages 8 .. HLOGN-1) and the cross-half butterfly of NB polynomials (consecutive half buffers of sm; polynomial b goes to
+// dst + b * dst_stride): own results go to shared memory for the partner, the partner's come back through DSMEM; half 0 keeps the sums
+// (times N^-1), half 1 the differences (times iw[1] N^-1).  One pair of cluster barriers serves all NB polynomials.
+template <int HLOGN, int TR, bool OUT_F, int NB = 1>
+__device__ __forceinline__ void inv_split_last(double *sm, const double *twc, u64 *dst, size_t dst_stride, const u64 *base_add, const NttTab &tb,
+                                               int tid, int half) {
+    constexpr int V0 = 8, R = HLOGN - V0, E = 1 << R, H = 1 << HLOGN;
+    static_assert(E >= 8, "the cross-half stage reads the partner in batches of 8");
     const double p = tb.pd, pinv = tb.pinv;
-    double x[E];
+#pragma unroll 1
+    for (int b = 0; b < NB; b++) {
+        double *s = sm + b * H;
+        for (int vt = tid; vt < (H >> R); vt += TR) {
+            double x[E];
 #pragma unroll
-    for (int e = 0; e < E; e++) x[e] = sm[swz(vt + (e << V0))];
+            for (int e = 0; e < E; e++) x[e] = s[swz(vt + (e << V0))];
 #pragma unroll
-    for (int u = 0; u < R; u++) {
-        const int h = 1 << u;
-        const bool rc = (tb.inv_recenter >> (V0 + u)) & 1;
+            for (int u = 0; u < R; u++) {
+                const int h = 1 << u;
+                const bool rc = (tb.inv_recenter >> (V0 + u)) & 1;
 #pragma unroll
-        for (int e = 0; e < E; e++) {
-            if (e & h) continue;
-            const double w = twc[(N >> (V0 + u + 1)) + (e >> (u + 1))];
-            const double a = x[e], bq = x[e + h];
-            x[e] = __dadd_rn(a, bq);
-            x[e + h] = fmodmul(__dsub_rn(a, bq), w, p, pinv);
-        }
-        if (rc) {
+                for (int e = 0; e < E; e++) {
+                    if (e & h) continue;
+                    const double w = twc[(H >> (V0 + u + 1)) + (e >> (u + 1))];
+                    const double a = x[e], bq = x[e + h];
+                    x[e] = __dadd_rn(a, bq);
+                    x[e + h] = fmodmul(__dsub_rn(a, bq), w, p, pinv);
+                }
+                if (rc) {
 #pragma unroll
-            for (int e = 0; e < E; e++)
-                if (!(e & h)) x[e] = frecenter(x[e], p, pinv);
+                    for (int e = 0; e < E; e++)
+                        if (!(e & h)) x[e] = frecenter(x[e], p, pinv);
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < E; e++) s[swz(vt + (e << V0))] = x[e];
         }
     }
-#pragma unroll
-    for (int e = 0; e < E; e++) sm[swz(vt + (e << V0))] = x[e];
     cluster_arrive();
     cluster_wait(); // both halves are complete and visible across the pair
     const unsigned peer = dsmem_base(sm, (unsigned)(half ^ 1));
     const double scale = half ? tb.inv_n_w_d : tb.inv_n_d;
+#pragma unroll 1
+    for (int b = 0; b < NB; b++) {
+        const double *s = sm + b * H;
+        u64 *d = dst + b * dst_stride;
+        for (int vt = tid; vt < (H >> R); vt += TR) {
 #pragma unroll
-    for (int e0 = 0; e0 < E; e0 += 8) { // the partner's values in batches of 8: all 32 next to x[] would spill
-        double r[8];
+            for (int e0 = 0; e0 < E; e0 += 8) { // own values back from shared memory, the partner's in batches of 8 (all at once would spill)
+                double r[8];
 #pragma unroll
-        for (int i = 0; i < 8; i++) r[i] = ld_dsmem(peer + 8u * (unsigned)swz(vt + ((e0 + i) << V0)));
+                for (int i = 0; i < 8; i++) r[i] = ld_dsmem(peer + 8u * (unsigned)(b * H + swz(vt + ((e0 + i) << V0))));
 #pragma unroll
-        for (int i = 0; i < 8; i++) {
-            const int idx = vt + ((e0 + i) << V0);
-            const double v = fmodmul(half ? __dsub_rn(r[i], x[e0 + i]) : __dadd_rn(x[e0 + i], r[i]), scale, p, pinv);
-            if constexpr (OUT_F) dst[idx] = lazy_bits(v);
-            else {
-                u64 o = fsmall_u(v, tb.mod.p);
-                if (base_add) o = addmod(o, base_add[idx], tb.mod.p);
-                dst[idx] = o;
+                for (int i = 0; i < 8; i++) {
+                    const int idx = vt + ((e0 + i) << V0);
+                    const double x = s[swz(idx)];
+                    const double v = fmodmul(half ? __dsub_rn(r[i], x) : __dadd_rn(x, r[i]), scale, p, pinv);
+                    if constexpr (OUT_F) d[idx] = lazy_bits(v);
+                    else {
+                        u64 o = fsmall_u(v, tb.mod.p);
+                        if (base_add) o = addmod(o, base_add[idx], tb.mod.p);
+                        d[idx] = o;
+                    }
+                }
             }
         }
     }
@@ -1019,7 +1055,7 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
     CNHE_VTN(H / 16, (inv_first_fp<SPLIT_LOGN, IN_F>(sm, s, tb, vt)));
     __syncthreads();
     CNHE_VTN(H / 16, (inv_pass_fp<SPLIT_LOGN, 4, 4, false, false>(sm, twc, d, ba, tb, vt))); __syncthreads();
-    inv_split_last<OUT_F>(sm, twc, d, ba, tb, tid, half);
+    inv_split_last<SPLIT_LOGN, TR, OUT_F>(sm, twc, d, 0, ba, tb, tid, half);
 }
 
 // ================================================================ fused key switch, N = 4096 / 8192
@@ -1216,6 +1252,99 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
             stg256(o + 4 * g, lazy_bits(a.x), lazy_bits(a.y), lazy_bits(b.x), lazy_bits(b.y));
         }
     }
+}
+
+// ================================================================ fused BEHZ square, N = 4096 / 8192
+// The square of a ciphertext in the extended base q u Bsk: d0 = c0^2, d1 = 2 c0 c1, d2 = c1^2 pointwise in the NTT domain, back in the
+// coefficient domain.  Within one residue l the forward transforms, the products and the inverse transforms never leave that residue,
+// so a cluster of two CTAs takes (ciphertext c, residue l) and only the lift before and the floor after cross residues.  As separate
+// kernels (lift -> forward -> tensor -> inverse -> floor) every step is an HBM round trip of the whole extended ciphertext: 245
+// polynomial passes per ciphertext at k = 5, kb = 6, against 125 here.  CTA h owns half h of the N-point transforms (the split form of
+// the N = 16384 kernels and of the fused key switch): it folds stage 0 into its loads of both halves of c0_l and c1_l (the partner's
+// reads of the same lines are L2 hits), runs the N/2-point forward passes of both, squares in registers right after the last forward
+// pass and runs the first inverse pass on the same 16 coefficients per thread, then the remaining inverse passes of the three products
+// together and the cross-half last stage (which carries N^-1) through DSMEM.  Lazy bounds: the forward output is re-centred where
+// split_out_rc says so (|c|^2 p < 2^51); |d1| <= 1.02 p is within the inverse's 1.25 p input bound; inv_recenter is the full transform's.
+// Sources: residue l < k is the canonical input residue itself, l >= k the lift's lazy Bsk residue ([c][2][kb][N]).  Output: lazy
+// doubles in the [c][3][kt][N] layout of the separate inverse transforms, which the floor reads.
+template <int HLOGN>
+__host__ __device__ constexpr int sq_fused_threads() { return (1 << HLOGN) / 16; }
+template <int HLOGN>
+__host__ __device__ constexpr int sq_fused_smem() { return (1 << HLOGN) * 8 * 3 + 2 * TWC * 8; } // three half buffers, two twiddle caches
+template <int HLOGN>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(sq_fused_threads<HLOGN>(), HLOGN == 12 ? 2 : 4)
+k_behz_square_fused(const u64 *const *__restrict__ ct_ptrs, const u64 *__restrict__ lift, u64 *__restrict__ d, const NttTab *__restrict__ tabs,
+                    int k, int kt) {
+    constexpr int H = 1 << HLOGN, TR = sq_fused_threads<HLOGN>(), N = 2 * H, R1 = HLOGN - 8;
+    extern __shared__ __align__(16) u64 sq_raw[];
+    double *sm = reinterpret_cast<double *>(sq_raw); // [3][H]: c0 then d0, c1 then d1, d2
+    double *twc = sm + 3 * H, *twci = twc + TWC;    // forward / inverse twiddles of this half
+    const int half = blockIdx.x & 1, l = (blockIdx.x >> 1) % kt, c = (blockIdx.x >> 1) / kt, tid = threadIdx.x;
+    NttTab tb = tabs[l];
+    const double w0 = __ldg(tb.wd + 1);
+    tb.wd = tb.wd_split + half * H;
+    tb.iwd = tb.iwd_split + half * H;
+    tb.fwd_recenter = tb.fwd_recenter_split;
+    const double p = tb.pd, pinv = tb.pinv;
+    FwdSrc fs;
+    fs.digit = false; fs.need_reduce = false; fs.shift = 0; fs.mask = 0;
+    load_twiddle_cache(twc, tb.wd, tid, TR);
+    load_twiddle_cache(twci, tb.iwd, tid, TR);
+    __syncthreads();
+#pragma unroll 1
+    for (int r = 0; r < 2; r++) {
+        if (l < k) {
+            fs.src = ct_ptrs[c] + ((size_t)r * k + l) * N;
+            CNHE_VTN(H >> R1, (fwd_split_first<HLOGN, false>(sm + r * H, twc, fs, tb, vt, w0, half != 0)));
+        } else {
+            fs.src = lift + ((size_t)(c * 2 + r) * (kt - k) + (l - k)) * N;
+            CNHE_VTN(H >> R1, (fwd_split_first<HLOGN, true>(sm + r * H, twc, fs, tb, vt, w0, half != 0)));
+        }
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int r = 0; r < 2; r++) CNHE_VTN(H / 16, (fwd_pass_fp<HLOGN, R1, 4, false, 1, false>(sm + r * H, twc, fs, tb, vt)));
+    __syncthreads();
+    {
+        // thread j owns coefficients 16j .. 16j+15 of every buffer from the last forward pass to the first inverse pass: no barrier.
+        // One group of 16 in registers per transform step (two plus the twiddles spill): c0 and c1 wait in their own slots
+        const int j = tid;
+        double x[16], y[16];
+#pragma unroll 1
+        for (int r = 0; r < 2; r++) {
+            ld_group16(sm + r * H, j, x);
+            fwd_last_stages<HLOGN, 2>(x, tb, j);
+            if (tb.split_out_rc) {
+#pragma unroll
+                for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
+            }
+            st_group16(sm + r * H, j, x);
+        }
+        // the products of k_behz_tensor_fp (square): d2 = c1^2, d1 = 2 c0 c1, d0 = c0^2, each overwriting a slot no longer read
+        ld_group16(sm + H, j, x);
+#pragma unroll
+        for (int e = 0; e < 16; e++) x[e] = fmodmul(x[e], x[e], p, pinv);
+        inv_first_stages<HLOGN>(x, tb, j);
+        st_group16(sm + 2 * H, j, x);
+        ld_group16(sm, j, x);
+        ld_group16(sm + H, j, y);
+#pragma unroll
+        for (int e = 0; e < 16; e++) {
+            const double cross = fmodmul(x[e], y[e], p, pinv);
+            y[e] = __dadd_rn(cross, cross);
+        }
+        inv_first_stages<HLOGN>(y, tb, j);
+        st_group16(sm + H, j, y);
+#pragma unroll
+        for (int e = 0; e < 16; e++) x[e] = fmodmul(x[e], x[e], p, pinv);
+        inv_first_stages<HLOGN>(x, tb, j);
+        st_group16(sm, j, x);
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int r = 0; r < 3; r++) CNHE_VTN(H / 16, (inv_pass_fp<HLOGN, 4, 4, false, false>(sm + r * H, twci, nullptr, nullptr, tb, vt)));
+    __syncthreads();
+    inv_split_last<HLOGN, TR, true, 3>(sm, twci, d + ((size_t)c * 3 * kt + l) * N + half * H, (size_t)kt * N, nullptr, tb, tid, half);
 }
 
 // ================================================================ persistent TMA-staged transforms, N = 4096 / 8192
@@ -1872,6 +2001,20 @@ cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u
     if (n_ct <= 0) return cudaSuccess;
     if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, key_packed, acc, n_ct, k, dm, tabs, s);
     if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, key_packed, acc, n_ct, k, dm, tabs, s);
+    return cudaErrorInvalidValue;
+}
+template <int HL>
+static cudaError_t launch_sq_fused(const u64 *const *ct_ptrs, const u64 *lift, u64 *d, int n_ct, int k, int kt, const NttTab *tabs, cudaStream_t s) {
+    cudaError_t e = cudaFuncSetAttribute(k_behz_square_fused<HL>, cudaFuncAttributeMaxDynamicSharedMemorySize, sq_fused_smem<HL>());
+    if (e != cudaSuccess) return e;
+    k_behz_square_fused<HL><<<2 * n_ct * kt, sq_fused_threads<HL>(), sq_fused_smem<HL>(), s>>>(ct_ptrs, lift, d, tabs, k, kt);
+    return cudaGetLastError();
+}
+cudaError_t launch_behz_square_fused(const u64 *const *ct_ptrs, const u64 *lift_bsk, u64 *d, int n_ct, int k, int kt, int logn, const NttTab *tabs,
+                                     cudaStream_t s) {
+    if (n_ct <= 0) return cudaSuccess;
+    if (logn == 13) return launch_sq_fused<12>(ct_ptrs, lift_bsk, d, n_ct, k, kt, tabs, s);
+    if (logn == 12) return launch_sq_fused<11>(ct_ptrs, lift_bsk, d, n_ct, k, kt, tabs, s);
     return cudaErrorInvalidValue;
 }
 template <int HL>

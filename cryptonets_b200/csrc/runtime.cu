@@ -500,7 +500,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     for (u64 p : c.q) moduli.push_back(p);
     for (u64 p : c.bsk) moduli.push_back(p);
     for (u64 p : c.t) moduli.push_back(p);
-    constexpr size_t TAB_WORDS = 9; // N-word tables per modulus: w, ws, iw, iws, wd, iwd, wd_hi, iwd_hi, wd_split
+    constexpr size_t TAB_WORDS = 10; // N-word tables per modulus: w, ws, iw, iws, wd, iwd, wd_hi, iwd_hi, wd_split, iwd_split
     std::vector<u64> host((size_t)n_mod * TAB_WORDS * N, 0);
     CNHE_CUDA(cudaMalloc((void **)&c.d_table_mem, host.size() * sizeof(u64)));
     c.h_tabs.resize(n_mod);
@@ -508,7 +508,8 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
         const u64 p = moduli[m];
         const u64 psi = hm::minimal_primitive_root(2ULL * N, p), ipsi = hm::inv(psi, p);
         u64 *w = &host[(size_t)m * TAB_WORDS * N], *ws = w + N, *iw = ws + N, *iws = iw + N;
-        double *wd = reinterpret_cast<double *>(iws + N), *iwd = wd + N, *wd_hi = iwd + N, *iwd_hi = wd_hi + N, *wd_split = iwd_hi + N;
+        double *wd = reinterpret_cast<double *>(iws + N), *iwd = wd + N, *wd_hi = iwd + N, *iwd_hi = wd_hi + N, *wd_split = iwd_hi + N,
+               *iwd_split = wd_split + N;
         u64 a = 1, b = 1;
         for (u64 i = 0; i < N; i++) {
             const u64 r = hm::bit_reverse(i, logN);
@@ -539,12 +540,13 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
                 for (int i = 0; i < 2; i++) iwd_hi[(u64)(12 + i) * T + j] = iwd[(N >> 3) + (j << 1) + i];
                 iwd_hi[(u64)14 * T + j] = iwd[(N >> 4) + j];
             }
-            const u64 H = N / 2; // the halves' forward tables of the fused key switch, laid out as wd_hi is at N = 16384
+            const u64 H = N / 2; // the halves' tables of the fused key switch (forward) and square (both), laid out as wd_hi / iwd_hi at N = 16384
             for (u64 h = 0; h < 2; h++)
                 for (u64 i = 1; i < H; i++) {
                     u64 m2 = 1;
                     while (2 * m2 <= i) m2 *= 2;
                     wd_split[h * H + i] = wd[i + m2 + h * m2];
+                    iwd_split[h * H + i] = iwd[i + m2 + h * m2];
                 }
         }
         NttTab &tb = c.h_tabs[m];
@@ -555,6 +557,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
         tb.wd_hi = reinterpret_cast<const double *>(base + 6 * (size_t)N);
         tb.iwd_hi = reinterpret_cast<const double *>(base + 7 * (size_t)N);
         tb.wd_split = reinterpret_cast<const double *>(base + 8 * (size_t)N);
+        tb.iwd_split = reinterpret_cast<const double *>(base + 9 * (size_t)N);
         tb.inv_n = hm::inv(N % p, p);
         tb.inv_n_s = hm::shoup(tb.inv_n, p);
         tb.mod = make_dmod(p);
@@ -826,9 +829,48 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
     }
 }
 
-static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, int c0, int m, u64 *out3) {
+// whether a product takes the fused square (forward transforms, tensor square and inverse transforms in one kernel, ntt.cu): every
+// pair is a square (a[i] == b[i]), N = 4096 / 8192 on the lazy FP64 path, the split schedule exact on every modulus of q u Bsk.
+// CNHE_MUL_FUSED=0 / =1 forces the separate kernels / the fused square wherever it applies (read per call: tests compare both in one process)
+static bool mul_fused(const Context &c, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b) {
+    if (c.logN != 12 && c.logN != 13) return false;
+    const int kt = c.k + c.kb;
+    if (!(c.lazy && c.fp_elementwise && fp_range(c, 0, kt))) return false;
+    for (int i = 0; i < kt; i++)
+        if (!c.h_tabs[i].split_ok) return false;
+    for (size_t i = 0; i < a.size(); i++)
+        if (a[i] != b[i]) return false;
+    const char *v = getenv("CNHE_MUL_FUSED");
+    return v ? atoi(v) != 0 : true;
+}
+// scratch words per ciphertext of multiply_chunk
+static size_t mul_words(const Context &c, bool fused) { return (size_t)(fused ? 2 * c.kb + 3 * (c.k + c.kb) : 7 * (c.k + c.kb)) * c.N; }
+static void multiply_floor(Context &c, int ch, const u64 *D, int m, bool lazy, u64 *out3) {
+    PROF(2, 8.0 * c.N * m * 3 * (2 * c.k + c.kb));
+    static const bool fold = getenv("CNHE_FLOOR_NOFOLD") == nullptr;
+    if (c.fp_elementwise && lazy && fold) c.check(launch_behz_floor_fold_fp(D, out3, m, c.logN, &c.ch[ch].floor_f, c.stream), "behz_floor_fold_fp");
+    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, m, c.ch[ch].t, c.logN, &c.h_bf, lazy, c.stream), "behz_floor_fp");
+    else c.check(launch_behz_floor(D, out3, m, c.ch[ch].t, c.logN, c.d_bc, c.stream), "behz_floor");
+}
+static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, int c0, int m, u64 *out3,
+                           bool fused) {
     const int k = c.k, kt = k + c.kb;
     const size_t N = c.N;
+    if (fused) {
+        const u64 *const *ptrs = upload_ptrs(c, std::vector<const u64 *>(a.begin() + c0, a.begin() + c0 + m));
+        u64 *L = c.ws_alloc((size_t)m * 2 * c.kb * N), *D = c.ws_alloc((size_t)m * 3 * kt * N);
+        {
+            PROF(2, 8.0 * N * m * 2 * (k + c.kb));
+            c.check(launch_behz_lift_bsk_fp(ptrs, L, m, c.logN, &c.h_bf, c.stream), "behz_lift_bsk_fp");
+        }
+        {
+            // HBM: both polynomials of every residue read once (the partner's reads are L2 hits), the three products written once
+            PROF(0, 8.0 * N * m * (2 * kt + 3 * kt));
+            c.check(launch_behz_square_fused(ptrs, L, D, m, k, kt, c.logN, c.d_tabs, c.stream), "behz_square_fused");
+        }
+        multiply_floor(c, ch, D, m, true, out3);
+        return;
+    }
     bool square = true;
     for (int i = 0; i < m; i++) square = square && a[c0 + i] == b[c0 + i];
     std::vector<const u64 *> pa(a.begin() + c0, a.begin() + c0 + m);
@@ -863,19 +905,16 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
         PROF(1, 16.0 * N * m * 3 * kt);
         c.check(launch_ntt_inverse(D, D, m * 3 * kt, c.logN, c.d_tabs, 0, kt, fmt, c.stream), "ntt_inverse");
     }
-    PROF(2, 8.0 * N * m * 3 * (kt + k));
-    static const bool fold = getenv("CNHE_FLOOR_NOFOLD") == nullptr;
-    if (c.fp_elementwise && lazy && fold) c.check(launch_behz_floor_fold_fp(D, out3, m, c.logN, &c.ch[ch].floor_f, c.stream), "behz_floor_fold_fp");
-    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, m, c.ch[ch].t, c.logN, &c.h_bf, lazy, c.stream), "behz_floor_fp");
-    else c.check(launch_behz_floor(D, out3, m, c.ch[ch].t, c.logN, c.d_bc, c.stream), "behz_floor");
+    multiply_floor(c, ch, D, m, lazy, out3);
 }
 void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3) {
     const int n = (int)a.size();
-    const int wave = c.wave((size_t)(7 * (c.k + c.kb)) * c.N);
+    const bool fused = mul_fused(c, a, b);
+    const int wave = c.wave(mul_words(c, fused));
     for (int c0 = 0; c0 < n; c0 += wave) {
         WsScope scope(c);
         const int m = std::min(wave, n - c0);
-        multiply_chunk(c, ch, a, b, c0, m, out3 + (size_t)c0 * 3 * c.k * c.N);
+        multiply_chunk(c, ch, a, b, c0, m, out3 + (size_t)c0 * 3 * c.k * c.N, fused);
     }
     c.note(Context::OP_MULTIPLY, ch, n);
 }
@@ -893,12 +932,13 @@ void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, co
     if (!c.ch[ch].have_rlk) throw Error(-3, "relinearization keys are missing");
     const int n = (int)a.size(), k = c.k;
     const size_t N = c.N;
-    const int wave = c.wave(((ks_fused(c, n) ? 0 : (size_t)c.dm_relin.D * k) + 7 * (k + c.kb) + 5 * k) * N);
+    const bool fused = mul_fused(c, a, b);
+    const int wave = c.wave((ks_fused(c, n) ? 0 : (size_t)c.dm_relin.D * k * N) + mul_words(c, fused) + 5 * k * N);
     for (int c0 = 0; c0 < n; c0 += wave) {
         WsScope scope(c); // stream-ordered frees: the next wave reuses the memory once these kernels are done
         const int m = std::min(wave, n - c0);
         u64 *ct3 = c.ws_alloc((size_t)m * 3 * k * N);
-        multiply_chunk(c, ch, a, b, c0, m, ct3);
+        multiply_chunk(c, ch, a, b, c0, m, ct3, fused);
         const size_t s3 = (size_t)3 * k * N;
         const BufRef &pk = c.ch[ch].rlk_packed;
         op_key_switch(c, ct3 + (size_t)2 * k * N, s3, m, c.ch[ch].rlk->p, c.dm_relin, ct3, s3, out2 + (size_t)c0 * 2 * k * N, pk ? pk->p : nullptr);
