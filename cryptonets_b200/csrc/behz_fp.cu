@@ -5,7 +5,6 @@
 // 128-bit integer product (4 mul.hi.u64 + 6 mul.lo.u64, the slowest instructions on the integer pipe).  Wherever SEAL's
 // algorithm depends on the *representative* of a residue (the fast base conversions sum [x c]_p * c' over the integers),
 // the canonical representative in [0,p) is formed first, exactly as in behz.cu.
-#include <cstdlib>
 #include "fparith.cuh"
 #include "kernels.h"
 
@@ -15,7 +14,7 @@ namespace cnhe {
 // unrolled every constant is an immediate c[bank][offset] operand of its DFMA -- no shared-memory copy, no LDS per product.
 static_assert(sizeof(BehzConstF) % 8 == 0 && sizeof(BehzConstF) <= 3584, "BehzConstF must fit the kernel parameter space");
 
-// LAZY (all kernels below): buffers exchanged with the NTT kernels hold lazy doubles (fparith.cuh) instead of canonical words.
+// LAZY (the kernels below that take it): buffers exchanged with the NTT kernels hold lazy doubles (fparith.cuh) instead of canonical words.
 // BSK_ONLY: only the Bsk residues are written, out [n_polys][kb][N] (the fused square reads the q residues from the ciphertext itself)
 template <bool LAZY, bool BSK_ONLY = false>
 __global__ void __launch_bounds__(256) k_behz_lift_fp(const u64 *const *__restrict__ ct_ptrs, u64 *__restrict__ out, int n_polys, int logn,
@@ -89,7 +88,7 @@ __global__ void __launch_bounds__(256) k_behz_tensor_fp(const u64 *a, const u64 
     }
 }
 
-template <bool LAZY>
+// canonical input (the lazy input of the product takes k_behz_floor_fold_fp)
 __global__ void __launch_bounds__(256) k_behz_floor_fp(const u64 *__restrict__ d, u64 *__restrict__ out, int n_polys, double t, int logn,
                                                       const __grid_constant__ BehzConstF F) {
     const int N = 1 << logn, k = F.k, kb = F.kb, kt = k + kb, na = kb - 1;
@@ -103,7 +102,7 @@ __global__ void __launch_bounds__(256) k_behz_floor_fp(const u64 *__restrict__ d
     for (int i = 0; i < KMAX; i++)
         if (i < k) {
             const double p = F.qd[i], pinv = F.qinv[i];
-            const double v = fmodmul(LAZY ? ld_lazy(src + (size_t)i * N) : u2d(src[(size_t)i * N]), t, p, pinv);
+            const double v = fmodmul(u2d(src[(size_t)i * N]), t, p, pinv);
             tmp[i] = fcanon(fmodmul(v, F.inv_qhat_mod_q[i], p, pinv), p, pinv);
         }
 #pragma unroll
@@ -114,7 +113,7 @@ __global__ void __launch_bounds__(256) k_behz_floor_fp(const u64 *__restrict__ d
 #pragma unroll
             for (int i = 0; i < KMAX; i++)
                 if (i < k) conv = __dadd_rn(conv, fmodmul(tmp[i], F.qhat_mod_bsk[j][i], p, pinv));
-            const double xb = fmodmul(LAZY ? ld_lazy(src + (size_t)(k + j) * N) : u2d(src[(size_t)(k + j) * N]), t, p, pinv);
+            const double xb = fmodmul(u2d(src[(size_t)(k + j) * N]), t, p, pinv);
             fl[j] = fmodmul(frecenter(__dsub_rn(xb, conv), p, pinv), F.inv_q_mod_bsk[j], p, pinv);
         }
     const double pm = F.bd[na], pminv = F.binv[na];
@@ -409,10 +408,9 @@ cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int
     else k_behz_tensor_fp<false><<<blocks_for(((size_t)n * kt) << logn), 256, 0, s>>>(a, b, d, n, logn, *f);
     return cudaGetLastError();
 }
-cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, int lazy, cudaStream_t s) {
+cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
-    if (lazy) k_behz_floor_fp<true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f);
-    else k_behz_floor_fp<false><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f);
+    k_behz_floor_fp<<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f);
     return cudaGetLastError();
 }
 cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s) {
@@ -424,13 +422,10 @@ cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, 
 cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, u64 *acc, int n, int D, int k, int logn, const BehzConstF *f, int lazy,
                              cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
-    static const int unr = getenv("CNHE_KSMAC") ? atoi(getenv("CNHE_KSMAC")) : 1;       // tuning knob: digits in flight per thread
-    static const int cts = getenv("CNHE_KSMAC_CT") ? atoi(getenv("CNHE_KSMAC_CT")) : 4; // ciphertexts per thread (key reuse)
     // key reuse pays once the launch fills the GPU anyway: with few ciphertexts (LoLa: 1-32 per call) four per thread leaves SMs idle
-    const int ct = n < 64 ? 1 : (cts == 1 || cts == 2 || (cts == 8 && lazy) ? cts : 4);
-    // full waves of lazy digits: the copy-engine-staged kernel (CNHE_KSMAC_TMA=0 keeps the register version)
-    const bool tma = getenv("CNHE_KSMAC_TMA") ? atoi(getenv("CNHE_KSMAC_TMA")) != 0 : true; // read per launch (tests compare both)
-    if (lazy && tma && ct == 4 && (1 << logn) % KT_X == 0) {
+    const int ct = n < 64 ? 1 : 4;
+    static_assert(1024 % KT_X == 0, "every ring (N >= 1024) is a whole number of tiles");
+    if (lazy && ct == 4) { // full waves of lazy digits: the copy-engine-staged kernel
         constexpr int smem = KT_STAGES * (4 + 2) * KT_X * 8 + 2 * KT_STAGES * 8;
         cudaError_t e = cudaFuncSetAttribute(k_ks_mac_tma<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return e;
@@ -439,22 +434,9 @@ cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, u64 *acc, int n,
         return cudaGetLastError();
     }
     const unsigned blocks = blocks_for(((size_t)((n + ct - 1) / ct) * k) << (logn - 1));
-    if (!lazy) {
-        if (ct == 4) k_ks_mac_fp<false, 1, 4><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-        else if (ct == 2) k_ks_mac_fp<false, 2, 2><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-        else k_ks_mac_fp<false, 4, 1><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-    } else if (ct == 8) {
-        k_ks_mac_fp<true, 1, 8><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-    } else if (ct == 4) {
-        if (unr == 2) k_ks_mac_fp<true, 2, 4><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-        else k_ks_mac_fp<true, 1, 4><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-    } else if (ct == 2) {
-        if (unr == 2) k_ks_mac_fp<true, 2, 2><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-        else k_ks_mac_fp<true, 1, 2><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-    } else if (unr == 1) k_ks_mac_fp<true, 1, 1><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-    else if (unr == 2) k_ks_mac_fp<true, 2, 1><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-    else if (unr == 8) k_ks_mac_fp<true, 8, 1><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
-    else k_ks_mac_fp<true, 4, 1><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
+    if (lazy) k_ks_mac_fp<true, 1, 1><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
+    else if (ct == 4) k_ks_mac_fp<false, 1, 4><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
+    else k_ks_mac_fp<false, 4, 1><<<blocks, 256, 0, s>>>(digits, key, acc, n, D, logn, *f);
     return cudaGetLastError();
 }
 

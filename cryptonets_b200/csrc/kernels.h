@@ -14,22 +14,22 @@ struct NttTab {
     DMod mod;
     // FP64 butterfly path (p < 2^50): the same twiddles as exact doubles, centred in (-p/2, p/2]
     const double *wd, *iwd;
-    // the 15N/16 twiddles of the four unit-stride stages, transposed for the persistent kernels: wd_hi[m * N/16 + j] is the m-th twiddle
-    // (m = 0..14: 1 + 2 + 4 + 8 per stage) of the 16-coefficient group j in the last forward pass; iwd_hi likewise for the first inverse pass
-    const double *wd_hi, *iwd_hi;
+    // N = 4096 / 8192: the 15N/16 inverse twiddles of the four unit-stride stages, transposed for the persistent inverse transform:
+    // iwd_hi[m * N/16 + j] is the m-th twiddle (m = 0..14: 8 + 4 + 2 + 1 per stage) of the 16-coefficient group j in the first pass
+    const double *iwd_hi;
     double pd, pinv, inv_n_d;
     double inv_n_w_d;                   // iw[1] * N^-1 mod p, centred: the last inverse stage carries the N^-1 scaling
     int fp_ok;                          // 1 when the FP64 path is exact for this modulus and N
     unsigned fwd_recenter, inv_recenter; // forward: bit i = re-centre at the start of pass i; inverse: bit v = re-centre the sums of stage v
-    // N = 16384 runs as two half-size transforms on a CTA pair (ntt.cu, "split"): wd_hi / iwd_hi then hold the two halves' twiddle
-    // tables ([half][8192], indexed like wd / iwd of an 8192-point transform) and this is the forward schedule of the passes 1+5 | 4 | 4
+    // Split form (ntt.cu, N = 4096 / 8192 / 16384): after the first stage the two halves of an N-point transform are independent
+    // N/2-point transforms -- the CTA-pair transforms of N = 16384, the fused key switch and the fused square run them.  wd_split /
+    // iwd_split hold the two halves' twiddle tables ([half][N/2], indexed like wd / iwd of an N/2-point transform), fwd_recenter_split
+    // is the forward schedule of the passes 1+(logN-9) | 4 | 4, split_ok = 1 when that schedule is exact, split_out_rc is fwd_out_rc
+    // for the fused kernels' output (N = 16384 has no other schedule: fwd_out_rc there covers the split one)
     unsigned fwd_recenter_split;
-    // N = 4096 / 8192: the two halves' forward twiddle tables ([half][N/2]) of the fused key switch, which runs the same split form
-    // (fwd_recenter_split is then its schedule: passes 1+(logN-9) | 4 | 4); split_ok = 1 when that schedule is exact, split_out_rc is
-    // fwd_out_rc for its output
     const double *wd_split;
     int split_ok, split_out_rc;
-    const double *iwd_split; // N = 4096 / 8192: the two halves' inverse twiddle tables of the fused square ([half][N/2], like iwd_hi at 16384)
+    const double *iwd_split;
     int fwd_out_rc;                    // lazy forward output must be re-centred (its bound squared would overflow the consumer's product)
     double fwd_out_bound;               // |forward lazy output| <= fwd_out_bound * p
 };
@@ -176,8 +176,8 @@ cudaError_t launch_behz_lift(const u64 *const *ct_ptrs, u64 *out, int n, int log
 cudaError_t launch_behz_tensor(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConst *bc, cudaStream_t s);
 // d (coefficient form) -> times t, fast_floor, fastbconv_sk -> out3[n][3][k][N]
 cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s);
-// lazy = 1: the buffers exchanged with the NTT kernels (lift output, tensor input/output, floor input, digit input, accumulator
-// output) hold lazy doubles (fparith.cuh) -- pair with NTT_IN_F / NTT_OUT_F on the transforms in between
+// lazy = 1: the buffers exchanged with the NTT kernels (lift output, tensor input/output, digit input, accumulator output) hold lazy
+// doubles (fparith.cuh) -- pair with NTT_IN_F / NTT_OUT_F on the transforms in between
 cudaError_t launch_behz_lift_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
 // lazy Bsk residues only, out [n][2][kb][N]: the source of the fused square's residues l >= k
 cudaError_t launch_behz_lift_bsk_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, cudaStream_t s);
@@ -187,7 +187,8 @@ cudaError_t launch_behz_lift_bsk_fp(const u64 *const *ct_ptrs, u64 *out, int n, 
 cudaError_t launch_behz_square_fused(const u64 *const *ct_ptrs, const u64 *lift_bsk, u64 *d, int n_ct, int k, int kt, int logn, const NttTab *tabs,
                                      cudaStream_t s);
 cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
-cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
+// canonical input; lazy input takes the folded kernel below
+cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s);
 // folded constants + software-pipelined loads (lazy input only)
 cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s);
 cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, u64 *acc, int n, int D, int k, int logn, const BehzConstF *f, int lazy,

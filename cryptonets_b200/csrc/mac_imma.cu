@@ -9,17 +9,17 @@
 // Same residues as k_mac_layer / k_mac_layer_fp (tests/test_gpu_kernels.py::test_mac_layer_*), 6 limb products instead of
 // K*M 64-bit modular multiply-adds per word: the layer becomes bound by reading its inputs once.
 //
-// CTA: 256 threads, a tile of TN (16 or 32) ciphertext words x up to 128 outputs; warp w owns outputs [16w, 16w+16).  Per 32-tap chunk
+// CTA: 256 threads, a tile of TN = 16 ciphertext words x up to 128 outputs (two CTAs per SM); warp w owns outputs [16w, 16w+16).  Per 32-tap chunk
 // the CTA loads 32 x TN words (each loader thread 4 taps of one word), cuts them into limbs and stores them tap-major per word
 // (32-byte rows with a half-row swizzle: conflict-free stores and ldmatrix); every warp then issues limbs x TN/8 MMAs against its A
 // fragment (weights pre-packed in fragment order on the host, L2 resident).
-#include <cstdlib>
 #include "fparith.cuh"
 #include "kernels.h"
 #include "plainops.cuh"
 
 namespace cnhe {
 
+constexpr int IM_TN = 16;     // ciphertext words per CTA
 constexpr int IM_ROW = 32;     // bytes per (word, limb) row of 32 taps; the two 16-byte halves are swapped on rows with bit 2 set, which
                                // makes both the loaders' 32-bit stores and the 8-row ldmatrix reads bank-conflict free
 
@@ -34,13 +34,13 @@ __device__ __forceinline__ void imma_s8u8(int (&c)[4], const uint4 &a, unsigned 
 }
 
 // wfrag: [m-tile][tap chunk][lane] uint4, the m16n8k32 A fragment of the (zero padded) signed 8-bit weight matrix
-template <int LIMBS, int TN>
-__global__ void __launch_bounds__(256, TN == 16 ? 2 : 1) k_mac_dense_imma(const u64 *const *__restrict__ in_ptrs, const uint4 *__restrict__ wfrag,
+template <int LIMBS>
+__global__ void __launch_bounds__(256, 2) k_mac_dense_imma(const u64 *const *__restrict__ in_ptrs, const uint4 *__restrict__ wfrag,
                                                       const uint4 *__restrict__ wfrag2, const u64 *__restrict__ bias,
                                                       int K, int M, u64 *const *__restrict__ out_ptrs, int k, int logn,
                                                       const BehzConst *__restrict__ bc, PlainConst pc) {
+    constexpr int TN = IM_TN, NT8 = TN / 8; // n8 tiles per warp
     __shared__ __align__(16) unsigned char sb[2][LIMBS][TN][IM_ROW];
-    constexpr int NT8 = TN / 8; // n8 tiles per warp
     const int N = 1 << logn;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const size_t col0 = (size_t)blockIdx.x * TN;            // first ciphertext word of the tile
@@ -143,31 +143,21 @@ __global__ void __launch_bounds__(256, TN == 16 ? 2 : 1) k_mac_dense_imma(const 
     }
 }
 
-template <int LIMBS, int TN>
+template <int LIMBS>
 static void imma_go(const u64 *const *in_ptrs, const uint4 *wf, const uint4 *wf2, const u64 *bias, int K, int M, u64 *const *out_ptrs, int k, int logn,
                     const BehzConst *bc, PlainConst pc, cudaStream_t s) {
     const size_t ct_words = (size_t)2 * k << logn;
-    dim3 grid((unsigned)(ct_words / TN), (unsigned)((M + 127) / 128));
-    k_mac_dense_imma<LIMBS, TN><<<grid, 256, 0, s>>>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc);
+    dim3 grid((unsigned)(ct_words / IM_TN), (unsigned)((M + 127) / 128));
+    k_mac_dense_imma<LIMBS><<<grid, 256, 0, s>>>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc);
 }
 cudaError_t launch_mac_dense_imma(const u64 *const *in_ptrs, const void *wfrag, const void *wfrag2, const u64 *bias, int K, int M, int limbs,
                                   u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {
     const uint4 *wf = reinterpret_cast<const uint4 *>(wfrag), *wf2 = reinterpret_cast<const uint4 *>(wfrag2);
-    static const int tn = getenv("CNHE_IMMA_TN") ? atoi(getenv("CNHE_IMMA_TN")) : 16; // ciphertext words per CTA (16: two CTAs per SM)
-    if (tn == 32) {
-        switch (limbs) {
-        case 5: imma_go<5, 32>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
-        case 6: imma_go<6, 32>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
-        case 7: imma_go<7, 32>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
-        default: return cudaErrorInvalidValue;
-        }
-    } else {
-        switch (limbs) {
-        case 5: imma_go<5, 16>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
-        case 6: imma_go<6, 16>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
-        case 7: imma_go<7, 16>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
-        default: return cudaErrorInvalidValue;
-        }
+    switch (limbs) {
+    case 5: imma_go<5>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
+    case 6: imma_go<6>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
+    case 7: imma_go<7>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
+    default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();
 }

@@ -12,9 +12,6 @@
 // written back is canonical, which is what makes the kernel bit-comparable with the CPU oracle.
 // Shared-memory layout: word i is stored at i ^ (((i>>4)&7)<<1) so that the unit-stride last pass (16 consecutive
 // words per thread, 16-byte accesses) and the strided passes (gap >= 16 words) are both bank-conflict free.
-#include <cstdlib>
-#include <cstring>
-
 #include <cuda.h> // CUtensorMap (the encoder is fetched through cudaGetDriverEntryPoint: no libcuda link dependency)
 
 #include "kernels.h"
@@ -556,7 +553,7 @@ __device__ __forceinline__ void fwd_last_fp(const double *sm, u64 *dst, const Nt
 
 #define CNHE_VTN(COUNT, stmt) _Pragma("unroll") for (int vt = tid; vt < (COUNT); vt += TR) { stmt; }
 __host__ __device__ constexpr int fp_threads(int logn) { return logn >= 13 ? (1 << logn) / 32 : (1 << logn) / 16; }
-__host__ __device__ constexpr int fp_min_blocks(int logn) { return logn >= 14 ? 1 : (logn == 13 ? 2 : 3); }
+__host__ __device__ constexpr int fp_min_blocks(int logn) { return logn == 13 ? 2 : 3; }
 
 // Ask L2 for the polynomial that the CTA taking this one's place will read (CTAs are dispatched in blockIdx order, so that
 // is about `resident` blocks ahead): its first-pass loads then hit L2 instead of waiting on HBM with the FP64 pipe idle.
@@ -573,8 +570,9 @@ template <int LOGN, bool IN_F, bool OUT_F>
 __device__ __forceinline__ void fwd_body_fp(double *sm, const FwdSrc &src, u64 *dst, const NttTab &tb, int tid) {
     constexpr int N = 1 << LOGN, TR = fp_threads(LOGN);
     double *twc = sm + N;
-    if constexpr (LOGN == 12 || LOGN == 14) { // loads first, then the twiddle cache fill (+2..3 % at N=4096/16384; -3 % at N=8192, which keeps the plain order)
-        constexpr int R1 = LOGN == 12 ? 4 : 5;
+    static_assert(LOGN <= 13, "N = 16384 runs on CTA pairs (k_ntt_forward_split)");
+    if constexpr (LOGN == 12) { // loads first, then the twiddle cache fill (+2..3 %; -3 % at N=8192, which keeps the plain order)
+        constexpr int R1 = 4;
         static_assert((N >> R1) == TR, "first pass: one virtual thread per thread");
         u64 raw[1 << R1];
         fwd_first_load<LOGN, R1, IN_F>(raw, src, tid);
@@ -582,13 +580,8 @@ __device__ __forceinline__ void fwd_body_fp(double *sm, const FwdSrc &src, u64 *
         __syncthreads();
         fwd_first_compute<LOGN, R1, IN_F>(sm, twc, raw, src, tb, tid);
         __syncthreads();
-        if constexpr (LOGN == 12) {
-            CNHE_VTN(N / 16, (fwd_pass_fp<12, 4, 4, false, 1, false>(sm, twc, src, tb, vt))); __syncthreads();
-            CNHE_VTN(N / 16, (fwd_last_fp<12, 2, OUT_F>(sm, dst, tb, vt)));
-        } else {
-            CNHE_VTN(N / 32, (fwd_pass_fp<14, 5, 5, false, 1, false>(sm, twc, src, tb, vt))); __syncthreads();
-            CNHE_VTN(N / 16, (fwd_last_fp<14, 2, OUT_F>(sm, dst, tb, vt)));
-        }
+        CNHE_VTN(N / 16, (fwd_pass_fp<12, 4, 4, false, 1, false>(sm, twc, src, tb, vt))); __syncthreads();
+        CNHE_VTN(N / 16, (fwd_last_fp<12, 2, OUT_F>(sm, dst, tb, vt)));
         return;
     }
     load_twiddle_cache(twc, tb.wd, tid, TR);
@@ -607,10 +600,8 @@ __device__ __forceinline__ void fwd_body_fp(double *sm, const FwdSrc &src, u64 *
         CNHE_VTN(N / 16, (fwd_last_fp<13, 2, OUT_F>(sm, dst, tb, vt)));
     }
 }
-// MINB: resident CTAs per SM the register allocation aims for (0 = fp_min_blocks).  N = 8192 with three (80 registers, 6 doubles spilled)
-// instead of two: a third CTA's memory phases fill the FP64 pipe's idle slots
-template <int LOGN, bool IN_F, bool OUT_F, int MINB = 0>
-__global__ void __launch_bounds__(fp_threads(LOGN), MINB ? MINB : fp_min_blocks(LOGN))
+template <int LOGN, bool IN_F, bool OUT_F>
+__global__ void __launch_bounds__(fp_threads(LOGN), fp_min_blocks(LOGN))
 k_ntt_forward_fp(const u64 *src, u64 *dst, const NttTab *__restrict__ tabs, int mod_base, int mod_count) {
     extern __shared__ __align__(16) u64 sm[];
     constexpr int N = 1 << LOGN;
@@ -623,8 +614,8 @@ k_ntt_forward_fp(const u64 *src, u64 *dst, const NttTab *__restrict__ tabs, int 
     fwd_body_fp<LOGN, IN_F, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (size_t)b * N, tb, tid);
 }
 // target: ciphertext c's polynomial with `k` residues starts at target + c * ct_stride (words)
-template <int LOGN, bool OUT_F, int MINB = 0>
-__global__ void __launch_bounds__(fp_threads(LOGN), MINB ? MINB : fp_min_blocks(LOGN))
+template <int LOGN, bool OUT_F>
+__global__ void __launch_bounds__(fp_threads(LOGN), fp_min_blocks(LOGN))
 k_ntt_forward_digits_fp(const u64 *target, size_t ct_stride, u64 *dst, const NttTab *__restrict__ tabs, int k, DigitMap dm) {
     extern __shared__ __align__(16) u64 sm[];
     constexpr int N = 1 << LOGN;
@@ -835,6 +826,7 @@ template <int LOGN, bool IN_F, bool OUT_F>
 __global__ void __launch_bounds__(fp_threads(LOGN), fp_min_blocks(LOGN))
 k_ntt_inverse_fp(const u64 *src, const u64 *base_add, int base_group, size_t base_stride, u64 *dst, const NttTab *__restrict__ tabs, int mod_base,
                  int mod_count) {
+    static_assert(LOGN <= 11, "N = 4096 / 8192 run on the persistent k_ntt_inverse_ws, N = 16384 on CTA pairs (k_ntt_inverse_split)");
     extern __shared__ __align__(16) u64 smraw[];
     constexpr int N = 1 << LOGN, TR = fp_threads(LOGN);
     const int b = blockIdx.x, tid = threadIdx.x;
@@ -855,25 +847,16 @@ k_ntt_inverse_fp(const u64 *src, const u64 *base_add, int base_group, size_t bas
     if constexpr (LOGN == 10) {
         CNHE_VTN(N / 16, (inv_pass_fp<10, 4, 4, false, false>(sm, twc, d, ba, tb, vt))); __syncthreads();
         CNHE_VTN(N / 16, (inv_pass_fp<10, 8, 2, true, OUT_F>(sm, twc, d, ba, tb, vt)));
-    } else if constexpr (LOGN == 11) {
+    } else {
         CNHE_VTN(N / 16, (inv_pass_fp<11, 4, 4, false, false>(sm, twc, d, ba, tb, vt))); __syncthreads();
         CNHE_VTN(N / 16, (inv_pass_fp<11, 8, 3, true, OUT_F>(sm, twc, d, ba, tb, vt)));
-    } else if constexpr (LOGN == 12) {
-        CNHE_VTN(N / 16, (inv_pass_fp<12, 4, 4, false, false>(sm, twc, d, ba, tb, vt))); __syncthreads();
-        CNHE_VTN(N / 16, (inv_pass_fp<12, 8, 4, true, OUT_F>(sm, twc, d, ba, tb, vt)));
-    } else if constexpr (LOGN == 13) {
-        CNHE_VTN(N / 16, (inv_pass_fp<13, 4, 4, false, false>(sm, twc, d, ba, tb, vt))); __syncthreads();
-        CNHE_VTN(N / 32, (inv_pass_fp<13, 8, 5, true, OUT_F>(sm, twc, d, ba, tb, vt)));
-    } else {
-        CNHE_VTN(N / 32, (inv_pass_fp<14, 4, 5, false, false>(sm, twc, d, ba, tb, vt))); __syncthreads();
-        CNHE_VTN(N / 32, (inv_pass_fp<14, 9, 5, true, OUT_F>(sm, twc, d, ba, tb, vt)));
     }
 }
 
 // ================================================================ N = 16384 on CTA pairs ("split")
 // A 16384-point polynomial is 128 KB of doubles: one CTA per SM, every warp of the SM at the same barrier, loads never overlapping
 // butterflies (0.36 of the HBM roofline against 0.50 at N = 8192).  After the first Cooley-Tukey stage the two halves of the polynomial
-// are independent 8192-point transforms with their own twiddle tables (NttTab::wd_hi holds them), so a cluster of two CTAs takes one
+// are independent 8192-point transforms with their own twiddle tables (NttTab::wd_split holds them), so a cluster of two CTAs takes one
 // polynomial: CTA h computes half h -- x[i] +- w x[i + N/2] on the way in from global memory (the pair reads the same lines at the same
 // time: one trip to HBM, the second read is an L2 hit), then the 5+4+4 passes of the 8192-point kernel in 64 KB of shared memory, 2-3 CTAs
 // per SM.  The inverse runs the 13 in-half stages first and the pair exchanges the halves through distributed shared memory for the last
@@ -926,7 +909,7 @@ __device__ __forceinline__ void fwd_split_body(double *sm, const FwdSrc &src, u6
     constexpr int TR = SPLIT_THREADS;
     double *twc = sm + SPLIT_H;
     const double w0 = __ldg(tb.wd + 1);
-    tb.wd = tb.wd_hi + half * SPLIT_H;
+    tb.wd = tb.wd_split + half * SPLIT_H;
     tb.fwd_recenter = tb.fwd_recenter_split;
     load_twiddle_cache(twc, tb.wd, tid, TR);
     __syncthreads();
@@ -1041,7 +1024,7 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
     constexpr int TR = SPLIT_THREADS, H = SPLIT_H;
     const int b = blockIdx.x >> 1, half = blockIdx.x & 1, tid = threadIdx.x;
     NttTab tb = tabs[mod_base + b % mod_count];
-    tb.iwd = tb.iwd_hi + half * H;
+    tb.iwd = tb.iwd_split + half * H;
     double *sm = reinterpret_cast<double *>(smraw);
     double *twc = sm + H;
     load_twiddle_cache(twc, tb.iwd, tid, TR);
@@ -1347,7 +1330,7 @@ k_behz_square_fused(const u64 *const *__restrict__ ct_ptrs, const u64 *__restric
     inv_split_last<HLOGN, TR, true, 3>(sm, twci, d + ((size_t)c * 3 * kt + l) * N + half * H, (size_t)kt * N, nullptr, tb, tid, half);
 }
 
-// ================================================================ persistent TMA-staged transforms, N = 4096 / 8192
+// ================================================================ persistent TMA-staged inverse transform, N = 4096 / 8192
 // One persistent CTA per SM.  Each CTA is pinned to ONE modulus (CTA c serves the polynomials whose table index is c mod #moduli), so
 // the twiddles it needs never change: the 15N/16 twiddles of the four unit-stride stages -- the ones that used to be fetched from L2 by
 // every polynomial (as many bytes as the polynomial itself, and the top stall of the one-CTA-per-polynomial kernel) -- are staged into
@@ -1358,8 +1341,10 @@ k_behz_square_fused(const u64 *const *__restrict__ ct_ptrs, const u64 *__restric
 // barriers of the group, results written straight from registers, then one elected thread refills the slot with the group's next
 // polynomial.  No compute warp ever waits on HBM or L2 for data or twiddles, there is no CTA launch/exit (store drain) per polynomial,
 // and the groups run out of phase so that one group's shared-memory round trips and slot refill hide under the other's FP64 work.
+// The forward transform stays one CTA per polynomial (k_ntt_forward_fp): staged the same way it gained nothing, and its digit-cutting
+// form was slower (DESIGN.md §4.2).
 constexpr int WS_GROUPS = 2, WS_GROUP_THREADS = 256, WS_THREADS = WS_GROUPS * WS_GROUP_THREADS;
-enum WsMode { WS_CANON = 0, WS_LAZY = 1, WS_DIGIT = 2 }; // how the first pass reads the staged words
+constexpr unsigned WS_STAGGER_NS = 5000; // group 1 starts this much later than group 0 (the groups should not walk through the passes in lockstep)
 
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long *bar, unsigned count) {
@@ -1399,138 +1384,25 @@ __device__ __forceinline__ void ws_delay(unsigned ns) {
 }
 __device__ __forceinline__ void group_sync(int g) { asm volatile("bar.sync %0, %1;" ::"r"(g + 1), "n"(WS_GROUP_THREADS) : "memory"); }
 
-struct WsJob {
-    long long row;  // first 128-byte row of the source polynomial in the tensor map
-    size_t dst_off; // destination offset in words
-    int shift;      // digit mode
-};
+// a __grid_constant__ kernel parameter: read from the parameter bank where used (passed as a plain value, the small record is copied
+// into registers and the kernel, already at 128 registers, spills more)
 struct WsArgs {
-    int n_polys, mod_base, mod_count; // plain: polynomial b uses table mod_base + b % mod_count, source row b * N/16, destination b * N
-    int D;                            // digit mode: b -> (c, d, l) as in k_ntt_forward_digits_fp, mod_count = k, mod_base = 0
-    long long ct_stride_rows;
-    unsigned char src[64], shift[64];
-    u64 mask;
-    // inverse: optional base added to the canonical result
+    int n_polys, mod_base, mod_count; // polynomial b uses table mod_base + b % mod_count, source row b * N/16, destination b * N
+    // optional base added to the canonical result
     const u64 *base_add;
     int base_group;
     size_t base_stride;
-    unsigned stagger_ns; // group 1 starts this much later than group 0 (the groups should not walk through the passes in lockstep)
 };
-template <int LOGN, int MODE>
-__device__ __forceinline__ WsJob ws_job(const WsArgs &a, int b) {
-    constexpr int N = 1 << LOGN;
-    WsJob j;
-    if constexpr (MODE == WS_DIGIT) {
-        const int l = b % a.mod_count, d = (b / a.mod_count) % a.D, c = b / (a.mod_count * a.D);
-        j.row = (long long)c * a.ct_stride_rows + (long long)a.src[d] * (N / 16);
-        j.dst_off = (((size_t)c * a.mod_count + l) * a.D + d) * N;
-        j.shift = a.shift[d];
-    } else {
-        j.row = (long long)b * (N / 16);
-        j.dst_off = (size_t)b * N;
-        j.shift = 0;
-    }
-    return j;
-}
 // stage polynomial `b` into a slot; called by one thread
-template <int LOGN, int MODE>
-__device__ __forceinline__ void ws_issue(const CUtensorMap *tmap, const WsArgs &a, double *slot, unsigned long long *full, int b) {
+template <int LOGN>
+__device__ __forceinline__ void ws_issue(const CUtensorMap *tmap, double *slot, unsigned long long *full, int b) {
     constexpr int N = 1 << LOGN;
     constexpr int BOX_ROWS = 256, BOXES = (N / 16) / BOX_ROWS;
-    const WsJob j = ws_job<LOGN, MODE>(a, b);
+    const long long row = (long long)b * (N / 16); // first 128-byte row of the polynomial in the tensor map
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // the slot's previous contents were read through the generic proxy
     mbar_expect_tx(full, (unsigned)(N * 8));
 #pragma unroll
-    for (int x = 0; x < BOXES; x++) tma_load_rows(slot + x * BOX_ROWS * 16, tmap, (int)(j.row + x * BOX_ROWS), full);
-}
-// first forward pass on the staged words: R stages on 2^R coefficients at stride N >> R, in place
-template <int LOGN, int R, int MODE>
-__device__ __forceinline__ void fwd_first_staged(double *sm, const double *twc, int shift, u64 mask, bool need_reduce, const NttTab &tb, int vt) {
-    constexpr int E = 1 << R, LG = LOGN - R;
-    const double p = tb.pd, pinv = tb.pinv;
-    double x[E];
-#pragma unroll
-    for (int e = 0; e < E; e++) {
-        const double raw = sm[swz(vt + (e << LG))];
-        if constexpr (MODE == WS_LAZY) x[e] = raw;
-        else {
-            u64 v = (u64)__double_as_longlong(raw);
-            if constexpr (MODE == WS_DIGIT) v = (v >> shift) & mask;
-            x[e] = u2d(v);
-            if (MODE == WS_DIGIT && need_reduce) x[e] = frecenter(x[e], p, pinv);
-        }
-    }
-#pragma unroll
-    for (int u = 0; u < R; u++) {
-        const int h = E >> (u + 1);
-#pragma unroll
-        for (int e = 0; e < E; e++) {
-            if (e & h) continue;
-            const double w = twc[(1 << u) + (e >> (R - u))];
-            const double t = fmodmul(x[e + h], w, p, pinv);
-            const double a = x[e];
-            x[e] = __dadd_rn(a, t);
-            x[e + h] = __dsub_rn(a, t);
-        }
-    }
-#pragma unroll
-    for (int e = 0; e < E; e++) sm[swz(vt + (e << LG))] = x[e];
-}
-// last forward pass with the unit-stride twiddles resident in shared memory (hi[m * T + j], m = 0..14): NV 16-coefficient groups per
-// thread (j0, j0 + jstride, ..); all of them are read before `after_load` runs, so the slot can be refilled under the arithmetic
-template <int LOGN, int PASS, bool OUT_F, int NV, class Hook>
-__device__ __forceinline__ void fwd_last_staged(const double *sm, u64 *dst, const NttTab &tb, const double *hi, int j0, int jstride, Hook after_load) {
-    constexpr int T = (1 << LOGN) / 16;
-    const double p = tb.pd, pinv = tb.pinv;
-    const bool rc = (tb.fwd_recenter >> PASS) & 1;
-    const double2 *smv = reinterpret_cast<const double2 *>(sm);
-    double xs[NV][16];
-#pragma unroll
-    for (int i = 0; i < NV; i++) {
-        const int j = j0 + i * jstride, xr = j & 7;
-#pragma unroll
-        for (int ch = 0; ch < 8; ch++) {
-            double2 v = smv[j * 8 + (ch ^ xr)];
-            xs[i][2 * ch] = v.x;
-            xs[i][2 * ch + 1] = v.y;
-        }
-    }
-    after_load();
-#pragma unroll
-    for (int i = 0; i < NV; i++) {
-    const int j = j0 + i * jstride;
-    double (&x)[16] = xs[i];
-    if (rc) {
-#pragma unroll
-        for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
-    }
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-        const int h = 8 >> u;
-#pragma unroll
-        for (int e = 0; e < 16; e++) {
-            if (e & h) continue;
-            const double w = hi[((1 << u) - 1 + (e >> (4 - u))) * T + j];
-            const double t = fmodmul(x[e + h], w, p, pinv);
-            const double a = x[e];
-            x[e] = __dadd_rn(a, t);
-            x[e + h] = __dsub_rn(a, t);
-        }
-    }
-    u64 *o = dst + 16 * j;
-    if constexpr (OUT_F) {
-        if (tb.fwd_out_rc) {
-#pragma unroll
-            for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
-        }
-#pragma unroll
-        for (int g = 0; g < 4; g++) stg256(o + 4 * g, lazy_bits(x[4 * g]), lazy_bits(x[4 * g + 1]), lazy_bits(x[4 * g + 2]), lazy_bits(x[4 * g + 3]));
-    } else {
-#pragma unroll
-        for (int g = 0; g < 4; g++)
-            stg256(o + 4 * g, fcanon_u(x[4 * g], p, pinv), fcanon_u(x[4 * g + 1], p, pinv), fcanon_u(x[4 * g + 2], p, pinv), fcanon_u(x[4 * g + 3], p, pinv));
-    }
-    }
+    for (int x = 0; x < BOXES; x++) tma_load_rows(slot + x * BOX_ROWS * 16, tmap, (int)(row + x * BOX_ROWS), full);
 }
 // first inverse pass on the staged words: stages 0..3 on 16 consecutive coefficients, in place; twiddles from the resident table
 template <int LOGN, bool IN_F>
@@ -1611,71 +1483,9 @@ __device__ __forceinline__ WsWalk ws_walk(int mc) {
     return w;
 }
 
-template <int LOGN, int MODE, bool OUT_F>
-__global__ void __launch_bounds__(WS_THREADS, 1)
-k_ntt_forward_ws(const __grid_constant__ CUtensorMap tmap, u64 *dst, const NttTab *__restrict__ tabs, const WsArgs a) {
-    static_assert(LOGN == 12 || LOGN == 13, "the staged transform covers N = 4096 and 8192");
-    constexpr int N = 1 << LOGN;
-    extern __shared__ unsigned char ws_raw[];
-    const int tid = threadIdx.x;
-    {
-        const WsSmem sm_ = ws_carve<LOGN>(ws_raw);
-        const WsWalk walk = ws_walk(a.mod_count);
-        if (tid == 0) {
-            const NttTab &tb0 = tabs[a.mod_base + walk.m];
-            *sm_.tab = tb0;
-            for (int g = 0; g < WS_GROUPS; g++) { mbar_init(&sm_.full[g], 1); mbar_init(&sm_.empty[g], WS_GROUP_THREADS); }
-            mbar_init(sm_.tbar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            mbar_expect_tx(sm_.tbar, (unsigned)((ws_hi_words<LOGN>() + TWC) * 8));
-            bulk_load(sm_.hi, tb0.wd_hi, ws_hi_words<LOGN>() * 8, sm_.tbar);
-            bulk_load(sm_.lo, tb0.wd, TWC * 8, sm_.tbar);
-            for (int g = 0; g < WS_GROUPS; g++)
-                if (walk.poly(g) < a.n_polys) ws_issue<LOGN, MODE>(&tmap, a, sm_.slots + (size_t)g * N, &sm_.full[g], walk.poly(g));
-        }
-        __syncthreads();
-        mbar_wait(sm_.tbar, 0);
-    }
-    const int g = tid / WS_GROUP_THREADS, gt = tid % WS_GROUP_THREADS;
-    if (g == 1 && a.stagger_ns) ws_delay(a.stagger_ns);
-    FwdSrc unused;
-    unused.src = nullptr; unused.digit = false; unused.need_reduce = false; unused.shift = 0; unused.mask = 0;
-#pragma unroll 1
-    for (int t = 0;; t++) {
-        // everything below is re-derived per polynomial on purpose: nothing but t stays live across the register-hungry radix-32 pass
-        const WsWalk walk = ws_walk(a.mod_count);
-        const int b = walk.poly(g + WS_GROUPS * t);
-        if (b >= a.n_polys) break;
-        const WsSmem sm_ = ws_carve<LOGN>(ws_raw);
-        const NttTab &tb = *sm_.tab;
-        double *sm = sm_.slots + (size_t)g * N;
-        const double *twc = sm_.lo, *hi = sm_.hi;
-        const bool need_reduce = MODE == WS_DIGIT && a.mask >= tb.mod.p;
-        const WsJob job = ws_job<LOGN, MODE>(a, b);
-        // once the last pass holds its inputs in registers the slot is dead: refill it with the group's next polynomial under the arithmetic
-        auto refill = [&]() { // every thread reports its reads done; only the elected thread waits for all of them before issuing the copy
-            mbar_arrive(&sm_.empty[g]);
-            const int nb = walk.poly(g + WS_GROUPS * (t + 1));
-            if (gt == 0 && nb < a.n_polys) {
-                mbar_wait(&sm_.empty[g], t & 1);
-                ws_issue<LOGN, MODE>(&tmap, a, sm, &sm_.full[g], nb);
-            }
-        };
-        mbar_wait(&sm_.full[g], t & 1);
-        if constexpr (LOGN == 13) {
-            CNHE_WS_VT(N / 32, (fwd_first_staged<13, 5, MODE>(sm, twc, job.shift, a.mask, need_reduce, tb, vt))); group_sync(g);
-            CNHE_WS_VT(N / 16, (fwd_pass_fp<13, 5, 4, false, 1, false>(sm, twc, unused, tb, vt))); group_sync(g);
-            fwd_last_staged<13, 2, OUT_F, 2>(sm, dst + job.dst_off, tb, hi, gt, WS_GROUP_THREADS, refill);
-        } else {
-            CNHE_WS_VT(N / 16, (fwd_first_staged<12, 4, MODE>(sm, twc, job.shift, a.mask, need_reduce, tb, vt))); group_sync(g);
-            CNHE_WS_VT(N / 16, (fwd_pass_fp<12, 4, 4, false, 1, false>(sm, twc, unused, tb, vt))); group_sync(g);
-            fwd_last_staged<12, 2, OUT_F, 1>(sm, dst + job.dst_off, tb, hi, gt, WS_GROUP_THREADS, refill);
-        }
-    }
-}
 template <int LOGN, bool IN_F, bool OUT_F>
 __global__ void __launch_bounds__(WS_THREADS, 1)
-k_ntt_inverse_ws(const __grid_constant__ CUtensorMap tmap, u64 *dst, const NttTab *__restrict__ tabs, const WsArgs a) {
+k_ntt_inverse_ws(const __grid_constant__ CUtensorMap tmap, u64 *dst, const NttTab *__restrict__ tabs, const __grid_constant__ WsArgs a) {
     static_assert(LOGN == 12 || LOGN == 13, "the staged transform covers N = 4096 and 8192");
     constexpr int N = 1 << LOGN;
     extern __shared__ unsigned char ws_raw[];
@@ -1693,13 +1503,13 @@ k_ntt_inverse_ws(const __grid_constant__ CUtensorMap tmap, u64 *dst, const NttTa
             bulk_load(sm_.hi, tb0.iwd_hi, ws_hi_words<LOGN>() * 8, sm_.tbar);
             bulk_load(sm_.lo, tb0.iwd, TWC * 8, sm_.tbar);
             for (int g = 0; g < WS_GROUPS; g++)
-                if (walk.poly(g) < a.n_polys) ws_issue<LOGN, WS_CANON>(&tmap, a, sm_.slots + (size_t)g * N, &sm_.full[g], walk.poly(g));
+                if (walk.poly(g) < a.n_polys) ws_issue<LOGN>(&tmap, sm_.slots + (size_t)g * N, &sm_.full[g], walk.poly(g));
         }
         __syncthreads();
         mbar_wait(sm_.tbar, 0);
     }
     const int g = tid / WS_GROUP_THREADS, gt = tid % WS_GROUP_THREADS;
-    if (g == 1 && a.stagger_ns) ws_delay(a.stagger_ns);
+    if (g == 1) ws_delay(WS_STAGGER_NS);
 #pragma unroll 1
     for (int t = 0;; t++) {
         const WsWalk walk = ws_walk(a.mod_count);
@@ -1720,7 +1530,7 @@ k_ntt_inverse_ws(const __grid_constant__ CUtensorMap tmap, u64 *dst, const NttTa
             const int nb = walk.poly(g + WS_GROUPS * (t + 1));
             if (gt == 0 && nb < a.n_polys) {
                 mbar_wait(&sm_.empty[g], t & 1);
-                ws_issue<LOGN, WS_CANON>(&tmap, a, sm, &sm_.full[g], nb);
+                ws_issue<LOGN>(&tmap, sm, &sm_.full[g], nb);
             }
         };
         mbar_wait(&sm_.full[g], t & 1);
@@ -1755,7 +1565,7 @@ static cudaError_t prep(K kern, int logn) {
     return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, ntt_kernel_smem_bytes(logn));
 }
 
-// ---- host side of the staged transforms: tensor map over the source array, persistent grid of one CTA per SM
+// ---- tensor maps (the persistent inverse transform, mac_umma.cu): the encoder is a driver entry point
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
                                   const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static EncodeTiledFn encode_tiled() {
@@ -1766,28 +1576,6 @@ static EncodeTiledFn encode_tiled() {
         return (EncodeTiledFn)p;
     }();
     return fn;
-}
-// CNHE_NTT_WS=0 switches the persistent kernels off altogether; CNHE_NTT_WS_FWD / CNHE_NTT_WS_INV override one direction
-static bool ws_flag(const char *name, bool dflt) {
-    const char *all = getenv("CNHE_NTT_WS"), *one = getenv(name);
-    if (encode_tiled() == nullptr) return false;
-    if (one) return atoi(one) != 0;
-    if (all) return atoi(all) != 0;
-    return dflt;
-}
-// Defaults: the persistent inverse transform, and the per-polynomial forward transform unless CNHE_NTT_WS_FWD=1 asks for the staged one
-// (the staged forward transform gains nothing over the per-polynomial one, and its digit-cutting form is slower).
-static bool ws_enabled_fwd() { return ws_flag("CNHE_NTT_WS_FWD", false); } // read per launch: tests flip it inside one process
-static bool ws_enabled_inv() { return ws_flag("CNHE_NTT_WS_INV", true); }
-// N = 8192 forward transforms with three CTAs per SM (CNHE_NTT_FWD_BLOCKS=3) or two (=2); read per launch
-static bool fwd_three_blocks() {
-    const char *v = getenv("CNHE_NTT_FWD_BLOCKS");
-    return v ? atoi(v) == 3 : false;
-}
-// N = 16384: CTA pairs unless CNHE_NTT_SPLIT=0 (read per launch, like the flags above)
-static bool split_enabled() {
-    const char *v = getenv("CNHE_NTT_SPLIT");
-    return v ? atoi(v) != 0 : true;
 }
 constexpr int SPLIT_SMEM = SPLIT_H * 8 + TWC * 8;
 template <class K>
@@ -1805,6 +1593,7 @@ static int sm_count() {
 }
 // rows of 16 words (128 bytes) starting at `base`; boxes of 256 rows, hardware swizzle = swz()
 static cudaError_t make_row_map(CUtensorMap *m, const u64 *base, size_t words) {
+    if (encode_tiled() == nullptr) return cudaErrorNotSupported; // every CUDA 12 driver (the least an sm_90a binary loads on) exports it
     const cuuint64_t dims[2] = {16, (cuuint64_t)(words / 16)};
     const cuuint64_t strides[1] = {128};
     const cuuint32_t box[2] = {16, 256}, estr[2] = {1, 1};
@@ -1828,22 +1617,6 @@ cudaError_t make_word_map_2d(void *map, const u64 *base, size_t inner_words, siz
                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
-static unsigned ws_stagger_ns() {
-    static const unsigned v = getenv("CNHE_WS_STAGGER") ? (unsigned)atoi(getenv("CNHE_WS_STAGGER")) : 5000u;
-    return v;
-}
-template <class K>
-static cudaError_t ws_launch(K kern, int smem, const CUtensorMap &map, u64 *dst, const NttTab *tabs, const WsArgs &a0, cudaStream_t s) {
-    WsArgs a = a0;
-    a.stagger_ns = ws_stagger_ns();
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    int grid = sm_count();
-    if (a.mod_count <= grid) grid -= grid % a.mod_count; // equally many CTAs per modulus: every CTA is pinned to one
-    if (a.n_polys < grid) grid = a.n_polys;
-    kern<<<grid, WS_THREADS, smem, s>>>(map, dst, tabs, a);
-    return cudaGetLastError();
-}
 
 #define CNHE_DISPATCH_LOGN(logn, ...)                                                                                 \
     switch (logn) {                                                                                                     \
@@ -1855,6 +1628,63 @@ static cudaError_t ws_launch(K kern, int smem, const CUtensorMap &map, u64 *dst,
     default: return cudaErrorInvalidValue;                                                                              \
     }
 
+// FP64 transforms by ring degree.  Forward: one CTA per polynomial up to N = 8192, CTA pairs at N = 16384.  Inverse: one CTA per
+// polynomial at N = 1024 / 2048, the persistent kernel at N = 4096 / 8192, CTA pairs at N = 16384.
+template <int L, bool LAZY>
+static cudaError_t launch_fwd_fp(const u64 *src, u64 *dst, int n_polys, const NttTab *tabs, int mod_base, int mod_count, cudaStream_t s) {
+    if constexpr (L == 14) {
+        cudaError_t e = split_prep(k_ntt_forward_split<LAZY, LAZY>);
+        if (e != cudaSuccess) return e;
+        k_ntt_forward_split<LAZY, LAZY><<<2 * n_polys, SPLIT_THREADS, SPLIT_SMEM, s>>>(src, dst, tabs, mod_base, mod_count);
+    } else {
+        cudaError_t e = prep(k_ntt_forward_fp<L, LAZY, LAZY>, L);
+        if (e != cudaSuccess) return e;
+        k_ntt_forward_fp<L, LAZY, LAZY><<<n_polys, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(src, dst, tabs, mod_base, mod_count);
+    }
+    return cudaGetLastError();
+}
+template <int L, bool OUT_F>
+static cudaError_t launch_fwd_digits_fp(const u64 *target, size_t ct_stride, u64 *dst, int n_polys, int k, const DigitMap &dm, const NttTab *tabs,
+                                        cudaStream_t s) {
+    if constexpr (L == 14) {
+        cudaError_t e = split_prep(k_ntt_forward_digits_split<OUT_F>);
+        if (e != cudaSuccess) return e;
+        k_ntt_forward_digits_split<OUT_F><<<2 * n_polys, SPLIT_THREADS, SPLIT_SMEM, s>>>(target, ct_stride, dst, tabs, k, dm);
+    } else {
+        cudaError_t e = prep(k_ntt_forward_digits_fp<L, OUT_F>, L);
+        if (e != cudaSuccess) return e;
+        k_ntt_forward_digits_fp<L, OUT_F><<<n_polys, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(target, ct_stride, dst, tabs, k, dm);
+    }
+    return cudaGetLastError();
+}
+template <int L, bool IN_F, bool OUT_F>
+static cudaError_t launch_inv_fp(const u64 *src, const u64 *base, int base_group, size_t base_stride, u64 *dst, int n_polys, const NttTab *tabs,
+                                 int mod_base, int mod_count, cudaStream_t s) {
+    if constexpr (L == 14) {
+        cudaError_t e = split_prep(k_ntt_inverse_split<IN_F, OUT_F>);
+        if (e != cudaSuccess) return e;
+        k_ntt_inverse_split<IN_F, OUT_F><<<2 * n_polys, SPLIT_THREADS, SPLIT_SMEM, s>>>(src, base, base_group, base_stride, dst, tabs, mod_base, mod_count);
+    } else if constexpr (L >= 12) { // tensor map over the source array, persistent grid of one CTA per SM
+        CUtensorMap map;
+        cudaError_t e = make_row_map(&map, src, (size_t)n_polys << L);
+        if (e != cudaSuccess) return e;
+        const WsArgs a = {n_polys, mod_base, mod_count, base, base_group, base_stride};
+        constexpr int smem = ws_smem_bytes<L>();
+        e = cudaFuncSetAttribute(k_ntt_inverse_ws<L, IN_F, OUT_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e != cudaSuccess) return e;
+        int grid = sm_count();
+        if (mod_count <= grid) grid -= grid % mod_count; // equally many CTAs per modulus: every CTA is pinned to one
+        if (n_polys < grid) grid = n_polys;
+        k_ntt_inverse_ws<L, IN_F, OUT_F><<<grid, WS_THREADS, smem, s>>>(map, dst, tabs, a);
+    } else {
+        cudaError_t e = prep(k_ntt_inverse_fp<L, IN_F, OUT_F>, L);
+        if (e != cudaSuccess) return e;
+        k_ntt_inverse_fp<L, IN_F, OUT_F><<<n_polys, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(src, base, base_group, base_stride, dst, tabs, mod_base,
+                                                                                                mod_count);
+    }
+    return cudaGetLastError();
+}
+
 // `fp`: 0 = integer Harvey butterflies; NTT_FP = FP64 butterflies, optionally | NTT_IN_F (source holds lazy doubles) | NTT_OUT_F
 // (destination receives lazy doubles instead of canonical words)
 cudaError_t launch_ntt_forward(const u64 *src, u64 *dst, int n_polys, int logn, const NttTab *tabs, int mod_base, int mod_count, int fp,
@@ -1863,54 +1693,8 @@ cudaError_t launch_ntt_forward(const u64 *src, u64 *dst, int n_polys, int logn, 
     if (fp & NTT_FP) {
         const bool lazy = (fp & (NTT_IN_F | NTT_OUT_F)) == (NTT_IN_F | NTT_OUT_F);
         if (!lazy && (fp & (NTT_IN_F | NTT_OUT_F))) return cudaErrorInvalidValue; // only canonical->canonical and lazy->lazy are built
-        if ((logn == 12 || logn == 13) && ws_enabled_fwd()) {
-            CUtensorMap map;
-            cudaError_t e = make_row_map(&map, src, (size_t)n_polys << logn);
-            if (e != cudaSuccess) return e;
-            WsArgs a;
-            memset(&a, 0, sizeof(a));
-            a.n_polys = n_polys; a.mod_base = mod_base; a.mod_count = mod_count;
-            if (logn == 13) return lazy ? ws_launch(k_ntt_forward_ws<13, WS_LAZY, true>, ws_smem_bytes<13>(), map, dst, tabs, a, s)
-                                        : ws_launch(k_ntt_forward_ws<13, WS_CANON, false>, ws_smem_bytes<13>(), map, dst, tabs, a, s);
-            return lazy ? ws_launch(k_ntt_forward_ws<12, WS_LAZY, true>, ws_smem_bytes<12>(), map, dst, tabs, a, s)
-                        : ws_launch(k_ntt_forward_ws<12, WS_CANON, false>, ws_smem_bytes<12>(), map, dst, tabs, a, s);
-        }
-        if (logn == 14 && split_enabled()) {
-            if (lazy) {
-                cudaError_t e = split_prep(k_ntt_forward_split<true, true>);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_split<true, true><<<2 * n_polys, SPLIT_THREADS, SPLIT_SMEM, s>>>(src, dst, tabs, mod_base, mod_count);
-            } else {
-                cudaError_t e = split_prep(k_ntt_forward_split<false, false>);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_split<false, false><<<2 * n_polys, SPLIT_THREADS, SPLIT_SMEM, s>>>(src, dst, tabs, mod_base, mod_count);
-            }
-            return cudaGetLastError();
-        }
-        if (logn == 13 && fwd_three_blocks()) {
-            if (lazy) {
-                cudaError_t e = prep(k_ntt_forward_fp<13, true, true, 3>, 13);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_fp<13, true, true, 3><<<n_polys, fp_threads(13), ntt_kernel_smem_bytes(13), s>>>(src, dst, tabs, mod_base, mod_count);
-            } else {
-                cudaError_t e = prep(k_ntt_forward_fp<13, false, false, 3>, 13);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_fp<13, false, false, 3><<<n_polys, fp_threads(13), ntt_kernel_smem_bytes(13), s>>>(src, dst, tabs, mod_base, mod_count);
-            }
-            return cudaGetLastError();
-        }
-        CNHE_DISPATCH_LOGN(logn, {
-            if (lazy) {
-                cudaError_t e = prep(k_ntt_forward_fp<L, true, true>, L);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_fp<L, true, true><<<n_polys, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(src, dst, tabs, mod_base, mod_count);
-            } else {
-                cudaError_t e = prep(k_ntt_forward_fp<L, false, false>, L);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_fp<L, false, false><<<n_polys, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(src, dst, tabs, mod_base, mod_count);
-            }
-        });
-        return cudaGetLastError();
+        CNHE_DISPATCH_LOGN(logn, return lazy ? launch_fwd_fp<L, true>(src, dst, n_polys, tabs, mod_base, mod_count, s)
+                                             : launch_fwd_fp<L, false>(src, dst, n_polys, tabs, mod_base, mod_count, s));
     }
     CNHE_DISPATCH_LOGN(logn, {
         cudaError_t e = prep(k_ntt_forward<L>, L);
@@ -1924,56 +1708,9 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
     if (n_ct <= 0) return cudaSuccess;
     if (fp & NTT_FP) {
         if (fp & NTT_IN_F) return cudaErrorInvalidValue; // digits are cut from canonical words
-        if ((logn == 12 || logn == 13) && ws_enabled_fwd() && ct_stride % 16 == 0) {
-            CUtensorMap map;
-            cudaError_t e = make_row_map(&map, target, (size_t)(n_ct - 1) * ct_stride + ((size_t)k << logn));
-            if (e != cudaSuccess) return e;
-            WsArgs a;
-            memset(&a, 0, sizeof(a));
-            a.n_polys = n_ct * dm.D * k; a.mod_base = 0; a.mod_count = k; a.D = dm.D; a.ct_stride_rows = (long long)(ct_stride / 16); a.mask = dm.mask;
-            memcpy(a.src, dm.src, 64); memcpy(a.shift, dm.shift, 64);
-            const bool of = fp & NTT_OUT_F;
-            if (logn == 13) return of ? ws_launch(k_ntt_forward_ws<13, WS_DIGIT, true>, ws_smem_bytes<13>(), map, dst, tabs, a, s)
-                                      : ws_launch(k_ntt_forward_ws<13, WS_DIGIT, false>, ws_smem_bytes<13>(), map, dst, tabs, a, s);
-            return of ? ws_launch(k_ntt_forward_ws<12, WS_DIGIT, true>, ws_smem_bytes<12>(), map, dst, tabs, a, s)
-                      : ws_launch(k_ntt_forward_ws<12, WS_DIGIT, false>, ws_smem_bytes<12>(), map, dst, tabs, a, s);
-        }
-        if (logn == 14 && split_enabled()) {
-            if (fp & NTT_OUT_F) {
-                cudaError_t e = split_prep(k_ntt_forward_digits_split<true>);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_digits_split<true><<<2 * n_ct * dm.D * k, SPLIT_THREADS, SPLIT_SMEM, s>>>(target, ct_stride, dst, tabs, k, dm);
-            } else {
-                cudaError_t e = split_prep(k_ntt_forward_digits_split<false>);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_digits_split<false><<<2 * n_ct * dm.D * k, SPLIT_THREADS, SPLIT_SMEM, s>>>(target, ct_stride, dst, tabs, k, dm);
-            }
-            return cudaGetLastError();
-        }
-        if (logn == 13 && fwd_three_blocks()) {
-            if (fp & NTT_OUT_F) {
-                cudaError_t e = prep(k_ntt_forward_digits_fp<13, true, 3>, 13);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_digits_fp<13, true, 3><<<n_ct * dm.D * k, fp_threads(13), ntt_kernel_smem_bytes(13), s>>>(target, ct_stride, dst, tabs, k, dm);
-            } else {
-                cudaError_t e = prep(k_ntt_forward_digits_fp<13, false, 3>, 13);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_digits_fp<13, false, 3><<<n_ct * dm.D * k, fp_threads(13), ntt_kernel_smem_bytes(13), s>>>(target, ct_stride, dst, tabs, k, dm);
-            }
-            return cudaGetLastError();
-        }
-        CNHE_DISPATCH_LOGN(logn, {
-            if (fp & NTT_OUT_F) {
-                cudaError_t e = prep(k_ntt_forward_digits_fp<L, true>, L);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_digits_fp<L, true><<<n_ct * dm.D * k, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(target, ct_stride, dst, tabs, k, dm);
-            } else {
-                cudaError_t e = prep(k_ntt_forward_digits_fp<L, false>, L);
-                if (e != cudaSuccess) return e;
-                k_ntt_forward_digits_fp<L, false><<<n_ct * dm.D * k, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(target, ct_stride, dst, tabs, k, dm);
-            }
-        });
-        return cudaGetLastError();
+        const int n_polys = n_ct * dm.D * k;
+        CNHE_DISPATCH_LOGN(logn, return (fp & NTT_OUT_F) ? launch_fwd_digits_fp<L, true>(target, ct_stride, dst, n_polys, k, dm, tabs, s)
+                                                         : launch_fwd_digits_fp<L, false>(target, ct_stride, dst, n_polys, k, dm, tabs, s));
     }
     CNHE_DISPATCH_LOGN(logn, {
         cudaError_t e = prep(k_ntt_forward_digits<L>, L);
@@ -2029,23 +1766,6 @@ cudaError_t launch_pack_keys48(const u64 *key, uint4 *out, int n_polys, int logn
     if (logn == 12) return launch_pk48<11>(key, out, n_polys, s);
     return cudaErrorInvalidValue;
 }
-template <int L, bool IN_F, bool OUT_F>
-static cudaError_t launch_inv_fp(const u64 *src, const u64 *base, int base_group, size_t base_stride, u64 *dst, int n_polys, const NttTab *tabs,
-                                 int mod_base, int mod_count, cudaStream_t s) {
-    cudaError_t e = prep(k_ntt_inverse_fp<L, IN_F, OUT_F>, L);
-    if (e != cudaSuccess) return e;
-    k_ntt_inverse_fp<L, IN_F, OUT_F><<<n_polys, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(src, base, base_group, base_stride, dst, tabs, mod_base,
-                                                                                            mod_count);
-    return cudaSuccess;
-}
-template <bool IN_F, bool OUT_F>
-static cudaError_t launch_inv_split(const u64 *src, const u64 *base, int base_group, size_t base_stride, u64 *dst, int n_polys, const NttTab *tabs,
-                                    int mod_base, int mod_count, cudaStream_t s) {
-    cudaError_t e = split_prep(k_ntt_inverse_split<IN_F, OUT_F>);
-    if (e != cudaSuccess) return e;
-    k_ntt_inverse_split<IN_F, OUT_F><<<2 * n_polys, SPLIT_THREADS, SPLIT_SMEM, s>>>(src, base, base_group, base_stride, dst, tabs, mod_base, mod_count);
-    return cudaGetLastError();
-}
 static cudaError_t launch_inv(const u64 *src, const u64 *base, int base_group, size_t base_stride, u64 *dst, int n_polys, int logn,
                               const NttTab *tabs, int mod_base, int mod_count, int fp, cudaStream_t s) {
     if (n_polys <= 0) return cudaSuccess;
@@ -2053,33 +1773,9 @@ static cudaError_t launch_inv(const u64 *src, const u64 *base, int base_group, s
     if (fp & NTT_FP) {
         const bool in_f = fp & NTT_IN_F, out_f = fp & NTT_OUT_F;
         if (out_f && (!in_f || base)) return cudaErrorInvalidValue; // built: canonical->canonical, lazy->lazy, lazy->canonical(+base)
-        if ((logn == 12 || logn == 13) && ws_enabled_inv()) {
-            CUtensorMap map;
-            cudaError_t e = make_row_map(&map, src, (size_t)n_polys << logn);
-            if (e != cudaSuccess) return e;
-            WsArgs a;
-            memset(&a, 0, sizeof(a));
-            a.n_polys = n_polys; a.mod_base = mod_base; a.mod_count = mod_count;
-            a.base_add = base; a.base_group = base_group; a.base_stride = base_stride;
-            if (logn == 13)
-                return out_f  ? ws_launch(k_ntt_inverse_ws<13, true, true>, ws_smem_bytes<13>(), map, dst, tabs, a, s)
-                       : in_f ? ws_launch(k_ntt_inverse_ws<13, true, false>, ws_smem_bytes<13>(), map, dst, tabs, a, s)
-                              : ws_launch(k_ntt_inverse_ws<13, false, false>, ws_smem_bytes<13>(), map, dst, tabs, a, s);
-            return out_f  ? ws_launch(k_ntt_inverse_ws<12, true, true>, ws_smem_bytes<12>(), map, dst, tabs, a, s)
-                   : in_f ? ws_launch(k_ntt_inverse_ws<12, true, false>, ws_smem_bytes<12>(), map, dst, tabs, a, s)
-                          : ws_launch(k_ntt_inverse_ws<12, false, false>, ws_smem_bytes<12>(), map, dst, tabs, a, s);
-        }
-        if (logn == 14 && split_enabled())
-            return out_f  ? launch_inv_split<true, true>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s)
-                   : in_f ? launch_inv_split<true, false>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s)
-                          : launch_inv_split<false, false>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s);
-        CNHE_DISPATCH_LOGN(logn, {
-            cudaError_t e = out_f  ? launch_inv_fp<L, true, true>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s)
-                            : in_f ? launch_inv_fp<L, true, false>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s)
-                                   : launch_inv_fp<L, false, false>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s);
-            if (e != cudaSuccess) return e;
-        });
-        return cudaGetLastError();
+        CNHE_DISPATCH_LOGN(logn, return out_f  ? launch_inv_fp<L, true, true>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s)
+                                        : in_f ? launch_inv_fp<L, true, false>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s)
+                                               : launch_inv_fp<L, false, false>(src, base, base_group, base_stride, dst, n_polys, tabs, mod_base, mod_count, s));
     }
     CNHE_DISPATCH_LOGN(logn, {
         cudaError_t e = prep(k_ntt_inverse<L>, L);

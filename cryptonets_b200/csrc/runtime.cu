@@ -500,7 +500,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     for (u64 p : c.q) moduli.push_back(p);
     for (u64 p : c.bsk) moduli.push_back(p);
     for (u64 p : c.t) moduli.push_back(p);
-    constexpr size_t TAB_WORDS = 10; // N-word tables per modulus: w, ws, iw, iws, wd, iwd, wd_hi, iwd_hi, wd_split, iwd_split
+    constexpr size_t TAB_WORDS = 9; // N-word tables per modulus: w, ws, iw, iws, wd, iwd, iwd_hi, wd_split, iwd_split
     std::vector<u64> host((size_t)n_mod * TAB_WORDS * N, 0);
     CNHE_CUDA(cudaMalloc((void **)&c.d_table_mem, host.size() * sizeof(u64)));
     c.h_tabs.resize(n_mod);
@@ -508,8 +508,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
         const u64 p = moduli[m];
         const u64 psi = hm::minimal_primitive_root(2ULL * N, p), ipsi = hm::inv(psi, p);
         u64 *w = &host[(size_t)m * TAB_WORDS * N], *ws = w + N, *iw = ws + N, *iws = iw + N;
-        double *wd = reinterpret_cast<double *>(iws + N), *iwd = wd + N, *wd_hi = iwd + N, *iwd_hi = wd_hi + N, *wd_split = iwd_hi + N,
-               *iwd_split = wd_split + N;
+        double *wd = reinterpret_cast<double *>(iws + N), *iwd = wd + N, *iwd_hi = iwd + N, *wd_split = iwd_hi + N, *iwd_split = wd_split + N;
         u64 a = 1, b = 1;
         for (u64 i = 0; i < N; i++) {
             const u64 r = hm::bit_reverse(i, logN);
@@ -520,31 +519,21 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
             a = hm::mul(a, psi, p);
             b = hm::mul(b, ipsi, p);
         }
-        if (logN == 14) { // twiddle tables of the two half-size transforms (see NttTab::fwd_recenter_split)
-            const u64 H = N / 2;
-            for (u64 h = 0; h < 2; h++)
-                for (u64 i = 1; i < H; i++) {
-                    u64 m2 = 1;
-                    while (2 * m2 <= i) m2 *= 2; // stage of index i: [m2, 2 m2)
-                    wd_hi[h * H + i] = wd[i + m2 + h * m2];
-                    iwd_hi[h * H + i] = iwd[i + m2 + h * m2];
-                }
-        } else { // transposed unit-stride twiddles (see NttTab::wd_hi)
+        if (logN == 12 || logN == 13) { // transposed unit-stride inverse twiddles (see NttTab::iwd_hi)
             const u64 T = N / 16;
-            const int S0 = logN - 4;
             for (u64 j = 0; j < T; j++) {
-                for (int u = 0; u < 4; u++)
-                    for (int i = 0; i < (1 << u); i++) wd_hi[(u64)((1 << u) - 1 + i) * T + j] = wd[((u64)1 << (S0 + u)) + (j << u) + i];
                 for (int i = 0; i < 8; i++) iwd_hi[(u64)i * T + j] = iwd[(N >> 1) + (j << 3) + i];
                 for (int i = 0; i < 4; i++) iwd_hi[(u64)(8 + i) * T + j] = iwd[(N >> 2) + (j << 2) + i];
                 for (int i = 0; i < 2; i++) iwd_hi[(u64)(12 + i) * T + j] = iwd[(N >> 3) + (j << 1) + i];
                 iwd_hi[(u64)14 * T + j] = iwd[(N >> 4) + j];
             }
-            const u64 H = N / 2; // the halves' tables of the fused key switch (forward) and square (both), laid out as wd_hi / iwd_hi at N = 16384
+        }
+        if (logN >= 12) { // twiddle tables of the two half-size transforms (see NttTab::wd_split)
+            const u64 H = N / 2;
             for (u64 h = 0; h < 2; h++)
                 for (u64 i = 1; i < H; i++) {
                     u64 m2 = 1;
-                    while (2 * m2 <= i) m2 *= 2;
+                    while (2 * m2 <= i) m2 *= 2; // stage of index i: [m2, 2 m2)
                     wd_split[h * H + i] = wd[i + m2 + h * m2];
                     iwd_split[h * H + i] = iwd[i + m2 + h * m2];
                 }
@@ -554,10 +543,9 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
         tb.w = base; tb.ws = base + N; tb.iw = base + 2 * (size_t)N; tb.iws = base + 3 * (size_t)N;
         tb.wd = reinterpret_cast<const double *>(base + 4 * (size_t)N);
         tb.iwd = reinterpret_cast<const double *>(base + 5 * (size_t)N);
-        tb.wd_hi = reinterpret_cast<const double *>(base + 6 * (size_t)N);
-        tb.iwd_hi = reinterpret_cast<const double *>(base + 7 * (size_t)N);
-        tb.wd_split = reinterpret_cast<const double *>(base + 8 * (size_t)N);
-        tb.iwd_split = reinterpret_cast<const double *>(base + 9 * (size_t)N);
+        tb.iwd_hi = reinterpret_cast<const double *>(base + 6 * (size_t)N);
+        tb.wd_split = reinterpret_cast<const double *>(base + 7 * (size_t)N);
+        tb.iwd_split = reinterpret_cast<const double *>(base + 8 * (size_t)N);
         tb.inv_n = hm::inv(N % p, p);
         tb.inv_n_s = hm::shoup(tb.inv_n, p);
         tb.mod = make_dmod(p);
@@ -847,9 +835,8 @@ static bool mul_fused(const Context &c, const std::vector<const u64 *> &a, const
 static size_t mul_words(const Context &c, bool fused) { return (size_t)(fused ? 2 * c.kb + 3 * (c.k + c.kb) : 7 * (c.k + c.kb)) * c.N; }
 static void multiply_floor(Context &c, int ch, const u64 *D, int m, bool lazy, u64 *out3) {
     PROF(2, 8.0 * c.N * m * 3 * (2 * c.k + c.kb));
-    static const bool fold = getenv("CNHE_FLOOR_NOFOLD") == nullptr;
-    if (c.fp_elementwise && lazy && fold) c.check(launch_behz_floor_fold_fp(D, out3, m, c.logN, &c.ch[ch].floor_f, c.stream), "behz_floor_fold_fp");
-    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, m, c.ch[ch].t, c.logN, &c.h_bf, lazy, c.stream), "behz_floor_fp");
+    if (c.fp_elementwise && lazy) c.check(launch_behz_floor_fold_fp(D, out3, m, c.logN, &c.ch[ch].floor_f, c.stream), "behz_floor_fold_fp");
+    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, m, c.ch[ch].t, c.logN, &c.h_bf, c.stream), "behz_floor_fp");
     else c.check(launch_behz_floor(D, out3, m, c.ch[ch].t, c.logN, c.d_bc, c.stream), "behz_floor");
 }
 static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, int c0, int m, u64 *out3,

@@ -277,7 +277,7 @@ extern "C" int cnhe_raw_behz_floor(cnhe_ctx *h, int channel, uint64_t d, int n, 
     API_BEGIN(h)
     if (channel < 0 || channel >= c.P) fail("bad channel");
     c.set_channel(channel);
-    if (c.fp_elementwise) c.check(launch_behz_floor_fp((const u64 *)d, (u64 *)out3, n, c.ch[channel].t, c.logN, &c.h_bf, 0, c.stream), "behz_floor_fp");
+    if (c.fp_elementwise) c.check(launch_behz_floor_fp((const u64 *)d, (u64 *)out3, n, c.ch[channel].t, c.logN, &c.h_bf, c.stream), "behz_floor_fp");
     else c.check(launch_behz_floor((const u64 *)d, (u64 *)out3, n, c.ch[channel].t, c.logN, c.d_bc, c.stream), "behz_floor");
     API_END
 }

@@ -13,13 +13,12 @@ CONFIGS = {
 }
 
 
-def _make_pair(name, aux):
+def _make_engine(name, aux):
     """aux: 'fast' = 48-bit auxiliary base + FP64 butterflies (the default product configuration);
             'seal' = SEAL 3.2's 61-bit auxiliary base (integer butterflies on those moduli), comparable stage by stage;
             'int'  = fast base but integer butterflies everywhere (CNHE_NTT_INT)."""
     import os
     from cryptonets_b200.engine import Engine
-    from oracle.oracle_py import Oracle
     cfg = CONFIGS[name]
     os.environ.pop("CNHE_AUX_BASE", None)
     os.environ.pop("CNHE_NTT_INT", None)
@@ -32,6 +31,14 @@ def _make_pair(name, aux):
     finally:
         os.environ.pop("CNHE_AUX_BASE", None)
         os.environ.pop("CNHE_NTT_INT", None)
+    return eng
+
+
+def _make_pair(name, aux):
+    """the engine of _make_engine(name, aux) and the oracle of the same parameters, both keyed with seed 1234"""
+    from oracle.oracle_py import Oracle
+    cfg = CONFIGS[name]
+    eng = _make_engine(name, aux)
     orc = Oracle(cfg["t"], cfg["N"], cfg["count"], cfg["dbc_r"], cfg["dbc_g"])
     assert eng.q == orc.q
     if aux == "seal":
@@ -331,27 +338,29 @@ def test_dense_layer_on_tensor_cores(pair, shape, capfd):
 
 
 @pytest.mark.parametrize("fwd,inv", [("1", "1"), ("0", "0"), ("1", "0"), ("0", "1")])
-def test_persistent_and_per_polynomial_transforms_agree(pair, fwd, inv, monkeypatch):
-    """The transforms exist twice for N = 4096 / 8192: one CTA per polynomial, and persistent CTAs fed by TMA (cp.async.bulk.tensor)
-    with the unit-stride twiddles resident in shared memory.  Every combination of the two (forward / inverse; the defaults are the
-    per-polynomial forward and the persistent inverse) must give the oracle's words: plain transforms on a batch that gives every CTA
-    several polynomials, the digit-cutting forward inside relinearise, and the lazy-double variants inside multiply."""
+def test_persistent_and_per_polynomial_transforms_agree(pair, fwd, inv):
+    """At N = 4096 / 8192 the inverse transform runs on persistent CTAs fed by TMA (cp.async.bulk.tensor) with the unit-stride
+    twiddles resident in shared memory, the forward one on one CTA per polynomial.  Both must give the oracle's words on a batch that
+    gives every CTA several polynomials (ragged tail), the inverse must bring the batch back, and so must the digit-cutting forward
+    inside relinearise and the lazy-double variants inside multiply.  fwd / inv = "1": that direction runs in place (src == dst; the
+    persistent kernel then overwrites each polynomial of the array it stages the next ones from), "0": out of place.  The other
+    rings run the same checks on their own kernels."""
     eng, orc, name = pair
-    monkeypatch.setenv("CNHE_NTT_WS_FWD", fwd)
-    monkeypatch.setenv("CNHE_NTT_WS_INV", inv)
     rng = np.random.default_rng(11)
     N, k, kt = eng.N, eng.k, eng.k + eng.kb
     tab = _mod_table(eng, orc)
     n = 64 * kt + 3  # more polynomials than CTAs x 2 groups for some moduli, ragged tail
     polys = np.stack([rng.integers(0, tab[b % kt][0], N, dtype=np.uint64) for b in range(n)])
     d, out = eng.dev_from(polys), eng.dev_alloc(polys.size)
-    eng.raw_ntt(d, out, n, 0, kt, False)
-    got = eng.dev_download(out, polys.size).reshape(polys.shape)
+    f_dst = d if fwd == "1" else out
+    eng.raw_ntt(d, f_dst, n, 0, kt, False)
+    got = eng.dev_download(f_dst, polys.size).reshape(polys.shape)
     for b in list(range(0, n, 37)) + [n - 1]:
         p, o, oid = tab[b % kt]
         assert np.array_equal(got[b], o.ntt(oid, polys[b])), b
-    eng.raw_ntt(out, out, n, 0, kt, True)
-    assert np.array_equal(eng.dev_download(out, polys.size).reshape(polys.shape), polys)
+    i_dst = f_dst if inv == "1" else (out if f_dst == d else d)
+    eng.raw_ntt(f_dst, i_dst, n, 0, kt, True)
+    assert np.array_equal(eng.dev_download(i_dst, polys.size).reshape(polys.shape), polys)
     eng.dev_free(d)
     eng.dev_free(out)
     m = 5
@@ -365,14 +374,24 @@ def test_persistent_and_per_polynomial_transforms_agree(pair, fwd, inv, monkeypa
 
 
 @pytest.mark.parametrize("split", ["1", "0"])
-def test_cta_pair_and_whole_polynomial_transforms_agree(pair, split, monkeypatch):
-    """N = 16384 runs on CTA pairs by default (two 8192-point halves, the cross-half stage on the way in / through distributed shared
-    memory on the way out); CNHE_NTT_SPLIT=0 keeps the one-CTA-per-polynomial kernels.  Both must give the oracle's words: plain
-    transforms out of place and IN PLACE (the pair reads both halves before either writes), the digit-cutting forward and the lazy
-    variants inside multiply + relinearise.  On the other rings, which have no CTA-pair kernels, either setting of the flag must leave
-    the same transforms exact."""
+def test_cta_pair_and_whole_polynomial_transforms_agree(pair, split):
+    """N = 16384 runs on CTA pairs on the FP64 path (two 8192-point halves, the cross-half stage on the way in / through distributed
+    shared memory on the way out) and on one CTA per polynomial on the integer path (moduli of 2^50 and above, CNHE_NTT_INT).  split =
+    "1" checks the ring's own engine, "0" an engine of the same parameters on integer butterflies.  Both must give the oracle's words:
+    plain transforms out of place and IN PLACE (the pair reads both halves before either writes), the digit-cutting forward and the
+    lazy variants inside multiply + relinearise.  The other rings run the same checks on their own kernels."""
     eng, orc, name = pair
-    monkeypatch.setenv("CNHE_NTT_SPLIT", split)
+    if split == "0":
+        eng = _make_engine(name, "int")
+        eng.keygen(1234)
+    try:
+        _check_transforms_and_product(eng, orc)
+    finally:
+        if split == "0":
+            eng.close()
+
+
+def _check_transforms_and_product(eng, orc):
     rng = np.random.default_rng(12)
     N, k, kt = eng.N, eng.k, eng.k + eng.kb
     tab = _mod_table(eng, orc)
@@ -481,21 +500,25 @@ def test_tensor_core_layers_randomised():
 
 
 def test_key_switch_mac_full_waves(pair, monkeypatch):
-    """Waves of 64 or more ciphertexts take the key-switch inner product through the copy-engine-staged kernel (cp.async.bulk ring, four
-    ciphertexts per CTA share the key words); smaller calls and CNHE_KSMAC_TMA=0 use the register kernels.  70 ciphertexts (a ragged last
-    group of two): multiply + relinearise must match the oracle on sampled ciphertexts and the register kernel on all of them."""
+    """Waves of 64 or more ciphertexts take the digit path's key-switch inner product (lazy FP64 path) through the copy-engine-staged
+    kernel (cp.async.bulk ring, four ciphertexts per CTA share the key words); CNHE_KS_FUSED=0 keeps every ring on the digit path.  70
+    ciphertexts (a ragged last group of two) drawn from six: multiply + relinearise must match the oracle on all of them, and where
+    the fused key switch is built its outputs must equal the digit path's."""
     eng, orc, name = pair
     N, k = eng.N, eng.k
     m = 70
     _, few = _fresh_cts(orc, 6, 21, nonce0=3000)
-    cts = np.stack([few[i % 6] for i in range(m)])
-    cts[1::2] = np.roll(cts[1::2], 1, axis=0)  # not all groups alike
+    src = np.arange(m) % 6
+    src[1::2] = np.roll(src[1::2], 1)  # not all groups alike
+    cts = np.stack([few[i] for i in src])
+    want = [orc.relinearize(orc.multiply(few[j], few[j])) for j in range(6)]
     a, o1, o2 = eng.dev_from(cts), eng.dev_alloc(m * 2 * k * N), eng.dev_alloc(m * 2 * k * N)
+    monkeypatch.setenv("CNHE_KS_FUSED", "0")
     eng.raw_multiply_relin(0, a, a, m, o1)
     got = eng.dev_download(o1, m * 2 * k * N).reshape(m, -1)
-    for i in (0, 3, 33, 67, 68, 69):
-        assert np.array_equal(got[i], orc.relinearize(orc.multiply(cts[i], cts[i]))), i
-    monkeypatch.setenv("CNHE_KSMAC_TMA", "0")
+    for i in range(m):
+        assert np.array_equal(got[i], want[src[i]]), i
+    monkeypatch.setenv("CNHE_KS_FUSED", "1")  # no effect where the fused key switch is not built
     eng.raw_multiply_relin(0, a, a, m, o2)
     assert np.array_equal(eng.dev_download(o2, m * 2 * k * N).reshape(m, -1), got)
     for d in (a, o1, o2):
