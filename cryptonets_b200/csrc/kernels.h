@@ -59,12 +59,13 @@ cudaError_t launch_ntt_inverse(const u64 *src, u64 *dst, int n_polys, int logn, 
 // ciphertext c's k-residue target polynomial starts at target + c * ct_stride (words)
 cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *dst, int n_ct, int k, const DigitMap &dm, int logn,
                                       const NttTab *tabs, int fp, cudaStream_t s);
-// Fused key-switch inner product (N = 4096 / 8192, FP64 path, lazy output): acc[c][p][l] = sum_d NTT_l(digit d of target[c]) * key[d][p][l],
-// key [D][2][k][N] canonical NTT form, acc [n_ct][2][k][N] lazy doubles (|x| <= 0.51 p) -- what launch_ntt_forward_digits followed by
-// launch_ks_mac_fp(lazy) compute, with no digit buffer.  key_packed: nullptr, or the copy of `key` made by launch_pack_keys48 (every
-// q_l < 2^48), which the kernel then reads instead
-cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, u64 *acc, int n_ct, int k,
-                                    const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s);
+// Fused key switch (N = 4096 / 8192, FP64 path): out[c][p][l] = base_c[p][l] + INTT_l(sum_d NTT_l(digit d of target[c]) * key[d][p][l])
+// (mod q_l, canonical), key [D][2][k][N] canonical NTT form, base polynomial p of ciphertext c at base + c * base_stride + p * k * N, out
+// packed [n_ct][2][k][N] -- what launch_ntt_forward_digits, launch_ks_mac_fp(lazy) and launch_ntt_inverse_add compute, with no digit
+// buffer and no accumulator.  out must overlap neither the target nor the base words: other CTAs still read them while one writes.
+// key_packed: nullptr, or the copy of `key` made by launch_pack_keys48 (every q_l < 2^48), which the kernel then reads instead
+cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *base, size_t base_stride,
+                                    u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s);
 // the fused key switch's packed key copy: n_polys canonical N-word polynomials (words < 2^48) -> 6N bytes each, thread-interleaved (ntt.cu)
 cudaError_t launch_pack_keys48(const u64 *key, uint4 *out, int n_polys, int logn, cudaStream_t s);
 // dst[b] = INTT(src[b]) + base[(b / base_group) * base_stride + (b % base_group) * N]  (mod p)

@@ -947,7 +947,8 @@ k_ntt_forward_digits_split(const u64 *target, size_t ct_stride, u64 *dst, const 
     fwd_split_body<false, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (((size_t)c * k + l) * dm.D + d) * (2 * SPLIT_H) + half * SPLIT_H, tb, half, tid);
 }
 // last in-half pass (stages 8 .. HLOGN-1) and the cross-half butterfly of NB polynomials (consecutive half buffers of sm; polynomial b goes to
-// dst + b * dst_stride): own results go to shared memory for the partner, the partner's come back through DSMEM; half 0 keeps the sums
+// dst + b * dst_stride and, with a base, adds base_add + b * dst_stride): own results go to shared memory for the partner, the partner's
+// come back through DSMEM; half 0 keeps the sums
 // (times N^-1), half 1 the differences (times iw[1] N^-1).  One pair of cluster barriers serves all NB polynomials.
 template <int HLOGN, int TR, bool OUT_F, int NB = 1>
 __device__ __forceinline__ void inv_split_last(double *sm, const double *twc, u64 *dst, size_t dst_stride, const u64 *base_add, const NttTab &tb,
@@ -992,6 +993,7 @@ __device__ __forceinline__ void inv_split_last(double *sm, const double *twc, u6
     for (int b = 0; b < NB; b++) {
         const double *s = sm + b * H;
         u64 *d = dst + b * dst_stride;
+        const u64 *ba = base_add ? base_add + b * dst_stride : nullptr;
         for (int vt = tid; vt < (H >> R); vt += TR) {
 #pragma unroll
             for (int e0 = 0; e0 < E; e0 += 8) { // own values back from shared memory, the partner's in batches of 8 (all at once would spill)
@@ -1006,7 +1008,7 @@ __device__ __forceinline__ void inv_split_last(double *sm, const double *twc, u6
                     if constexpr (OUT_F) d[idx] = lazy_bits(v);
                     else {
                         u64 o = fsmall_u(v, tb.mod.p);
-                        if (base_add) o = addmod(o, base_add[idx], tb.mod.p);
+                        if (ba) o = addmod(o, ba[idx], tb.mod.p);
                         d[idx] = o;
                     }
                 }
@@ -1042,7 +1044,8 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
 }
 
 // ================================================================ fused key switch, N = 4096 / 8192
-// acc[c][p][l] = sum_d NTT_l(digit_d(target_c)) * key[d][p][l]  without the digit transforms ever reaching HBM.  The digit path
+// out[c][p][l] = base_c[p][l] + INTT_l(sum_d NTT_l(digit_d(target_c)) * key[d][p][l])  without the digit transforms or the NTT-domain
+// accumulator ever reaching HBM.  The digit path
 // (k_ntt_forward_digits_fp + k_ks_mac_tma) writes every digit transform as lazy doubles and reads it back once: 2 x 64 KiB per transform at
 // N = 8192, 31 GB per CryptoNets step, more than the FP64 work of the transforms costs on an H100.  Here a CTA owns one half of the
 // transform of one (ciphertext c, residue l) and walks all D digits: after the first stage the two halves of an N-point transform are
@@ -1052,7 +1055,14 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
 // accumulates them in shared memory ([key poly][coefficient pair][thread]: every thread touches only its own slots, no extra barrier).
 // The twiddle cache is filled once per CTA instead of once per transform, and the next digit's source words are in flight while the CTA
 // waits at the barrier that ends the current digit.  Same arithmetic as the MAC kernels (fmodmul + dadd, re-centred every 8 digits and
-// at the end), so the accumulator leaves with |x| <= 0.51 p in the layout launch_ntt_inverse_add consumes.
+// at the end), so the accumulators end at |x| <= 0.51 p, within the inverse transform's 1.25 p input bound.
+// Epilogue: the pair of CTAs is a cluster and finishes the key switch as k_behz_square_fused does: thread j holds coefficients 16j..16j+15
+// of both accumulators, exactly the group the split inverse's first four stages work on, so it runs them in registers and stores the two
+// results as consecutive half buffers (polynomial 0 over the work buffer, polynomial 1 over the polynomial-0 accumulator), then the
+// remaining in-half pass of both and the cross-half stage (N^-1, canonical output, plus the base word) through DSMEM.  The base half is
+// prefetched to L2 during the last digit.  Compared with writing the accumulator and running k_ntt_inverse_ws, every (ciphertext,
+// polynomial, residue) saves an 8N-byte HBM write and read and a second kernel.  Other CTAs may still read target and base words while a
+// cluster writes its output: `out` must overlap neither (the host takes the digit path otherwise).
 // Keys: with PK the kernel reads the 48-bit packed copy of launch_pack_keys48 instead of the canonical u64 keys.  The key loads are the
 // kernel's costliest memory traffic (keys replaced by register values: -35 % kernel time at N = 8192, source words: -3.5 %, DESIGN
 // §4.4): a thread's 16 u64 words are 128 contiguous bytes, so each 16-byte load of a warp touches 32 cache lines and the lines are
@@ -1062,7 +1072,7 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
 template <int HLOGN>
 __host__ __device__ constexpr int ks_fused_threads() { return (1 << HLOGN) / 16; }
 template <int HLOGN>
-__host__ __device__ constexpr int ks_fused_smem() { return (1 << HLOGN) * 8 * 3 + TWC * 8; } // work buffer, two accumulators, twiddle cache
+__host__ __device__ constexpr int ks_fused_smem() { return (1 << HLOGN) * 8 * 3 + 2 * TWC * 8; } // work buffer, two accumulators, two twiddle caches
 // a word below 2^48 given as its low 32 bits and bits 32..47, as an exact double (u2d of the same word)
 __device__ __forceinline__ double u48d(unsigned lo, unsigned hi16) { return __dsub_rn(__hiloint2double((int)(hi16 | 0x43300000u), (int)lo), FP_TWO52); }
 // packed copy: the 16 key words of (polynomial b, half, thread j), 48 bits each, little-endian in 24 u32: word 2m in u32 3m and the low
@@ -1087,19 +1097,20 @@ __global__ void __launch_bounds__(256) k_pack_keys48(const u64 *__restrict__ key
     for (int g = 0; g < 6; g++) o[g * TR] = make_uint4(u[4 * g], u[4 * g + 1], u[4 * g + 2], u[4 * g + 3]);
 }
 template <int HLOGN, bool PK>
-__global__ void __launch_bounds__(ks_fused_threads<HLOGN>(), HLOGN == 12 ? 2 : 4)
-k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *__restrict__ key, const uint4 *__restrict__ keyp, u64 *__restrict__ acc,
-                   const NttTab *__restrict__ tabs, int k, DigitMap dm) {
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(ks_fused_threads<HLOGN>(), HLOGN == 12 ? 2 : 4)
+k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *__restrict__ key, const uint4 *__restrict__ keyp,
+                   const u64 *__restrict__ base, size_t base_stride, u64 *__restrict__ out, const NttTab *__restrict__ tabs, int k, DigitMap dm) {
     constexpr int H = 1 << HLOGN, TR = ks_fused_threads<HLOGN>(), N = 2 * H;
     constexpr int R1 = HLOGN - 8, E1 = 1 << R1, LG1 = HLOGN - R1; // first pass: stage 0 on the loads, then R1 stages; then 4 + 4
     extern __shared__ __align__(16) u64 ks_raw[];
-    double *sm = reinterpret_cast<double *>(ks_raw);
-    double *twc = sm + H;
-    double2 *accv = reinterpret_cast<double2 *>(twc + TWC); // [p][e/2][TR]
+    double *sm = reinterpret_cast<double *>(ks_raw);           // [3][H]: work buffer, then the inverse's two half buffers
+    double2 *accv = reinterpret_cast<double2 *>(sm + H);       // [p][e/2][TR]
+    double *twc = sm + 3 * H, *twci = twc + TWC;               // forward / inverse twiddles of this half
     const int half = blockIdx.x & 1, l = (blockIdx.x >> 1) % k, c = (blockIdx.x >> 1) / k, tid = threadIdx.x;
     NttTab tb = tabs[l];
     const double w0 = __ldg(tb.wd + 1);
     tb.wd = tb.wd_split + half * H;
+    tb.iwd = tb.iwd_split + half * H;
     tb.fwd_recenter = tb.fwd_recenter_split;
     const double p = tb.pd, pinv = tb.pinv;
     const bool need_reduce = dm.mask >= tb.mod.p;
@@ -1107,6 +1118,7 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
     const size_t kpoly = (size_t)k * N, kstride = 2 * kpoly;
     const u64 *key_l = key + (size_t)l * N + half * H + 16 * tid;
     load_twiddle_cache(twc, tb.wd, tid, TR);
+    load_twiddle_cache(twci, tb.iwd, tid, TR);
 #pragma unroll
     for (int i = 0; i < 16; i++) accv[i * TR + tid] = make_double2(0.0, 0.0);
     auto cut = [&](u64 v, int shift) { // digit of a canonical word: exact below 2^50
@@ -1117,6 +1129,13 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
     for (int d = 0; d < dm.D; d++) {
         const u64 *src = src_c + (size_t)dm.src[d] * N;
         const int shift = dm.shift[d];
+        if (d == dm.D - 1) { // the epilogue adds this half of both base polynomials: have them waiting in L2
+#pragma unroll
+            for (int kp = 0; kp < 2; kp++) {
+                const char *pb = reinterpret_cast<const char *>(base + (size_t)c * base_stride + kp * kpoly + (size_t)l * N + half * H);
+                for (int i = tid * 128; i < H * 8; i += TR * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(pb + i));
+            }
+        }
         constexpr int VT1 = (H >> R1) / TR; // first-pass virtual threads per thread
         double xs[VT1][E1]; // stage 0 of the N-point transform, computed while other warps finish the previous digit
 #pragma unroll
@@ -1226,15 +1245,29 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
             }
         }
     }
+    {
+        // inverse stages 0..3 of both accumulators in registers.  Polynomial 0 goes over the work buffer: thread j's group there is the one it
+        // read itself in the last forward pass.  Polynomial 1 goes over the polynomial-0 accumulator once every thread has read its slots.
+        double x[16];
 #pragma unroll
-    for (int kp = 0; kp < 2; kp++) {
-        u64 *o = acc + ((size_t)(c * 2 + kp) * k + l) * N + half * H + 16 * tid;
+        for (int kp = 0; kp < 2; kp++) {
 #pragma unroll
-        for (int g = 0; g < 4; g++) {
-            const double2 a = accv[(kp * 8 + 2 * g) * TR + tid], b = accv[(kp * 8 + 2 * g + 1) * TR + tid];
-            stg256(o + 4 * g, lazy_bits(a.x), lazy_bits(a.y), lazy_bits(b.x), lazy_bits(b.y));
+            for (int i = 0; i < 8; i++) {
+                const double2 a = accv[(kp * 8 + i) * TR + tid];
+                x[2 * i] = a.x;
+                x[2 * i + 1] = a.y;
+            }
+            inv_first_stages<HLOGN>(x, tb, tid);
+            if (kp) __syncthreads();
+            st_group16(sm + kp * H, tid, x);
         }
     }
+    __syncthreads();
+#pragma unroll 1
+    for (int r = 0; r < 2; r++) CNHE_VTN(H / 16, (inv_pass_fp<HLOGN, 4, 4, false, false>(sm + r * H, twci, nullptr, nullptr, tb, vt)));
+    __syncthreads();
+    const size_t ol = (size_t)l * N + half * H;
+    inv_split_last<HLOGN, TR, false, 2>(sm, twci, out + (size_t)c * kstride + ol, kpoly, base + (size_t)c * base_stride + ol, tb, tid, half);
 }
 
 // ================================================================ fused BEHZ square, N = 4096 / 8192
@@ -1720,24 +1753,25 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
     return cudaGetLastError();
 }
 template <int HL, bool PK>
-static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, u64 *acc, int n_ct, int k, const DigitMap &dm,
-                                   const NttTab *tabs, cudaStream_t s) {
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, const u64 *base, size_t base_stride,
+                                   u64 *out, int n_ct, int k, const DigitMap &dm, const NttTab *tabs, cudaStream_t s) {
     cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL, PK>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
     if (e != cudaSuccess) return e;
-    k_key_switch_fused<HL, PK><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, key, keyp, acc, tabs, k, dm);
+    k_key_switch_fused<HL, PK><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, key, keyp, base, base_stride, out,
+                                                                                               tabs, k, dm);
     return cudaGetLastError();
 }
 template <int HL>
-static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, u64 *acc, int n_ct, int k, const DigitMap &dm,
-                                   const NttTab *tabs, cudaStream_t s) {
-    return keyp ? launch_ks_fused<HL, true>(target, ct_stride, key, keyp, acc, n_ct, k, dm, tabs, s)
-                : launch_ks_fused<HL, false>(target, ct_stride, key, keyp, acc, n_ct, k, dm, tabs, s);
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, const u64 *base, size_t base_stride,
+                                   u64 *out, int n_ct, int k, const DigitMap &dm, const NttTab *tabs, cudaStream_t s) {
+    return keyp ? launch_ks_fused<HL, true>(target, ct_stride, key, keyp, base, base_stride, out, n_ct, k, dm, tabs, s)
+                : launch_ks_fused<HL, false>(target, ct_stride, key, keyp, base, base_stride, out, n_ct, k, dm, tabs, s);
 }
-cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, u64 *acc, int n_ct, int k,
-                                    const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s) {
+cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *base, size_t base_stride,
+                                    u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s) {
     if (n_ct <= 0) return cudaSuccess;
-    if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, key_packed, acc, n_ct, k, dm, tabs, s);
-    if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, key_packed, acc, n_ct, k, dm, tabs, s);
+    if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, key_packed, base, base_stride, out, n_ct, k, dm, tabs, s);
+    if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, key_packed, base, base_stride, out, n_ct, k, dm, tabs, s);
     return cudaErrorInvalidValue;
 }
 template <int HL>

@@ -778,6 +778,7 @@ static bool ks_fused(const Context &c, int n) {
     if (v) return atoi(v) != 0;
     return n >= KS_FUSED_MIN;
 }
+static bool spans_overlap(const u64 *a, size_t a_words, const u64 *b, size_t b_words) { return a < b + b_words && b < a + a_words; }
 // out[i] = (base_i + sum_d NTT^-1(NTT(digit_d(target_i)) * key_d)): ciphertext i's target polynomial (k residues) is at
 // target + i * target_stride, its base (2 polynomials) at base + i * base_stride; out is packed [n][2][k][N]
 void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, const u64 *key, const DigitMap &dm, const u64 *base,
@@ -786,19 +787,27 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
     const size_t N = c.N;
     const int fpq = fp_range(c, 0, k);
     const bool lazy = c.lazy && fpq;
-    const bool fused = ks_fused(c, n);
-    const int wave = c.wave(((fused ? 0 : (size_t)dm.D * k) + 2 * k) * N);
+    // the fused kernel writes `out` while other CTAs still read target and base words, so it serves only calls whose output overlaps
+    // neither; every internal caller passes scratch, an in-place cnhe_raw_relinearize (out2 inside in3) takes the digit path
+    const size_t out_words = (size_t)n * 2 * k * N;
+    const bool fused = n > 0 && ks_fused(c, n) && !spans_overlap(out, out_words, target, (n - 1) * target_stride + k * N) &&
+                       !spans_overlap(out, out_words, base, (n - 1) * base_stride + 2 * k * N);
+    const int wave = c.wave(fused ? 0 : ((size_t)dm.D * k + 2 * k) * N);
     for (int c0 = 0; c0 < n; c0 += wave) {
         WsScope scope(c);
         const int m = std::min(wave, n - c0);
-        u64 *acc = c.ws_alloc((size_t)m * 2 * k * N);
         if (fused) {
-            // HBM: the target residues once (the pair and the other residues' CTAs share them through L2), the keys once, the accumulator
+            // HBM: the target residues once (the pair and the other residues' CTAs share them through L2), the keys once, the output.  The
+            // base words the epilogue adds (another 8N bytes per output polynomial, mostly prefetched) are not booked: the figure keeps the
+            // meaning it had when the kernel wrote an accumulator of the output's size
             PROF(3, 8.0 * N * ((double)m * k + (double)m * 2 * k) + (key_packed ? 6.0 : 8.0) * N * dm.D * 2 * k);
-            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, key, reinterpret_cast<const uint4 *>(key_packed), acc,
-                                            m, k, dm, c.logN, c.d_tabs, c.stream),
+            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, key, reinterpret_cast<const uint4 *>(key_packed),
+                                            base + (size_t)c0 * base_stride, base_stride, out + (size_t)c0 * 2 * k * N, m, k, dm, c.logN, c.d_tabs, c.stream),
                     "key_switch_fused");
-        } else {
+            continue;
+        }
+        u64 *acc = c.ws_alloc((size_t)m * 2 * k * N);
+        {
             u64 *digits = c.ws_alloc((size_t)m * dm.D * k * N);
             {
                 PROF(0, 16.0 * N * (double)m * dm.D * k); // SURVEY 8d: 16N bytes per transform (8N digit source read + 8N written)

@@ -3,9 +3,10 @@ stream), per-family device times and the HBM bytes the two key-switch forms need
 
     python tools/keyswitch_bench.py [n ...] [--iters I] [--path auto|fused|digits]
 
-During a relinearise-only call family 0 (ntt_forward) is the digit transforms alone, family 3 (keyswitch_mac) the key product -- or,
-on the fused path, digit transforms and key product together -- and family 1 (ntt_inverse) the inverse transforms with the base
-addition.  `--path` sets CNHE_KS_FUSED for the run (auto: the library's own choice by n).  One JSON line per n.
+During a relinearise-only call on the digit path family 0 (ntt_forward) is the digit transforms, family 3 (keyswitch_mac) the key
+product and family 1 (ntt_inverse) the inverse transforms with the base addition.  On the fused path family 3 is the one kernel that
+does all three, and families 0 and 1 stay empty.  `--path` sets CNHE_KS_FUSED for the run (auto: the library's own choice by n).  One
+JSON line per n.
 
 The fused kernel's operands come from L2: every (ciphertext, residue, half) CTA reads both halves of the source residue (8N bytes) and
 its half of the two key polynomials (8N bytes as u64 words, 6N in the 48-bit packed copy the library uses while every q_l < 2^48) per
@@ -34,12 +35,15 @@ D = sum((int(q).bit_length() + 9) // 10 for q in eng.q)  # base-2^10 digits of e
 q = np.array(eng.q, dtype=np.uint64)
 packed = max(eng.q) < 1 << 48
 rng = np.random.default_rng(0)
-# FP64 warp instructions per (ciphertext, residue, half) and digit of the fused kernel at N = 8192 (4096-point halves, 256 threads, 16
-# coefficients each): stage 0 folded into the loads (16 modular products + 16 adds), 12 radix-2 stages of 8 butterflies (6 + 2), the key
-# product (32 modular products + 32 adds), digit conversions (32 u2d) and key conversions (32 u2d)
+# FP64 instructions per thread of a (ciphertext, residue, half) CTA of the fused kernel at N = 8192 (4096-point halves, 256 threads, 16
+# coefficients each).  Per digit: stage 0 folded into the loads (16 modular products + 16 adds), 12 radix-2 stages of 8 butterflies
+# (6 + 2), the key product (32 modular products + 32 adds), digit conversions (32 u2d) and key conversions (32 u2d).  Once per CTA, the
+# epilogue's inverse of both key polynomials: 12 in-half stages of 8 butterflies each, then the cross-half stage (16 adds and modular
+# products by N^-1) and 16 conversions to integers
 FMODMUL, BFLY = 6, 8
 DP_PER_THREAD = 16 * (FMODMUL + 1) + 12 * 8 * BFLY + 32 * (FMODMUL + 1) + 32 + 32
-DP_WARP_INSTR_PER_CT = DP_PER_THREAD * (256 // 32) * 2 * k * D
+DP_INVERSE_PER_THREAD = 2 * (12 * 8 * BFLY + 16 * (FMODMUL + 1) + 16)
+DP_WARP_INSTR_PER_CT = (DP_PER_THREAD * D + DP_INVERSE_PER_THREAD) * (256 // 32) * 2 * k
 for n in args.n:
     host = (rng.integers(0, 1 << 62, (n, 3, k, N), dtype=np.uint64) % q[None, None, :, None]).astype(np.uint64)
     a = eng.dev_from(host)
@@ -59,12 +63,12 @@ for n in args.n:
     w = 8.0 * N
     bytes_digits = w * (n * k * D * 2 + n * k * D + D * 2 * k + n * 2 * k)  # digit source + digits written, digits + keys read, acc written
     key_word = 6.0 if packed else 8.0  # bytes per key word the fused kernel reads (packed copy while every q_l < 2^48)
-    bytes_fused = w * (n * k + n * 2 * k) + key_word * N * D * 2 * k  # target residues, acc, keys
-    bytes_inverse = w * (n * 2 * k * 3)  # acc read, base read, out written
+    bytes_inverse = w * (n * 2 * k * 3)  # acc read, base read, out written (digit path only)
+    bytes_fused = w * (n * k + n * 2 * k * 2) + key_word * N * D * 2 * k  # target residues, base read, out written, keys
     cta_digits = n * 2 * k * D
     l2_u64, l2_packed = cta_digits * (8.0 * N + 8.0 * N), cta_digits * (8.0 * N + 6.0 * N)  # source + keys, per key form
     rec = {"n": n, "path": "fused" if fused else "digits", "ms": round(ms, 3), "us_per_ct": round(ms * 1e3 / n, 2), "families_ms": fam,
-           "hbm_bytes": {"digits_path": bytes_digits + bytes_inverse, "fused_path": bytes_fused + bytes_inverse}}
+           "hbm_bytes": {"digits_path": bytes_digits + bytes_inverse, "fused_path": bytes_fused}}
     if fused and fam.get("keyswitch_mac"):
         rate = DP_WARP_INSTR_PER_CT * n / (fam["keyswitch_mac"] * 1e-3)
         rec["fused_fp64_warp_instr_per_s"] = float("%.4g" % rate)
