@@ -32,6 +32,13 @@ _SIGS = {
     "cnhe_context_load": [C.c_void_p, sz, i32, C.POINTER(C.c_void_p)],
     "cnhe_keys_save_compact": [C.c_void_p, i32, U64P, i32, C.c_void_p, sz, C.POINTER(sz)],
     "cnhe_context_load_compact": [C.c_void_p, sz, i32, C.POINTER(C.c_void_p)],
+    "cnhe_context_add_client_compact": [C.c_void_p, C.c_void_p, sz, C.POINTER(i32)],
+    "cnhe_context_remove_client": [C.c_void_p, i32],
+    "cnhe_vec_set_key_slot": [VECP, i32],
+    "cnhe_vec_key_slot": [VECP, C.POINTER(i32)],
+    "cnhe_vecs_rotate": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
+    "cnhe_vecs_stack_batch": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
+    "cnhe_mat_mul_rowmajor_batch": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_vec_write": [C.c_void_p, VECP, C.c_void_p, sz, C.POINTER(sz)],
     "cnhe_vec_read": [C.c_void_p, C.c_char_p, sz, C.POINTER(VECP), C.POINTER(sz)],
     "cnhe_keys_generate_secure": [C.c_void_p],

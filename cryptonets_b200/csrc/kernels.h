@@ -63,9 +63,11 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
 // (mod q_l, canonical), key [D][2][k][N] canonical NTT form, base polynomial p of ciphertext c at base + c * base_stride + p * k * N, out
 // packed [n_ct][2][k][N] -- what launch_ntt_forward_digits, launch_ks_mac_fp(lazy) and launch_ntt_inverse_add compute, with no digit
 // buffer and no accumulator.  out must overlap neither the target nor the base words: other CTAs still read them while one writes.
-// key_packed: nullptr, or the copy of `key` made by launch_pack_keys48 (every q_l < 2^48), which the kernel then reads instead
-cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *base, size_t base_stride,
-                                    u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s);
+// key_packed: nullptr, or the copy of `key` made by launch_pack_keys48 (every q_l < 2^48), which the kernel then reads instead.
+// key_tab: nullptr, or a device table of n_ct key bases (ciphertext c reads key_tab[c] in place of key, or of key_packed when that is set)
+cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab,
+                                    const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn,
+                                    const NttTab *tabs, cudaStream_t s);
 // the fused key switch's packed key copy: n_polys canonical N-word polynomials (words < 2^48) -> 6N bytes each, thread-interleaved (ntt.cu)
 cudaError_t launch_pack_keys48(const u64 *key, uint4 *out, int n_polys, int logn, cudaStream_t s);
 // dst[b] = INTT(src[b]) + base[(b / base_group) * base_stride + (b % base_group) * N]  (mod p)
@@ -192,10 +194,12 @@ cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int
 cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s);
 // folded constants + software-pipelined loads (lazy input only)
 cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s);
-cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, u64 *acc, int n, int D, int k, int logn, const BehzConstF *f, int lazy,
-                             cudaStream_t s);
+cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,
+                             const BehzConstF *f, int lazy, cudaStream_t s);
 // ---- K6: key-switch inner product. digits [n][D][k][N] (NTT), key [D][2][k][N] (NTT) -> acc [n][2][k][N] (NTT)
-cudaError_t launch_ks_mac(const u64 *digits, const u64 *key, u64 *acc, int n, int D, int k, int logn, const BehzConst *bc, cudaStream_t s);
+// key_tab: nullptr, or a device table of n key bases (ciphertext c reads key_tab[c] in place of key)
+cudaError_t launch_ks_mac(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn, const BehzConst *bc,
+                          cudaStream_t s);
 // split a size-3 array [n][3][k][N] view: base[n][2][k][N] = (c0,c1), c2[n][k][N]
 
 // ---- sampling / encode / encrypt / decrypt

@@ -1069,6 +1069,8 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
 // fetched from L2 again before the thread's next load uses their second half.  The packed copy holds the same words in 6 bytes each,
 // laid out [D][2][k][half][6][TR] in 16-byte groups: group g of thread j is its bytes 16g..16g+15, so a warp's load is 512 contiguous
 // bytes and a thread reads 96 B instead of 128.
+// key_tab: nullptr (every ciphertext uses key / keyp), or a device table of one key base per ciphertext -- packed copies with PK, u64
+// keys without -- for calls whose ciphertexts belong to different key slots.  Same grid, same arithmetic either way.
 template <int HLOGN>
 __host__ __device__ constexpr int ks_fused_threads() { return (1 << HLOGN) / 16; }
 template <int HLOGN>
@@ -1099,7 +1101,8 @@ __global__ void __launch_bounds__(256) k_pack_keys48(const u64 *__restrict__ key
 template <int HLOGN, bool PK>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(ks_fused_threads<HLOGN>(), HLOGN == 12 ? 2 : 4)
 k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *__restrict__ key, const uint4 *__restrict__ keyp,
-                   const u64 *__restrict__ base, size_t base_stride, u64 *__restrict__ out, const NttTab *__restrict__ tabs, int k, DigitMap dm) {
+                   const u64 *const *__restrict__ key_tab, const u64 *__restrict__ base, size_t base_stride, u64 *__restrict__ out,
+                   const NttTab *__restrict__ tabs, int k, DigitMap dm) {
     constexpr int H = 1 << HLOGN, TR = ks_fused_threads<HLOGN>(), N = 2 * H;
     constexpr int R1 = HLOGN - 8, E1 = 1 << R1, LG1 = HLOGN - R1; // first pass: stage 0 on the loads, then R1 stages; then 4 + 4
     extern __shared__ __align__(16) u64 ks_raw[];
@@ -1116,6 +1119,10 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
     const bool need_reduce = dm.mask >= tb.mod.p;
     const u64 *src_c = target + (size_t)c * ct_stride;
     const size_t kpoly = (size_t)k * N, kstride = 2 * kpoly;
+    if (key_tab) { // per-ciphertext keys (several clients' key slots in one call): the table holds the form this instantiation reads
+        if constexpr (PK) keyp = reinterpret_cast<const uint4 *>(key_tab[c]);
+        else key = key_tab[c];
+    }
     const u64 *key_l = key + (size_t)l * N + half * H + 16 * tid;
     load_twiddle_cache(twc, tb.wd, tid, TR);
     load_twiddle_cache(twci, tb.iwd, tid, TR);
@@ -1753,25 +1760,28 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
     return cudaGetLastError();
 }
 template <int HL, bool PK>
-static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, const u64 *base, size_t base_stride,
-                                   u64 *out, int n_ct, int k, const DigitMap &dm, const NttTab *tabs, cudaStream_t s) {
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, const u64 *const *key_tab,
+                                   const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, const NttTab *tabs,
+                                   cudaStream_t s) {
     cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL, PK>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
     if (e != cudaSuccess) return e;
-    k_key_switch_fused<HL, PK><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, key, keyp, base, base_stride, out,
-                                                                                               tabs, k, dm);
+    k_key_switch_fused<HL, PK><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, key, keyp, key_tab, base,
+                                                                                               base_stride, out, tabs, k, dm);
     return cudaGetLastError();
 }
 template <int HL>
-static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, const u64 *base, size_t base_stride,
-                                   u64 *out, int n_ct, int k, const DigitMap &dm, const NttTab *tabs, cudaStream_t s) {
-    return keyp ? launch_ks_fused<HL, true>(target, ct_stride, key, keyp, base, base_stride, out, n_ct, k, dm, tabs, s)
-                : launch_ks_fused<HL, false>(target, ct_stride, key, keyp, base, base_stride, out, n_ct, k, dm, tabs, s);
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, const u64 *const *key_tab,
+                                   const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, const NttTab *tabs,
+                                   cudaStream_t s) {
+    return keyp ? launch_ks_fused<HL, true>(target, ct_stride, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s)
+                : launch_ks_fused<HL, false>(target, ct_stride, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
 }
-cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *base, size_t base_stride,
-                                    u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s) {
+cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab,
+                                    const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn,
+                                    const NttTab *tabs, cudaStream_t s) {
     if (n_ct <= 0) return cudaSuccess;
-    if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, key_packed, base, base_stride, out, n_ct, k, dm, tabs, s);
-    if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, key_packed, base, base_stride, out, n_ct, k, dm, tabs, s);
+    if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+    if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
     return cudaErrorInvalidValue;
 }
 template <int HL>

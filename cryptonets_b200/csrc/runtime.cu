@@ -37,7 +37,7 @@ void Context::note(OpKind kind, int channel, int n, const u64 *first_out, const 
     if (!trace_noise || kind == OP_ADD_MANY_ITEMS) return;
     int budget = -1;
     const int b0 = in0 ? known_budget(in0) : -1, b1 = in1 ? known_budget(in1) : -1; // before the output (possibly in place) is re-measured
-    if (first_out && channel >= 0 && channel < P && ch[channel].have_sk) {
+    if (first_out && channel >= 0 && channel < P && ch[channel].have_sk && !foreign) { // other slots' ciphertexts: only slot 0's key is here
         budget = op_noise_budget(*this, channel, first_out);
         // the call wrote n ciphertexts starting here: whatever was recorded for these addresses (recycled blocks) is stale now
         budget_of.erase(budget_of.lower_bound(first_out), budget_of.lower_bound(first_out + (size_t)n * ct_words()));
@@ -266,6 +266,7 @@ Context::~Context() {
     recycle_on = false; // buffers released from here on go straight back to the driver
     temps.clear();
     ch.clear();
+    clients.clear(); // key slots: their buffers hold this context as owner, so they go before it does
     drop_recycled();
     if (d_bc) cudaFree(d_bc);
     if (d_bf) cudaFree(d_bf);
@@ -781,9 +782,66 @@ static bool ks_fused(const Context &c, int n) {
 static bool spans_overlap(const u64 *a, size_t a_words, const u64 *b, size_t b_words) { return a < b + b_words && b < a + a_words; }
 // out[i] = (base_i + sum_d NTT^-1(NTT(digit_d(target_i)) * key_d)): ciphertext i's target polynomial (k residues) is at
 // target + i * target_stride, its base (2 polynomials) at base + i * base_stride; out is packed [n][2][k][N]
-void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, const u64 *key, const DigitMap &dm, const u64 *base,
-                   size_t base_stride, u64 *out, const u64 *key_packed) {
+const KeySet &Context::keys(int channel, int s) const {
+    if (!slot_live(s)) throw Error(-1, "no such key slot");
+    return s == 0 ? ch[channel] : clients[s - 1][channel];
+}
+KsKeys KsKeys::slice(int c0, int m) const {
+    KsKeys r = *this;
+    if (!per_ct()) return r;
+    r.keys.assign(keys.begin() + c0, keys.begin() + c0 + m);
+    if (!packs.empty()) r.packs.assign(packs.begin() + c0, packs.begin() + c0 + m);
+    return r;
+}
+// collects each ciphertext's key set (per-ciphertext table or the call's slot) into KsKeys; a call of one slot stays uniform
+template <class Pick>
+static KsKeys pick_keys(Context &c, int ch, int n, const int *slots, Pick pick) {
+    KsKeys r;
+    if (slots) {
+        bool uniform = true;
+        for (int i = 0; i < n; i++) uniform = uniform && slots[i] == slots[0];
+        if (!uniform) {
+            bool packed = true;
+            for (int i = 0; i < n; i++) {
+                const u64 *key, *pk;
+                pick(c.keys(ch, slots[i]), key, pk);
+                r.keys.push_back(key);
+                r.packs.push_back(pk);
+                packed = packed && pk;
+            }
+            if (!packed) r.packs.clear();
+            return r;
+        }
+    }
+    pick(c.keys(ch, slots && n ? slots[0] : c.slot), r.key, r.packed);
+    return r;
+}
+KsKeys relin_keys(Context &c, int ch, int n, const int *slots) {
+    return pick_keys(c, ch, n, slots, [](const KeySet &ks, const u64 *&key, const u64 *&pk) {
+        if (!ks.have_rlk) throw Error(-3, "relinearization keys are missing");
+        key = ks.rlk->p;
+        pk = ks.rlk_packed ? ks.rlk_packed->p : nullptr;
+    });
+}
+KsKeys galois_keys(Context &c, int ch, int n, const int *slots, u64 elt) {
+    return pick_keys(c, ch, n, slots, [elt](const KeySet &ks, const u64 *&key, const u64 *&pk) {
+        auto it = ks.glk.find(elt);
+        if (it == ks.glk.end()) throw Error(-3, "Galois key not present");
+        key = it->second->p;
+        pk = nullptr;
+    });
+}
+// whether every ciphertext's key slot holds the Galois key of elt
+static bool has_galois(const Context &c, int ch, int n, const int *slots, u64 elt) {
+    if (!slots) return c.keys(ch, c.slot).glk.count(elt) != 0;
+    for (int i = 0; i < n; i++)
+        if (!c.keys(ch, slots[i]).glk.count(elt)) return false;
+    return true;
+}
+void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, const KsKeys &keys, const DigitMap &dm, const u64 *base,
+                   size_t base_stride, u64 *out) {
     const int k = c.k;
+    const u64 *key_packed = keys.per_ct() ? (keys.packs.empty() ? nullptr : keys.packs[0]) : keys.packed;
     const size_t N = c.N;
     const int fpq = fp_range(c, 0, k);
     const bool lazy = c.lazy && fpq;
@@ -796,13 +854,19 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
     for (int c0 = 0; c0 < n; c0 += wave) {
         WsScope scope(c);
         const int m = std::min(wave, n - c0);
+        // a call of several key slots passes one key base per ciphertext (the packed copies when every slot has one)
+        const u64 *const *key_tab = nullptr;
+        if (keys.per_ct()) {
+            const std::vector<const u64 *> &tab = fused && key_packed ? keys.packs : keys.keys;
+            key_tab = upload_ptrs(c, std::vector<const u64 *>(tab.begin() + c0, tab.begin() + c0 + m));
+        }
         if (fused) {
             // HBM: the target residues once (the pair and the other residues' CTAs share them through L2), the keys once, the output.  The
             // base words the epilogue adds (another 8N bytes per output polynomial, mostly prefetched) are not booked: the figure keeps the
             // meaning it had when the kernel wrote an accumulator of the output's size
             PROF(3, 8.0 * N * ((double)m * k + (double)m * 2 * k) + (key_packed ? 6.0 : 8.0) * N * dm.D * 2 * k);
-            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, key, reinterpret_cast<const uint4 *>(key_packed),
-                                            base + (size_t)c0 * base_stride, base_stride, out + (size_t)c0 * 2 * k * N, m, k, dm, c.logN, c.d_tabs, c.stream),
+            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, keys.key, reinterpret_cast<const uint4 *>(key_packed),
+                                            key_tab, base + (size_t)c0 * base_stride, base_stride, out + (size_t)c0 * 2 * k * N, m, k, dm, c.logN, c.d_tabs, c.stream),
                     "key_switch_fused");
             continue;
         }
@@ -816,8 +880,8 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
                         "ntt_forward_digits");
             }
             PROF(3, 8.0 * N * ((double)m * dm.D * k + (double)dm.D * 2 * k + (double)m * 2 * k));
-            if (c.fp_elementwise) c.check(launch_ks_mac_fp(digits, key, acc, m, dm.D, k, c.logN, &c.h_bf, lazy, c.stream), "ks_mac_fp");
-            else c.check(launch_ks_mac(digits, key, acc, m, dm.D, k, c.logN, c.d_bc, c.stream), "ks_mac");
+            if (c.fp_elementwise) c.check(launch_ks_mac_fp(digits, keys.key, key_tab, acc, m, dm.D, k, c.logN, &c.h_bf, lazy, c.stream), "ks_mac_fp");
+            else c.check(launch_ks_mac(digits, keys.key, key_tab, acc, m, dm.D, k, c.logN, c.d_bc, c.stream), "ks_mac");
         }
         PROF(1, 24.0 * N * m * 2 * k);
         c.check(launch_ntt_inverse_add(acc, base + (size_t)c0 * base_stride, 2 * k, base_stride, out + (size_t)c0 * 2 * k * N, m * 2 * k, c.logN,
@@ -914,19 +978,18 @@ void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const st
     }
     c.note(Context::OP_MULTIPLY, ch, n);
 }
-void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2) {
-    if (!c.ch[ch].have_rlk) throw Error(-3, "relinearization keys are missing");
+void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots) {
+    const KsKeys keys = relin_keys(c, ch, n, slots);
     const int k = c.k;
     const size_t N = c.N;
     // the size-3 layout [c0 c1 c2] is consumed in place: c2 is the key-switch target, (c0, c1) the base it is added to
     const size_t s3 = (size_t)3 * k * N;
-    const BufRef &pk = c.ch[ch].rlk_packed;
-    op_key_switch(c, in3 + (size_t)2 * k * N, s3, n, c.ch[ch].rlk->p, c.dm_relin, in3, s3, out2, pk ? pk->p : nullptr);
+    op_key_switch(c, in3 + (size_t)2 * k * N, s3, n, keys, c.dm_relin, in3, s3, out2);
     c.note(Context::OP_RELINEARIZE, ch, n, out2);
 }
-void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2) {
-    if (!c.ch[ch].have_rlk) throw Error(-3, "relinearization keys are missing");
+void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2, const int *slots) {
     const int n = (int)a.size(), k = c.k;
+    const KsKeys keys = relin_keys(c, ch, n, slots);
     const size_t N = c.N;
     const bool fused = mul_fused(c, a, b);
     const int wave = c.wave((ks_fused(c, n) ? 0 : (size_t)c.dm_relin.D * k * N) + mul_words(c, fused) + 5 * k * N);
@@ -936,8 +999,7 @@ void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, co
         u64 *ct3 = c.ws_alloc((size_t)m * 3 * k * N);
         multiply_chunk(c, ch, a, b, c0, m, ct3, fused);
         const size_t s3 = (size_t)3 * k * N;
-        const BufRef &pk = c.ch[ch].rlk_packed;
-        op_key_switch(c, ct3 + (size_t)2 * k * N, s3, m, c.ch[ch].rlk->p, c.dm_relin, ct3, s3, out2 + (size_t)c0 * 2 * k * N, pk ? pk->p : nullptr);
+        op_key_switch(c, ct3 + (size_t)2 * k * N, s3, m, keys.slice(c0, m), c.dm_relin, ct3, s3, out2 + (size_t)c0 * 2 * k * N);
     }
     c.op_count[Context::OP_MULTIPLY] += (uint64_t)n;
     c.note(Context::OP_RELINEARIZE, ch, n, out2, a[0], b[0]);
@@ -954,9 +1016,8 @@ u64 galois_elt_from_step(const Context &c, int steps) { // Evaluator::galois_elt
     for (u64 i = 0; i < s; i++) e = (e * 3) & (m - 1);
     return e;
 }
-void op_apply_galois(Context &c, int ch, const u64 *in, int n, u64 elt, u64 *out, bool add_back) {
-    auto it = c.ch[ch].glk.find(elt);
-    if (it == c.ch[ch].glk.end()) throw Error(-3, "Galois key not present");
+void op_apply_galois(Context &c, int ch, const u64 *in, int n, u64 elt, u64 *out, bool add_back, const int *slots) {
+    const KsKeys keys = galois_keys(c, ch, n, slots, elt);
     const int k = c.k;
     const size_t N = c.N;
     const u64 m2 = 2ULL * N;
@@ -967,18 +1028,18 @@ void op_apply_galois(Context &c, int ch, const u64 *in, int n, u64 elt, u64 *out
         const int m = std::min(c.chunk, n - c0);
         u64 *base = c.ws_alloc((size_t)m * 2 * k * N), *p1 = c.ws_alloc((size_t)m * k * N);
         c.check(launch_galois(in + (size_t)c0 * 2 * k * N, base, p1, m, einv, k, c.logN, c.d_bc, c.stream, add_back ? 1 : 0), "galois");
-        op_key_switch(c, p1, (size_t)k * N, m, it->second->p, c.dm_galois, base, (size_t)2 * k * N, out + (size_t)c0 * 2 * k * N);
+        op_key_switch(c, p1, (size_t)k * N, m, keys.slice(c0, m), c.dm_galois, base, (size_t)2 * k * N, out + (size_t)c0 * 2 * k * N);
     }
     c.note(elt == m2 - 1 ? Context::OP_ROTATE_COLUMNS : Context::OP_ROTATE_ROWS_HOP, ch, n, out, in);
     if (add_back) c.note(Context::OP_ADD, ch, n, out, in, out); // the reference issues Rotate + Add: both are counted
 }
 // x + rotate(x) in one pass (in == out allowed): the permutation kernel folds the unrotated ciphertext into the key switch's base.  Returns
 // false when the step has no key of its own (multi-hop rotation) or per-operation noise tracing wants the rotated ciphertext on its own.
-bool op_rotate_add(Context &c, int ch, const u64 *in, int n, int steps, bool columns, u64 *out) {
+bool op_rotate_add(Context &c, int ch, const u64 *in, int n, int steps, bool columns, u64 *out, const int *slots) {
     if (c.trace_noise) return false;
     const u64 elt = columns ? 2ULL * c.N - 1 : galois_elt_from_step(c, steps);
-    if (!c.ch[ch].glk.count(elt)) return false;
-    op_apply_galois(c, ch, in, n, elt, out, true);
+    if (!has_galois(c, ch, n, slots, elt)) return false;
+    op_apply_galois(c, ch, in, n, elt, out, true, slots);
     return true;
 }
 static std::vector<int> naf(int value) { // non-adjacent form, least significant term first (SEAL util::naf)
@@ -992,32 +1053,33 @@ static std::vector<int> naf(int value) { // non-adjacent form, least significant
     }
     return res;
 }
-void op_rotate_rows(Context &c, int ch, const u64 *in, int n, int steps, u64 *out) { // Evaluator::rotate_internal
+void op_rotate_rows(Context &c, int ch, const u64 *in, int n, int steps, u64 *out, const int *slots) { // Evaluator::rotate_internal
     const size_t words = (size_t)n * c.ct_words();
     if (steps == 0) {
         if (in != out) { CNHE_CUDA(cudaMemcpyAsync(out, in, words * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(out, in); }
         return;
     }
     const u64 elt = galois_elt_from_step(c, steps);
-    if (c.ch[ch].glk.count(elt)) { op_apply_galois(c, ch, in, n, elt, out); return; }
+    if (has_galois(c, ch, n, slots, elt)) { op_apply_galois(c, ch, in, n, elt, out, false, slots); return; }
     std::vector<int> hops = naf(steps);
     if (hops.size() == 1) throw Error(-3, "Galois key not present");
     const u64 *cur = in;
     for (size_t h = 0; h < hops.size(); h++) {
         if ((size_t)std::abs(hops[h]) == (c.N >> 1)) continue;
         u64 *nxt = (h + 1 == hops.size()) ? out : c.ws_alloc(words);
-        op_rotate_rows(c, ch, cur, n, hops[h], nxt);
+        op_rotate_rows(c, ch, cur, n, hops[h], nxt, slots);
         cur = nxt;
     }
     if (cur != out) { CNHE_CUDA(cudaMemcpyAsync(out, cur, words * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(out, cur); }
 }
-void op_rotate_columns(Context &c, int ch, const u64 *in, int n, u64 *out) { op_apply_galois(c, ch, in, n, 2ULL * c.N - 1, out); }
+void op_rotate_columns(Context &c, int ch, const u64 *in, int n, u64 *out, const int *slots) {
+    op_apply_galois(c, ch, in, n, 2ULL * c.N - 1, out, false, slots);
+}
 
 // apply_galois on n ciphertexts scattered in memory (pointer table) -> packed out[n]
-static void apply_galois_gather(Context &c, int ch, const std::vector<const u64 *> &ins, u64 elt, u64 *out) {
-    auto it = c.ch[ch].glk.find(elt);
-    if (it == c.ch[ch].glk.end()) throw Error(-3, "Galois key not present");
+static void apply_galois_gather(Context &c, int ch, const std::vector<const u64 *> &ins, u64 elt, u64 *out, const int *slots) {
     const int k = c.k, n = (int)ins.size();
+    const KsKeys keys = galois_keys(c, ch, n, slots, elt);
     const size_t N = c.N;
     const u64 m2 = 2ULL * N;
     u64 einv = 0;
@@ -1028,7 +1090,7 @@ static void apply_galois_gather(Context &c, int ch, const std::vector<const u64 
         std::vector<const u64 *> part(ins.begin() + c0, ins.begin() + c0 + m);
         u64 *base = c.ws_alloc((size_t)m * 2 * k * N), *p1 = c.ws_alloc((size_t)m * k * N);
         c.check(launch_galois_gather(upload_ptrs(c, part), base, p1, m, einv, k, c.logN, c.d_bc, c.stream), "galois");
-        op_key_switch(c, p1, (size_t)k * N, m, it->second->p, c.dm_galois, base, (size_t)2 * k * N, out + (size_t)c0 * 2 * k * N);
+        op_key_switch(c, p1, (size_t)k * N, m, keys.slice(c0, m), c.dm_galois, base, (size_t)2 * k * N, out + (size_t)c0 * 2 * k * N);
     }
     c.op_count[elt == m2 - 1 ? Context::OP_ROTATE_COLUMNS : Context::OP_ROTATE_ROWS_HOP] += (uint64_t)n;
     if (c.trace_noise) // one record per ciphertext, as the unbatched path would have written
@@ -1041,13 +1103,15 @@ void op_rotate_rows_multi(Context &c, int ch, const std::vector<RotateJob> &jobs
     const size_t ctw = c.ct_words();
     struct State { std::vector<int> hops; size_t next; const u64 *cur; };
     std::vector<State> st(jobs.size());
+    std::vector<int> slots(jobs.size());
+    for (size_t j = 0; j < jobs.size(); j++) slots[j] = jobs[j].slot < 0 ? c.slot : jobs[j].slot;
     for (size_t j = 0; j < jobs.size(); j++) {
         const RotateJob &job = jobs[j];
         st[j].next = 0;
         st[j].cur = job.src;
         if (job.steps == 0) continue;
         const u64 elt = galois_elt_from_step(c, job.steps);
-        if (c.ch[ch].glk.count(elt)) st[j].hops = {job.steps};
+        if (has_galois(c, ch, (int)slots.size(), slots.data(), elt)) st[j].hops = {job.steps};
         else {
             for (int h : naf(job.steps))
                 if ((size_t)std::abs(h) != (c.N >> 1)) st[j].hops.push_back(h); // rotate_internal skips a hop of exactly N/2
@@ -1065,9 +1129,10 @@ void op_rotate_rows_multi(Context &c, int ch, const std::vector<RotateJob> &jobs
             if (it->second.size() > best->second.size()) best = it;
         const std::vector<size_t> &js = best->second;
         std::vector<const u64 *> ins;
-        for (size_t j : js) ins.push_back(st[j].cur);
+        std::vector<int> in_slots;
+        for (size_t j : js) { ins.push_back(st[j].cur); in_slots.push_back(slots[j]); }
         u64 *out = c.ws_alloc(js.size() * ctw);
-        apply_galois_gather(c, ch, ins, galois_elt_from_step(c, best->first), out);
+        apply_galois_gather(c, ch, ins, galois_elt_from_step(c, best->first), out, in_slots.data());
         for (size_t i = 0; i < js.size(); i++) {
             st[js[i]].cur = out + i * ctw;
             st[js[i]].next++;
@@ -1341,8 +1406,8 @@ BufRef &key_slot(Context &c, int channel, int what, u64 arg, size_t &words, bool
     if (!*slot) throw Error(-3, "key is missing");
     return *slot;
 }
-void rlk_ready(Context &c, int channel) {
-    Channel &ch = c.ch[channel];
+void rlk_ready(Context &c, int channel) { rlk_ready(c, c.ch[channel]); }
+void rlk_ready(Context &c, KeySet &ch) {
     ch.have_rlk = true;
     ch.rlk_packed.reset();
     bool small = true;
@@ -1494,20 +1559,39 @@ void op_keys_save_compact(Context &c, int chi, int sets, const std::vector<u64> 
         emit(rs, &c.dm_galois);
     }
 }
-void op_keys_load_compact(Context &c, int chi, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key) {
+// pairs of one blob channel in order: public key, relinearisation digits, Galois digits of each element; `slot_of` gives each set's key buffer
+template <class SlotOf>
+static void keys_load_compact(Context &c, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key, SlotOf slot_of,
+                              bool skip_pk = false) {
     const CompactShape sh = compact_shape(c);
     u64 kappa = 0;
     auto expand = [&](int what, u64 arg) {
         size_t words;
-        BufRef &slot = key_slot(c, chi, what, arg, words, true);
+        BufRef &slot = slot_of(what, arg, words);
         const int D = (int)(words / c.ct_words());
         c.check(launch_compact_expand(slot->p, packed + kappa * sh.off[c.k], key, PURPOSE_KEYS_A, kappa, D, sh, c.d_bc, c.stream), "compact_expand");
         kappa += D;
     };
-    if (sets & 1) { expand(1, 0); c.ch[chi].have_pk = true; }
+    if (sets & 1) {
+        if (skip_pk) kappa += 1; // a key slot evaluates only: the public key pair is left in the blob
+        else expand(1, 0);
+    }
     if (sets & 2) expand(2, 0);
     for (u64 elt : elts) expand(3, elt);
+}
+void op_keys_load_compact(Context &c, int chi, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key) {
+    keys_load_compact(c, sets, elts, packed, key, [&](int what, u64 arg, size_t &words) -> BufRef & { return key_slot(c, chi, what, arg, words, true); });
+    if (sets & 1) c.ch[chi].have_pk = true;
     if (sets & 2) rlk_ready(c, chi); // synchronises the channel's stream
+}
+void op_keys_load_compact(Context &c, KeySet &dst, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key) {
+    keys_load_compact(c, sets, elts, packed, key, [&](int what, u64 arg, size_t &words) -> BufRef & {
+        BufRef &b = what == 2 ? dst.rlk : dst.glk[arg];
+        words = (size_t)(what == 2 ? c.dm_relin.D : c.dm_galois.D) * c.ct_words();
+        if (!b) b = c.alloc(words);
+        return b;
+    }, true);
+    if (sets & 2) rlk_ready(c, dst); // synchronises the stream
 }
 
 void keys_generate(Context &c, u64 seed) { keys_generate_impl(c, false, seed); }

@@ -37,14 +37,19 @@ struct DevBuf {
 };
 typedef std::shared_ptr<DevBuf> BufRef;
 
-struct Channel { // one plaintext modulus (one AtomicSealBfvEncryptedEnvironment)
+// the evaluation keys of one client under one plaintext modulus
+struct KeySet {
+    bool have_rlk = false;
+    BufRef rlk;
+    BufRef rlk_packed; // rlk with 48-bit words for the fused key switch (set by rlk_ready when that kernel can run and every q_l < 2^48)
+    std::map<u64, BufRef> glk;
+};
+struct Channel : KeySet { // one plaintext modulus (one AtomicSealBfvEncryptedEnvironment); its own keys are key slot 0
     u64 t = 0;
     PlainConst pc;
     int mod_id = 0; // NTT table id of t
-    bool have_sk = false, have_pk = false, have_rlk = false;
-    BufRef sk, pk, rlk;
-    BufRef rlk_packed; // rlk with 48-bit words for the fused key switch (set by rlk_ready when that kernel can run and every q_l < 2^48)
-    std::map<u64, BufRef> glk;
+    bool have_sk = false, have_pk = false;
+    BufRef sk, pk;
     RngKey rng;    // secure (ChaCha20 keyed from the OS) unless a deterministic test seed was requested explicitly
     u64 nonce = 1; // running encryption counter (32 bits enter the stream id; a secure channel re-keys before it wraps)
     FloorConstF floor_f; // folded fast_floor constants for this t (valid when the context's fp_elementwise is set)
@@ -69,6 +74,13 @@ struct Context {
     DigitMap dm_relin, dm_galois;
     std::vector<u64> galois_elts;
     std::vector<Channel> ch;
+    // Key slots: slot 0 is the channels' own keys, slot s >= 1 another client's evaluation keys, clients[s - 1][channel] (an empty entry
+    // is a removed slot).  Every ciphertext is bound to one slot; a key switch takes each ciphertext's keys from its slot.
+    std::vector<std::vector<KeySet>> clients;
+    int slot = 0; // key slot of the ciphertexts the current public call works on (reset to 0 by every call; vec.cu sets it from the operands)
+    bool foreign = false; // the current call touches ciphertexts of a slot other than 0: the noise trace cannot measure them (no secret key)
+    bool slot_live(int s) const { return s == 0 || (s > 0 && (size_t)s <= clients.size() && !clients[s - 1].empty()); }
+    const KeySet &keys(int channel, int s) const;
     // one CUDA stream per plaintext-modulus channel (the reference runs one Task per prime, EncryptedSealBfvVector.cs:225-236):
     // channels are independent until decryption, so their kernels and host<->device copies overlap.  `stream` is the stream of the
     // channel currently being issued (set_channel).
@@ -190,6 +202,7 @@ BufRef &key_slot(Context &c, int channel, int what, u64 arg, size_t &words, bool
 // marks a channel's relinearisation keys present once they are written to its rlk slot (generated or loaded), and rebuilds the packed
 // copy the fused key switch reads; returns once that copy is complete
 void rlk_ready(Context &c, int channel);
+void rlk_ready(Context &c, KeySet &ks); // the same for a key slot's key set
 
 // ---- ciphertext-array operations (all asynchronous on c.stream; device pointers)
 // upload a host array of device pointers into workspace memory
@@ -199,20 +212,33 @@ u64 *const *upload_ptrs_mut(Context &c, const std::vector<u64 *> &ptrs);
 void op_ntt(Context &c, const u64 *src, u64 *dst, int n_polys, int mod_base, int mod_count, bool inverse);
 // out3[n][3][k][N] = a[i] * b[i]  (BEHZ).  a_ptrs/b_ptrs: host vectors of device ciphertext pointers.
 void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3);
-void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2);
-void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2);
-// key_packed: the channel's rlk_packed for relinearisation (nullptr: the fused kernel reads the u64 keys)
-void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, const u64 *key, const DigitMap &dm, const u64 *base,
-                   size_t base_stride, u64 *out, const u64 *key_packed = nullptr);
-void op_apply_galois(Context &c, int ch, const u64 *in, int n, u64 elt, u64 *out, bool add_back = false);
-bool op_rotate_add(Context &c, int ch, const u64 *in, int n, int steps, bool columns, u64 *out); // out = in + rotate(in) in one pass, if possible
-void op_rotate_rows(Context &c, int ch, const u64 *in, int n, int steps, u64 *out); // steps == 0 copies
-void op_rotate_columns(Context &c, int ch, const u64 *in, int n, u64 *out);
+// Key-switching operations take the keys of ciphertext i from key slot slots[i] when a per-ciphertext slot table is given (n entries,
+// host), otherwise every ciphertext uses the call's slot c.slot.  A missing key is CNHE_ERR_STATE.
+void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots = nullptr);
+void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2,
+                       const int *slots = nullptr);
+// the keys of a key switch: one set for every ciphertext, or one per ciphertext (several key slots in one call)
+struct KsKeys {
+    const u64 *key = nullptr, *packed = nullptr; // uniform call; packed: the 48-bit copy for the fused kernel (nullptr: u64 keys)
+    std::vector<const u64 *> keys, packs;        // per ciphertext (empty: uniform); packs empty when some key has no packed copy
+    bool per_ct() const { return !keys.empty(); }
+    KsKeys slice(int c0, int m) const;
+};
+KsKeys relin_keys(Context &c, int ch, int n, const int *slots);
+KsKeys galois_keys(Context &c, int ch, int n, const int *slots, u64 elt);
+void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, const KsKeys &keys, const DigitMap &dm, const u64 *base,
+                   size_t base_stride, u64 *out);
+void op_apply_galois(Context &c, int ch, const u64 *in, int n, u64 elt, u64 *out, bool add_back = false, const int *slots = nullptr);
+// out = in + rotate(in) in one pass, if possible
+bool op_rotate_add(Context &c, int ch, const u64 *in, int n, int steps, bool columns, u64 *out, const int *slots = nullptr);
+void op_rotate_rows(Context &c, int ch, const u64 *in, int n, int steps, u64 *out, const int *slots = nullptr); // steps == 0 copies
+void op_rotate_columns(Context &c, int ch, const u64 *in, int n, u64 *out, const int *slots = nullptr);
 // Many independent single-ciphertext row rotations with DIFFERENT step counts (Interleave / Stack / Duplicate rotate every vector by its
 // own offset): each job walks the hop sequence rotate_rows would take for it (exact key or NAF hops), and hops with the same Galois
 // element are batched across jobs into one key-switch wave.  Per ciphertext the operations and their order are exactly those of
-// op_rotate_rows, so the outputs are bit-identical.
-struct RotateJob { const u64 *src; int steps; u64 *dst; };
+// op_rotate_rows, so the outputs are bit-identical.  slot < 0: the call's slot.  A step takes its exact key only when every job's slot
+// holds it (the hops are planned from the elements the call's slots have in common).
+struct RotateJob { const u64 *src; int steps; u64 *dst; int slot = -1; };
 void op_rotate_rows_multi(Context &c, int ch, const std::vector<RotateJob> &jobs);
 u64 galois_elt_from_step(const Context &c, int steps);
 // dense plaintext (coefficient form mod t, [n or 1][N]) times ciphertexts [n][2kN]
@@ -244,6 +270,8 @@ size_t compact_key_pairs(const Context &c, int sets, size_t n_galois);
 void op_keys_save_compact(Context &c, int ch, int sets, const std::vector<u64> &elts, u64 nonce0, const CompactKey &key, u64 *packed);
 // packed b [pairs][off[k]] (device) + K_c -> the channel's key slots; returns once the keys are complete
 void op_keys_load_compact(Context &c, int ch, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key);
+// the same into a key slot's key set (relinearisation and Galois keys; a public key pair in the blob is skipped)
+void op_keys_load_compact(Context &c, KeySet &dst, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key);
 int op_noise_budget(Context &c, int ch, const u64 *ct);
 
 } // namespace cnhe

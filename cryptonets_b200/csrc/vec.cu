@@ -332,6 +332,7 @@ cnhe_vec *new_vec(Context &c, uint64_t dim, double scale, int format, bool enc, 
     v->scale = scale;
     v->format = format;
     v->enc = enc;
+    v->slot = c.slot;
     v->blocks = blocks;
     v->buf.resize(c.P);
     v->off.assign(c.P, 0);
@@ -347,6 +348,29 @@ static cnhe_vec *alias_of(const cnhe_vec *a) { return new cnhe_vec(*a); } // sha
 void same_ctx(Context &c, const cnhe_vec *v) {
     if (!v) fail("null vector");
     if (v->ctx != &c) fail("vector belongs to another context");
+}
+int use_slot(Context &c, const cnhe_vec *const *vs, int n) {
+    int s = -1;
+    for (int i = 0; i < n; i++) {
+        if (!vs[i] || !vs[i]->enc) continue;
+        if (s >= 0 && vs[i]->slot != s) fail("encrypted operands belong to different key slots");
+        s = vs[i]->slot;
+    }
+    if (s < 0) s = 0;
+    if (!c.slot_live(s)) fail("the vector's key slot was removed");
+    c.slot = s;
+    c.foreign = s != 0;
+    return s;
+}
+// key slot of each encrypted vector, checked against the context (layer entry points that serve several clients in one call)
+static std::vector<int> vec_slots(Context &c, const cnhe_vec *const *vs, int n) {
+    std::vector<int> s(n);
+    for (int i = 0; i < n; i++) {
+        s[i] = vs[i]->slot;
+        if (!c.slot_live(s[i])) fail("the vector's key slot was removed");
+        if (s[i] != 0) c.foreign = true;
+    }
+    return s;
 }
 // SplitBigNumbers ("EncryptedSealBfvVector.cs:352-365"): round(v*scale) -> +bigFactor if negative -> residues
 static void split_values(Context &c, const double *v, uint64_t n, double scale, std::vector<std::vector<u64>> &res) {
@@ -511,6 +535,7 @@ static void decrypt_channel(Context &c, const cnhe_vec *v, int ch, std::vector<u
     if (!v->enc && v->format == CNHE_SPARSE) { res = v->scalars[ch]; return; }
     u64 *plain;
     if (v->enc) {
+        if (v->slot != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
         plain = c.ws_alloc((size_t)v->blocks * N);
         op_decrypt(c, ch, v->ptr(ch), v->blocks, plain);
     } else plain = v->ptr(ch);
@@ -937,6 +962,77 @@ extern "C" int cnhe_context_load_compact(const uint8_t *blob, size_t len, int de
     } catch (const Error &e) { return set_err(e.code, e.what()); } catch (const std::exception &e) { return set_err(CNHE_ERR_INVALID, e.what()); }
     return CNHE_OK;
 }
+// ---------------------------------------------------------------------------------------------------- key slots (several clients)
+extern "C" int cnhe_context_add_client_compact(cnhe_ctx *h, const uint8_t *blob, size_t len, int *slot) {
+    API_BEGIN(h)
+    if (!blob || !slot) fail("null argument");
+    const KeyBlob kb = parse_compact_keys(blob, len); // every header field and the exact length, before anything is allocated
+    bool same = kb.N == c.N && (int)kb.k == c.k && (int)kb.P == c.P && (int)kb.dbc_relin == c.dbc_relin && (int)kb.dbc_galois == c.dbc_galois;
+    for (int l = 0; same && l < c.k; l++) same = kb.q[l] == c.q[l];
+    for (int ch = 0; same && ch < c.P; ch++) same = kb.t[ch] == c.t[ch];
+    if (!same) fail("compact key blob: parameters differ from the context's");
+    if (compact_key_pairs(c, (int)kb.sets, kb.elts.size()) * compact_shape(c).off[c.k] != kb.channel_words)
+        fail("compact key blob: key sizes do not match the context");
+    // slot numbers are never reused: a vector still bound to a removed slot is refused instead of meeting another client's keys
+    std::vector<KeySet> keys(c.P);
+    for (int ci = 0; ci < c.P && kb.channel_words; ci++) {
+        c.set_channel(ci);
+        u64 *stage = c.ws_alloc(kb.channel_words);
+        CNHE_CUDA(cudaMemcpyAsync(stage, blob + kb.header_bytes + (size_t)ci * kb.channel_words * 8, kb.channel_words * 8, cudaMemcpyHostToDevice,
+                                  c.stream));
+        op_keys_load_compact(c, keys[ci], (int)kb.sets, kb.elts, stage, kb.keys[ci]);
+        c.sync();
+        ws_release_all(c);
+    }
+    c.clients.push_back(std::move(keys));
+    *slot = (int)c.clients.size();
+    API_END
+}
+extern "C" int cnhe_context_remove_client(cnhe_ctx *h, int slot) {
+    API_BEGIN(h)
+    if (slot < 1 || !c.slot_live(slot)) fail("no such key slot");
+    c.sync(); // no queued key switch still reads the keys
+    c.clients[slot - 1].clear();
+    API_END
+}
+extern "C" int cnhe_vec_set_key_slot(cnhe_vec *v, int slot) {
+    if (!v) return set_err(CNHE_ERR_INVALID, "null vector");
+    std::lock_guard<std::recursive_mutex> lock(v->ctx->mu);
+    if (!v->enc) return set_err(CNHE_ERR_INVALID, "plain vectors have no key slot");
+    if (!v->ctx->slot_live(slot)) return set_err(CNHE_ERR_INVALID, "no such key slot");
+    v->slot = slot;
+    return CNHE_OK;
+}
+extern "C" int cnhe_vec_key_slot(const cnhe_vec *v, int *slot) {
+    if (!v || !slot) return set_err(CNHE_ERR_INVALID, "null argument");
+    *slot = v->enc ? v->slot : -1;
+    return CNHE_OK;
+}
+// Rotate (first block) of n vectors by the same amount, their key slots may differ: the hops of all vectors share each key-switch wave
+extern "C" int cnhe_vecs_rotate(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int amount, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n < 1 || !vecs || !out) fail("bad arguments");
+    for (int i = 0; i < n; i++) {
+        same_ctx(c, vecs[i]);
+        if (!vecs[i]->enc) fail("Rotate operates only on encrypted data");
+        if (vecs[i]->format == CNHE_SPARSE) fail("Rotate operates only on dense vectors");
+    }
+    const std::vector<int> slots = vec_slots(c, vecs, n);
+    std::vector<std::unique_ptr<cnhe_vec>> outs(n);
+    for (int i = 0; i < n; i++) {
+        outs[i].reset(new_vec(c, vecs[i]->dim, vecs[i]->scale, CNHE_DENSE, true, 1));
+        outs[i]->slot = slots[i];
+        alloc_channels(outs[i].get());
+    }
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        std::vector<RotateJob> jobs;
+        for (int i = 0; i < n; i++) jobs.push_back({vecs[i]->ptr(ch), amount, outs[i]->ptr(ch), slots[i]});
+        op_rotate_rows_multi(c, ch, jobs);
+    }
+    for (int i = 0; i < n; i++) out[i] = outs[i].release();
+    API_END
+}
 extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap) {
     API_BEGIN(h)
     if (n < 1 || !dst) fail("bad arguments");
@@ -1002,6 +1098,7 @@ extern "C" int cnhe_noise_budget(cnhe_ctx *h, const cnhe_vec *v, int channel, in
     API_BEGIN(h)
     same_ctx(c, v);
     if (!v->enc || channel < 0 || channel >= c.P || block < 0 || block >= v->blocks) fail("bad arguments");
+    if (v->slot != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
     *bits = op_noise_budget(c, channel, v->block(channel, block));
     API_END
 }
@@ -1064,12 +1161,14 @@ static cnhe_vec *addsub(Context &c, const cnhe_vec *a, const cnhe_vec *b, bool s
 extern "C" int cnhe_vec_add(cnhe_ctx *h, const cnhe_vec *a, const cnhe_vec *b, cnhe_vec **out) {
     API_BEGIN(h)
     same_ctx(c, a); same_ctx(c, b);
+    use_slot(c, {a, b});
     *out = addsub(c, a, b, false);
     API_END
 }
 extern "C" int cnhe_vec_sub(cnhe_ctx *h, const cnhe_vec *a, const cnhe_vec *b, cnhe_vec **out) {
     API_BEGIN(h)
     same_ctx(c, a); same_ctx(c, b);
+    use_slot(c, {a, b});
     *out = addsub(c, a, b, true);
     API_END
 }
@@ -1136,6 +1235,7 @@ static cnhe_vec *pointwise_multiply(Context &c, const cnhe_vec *a, const cnhe_ve
 extern "C" int cnhe_vec_pointwise_multiply(cnhe_ctx *h, const cnhe_vec *a, const cnhe_vec *b, cnhe_vec **out) {
     API_BEGIN(h)
     same_ctx(c, a); same_ctx(c, b);
+    use_slot(c, {a, b});
     *out = pointwise_multiply(c, a, b);
     API_END
 }
@@ -1194,12 +1294,14 @@ static cnhe_vec *sum_all_slots(Context &c, const cnhe_vec *a, uint64_t length, i
 extern "C" int cnhe_vec_sum_all_slots(cnhe_ctx *h, const cnhe_vec *a, uint64_t length, int force_column, cnhe_vec **out) {
     API_BEGIN(h)
     same_ctx(c, a);
+    use_slot(c, {a});
     *out = sum_all_slots(c, a, length, force_column);
     API_END
 }
 extern "C" int cnhe_vec_dot_product(cnhe_ctx *h, const cnhe_vec *a, const cnhe_vec *b, uint64_t length, int force_column, cnhe_vec **out) {
     API_BEGIN(h)
     same_ctx(c, a); same_ctx(c, b);
+    use_slot(c, {a, b});
     std::unique_ptr<cnhe_vec> mul(pointwise_multiply(c, a, b)); // AtomicSealBfvVector.cs:964-977
     *out = sum_all_slots(c, mul.get(), length, force_column);
     API_END
@@ -1208,6 +1310,7 @@ extern "C" int cnhe_vec_dot_product(cnhe_ctx *h, const cnhe_vec *a, const cnhe_v
 extern "C" int cnhe_vec_rotate(cnhe_ctx *h, const cnhe_vec *a, int amount, cnhe_vec **out) {
     API_BEGIN(h)
     same_ctx(c, a);
+    use_slot(c, {a});
     if (!a->enc) fail("Rotate operates only on encrypted data");
     if (a->format == CNHE_SPARSE) fail("Rotate operates only on dense vectors");
     cnhe_vec *o = new_vec(c, a->dim, a->scale, CNHE_DENSE, true, 1);
@@ -1224,6 +1327,7 @@ extern "C" int cnhe_vec_rotate(cnhe_ctx *h, const cnhe_vec *a, int amount, cnhe_
 extern "C" int cnhe_vec_duplicate(cnhe_ctx *h, const cnhe_vec *a, uint64_t count, cnhe_vec **out) {
     API_BEGIN(h)
     same_ctx(c, a);
+    use_slot(c, {a});
     uint64_t shift = 1;
     while (shift < a->dim) shift *= 2;
     if (!a->enc) fail("Duplicate operates only on encrypted data");
@@ -1268,6 +1372,7 @@ extern "C" int cnhe_vec_permute(cnhe_ctx *h, const cnhe_vec *a, const cnhe_vec *
                                 cnhe_vec **out) {
     API_BEGIN(h)
     same_ctx(c, a);
+    use_slot(c, {a});
     if (a->format != CNHE_DENSE) fail("Permute works only on dense vectors");
     if (!a->enc) fail("can permute only encrypted vectors");
     if (a->blocks > 1) fail("can permute only a single block");
@@ -1307,6 +1412,7 @@ extern "C" int cnhe_vecs_generate_sparse_of_array(cnhe_ctx *h, const cnhe_vec *c
     API_BEGIN(h)
     if (n < 1) fail("empty array");
     for (int i = 0; i < n; i++) { same_ctx(c, vecs[i]); if (!vecs[i]->enc) fail("expecting encrypted vectors"); }
+    use_slot(c, vecs, n);
     cnhe_vec *o = new_vec(c, (uint64_t)n, vecs[0]->scale, CNHE_SPARSE, true, n);
     alloc_channels(o);
     for (int ch = 0; ch < c.P; ch++) {
@@ -1319,29 +1425,20 @@ extern "C" int cnhe_vecs_generate_sparse_of_array(cnhe_ctx *h, const cnhe_vec *c
 }
 
 // Inteleave (AtomicSealBfvVector.cs:600-722): place vector k at slot offset shift*k
-static void interleave_channel(Context &c, int ch, const std::vector<const cnhe_vec *> &vecs, int shift, int out_blocks, u64 *out) {
+// Phase 1 of one interleave: where every vector goes, and the rotation jobs that put it there (under key slot `slot`)
+struct Placed { int kind, start_block, end_block, in_block; u64 *v; }; // kind 0 lower, 1 upper, 2 straddles into the next block, 3 straddles lower/upper
+static void interleave_place(Context &c, int ch, const std::vector<const cnhe_vec *> &vecs, int shift, int out_blocks, int slot,
+                             std::vector<Placed> &placed, std::vector<RotateJob> &jobs) {
     const int block_size = (int)c.N, half = block_size / 2;
     const size_t ctw = c.ct_words();
     const int abs_shift = shift < 0 ? -shift : shift;
     if (shift < 0 && out_blocks > 1) fail("Negative shifts with multiple output blocks are not implemented yet");
     if (abs_shift > half && out_blocks > 1) fail("Shifts of more than half block size with multiple output blocks are not implemented yet");
     if ((long long)abs_shift * (long long)vecs.size() > (long long)block_size * out_blocks) fail("not enough room for interleaving");
-    std::vector<std::vector<const u64 *>> lower(out_blocks), upper(out_blocks);
-    auto ones_plain = [&](int count) { // BatchEncoder.Encode of `count` ones
-        std::vector<u64> v(block_size, 0);
-        for (int i = 0; i < count; i++) v[i] = 1;
-        u64 *dv = c.ws_alloc(block_size), *pl = c.ws_alloc(block_size);
-        CNHE_CUDA(cudaMemcpyAsync(dv, v.data(), (size_t)block_size * 8, cudaMemcpyHostToDevice, c.stream));
-        op_encode(c, ch, dv, 1, block_size, pl);
-        c.sync();
-        return pl;
-    };
-    // phase 1: every vector's rotation (RotateRowsInplace of its own offset, ":625-660") -- independent of each other, so they are
-    // queued and executed together: hops with the same Galois element share one key-switch wave (same per-ciphertext operations
-    // and order as one rotate_rows call per vector, hence the same ciphertexts)
-    struct Placed { int kind, start_block, end_block, in_block; u64 *v; }; // kind 0 lower, 1 upper, 2 straddles into the next block, 3 straddles lower/upper
-    std::vector<Placed> placed(vecs.size());
-    std::vector<RotateJob> jobs;
+    // every vector's rotation (RotateRowsInplace of its own offset, ":625-660") -- independent of each other, so they are queued and
+    // executed together: hops with the same Galois element share one key-switch wave (same per-ciphertext operations and order as one
+    // rotate_rows call per vector, hence the same ciphertexts)
+    placed.assign(vecs.size(), Placed{});
     for (size_t kk = 0; kk < vecs.size(); kk++) {
         long long this_shift = (long long)shift * (long long)kk;
         if (this_shift < 0) this_shift = half + this_shift;
@@ -1355,18 +1452,35 @@ static void interleave_channel(Context &c, int ch, const std::vector<const cnhe_
             CNHE_CUDA(cudaMemcpyAsync(v, src, ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(v, src);
             pl.kind = 0;
         } else if (in_block + abs_shift < half) {
-            jobs.push_back({src, -(int)this_shift, v});
+            jobs.push_back({src, -(int)this_shift, v, slot});
             pl.kind = 0;
         } else if (in_block >= half) {
-            jobs.push_back({src, -(in_block - half), v});
+            jobs.push_back({src, -(in_block - half), v, slot});
             pl.kind = start_block == end_block ? 1 : 2;
         } else {
-            jobs.push_back({src, -in_block, v});
+            jobs.push_back({src, -in_block, v, slot});
             pl.kind = 3;
         }
     }
-    op_rotate_rows_multi(c, ch, jobs);
-    // phase 2: split the vectors that straddle a half / block boundary with a one-hot-prefix mask (":640-672") and file every piece
+}
+// Phase 2 (after the rotation jobs ran): split the vectors that straddle a half / block boundary and sum every output block; key
+// switches use the call's slot c.slot
+static void interleave_finish(Context &c, int ch, const std::vector<const cnhe_vec *> &vecs, int shift, int out_blocks,
+                              const std::vector<Placed> &placed, u64 *out) {
+    const int block_size = (int)c.N, half = block_size / 2;
+    const size_t ctw = c.ct_words();
+    const int abs_shift = shift < 0 ? -shift : shift;
+    std::vector<std::vector<const u64 *>> lower(out_blocks), upper(out_blocks);
+    auto ones_plain = [&](int count) { // BatchEncoder.Encode of `count` ones
+        std::vector<u64> v(block_size, 0);
+        for (int i = 0; i < count; i++) v[i] = 1;
+        u64 *dv = c.ws_alloc(block_size), *pl = c.ws_alloc(block_size);
+        CNHE_CUDA(cudaMemcpyAsync(dv, v.data(), (size_t)block_size * 8, cudaMemcpyHostToDevice, c.stream));
+        op_encode(c, ch, dv, 1, block_size, pl);
+        c.sync();
+        return pl;
+    };
+    // split the vectors that straddle a half / block boundary with a one-hot-prefix mask (":640-672") and file every piece
     for (size_t kk = 0; kk < vecs.size(); kk++) {
         const Placed &pl = placed[kk];
         u64 *v = pl.v;
@@ -1410,10 +1524,18 @@ static void interleave_channel(Context &c, int ch, const std::vector<const cnhe_
         }
     }
 }
+static void interleave_channel(Context &c, int ch, const std::vector<const cnhe_vec *> &vecs, int shift, int out_blocks, u64 *out) {
+    std::vector<Placed> placed;
+    std::vector<RotateJob> jobs;
+    interleave_place(c, ch, vecs, shift, out_blocks, c.slot, placed, jobs);
+    op_rotate_rows_multi(c, ch, jobs);
+    interleave_finish(c, ch, vecs, shift, out_blocks, placed, out);
+}
 static cnhe_vec *interleave(Context &c, const cnhe_vec *const *vecs, int n, int shift) { // AtomicSealBfvVector.cs:729-750
     if (n < 1) fail("empty array");
     std::vector<const cnhe_vec *> vv(vecs, vecs + n);
     for (auto v : vv) { same_ctx(c, v); if (!v->enc) fail("expecting encrypted vectors"); }
+    use_slot(c, vecs, n);
     if (vv[0]->format != CNHE_DENSE) fail("Expecting dense vector");
     int out_blocks = 1;
     if (shift > 0) out_blocks = (int)std::ceil((double)(vv[0]->dim * (uint64_t)n) / (double)c.N);
@@ -1437,6 +1559,46 @@ extern "C" int cnhe_vecs_stack(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, 
     cnhe_vec *o = interleave(c, vecs, n, (int)vecs[0]->dim);
     o->dim = vecs[0]->dim * (uint64_t)n;
     *out = o;
+    API_END
+}
+// cnhe_vecs_stack of B groups of n vectors each (one LoLa vectorize layer per client; the groups' key slots may differ): out[b] is
+// bit-identical to cnhe_vecs_stack(vecs + b * n, n).  The rotations of all groups run as one set of jobs (one key-switch wave per hop
+// for all clients), then each group's masks and sums.
+extern "C" int cnhe_vecs_stack_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int B, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n < 1 || B < 1 || !vecs || !out) fail("bad arguments");
+    std::vector<std::vector<const cnhe_vec *>> groups(B);
+    std::vector<int> gslot(B), out_blocks(B);
+    for (int b = 0; b < B; b++) {
+        groups[b].assign(vecs + (size_t)b * n, vecs + (size_t)(b + 1) * n);
+        for (auto v : groups[b]) { same_ctx(c, v); if (!v->enc) fail("expecting encrypted vectors"); }
+        if (groups[b][0]->format != CNHE_DENSE) fail("Expecting dense vector");
+        gslot[b] = use_slot(c, groups[b].data(), n);
+        const int shift = (int)groups[b][0]->dim;
+        out_blocks[b] = shift > 0 ? (int)std::ceil((double)(groups[b][0]->dim * (uint64_t)n) / (double)c.N) : 1;
+    }
+    for (int b = 0; b < B; b++) c.foreign = c.foreign || gslot[b] != 0;
+    std::vector<std::unique_ptr<cnhe_vec>> outs(B);
+    for (int b = 0; b < B; b++) {
+        c.slot = gslot[b];
+        outs[b].reset(new_vec(c, groups[b][0]->dim, groups[b][0]->scale, CNHE_DENSE, true, out_blocks[b]));
+        alloc_channels(outs[b].get());
+    }
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        std::vector<std::vector<Placed>> placed(B);
+        std::vector<RotateJob> jobs;
+        for (int b = 0; b < B; b++) interleave_place(c, ch, groups[b], (int)groups[b][0]->dim, out_blocks[b], gslot[b], placed[b], jobs);
+        op_rotate_rows_multi(c, ch, jobs);
+        for (int b = 0; b < B; b++) {
+            c.slot = gslot[b];
+            interleave_finish(c, ch, groups[b], (int)groups[b][0]->dim, out_blocks[b], placed[b], outs[b]->ptr(ch));
+        }
+    }
+    for (int b = 0; b < B; b++) {
+        outs[b]->dim = groups[b][0]->dim * (uint64_t)n;
+        out[b] = outs[b].release();
+    }
     API_END
 }
 
@@ -1628,6 +1790,20 @@ static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int
             if (bias[m]->scale != in[0]->scale * weights[0]->scale) fail("Scales do not match.");
             const_bias = const_bias && bias[m]->is_const;
         }
+    }
+    // The scalar MAC is key-independent, so one call may serve several clients (their images' columns side by side, each output's
+    // gather row inside one client's columns): every output takes the key slot its taps share; taps of two slots in one output are refused
+    const std::vector<int> in_slot = vec_slots(c, in, n_in);
+    std::vector<int> out_slot(M, -1);
+    for (int m = 0; m < M; m++) {
+        for (int kk = 0; kk < (gather ? K : n_in); kk++) {
+            const int g = gather ? gather[(size_t)m * K + kk] : kk;
+            if (g < 0) continue;
+            if (g >= n_in) fail("gather index out of range");
+            if (out_slot[m] >= 0 && out_slot[m] != in_slot[g]) fail("encrypted operands belong to different key slots");
+            out_slot[m] = in_slot[g];
+        }
+        if (out_slot[m] < 0) out_slot[m] = in_slot[0];
     }
     // 128-bit accumulator bound: K products of (q_l - 1)^2
     int maxbits = 0;
@@ -1842,6 +2018,7 @@ static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int
     }
     for (int m = 0; m < M; m++) {
         cnhe_vec *o = new_vec(c, in[0]->dim, out_scale, CNHE_DENSE, true, bl);
+        o->slot = out_slot[m];
         for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
             o->buf[ch] = big[ch];
@@ -1865,6 +2042,11 @@ extern "C" int cnhe_mat_mul_colmajor_sparse(cnhe_ctx *h, const cnhe_vec *const *
     if ((uint64_t)K != sparse->dim) fail("dimensions do not match");
     if (sparse->format != CNHE_SPARSE) fail("expecting a sparse vector");
     if (!cols[0]->enc && !sparse->enc) fail("at least one parameter has to be encrypted");
+    {
+        std::vector<const cnhe_vec *> all(cols, cols + K);
+        all.push_back(sparse);
+        use_slot(c, all.data(), K + 1);
+    }
     if (cols[0]->enc && !sparse->enc) {
         mac_layer(c, cols, K, nullptr, &sparse, nullptr, 1, K, out);
     } else {
@@ -1902,22 +2084,23 @@ extern "C" int cnhe_mat_mul_colmajor_sparse(cnhe_ctx *h, const cnhe_vec *const *
 }
 // Batched SumAllSlots (AtomicSealBfvVector.cs:888-955) on n single-block ciphertexts in place: the same rotate-and-add ladder,
 // one key-switch wave per step for all n.
-static uint64_t sum_slots_batched(Context &c, int ch, u64 *cts, int n, uint64_t length) {
+// slots: per-ciphertext key slots (nullptr: the call's slot)
+static uint64_t sum_slots_batched(Context &c, int ch, u64 *cts, int n, uint64_t length, const int *slots = nullptr) {
     const size_t N = c.N, words = (size_t)n * c.ct_words();
     uint64_t len = length;
     u64 *tmp = c.ws_alloc(words);
     // every step is x += rotate(x): fused into the rotation (the permutation kernel folds x into the key switch's base) when the step
     // has its own Galois key -- it does for the powers of two the ladder walks -- else rotate, then add
     if (len >= N / 2) {
-        if (!op_rotate_add(c, ch, cts, n, 0, true, cts)) {
-            op_rotate_columns(c, ch, cts, n, tmp);
+        if (!op_rotate_add(c, ch, cts, n, 0, true, cts, slots)) {
+            op_rotate_columns(c, ch, cts, n, tmp, slots);
             do_add(c, ch, cts, tmp, cts, words, 0);
         }
         len = N / 2;
     }
     for (uint64_t steps = 1; steps < len; steps *= 2) {
-        if (op_rotate_add(c, ch, cts, n, -(int)steps, false, cts)) continue;
-        op_rotate_rows(c, ch, cts, n, -(int)steps, tmp);
+        if (op_rotate_add(c, ch, cts, n, -(int)steps, false, cts, slots)) continue;
+        op_rotate_rows(c, ch, cts, n, -(int)steps, tmp, slots);
         do_add(c, ch, cts, tmp, cts, words, 0);
     }
     return len;
@@ -1939,6 +2122,7 @@ extern "C" int cnhe_mat_mul_rowmajor_shard(cnhe_ctx *h, const cnhe_vec *const *r
     if (first_row < 0 || first_row + n_rows > total_rows) fail("row slice out of range");
     same_ctx(c, v);
     if (!v->enc) fail("at least one parameter has to be encrypted");
+    use_slot(c, {v});
     if (v->format != CNHE_DENSE) fail("Expecting dense vector format");
     if (v->blocks != 1) fail("row-major multiplication expects a single-block vector");
     for (int r = 0; r < n_rows; r++) {
@@ -1984,6 +2168,91 @@ extern "C" int cnhe_mat_mul_rowmajor_shard(cnhe_ctx *h, const cnhe_vec *const *r
     *out = guard.release();
     API_END
 }
+// The row-major product of one plain matrix with B encrypted vectors that may belong to different key slots (one inference per client):
+// out[b] is what cnhe_mat_mul_rowmajor(rows, n_rows, vs[b], force_dense) returns, bit for bit.  The B * n_rows products are flattened
+// (product p = b * n_rows + r) and go through each stage in waves of up to 1024: the broadcast plain products, one rotate-and-add
+// ladder for the whole wave (every key switch of a step in one wave, each ciphertext under its own slot's keys), then per input the
+// one-hot masks and the sum into its dense output, or its sparse elements.
+extern "C" int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, int force_dense,
+                                           cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n_rows < 1 || B < 1 || !vs || !out) fail("bad arguments");
+    for (int b = 0; b < B; b++) {
+        same_ctx(c, vs[b]);
+        if (!vs[b]->enc) fail("at least one parameter has to be encrypted");
+        if (vs[b]->format != CNHE_DENSE) fail("Expecting dense vector format");
+        if (vs[b]->blocks != 1) fail("row-major multiplication expects a single-block vector");
+        if (vs[b]->dim != vs[0]->dim || vs[b]->scale != vs[0]->scale) fail("the input vectors must share dimension and scale");
+    }
+    for (int r = 0; r < n_rows; r++) {
+        same_ctx(c, rows[r]);
+        if (rows[r]->enc) fail("encrypted rows are not supported by the batched row-major product");
+        if (rows[r]->dim != vs[0]->dim) fail("Dimensions do not match");
+        if (rows[r]->format != CNHE_DENSE) fail("Format mismatch");
+        if (rows[r]->scale != rows[0]->scale) fail("row scales differ");
+    }
+    const size_t N = c.N, ctw = c.ct_words();
+    if (force_dense && (size_t)n_rows > N) fail("column out of range");
+    const std::vector<int> vslot = vec_slots(c, vs, B);
+    const double out_scale = vs[0]->scale * rows[0]->scale;
+    std::vector<std::unique_ptr<cnhe_vec>> outs(B);
+    std::vector<BufRef> big(c.P); // sparse outputs: one [B][n_rows] block, product p lands in its place
+    for (int b = 0; b < B; b++) {
+        outs[b].reset(new_vec(c, (uint64_t)n_rows, out_scale, force_dense ? CNHE_DENSE : CNHE_SPARSE, true, force_dense ? 1 : n_rows));
+        outs[b]->slot = vslot[b];
+        if (force_dense) alloc_channels(outs[b].get());
+    }
+    if (!force_dense)
+        for (int ch = 0; ch < c.P; ch++) {
+            c.set_channel(ch);
+            big[ch] = c.alloc((size_t)B * n_rows * ctw);
+            for (int b = 0; b < B; b++) { outs[b]->buf[ch] = big[ch]; outs[b]->off[ch] = (size_t)b * n_rows * ctw; }
+        }
+    // products per wave: 1024 as in cnhe_mat_mul_rowmajor, fewer when the wave's scratch (the products, the ladder's rotated copies and
+    // the masked products: three ciphertexts per product) would pass 8 GiB -- N = 16384 with nine primes takes 728
+    const int total = B * n_rows, RC = (int)std::max<size_t>(16, std::min<size_t>(1024, ((size_t)1 << 30) / (3 * ctw)));
+    std::vector<int> pslot(total);
+    for (int p = 0; p < total; p++) pslot[p] = vslot[p / n_rows];
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        std::vector<char> first(B, 1);
+        for (int p0 = 0; p0 < total; p0 += RC) {
+            WsScope scope(c);
+            const int m = std::min(RC, total - p0);
+            u64 *prod = force_dense ? c.ws_alloc((size_t)m * ctw) : big[ch]->p + (size_t)p0 * ctw;
+            // segments of the wave: the rows r0..r0+len of input b
+            struct Seg { int b, r0, len, off; };
+            std::vector<Seg> segs;
+            for (int p = p0; p < p0 + m;) {
+                const int b = p / n_rows, r0 = p % n_rows, len = std::min(n_rows - r0, p0 + m - p);
+                segs.push_back({b, r0, len, p - p0});
+                p += len;
+            }
+            u64 *plains = c.ws_alloc((size_t)m * N);
+            for (const Seg &sg : segs) {
+                for (int i = 0; i < sg.len; i++)
+                    CNHE_CUDA(cudaMemcpyAsync(plains + (size_t)(sg.off + i) * N, rows[sg.r0 + i]->ptr(ch), N * 8, cudaMemcpyDeviceToDevice, c.stream));
+                op_multiply_plain_dense_bcast(c, ch, vs[sg.b]->ptr(ch), plains + (size_t)sg.off * N, sg.len, prod + (size_t)sg.off * ctw);
+            }
+            sum_slots_batched(c, ch, prod, m, CNHE_ALL_SLOTS, pslot.data() + p0);
+            if (force_dense) {
+                u64 *masks = c.ws_alloc((size_t)m * N);
+                for (const Seg &sg : segs) op_encode_onehot(c, ch, sg.len, sg.r0, masks + (size_t)sg.off * N);
+                op_multiply_plain_dense(c, ch, prod, m, masks, true, prod);
+                for (const Seg &sg : segs) {
+                    std::vector<const u64 *> terms;
+                    if (!first[sg.b]) terms.push_back(outs[sg.b]->ptr(ch));
+                    for (int i = 0; i < sg.len; i++) terms.push_back(prod + (size_t)(sg.off + i) * ctw);
+                    do_add_many(c, ch, terms, outs[sg.b]->ptr(ch));
+                    first[sg.b] = 0;
+                }
+                c.sync();
+            }
+        }
+    }
+    for (int b = 0; b < B; b++) out[b] = outs[b].release();
+    API_END
+}
 // SquareActivation over a whole matrix: every column PointwiseMultiply'd with itself in one wave per channel
 extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, cnhe_vec **out) {
     API_BEGIN(h)
@@ -1995,6 +2264,10 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
         first[i + 1] = first[i] + in[i]->blocks;
     }
     const int total = first[n];
+    // the vectors may belong to different key slots (several clients' layers in one call): each ciphertext is relinearised under its own
+    const std::vector<int> vslot = vec_slots(c, in, n);
+    std::vector<int> ct_slot;
+    for (int i = 0; i < n; i++) ct_slot.insert(ct_slot.end(), in[i]->blocks, vslot[i]);
     std::vector<BufRef> big(c.P);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
@@ -2002,10 +2275,11 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
         std::vector<const u64 *> ptrs;
         for (int i = 0; i < n; i++)
             for (int b = 0; b < in[i]->blocks; b++) ptrs.push_back(in[i]->block(ch, b));
-        op_multiply_relin(c, ch, ptrs, ptrs, big[ch]->p);
+        op_multiply_relin(c, ch, ptrs, ptrs, big[ch]->p, ct_slot.data());
     }
     for (int i = 0; i < n; i++) {
         cnhe_vec *o = new_vec(c, in[i]->dim, in[i]->scale * in[i]->scale, in[i]->format, true, in[i]->blocks);
+        o->slot = vslot[i];
         for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
             o->buf[ch] = big[ch];

@@ -1,5 +1,6 @@
 // Internal header shared by the translation units that implement the C ABI (vec.cu: vectors, layers; wire.cu: wire formats).
 #pragma once
+#include <initializer_list>
 #include <memory>
 #include <string>
 #include <vector>
@@ -19,6 +20,7 @@ struct cnhe_vec {
     double scale = 1.0;
     int format = CNHE_DENSE;
     bool enc = false;
+    int slot = 0;   // encrypted: the key slot whose evaluation keys its key switches use (plain vectors ignore it)
     int blocks = 0; // ciphertexts / plaintexts per channel
     std::vector<BufRef> buf; // per channel: enc -> blocks*2kN words, plain dense -> blocks*N words, plain sparse -> `blocks` scalars
     std::vector<size_t> off;
@@ -40,6 +42,8 @@ int set_err(int code, const std::string &m); // thread-local last error (vec.cu)
         std::lock_guard<std::recursive_mutex> lock(c.mu);                                                              \
         CNHE_CUDA(cudaSetDevice(c.device));                                                                            \
         c.set_channel(0);                                                                                              \
+        c.slot = 0;                                                                                                    \
+        c.foreign = false;                                                                                             \
         ws_release_all(c);
 #define API_END                                                                                                        \
     }                                                                                                                  \
@@ -47,7 +51,11 @@ int set_err(int code, const std::string &m); // thread-local last error (vec.cu)
     catch (const std::exception &e) { return set_err(CNHE_ERR_INVALID, e.what()); }                                   \
     return CNHE_OK;
 static inline void fail(const char *m) { throw Error(CNHE_ERR_INVALID, m); }
-cnhe_vec *new_vec(Context &c, uint64_t dim, double scale, int format, bool enc, int blocks);
+cnhe_vec *new_vec(Context &c, uint64_t dim, double scale, int format, bool enc, int blocks); // bound to the call's key slot c.slot
+// the key slot the encrypted vectors among vs share (plain and null entries have none), made the call's slot; CNHE_ERR_INVALID when two
+// encrypted vectors belong to different slots or the slot was removed
+int use_slot(Context &c, const cnhe_vec *const *vs, int n);
+static inline int use_slot(Context &c, std::initializer_list<const cnhe_vec *> vs) { return use_slot(c, vs.begin(), (int)vs.size()); }
 void alloc_channels(cnhe_vec *v);
 void same_ctx(Context &c, const cnhe_vec *v);
 

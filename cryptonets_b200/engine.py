@@ -81,6 +81,17 @@ class Vec:
         check(self.eng.L.cnhe_vec_export_raw(self.eng.h, self.h, channel, block, _p(out), out.size))
         return out
 
+    @property
+    def key_slot(self):
+        """The key slot whose evaluation keys this encrypted vector's key switches use (-1: a plain vector)."""
+        s = C.c_int()
+        check(self.eng.L.cnhe_vec_key_slot(self.h, C.byref(s)))
+        return s.value
+
+    def set_key_slot(self, slot):
+        """Bind this encrypted vector to a key slot (a ciphertext uploaded by the client whose keys are in that slot)."""
+        check(self.eng.L.cnhe_vec_set_key_slot(self.h, int(slot)))
+
     def device_ptr(self, channel=0):
         p, w = C.c_uint64(), C.c_size_t()
         check(self.eng.L.cnhe_vec_device_ptr(self.h, channel, C.byref(p), C.byref(w)))
@@ -224,6 +235,17 @@ class Engine:
         buf = (C.c_ubyte * need.value)()
         check(self.L.cnhe_keys_save_compact(self.h, sets, elts, n, buf, need.value, C.byref(need)))
         return bytes(buf)
+
+    def add_client_compact(self, blob):
+        """Load another client's compact evaluation keys (save_compact_keys of the client's engine; same parameters) into a new key slot;
+        returns the slot number.  Vectors bound to it with Vec.set_key_slot are evaluated under those keys."""
+        buf = (C.c_ubyte * len(blob)).from_buffer_copy(blob)
+        s = C.c_int()
+        check(self.L.cnhe_context_add_client_compact(self.h, buf, len(blob), C.byref(s)))
+        return s.value
+
+    def remove_client(self, slot):
+        check(self.L.cnhe_context_remove_client(self.h, int(slot)))
 
     def write_vector(self, vec):
         """EncryptedSealBfvVector.Write: the text form of one vector."""
@@ -445,6 +467,13 @@ class Engine:
         check(self.L.cnhe_vec_rotate(self.h, a.h, int(amount), C.byref(out)))
         return Vec(self, out)
 
+    def rotate_many(self, vecs, amount):
+        """rotate() of every vector by the same amount in one pass; their key slots may differ."""
+        n = len(vecs)
+        out = (VECP * n)()
+        check(self.L.cnhe_vecs_rotate(self.h, _vec_array(vecs), n, int(amount), out))
+        return self._wrap_many(out, n, like=vecs)
+
     def duplicate(self, a, count):
         out = VECP()
         check(self.L.cnhe_vec_duplicate(self.h, a.h, int(count), C.byref(out)))
@@ -466,6 +495,15 @@ class Engine:
         check(self.L.cnhe_vecs_stack(self.h, _vec_array(vecs), len(vecs), C.byref(out)))
         return Vec(self, out)
 
+    def stack_many(self, groups):
+        """stack(g) for every group g (equal lengths; one per client, their key slots may differ) in one pass."""
+        B, n = len(groups), len(groups[0])
+        if any(len(g) != n for g in groups):
+            raise ValueError("every group must have the same number of vectors")
+        out = (VECP * B)()
+        check(self.L.cnhe_vecs_stack_batch(self.h, _vec_array([v for g in groups for v in g]), n, B, out))
+        return self._wrap_many(out, B, like=[g[0] for g in groups])
+
     def generate_sparse_of_array(self, vecs):
         out = VECP()
         check(self.L.cnhe_vecs_generate_sparse_of_array(self.h, _vec_array(vecs), len(vecs), C.byref(out)))
@@ -480,6 +518,13 @@ class Engine:
         out = VECP()
         check(self.L.cnhe_mat_mul_rowmajor(self.h, _vec_array(rows), len(rows), v.h, int(force_dense), C.byref(out)))
         return Vec(self, out)
+
+    def mat_mul_rowmajor_batch(self, rows, vs, force_dense=False):
+        """mat_mul_rowmajor(rows, v, force_dense) for every v in vs in one pass (one input per client; their key slots may differ)."""
+        B = len(vs)
+        out = (VECP * B)()
+        check(self.L.cnhe_mat_mul_rowmajor_batch(self.h, _vec_array(rows), len(rows), _vec_array(vs), B, int(force_dense), out))
+        return self._wrap_many(out, B)
 
     def mat_mul_rowmajor_shard(self, rows, v, force_dense, first_row, total_rows):
         out = VECP()
@@ -497,9 +542,12 @@ class Engine:
             None if bias is None else _vec_array(bias), M, K, out))
         return self._wrap_many(out, M)
 
-    def _wrap_many(self, out, n):
-        """Vec handles for the n outputs of one batched call: they share dim/scale/format/blocks, so the metadata is queried once."""
+    def _wrap_many(self, out, n, like=None):
+        """Vec handles for the n outputs of one batched call: they share dim/scale/format/blocks, so the metadata is queried once.
+        like: the inputs of a call whose outputs follow their own input's shape -- shared only when those inputs share theirs."""
         vecs = [Vec(self, out[i]) for i in range(n)]
+        if like is not None and any(v.meta() != like[0].meta() for v in like[1:]):
+            return vecs
         if n > 1:
             m = vecs[0].meta()
             for v in vecs[1:]:
@@ -510,7 +558,7 @@ class Engine:
         n = len(inputs)
         out = (VECP * n)()
         check(self.L.cnhe_layer_square(self.h, _vec_array(inputs), n, out))
-        return self._wrap_many(out, n)
+        return self._wrap_many(out, n, like=inputs)
 
     # ---- raw device arrays (micro-benchmarks, kernel parity tests)
     def dev_alloc(self, words):

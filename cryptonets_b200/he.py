@@ -322,10 +322,53 @@ class B200BfvFactory:
         for c1 (include/cnhe.h, cnhe_vecs_encrypt_compact).  Needs the secret key; the matrix format travels out of band."""
         return self.engine.encrypt_compact(np.ascontiguousarray(self._rows(m, fmt)), scale)
 
-    def LoadCompactMatrix(self, data, fmt):
-        """The matrix of a compact blob (GetEncryptedMatrixCompact), expanded on the GPU; `fmt` is the format it was made with."""
-        vecs = [B200BfvVector(self, v) for v in self.engine.import_compact(data)]
-        return B200BfvMatrix(self, vecs, fmt, CopyVectors=False)
+    def LoadCompactMatrix(self, data, fmt, slot=0):
+        """The matrix of a compact blob (GetEncryptedMatrixCompact), expanded on the GPU; `fmt` is the format it was made with.  slot: the
+        key slot (AddClientKeys) of the client that encrypted it."""
+        vs = self.engine.import_compact(data)
+        if slot:
+            for v in vs:
+                v.set_key_slot(slot)
+        return B200BfvMatrix(self, [B200BfvVector(self, v) for v in vs], fmt, CopyVectors=False)
+
+    # ---- several clients in one context (include/cnhe.h, key slots)
+    def AddClientKeys(self, blob):
+        """Another client's compact evaluation keys (its SaveCompactKeys; same parameters) in a new key slot; returns the slot."""
+        return self.engine.add_client_compact(blob)
+
+    def RemoveClient(self, slot):
+        self.engine.remove_client(slot)
+
+    def SquareBatch(self, matrices):
+        """SquareActivation of several matrices (possibly of different clients) in one relinearisation wave."""
+        vecs = [v.vec for m in matrices for v in m.vectors]
+        out, i, res = self.engine.layer_square(vecs), 0, []
+        for m in matrices:
+            n = len(m.vectors)
+            res.append(B200BfvMatrix(self, [B200BfvVector(self, o) for o in out[i:i + n]], m.Format, CopyVectors=False))
+            i += n
+        return res
+
+    def StackBatch(self, matrices):
+        """ConvertToColumnVector of several column-major matrices (one per client) in one pass."""
+        return [B200BfvVector(self, o) for o in self.engine.stack_many([[v.vec for v in m.vectors] for m in matrices])]
+
+    def ConvBatch(self, matrices, weights):
+        """[m.Mul(w) for w in weights] for every column-major matrix m (one per client, same shape) in one scalar-MAC call: the
+        clients' columns side by side, output (b, k) gathering client b's columns with weights[k]."""
+        B, K = len(matrices), len(matrices[0].vectors)
+        if any(len(m.vectors) != K for m in matrices) or any(w.Dim != K for w in weights):
+            raise Exception("dimensions do not match")
+        M = B * len(weights)
+        gather = [b * K + kk for b in range(B) for _ in weights for kk in range(K)]
+        out = self.engine.layer_conv_dense([v.vec for m in matrices for v in m.vectors], gather, [w.vec for _ in range(B) for w in weights], None, M, K)
+        n = len(weights)
+        return [[B200BfvVector(self, o) for o in out[b * n:(b + 1) * n]] for b in range(B)]
+
+    def MulRowMajorBatch(self, weights, vectors, ForceDenseFormat=False):
+        """weights.Mul(v, ForceDenseFormat=...) of a plain row-major matrix for every v (one per client) in one pass."""
+        out = self.engine.mat_mul_rowmajor_batch([r.vec for r in weights.vectors], [v.vec for v in vectors], ForceDenseFormat)
+        return [B200BfvVector(self, o) for o in out]
 
     def GetMatrix(self, vectors, fmt, CopyVectors=True):
         return B200BfvMatrix(self, vectors, fmt, CopyVectors=CopyVectors)

@@ -133,6 +133,11 @@ class BaseLayer:
     def Apply(self, m):
         raise NotImplementedError
 
+    def ApplyBatch(self, ms):
+        """Apply to one matrix per client (one inference each; on a multi-client factory their key slots may differ).  Layers without a
+        batched form apply one matrix at a time; the outputs are the same either way."""
+        return [self.Apply(m) for m in ms]
+
     def GetNext(self):
         if not self.layerPrepared:
             self.Prepare()
@@ -277,6 +282,12 @@ class SquareActivation(BaseLayer):
 
     def Apply(self, m):
         return m.ElementWiseMultiply(m, self.Factory.AllocateComputationEnv())
+
+    def ApplyBatch(self, ms):
+        batch = getattr(self.Factory, "SquareBatch", None)
+        if batch is None or len(ms) < 2:
+            return super().ApplyBatch(ms)
+        return batch(ms)
 
     def GetOutputScale(self):
         s = self.Source.GetOutputScale()
@@ -460,6 +471,23 @@ class LLPoolLayer(_ConvLayerBase):
             mul.Dispose()
         return f.GetMatrix(res, EMatrixFormat.ColumnMajor, CopyVectors=False)
 
+    def ApplyBatch(self, ms):
+        """Every client's convolution in one scalar-MAC call (the MAC is key-independent; each output reads one client's columns), then
+        each output's bias."""
+        f = self.Factory
+        batch = getattr(f, "ConvBatch", None)
+        if (batch is None or len(ms) < 2 or self.Weights is None or any(m.Format != EMatrixFormat.ColumnMajor or not m.IsEncrypted for m in ms)
+                or any(m.ColumnCount != ms[0].ColumnCount or m.vectors[0].Dim != ms[0].vectors[0].Dim for m in ms)):
+            return super().ApplyBatch(ms)
+        env = f.AllocateComputationEnv()
+        out = []
+        for muls in batch(ms, self.weightWindows):
+            res = [mul.Add(self.biasVectors[k], env) for k, mul in enumerate(muls)]
+            for mul in muls:
+                mul.Dispose()
+            out.append(f.GetMatrix(res, EMatrixFormat.ColumnMajor, CopyVectors=False))
+        return out
+
 
 class LLVectorizeLayer(BaseLayer):
     """`NeuralNetworks/LLVectorizeLayer.cs:8-24`"""
@@ -469,6 +497,14 @@ class LLVectorizeLayer(BaseLayer):
     def Apply(self, m):
         vec = m.ConvertToColumnVector(self.Factory.AllocateComputationEnv())
         return self.Factory.GetMatrix([vec], EMatrixFormat.ColumnMajor, CopyVectors=False)
+
+    def ApplyBatch(self, ms):
+        """Every client's vectorisation in one pass: the rotations of all clients share key-switch waves (cnhe_vecs_stack_batch)."""
+        f = self.Factory
+        batch = getattr(f, "StackBatch", None)
+        if batch is None or len(ms) < 2 or any(m.ColumnCount != ms[0].ColumnCount for m in ms):
+            return super().ApplyBatch(ms)
+        return [f.GetMatrix([v], EMatrixFormat.ColumnMajor, CopyVectors=False) for v in batch(ms)]
 
     def OutputDimension(self):
         return self.OutputDim if self.OutputDim > 0 else super().OutputDimension()
@@ -538,6 +574,20 @@ class LLDenseLayer(BaseLayer):
         res = mul.Add(self.BiasVector, env)
         mul.Dispose()
         return self.Factory.GetMatrix([res], EMatrixFormat.ColumnMajor, CopyVectors=False)
+
+    def ApplyBatch(self, ms):
+        """Every client's row-major product in one pass (cnhe_mat_mul_rowmajor_batch), then each one's bias."""
+        f = self.Factory
+        batch = getattr(f, "MulRowMajorBatch", None)
+        if (batch is None or len(ms) < 2 or self.Shard is not None or self.InputFormat != EVectorFormat.dense or not self.WeightsMatrix.Batched
+                or any(m.ColumnCount != 1 or not m.GetColumn(0).IsEncrypted or m.GetColumn(0).vec.blocks != 1 for m in ms)):
+            return super().ApplyBatch(ms)
+        env = f.AllocateComputationEnv()
+        out = []
+        for mul in batch(self.WeightsMatrix, [m.GetColumn(0) for m in ms], self.ForceDenseFormat):
+            out.append(f.GetMatrix([mul.Add(self.BiasVector, env)], EMatrixFormat.ColumnMajor, CopyVectors=False))
+            mul.Dispose()
+        return out
 
     def Dispose(self):
         if self.WeightsMatrix is not None:

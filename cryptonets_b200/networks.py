@@ -90,6 +90,30 @@ def lola_small(factory, images, weights=None):
     return dense4, reader
 
 
+def serve_batch(net, inputs):
+    """Runs one inference per client through the layers that follow the network's EncryptLayer, all clients together: each layer takes
+    the list of matrices (BaseLayer.ApplyBatch), so the key switches of all clients share waves.  inputs: one encrypted input matrix per
+    client, already on the server's factory and bound to that client's key slot (LoadCompactMatrix(..., slot=)); the caller keeps them.
+    Returns one output matrix per client -- the same ciphertexts each would get from a server that holds only its keys."""
+    chain, layer = [], net
+    while not isinstance(layer, EncryptLayer):
+        chain.append(layer)
+        layer = layer.Source
+    chain.reverse()
+    for layer in chain:
+        if not layer.layerPrepared:
+            layer.Prepare()
+            layer.layerPrepared = True
+    ms = list(inputs)
+    for layer in chain:
+        out = layer.ApplyBatch(ms)
+        for m, o in zip(ms, out):
+            if o is not m and not any(m is i for i in inputs):
+                m.Dispose()
+        ms = out
+    return ms
+
+
 def lola(factory, images, weights=None):
     """LoLa (`LowLatencyCryptoNets/LoLaCryptonets.cs:203-276`): im2col input, 8-way packed dense layer, interleave, square, dense."""
     w = weights or cryptonets_weights()

@@ -133,6 +133,22 @@ int cnhe_context_load(const uint8_t *archive, size_t len, int device, cnhe_ctx *
  * allocated (CNHE_ERR_INVALID, no context).  Returns once the keys are complete. */
 int cnhe_keys_save_compact(cnhe_ctx *, int sets, const uint64_t *galois_elts, int n_galois, uint8_t *dst, size_t cap, size_t *needed);
 int cnhe_context_load_compact(const uint8_t *blob, size_t len, int device, cnhe_ctx **out);
+/* Key slots: one context serves several clients, each with its own secret key.  Slot 0 is the context's own keys; every other slot holds
+ * one client's evaluation keys.  cnhe_context_add_client_compact loads a compact key blob (format above; its public key, if any, is not
+ * kept) into a new slot and returns its number in *slot: the relinearisation keys (with the fused key switch's packed copy) and the
+ * listed Galois elements.  The blob is checked on the host before anything is allocated -- every header field, the exact length, and N,
+ * k, every q_l, P, every t_c and both decomposition bit counts against the context's -- a defect or mismatch is CNHE_ERR_INVALID.
+ * Returns once the keys are complete.  cnhe_context_remove_client frees a slot; its number is not handed out again, and operations on
+ * vectors still bound to it fail with CNHE_ERR_INVALID.
+ * Every encrypted vector is bound to a slot (0 when created, imported or read); cnhe_vec_set_key_slot binds it to another one (a
+ * ciphertext a client encrypted and uploaded), cnhe_vec_key_slot reports it (-1 for a plain vector, which has none).  Results inherit
+ * their operands' slot; two encrypted operands of different slots are CNHE_ERR_INVALID; a key switch that needs a key the slot does not
+ * hold is CNHE_ERR_STATE, as a missing key is on a single-client context (a multi-hop rotation is planned from the Galois elements every
+ * slot of the call holds).  Decryption and noise budgets need the secret key: slot 0 only (CNHE_ERR_STATE otherwise). */
+int cnhe_context_add_client_compact(cnhe_ctx *, const uint8_t *blob, size_t len, int *slot);
+int cnhe_context_remove_client(cnhe_ctx *, int slot);
+int cnhe_vec_set_key_slot(cnhe_vec *, int slot);
+int cnhe_vec_key_slot(const cnhe_vec *, int *slot);
 int cnhe_vec_write(cnhe_ctx *, const cnhe_vec *, char *dst, size_t cap, size_t *needed);
 int cnhe_vec_read(cnhe_ctx *, const char *text, size_t len, cnhe_vec **out, size_t *consumed);
 
@@ -207,7 +223,13 @@ int cnhe_vec_permute(cnhe_ctx *, const cnhe_vec *a, const cnhe_vec *const *selec
                      uint64_t output_dim, cnhe_vec **out);                                   /* :1436-1475 */
 int cnhe_vecs_interleave(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int shift, cnhe_vec **out); /* :600-750 */
 int cnhe_vecs_stack(cnhe_ctx *, const cnhe_vec *const *vecs, int n, cnhe_vec **out);         /* :756-761 */
+/* cnhe_vecs_stack of B groups of n vectors, vecs [B][n] (one LoLa vectorize layer per client; the groups' key slots may differ, a group's
+ * must not): out[b] is bit-identical to cnhe_vecs_stack(vecs + b * n, n), the rotations of all groups share key-switch waves. */
+int cnhe_vecs_stack_batch(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int B, cnhe_vec **out /*B*/);
 int cnhe_vecs_generate_sparse_of_array(cnhe_ctx *, const cnhe_vec *const *vecs, int n, cnhe_vec **out); /* :1347-1359 */
+/* cnhe_vec_rotate of n vectors by the same amount in one pass (out[i] = rotation of vecs[i]); the vectors may belong to different key
+ * slots.  Bit-identical to n cnhe_vec_rotate calls. */
+int cnhe_vecs_rotate(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int amount, cnhe_vec **out /*n*/);
 
 /* ---- IMatrix.Mul and the fused layer entry points ------------------------------------------------------------------ */
 /* ColumnMajor matrix x sparse vector ("EncryptedSealBfvMatrix.cs:70-78" -> "AtomicSealBfvVector.cs:434-521") */
@@ -220,12 +242,18 @@ int cnhe_mat_mul_rowmajor(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, c
  * to the full product ("EncryptedSealBfvMatrix.cs:92-116" sums the masked rows the same way); otherwise this slice's sparse elements. */
 int cnhe_mat_mul_rowmajor_shard(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *v, int force_dense, int first_row,
                                 int total_rows, cnhe_vec **out);
+/* cnhe_mat_mul_rowmajor of one plain matrix with B vectors at once (one inference per client; their key slots may differ): out[b] is
+ * bit-identical to cnhe_mat_mul_rowmajor(rows, n_rows, vs[b], force_dense), the key switches of all B x n_rows products share waves. */
+int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, int force_dense,
+                                cnhe_vec **out /*B*/);
 /* Whole PoolLayer.Apply with weights ("NeuralNetworks/PoolLayer.cs:149-229"): out[m] = sum_k weights[m][k] * in[gather[m*K+k]]
- * + bias[m].  weights[m] is a plain SPARSE vector of dim K, bias[m] a plain DENSE vector (or NULL); gather < 0 is a
+ * + bias[m].  The inputs may belong to different key slots (several clients' images side by side) as long as each output's taps share
+ * one; the output takes it.  weights[m] is a plain SPARSE vector of dim K, bias[m] a plain DENSE vector (or NULL); gather < 0 is a
  * padded tap (the reference multiplies a fresh encryption of zero there; we add nothing -- same decryption). */
 int cnhe_layer_conv_dense(cnhe_ctx *, const cnhe_vec *const *in, int n_in, const int32_t *gather, const cnhe_vec *const *weights,
                           const cnhe_vec *const *bias, int M, int K, cnhe_vec **out /*M*/);
-/* SquareActivation.Apply over a whole matrix ("NeuralNetworks/SquareActivation.cs:10-13"): out[i] = in[i] (.) in[i] */
+/* SquareActivation.Apply over a whole matrix ("NeuralNetworks/SquareActivation.cs:10-13"): out[i] = in[i] (.) in[i].  The vectors may
+ * belong to different key slots (several clients' layers in one call): each is relinearised under its own slot's keys. */
 int cnhe_layer_square(cnhe_ctx *, const cnhe_vec *const *in, int n, cnhe_vec **out /*n*/);
 
 /* ---- micro-benchmark / kernel-level entry points on caller-owned device memory ("raw") --------------------------- */

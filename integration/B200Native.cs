@@ -49,6 +49,10 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_load(byte[] archive, UIntPtr len, int device, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_keys_save_compact(IntPtr a0, int sets, ulong[] galois_elts, int n_galois, byte[] dst, UIntPtr cap, out UIntPtr needed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_load_compact(byte[] blob, UIntPtr len, int device, out IntPtr @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_add_client_compact(IntPtr a0, byte[] blob, UIntPtr len, out int slot);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_remove_client(IntPtr a0, int slot);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_set_key_slot(IntPtr a0, int slot);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_key_slot(IntPtr a0, out int slot);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_write(IntPtr a0, IntPtr a1, byte[] dst, UIntPtr cap, out UIntPtr needed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_read(IntPtr a0, byte[] text, UIntPtr len, out IntPtr @out, out UIntPtr consumed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_encrypt(IntPtr a0, double[] v, ulong dim, double scale, int format, out IntPtr @out);
@@ -83,8 +87,11 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_interleave(IntPtr a0, IntPtr[] vecs, int n, int shift, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_stack(IntPtr a0, IntPtr[] vecs, int n, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_generate_sparse_of_array(IntPtr a0, IntPtr[] vecs, int n, out IntPtr @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_rotate(IntPtr a0, IntPtr[] vecs, int n, int amount, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_stack_batch(IntPtr a0, IntPtr[] vecs, int n, int B, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_colmajor_sparse(IntPtr a0, IntPtr[] cols, int K, IntPtr sparse, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_rowmajor(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr v, int force_dense, out IntPtr @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_rowmajor_batch(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr[] vs, int B, int force_dense, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_rowmajor_shard(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr v, int force_dense, int first_row, int total_rows, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_conv_dense(IntPtr a0, IntPtr[] @in, int n_in, int[] gather, IntPtr[] weights, IntPtr[] bias, int M, int K, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_square(IntPtr a0, IntPtr[] @in, int n, IntPtr[] @out);
