@@ -30,6 +30,12 @@ struct NttTab {
     const double *wd_split;
     int split_ok, split_out_rc;
     const double *iwd_split;
+    // N = 4096 / 8192: the same halves' twiddles of the four unit-stride stages regrouped per thread for the fused kernels (ntt.cu,
+    // fwd_last_stages_grp / inv_first_stages_grp): thread j's 15 twiddles, padded to 16, as double2 groups [half][group 0..7][thread j
+    // of N/32], so a warp's load of one group is 512 contiguous bytes.  Forward (the last four stages of a half): group 0 = the first of
+    // them's twiddle and a pad word, 1 = the second's two, 2..3 the third's four, 4..7 the fourth's eight.  Inverse (stages 0..3):
+    // groups 0..3 stage 0, 4..5 stage 1, 6 stage 2, 7 = stage 3's twiddle and a pad word.  Built for the q and Bsk moduli only
+    const double *wd_split_grp, *iwd_split_grp;
     int fwd_out_rc;                    // lazy forward output must be re-centred (its bound squared would overflow the consumer's product)
     double fwd_out_bound;               // |forward lazy output| <= fwd_out_bound * p
 };

@@ -488,6 +488,19 @@ __device__ __forceinline__ void st_group16(double *sm, int j, const double (&x)[
 #pragma unroll
     for (int ch = 0; ch < 8; ch++) smv[j * 8 + (ch ^ xr)] = make_double2(x[2 * ch], x[2 * ch + 1]);
 }
+// stage LOGN-4+u of the forward transform on 16 consecutive coefficients; tw[i] is the twiddle of their i-th butterfly block (2^u of them)
+template <int U>
+__device__ __forceinline__ void fwd_last_stage(double (&x)[16], const double *tw, double p, double pinv) {
+    constexpr int h = 8 >> U;
+#pragma unroll
+    for (int e = 0; e < 16; e++) {
+        if (e & h) continue;
+        const double t = fmodmul(x[e + h], tw[e >> (4 - U)], p, pinv);
+        const double a = x[e];
+        x[e] = __dadd_rn(a, t);
+        x[e + h] = __dsub_rn(a, t);
+    }
+}
 // stages [LOGN-4, LOGN) of the forward transform on the 16 consecutive coefficients of group j (pass PASS of the schedule)
 template <int LOGN, int PASS>
 __device__ __forceinline__ void fwd_last_stages(double (&x)[16], const NttTab &tb, int j) {
@@ -515,19 +528,41 @@ __device__ __forceinline__ void fwd_last_stages(double (&x)[16], const NttTab &t
             tw[7 + 2 * i] = c.x; tw[8 + 2 * i] = c.y;
         }
     }
+    fwd_last_stage<0>(x, tw, p, pinv);
+    fwd_last_stage<1>(x, tw + 1, p, pinv);
+    fwd_last_stage<2>(x, tw + 3, p, pinv);
+    fwd_last_stage<3>(x, tw + 7, p, pinv);
+}
+// NG twiddle groups of one thread (grouped tables, NttTab::wd_split_grp): g points at its first group, groups are `stride` apart
+template <int NG>
+__device__ __forceinline__ void ld_tw_groups(double *tw, const double2 *g, int stride) {
 #pragma unroll
-    for (int u = 0; u < 4; u++) {
-        const int h = 8 >> u;
-#pragma unroll
-        for (int e = 0; e < 16; e++) {
-            if (e & h) continue;
-            const double w = tw[(1 << u) - 1 + (e >> (4 - u))];
-            const double t = fmodmul(x[e + h], w, p, pinv);
-            const double a = x[e];
-            x[e] = __dadd_rn(a, t);
-            x[e + h] = __dsub_rn(a, t);
-        }
+    for (int i = 0; i < NG; i++) {
+        const double2 v = __ldg(g + i * stride);
+        tw[2 * i] = v.x;
+        tw[2 * i + 1] = v.y;
     }
+}
+// The same on the half transforms of the fused kernels, twiddles from the grouped table (NttTab::wd_split_grp): g = this half's groups,
+// [group][LOGN-point transform's N/16 threads].  Each stage loads its own groups just before its butterflies: every warp load is 512
+// contiguous bytes, where the strided table puts the 32 lanes of the last stage's loads on 16 cache lines
+template <int LOGN, int PASS>
+__device__ __forceinline__ void fwd_last_stages_grp(double (&x)[16], const NttTab &tb, const double2 *g, int j) {
+    constexpr int T = (1 << LOGN) / 16;
+    const double p = tb.pd, pinv = tb.pinv;
+    if ((tb.fwd_recenter >> PASS) & 1) {
+#pragma unroll
+        for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
+    }
+    double tw[8];
+    tw[0] = __ldg(reinterpret_cast<const double *>(g + j)); // group 0: the twiddle and a pad word
+    fwd_last_stage<0>(x, tw, p, pinv);
+    ld_tw_groups<1>(tw, g + T + j, T);
+    fwd_last_stage<1>(x, tw, p, pinv);
+    ld_tw_groups<2>(tw, g + 2 * T + j, T);
+    fwd_last_stage<2>(x, tw, p, pinv);
+    ld_tw_groups<4>(tw, g + 4 * T + j, T);
+    fwd_last_stage<3>(x, tw, p, pinv);
 }
 // Last forward pass: stages [LOGN-4, LOGN) on 16 consecutive words; canonical result goes straight to HBM.
 template <int LOGN, int PASS, bool OUT_F>
@@ -631,11 +666,28 @@ k_ntt_forward_digits_fp(const u64 *target, size_t ct_stride, u64 *dst, const Ntt
     fwd_body_fp<LOGN, false, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (((size_t)c * k + l) * dm.D + d) * N, tb, tid); // [c][l][d]
 }
 
-// ---- inverse, FP64: stages 0..3 on the 16 consecutive coefficients of group j
+// ---- inverse, FP64: stage U (0..3) on 16 consecutive coefficients; tw[i] is the twiddle of their i-th butterfly block (8 >> U of them)
+template <int U>
+__device__ __forceinline__ void inv_first_stage(double (&x)[16], const double *tw, const NttTab &tb) {
+    constexpr int h = 1 << U;
+    const double p = tb.pd, pinv = tb.pinv;
+#pragma unroll
+    for (int e = 0; e < 16; e++) {
+        if (e & h) continue;
+        const double a = x[e], bq = x[e + h];
+        x[e] = __dadd_rn(a, bq);
+        x[e + h] = fmodmul(__dsub_rn(a, bq), tw[e >> (U + 1)], p, pinv);
+    }
+    if ((tb.inv_recenter >> U) & 1) { // uniform branch: the host schedules a re-centring of the sums on very few stages
+#pragma unroll
+        for (int e = 0; e < 16; e++)
+            if (!(e & h)) x[e] = frecenter(x[e], p, pinv);
+    }
+}
+// stages 0..3 on the 16 consecutive coefficients of group j
 template <int LOGN>
 __device__ __forceinline__ void inv_first_stages(double (&x)[16], const NttTab &tb, int j) {
     constexpr int N = 1 << LOGN;
-    const double p = tb.pd, pinv = tb.pinv;
     // stage u uses 8 >> u consecutive inverse twiddles: 8 + 4 + 2 + 1 doubles per thread, 16-byte loads
     double tw[15];
 #pragma unroll
@@ -653,24 +705,26 @@ __device__ __forceinline__ void inv_first_stages(double (&x)[16], const NttTab &
         tw[12] = a.x; tw[13] = a.y;
         tw[14] = __ldg(tb.iwd + ((N >> 4) + j));
     }
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-        const int h = 1 << u;
-        const bool rc = (tb.inv_recenter >> u) & 1;
-#pragma unroll
-        for (int e = 0; e < 16; e++) {
-            if (e & h) continue;
-            const double w = tw[(16 - (16 >> u)) + (e >> (u + 1))];
-            const double a = x[e], bq = x[e + h];
-            x[e] = __dadd_rn(a, bq);
-            x[e + h] = fmodmul(__dsub_rn(a, bq), w, p, pinv);
-        }
-        if (rc) { // uniform branch: the host schedules a re-centring of the sums on very few stages
-#pragma unroll
-            for (int e = 0; e < 16; e++)
-                if (!(e & h)) x[e] = frecenter(x[e], p, pinv);
-        }
-    }
+    inv_first_stage<0>(x, tw, tb);
+    inv_first_stage<1>(x, tw + 8, tb);
+    inv_first_stage<2>(x, tw + 12, tb);
+    inv_first_stage<3>(x, tw + 14, tb);
+}
+// The same on the half transforms of the fused kernels, twiddles from the grouped table (NttTab::iwd_split_grp): g = this half's groups,
+// [group][LOGN-point transform's N/16 threads].  Each stage loads its own groups just before its butterflies (all 15 twiddles at once
+// spill in k_behz_square_fused)
+template <int LOGN>
+__device__ __forceinline__ void inv_first_stages_grp(double (&x)[16], const NttTab &tb, const double2 *g, int j) {
+    constexpr int T = (1 << LOGN) / 16;
+    double tw[8];
+    ld_tw_groups<4>(tw, g + j, T);
+    inv_first_stage<0>(x, tw, tb);
+    ld_tw_groups<2>(tw, g + 4 * T + j, T);
+    inv_first_stage<1>(x, tw, tb);
+    ld_tw_groups<1>(tw, g + 6 * T + j, T);
+    inv_first_stage<2>(x, tw, tb);
+    tw[0] = __ldg(reinterpret_cast<const double *>(g + 7 * T + j)); // group 7: the twiddle and a pad word
+    inv_first_stage<3>(x, tw, tb);
 }
 // first pass reads 16 consecutive words per virtual thread straight from HBM (256-bit loads)
 template <int LOGN, bool IN_F>
@@ -1115,6 +1169,8 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
     tb.wd = tb.wd_split + half * H;
     tb.iwd = tb.iwd_split + half * H;
     tb.fwd_recenter = tb.fwd_recenter_split;
+    const double2 *twg = reinterpret_cast<const double2 *>(tb.wd_split_grp + half * H);   // last forward pass, grouped
+    const double2 *twgi = reinterpret_cast<const double2 *>(tb.iwd_split_grp + half * H); // first inverse stages, grouped
     const double p = tb.pd, pinv = tb.pinv;
     const bool need_reduce = dm.mask >= tb.mod.p;
     const u64 *src_c = target + (size_t)c * ct_stride;
@@ -1180,35 +1236,11 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
             unused.src = nullptr; unused.digit = false; unused.need_reduce = false; unused.shift = 0; unused.mask = 0;
             fwd_pass_fp<HLOGN, R1, 4, false, 1, false>(sm, twc, unused, tb, tid);
         }
-        __syncthreads();
+        __syncwarp(); // the middle pass wrote 256-coefficient block tid >> 4, whose groups 16j..16j+15 this half warp reads next
         // last pass (stages HLOGN-4 .. HLOGN-1 on 16 consecutive coefficients), then the key product
-        constexpr int S0 = HLOGN - 4;
-        const int j = tid, xr = j & 7;
-        const double2 *smv = reinterpret_cast<const double2 *>(sm);
         double x[16];
-#pragma unroll
-        for (int ch = 0; ch < 8; ch++) {
-            const double2 v = smv[j * 8 + (ch ^ xr)];
-            x[2 * ch] = v.x;
-            x[2 * ch + 1] = v.y;
-        }
-        if ((tb.fwd_recenter >> 2) & 1) {
-#pragma unroll
-            for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
-        }
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            const int h = 8 >> u;
-#pragma unroll
-            for (int e = 0; e < 16; e++) {
-                if (e & h) continue;
-                const double w = __ldg(tb.wd + (1 << (S0 + u)) + (j << u) + (e >> (4 - u)));
-                const double t = fmodmul(x[e + h], w, p, pinv);
-                const double a = x[e];
-                x[e] = __dadd_rn(a, t);
-                x[e + h] = __dsub_rn(a, t);
-            }
-        }
+        ld_group16(sm, tid, x);
+        fwd_last_stages_grp<HLOGN, 2>(x, tb, twg, tid);
         if (tb.split_out_rc) {
 #pragma unroll
             for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
@@ -1264,12 +1296,12 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
                 x[2 * i] = a.x;
                 x[2 * i + 1] = a.y;
             }
-            inv_first_stages<HLOGN>(x, tb, tid);
+            inv_first_stages_grp<HLOGN>(x, tb, twgi, tid);
             if (kp) __syncthreads();
             st_group16(sm + kp * H, tid, x);
         }
     }
-    __syncthreads();
+    __syncwarp(); // inv_pass_fp<.., 4, 4> works on 256-coefficient block tid >> 4 of each buffer: the groups this half warp just stored
 #pragma unroll 1
     for (int r = 0; r < 2; r++) CNHE_VTN(H / 16, (inv_pass_fp<HLOGN, 4, 4, false, false>(sm + r * H, twci, nullptr, nullptr, tb, vt)));
     __syncthreads();
@@ -1327,16 +1359,19 @@ k_behz_square_fused(const u64 *const *__restrict__ ct_ptrs, const u64 *__restric
     __syncthreads();
 #pragma unroll 1
     for (int r = 0; r < 2; r++) CNHE_VTN(H / 16, (fwd_pass_fp<HLOGN, R1, 4, false, 1, false>(sm + r * H, twc, fs, tb, vt)));
-    __syncthreads();
+    __syncwarp(); // the pass above wrote 256-coefficient block tid >> 4 of each buffer, whose groups 16j..16j+15 this half warp reads next
     {
         // thread j owns coefficients 16j .. 16j+15 of every buffer from the last forward pass to the first inverse pass: no barrier.
         // One group of 16 in registers per transform step (two plus the twiddles spill): c0 and c1 wait in their own slots
         const int j = tid;
+        const double2 *twg = reinterpret_cast<const double2 *>(tb.wd_split_grp + half * H);
+        const double2 *twgi = reinterpret_cast<const double2 *>(tb.iwd_split_grp + half * H);
         double x[16], y[16];
 #pragma unroll 1
         for (int r = 0; r < 2; r++) {
             ld_group16(sm + r * H, j, x);
-            fwd_last_stages<HLOGN, 2>(x, tb, j);
+            if constexpr (HLOGN == 12) fwd_last_stages_grp<HLOGN, 2>(x, tb, twg, j);
+            else fwd_last_stages<HLOGN, 2>(x, tb, j); // N = 4096: with the grouped loads ptxas spills 8 bytes here
             if (tb.split_out_rc) {
 #pragma unroll
                 for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
@@ -1347,7 +1382,7 @@ k_behz_square_fused(const u64 *const *__restrict__ ct_ptrs, const u64 *__restric
         ld_group16(sm + H, j, x);
 #pragma unroll
         for (int e = 0; e < 16; e++) x[e] = fmodmul(x[e], x[e], p, pinv);
-        inv_first_stages<HLOGN>(x, tb, j);
+        inv_first_stages_grp<HLOGN>(x, tb, twgi, j);
         st_group16(sm + 2 * H, j, x);
         ld_group16(sm, j, x);
         ld_group16(sm + H, j, y);
@@ -1356,14 +1391,14 @@ k_behz_square_fused(const u64 *const *__restrict__ ct_ptrs, const u64 *__restric
             const double cross = fmodmul(x[e], y[e], p, pinv);
             y[e] = __dadd_rn(cross, cross);
         }
-        inv_first_stages<HLOGN>(y, tb, j);
+        inv_first_stages_grp<HLOGN>(y, tb, twgi, j);
         st_group16(sm + H, j, y);
 #pragma unroll
         for (int e = 0; e < 16; e++) x[e] = fmodmul(x[e], x[e], p, pinv);
-        inv_first_stages<HLOGN>(x, tb, j);
+        inv_first_stages_grp<HLOGN>(x, tb, twgi, j);
         st_group16(sm, j, x);
     }
-    __syncthreads();
+    __syncwarp(); // inv_pass_fp<.., 4, 4> works on 256-coefficient block tid >> 4 of each buffer: the groups this half warp just stored
 #pragma unroll 1
     for (int r = 0; r < 3; r++) CNHE_VTN(H / 16, (inv_pass_fp<HLOGN, 4, 4, false, false>(sm + r * H, twci, nullptr, nullptr, tb, vt)));
     __syncthreads();

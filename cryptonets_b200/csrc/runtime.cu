@@ -501,7 +501,8 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     for (u64 p : c.q) moduli.push_back(p);
     for (u64 p : c.bsk) moduli.push_back(p);
     for (u64 p : c.t) moduli.push_back(p);
-    constexpr size_t TAB_WORDS = 9; // N-word tables per modulus: w, ws, iw, iws, wd, iwd, iwd_hi, wd_split, iwd_split
+    // N-word tables per modulus: w, ws, iw, iws, wd, iwd, iwd_hi, wd_split, iwd_split, wd_split_grp, iwd_split_grp
+    constexpr size_t TAB_WORDS = 11;
     std::vector<u64> host((size_t)n_mod * TAB_WORDS * N, 0);
     CNHE_CUDA(cudaMalloc((void **)&c.d_table_mem, host.size() * sizeof(u64)));
     c.h_tabs.resize(n_mod);
@@ -539,6 +540,23 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
                     iwd_split[h * H + i] = iwd[i + m2 + h * m2];
                 }
         }
+        if ((logN == 12 || logN == 13) && m < k + kb) { // per-thread twiddle groups of the fused kernels (see NttTab::wd_split_grp)
+            const u64 H = N / 2, T = H / 16, S0 = logN - 5; // S0: first of the half's last four forward stages
+            double *wd_grp = iwd_split + N, *iwd_grp = wd_grp + N;
+            for (u64 h = 0; h < 2; h++)
+                for (u64 j = 0; j < T; j++) {
+                    double f[16] = {}, v[16] = {}; // word 2g + e goes to element e of group g
+                    for (u64 u = 0; u < 4; u++) {
+                        for (u64 i = 0; i < (1u << u); i++) f[(u ? 1u << u : 0) + i] = wd_split[h * H + (1u << (S0 + u)) + (j << u) + i];
+                        for (u64 i = 0; i < (8u >> u); i++) v[16 - (16 >> u) + i] = iwd_split[h * H + (H >> (u + 1)) + (j << (3 - u)) + i];
+                    }
+                    for (u64 g = 0; g < 8; g++)
+                        for (u64 e = 0; e < 2; e++) {
+                            wd_grp[h * H + (g * T + j) * 2 + e] = f[2 * g + e];
+                            iwd_grp[h * H + (g * T + j) * 2 + e] = v[2 * g + e];
+                        }
+                }
+        }
         NttTab &tb = c.h_tabs[m];
         u64 *base = c.d_table_mem + (size_t)m * TAB_WORDS * N;
         tb.w = base; tb.ws = base + N; tb.iw = base + 2 * (size_t)N; tb.iws = base + 3 * (size_t)N;
@@ -547,6 +565,8 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
         tb.iwd_hi = reinterpret_cast<const double *>(base + 6 * (size_t)N);
         tb.wd_split = reinterpret_cast<const double *>(base + 7 * (size_t)N);
         tb.iwd_split = reinterpret_cast<const double *>(base + 8 * (size_t)N);
+        tb.wd_split_grp = reinterpret_cast<const double *>(base + 9 * (size_t)N);
+        tb.iwd_split_grp = reinterpret_cast<const double *>(base + 10 * (size_t)N);
         tb.inv_n = hm::inv(N % p, p);
         tb.inv_n_s = hm::shoup(tb.inv_n, p);
         tb.mod = make_dmod(p);

@@ -44,6 +44,27 @@ FMODMUL, BFLY = 6, 8
 DP_PER_THREAD = 16 * (FMODMUL + 1) + 12 * 8 * BFLY + 32 * (FMODMUL + 1) + 32 + 32
 DP_INVERSE_PER_THREAD = 2 * (12 * 8 * BFLY + 16 * (FMODMUL + 1) + 16)
 DP_WARP_INSTR_PER_CT = (DP_PER_THREAD * D + DP_INVERSE_PER_THREAD) * (256 // 32) * 2 * k
+
+
+def l1_wavefronts_per_cta_digit(key_word, grouped):
+    """128-byte L1 / shared-memory data-path wavefronts of one CTA and one digit (N = 8192: 4096-point half, 256 threads, 8 warps),
+    counted from the shapes: work buffer (pass-1 store, pass-2 load + store, last-pass load), accumulators (two polynomials, load +
+    store), twiddle-cache reads of passes 1-2 (15 distinct words per thread and pass, one wavefront per warp load), source words (both
+    halves, coalesced), key words (two polynomials, coalesced) and the last pass's 15 twiddles per thread: 8 warp loads of 512
+    contiguous bytes from the grouped table, or scalar loads whose lanes sit 2^u words apart at stage u (a warp load touches
+    min(32, 2^(u+1)) lines, 2^u loads per stage).  A model: not measured."""
+    H, T, W = 4096, 256, 8
+    work = 4 * H * 8 // 128
+    acc = 2 * 2 * H * 8 // 128
+    twc = 2 * 15 * W
+    src = 2 * H * 8 // 128
+    keys = int(2 * H * key_word) // 128
+    last = W * (8 * 4 if grouped else sum((1 << u) * min(32, 1 << (u + 1)) for u in range(4)))
+    return work + acc + twc + src + keys + last
+
+
+# FP64 issue cycles of the same CTA-digit: 8 warps x DP_PER_THREAD instructions at 2 warp instructions per clock per SM
+FP64_CYCLES_PER_CTA_DIGIT = DP_PER_THREAD * 8 / 2
 for n in args.n:
     host = (rng.integers(0, 1 << 62, (n, 3, k, N), dtype=np.uint64) % q[None, None, :, None]).astype(np.uint64)
     a = eng.dev_from(host)
@@ -73,6 +94,10 @@ for n in args.n:
         rate = DP_WARP_INSTR_PER_CT * n / (fam["keyswitch_mac"] * 1e-3)
         rec["fused_fp64_warp_instr_per_s"] = float("%.4g" % rate)
         rec["fused_fp64_issue_share"] = round(rate / 522.7e9, 3)  # 132 SMs x 2 FP64 warp instructions / clock x 1.98 GHz
+        # modelled L1 data-path load next to the FP64 pipe's, per CTA-digit: the library reads the grouped last-pass twiddles
+        wf = {lay: l1_wavefronts_per_cta_digit(key_word, lay == "grouped") for lay in ("strided", "grouped")}
+        rec["model_l1_wavefronts_per_cta_digit"] = wf
+        rec["model_l1_cycles_per_fp64_cycle"] = {lay: round(v / FP64_CYCLES_PER_CTA_DIGIT, 3) for lay, v in wf.items()}
         l2 = l2_packed if packed else l2_u64
         rec["fused_l2_bytes"] = {"u64_keys": l2_u64, "packed_keys": l2_packed}
         rec["fused_l2_tb_s"] = round(l2 / (fam["keyswitch_mac"] * 1e-3) / 1e12, 2)
