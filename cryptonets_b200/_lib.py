@@ -39,6 +39,11 @@ _SIGS = {
     "cnhe_vecs_rotate": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_vecs_stack_batch": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_mat_mul_rowmajor_batch": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
+    "cnhe_diag_prepare": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(C.c_void_p)],
+    "cnhe_diag_info": [C.c_void_p, C.POINTER(i32), U64P, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), U64P],
+    "cnhe_diag_export": [C.c_void_p, C.c_void_p, i32, i32, U64P, sz, C.POINTER(i32)],
+    "cnhe_diag_destroy": [C.c_void_p],
+    "cnhe_mat_mul_diagonal": [C.c_void_p, C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP)],
     "cnhe_vec_write": [C.c_void_p, VECP, C.c_void_p, sz, C.POINTER(sz)],
     "cnhe_vec_read": [C.c_void_p, C.c_char_p, sz, C.POINTER(VECP), C.POINTER(sz)],
     "cnhe_keys_generate_secure": [C.c_void_p],

@@ -1,0 +1,110 @@
+// Kernels of the diagonal (Halevi-Shoup) matrix-vector product with baby-step / giant-step (DESIGN.md section 4.10).
+//
+// Slot layout: slot i of a plaintext sits at row a = i / (N/2), column x = i % (N/2) (the BatchEncoder's matrix); rotate_rows(s) moves
+// column x + s of both rows to column x, rotate_columns swaps the rows.  Diagonal (b, s) of a matrix M holds, at slot (a, x), the weight
+// M[(a, x), (a ^ b, x + s mod N/2)].  With s = n1 g + h the stored plaintext is that diagonal rotated right by n1 g, so that
+//   y = sum_g rotate_rows(n1 g)( sum_{b,h} D'[g][b,h] (.) rotate_columns^b rotate_rows(h)(v) ).
+#include "fparith.cuh"
+#include "kernels.h"
+
+namespace cnhe {
+
+static inline unsigned diag_blocks(size_t threads) { return (unsigned)((threads + 255) / 256); }
+
+// flags[b * N/2 + s] = 1 when diagonal (b, s) of the R x dim matrix has a nonzero weight.  vals [R][N]: the rows' slot values mod t.
+__global__ void __launch_bounds__(256) k_diag_flags(const u64 *__restrict__ vals, int R, int dim, int logn, unsigned *__restrict__ flags) {
+    const int N = 1 << logn, half = N >> 1;
+    const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= (size_t)R << logn) return;
+    const int r = (int)(gid >> logn), bs = (int)(gid & (N - 1)); // bs = b * N/2 + s
+    const int b = bs >> (logn - 1), s = bs & (half - 1);
+    const int a = r >> (logn - 1), x = r & (half - 1);
+    const int col = ((a ^ b) << (logn - 1)) | ((x + s) & (half - 1));
+    if (col < dim && vals[(size_t)r * N + col] != 0) flags[bs] = 1;
+}
+
+// out[j][(a, x)] = M[(a, x - n1 g_j mod N/2), (a ^ b_j, x + h_j mod N/2)] (0 outside R x dim): the pre-rotated diagonal j, in slot order.
+// desc[j] = (b_j, n1 g_j, h_j).
+__global__ void __launch_bounds__(256) k_diag_gather(const u64 *__restrict__ vals, int R, int dim, const int3 *__restrict__ desc, int nd, int logn,
+                                                     u64 *__restrict__ out) {
+    const int N = 1 << logn, half = N >> 1;
+    const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= (size_t)nd << logn) return;
+    const int j = (int)(gid >> logn), i = (int)(gid & (N - 1));
+    const int3 d = desc[j];
+    const int a = i >> (logn - 1), x = i & (half - 1);
+    const int r = (a << (logn - 1)) | ((x - d.y) & (half - 1));
+    const int col = ((a ^ d.x) << (logn - 1)) | ((x + d.z) & (half - 1));
+    out[gid] = r < R && col < dim ? vals[(size_t)r * N + col] : 0;
+}
+
+// acc[g][b][p][l][i] = sum_{j in [g_start[g], g_start[g+1])} dhat[j][l][i] * xhat[xsel[j]][b][p][l][i]  (mod q_l, canonical out)
+// dhat: the wave's lifted diagonals in NTT form [nd][k][N]; xhat: the baby-step ciphertexts in NTT form [2 n1][B][2][k][N], canonical.
+// One thread per (g, l, i) keeps CB clients' two accumulators in registers, so a diagonal word is loaded once for CB clients and both
+// polynomials (B > CB: once per CB clients).  The CTAs of one (l, coefficient tile) are consecutive over g: the giant steps of a wave read
+// the same baby-step words at about the same time, and those reads are served by L2.  Arithmetic as in k_ks_mac_fp: fmodmul products of
+// canonical operands (|.| <= 0.51 q), summed with dadd and re-centred every 8 terms.
+template <int CB>
+__global__ void __launch_bounds__(256) k_diag_mac(const u64 *__restrict__ dhat, const u64 *__restrict__ xhat, const int *__restrict__ g_start,
+                                                  const int *__restrict__ xsel, u64 *__restrict__ acc, int ng, int B, int logn,
+                                                  const __grid_constant__ BehzConstF F) {
+    const int N = 1 << logn, k = F.k, tiles = N >> 8;
+    const int g = blockIdx.x % ng, tile = (blockIdx.x / ng) % tiles, l = blockIdx.x / (ng * tiles);
+    const int i = (tile << 8) + threadIdx.x;
+    const double p = F.qd[l], pinv = F.qinv[l];
+    const size_t kN = (size_t)k * N, ct = 2 * kN;
+    const int j0 = g_start[g], j1 = g_start[g + 1];
+    for (int b0 = 0; b0 < B; b0 += CB) {
+        double a[CB][2];
+#pragma unroll
+        for (int cb = 0; cb < CB; cb++) a[cb][0] = a[cb][1] = 0.0;
+        for (int j = j0; j < j1; j++) {
+            const double d = u2d(dhat[(size_t)j * kN + (size_t)l * N + i]);
+            const u64 *xs = xhat + ((size_t)xsel[j] * B + b0) * ct + (size_t)l * N + i;
+#pragma unroll
+            for (int cb = 0; cb < CB; cb++) {
+                if (b0 + cb < B) {
+                    a[cb][0] = __dadd_rn(a[cb][0], fmodmul(u2d(xs[cb * ct]), d, p, pinv));
+                    a[cb][1] = __dadd_rn(a[cb][1], fmodmul(u2d(xs[cb * ct + kN]), d, p, pinv));
+                }
+            }
+            if (((j - j0) & 7) == 7) { // sums of 8 fresh products stay below 4.1 q; re-centre before they could leave the exact range
+#pragma unroll
+                for (int cb = 0; cb < CB; cb++) {
+                    a[cb][0] = frecenter(a[cb][0], p, pinv);
+                    a[cb][1] = frecenter(a[cb][1], p, pinv);
+                }
+            }
+        }
+#pragma unroll
+        for (int cb = 0; cb < CB; cb++) {
+            if (b0 + cb >= B) break;
+            u64 *o = acc + ((size_t)g * B + b0 + cb) * ct + (size_t)l * N + i;
+            o[0] = fsmall_u(frecenter(a[cb][0], p, pinv), F.q_u[l]);
+            o[kN] = fsmall_u(frecenter(a[cb][1], p, pinv), F.q_u[l]);
+        }
+    }
+}
+
+cudaError_t launch_diag_flags(const u64 *vals, int R, int dim, int logn, unsigned *flags, cudaStream_t s) {
+    if (R <= 0) return cudaSuccess;
+    k_diag_flags<<<diag_blocks((size_t)R << logn), 256, 0, s>>>(vals, R, dim, logn, flags);
+    return cudaGetLastError();
+}
+cudaError_t launch_diag_gather(const u64 *vals, int R, int dim, const int *desc, int nd, int logn, u64 *out, cudaStream_t s) {
+    if (nd <= 0) return cudaSuccess;
+    k_diag_gather<<<diag_blocks((size_t)nd << logn), 256, 0, s>>>(vals, R, dim, reinterpret_cast<const int3 *>(desc), nd, logn, out);
+    return cudaGetLastError();
+}
+cudaError_t launch_diag_mac(const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B, int k, int logn,
+                            const BehzConstF *f, cudaStream_t s) {
+    if (ng <= 0 || B <= 0) return cudaSuccess;
+    const unsigned grid = (unsigned)ng * (unsigned)((1 << logn) >> 8) * (unsigned)k;
+    if (B == 1) k_diag_mac<1><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
+    else if (B == 2) k_diag_mac<2><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
+    else if (B <= 4) k_diag_mac<4><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
+    else k_diag_mac<8><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
+    return cudaGetLastError();
+}
+
+} // namespace cnhe

@@ -208,6 +208,16 @@ cudaError_t launch_ks_mac(const u64 *digits, const u64 *key, const u64 *const *k
                           cudaStream_t s);
 // split a size-3 array [n][3][k][N] view: base[n][2][k][N] = (c0,c1), c2[n][k][N]
 
+// ---- diagonal matrix-vector product (diag.cu; slot layout and indices there)
+// flags[b * N/2 + s] = 1 where diagonal (b, s) of the R x dim matrix whose rows' slot values are vals [R][N] has a nonzero weight
+// (flags is not cleared)
+cudaError_t launch_diag_flags(const u64 *vals, int R, int dim, int logn, unsigned *flags, cudaStream_t s);
+// out[j] (slot values [nd][N]) = diagonal (b, n1 g + h) rotated right by n1 g, desc[j] = (b, n1 g, h) as three ints (device)
+cudaError_t launch_diag_gather(const u64 *vals, int R, int dim, const int *desc, int nd, int logn, u64 *out, cudaStream_t s);
+// acc[g][b][p][l] = sum_{j = g_start[g]}^{g_start[g+1]-1} dhat[j][l] * xhat[xsel[j]][b][p][l]  (NTT form, canonical in and out; FP64 path)
+cudaError_t launch_diag_mac(const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B, int k, int logn,
+                            const BehzConstF *f, cudaStream_t s);
+
 // ---- sampling / encode / encrypt / decrypt
 enum SampleKind { SAMPLE_TERNARY = 0, SAMPLE_NOISE = 1, SAMPLE_UNIFORM = 2 };
 // out[i][l][x] for i<n: stream ids stream0 + i*stream_step (+ l for UNIFORM); lifted into each residue

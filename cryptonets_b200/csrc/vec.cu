@@ -2289,3 +2289,311 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
     }
     API_END
 }
+
+// ---------------------------------------------------------------------------------------------------- diagonal matrix-vector product
+// A plain matrix prepared for the diagonal (Halevi-Shoup) product with baby-step / giant-step (DESIGN.md section 4.10, slot layout in
+// diag.cu): its nonzero generalised diagonals (b, s = n1 g + h), each rotated right by n1 g and encoded, ordered by g, then b, then h.
+struct DiagEntry { int b, g, h; };
+struct cnhe_diag {
+    Context *ctx = nullptr;
+    int n_rows = 0;
+    uint64_t dim = 0;
+    double scale = 1.0;
+    int n1 = 1, n2 = 1;
+    std::vector<DiagEntry> diags;
+    std::vector<BufRef> plains; // per channel: [diags][N] plaintexts, coefficient form mod t
+};
+// key switches of rotate_rows(steps), 0 <= steps < N/2, on a context holding the Galois elements c.galois_elts: one with the step's own
+// key, else one per NAF term (rotate_internal's hops; a term of N/2 is skipped)
+static std::vector<int> rotation_hops(const Context &c) {
+    const int half = (int)(c.N / 2);
+    const u64 m = 2ULL * c.N;
+    std::vector<int> hops(half, 0);
+    u64 e = 1;
+    for (int s = 1; s < half; s++) {
+        e = (e * 3) & (m - 1);
+        if (std::find(c.galois_elts.begin(), c.galois_elts.end(), e) != c.galois_elts.end()) { hops[s] = 1; continue; }
+        for (int v = s, i = 0; v; i++) {
+            const int zi = (v & 1) ? 2 - (v & 3) : 0;
+            v = (v - zi) >> 1;
+            if (zi && (1 << i) != half) hops[s]++;
+        }
+    }
+    return hops;
+}
+// key switches per input vector with n1 baby steps: rotate_rows(h) of v -- and of rotate_columns(v), one more, when a diagonal has b = 1 --
+// for every h a nonzero diagonal (b, n1 g + h) uses, and rotate_rows(n1 g) for every g that has one.  nz: [2][N/2] nonzero flags
+static long diag_cost(const std::vector<char> &nz, const std::vector<int> &hops, int n1) {
+    const int half = (int)hops.size();
+    std::vector<char> baby(2 * (size_t)n1, 0), giant(half / n1, 0);
+    for (int b = 0; b < 2; b++)
+        for (int s = 0; s < half; s++)
+            if (nz[(size_t)b * half + s]) { baby[(size_t)b * n1 + s % n1] = 1; giant[s / n1] = 1; }
+    long cost = 0;
+    for (int h = 0; h < n1; h++) {
+        if (baby[h]) cost += hops[h];
+        if (baby[n1 + h]) cost += hops[h];
+    }
+    for (int h = 0; h < n1; h++)
+        if (baby[n1 + h]) { cost += 1; break; }
+    for (int g = 1; g < half / n1; g++)
+        if (giant[g]) cost += hops[(size_t)n1 * g];
+    return cost;
+}
+
+extern "C" int cnhe_diag_prepare(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int baby_steps, cnhe_diag **out) {
+    API_BEGIN(h)
+    if (!rows || !out || n_rows < 1) fail("bad arguments");
+    const size_t N = c.N;
+    const int half = (int)(N / 2);
+    for (int r = 0; r < n_rows; r++) {
+        same_ctx(c, rows[r]);
+        if (rows[r]->enc) fail("the diagonal product takes a plain matrix");
+        if (rows[r]->format != CNHE_DENSE) fail("Expecting dense vector format");
+        if (rows[r]->blocks != 1) fail("the diagonal product expects single-block rows");
+        if (rows[r]->dim != rows[0]->dim) fail("Dimensions do not match");
+        if (rows[r]->scale != rows[0]->scale) fail("row scales differ");
+    }
+    if ((size_t)n_rows > N) fail("more rows than slots");
+    if (baby_steps < 0 || (baby_steps & (baby_steps - 1)) || baby_steps > half) fail("baby_steps must be 0 or a power of two dividing N/2");
+    const int R = n_rows, dim = (int)rows[0]->dim;
+    std::unique_ptr<cnhe_diag> d(new cnhe_diag());
+    d->ctx = &c;
+    d->n_rows = R;
+    d->dim = rows[0]->dim;
+    d->scale = rows[0]->scale;
+    // every channel's rows decoded to slot values, and the diagonals with a nonzero weight in some channel
+    std::vector<BufRef> vals(c.P), flags(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        WsScope scope(c);
+        u64 *plain = c.ws_alloc((size_t)R * N);
+        for (int r = 0; r < R; r++)
+            CNHE_CUDA(cudaMemcpyAsync(plain + (size_t)r * N, rows[r]->ptr(ch), N * 8, cudaMemcpyDeviceToDevice, c.stream));
+        vals[ch] = c.alloc((size_t)R * N);
+        op_decode(c, ch, plain, R, vals[ch]->p);
+        flags[ch] = c.alloc(N / 2); // N unsigned flags
+        CNHE_CUDA(cudaMemsetAsync(flags[ch]->p, 0, N * sizeof(unsigned), c.stream));
+        c.check(launch_diag_flags(vals[ch]->p, R, dim, c.logN, reinterpret_cast<unsigned *>(flags[ch]->p), c.stream), "diag_flags");
+    }
+    std::vector<char> nz(N, 0);
+    {
+        std::vector<unsigned> hf(N);
+        for (int ch = 0; ch < c.P; ch++) {
+            c.set_channel(ch);
+            CNHE_CUDA(cudaMemcpyAsync(hf.data(), flags[ch]->p, N * sizeof(unsigned), cudaMemcpyDeviceToHost, c.stream));
+            CNHE_CUDA(cudaStreamSynchronize(c.stream));
+            for (size_t i = 0; i < N; i++) nz[i] |= hf[i] != 0;
+        }
+    }
+    const std::vector<int> hops = rotation_hops(c);
+    int n1 = baby_steps;
+    if (!n1) {
+        long best = -1;
+        for (int t = 1; t <= half; t *= 2) {
+            const long cost = diag_cost(nz, hops, t);
+            if (best < 0 || cost < best) { best = cost; n1 = t; }
+        }
+    }
+    d->n1 = n1;
+    d->n2 = half / n1;
+    for (int g = 0; g < d->n2; g++)
+        for (int b = 0; b < 2; b++)
+            for (int hh = 0; hh < n1; hh++)
+                if (nz[(size_t)b * half + g * n1 + hh]) d->diags.push_back({b, g, hh});
+    if (d->diags.empty()) d->diags.push_back({0, 0, 0}); // an all-zero matrix keeps one (zero) diagonal: its product is an encryption of 0
+    const int nd = (int)d->diags.size();
+    std::vector<int> desc((size_t)3 * nd);
+    for (int j = 0; j < nd; j++) {
+        desc[3 * j] = d->diags[j].b;
+        desc[3 * j + 1] = n1 * d->diags[j].g;
+        desc[3 * j + 2] = d->diags[j].h;
+    }
+    d->plains.resize(c.P);
+    const int DW = 2048; // diagonals gathered per wave
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        WsScope scope(c);
+        d->plains[ch] = c.alloc((size_t)nd * N);
+        int *ddesc = reinterpret_cast<int *>(c.ws_alloc(((size_t)3 * nd + 1) / 2));
+        c.h2d(ddesc, desc.data(), desc.size() * sizeof(int));
+        for (int j0 = 0; j0 < nd; j0 += DW) {
+            WsScope wave(c);
+            const int m = std::min(DW, nd - j0);
+            u64 *dv = c.ws_alloc((size_t)m * N);
+            c.check(launch_diag_gather(vals[ch]->p, R, dim, ddesc + 3 * j0, m, c.logN, dv, c.stream), "diag_gather");
+            op_encode(c, ch, dv, m, (int)N, d->plains[ch]->p + (size_t)j0 * N);
+        }
+    }
+    c.sync();
+    *out = d.release();
+    API_END
+}
+
+extern "C" int cnhe_diag_info(const cnhe_diag *d, int *n_rows, uint64_t *dim, int *n1, int *n2, int *n_diags, uint64_t *device_bytes) {
+    if (!d) return set_err(CNHE_ERR_INVALID, "null matrix");
+    if (n_rows) *n_rows = d->n_rows;
+    if (dim) *dim = d->dim;
+    if (n1) *n1 = d->n1;
+    if (n2) *n2 = d->n2;
+    if (n_diags) *n_diags = (int)d->diags.size();
+    if (device_bytes) *device_bytes = (uint64_t)d->plains.size() * d->diags.size() * d->ctx->N * 8;
+    return CNHE_OK;
+}
+
+extern "C" int cnhe_diag_export(cnhe_ctx *h, const cnhe_diag *d, int channel, int index, uint64_t *dst, size_t cap_words, int *bgh) {
+    API_BEGIN(h)
+    if (!d || d->ctx != &c) fail("matrix belongs to another context");
+    if (channel < 0 || channel >= c.P || index < 0 || index >= (int)d->diags.size()) fail("index out of range");
+    if (dst) {
+        if (cap_words < c.N) fail("buffer too small");
+        c.set_channel(channel);
+        CNHE_CUDA(cudaMemcpyAsync(dst, d->plains[channel]->p + (size_t)index * c.N, c.N * 8, cudaMemcpyDeviceToHost, c.stream));
+        CNHE_CUDA(cudaStreamSynchronize(c.stream));
+    }
+    if (bgh) {
+        bgh[0] = d->diags[index].b;
+        bgh[1] = d->diags[index].g;
+        bgh[2] = d->diags[index].h;
+    }
+    API_END
+}
+
+extern "C" int cnhe_diag_destroy(cnhe_diag *d) {
+    if (!d) return CNHE_OK;
+    try {
+        std::lock_guard<std::recursive_mutex> lock(d->ctx->mu);
+        cudaSetDevice(d->ctx->device);
+        delete d;
+    } catch (...) { return set_err(CNHE_ERR_INVALID, "destroy failed"); }
+    return CNHE_OK;
+}
+
+// y = sum_g rotate_rows(n1 g)( sum_{b,h} D'[g][b,h] (.) rotate_columns^b rotate_rows(h)(v) ) for B vectors at once (one per client; their key
+// slots may differ).  Per channel: the baby-step rotations of every client in one op_rotate_rows_multi (after one column rotation per
+// client when a diagonal has b = 1), their forward transforms, then waves of giant steps -- the wave's diagonals lifted and transformed,
+// every client's inner sums in the NTT domain (k_diag_mac; dyadic products and additions off the FP64 path: the same residues), the
+// inverse transforms -- and finally the giant-step rotations of every (g, client) in one op_rotate_rows_multi and each client's sum.
+// Each inner sum equals the sum of the separate multiply_plain results, since the inverse transform is linear mod q_l.
+extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe_vec *const *vs, int B, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (!d || !vs || !out || B < 1) fail("bad arguments");
+    if (d->ctx != &c) fail("matrix belongs to another context");
+    for (int b = 0; b < B; b++) {
+        same_ctx(c, vs[b]);
+        if (!vs[b]->enc) fail("at least one parameter has to be encrypted");
+        if (vs[b]->format != CNHE_DENSE) fail("Expecting dense vector format");
+        if (vs[b]->blocks != 1) fail("the diagonal product expects a single-block vector");
+        if (vs[b]->dim != d->dim) fail("Dimensions do not match");
+        if (vs[b]->scale != vs[0]->scale) fail("the input vectors must share scale");
+    }
+    const std::vector<int> vslot = vec_slots(c, vs, B);
+    const size_t N = c.N, ctw = c.ct_words(), kN = (size_t)c.k * N;
+    const int k = c.k, n1 = d->n1, nd = (int)d->diags.size();
+    // baby steps in use and their place in the baby-step buffer; giant steps in use and where their diagonals start
+    std::vector<int> xidx(2 * (size_t)n1, -1), xsel(nd), gs, gstart;
+    for (const DiagEntry &e : d->diags) xidx[(size_t)e.b * n1 + e.h] = 0;
+    int nx = 0;
+    for (int &x : xidx)
+        if (x == 0) x = nx++;
+    bool col = false;
+    for (int j = 0; j < nd; j++) {
+        const DiagEntry &e = d->diags[j];
+        xsel[j] = xidx[(size_t)e.b * n1 + e.h];
+        col = col || e.b == 1;
+        if (j == 0 || e.g != d->diags[j - 1].g) { gs.push_back(e.g); gstart.push_back(j); }
+    }
+    gstart.push_back(nd);
+    const int ng = (int)gs.size();
+    bool fp = c.fp_elementwise;
+    for (int l = 0; l < k; l++) fp = fp && c.h_tabs[l].fp_ok;
+    const int fpq = fp ? 1 : 0;
+    std::vector<std::unique_ptr<cnhe_vec>> outs(B);
+    for (int b = 0; b < B; b++) {
+        outs[b].reset(new_vec(c, (uint64_t)d->n_rows, vs[0]->scale * d->scale, CNHE_DENSE, true, 1));
+        outs[b]->slot = vslot[b];
+        alloc_channels(outs[b].get());
+    }
+    // diagonals per wave: their lifted NTT forms stay under 8 GiB (a wave always takes at least one giant step)
+    const int cap = (int)std::max<size_t>(1, ((size_t)1 << 30) / kN);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        WsScope scope(c);
+        // baby steps: X[xidx[b n1 + h]][client] = rotate_rows(h)(rotate_columns^b(v)), then their NTT forms
+        u64 *X = c.ws_alloc((size_t)nx * B * ctw);
+        u64 *kv = col ? c.ws_alloc((size_t)B * ctw) : nullptr;
+        if (col)
+            for (int b = 0; b < B; b++) op_rotate_columns(c, ch, vs[b]->ptr(ch), 1, kv + (size_t)b * ctw, &vslot[b]);
+        {
+            std::vector<RotateJob> jobs;
+            for (int i = 0; i < 2 * n1; i++) {
+                if (xidx[i] < 0) continue;
+                for (int b = 0; b < B; b++)
+                    jobs.push_back({i >= n1 ? kv + (size_t)b * ctw : vs[b]->ptr(ch), i % n1, X + ((size_t)xidx[i] * B + b) * ctw, vslot[b]});
+            }
+            op_rotate_rows_multi(c, ch, jobs);
+        }
+        op_ntt(c, X, X, nx * B * 2 * k, 0, k, false);
+        u64 *acc = c.ws_alloc((size_t)ng * B * ctw); // [g][client], coefficient form once its wave is done
+        const int *dxsel = nullptr;
+        if (fp) {
+            int *p = reinterpret_cast<int *>(c.ws_alloc(((size_t)nd + 1) / 2));
+            c.h2d(p, xsel.data(), (size_t)nd * sizeof(int));
+            dxsel = p;
+        }
+        for (int gi0 = 0; gi0 < ng;) {
+            WsScope wave(c);
+            int gi1 = gi0 + 1;
+            while (gi1 < ng && gstart[gi1 + 1] - gstart[gi0] <= cap) gi1++;
+            const int j0 = gstart[gi0], m = gstart[gi1] - j0, gw = gi1 - gi0;
+            u64 *L = c.ws_alloc((size_t)m * kN);
+            c.check(launch_plain_lift(d->plains[ch]->p + (size_t)j0 * N, L, m, (int)N, k, c.logN, c.d_bc, c.ch[ch].pc, c.stream), "plain_lift");
+            op_ntt(c, L, L, m * k, 0, k, false);
+            u64 *A = acc + (size_t)gi0 * B * ctw;
+            if (fp) {
+                std::vector<int> st(gw + 1);
+                for (int i = 0; i <= gw; i++) st[i] = gstart[gi0 + i] - j0;
+                int *dst = reinterpret_cast<int *>(c.ws_alloc(((size_t)gw + 2) / 2));
+                c.h2d(dst, st.data(), st.size() * sizeof(int));
+                c.check(launch_diag_mac(L, X, dst, dxsel + j0, A, gw, B, k, c.logN, &c.h_bf, c.stream), "diag_mac");
+            } else {
+                u64 *tmp = c.ws_alloc((size_t)B * ctw);
+                for (int gi = gi0; gi < gi1; gi++) {
+                    u64 *Ag = acc + (size_t)gi * B * ctw;
+                    for (int j = gstart[gi]; j < gstart[gi + 1]; j++) {
+                        const u64 *xs = X + (size_t)xsel[j] * B * ctw, *dj = L + (size_t)(j - j0) * kN;
+                        if (j == gstart[gi]) { c.check(launch_dyadic_bcast(xs, dj, Ag, B, 2, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic"); continue; }
+                        c.check(launch_dyadic_bcast(xs, dj, tmp, B, 2, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic");
+                        c.check(launch_ct_add(Ag, tmp, Ag, (size_t)B * ctw, k, c.logN, c.d_bc, 0, c.stream), "ct_add");
+                    }
+                }
+            }
+            op_ntt(c, A, A, gw * B * 2 * k, 0, k, true);
+            gi0 = gi1;
+        }
+        c.note(Context::OP_MULTIPLY_PLAIN, ch, B * nd);
+        if (nd > ng) c.note(Context::OP_ADD, ch, B * (nd - ng));
+        // giant steps, in place, then each client's sum over g
+        {
+            std::vector<RotateJob> jobs;
+            for (int gi = 0; gi < ng; gi++)
+                for (int b = 0; b < B; b++) {
+                    u64 *p = acc + ((size_t)gi * B + b) * ctw;
+                    jobs.push_back({p, n1 * gs[gi], p, vslot[b]});
+                }
+            op_rotate_rows_multi(c, ch, jobs);
+        }
+        for (int b = 0; b < B; b++) {
+            if (ng == 1) {
+                CNHE_CUDA(cudaMemcpyAsync(outs[b]->ptr(ch), acc + (size_t)b * ctw, ctw * 8, cudaMemcpyDeviceToDevice, c.stream));
+                c.note_copy(outs[b]->ptr(ch), acc + (size_t)b * ctw);
+                continue;
+            }
+            std::vector<const u64 *> terms;
+            for (int gi = 0; gi < ng; gi++) terms.push_back(acc + ((size_t)gi * B + b) * ctw);
+            do_add_many(c, ch, terms, outs[b]->ptr(ch));
+        }
+    }
+    for (int b = 0; b < B; b++) out[b] = outs[b].release();
+    API_END
+}

@@ -98,6 +98,43 @@ class Vec:
         return p.value, w.value
 
 
+class Diag:
+    """Owning handle of a cnhe_diag: a plain matrix prepared for the diagonal (baby-step / giant-step) product."""
+
+    __slots__ = ("eng", "h", "__weakref__")
+
+    def __init__(self, eng, handle):
+        self.eng = eng
+        self.h = C.c_void_p(handle) if not isinstance(handle, C.c_void_p) else handle
+        eng._live.add(self)
+
+    def dispose(self):
+        if self.h:
+            if self.eng.h:
+                self.eng.L.cnhe_diag_destroy(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.dispose()
+        except Exception:
+            pass
+
+    def info(self):
+        """dict(n_rows, dim, n1, n2, n_diags, device_bytes): n1 baby steps, n2 giant steps, the stored (nonzero) diagonals."""
+        r, n1, n2, nd = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        dim, nb = C.c_uint64(), C.c_uint64()
+        check(self.eng.L.cnhe_diag_info(self.h, C.byref(r), C.byref(dim), C.byref(n1), C.byref(n2), C.byref(nd), C.byref(nb)))
+        return dict(n_rows=r.value, dim=dim.value, n1=n1.value, n2=n2.value, n_diags=nd.value, device_bytes=nb.value)
+
+    def export(self, channel, index):
+        """(plaintext coefficients mod t [N], (b, g, h)) of stored diagonal `index` (stored by g, then b, then h)."""
+        out = np.zeros(self.eng.N, np.uint64)
+        bgh = (C.c_int * 3)()
+        check(self.eng.L.cnhe_diag_export(self.eng.h, self.h, int(channel), int(index), _p(out), out.size, bgh))
+        return out, (bgh[0], bgh[1], bgh[2])
+
+
 class Engine:
     """One cnhe_ctx: parameters, device tables and keys for P plaintext moduli (== EncryptedSealBfvFactory)."""
 
@@ -530,6 +567,21 @@ class Engine:
         out = VECP()
         check(self.L.cnhe_mat_mul_rowmajor_shard(self.h, _vec_array(rows), len(rows), v.h, int(force_dense), int(first_row), int(total_rows), C.byref(out)))
         return Vec(self, out)
+
+    def diag_prepare(self, rows, baby_steps=0):
+        """The plain row vectors of a matrix (as mat_mul_rowmajor takes them) prepared for mat_mul_diagonal; baby_steps = 0 lets the library
+        pick n1.  The rows may be disposed afterwards."""
+        out = C.c_void_p()
+        check(self.L.cnhe_diag_prepare(self.h, _vec_array(rows), len(rows), int(baby_steps), C.byref(out)))
+        return Diag(self, out)
+
+    def mat_mul_diagonal(self, diag, vs):
+        """The diagonal product of a prepared matrix with every encrypted vector of vs (one per client; their key slots may differ): each
+        output decrypts to mat_mul_rowmajor(rows, v, force_dense=True)."""
+        B = len(vs)
+        out = (VECP * B)()
+        check(self.L.cnhe_mat_mul_diagonal(self.h, diag.h, _vec_array(vs), B, out))
+        return self._wrap_many(out, B)
 
     def layer_conv_dense(self, inputs, gather, weights, bias, M, K):
         g = None

@@ -179,6 +179,13 @@ class B200BfvMatrix:
             raise Exception("Internal probloem: expecting the output to be dense")
         return total
 
+    def PrepareDiagonal(self, baby_steps=0):
+        """This plain row-major matrix prepared for the diagonal (baby-step / giant-step) product, B200BfvFactory.MulDiagonalBatch; the
+        rows stay owned by this matrix.  baby_steps = 0 picks the number of baby steps with the fewest key switches."""
+        if self.Format != EMatrixFormat.RowMajor:
+            raise Exception("the diagonal product expects a RowMajor matrix")
+        return B200BfvDiagonalMatrix(self.factory, self.eng.diag_prepare([r.vec for r in self.vectors], baby_steps))
+
     def _check(self, m):
         if m.Format != self.Format:
             raise Exception("Format mismatch")
@@ -234,6 +241,25 @@ class B200BfvMatrix:
         if self.Format != EMatrixFormat.ColumnMajor:
             raise Exception("Expecting ColumnMajor matrix")
         return B200BfvVector(self.factory, self.eng.interleave([v.vec for v in self.vectors], shift))
+
+
+class B200BfvDiagonalMatrix:
+    """A plain matrix held as its pre-rotated generalised diagonals on the device (include/cnhe.h, cnhe_diag_prepare)."""
+
+    def __init__(self, factory, diag):
+        self.factory = factory
+        self.diag = diag
+
+    def Info(self):
+        return self.diag.info()
+
+    RowCount = property(lambda s: s.diag.info()["n_rows"])
+    ColumnCount = property(lambda s: s.diag.info()["dim"])
+
+    def Dispose(self):
+        if self.diag is not None:
+            self.diag.dispose()
+            self.diag = None
 
 
 def _read_block(reader, end_marker):
@@ -369,6 +395,11 @@ class B200BfvFactory:
         """weights.Mul(v, ForceDenseFormat=...) of a plain row-major matrix for every v (one per client) in one pass."""
         out = self.engine.mat_mul_rowmajor_batch([r.vec for r in weights.vectors], [v.vec for v in vectors], ForceDenseFormat)
         return [B200BfvVector(self, o) for o in out]
+
+    def MulDiagonalBatch(self, diag, vectors):
+        """diag (B200BfvMatrix.PrepareDiagonal) times every encrypted vector (one per client; key slots may differ) in one pass; each result
+        decrypts to the matrix's Mul(v, ForceDenseFormat=True)."""
+        return [B200BfvVector(self, o) for o in self.engine.mat_mul_diagonal(diag.diag, [v.vec for v in vectors])]
 
     def GetMatrix(self, vectors, fmt, CopyVectors=True):
         return B200BfvMatrix(self, vectors, fmt, CopyVectors=CopyVectors)

@@ -522,6 +522,11 @@ class LLDenseLayer(BaseLayer):
         self.WeightsMatrix = None
         self.BiasVector = None
         self.Shard = None  # (rank, world, process group): split the rows of this layer over the ranks of ONE inference (SURVEY.md 8e)
+        # "rows": the reference's product (per row a multiply, SumAllSlots and a one-hot mask); "diagonal": the baby-step / giant-step
+        # diagonal product (DESIGN.md section 4.10), same decrypted output, ForceDenseFormat with a dense input only, no Shard.  The Raw
+        # backend computes M v directly either way.
+        self.Method = "rows"
+        self.DiagonalMatrix = None
         self._first_row = 0
         super().__init__(**kw)
 
@@ -533,6 +538,12 @@ class LLDenseLayer(BaseLayer):
             return
         if self.ForceDenseFormat and self.InputFormat == EVectorFormat.sparse:
             raise Exception("forcing dense format is only available when the input is dense")
+        if self.Method not in ("rows", "diagonal"):
+            raise Exception("unknown dense layer method %r" % (self.Method,))
+        if self.Method == "diagonal" and not (self.ForceDenseFormat and self.InputFormat == EVectorFormat.dense):
+            raise Exception("the diagonal method needs ForceDenseFormat and a dense input")
+        if self.Method == "diagonal" and self.Shard is not None:
+            raise Exception("the diagonal method cannot be combined with Shard")
         f = self.Factory
         rows = len(self.Bias)
         w = np.asarray(self.Weights, dtype=np.float64).reshape(rows, -1)
@@ -549,6 +560,10 @@ class LLDenseLayer(BaseLayer):
         else:
             self.BiasVector = f.GetPlainVector(np.asarray(self.Bias), EVectorFormat.dense, bscale)
             self.WeightsMatrix = f.GetPlainMatrix(w, EMatrixFormat.ColumnMajor, self.WeightsScale)
+        if self.Method == "diagonal" and hasattr(self.WeightsMatrix, "PrepareDiagonal"):
+            self.DiagonalMatrix = self.WeightsMatrix.PrepareDiagonal()
+            self.WeightsMatrix.Dispose()  # the diagonals replace the row plaintexts
+            self.WeightsMatrix = None
         self.layerPrepared = True
 
     def OutputDimension(self):
@@ -558,7 +573,9 @@ class LLDenseLayer(BaseLayer):
         if m.ColumnCount > 1:
             raise Exception("Expecting only one column")
         env = self.Factory.AllocateComputationEnv()
-        if self.Shard is not None:
+        if self.DiagonalMatrix is not None:
+            mul = self.Factory.MulDiagonalBatch(self.DiagonalMatrix, [m.GetColumn(0)])[0]
+        elif self.Shard is not None:
             from . import parallel
             rank, world, group = self.Shard
             rows = len(self.Bias)
@@ -578,6 +595,13 @@ class LLDenseLayer(BaseLayer):
     def ApplyBatch(self, ms):
         """Every client's row-major product in one pass (cnhe_mat_mul_rowmajor_batch), then each one's bias."""
         f = self.Factory
+        if self.DiagonalMatrix is not None:  # every client's diagonal product in one pass
+            env = f.AllocateComputationEnv()
+            out = []
+            for mul in f.MulDiagonalBatch(self.DiagonalMatrix, [self._single_column(m) for m in ms]):
+                out.append(f.GetMatrix([mul.Add(self.BiasVector, env)], EMatrixFormat.ColumnMajor, CopyVectors=False))
+                mul.Dispose()
+            return out
         batch = getattr(f, "MulRowMajorBatch", None)
         if (batch is None or len(ms) < 2 or self.Shard is not None or self.InputFormat != EVectorFormat.dense or not self.WeightsMatrix.Batched
                 or any(m.ColumnCount != 1 or not m.GetColumn(0).IsEncrypted or m.GetColumn(0).vec.blocks != 1 for m in ms)):
@@ -589,12 +613,20 @@ class LLDenseLayer(BaseLayer):
             mul.Dispose()
         return out
 
+    @staticmethod
+    def _single_column(m):
+        if m.ColumnCount > 1:
+            raise Exception("Expecting only one column")
+        return m.GetColumn(0)
+
     def Dispose(self):
         if self.WeightsMatrix is not None:
             self.WeightsMatrix.Dispose()
+        if self.DiagonalMatrix is not None:
+            self.DiagonalMatrix.Dispose()
         if self.BiasVector is not None:
             self.BiasVector.Dispose()
-        self.WeightsMatrix = self.BiasVector = None
+        self.WeightsMatrix = self.DiagonalMatrix = self.BiasVector = None
 
 
 class LLSingleLineReader(MatrixSource):

@@ -246,6 +246,28 @@ int cnhe_mat_mul_rowmajor_shard(cnhe_ctx *, const cnhe_vec *const *rows, int n_r
  * bit-identical to cnhe_mat_mul_rowmajor(rows, n_rows, vs[b], force_dense), the key switches of all B x n_rows products share waves. */
 int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, int force_dense,
                                 cnhe_vec **out /*B*/);
+/* Diagonal (Halevi-Shoup) product with baby-step / giant-step, the opt-in alternative to the ForceDenseFormat row-major product above for
+ * large dense layers: about sqrt(N) rotations per input instead of 14 per row, and no one-hot mask multiply (DESIGN.md section 4.10).
+ * Slot i sits at row i / (N/2), column i % (N/2) of the BatchEncoder's matrix.  Diagonal (b, s) of a matrix M (b in {0, 1}, s < N/2)
+ * holds M[(a, x), (a ^ b, x + s mod N/2)] at slot (a, x); with s = n1 g + h it is stored rotated right by n1 g, and
+ *   y = sum_g rotate_rows(n1 g)( sum_{b,h} diag'(b, n1 g + h) (.) rotate_columns^b rotate_rows(h)(v) ).
+ * cnhe_diag_prepare: rows are n_rows <= N plain, dense, single-block vectors of one dim and one scale (what cnhe_mat_mul_rowmajor takes);
+ *   the diagonals are formed, pre-rotated and encoded on the GPU, all-zero ones dropped (an all-zero matrix keeps one zero diagonal).
+ *   baby_steps: n1, a power of two dividing N/2, or 0 to take the n1 with the fewest key switches per input, counted from the rotation hops
+ *   over the context's Galois elements.  Anything else is CNHE_ERR_INVALID.  The rows may be destroyed afterwards.
+ * cnhe_diag_info: rows, dim, n1, n2 = N/2 / n1, stored diagonals and the device bytes they hold (any pointer may be NULL).
+ * cnhe_diag_export: stored diagonal `index` of a channel (N coefficients, mod t) and its (b, g, h) in bgh[3] (either may be NULL);
+ *   diagonals are stored by g, then b, then h.
+ * cnhe_mat_mul_diagonal: out[b] = M vs[b] for B encrypted, dense, single-block vectors of dim M's dim and one scale; their key slots may
+ *   differ, out[b] keeps vs[b]'s.  out[b] is dense of dim n_rows and scale vs.scale * row scale, and decrypts to what
+ *   cnhe_mat_mul_rowmajor(rows, vs[b], force_dense = 1) decrypts to (it is a different ciphertext).  A missing Galois key is CNHE_ERR_STATE.
+ *   Counted as row-rotation hops, column rotations, plain multiplications, additions and one AddMany per output. */
+typedef struct cnhe_diag cnhe_diag;
+int cnhe_diag_prepare(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, int baby_steps, cnhe_diag **out);
+int cnhe_diag_info(const cnhe_diag *, int *n_rows, uint64_t *dim, int *n1, int *n2, int *n_diags, uint64_t *device_bytes);
+int cnhe_diag_export(cnhe_ctx *, const cnhe_diag *, int channel, int index, uint64_t *dst, size_t cap_words, int *bgh);
+int cnhe_diag_destroy(cnhe_diag *);
+int cnhe_mat_mul_diagonal(cnhe_ctx *, const cnhe_diag *, const cnhe_vec *const *vs, int B, cnhe_vec **out /*B*/);
 /* Whole PoolLayer.Apply with weights ("NeuralNetworks/PoolLayer.cs:149-229"): out[m] = sum_k weights[m][k] * in[gather[m*K+k]]
  * + bias[m].  The inputs may belong to different key slots (several clients' images side by side) as long as each output's taps share
  * one; the output takes it.  weights[m] is a plain SPARSE vector of dim K, bias[m] a plain DENSE vector (or NULL); gather < 0 is a
