@@ -1036,14 +1036,17 @@ u64 galois_elt_from_step(const Context &c, int steps) { // Evaluator::galois_elt
     for (u64 i = 0; i < s; i++) e = (e * 3) & (m - 1);
     return e;
 }
+static u64 galois_inverse(uint32_t N, u64 elt) { // elt^-1 mod 2N
+    const u64 m2 = 2ULL * N;
+    for (u64 x = 1; x < m2; x += 2)
+        if (((x * elt) & (m2 - 1)) == 1) return x;
+    return 0;
+}
 void op_apply_galois(Context &c, int ch, const u64 *in, int n, u64 elt, u64 *out, bool add_back, const int *slots) {
     const KsKeys keys = galois_keys(c, ch, n, slots, elt);
     const int k = c.k;
     const size_t N = c.N;
-    const u64 m2 = 2ULL * N;
-    u64 einv = 0;
-    for (u64 x = 1; x < m2; x += 2)
-        if (((x * elt) & (m2 - 1)) == 1) { einv = x; break; }
+    const u64 m2 = 2ULL * N, einv = galois_inverse(c.N, elt);
     for (int c0 = 0; c0 < n; c0 += c.chunk) {
         const int m = std::min(c.chunk, n - c0);
         u64 *base = c.ws_alloc((size_t)m * 2 * k * N), *p1 = c.ws_alloc((size_t)m * k * N);
@@ -1062,16 +1065,21 @@ bool op_rotate_add(Context &c, int ch, const u64 *in, int n, int steps, bool col
     op_apply_galois(c, ch, in, n, elt, out, true, slots);
     return true;
 }
-static std::vector<int> naf(int value) { // non-adjacent form, least significant term first (SEAL util::naf)
+std::vector<int> naf_hops(uint32_t N, int steps) {
     std::vector<int> res;
-    const bool sign = value < 0;
-    int v = sign ? -value : value;
-    for (int i = 0; v; i++) {
+    const bool sign = steps < 0;
+    int v = sign ? -steps : steps;
+    for (int i = 0; v; i++) { // non-adjacent form, least significant term first (SEAL util::naf)
         const int zi = (v & 1) ? 2 - (v & 3) : 0;
         v = (v - zi) >> 1;
-        if (zi) res.push_back((sign ? -zi : zi) * (1 << i));
+        if (zi && (1u << i) != N / 2) res.push_back((sign ? -zi : zi) * (1 << i));
     }
     return res;
+}
+// the row rotations a rotation by `steps` (!= 0) is made of: the step itself when every ciphertext's key slot holds its key, else its hops
+static std::vector<int> row_hops(const Context &c, int ch, int n, const int *slots, int steps) {
+    if (has_galois(c, ch, n, slots, galois_elt_from_step(c, steps))) return {steps};
+    return naf_hops(c.N, steps);
 }
 void op_rotate_rows(Context &c, int ch, const u64 *in, int n, int steps, u64 *out, const int *slots) { // Evaluator::rotate_internal
     const size_t words = (size_t)n * c.ct_words();
@@ -1079,18 +1087,14 @@ void op_rotate_rows(Context &c, int ch, const u64 *in, int n, int steps, u64 *ou
         if (in != out) { CNHE_CUDA(cudaMemcpyAsync(out, in, words * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(out, in); }
         return;
     }
-    const u64 elt = galois_elt_from_step(c, steps);
-    if (has_galois(c, ch, n, slots, elt)) { op_apply_galois(c, ch, in, n, elt, out, false, slots); return; }
-    std::vector<int> hops = naf(steps);
-    if (hops.size() == 1) throw Error(-3, "Galois key not present");
+    // each hop takes its own Galois key: a missing one is CNHE_ERR_STATE
+    const std::vector<int> hops = row_hops(c, ch, n, slots, steps);
     const u64 *cur = in;
     for (size_t h = 0; h < hops.size(); h++) {
-        if ((size_t)std::abs(hops[h]) == (c.N >> 1)) continue;
-        u64 *nxt = (h + 1 == hops.size()) ? out : c.ws_alloc(words);
-        op_rotate_rows(c, ch, cur, n, hops[h], nxt, slots);
+        u64 *nxt = h + 1 == hops.size() ? out : c.ws_alloc(words);
+        op_apply_galois(c, ch, cur, n, galois_elt_from_step(c, hops[h]), nxt, false, slots);
         cur = nxt;
     }
-    if (cur != out) { CNHE_CUDA(cudaMemcpyAsync(out, cur, words * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(out, cur); }
 }
 void op_rotate_columns(Context &c, int ch, const u64 *in, int n, u64 *out, const int *slots) {
     op_apply_galois(c, ch, in, n, 2ULL * c.N - 1, out, false, slots);
@@ -1101,10 +1105,7 @@ static void apply_galois_gather(Context &c, int ch, const std::vector<const u64 
     const int k = c.k, n = (int)ins.size();
     const KsKeys keys = galois_keys(c, ch, n, slots, elt);
     const size_t N = c.N;
-    const u64 m2 = 2ULL * N;
-    u64 einv = 0;
-    for (u64 x = 1; x < m2; x += 2)
-        if (((x * elt) & (m2 - 1)) == 1) { einv = x; break; }
+    const u64 m2 = 2ULL * N, einv = galois_inverse(c.N, elt);
     for (int c0 = 0; c0 < n; c0 += c.chunk) {
         const int m = std::min(c.chunk, n - c0);
         std::vector<const u64 *> part(ins.begin() + c0, ins.begin() + c0 + m);
@@ -1126,17 +1127,9 @@ void op_rotate_rows_multi(Context &c, int ch, const std::vector<RotateJob> &jobs
     std::vector<int> slots(jobs.size());
     for (size_t j = 0; j < jobs.size(); j++) slots[j] = jobs[j].slot < 0 ? c.slot : jobs[j].slot;
     for (size_t j = 0; j < jobs.size(); j++) {
-        const RotateJob &job = jobs[j];
         st[j].next = 0;
-        st[j].cur = job.src;
-        if (job.steps == 0) continue;
-        const u64 elt = galois_elt_from_step(c, job.steps);
-        if (has_galois(c, ch, (int)slots.size(), slots.data(), elt)) st[j].hops = {job.steps};
-        else {
-            for (int h : naf(job.steps))
-                if ((size_t)std::abs(h) != (c.N >> 1)) st[j].hops.push_back(h); // rotate_internal skips a hop of exactly N/2
-            if (naf(job.steps).size() == 1) throw Error(-3, "Galois key not present");
-        }
+        st[j].cur = jobs[j].src;
+        if (jobs[j].steps) st[j].hops = row_hops(c, ch, (int)slots.size(), slots.data(), jobs[j].steps);
     }
     for (;;) {
         // the hop value most jobs are waiting for next
@@ -1484,14 +1477,10 @@ static KeyRandom sampled(u64 purpose_a, u64 purpose_e, u64 key_tag) {
 // receives the permuted second part
 static void galois_secret(Context &c, const u64 *sk_coeff, u64 elt, u64 *rs) {
     const size_t kN = (size_t)c.k * c.N;
-    const u64 m2 = 2ULL * c.N;
-    u64 einv = 0;
-    for (u64 x = 1; x < m2; x += 2)
-        if (((x * elt) & (m2 - 1)) == 1) { einv = x; break; }
     u64 *pair = c.ws_alloc(2 * kN), *base = c.ws_alloc(2 * kN);
     CNHE_CUDA(cudaMemcpyAsync(pair, sk_coeff, kN * 8, cudaMemcpyDeviceToDevice, c.stream));
     CNHE_CUDA(cudaMemcpyAsync(pair + kN, sk_coeff, kN * 8, cudaMemcpyDeviceToDevice, c.stream));
-    c.check(launch_galois(pair, base, rs, 1, einv, c.k, c.logN, c.d_bc, c.stream), "galois");
+    c.check(launch_galois(pair, base, rs, 1, galois_inverse(c.N, elt), c.k, c.logN, c.d_bc, c.stream), "galois");
     c.check(launch_ntt_forward(rs, rs, c.k, c.logN, c.d_tabs, 0, c.k, fp_range(c, 0, c.k), c.stream), "ntt_forward");
 }
 static void keys_generate_impl(Context &c, bool secure, u64 seed) {

@@ -241,6 +241,9 @@ void op_rotate_columns(Context &c, int ch, const u64 *in, int n, u64 *out, const
 struct RotateJob { const u64 *src; int steps; u64 *dst; int slot = -1; };
 void op_rotate_rows_multi(Context &c, int ch, const std::vector<RotateJob> &jobs);
 u64 galois_elt_from_step(const Context &c, int steps);
+// the hops of a row rotation by `steps` whose Galois key is missing (Evaluator::rotate_internal): the NAF terms of steps, least significant
+// first, without a term of +-N/2, which maps each row of N/2 slots onto itself
+std::vector<int> naf_hops(uint32_t N, int steps);
 // dense plaintext (coefficient form mod t, [n or 1][N]) times ciphertexts [n][2kN]
 void op_multiply_plain_dense(Context &c, int ch, const u64 *ct, int n, const u64 *plain, bool plain_per_ct, u64 *out);
 void op_multiply_plain_dense_bcast(Context &c, int ch, const u64 *ct, const u64 *plains, int n, u64 *out);

@@ -344,6 +344,14 @@ void alloc_channels(cnhe_vec *v) {
         v->buf[ch] = v->ctx->alloc((size_t)v->blocks * v->unit());
     }
 }
+// v's blocks as a view of one slab per channel, starting `ct` ciphertexts in: the outputs of a batched call share one allocation
+static cnhe_vec *slab_view(cnhe_vec *v, const std::vector<BufRef> &slab, size_t ct) {
+    for (int ch = 0; ch < v->ctx->P; ch++) {
+        v->buf[ch] = slab[ch];
+        v->off[ch] = ct * v->ctx->ct_words();
+    }
+    return v;
+}
 static cnhe_vec *alias_of(const cnhe_vec *a) { return new cnhe_vec(*a); } // shares the reference-counted buffers
 void same_ctx(Context &c, const cnhe_vec *v) {
     if (!v) fail("null vector");
@@ -516,15 +524,7 @@ extern "C" int cnhe_vecs_encrypt(cnhe_ctx *h, const double *v, int n, uint64_t d
         op_encrypt(c, ch, plain, N, n * bl, (int)N, take_nonces(c, ch, (u64)n * bl), big[ch]->p);
         c.sync();
     }
-    for (int i = 0; i < n; i++) {
-        cnhe_vec *o = new_vec(c, dim, scale, CNHE_DENSE, true, bl);
-        for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-            o->buf[ch] = big[ch];
-            o->off[ch] = (size_t)i * bl * c.ct_words();
-        }
-        out[i] = o;
-    }
+    for (int i = 0; i < n; i++) out[i] = slab_view(new_vec(c, dim, scale, CNHE_DENSE, true, bl), big, (size_t)i * bl);
     API_END
 }
 
@@ -694,12 +694,7 @@ extern "C" int cnhe_vecs_import_raw(cnhe_ctx *h, const uint64_t *src, int n, int
         CNHE_CUDA(cudaEventRecord(c.ev_copy, c.copy_stream));
         CNHE_CUDA(cudaStreamWaitEvent(c.stream, c.ev_copy, 0));
     }
-    for (int i = 0; i < n; i++) {
-        cnhe_vec *o = new_vec(c, dim, scale, format, true, blocks);
-        for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch); o->buf[ch] = big[ch]; o->off[ch] = (size_t)i * per; }
-        out[i] = o;
-    }
+    for (int i = 0; i < n; i++) out[i] = slab_view(new_vec(c, dim, scale, format, true, blocks), big, (size_t)i * blocks);
     API_END
 }
 // ---------------------------------------------------------------------------------------- compact upload (format: csrc/compact.cu)
@@ -798,7 +793,6 @@ extern "C" int cnhe_vecs_import_compact(cnhe_ctx *h, const uint8_t *src, size_t 
     *n = (int)hd.n;
     if (cap < (int)hd.n) fail("output array too small for the blob's vectors");
     const int nct = (int)(hd.n * hd.B);
-    const size_t per = (size_t)hd.B * c.ct_words();
     std::vector<BufRef> big(c.P);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
@@ -810,14 +804,7 @@ extern "C" int cnhe_vecs_import_compact(cnhe_ctx *h, const uint8_t *src, size_t 
         CNHE_CUDA(cudaEventRecord(c.ev_copy, c.copy_stream));
         CNHE_CUDA(cudaStreamWaitEvent(c.stream, c.ev_copy, 0));
     }
-    for (uint32_t i = 0; i < hd.n; i++) {
-        cnhe_vec *o = new_vec(c, hd.dim, hd.scale, CNHE_DENSE, true, (int)hd.B);
-        for (int ch = 0; ch < c.P; ch++) {
-            o->buf[ch] = big[ch];
-            o->off[ch] = (size_t)i * per;
-        }
-        out[i] = o;
-    }
+    for (uint32_t i = 0; i < hd.n; i++) out[i] = slab_view(new_vec(c, hd.dim, hd.scale, CNHE_DENSE, true, (int)hd.B), big, (size_t)i * hd.B);
     API_END
 }
 // ---------------------------------------------------------------------------------------- compact key sets (format: csrc/compact.cu)
@@ -1240,6 +1227,28 @@ extern "C" int cnhe_vec_pointwise_multiply(cnhe_ctx *h, const cnhe_vec *a, const
     API_END
 }
 
+// The rotate-and-add ladder of SumAllSlots (AtomicSealBfvVector.cs:888-955) on n single-block ciphertexts in place, one key-switch wave per
+// step for all n; returns the summed length.  slots: per-ciphertext key slots (nullptr: the call's slot)
+static uint64_t sum_slots_batched(Context &c, int ch, u64 *cts, int n, uint64_t length, const int *slots = nullptr) {
+    const size_t N = c.N, words = (size_t)n * c.ct_words();
+    uint64_t len = length;
+    u64 *tmp = c.ws_alloc(words);
+    // every step is x += rotate(x): fused into the rotation (the permutation kernel folds x into the key switch's base) when the step
+    // has its own Galois key -- it does for the powers of two the ladder walks -- else rotate, then add
+    if (len >= N / 2) {
+        if (!op_rotate_add(c, ch, cts, n, 0, true, cts, slots)) {
+            op_rotate_columns(c, ch, cts, n, tmp, slots);
+            do_add(c, ch, cts, tmp, cts, words, 0);
+        }
+        len = N / 2;
+    }
+    for (uint64_t steps = 1; steps < len; steps *= 2) { // RotateRowsAndAdd(sum, steps): RotateRows(c, -steps)
+        if (op_rotate_add(c, ch, cts, n, -(int)steps, false, cts, slots)) continue;
+        op_rotate_rows(c, ch, cts, n, -(int)steps, tmp, slots);
+        do_add(c, ch, cts, tmp, cts, words, 0);
+    }
+    return len;
+}
 // SumAllSlots (AtomicSealBfvVector.cs:888-955)
 static cnhe_vec *sum_all_slots(Context &c, const cnhe_vec *a, uint64_t length, int force_column) {
     if (a->format != CNHE_DENSE) fail("Expecting dense vector format");
@@ -1254,7 +1263,6 @@ static cnhe_vec *sum_all_slots(Context &c, const cnhe_vec *a, uint64_t length, i
     alloc_channels(o);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
-        len = length;
         u64 *sum = o->ptr(ch);
         if (a->blocks > 1) { // AddMany over the blocks
             std::vector<const u64 *> ptrs = block_ptrs(a, ch);
@@ -1262,19 +1270,7 @@ static cnhe_vec *sum_all_slots(Context &c, const cnhe_vec *a, uint64_t length, i
         } else {
             CNHE_CUDA(cudaMemcpyAsync(sum, a->ptr(ch), ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(sum, a->ptr(ch));
         }
-        u64 *tmp = c.ws_alloc(ctw);
-        if (len >= N / 2) {
-            if (!op_rotate_add(c, ch, sum, 1, 0, true, sum)) { // x += rotate(x) in one pass when the step has its own key
-                op_rotate_columns(c, ch, sum, 1, tmp);
-                do_add(c, ch, sum, tmp, sum, ctw, 0);
-            }
-            len = N / 2;
-        }
-        for (uint64_t steps = 1; steps < len; steps *= 2) { // RotateRowsAndAdd(sum, steps): RotateRows(c, -steps)
-            if (op_rotate_add(c, ch, sum, 1, -(int)steps, false, sum)) continue;
-            op_rotate_rows(c, ch, sum, 1, -(int)steps, tmp);
-            do_add(c, ch, sum, tmp, sum, ctw, 0);
-        }
+        len = sum_slots_batched(c, ch, sum, 1, length);
         if (force_column >= 0) { // one-hot mask (":936-945")
             if ((size_t)force_column >= N) fail("column out of range");
             std::vector<u64> onehot(N, 0);
@@ -1524,81 +1520,61 @@ static void interleave_finish(Context &c, int ch, const std::vector<const cnhe_v
         }
     }
 }
-static void interleave_channel(Context &c, int ch, const std::vector<const cnhe_vec *> &vecs, int shift, int out_blocks, u64 *out) {
-    std::vector<Placed> placed;
-    std::vector<RotateJob> jobs;
-    interleave_place(c, ch, vecs, shift, out_blocks, c.slot, placed, jobs);
-    op_rotate_rows_multi(c, ch, jobs);
-    interleave_finish(c, ch, vecs, shift, out_blocks, placed, out);
-}
-static cnhe_vec *interleave(Context &c, const cnhe_vec *const *vecs, int n, int shift) { // AtomicSealBfvVector.cs:729-750
-    if (n < 1) fail("empty array");
-    std::vector<const cnhe_vec *> vv(vecs, vecs + n);
-    for (auto v : vv) { same_ctx(c, v); if (!v->enc) fail("expecting encrypted vectors"); }
-    use_slot(c, vecs, n);
-    if (vv[0]->format != CNHE_DENSE) fail("Expecting dense vector");
-    int out_blocks = 1;
-    if (shift > 0) out_blocks = (int)std::ceil((double)(vv[0]->dim * (uint64_t)n) / (double)c.N);
-    cnhe_vec *o = new_vec(c, vv[0]->dim, vv[0]->scale, CNHE_DENSE, true, out_blocks);
-    std::unique_ptr<cnhe_vec> guard(o);
-    alloc_channels(o);
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        interleave_channel(c, ch, vv, shift, out_blocks, o->ptr(ch));
-    }
-    return guard.release();
-}
-extern "C" int cnhe_vecs_interleave(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int shift, cnhe_vec **out) {
-    API_BEGIN(h)
-    *out = interleave(c, vecs, n, shift);
-    API_END
-}
-extern "C" int cnhe_vecs_stack(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, cnhe_vec **out) { // AtomicSealBfvVector.cs:756-761
-    API_BEGIN(h)
-    if (n < 1) fail("empty array");
-    cnhe_vec *o = interleave(c, vecs, n, (int)vecs[0]->dim);
-    o->dim = vecs[0]->dim * (uint64_t)n;
-    *out = o;
-    API_END
-}
-// cnhe_vecs_stack of B groups of n vectors each (one LoLa vectorize layer per client; the groups' key slots may differ): out[b] is
-// bit-identical to cnhe_vecs_stack(vecs + b * n, n).  The rotations of all groups run as one set of jobs (one key-switch wave per hop
-// for all clients), then each group's masks and sums.
-extern "C" int cnhe_vecs_stack_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int B, cnhe_vec **out) {
-    API_BEGIN(h)
+// Interleave (AtomicSealBfvVector.cs:729-750) of B groups of n vectors each, one output per group; the groups' key slots may differ (one
+// LoLa vectorize layer per client).  The rotations of all groups run as one set of jobs (one key-switch wave per hop for all groups), then
+// each group's masks and sums under its own slot: out[b] is bit-identical to the interleave of group b alone.  stack: Stack
+// (":756-761"), the interleave with shift = dim whose output has dimension dim * n; otherwise every group takes `shift`.
+static void interleave_groups(Context &c, const cnhe_vec *const *vecs, int n, int B, int shift, bool stack, cnhe_vec **out) {
     if (n < 1 || B < 1 || !vecs || !out) fail("bad arguments");
-    std::vector<std::vector<const cnhe_vec *>> groups(B);
-    std::vector<int> gslot(B), out_blocks(B);
+    struct Group { std::vector<const cnhe_vec *> vecs; int shift, out_blocks, slot; std::vector<Placed> placed; };
+    std::vector<Group> gs(B);
+    bool foreign = false;
     for (int b = 0; b < B; b++) {
-        groups[b].assign(vecs + (size_t)b * n, vecs + (size_t)(b + 1) * n);
-        for (auto v : groups[b]) { same_ctx(c, v); if (!v->enc) fail("expecting encrypted vectors"); }
-        if (groups[b][0]->format != CNHE_DENSE) fail("Expecting dense vector");
-        gslot[b] = use_slot(c, groups[b].data(), n);
-        const int shift = (int)groups[b][0]->dim;
-        out_blocks[b] = shift > 0 ? (int)std::ceil((double)(groups[b][0]->dim * (uint64_t)n) / (double)c.N) : 1;
+        Group &g = gs[b];
+        g.vecs.assign(vecs + (size_t)b * n, vecs + (size_t)(b + 1) * n);
+        for (auto v : g.vecs) { same_ctx(c, v); if (!v->enc) fail("expecting encrypted vectors"); }
+        if (g.vecs[0]->format != CNHE_DENSE) fail("Expecting dense vector");
+        g.slot = use_slot(c, g.vecs.data(), n);
+        foreign = foreign || g.slot != 0;
+        g.shift = stack ? (int)g.vecs[0]->dim : shift;
+        g.out_blocks = g.shift > 0 ? (int)std::ceil((double)(g.vecs[0]->dim * (uint64_t)n) / (double)c.N) : 1;
     }
-    for (int b = 0; b < B; b++) c.foreign = c.foreign || gslot[b] != 0;
+    c.foreign = foreign;
     std::vector<std::unique_ptr<cnhe_vec>> outs(B);
     for (int b = 0; b < B; b++) {
-        c.slot = gslot[b];
-        outs[b].reset(new_vec(c, groups[b][0]->dim, groups[b][0]->scale, CNHE_DENSE, true, out_blocks[b]));
+        c.slot = gs[b].slot;
+        outs[b].reset(new_vec(c, gs[b].vecs[0]->dim, gs[b].vecs[0]->scale, CNHE_DENSE, true, gs[b].out_blocks));
         alloc_channels(outs[b].get());
     }
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
-        std::vector<std::vector<Placed>> placed(B);
         std::vector<RotateJob> jobs;
-        for (int b = 0; b < B; b++) interleave_place(c, ch, groups[b], (int)groups[b][0]->dim, out_blocks[b], gslot[b], placed[b], jobs);
+        for (Group &g : gs) interleave_place(c, ch, g.vecs, g.shift, g.out_blocks, g.slot, g.placed, jobs);
         op_rotate_rows_multi(c, ch, jobs);
         for (int b = 0; b < B; b++) {
-            c.slot = gslot[b];
-            interleave_finish(c, ch, groups[b], (int)groups[b][0]->dim, out_blocks[b], placed[b], outs[b]->ptr(ch));
+            c.slot = gs[b].slot;
+            interleave_finish(c, ch, gs[b].vecs, gs[b].shift, gs[b].out_blocks, gs[b].placed, outs[b]->ptr(ch));
         }
     }
     for (int b = 0; b < B; b++) {
-        outs[b]->dim = groups[b][0]->dim * (uint64_t)n;
+        if (stack) outs[b]->dim *= (uint64_t)n;
         out[b] = outs[b].release();
     }
+}
+extern "C" int cnhe_vecs_interleave(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int shift, cnhe_vec **out) {
+    API_BEGIN(h)
+    interleave_groups(c, vecs, n, 1, shift, false, out);
+    API_END
+}
+extern "C" int cnhe_vecs_stack(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, cnhe_vec **out) {
+    API_BEGIN(h)
+    interleave_groups(c, vecs, n, 1, 0, true, out);
+    API_END
+}
+// cnhe_vecs_stack of B groups of n vectors each: out[b] is bit-identical to cnhe_vecs_stack(vecs + b * n, n)
+extern "C" int cnhe_vecs_stack_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int B, cnhe_vec **out) {
+    API_BEGIN(h)
+    interleave_groups(c, vecs, n, B, 0, true, out);
     API_END
 }
 
@@ -2017,14 +1993,8 @@ static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int
             }
     }
     for (int m = 0; m < M; m++) {
-        cnhe_vec *o = new_vec(c, in[0]->dim, out_scale, CNHE_DENSE, true, bl);
-        o->slot = out_slot[m];
-        for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-            o->buf[ch] = big[ch];
-            o->off[ch] = (size_t)m * bl * c.ct_words();
-        }
-        out[m] = o;
+        out[m] = slab_view(new_vec(c, in[0]->dim, out_scale, CNHE_DENSE, true, bl), big, (size_t)m * bl);
+        out[m]->slot = out_slot[m];
     }
 }
 extern "C" int cnhe_layer_conv_dense(cnhe_ctx *h, const cnhe_vec *const *in, int n_in, const int32_t *gather, const cnhe_vec *const *weights,
@@ -2082,101 +2052,17 @@ extern "C" int cnhe_mat_mul_colmajor_sparse(cnhe_ctx *h, const cnhe_vec *const *
     }
     API_END
 }
-// Batched SumAllSlots (AtomicSealBfvVector.cs:888-955) on n single-block ciphertexts in place: the same rotate-and-add ladder,
-// one key-switch wave per step for all n.
-// slots: per-ciphertext key slots (nullptr: the call's slot)
-static uint64_t sum_slots_batched(Context &c, int ch, u64 *cts, int n, uint64_t length, const int *slots = nullptr) {
-    const size_t N = c.N, words = (size_t)n * c.ct_words();
-    uint64_t len = length;
-    u64 *tmp = c.ws_alloc(words);
-    // every step is x += rotate(x): fused into the rotation (the permutation kernel folds x into the key switch's base) when the step
-    // has its own Galois key -- it does for the powers of two the ladder walks -- else rotate, then add
-    if (len >= N / 2) {
-        if (!op_rotate_add(c, ch, cts, n, 0, true, cts, slots)) {
-            op_rotate_columns(c, ch, cts, n, tmp, slots);
-            do_add(c, ch, cts, tmp, cts, words, 0);
-        }
-        len = N / 2;
-    }
-    for (uint64_t steps = 1; steps < len; steps *= 2) {
-        if (op_rotate_add(c, ch, cts, n, -(int)steps, false, cts, slots)) continue;
-        op_rotate_rows(c, ch, cts, n, -(int)steps, tmp, slots);
-        do_add(c, ch, cts, tmp, cts, words, 0);
-    }
-    return len;
-}
 // RowMajor matrix x vector (EncryptedSealBfvMatrix.cs:79-120): per row DotProduct(row, v) = PointwiseMultiply + SumAllSlots, then
 // GenerateSparseOfArray, or (ForceDenseFormat) a one-hot mask per row and the sum of all rows.  All rows go through each stage
 // together instead of one DotProduct per row.
-extern "C" int cnhe_mat_mul_rowmajor(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *v, int force_dense, cnhe_vec **out) {
-    return cnhe_mat_mul_rowmajor_shard(h, rows, n_rows, v, force_dense, 0, n_rows, out);
-}
-// The same product for a contiguous SLICE of the matrix rows (rows[i] is global row first_row + i of a matrix with total_rows rows):
-// the unit of the intra-inference multi-GPU split (SURVEY.md 8e: CIFAR's 5488 dense rows over 4 GPUs).  ForceDense: the one-hot masks sit
-// at the global columns, so the partial results of the ranks add up to the full product (the reference sums the masked rows too,
-// EncryptedSealBfvMatrix.cs:92-116); otherwise the output holds this slice's sparse elements only.
-extern "C" int cnhe_mat_mul_rowmajor_shard(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *v, int force_dense, int first_row,
-                                           int total_rows, cnhe_vec **out) {
-    API_BEGIN(h)
-    if (n_rows < 1) fail("empty matrix");
-    if (first_row < 0 || first_row + n_rows > total_rows) fail("row slice out of range");
-    same_ctx(c, v);
-    if (!v->enc) fail("at least one parameter has to be encrypted");
-    use_slot(c, {v});
-    if (v->format != CNHE_DENSE) fail("Expecting dense vector format");
-    if (v->blocks != 1) fail("row-major multiplication expects a single-block vector");
-    for (int r = 0; r < n_rows; r++) {
-        same_ctx(c, rows[r]);
-        if (rows[r]->enc) fail("encrypted rows are not supported by the batched row-major product");
-        if (rows[r]->dim != v->dim) fail("Dimensions do not match");
-        if (rows[r]->format != v->format) fail("Format mismatch");
-        if (rows[r]->scale != rows[0]->scale) fail("row scales differ");
-    }
-    const size_t N = c.N, ctw = c.ct_words();
-    if (force_dense && (size_t)total_rows > N) fail("column out of range");
-    const int out_blocks = force_dense ? 1 : n_rows;
-    cnhe_vec *o = new_vec(c, (uint64_t)(force_dense ? total_rows : n_rows), v->scale * rows[0]->scale, force_dense ? CNHE_DENSE : CNHE_SPARSE, true, out_blocks);
-    std::unique_ptr<cnhe_vec> guard(o);
-    alloc_channels(o);
-    const int RC = 1024; // rows per wave
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        bool first = true;
-        for (int r0 = 0; r0 < n_rows; r0 += RC) {
-            WsScope scope(c);
-            const int m = std::min(RC, n_rows - r0);
-            u64 *plains = c.ws_alloc((size_t)m * N);
-            for (int i = 0; i < m; i++)
-                CNHE_CUDA(cudaMemcpyAsync(plains + (size_t)i * N, rows[r0 + i]->ptr(ch), N * 8, cudaMemcpyDeviceToDevice, c.stream));
-            u64 *prod = force_dense ? c.ws_alloc((size_t)m * ctw) : o->block(ch, r0);
-            op_multiply_plain_dense_bcast(c, ch, v->ptr(ch), plains, m, prod);
-            sum_slots_batched(c, ch, prod, m, CNHE_ALL_SLOTS);
-            if (force_dense) {
-                // one-hot masks for columns r0..r0+m (EncryptedSealBfvMatrix.cs:96, AtomicSealBfvVector.cs:936-945)
-                u64 *masks = c.ws_alloc((size_t)m * N);
-                op_encode_onehot(c, ch, m, first_row + r0, masks); // built on the device (was a 134 MB pageable upload per 1024-row wave)
-                op_multiply_plain_dense(c, ch, prod, m, masks, true, prod);
-                std::vector<const u64 *> terms;
-                if (!first) terms.push_back(o->ptr(ch));
-                for (int i = 0; i < m; i++) terms.push_back(prod + (size_t)i * ctw);
-                do_add_many(c, ch, terms, o->ptr(ch));
-                c.sync();
-            }
-            first = false;
-        }
-    }
-    *out = guard.release();
-    API_END
-}
-// The row-major product of one plain matrix with B encrypted vectors that may belong to different key slots (one inference per client):
-// out[b] is what cnhe_mat_mul_rowmajor(rows, n_rows, vs[b], force_dense) returns, bit for bit.  The B * n_rows products are flattened
-// (product p = b * n_rows + r) and go through each stage in waves of up to 1024: the broadcast plain products, one rotate-and-add
-// ladder for the whole wave (every key switch of a step in one wave, each ciphertext under its own slot's keys), then per input the
-// one-hot masks and the sum into its dense output, or its sparse elements.
-extern "C" int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, int force_dense,
-                                           cnhe_vec **out) {
-    API_BEGIN(h)
-    if (n_rows < 1 || B < 1 || !vs || !out) fail("bad arguments");
+// rows[i] is row first_row + i of a matrix with total_rows rows; vs are B encrypted vectors that may belong to different key slots (one
+// inference per client), out[b] the product with vs[b].  The B * n_rows products are flattened (product p = b * n_rows + r) and go through
+// each stage in waves: the broadcast plain products, one rotate-and-add ladder for the whole wave (every key switch of a step in one wave,
+// each ciphertext under its own slot's keys), then per input the one-hot masks at the global columns first_row + r and the sum into its
+// dense output of dimension total_rows, or its sparse elements.
+static void mat_mul_rowmajor(Context &c, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, bool force_dense, int first_row,
+                             int total_rows, cnhe_vec **out) {
+    if (!rows || n_rows < 1 || !vs || B < 1 || !out) fail("bad arguments");
     for (int b = 0; b < B; b++) {
         same_ctx(c, vs[b]);
         if (!vs[b]->enc) fail("at least one parameter has to be encrypted");
@@ -2192,24 +2078,26 @@ extern "C" int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *h, const cnhe_vec *const *r
         if (rows[r]->scale != rows[0]->scale) fail("row scales differ");
     }
     const size_t N = c.N, ctw = c.ct_words();
-    if (force_dense && (size_t)n_rows > N) fail("column out of range");
+    if (force_dense && (size_t)total_rows > N) fail("column out of range");
     const std::vector<int> vslot = vec_slots(c, vs, B);
     const double out_scale = vs[0]->scale * rows[0]->scale;
     std::vector<std::unique_ptr<cnhe_vec>> outs(B);
-    std::vector<BufRef> big(c.P); // sparse outputs: one [B][n_rows] block, product p lands in its place
     for (int b = 0; b < B; b++) {
-        outs[b].reset(new_vec(c, (uint64_t)n_rows, out_scale, force_dense ? CNHE_DENSE : CNHE_SPARSE, true, force_dense ? 1 : n_rows));
+        outs[b].reset(new_vec(c, (uint64_t)(force_dense ? total_rows : n_rows), out_scale, force_dense ? CNHE_DENSE : CNHE_SPARSE, true,
+                              force_dense ? 1 : n_rows));
         outs[b]->slot = vslot[b];
         if (force_dense) alloc_channels(outs[b].get());
     }
-    if (!force_dense)
+    std::vector<BufRef> big(c.P); // sparse outputs: one [B][n_rows] slab, product p lands in its place
+    if (!force_dense) {
         for (int ch = 0; ch < c.P; ch++) {
             c.set_channel(ch);
             big[ch] = c.alloc((size_t)B * n_rows * ctw);
-            for (int b = 0; b < B; b++) { outs[b]->buf[ch] = big[ch]; outs[b]->off[ch] = (size_t)b * n_rows * ctw; }
         }
-    // products per wave: 1024 as in cnhe_mat_mul_rowmajor, fewer when the wave's scratch (the products, the ladder's rotated copies and
-    // the masked products: three ciphertexts per product) would pass 8 GiB -- N = 16384 with nine primes takes 728
+        for (int b = 0; b < B; b++) slab_view(outs[b].get(), big, (size_t)b * n_rows);
+    }
+    // products per wave: 1024, fewer when the wave's scratch (the products, the ladder's rotated copies and the masked products: three
+    // ciphertexts per product) would pass 8 GiB -- the largest context, N = 16384 with nine primes, allows 1213
     const int total = B * n_rows, RC = (int)std::max<size_t>(16, std::min<size_t>(1024, ((size_t)1 << 30) / (3 * ctw)));
     std::vector<int> pslot(total);
     for (int p = 0; p < total; p++) pslot[p] = vslot[p / n_rows];
@@ -2236,8 +2124,9 @@ extern "C" int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *h, const cnhe_vec *const *r
             }
             sum_slots_batched(c, ch, prod, m, CNHE_ALL_SLOTS, pslot.data() + p0);
             if (force_dense) {
+                // one-hot masks (EncryptedSealBfvMatrix.cs:96, AtomicSealBfvVector.cs:936-945), built on the device
                 u64 *masks = c.ws_alloc((size_t)m * N);
-                for (const Seg &sg : segs) op_encode_onehot(c, ch, sg.len, sg.r0, masks + (size_t)sg.off * N);
+                for (const Seg &sg : segs) op_encode_onehot(c, ch, sg.len, first_row + sg.r0, masks + (size_t)sg.off * N);
                 op_multiply_plain_dense(c, ch, prod, m, masks, true, prod);
                 for (const Seg &sg : segs) {
                     std::vector<const u64 *> terms;
@@ -2251,6 +2140,29 @@ extern "C" int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *h, const cnhe_vec *const *r
         }
     }
     for (int b = 0; b < B; b++) out[b] = outs[b].release();
+}
+extern "C" int cnhe_mat_mul_rowmajor(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *v, int force_dense, cnhe_vec **out) {
+    API_BEGIN(h)
+    mat_mul_rowmajor(c, rows, n_rows, &v, 1, force_dense != 0, 0, n_rows, out);
+    API_END
+}
+// The same product for a contiguous SLICE of the matrix rows (rows[i] is global row first_row + i of a matrix with total_rows rows):
+// the unit of the intra-inference multi-GPU split (SURVEY.md 8e: CIFAR's 5488 dense rows over 4 GPUs).  ForceDense: the one-hot masks sit
+// at the global columns, so the partial results of the ranks add up to the full product (the reference sums the masked rows too,
+// EncryptedSealBfvMatrix.cs:92-116); otherwise the output holds this slice's sparse elements only.
+extern "C" int cnhe_mat_mul_rowmajor_shard(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *v, int force_dense, int first_row,
+                                           int total_rows, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (first_row < 0 || first_row + n_rows > total_rows) fail("row slice out of range");
+    mat_mul_rowmajor(c, rows, n_rows, &v, 1, force_dense != 0, first_row, total_rows, out);
+    API_END
+}
+// The row-major product of one plain matrix with B encrypted vectors (one inference per client): out[b] is what
+// cnhe_mat_mul_rowmajor(rows, n_rows, vs[b], force_dense) returns, bit for bit.
+extern "C" int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, int force_dense,
+                                           cnhe_vec **out) {
+    API_BEGIN(h)
+    mat_mul_rowmajor(c, rows, n_rows, vs, B, force_dense != 0, 0, n_rows, out);
     API_END
 }
 // SquareActivation over a whole matrix: every column PointwiseMultiply'd with itself in one wave per channel
@@ -2278,14 +2190,8 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
         op_multiply_relin(c, ch, ptrs, ptrs, big[ch]->p, ct_slot.data());
     }
     for (int i = 0; i < n; i++) {
-        cnhe_vec *o = new_vec(c, in[i]->dim, in[i]->scale * in[i]->scale, in[i]->format, true, in[i]->blocks);
-        o->slot = vslot[i];
-        for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-            o->buf[ch] = big[ch];
-            o->off[ch] = (size_t)first[i] * c.ct_words();
-        }
-        out[i] = o;
+        out[i] = slab_view(new_vec(c, in[i]->dim, in[i]->scale * in[i]->scale, in[i]->format, true, in[i]->blocks), big, first[i]);
+        out[i]->slot = vslot[i];
     }
     API_END
 }
@@ -2304,7 +2210,7 @@ struct cnhe_diag {
     std::vector<BufRef> plains; // per channel: [diags][N] plaintexts, coefficient form mod t
 };
 // key switches of rotate_rows(steps), 0 <= steps < N/2, on a context holding the Galois elements c.galois_elts: one with the step's own
-// key, else one per NAF term (rotate_internal's hops; a term of N/2 is skipped)
+// key, else one per hop
 static std::vector<int> rotation_hops(const Context &c) {
     const int half = (int)(c.N / 2);
     const u64 m = 2ULL * c.N;
@@ -2312,12 +2218,8 @@ static std::vector<int> rotation_hops(const Context &c) {
     u64 e = 1;
     for (int s = 1; s < half; s++) {
         e = (e * 3) & (m - 1);
-        if (std::find(c.galois_elts.begin(), c.galois_elts.end(), e) != c.galois_elts.end()) { hops[s] = 1; continue; }
-        for (int v = s, i = 0; v; i++) {
-            const int zi = (v & 1) ? 2 - (v & 3) : 0;
-            v = (v - zi) >> 1;
-            if (zi && (1 << i) != half) hops[s]++;
-        }
+        const bool own = std::find(c.galois_elts.begin(), c.galois_elts.end(), e) != c.galois_elts.end();
+        hops[s] = own ? 1 : (int)naf_hops(c.N, s).size();
     }
     return hops;
 }
