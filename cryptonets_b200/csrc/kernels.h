@@ -223,13 +223,15 @@ enum SampleKind { SAMPLE_TERNARY = 0, SAMPLE_NOISE = 1, SAMPLE_UNIFORM = 2 };
 // out[i][l][x] for i<n: stream ids stream0 + i*stream_step (+ l for UNIFORM); lifted into each residue
 // Dense layer (every output reads the same K inputs) on the integer tensor cores: wfrag = signed 8-bit weights packed as m16n8k32
 // A fragments [ceil(M/16)][ceil(K/32)][32 lanes][16 bytes]; weights in [-254, 254] are split W = W1 + W2 (wfrag2, may be null);
-// limbs = ceil(bits(q)/8); needs K*254*255 < 2^31
+// limbs = ceil(bits(q)/8); needs K*254*255 < 2^31 and every coefficient prime below 2^50 (the limb sums are joined modulo q_l in FP64:
+// (double)p must be exact and fcanon_u's input below 2^51; wider moduli belong to the 128-bit launch_mac_layer)
 cudaError_t launch_mac_dense_imma(const u64 *const *in_ptrs, const void *wfrag, const void *wfrag2, const u64 *bias, int K, int M, int limbs,
                                   u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
 // Scalar-MAC layers on wgmma (mac_umma.cu).  The layer's inputs are rows of one slab (input i at slab + i * slab_stride_words); a
 // BUNDLE is up to 128 outputs whose taps lie in a window of consecutive inputs: chunk j of the bundle multiplies the 32 inputs that start
 // at row chunk_rows[chunk0 + j] (bit 30 set: a row of the scratch slab that holds the W2 taps) with the 128 x 32 weight block at
-// wpack + a_off + j * 4096.  Outputs and constant biases are listed in bundle order (out0 = first entry of the bundle).
+// wpack + a_off + j * 4096.  Outputs and constant biases are listed in bundle order (out0 = first entry of the bundle).  The epilogue
+// joins the limb sums in FP64, exact only when every coefficient prime is below 2^50, as for launch_mac_dense_imma.
 struct UmBundle {
     int chunk0, n_chunks, a_off, n_out, out0;
 };

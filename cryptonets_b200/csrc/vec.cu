@@ -1857,19 +1857,21 @@ static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int
                 wmax = std::max(wmax, std::fabs(d));
             }
         const bool fp_mac = maxbits <= 50 && wmax < 131072.0 && (double)K * wmax * 67108864.0 < 4503599627370496.0 && !getenv("CNHE_MAC_INT");
-        // dense layer (one gather row shared by every output, 8-bit weights): exact integer GEMM on the tensor cores (mac_imma.cu)
+        // dense layer (one gather row shared by every output, 8-bit weights): exact integer GEMM on the tensor cores (mac_imma.cu).  Both
+        // tensor-core kernels join the limb sums in an FP64 epilogue that is exact only for moduli below 2^50 ((double)p, fcanon_u's
+        // |x| < 2^51); wider moduli (N = 2048's 54-bit default, custom ones) take the 128-bit k_mac_layer
         const int limbs = (maxbits + 7) / 8;
-        const bool imma = order_rows == 1 && wmax <= 254.0 && K >= 32 && M >= 8 && limbs >= 5 && limbs <= 7 && (double)K * 254.0 * 255.0 < 2147483648.0 &&
-                          !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
+        const bool imma = order_rows == 1 && wmax <= 254.0 && K >= 32 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 &&
+                          (double)K * 254.0 * 255.0 < 2147483648.0 && !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
         // ... or, for any layer whose inputs are evenly spaced rows of one slab (the previous layer's output, an imported batch) and whose
-        // weights stay within +-254: wgmma (mac_umma.cu), dense and convolution alike
+        // weights stay within +-254: wgmma (mac_umma.cu), dense and convolution alike, under the same modulus bound
         std::shared_ptr<UmmaPlan> plan;
         long long tap_stride = 0;
         {
             // (M >= 8: LoLa's per-map products come one output at a time -- a 128-row MMA per tile would be 99 % padding and the kernel's
             // per-tile latency more than the whole scalar-MAC launch)
-            bool slab = bl == 1 && n_in >= 2 && M >= 8 && limbs >= 5 && limbs <= 7 && wmax <= 254.0 && !getenv("CNHE_MAC_NO_UMMA") && !getenv("CNHE_MAC_NO_IMMA") &&
-                        !getenv("CNHE_MAC_INT");
+            bool slab = bl == 1 && n_in >= 2 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 && wmax <= 254.0 && !getenv("CNHE_MAC_NO_UMMA") &&
+                        !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
             if (slab) {
                 tap_stride = in[1]->block(ch, 0) - in[0]->block(ch, 0);
                 slab = tap_stride >= (long long)c.ct_words() && tap_stride % 2 == 0;

@@ -13,10 +13,14 @@ import pytest
 
 import worst_case_inputs as W
 
-RINGS = {  # name: (t, N, coefficient-modulus count, relinearisation dbc) -- the configurations the GPU tests run
+RINGS = {  # name: (t, N, coefficient-modulus count, relinearisation dbc[, custom q]) -- the configurations the GPU tests run
     "default4096": (40961, 4096, -1, 10),
     "cryptonets8192": (549764251649, 8192, -1, 10),
     "cifar16384": (957181001729, 16384, 8, 60),
+    # tests/test_gpu_ring_and_modulus_edges.py: the largest 36-, 40- and 44-bit primes = 1 mod 2048 (logN = 10), the two largest 49-bit
+    # primes = 1 mod 4096 (logN = 11, the widest modulus of the FP64 schedule)
+    "n1024-fp": (12289, 1024, -1, 10, [0xfffffd001, 0xffffff7801, 0xfffffffc001]),
+    "n2048-fp49": (40961, 2048, -1, 10, [0x1ffffffff9001, 0x1fffffffe7001]),
 }
 
 
@@ -61,8 +65,8 @@ def ring(name):
     """oracle, engine-side modulus list [(kind, p, oracle, table id)] of one ring"""
     if name not in _CACHE:
         from oracle.oracle_py import Oracle
-        t, N, count, dbc = RINGS[name]
-        orc = Oracle(t, N, count, dbc, dbc)
+        t, N, count, dbc, *custom = RINGS[name]
+        orc = Oracle(t, N, count, dbc, dbc, custom_q=custom[0] if custom else None)
         bo = Oracle(t, N, custom_q=fast_bsk(orc.q, t, N))
         mods = [("q", orc.q[i], orc, i) for i in range(orc.k)] + [("bsk", p, bo, j) for j, p in enumerate(bo.q)]
         _CACHE[name] = (orc, mods)
@@ -93,6 +97,14 @@ def _over(peak):
 
 def _bits(mask):
     return [b for b in range(32) if (mask >> b) & 1]
+
+
+def _segment_sum(p, rad, mask, i):
+    """largest magnitude any input can reach in the segment of forward passes holding pass i under re-centre mask `mask`: the segment
+    starts at the input (p - 1) or at a re-centre (p / 2) and adds at most p / 2 per stage"""
+    first = max([j for j in range(i + 1) if (mask >> j) & 1], default=0)
+    end = min([j for j in range(i + 1, len(rad)) if (mask >> j) & 1], default=len(rad))
+    return ((p // 2) if (mask >> first) & 1 else p - 1) + sum(rad[first:end]) * (p // 2)
 
 
 @pytest.mark.parametrize("name", list(RINGS))
@@ -133,13 +145,18 @@ def test_forward_worst_case_reaches_its_bound(name):
                 assert peak < W.TWO52, (kind, label, out_index)
                 for b in _bits(mask):
                     _, peak_wo = W.lazy_forward(a, p, wd, rad, mask & ~(1 << b))
-                    assert peak_wo > LIMIT, (kind, label, b, out_index, peak_wo / p)
+                    if peak_wo > LIMIT:
+                        note = _over(peak_wo)
+                    else:  # then no input reaches the limit without this bit: even the segment's analytic sum stays below 2^52
+                        bound = _segment_sum(p, rad, mask & ~(1 << b), b)
+                        assert bound < W.TWO52 and peak_wo >= 0.9 * bound, (kind, label, b, out_index, peak_wo / p)
+                        note = " (margin: the analytic sum 2^%.2f is below 2^52; the schedule's bound adds the products' rounding)" % np.log2(bound)
                     if out_index == 0:
                         lines.append("N=%d %s %d-bit %s pass %d: peak %.2f p (2^%.2f) with, %.2f p (2^%.2f) without%s" % (
-                            N, kind, p.bit_length(), label, b, peak / p, np.log2(peak), peak_wo / p, np.log2(peak_wo), _over(peak_wo)))
-        # digit planes (the fused key switch's forward): inputs below 2^dbc
+                            N, kind, p.bit_length(), label, b, peak / p, np.log2(peak), peak_wo / p, np.log2(peak_wo), note))
+        # digit planes (the fused key switch's forward, built at N = 4096 / 8192): inputs below 2^dbc
         dbc = RINGS[name][3]
-        if kind == "q" and dbc < p.bit_length():
+        if kind == "q" and dbc < p.bit_length() and logN in (12, 13):
             a = W.forward_worst_case(p, wd, N - 1, dbc)
             assert int(a.max()) < 1 << dbc
             x, _ = W.lazy_forward(a, p, wd, W.split_radices(logN), 0)
@@ -209,7 +226,7 @@ def test_mont_rq_words():
 def test_auxiliary_base_bound_at_the_all_max_ciphertext():
     """B * m_sk > 2^8 N t q: the all-(q_i - 1) ciphertext's negacyclic square has coefficients near N Q^2, and the fast base covers
     them with the 2^8 margin the BEHZ floor needs"""
-    for name, (t, N, count, dbc) in RINGS.items():
+    for name, (t, N, *_) in RINGS.items():
         orc, mods = ring(name)
         Q = 1
         for p in orc.q:
