@@ -39,6 +39,11 @@ _SIGS = {
     "cnhe_vecs_rotate": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_vecs_stack_batch": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_mat_mul_rowmajor_batch": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
+    "cnhe_mat_dot_rows_batch": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP), i32, u64, C.POINTER(VECP)],
+    "cnhe_vecs_duplicate_batch": [C.c_void_p, C.POINTER(VECP), i32, u64, C.POINTER(VECP)],
+    "cnhe_vecs_permute_batch": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP), C.POINTER(i32), i32, i32, u64, C.POINTER(VECP)],
+    "cnhe_vecs_interleave_batch": [C.c_void_p, C.POINTER(VECP), i32, i32, i32, C.POINTER(VECP)],
+    "cnhe_vecs_multiply_plain": [C.c_void_p, C.POINTER(VECP), i32, VECP, C.POINTER(VECP)],
     "cnhe_diag_prepare": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(C.c_void_p)],
     "cnhe_diag_info": [C.c_void_p, C.POINTER(i32), U64P, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), U64P],
     "cnhe_diag_export": [C.c_void_p, C.c_void_p, i32, i32, U64P, sz, C.POINTER(i32)],

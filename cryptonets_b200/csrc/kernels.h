@@ -157,6 +157,10 @@ cudaError_t launch_plain_lift(const u64 *plain, u64 *lifted, int n, int coeffs, 
 // out[c][part][l][x] = a[c or 0][part][l][x] * b[c or 0][l][x]
 cudaError_t launch_dyadic_bcast(const u64 *a, const u64 *b, u64 *out, int n, int size, int a_per_ct, int b_per_ct, int k, int logn,
                                 const BehzConst *bc, cudaStream_t s);
+// out[b * out_rows + r][p][l][x] = ct[b][p][l][x] * pl[r][l][x]: B ciphertexts [B][2][k][N] times R lifted plaintexts [R][k][N], NTT form,
+// canonical in and out (FP64 path: every q_l < 2^50; the same words as launch_dyadic_bcast)
+cudaError_t launch_dyadic_outer(const u64 *ct, const u64 *pl, u64 *out, int B, int R, int out_rows, int k, int logn, const BehzConstF *f,
+                                cudaStream_t s);
 // Galois: out[c] = (perm(c0), 0), perm1[c] = perm(c1)   (util::apply_galois)
 cudaError_t launch_galois(const u64 *in, u64 *out_base, u64 *perm_c1, int n, u64 elt_inv, int k, int logn, const BehzConst *bc, cudaStream_t s,
                           int add_back = 0); // add_back: base = (c0 + perm(c0), c1) -> key switch + base = x + rotate(x)

@@ -8,6 +8,7 @@
 // Encryptor::preencrypt, negacyclic_multiply_poly_mono_coeffmod (exponent 0), dyadic_product_coeffmod,
 // util::apply_galois, BatchEncoder::encode/decode index map.
 // All are HBM-bound streaming kernels except the MAC layer, which is integer-ALU bound (DESIGN.md section 5).
+#include "fparith.cuh"
 #include "kernels.h"
 #include "plainops.cuh"
 
@@ -95,6 +96,36 @@ __global__ void __launch_bounds__(256) k_dyadic_bcast(const u64 *a, const u64 *b
     const size_t c = i / (size * kN), r = i % kN;
     const int l = (int)(r >> logn);
     out[i] = mulmod(a[a_per_ct ? i : i % (size * kN)], b[(b_per_ct ? c : 0) * kN + r], bc->q[l]);
+}
+// out[b * out_rows + r][p][l][i] = ct[b][p][l][i] * pl[r][l][i]  (NTT form, canonical in and out; every q_l < 2^50).  One thread per
+// (r, l, i) loads the plaintext word once and multiplies it into CB clients' two polynomials (B > CB: once per CB clients).  The CTAs of one (l, coefficient
+// tile) are consecutive over r, so the R rows read the same ciphertext words at about the same time, from L2.  fmodmul of canonical
+// operands is congruent to the product and within (-q, q); re-centred and made canonical it is the unique residue mulmod gives.
+template <int CB>
+__global__ void __launch_bounds__(256) k_dyadic_outer(const u64 *__restrict__ ct, const u64 *__restrict__ pl, u64 *__restrict__ out, int B, int R,
+                                                     int out_rows, int logn, const __grid_constant__ BehzConstF F) {
+    const int N = 1 << logn, k = F.k, tiles = N >> 8;
+    const int r = blockIdx.x % R, tile = (blockIdx.x / R) % tiles, l = blockIdx.x / (R * tiles);
+    const int i = (tile << 8) + threadIdx.x;
+    const double p = F.qd[l], pinv = F.qinv[l];
+    const size_t kN = (size_t)k * N, ctw = 2 * kN, at = (size_t)l * N + i;
+    const double d = u2d(pl[(size_t)r * kN + at]);
+    for (int b0 = 0; b0 < B; b0 += CB) {
+        double x[CB][2];
+#pragma unroll
+        for (int cb = 0; cb < CB; cb++)
+            if (b0 + cb < B) {
+                x[cb][0] = u2d(ct[(size_t)(b0 + cb) * ctw + at]);
+                x[cb][1] = u2d(ct[(size_t)(b0 + cb) * ctw + kN + at]);
+            }
+#pragma unroll
+        for (int cb = 0; cb < CB; cb++) {
+            if (b0 + cb >= B) break;
+            u64 *o = out + ((size_t)(b0 + cb) * out_rows + r) * ctw + at;
+            o[0] = fsmall_u(frecenter(fmodmul(x[cb][0], d, p, pinv), p, pinv), F.q_u[l]);
+            o[kN] = fsmall_u(frecenter(fmodmul(x[cb][1], d, p, pinv), p, pinv), F.q_u[l]);
+        }
+    }
 }
 
 // ---------------------------------------------------------------- Galois permutation (gather form)
@@ -421,6 +452,16 @@ cudaError_t launch_dyadic_bcast(const u64 *a, const u64 *b, u64 *out, int n, int
                                 const BehzConst *bc, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     k_dyadic_bcast<<<blocks_for(((size_t)n * size * k) << logn), 256, 0, s>>>(a, b, out, n, size, a_per_ct, b_per_ct, k, logn, bc);
+    return cudaGetLastError();
+}
+cudaError_t launch_dyadic_outer(const u64 *ct, const u64 *pl, u64 *out, int B, int R, int out_rows, int k, int logn, const BehzConstF *f,
+                                cudaStream_t s) {
+    if (B <= 0 || R <= 0) return cudaSuccess;
+    const unsigned grid = (unsigned)R * (unsigned)((1 << logn) >> 8) * (unsigned)k;
+    if (B == 1) k_dyadic_outer<1><<<grid, 256, 0, s>>>(ct, pl, out, B, R, out_rows, logn, *f);
+    else if (B == 2) k_dyadic_outer<2><<<grid, 256, 0, s>>>(ct, pl, out, B, R, out_rows, logn, *f);
+    else if (B <= 4) k_dyadic_outer<4><<<grid, 256, 0, s>>>(ct, pl, out, B, R, out_rows, logn, *f);
+    else k_dyadic_outer<8><<<grid, 256, 0, s>>>(ct, pl, out, B, R, out_rows, logn, *f);
     return cudaGetLastError();
 }
 cudaError_t launch_galois(const u64 *in, u64 *out_base, u64 *perm_c1, int n, u64 elt_inv, int k, int logn, const BehzConst *bc, cudaStream_t s,

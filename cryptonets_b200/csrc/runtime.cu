@@ -1189,6 +1189,41 @@ void op_multiply_plain_dense_bcast(Context &c, int ch, const u64 *ct, const u64 
     }
     c.note(Context::OP_MULTIPLY_PLAIN, ch, n, out, ct);
 }
+// B ciphertexts times the same R dense plaintexts: out[b * R + r] = cts[b] * plains[r], each product the words
+// op_multiply_plain_dense_bcast(cts[b], plains) gives.  Every ciphertext is transformed once and every plaintext once per wave of rows
+// (R k (B - 1) forward transforms fewer than B broadcast calls); the FP64 path multiplies them in k_dyadic_outer, the integer path
+// (CNHE_NTT_INT, a q_l >= 2^50) runs the broadcast kernel per ciphertext on the shared transforms.  One ciphertext is the broadcast call.
+void op_multiply_plain_dense_outer(Context &c, int ch, const std::vector<const u64 *> &cts, const u64 *plains, int R, u64 *out) {
+    const int k = c.k, B = (int)cts.size(), fpq = fp_range(c, 0, k);
+    const size_t N = c.N, kN = (size_t)k * N, ctw = 2 * kN;
+    if (B < 1 || R < 1) return;
+    if (B == 1) return op_multiply_plain_dense_bcast(c, ch, cts[0], plains, R, out);
+    const bool fp = c.fp_elementwise && fpq;
+    WsScope scope(c);
+    u64 *ctn = c.ws_alloc((size_t)B * ctw);
+    bool packed = true;
+    for (int b = 1; b < B && packed; b++) packed = cts[b] == cts[0] + (size_t)b * ctw;
+    if (packed) c.check(launch_ntt_forward(cts[0], ctn, B * 2 * k, c.logN, c.d_tabs, 0, k, fpq, c.stream), "ntt_forward");
+    else
+        for (int b = 0; b < B; b++)
+            c.check(launch_ntt_forward(cts[b], ctn + (size_t)b * ctw, 2 * k, c.logN, c.d_tabs, 0, k, fpq, c.stream), "ntt_forward");
+    // rows per wave: their lifted transforms stay under 8 GiB
+    const int RW = (int)std::max<size_t>(1, std::min<size_t>((size_t)R, ((size_t)1 << 30) / kN));
+    for (int r0 = 0; r0 < R; r0 += RW) {
+        WsScope wave(c);
+        const int m = std::min(RW, R - r0);
+        u64 *lifted = c.ws_alloc((size_t)m * kN);
+        c.check(launch_plain_lift(plains + (size_t)r0 * N, lifted, m, (int)N, k, c.logN, c.d_bc, c.ch[ch].pc, c.stream), "plain_lift");
+        c.check(launch_ntt_forward(lifted, lifted, m * k, c.logN, c.d_tabs, 0, k, fpq, c.stream), "ntt_forward");
+        if (fp) c.check(launch_dyadic_outer(ctn, lifted, out + (size_t)r0 * ctw, B, m, R, k, c.logN, &c.h_bf, c.stream), "dyadic_outer");
+        else
+            for (int b = 0; b < B; b++)
+                c.check(launch_dyadic_bcast(ctn + (size_t)b * ctw, lifted, out + ((size_t)b * R + r0) * ctw, m, 2, 0, 1, k, c.logN, c.d_bc, c.stream),
+                        "dyadic");
+    }
+    c.check(launch_ntt_inverse(out, out, B * R * 2 * k, c.logN, c.d_tabs, 0, k, fpq, c.stream), "ntt_inverse");
+    for (int b = 0; b < B; b++) c.note(Context::OP_MULTIPLY_PLAIN, ch, R, out + (size_t)b * R * ctw, cts[b]);
+}
 void op_encode(Context &c, int ch, const u64 *values, int n, int count, u64 *plain) {
     c.check(launch_encode_scatter(values, plain, n, count, c.d_index_map, c.logN, c.stream), "encode_scatter");
     c.check(launch_ntt_inverse(plain, plain, n, c.logN, c.d_tabs, c.ch[ch].mod_id, 1, fp_range(c, c.ch[ch].mod_id, 1), c.stream), "ntt_inverse(t)");

@@ -247,6 +247,9 @@ std::vector<int> naf_hops(uint32_t N, int steps);
 // dense plaintext (coefficient form mod t, [n or 1][N]) times ciphertexts [n][2kN]
 void op_multiply_plain_dense(Context &c, int ch, const u64 *ct, int n, const u64 *plain, bool plain_per_ct, u64 *out);
 void op_multiply_plain_dense_bcast(Context &c, int ch, const u64 *ct, const u64 *plains, int n, u64 *out);
+// B ciphertexts times R dense plaintexts (contiguous [R][N]): out [B][R][2kN], out[b * R + r] = cts[b] * plains[r], word for word what
+// op_multiply_plain_dense_bcast(cts[b], plains, R) writes; counted as B * R plain multiplications
+void op_multiply_plain_dense_outer(Context &c, int ch, const std::vector<const u64 *> &cts, const u64 *plains, int R, u64 *out);
 // values [n][count] (mod t, device) -> plain [n][N] coefficient form
 void op_encode(Context &c, int ch, const u64 *values, int n, int count, u64 *plain);
 void op_decode(Context &c, int ch, const u64 *plain, int n, u64 *values);

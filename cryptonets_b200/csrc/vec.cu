@@ -1577,6 +1577,206 @@ extern "C" int cnhe_vecs_stack_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, i
     interleave_groups(c, vecs, n, B, 0, true, out);
     API_END
 }
+// cnhe_vecs_interleave of B groups of n vectors each: out[b] is bit-identical to cnhe_vecs_interleave(vecs + b * n, n, shift)
+extern "C" int cnhe_vecs_interleave_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int B, int shift, cnhe_vec **out) {
+    API_BEGIN(h)
+    interleave_groups(c, vecs, n, B, shift, false, out);
+    API_END
+}
+
+// ---------------------------------------------------------------------------------------------------- one operation, B clients
+// The B inputs of a batched vector operation: the same context, live key slots, and one dim, scale, format and block count
+static std::vector<int> batch_inputs(Context &c, const cnhe_vec *const *vecs, int B, cnhe_vec **out) {
+    if (!vecs || B < 1 || !out) fail("bad arguments");
+    for (int b = 0; b < B; b++) {
+        same_ctx(c, vecs[b]);
+        if (vecs[b]->dim != vecs[0]->dim || vecs[b]->scale != vecs[0]->scale || vecs[b]->format != vecs[0]->format ||
+            vecs[b]->blocks != vecs[0]->blocks || vecs[b]->enc != vecs[0]->enc)
+            fail("the input vectors must share dimension, scale, format and block count");
+    }
+    return vec_slots(c, vecs, B);
+}
+// B single-ciphertext outputs in one slab per channel, bound to their inputs' slots
+static std::vector<std::unique_ptr<cnhe_vec>> batch_outputs(Context &c, int n, const std::vector<int> &slot_of, uint64_t dim, double scale) {
+    std::vector<BufRef> big(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        big[ch] = c.alloc((size_t)n * c.ct_words());
+    }
+    std::vector<std::unique_ptr<cnhe_vec>> outs(n);
+    for (int i = 0; i < n; i++) {
+        outs[i].reset(slab_view(new_vec(c, dim, scale, CNHE_DENSE, true, 1), big, (size_t)i));
+        outs[i]->slot = slot_of[i];
+    }
+    return outs;
+}
+// cnhe_vec_duplicate of B vectors (one per client; key slots may differ): the column rotations in one call, every client's count - 1 row
+// rotations in one op_rotate_rows_multi, then each client's additions in the reference's order.  out[b] is bit-identical to the single call.
+extern "C" int cnhe_vecs_duplicate_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int B, uint64_t count, cnhe_vec **out) {
+    API_BEGIN(h)
+    const std::vector<int> slots = batch_inputs(c, vecs, B, out);
+    const cnhe_vec *a = vecs[0];
+    uint64_t shift = 1;
+    while (shift < a->dim) shift *= 2;
+    if (!a->enc) fail("Duplicate operates only on encrypted data");
+    if (a->format == CNHE_SPARSE) fail("Duplicate operates only on dense vectors");
+    const size_t N = c.N, ctw = c.ct_words();
+    if (shift * count > N) fail("Packed vector must fit in a single ciphertext");
+    auto outs = batch_outputs(c, B, slots, count * shift, a->scale);
+    bool column = false;
+    for (uint64_t i = 1; i < count; i++) column = column || (long long)(i * shift) * 2 >= (long long)N;
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        u64 *rotator = nullptr;
+        if (column) { // rotate_columns of every input (":1387-1394"), gathered so that one call serves all
+            u64 *in = c.ws_alloc((size_t)B * ctw);
+            rotator = c.ws_alloc((size_t)B * ctw);
+            for (int b = 0; b < B; b++)
+                { CNHE_CUDA(cudaMemcpyAsync(in + (size_t)b * ctw, vecs[b]->ptr(ch), ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(in + (size_t)b * ctw, vecs[b]->ptr(ch)); }
+            op_rotate_columns(c, ch, in, B, rotator, slots.data());
+        }
+        std::vector<RotateJob> jobs;
+        std::vector<u64 *> pieces;
+        for (int b = 0; b < B; b++) {
+            u64 *res = outs[b]->ptr(ch);
+            CNHE_CUDA(cudaMemcpyAsync(res, vecs[b]->ptr(ch), ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(res, vecs[b]->ptr(ch));
+            for (uint64_t i = 1; i < count; i++) {
+                long long target = (long long)(i * shift);
+                const u64 *src = vecs[b]->ptr(ch);
+                if (target * 2 >= (long long)N) {
+                    src = rotator + (size_t)b * ctw;
+                    target -= (long long)N / 2;
+                }
+                u64 *tmp = c.ws_alloc(ctw);
+                jobs.push_back({src, -(int)target, tmp, slots[b]});
+                pieces.push_back(tmp);
+            }
+        }
+        op_rotate_rows_multi(c, ch, jobs);
+        const size_t per = count > 0 ? count - 1 : 0;
+        for (int b = 0; b < B; b++)
+            for (size_t i = 0; i < per; i++) do_add(c, ch, outs[b]->ptr(ch), pieces[b * per + i], outs[b]->ptr(ch), ctw, 0);
+    }
+    for (int b = 0; b < B; b++) out[b] = outs[b].release();
+    API_END
+}
+// cnhe_vec_permute of B vectors (one per client) with the same n_perm permutations of n_sel selections each: out[b * n_perm + j] is
+// bit-identical to cnhe_vec_permute(vecs[b], selections + j * n_sel, shifts + j * n_sel, n_sel, output_dim).  Per wave of clients the
+// mask products are one outer product of the clients and the distinct selections, and every (client, permutation, selection) rotation
+// goes into one op_rotate_rows_multi; then each output's sum in the reference's order (":1446-1461").
+extern "C" int cnhe_vecs_permute_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int B, const cnhe_vec *const *selections, const int *shifts,
+                                       int n_perm, int n_sel, uint64_t output_dim, cnhe_vec **out) {
+    API_BEGIN(h)
+    const std::vector<int> slots = batch_inputs(c, vecs, B, out);
+    if (!selections || !shifts || n_perm < 1 || n_sel < 1) fail("bad arguments");
+    const cnhe_vec *a = vecs[0];
+    if (a->format != CNHE_DENSE) fail("Permute works only on dense vectors");
+    if (!a->enc) fail("can permute only encrypted vectors");
+    if (a->blocks > 1) fail("can permute only a single block");
+    std::vector<int> sel_index((size_t)n_perm * n_sel, -1); // each non-null selection's place among the distinct ones
+    std::vector<const cnhe_vec *> distinct;
+    std::vector<double> out_scale(n_perm);
+    for (int j = 0; j < n_perm; j++) {
+        const cnhe_vec *const *sel = selections + (size_t)j * n_sel;
+        int first = -1;
+        for (int i = 0; i < n_sel; i++) {
+            if (!sel[i]) continue;
+            same_ctx(c, sel[i]);
+            if (first < 0) first = i;
+            if (sel[i]->dim != a->dim) fail("dimension of selection vector does not match dimension of data vector");
+            if (sel[i]->scale != sel[first]->scale) fail("scales of all selection vectors should be the same");
+            if (sel[i]->enc) fail("encrypted size must be 2 (rotating the size-3 product of an encrypted selection is rejected by SEAL)");
+            if (sel[i]->format != CNHE_DENSE) fail("selection vectors must be dense");
+            const size_t d = std::find(distinct.begin(), distinct.end(), sel[i]) - distinct.begin();
+            if (d == distinct.size()) distinct.push_back(sel[i]);
+            sel_index[(size_t)j * n_sel + i] = (int)d;
+        }
+        if (first < 0) fail("permuting with no selected values is illigal");
+        out_scale[j] = a->scale * sel[first]->scale;
+    }
+    const int S = (int)distinct.size(), terms = (int)std::count_if(sel_index.begin(), sel_index.end(), [](int s) { return s >= 0; });
+    const size_t N = c.N, ctw = c.ct_words();
+    std::vector<int> out_slot((size_t)B * n_perm);
+    for (size_t o = 0; o < out_slot.size(); o++) out_slot[o] = slots[o / n_perm];
+    auto outs = batch_outputs(c, B * n_perm, out_slot, output_dim, 0);
+    for (int b = 0; b < B; b++)
+        for (int j = 0; j < n_perm; j++) outs[(size_t)b * n_perm + j]->scale = out_scale[j];
+    // clients per wave: their products and rotated terms stay under 8 GiB
+    const int BW = (int)std::max<size_t>(1, ((size_t)1 << 30) / ((size_t)(S + terms) * ctw));
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        WsScope scope(c);
+        u64 *plains = c.ws_alloc((size_t)S * N);
+        for (int s = 0; s < S; s++) CNHE_CUDA(cudaMemcpyAsync(plains + (size_t)s * N, distinct[s]->ptr(ch), N * 8, cudaMemcpyDeviceToDevice, c.stream));
+        for (int b0 = 0; b0 < B; b0 += BW) {
+            WsScope wave(c);
+            const int nb = std::min(BW, B - b0);
+            u64 *prod = c.ws_alloc((size_t)nb * S * ctw), *rot = c.ws_alloc((size_t)nb * terms * ctw);
+            std::vector<const u64 *> cts(nb);
+            for (int j = 0; j < nb; j++) cts[j] = vecs[b0 + j]->ptr(ch);
+            op_multiply_plain_dense_outer(c, ch, cts, plains, S, prod);
+            std::vector<RotateJob> jobs; // (client, permutation, selection) in that order: the terms of an output are consecutive
+            for (int bb = 0; bb < nb; bb++)
+                for (size_t q = 0; q < sel_index.size(); q++)
+                    if (sel_index[q] >= 0)
+                        jobs.push_back({prod + ((size_t)bb * S + sel_index[q]) * ctw, shifts[q], rot + jobs.size() * ctw, slots[b0 + bb]});
+            op_rotate_rows_multi(c, ch, jobs);
+            const u64 *r = rot;
+            for (int bb = 0; bb < nb; bb++)
+                for (int j = 0; j < n_perm; j++) {
+                    u64 *o = outs[(size_t)(b0 + bb) * n_perm + j]->ptr(ch);
+                    for (int i = 0, have = 0; i < n_sel; i++) {
+                        if (sel_index[(size_t)j * n_sel + i] < 0) continue;
+                        if (!have) { CNHE_CUDA(cudaMemcpyAsync(o, r, ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(o, r); }
+                        else do_add(c, ch, o, r, o, ctw, 0);
+                        have = 1;
+                        r += ctw;
+                    }
+                }
+        }
+    }
+    for (size_t o = 0; o < outs.size(); o++) out[o] = outs[o].release();
+    API_END
+}
+// cnhe_vec_pointwise_multiply(vecs[i], plain) of n encrypted vectors and one plain dense vector, one outer product per channel and block:
+// out[i] is bit-identical to the single call
+extern "C" int cnhe_vecs_multiply_plain(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, const cnhe_vec *plain, cnhe_vec **out) {
+    API_BEGIN(h)
+    const std::vector<int> slots = batch_inputs(c, vecs, n, out);
+    same_ctx(c, plain);
+    const cnhe_vec *a = vecs[0];
+    if (!a->enc) fail("multiplying two plaintexts is not implemented");
+    if (plain->enc || plain->format != CNHE_DENSE) fail("expecting a plain dense vector");
+    check_pair(a, plain);
+    if (a->blocks != plain->blocks) fail("Dimensions do not match");
+    const int bl = a->blocks;
+    const size_t ctw = c.ct_words();
+    std::vector<BufRef> big(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        big[ch] = c.alloc((size_t)n * bl * ctw);
+    }
+    std::vector<std::unique_ptr<cnhe_vec>> outs(n);
+    for (int i = 0; i < n; i++) {
+        outs[i].reset(slab_view(new_vec(c, a->dim, a->scale * plain->scale, a->format, true, bl), big, (size_t)i * bl));
+        outs[i]->slot = slots[i];
+    }
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        WsScope scope(c);
+        for (int j = 0; j < bl; j++) {
+            std::vector<const u64 *> cts(n);
+            for (int i = 0; i < n; i++) cts[i] = vecs[i]->block(ch, j);
+            u64 *dst = bl == 1 ? big[ch]->p : c.ws_alloc((size_t)n * ctw);
+            op_multiply_plain_dense_outer(c, ch, cts, plain->block(ch, j), 1, dst);
+            if (bl > 1)
+                for (int i = 0; i < n; i++)
+                    CNHE_CUDA(cudaMemcpyAsync(outs[i]->block(ch, j), dst + (size_t)i * ctw, ctw * 8, cudaMemcpyDeviceToDevice, c.stream));
+        }
+    }
+    for (int i = 0; i < n; i++) out[i] = outs[i].release();
+    API_END
+}
 
 // ---------------------------------------------------------------------------------------------------- matrix x vector, layers
 struct RowHash {
@@ -2059,11 +2259,13 @@ extern "C" int cnhe_mat_mul_colmajor_sparse(cnhe_ctx *h, const cnhe_vec *const *
 // together instead of one DotProduct per row.
 // rows[i] is row first_row + i of a matrix with total_rows rows; vs are B encrypted vectors that may belong to different key slots (one
 // inference per client), out[b] the product with vs[b].  The B * n_rows products are flattened (product p = b * n_rows + r) and go through
-// each stage in waves: the broadcast plain products, one rotate-and-add ladder for the whole wave (every key switch of a step in one wave,
-// each ciphertext under its own slot's keys), then per input the one-hot masks at the global columns first_row + r and the sum into its
-// dense output of dimension total_rows, or its sparse elements.
+// each stage in waves -- whole clients when the rows fit in one wave, else slices of one client's rows: the plain products (one outer
+// product of the wave's clients and rows when it holds several clients, else the broadcast product), one rotate-and-add ladder over
+// `length` slots for the whole wave (every key switch of a step in one wave, each ciphertext under its own slot's keys), then per input the
+// one-hot masks at the global columns first_row + r and the sum into its dense output of dimension total_rows, or its sparse elements.
+// dot: no matrix output -- out[b * n_rows + r] is DotProduct(rows[r], vs[b], length) as cnhe_vec_dot_product returns it.
 static void mat_mul_rowmajor(Context &c, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, bool force_dense, int first_row,
-                             int total_rows, cnhe_vec **out) {
+                             int total_rows, cnhe_vec **out, uint64_t length = CNHE_ALL_SLOTS, bool dot = false) {
     if (!rows || n_rows < 1 || !vs || B < 1 || !out) fail("bad arguments");
     for (int b = 0; b < B; b++) {
         same_ctx(c, vs[b]);
@@ -2079,69 +2281,78 @@ static void mat_mul_rowmajor(Context &c, const cnhe_vec *const *rows, int n_rows
         if (rows[r]->format != CNHE_DENSE) fail("Format mismatch");
         if (rows[r]->scale != rows[0]->scale) fail("row scales differ");
     }
+    if (length == 0) fail("Can't sum over less then one element");
     const size_t N = c.N, ctw = c.ct_words();
     if (force_dense && (size_t)total_rows > N) fail("column out of range");
     const std::vector<int> vslot = vec_slots(c, vs, B);
     const double out_scale = vs[0]->scale * rows[0]->scale;
-    std::vector<std::unique_ptr<cnhe_vec>> outs(B);
-    for (int b = 0; b < B; b++) {
-        outs[b].reset(new_vec(c, (uint64_t)(force_dense ? total_rows : n_rows), out_scale, force_dense ? CNHE_DENSE : CNHE_SPARSE, true,
-                              force_dense ? 1 : n_rows));
-        outs[b]->slot = vslot[b];
-        if (force_dense) alloc_channels(outs[b].get());
+    const int n_out = dot ? B * n_rows : B;
+    std::vector<std::unique_ptr<cnhe_vec>> outs(n_out);
+    for (int o = 0; o < n_out; o++) {
+        if (dot) outs[o].reset(new_vec(c, vs[0]->dim, out_scale, CNHE_DENSE, true, 1));
+        else outs[o].reset(new_vec(c, (uint64_t)(force_dense ? total_rows : n_rows), out_scale, force_dense ? CNHE_DENSE : CNHE_SPARSE, true,
+                                   force_dense ? 1 : n_rows));
+        outs[o]->slot = vslot[dot ? o / n_rows : o];
+        if (force_dense) alloc_channels(outs[o].get());
     }
-    std::vector<BufRef> big(c.P); // sparse outputs: one [B][n_rows] slab, product p lands in its place
+    std::vector<BufRef> big(c.P); // sparse outputs and dot products: one [B][n_rows] slab, product p lands in its place
     if (!force_dense) {
         for (int ch = 0; ch < c.P; ch++) {
             c.set_channel(ch);
             big[ch] = c.alloc((size_t)B * n_rows * ctw);
         }
-        for (int b = 0; b < B; b++) slab_view(outs[b].get(), big, (size_t)b * n_rows);
+        for (int o = 0; o < n_out; o++) slab_view(outs[o].get(), big, dot ? (size_t)o : (size_t)o * n_rows);
     }
     // products per wave: 1024, fewer when the wave's scratch (the products, the ladder's rotated copies and the masked products: three
     // ciphertexts per product) would pass 8 GiB -- the largest context, N = 16384 with nine primes, allows 1213
     const int total = B * n_rows, RC = (int)std::max<size_t>(16, std::min<size_t>(1024, ((size_t)1 << 30) / (3 * ctw)));
+    struct Wave { int b0, nb, r0, nr; };
+    std::vector<Wave> waves;
+    if (n_rows <= RC)
+        for (int b0 = 0; b0 < B; b0 += RC / n_rows) waves.push_back({b0, std::min(RC / n_rows, B - b0), 0, n_rows});
+    else
+        for (int b = 0; b < B; b++)
+            for (int r0 = 0; r0 < n_rows; r0 += RC) waves.push_back({b, 1, r0, std::min(RC, n_rows - r0)});
     std::vector<int> pslot(total);
     for (int p = 0; p < total; p++) pslot[p] = vslot[p / n_rows];
+    uint64_t len = length;
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
         std::vector<char> first(B, 1);
-        for (int p0 = 0; p0 < total; p0 += RC) {
+        for (const Wave &w : waves) {
             WsScope scope(c);
-            const int m = std::min(RC, total - p0);
+            const int p0 = w.b0 * n_rows + w.r0, m = w.nb * w.nr;
             u64 *prod = force_dense ? c.ws_alloc((size_t)m * ctw) : big[ch]->p + (size_t)p0 * ctw;
-            // segments of the wave: the rows r0..r0+len of input b
-            struct Seg { int b, r0, len, off; };
-            std::vector<Seg> segs;
-            for (int p = p0; p < p0 + m;) {
-                const int b = p / n_rows, r0 = p % n_rows, len = std::min(n_rows - r0, p0 + m - p);
-                segs.push_back({b, r0, len, p - p0});
-                p += len;
-            }
-            u64 *plains = c.ws_alloc((size_t)m * N);
-            for (const Seg &sg : segs) {
-                for (int i = 0; i < sg.len; i++)
-                    CNHE_CUDA(cudaMemcpyAsync(plains + (size_t)(sg.off + i) * N, rows[sg.r0 + i]->ptr(ch), N * 8, cudaMemcpyDeviceToDevice, c.stream));
-                op_multiply_plain_dense_bcast(c, ch, vs[sg.b]->ptr(ch), plains + (size_t)sg.off * N, sg.len, prod + (size_t)sg.off * ctw);
-            }
-            sum_slots_batched(c, ch, prod, m, CNHE_ALL_SLOTS, pslot.data() + p0);
+            u64 *plains = c.ws_alloc((size_t)w.nr * N);
+            for (int i = 0; i < w.nr; i++)
+                CNHE_CUDA(cudaMemcpyAsync(plains + (size_t)i * N, rows[w.r0 + i]->ptr(ch), N * 8, cudaMemcpyDeviceToDevice, c.stream));
+            std::vector<const u64 *> cts(w.nb);
+            for (int j = 0; j < w.nb; j++) cts[j] = vs[w.b0 + j]->ptr(ch);
+            op_multiply_plain_dense_outer(c, ch, cts, plains, w.nr, prod);
+            len = sum_slots_batched(c, ch, prod, m, length, pslot.data() + p0);
             if (force_dense) {
                 // one-hot masks (EncryptedSealBfvMatrix.cs:96, AtomicSealBfvVector.cs:936-945), built on the device
                 u64 *masks = c.ws_alloc((size_t)m * N);
-                for (const Seg &sg : segs) op_encode_onehot(c, ch, sg.len, first_row + sg.r0, masks + (size_t)sg.off * N);
+                for (int j = 0; j < w.nb; j++) op_encode_onehot(c, ch, w.nr, first_row + w.r0, masks + (size_t)j * w.nr * N);
                 op_multiply_plain_dense(c, ch, prod, m, masks, true, prod);
-                for (const Seg &sg : segs) {
+                for (int j = 0; j < w.nb; j++) {
+                    const int b = w.b0 + j;
                     std::vector<const u64 *> terms;
-                    if (!first[sg.b]) terms.push_back(outs[sg.b]->ptr(ch));
-                    for (int i = 0; i < sg.len; i++) terms.push_back(prod + (size_t)(sg.off + i) * ctw);
-                    do_add_many(c, ch, terms, outs[sg.b]->ptr(ch));
-                    first[sg.b] = 0;
+                    if (!first[b]) terms.push_back(outs[b]->ptr(ch));
+                    for (int i = 0; i < w.nr; i++) terms.push_back(prod + ((size_t)j * w.nr + i) * ctw);
+                    do_add_many(c, ch, terms, outs[b]->ptr(ch));
+                    first[b] = 0;
                 }
                 c.sync();
             }
         }
     }
-    for (int b = 0; b < B; b++) out[b] = outs[b].release();
+    if (dot) // SumAllSlots' bookkeeping (AtomicSealBfvVector.cs:946-954)
+        for (auto &o : outs) {
+            o->dim = len >= N / 2 ? 1 : o->dim;
+            o->format = len >= N ? CNHE_SPARSE : CNHE_DENSE;
+        }
+    for (int o = 0; o < n_out; o++) out[o] = outs[o].release();
 }
 extern "C" int cnhe_mat_mul_rowmajor(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *v, int force_dense, cnhe_vec **out) {
     API_BEGIN(h)
@@ -2165,6 +2376,15 @@ extern "C" int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *h, const cnhe_vec *const *r
                                            cnhe_vec **out) {
     API_BEGIN(h)
     mat_mul_rowmajor(c, rows, n_rows, vs, B, force_dense != 0, 0, n_rows, out);
+    API_END
+}
+// DotProduct(rows[r], vs[b], length) of every plain row with every encrypted vector (LLPackedDenseLayer's partial sums, one per client):
+// out[b * n_rows + r] is bit-identical to cnhe_vec_dot_product(rows[r], vs[b], length, -1), the row-major product's waves without its
+// final masks
+extern "C" int cnhe_mat_dot_rows_batch(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, uint64_t length,
+                                       cnhe_vec **out) {
+    API_BEGIN(h)
+    mat_mul_rowmajor(c, rows, n_rows, vs, B, false, 0, n_rows, out, length, true);
     API_END
 }
 // SquareActivation over a whole matrix: every column PointwiseMultiply'd with itself in one wave per channel

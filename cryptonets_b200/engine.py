@@ -563,6 +563,49 @@ class Engine:
         check(self.L.cnhe_mat_mul_rowmajor_batch(self.h, _vec_array(rows), len(rows), _vec_array(vs), B, int(force_dense), out))
         return self._wrap_many(out, B)
 
+    def dot_rows_batch(self, rows, vs, length=ALL_SLOTS):
+        """[[dot_product(r, v, length) for r in rows] for v in vs] in one pass (one input per client; their key slots may differ), flattened
+        client by client."""
+        B, R = len(vs), len(rows)
+        out = (VECP * (B * R))()
+        check(self.L.cnhe_mat_dot_rows_batch(self.h, _vec_array(rows), R, _vec_array(vs), B, int(length), out))
+        return self._wrap_many(out, B * R)
+
+    def duplicate_many(self, vecs, count):
+        """duplicate(v, count) for every v (one per client) in one pass."""
+        B = len(vecs)
+        out = (VECP * B)()
+        check(self.L.cnhe_vecs_duplicate_batch(self.h, _vec_array(vecs), B, int(count), out))
+        return self._wrap_many(out, B)
+
+    def permute_many(self, vecs, perms, output_dim):
+        """[permute(v, sel, shifts, output_dim) for (sel, shifts) in perms] for every v (one per client) in one pass, flattened client by
+        client; every permutation has the same number of selections (None entries are skipped)."""
+        B, P, S = len(vecs), len(perms), len(perms[0][0])
+        if any(len(sel) != S or len(sh) != S for sel, sh in perms):
+            raise ValueError("every permutation must have the same number of selections and shifts")
+        sh = (C.c_int * (P * S))(*[int(s) for _, shifts in perms for s in shifts])
+        out = (VECP * (B * P))()
+        check(self.L.cnhe_vecs_permute_batch(self.h, _vec_array(vecs), B, _vec_array([s for sel, _ in perms for s in sel]), sh, P, S, int(output_dim),
+                                             out))
+        return self._wrap_many(out, B * P)
+
+    def interleave_many(self, groups, shift):
+        """interleave(g, shift) for every group g (equal lengths; one per client) in one pass."""
+        B, n = len(groups), len(groups[0])
+        if any(len(g) != n for g in groups):
+            raise ValueError("every group must have the same number of vectors")
+        out = (VECP * B)()
+        check(self.L.cnhe_vecs_interleave_batch(self.h, _vec_array([v for g in groups for v in g]), n, B, int(shift), out))
+        return self._wrap_many(out, B)
+
+    def multiply_plain_many(self, vecs, plain):
+        """pointwise_multiply(v, plain) for every encrypted v and one plain dense vector in one pass."""
+        n = len(vecs)
+        out = (VECP * n)()
+        check(self.L.cnhe_vecs_multiply_plain(self.h, _vec_array(vecs), n, plain.h, out))
+        return self._wrap_many(out, n)
+
     def mat_mul_rowmajor_shard(self, rows, v, force_dense, first_row, total_rows):
         out = VECP()
         check(self.L.cnhe_mat_mul_rowmajor_shard(self.h, _vec_array(rows), len(rows), v.h, int(force_dense), int(first_row), int(total_rows), C.byref(out)))

@@ -396,6 +396,32 @@ class B200BfvFactory:
         out = self.engine.mat_mul_rowmajor_batch([r.vec for r in weights.vectors], [v.vec for v in vectors], ForceDenseFormat)
         return [B200BfvVector(self, o) for o in out]
 
+    def DuplicateBatch(self, vectors, count):
+        """v.Duplicate(count) for every encrypted vector (one per client; key slots may differ) in one pass."""
+        return [B200BfvVector(self, o) for o in self.engine.duplicate_many([v.vec for v in vectors], count)]
+
+    def PermuteBatch(self, vector_list, selections, shifts, outputDim):
+        """[v.Permute(selections[j], shifts[j], outputDim) for j] for every encrypted vector (one per client) in one pass; one list of
+        permuted vectors per client."""
+        perms = [([None if s is None else s.vec for s in sel], sh) for sel, sh in zip(selections, shifts)]
+        out, P = self.engine.permute_many([v.vec for v in vector_list], perms, outputDim), len(perms)
+        return [[B200BfvVector(self, o) for o in out[b * P:(b + 1) * P]] for b in range(len(vector_list))]
+
+    def DotRowsBatch(self, weights, vectors, length=None):
+        """[weights.GetRow(r).DotProduct(v, length=length) for r] of a plain row-major matrix for every v (one per client) in one pass; one
+        list of products per client."""
+        R = len(weights.vectors)
+        out = self.engine.dot_rows_batch([r.vec for r in weights.vectors], [v.vec for v in vectors], ALL_SLOTS if length is None else length)
+        return [[B200BfvVector(self, o) for o in out[b * R:(b + 1) * R]] for b in range(len(vectors))]
+
+    def InterleaveBatch(self, matrices, shift):
+        """m.Interleave(shift) of several column-major matrices (one per client, same column count) in one pass."""
+        return [B200BfvVector(self, o) for o in self.engine.interleave_many([[v.vec for v in m.vectors] for m in matrices], shift)]
+
+    def MultiplyPlainBatch(self, vectors, plain):
+        """v.PointwiseMultiply(plain) for every encrypted vector and one plain dense vector in one pass."""
+        return [B200BfvVector(self, o) for o in self.engine.multiply_plain_many([v.vec for v in vectors], plain.vec)]
+
     def MulDiagonalBatch(self, diag, vectors):
         """diag (B200BfvMatrix.PrepareDiagonal) times every encrypted vector (one per client; key slots may differ) in one pass; each result
         decrypts to the matrix's Mul(v, ForceDenseFormat=True)."""

@@ -433,6 +433,23 @@ def _is_column(m, v):
     return any(v is c for c in getattr(m, "vectors", []) or [])
 
 
+def _batchable(f, name, ms, columns=None):
+    """The factory's batched entry point `name` when it applies to these matrices (one per client): at least two, encrypted column-major
+    matrices with the same column count (`columns` when given) and columns of one dimension, scale and block count.  None otherwise
+    (the Raw backend, one client, differing shapes): the layer then applies one matrix at a time."""
+    batch = getattr(f, name, None)
+    if batch is None or len(ms) < 2:
+        return None
+    ref = ms[0].vectors[0]
+    for m in ms:
+        if m.Format != EMatrixFormat.ColumnMajor or m.ColumnCount != ms[0].ColumnCount or (columns is not None and m.ColumnCount != columns):
+            return None
+        for v in m.vectors:
+            if not v.IsEncrypted or v.Dim != ref.Dim or v.Scale != ref.Scale or v.Format != ref.Format or v.vec.blocks != ref.vec.blocks:
+                return None
+    return batch
+
+
 class LLPoolLayer(_ConvLayerBase):
     """`NeuralNetworks/LLPoolLayer.cs:10-153`: the input matrix is [corners x offsets] (im2col), one column per offset."""
 
@@ -653,6 +670,16 @@ class LLDuplicateLayer(BaseLayer):
         cols = [m.GetColumn(i).Duplicate(int(self.Count), env) for i in range(m.ColumnCount)]
         return self.Factory.GetMatrix(cols, m.Format, CopyVectors=False)
 
+    def ApplyBatch(self, ms):
+        """Every column of every client duplicated in one pass (cnhe_vecs_duplicate_batch)."""
+        f = self.Factory
+        batch = _batchable(f, "DuplicateBatch", ms)
+        if batch is None:
+            return super().ApplyBatch(ms)
+        n = ms[0].ColumnCount
+        out = batch([v for m in ms for v in m.vectors], int(self.Count))
+        return [f.GetMatrix(out[b * n:(b + 1) * n], m.Format, CopyVectors=False) for b, m in enumerate(ms)]
+
     def OutputDimension(self):
         shift, dim = 1, self.Source.OutputDimension()
         while shift < dim:
@@ -688,6 +715,19 @@ class LLInterleaveLayer(BaseLayer):
         packed = cm.Interleave(self.Shift, env)
         cm.Dispose()
         return f.GetMatrix([packed], EMatrixFormat.ColumnMajor, CopyVectors=False)
+
+    def ApplyBatch(self, ms):
+        """Every client's mask products in one pass (cnhe_vecs_multiply_plain), then every client's interleave (cnhe_vecs_interleave_batch)."""
+        f = self.Factory
+        if _batchable(f, "MultiplyPlainBatch", ms) is None or not hasattr(f, "InterleaveBatch"):
+            return super().ApplyBatch(ms)
+        n = ms[0].ColumnCount
+        clean = f.MultiplyPlainBatch([v for m in ms for v in m.vectors], self.mask)
+        cms = [f.GetMatrix(clean[b * n:(b + 1) * n], EMatrixFormat.ColumnMajor, CopyVectors=False) for b in range(len(ms))]
+        packed = f.InterleaveBatch(cms, self.Shift)
+        for cm in cms:
+            cm.Dispose()
+        return [f.GetMatrix([v], EMatrixFormat.ColumnMajor, CopyVectors=False) for v in packed]
 
     def OutputDimension(self):
         return self.InputGrossDimension
@@ -749,6 +789,20 @@ class LLPackedDenseLayer(BaseLayer):
             mul.Dispose()
         return self.Factory.GetMatrix(res, EMatrixFormat.ColumnMajor, CopyVectors=False)
 
+    def ApplyBatch(self, ms):
+        """Every row's partial dot product with every client's vector in one pass (cnhe_mat_dot_rows_batch), then each row's bias."""
+        f = self.Factory
+        batch = _batchable(f, "DotRowsBatch", ms, columns=1)
+        if batch is None or ms[0].vectors[0].vec.blocks != 1:
+            return super().ApplyBatch(ms)
+        env = f.AllocateComputationEnv()
+        out = []
+        for muls in batch(self.WeightsMatrix, [m.GetColumn(0) for m in ms], int(self.PackingShift)):
+            out.append(f.GetMatrix([mul.Add(self.BiasMatrix.GetRow(k), env) for k, mul in enumerate(muls)], EMatrixFormat.ColumnMajor, CopyVectors=False))
+            for mul in muls:
+                mul.Dispose()
+        return out
+
     def Dispose(self):
         for mat in (self.WeightsMatrix, self.BiasMatrix):
             if mat is not None:
@@ -805,6 +859,19 @@ class LLInterleavedDenseLayer(BaseLayer):
         v = mul.Add(self.BiasVector, env)
         mul.Dispose()
         return self.Factory.GetMatrix([v], EMatrixFormat.ColumnMajor, CopyVectors=False)
+
+    def ApplyBatch(self, ms):
+        """Every client's sparse row-major product in one pass (cnhe_mat_mul_rowmajor_batch), then each one's bias."""
+        f = self.Factory
+        batch = _batchable(f, "MulRowMajorBatch", ms, columns=1)
+        if batch is None or ms[0].vectors[0].vec.blocks != 1 or not self.WeightsMatrix.Batched:
+            return super().ApplyBatch(ms)
+        env = f.AllocateComputationEnv()
+        out = []
+        for mul in batch(self.WeightsMatrix, [m.GetColumn(0) for m in ms], False):
+            out.append(f.GetMatrix([mul.Add(self.BiasVector, env)], EMatrixFormat.ColumnMajor, CopyVectors=False))
+            mul.Dispose()
+        return out
 
     def Dispose(self):
         if self.WeightsMatrix is not None:
@@ -927,6 +994,17 @@ class LLPreConvLayer(BaseLayer):
         v = m.GetColumn(0)
         cols = [v.Permute(self.masks[k], self.shifts[k], self.outputDim, env) for k in range(len(self.masks))]
         return self.Factory.GetMatrix(cols, EMatrixFormat.ColumnMajor, CopyVectors=False)
+
+    def ApplyBatch(self, ms):
+        """Every client's permutations in one pass (cnhe_vecs_permute_batch): one outer mask product, one wave per rotation hop."""
+        f = self.Factory
+        batch = _batchable(f, "PermuteBatch", ms, columns=1)
+        if batch is None:
+            return super().ApplyBatch(ms)
+        if not self.layerPrepared:
+            self.Prepare()
+        return [f.GetMatrix(cols, EMatrixFormat.ColumnMajor, CopyVectors=False)
+                for cols in batch([m.GetColumn(0) for m in ms], self.masks, self.shifts, self.outputDim)]
 
     def OutputDimension(self):
         if not self.layerPrepared:

@@ -227,6 +227,20 @@ int cnhe_vecs_stack(cnhe_ctx *, const cnhe_vec *const *vecs, int n, cnhe_vec **o
  * must not): out[b] is bit-identical to cnhe_vecs_stack(vecs + b * n, n), the rotations of all groups share key-switch waves. */
 int cnhe_vecs_stack_batch(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int B, cnhe_vec **out /*B*/);
 int cnhe_vecs_generate_sparse_of_array(cnhe_ctx *, const cnhe_vec *const *vecs, int n, cnhe_vec **out); /* :1347-1359 */
+/* One vector operation for B vectors at once (one per client, as many LoLa layers serve several clients in one pass; their key slots may
+ * differ).  Each output is bit-identical to the single call named; every key-switching stage runs as one wave over all clients, and the
+ * plain products of several clients with the same plaintexts transform each plaintext once.  The inputs must share dimension, scale,
+ * format, block count and encryption (CNHE_ERR_INVALID otherwise, as for B < 1); other refusals are the single call's.
+ * cnhe_vecs_duplicate_batch: out[b] = cnhe_vec_duplicate(vecs[b], count).
+ * cnhe_vecs_permute_batch: out[b * n_perm + j] = cnhe_vec_permute(vecs[b], selections + j * n_sel, shifts + j * n_sel, n_sel, output_dim)
+ *   (selections [n_perm][n_sel], NULL entries skipped; LLPreConvLayer's permutations of one image).
+ * cnhe_vecs_interleave_batch: out[b] = cnhe_vecs_interleave(vecs + b * n, n, shift), vecs [B][n].
+ * cnhe_vecs_multiply_plain: out[i] = cnhe_vec_pointwise_multiply(vecs[i], plain) for n encrypted vectors and one plain dense vector. */
+int cnhe_vecs_duplicate_batch(cnhe_ctx *, const cnhe_vec *const *vecs, int B, uint64_t count, cnhe_vec **out /*B*/);
+int cnhe_vecs_permute_batch(cnhe_ctx *, const cnhe_vec *const *vecs, int B, const cnhe_vec *const *selections, const int *shifts, int n_perm,
+                            int n_sel, uint64_t output_dim, cnhe_vec **out /*B*n_perm*/);
+int cnhe_vecs_interleave_batch(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int B, int shift, cnhe_vec **out /*B*/);
+int cnhe_vecs_multiply_plain(cnhe_ctx *, const cnhe_vec *const *vecs, int n, const cnhe_vec *plain, cnhe_vec **out /*n*/);
 /* cnhe_vec_rotate of n vectors by the same amount in one pass (out[i] = rotation of vecs[i]); the vectors may belong to different key
  * slots.  Bit-identical to n cnhe_vec_rotate calls. */
 int cnhe_vecs_rotate(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int amount, cnhe_vec **out /*n*/);
@@ -246,6 +260,11 @@ int cnhe_mat_mul_rowmajor_shard(cnhe_ctx *, const cnhe_vec *const *rows, int n_r
  * bit-identical to cnhe_mat_mul_rowmajor(rows, n_rows, vs[b], force_dense), the key switches of all B x n_rows products share waves. */
 int cnhe_mat_mul_rowmajor_batch(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, int force_dense,
                                 cnhe_vec **out /*B*/);
+/* DotProduct of every plain row with every encrypted vector (LLPackedDenseLayer's partial sums for B clients): out[b * n_rows + r] is
+ * bit-identical to cnhe_vec_dot_product(rows[r], vs[b], length, -1), dimension and format included.  Rows and vectors as
+ * cnhe_mat_mul_rowmajor_batch takes them. */
+int cnhe_mat_dot_rows_batch(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *const *vs, int B, uint64_t length,
+                            cnhe_vec **out /*B*n_rows*/);
 /* Diagonal (Halevi-Shoup) product with baby-step / giant-step, the opt-in alternative to the ForceDenseFormat row-major product above for
  * large dense layers: about sqrt(N) rotations per input instead of 14 per row, and no one-hot mask multiply (DESIGN.md section 4.10).
  * Slot i sits at row i / (N/2), column i % (N/2) of the BatchEncoder's matrix.  Diagonal (b, s) of a matrix M (b in {0, 1}, s < N/2)

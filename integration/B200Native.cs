@@ -92,6 +92,11 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_colmajor_sparse(IntPtr a0, IntPtr[] cols, int K, IntPtr sparse, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_rowmajor(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr v, int force_dense, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_rowmajor_batch(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr[] vs, int B, int force_dense, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_dot_rows_batch(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr[] vs, int B, ulong length, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_duplicate_batch(IntPtr a0, IntPtr[] vecs, int B, ulong count, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_permute_batch(IntPtr a0, IntPtr[] vecs, int B, IntPtr[] selections, int[] shifts, int n_perm, int n_sel, ulong output_dim, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_interleave_batch(IntPtr a0, IntPtr[] vecs, int n, int B, int shift, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_multiply_plain(IntPtr a0, IntPtr[] vecs, int n, IntPtr plain, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_rowmajor_shard(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr v, int force_dense, int first_row, int total_rows, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_diag_prepare(IntPtr a0, IntPtr[] rows, int n_rows, int baby_steps, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_diag_info(IntPtr a0, out int n_rows, out ulong dim, out int n1, out int n2, out int n_diags, out ulong device_bytes);

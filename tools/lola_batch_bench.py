@@ -1,13 +1,15 @@
 """Multi-client LoLa serving: images/s and per-batch latency of B clients' inferences run together (networks.serve_batch), each client
 with its own secret key and compact key set in a key slot of one server context.
 
-    python tools/lola_batch_bench.py [--nets lola_small,lola_cifar] [--batches 1,8,32,128] [--reps 3]
+    python tools/lola_batch_bench.py [--nets lola_small,lola,lola_dense,lola_cifar] [--batches 1,8,32,128] [--reps 3]
 
 Timing: CUDA events on the server context around serve_batch, after one warm-up batch of every B.  Also reported: the share of
 key-switch launches that took the fused kernel (cnhe_prof_collect in a separate, untimed pass; INFERRED, not counted: the fused
 kernel runs its inverse transforms itself, so the inverse-transform launches (family 1) are taken as digit-path key switches -- at
-N = 16384 the multiplies' inverse transforms are counted there too), and the card name, power limit and
-maximum SM clock from nvidia-smi (queries only).  Prints one JSON line per (net, B)."""
+N = 16384 the multiplies' inverse transforms are counted there too), the device time per kernel family in that profiled pass, and the
+card name, power limit and maximum SM clock from nvidia-smi (queries only).  Prints one JSON line per (net, B).  Every network runs with
+the reference's parameters (lola_small, LoLa-Dense and LoLa-CIFAR with their SmallModulusCount; timing does not need the scores to
+decrypt)."""
 import argparse
 import json
 import os
@@ -31,9 +33,14 @@ def setup(net_name, B):
     from cryptonets_b200.he import B200BfvFactory
     from cryptonets_b200.interfaces import EMatrixFormat
     from cryptonets_b200 import networks as nw
+    w60 = dict(DecompositionBitCount=60, GaloisDecompositionBitCount=60)
     if net_name == "lola_small":
         build, primes, n, kw, count, imgs = nw.lola_small, nw.LOLA_SMALL_PRIMES, 8192, dict(DecompositionBitCount=40, GaloisDecompositionBitCount=40), 3, \
             nw.synthetic_mnist(B, seed=1)
+    elif net_name == "lola":
+        build, primes, n, kw, count, imgs = nw.lola, nw.LOLA_PRIMES, 8192, {}, -1, nw.synthetic_mnist(B, seed=1)
+    elif net_name == "lola_dense":
+        build, primes, n, kw, count, imgs = nw.lola_dense, nw.LOLA_DENSE_PRIMES, 16384, w60, 7, nw.synthetic_mnist(B, seed=1)
     else:
         build, primes, n, kw, count, imgs = nw.lola_cifar, nw.CIFAR_PRIMES, 16384, dict(DecompositionBitCount=60, GaloisDecompositionBitCount=60), 8, \
             nw.synthetic_cifar(B, seed=1)
@@ -91,7 +98,7 @@ def fused_share(server, net, inputs):
     # per key switch the digit path launches one MAC and one inverse-add; the only other inverse transforms of these networks are the
     # plain multiplies', which do not run under a profiling scope
     digit = min(prof["ntt_inverse"]["launches"], ks)
-    return (ks - digit) / ks if ks else 0.0, ks
+    return (ks - digit) / ks if ks else 0.0, ks, {k: round(v["ms"], 2) for k, v in prof.items()}
 
 
 def main():
@@ -107,10 +114,10 @@ def main():
             server, net, inputs = setup(net_name, B)
             run(server, net, inputs)  # warm-up of this B
             times = sorted(run(server, net, inputs) for _ in range(args.reps))
-            share, ks = fused_share(server, net, inputs)
+            share, ks, families = fused_share(server, net, inputs)
             med = times[len(times) // 2]
             print(json.dumps(dict(net=net_name, B=B, batch_ms=round(med, 2), images_per_s=round(1000.0 * B / med, 1), keyswitch_launches=ks,
-                                  fused_share=round(share, 3), reps=args.reps, **info)), flush=True)
+                                  fused_share=round(share, 3), family_ms=families, reps=args.reps, **info)), flush=True)
             server.Dispose()
 
 
