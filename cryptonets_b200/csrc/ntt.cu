@@ -1106,13 +1106,16 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
 // independent N/2-point transforms (the split form of the N = 16384 kernels), so CTA h folds stage 0 into its loads (it reads both halves
 // of the source residue, an L2 hit: the partner and the other residues' CTAs read the same lines at about the same time), runs the
 // N/2-point passes in shared memory and, in the last pass, multiplies its 16 coefficients per thread by the matching key words and
-// accumulates them in shared memory ([key poly][coefficient pair][thread]: every thread touches only its own slots, no extra barrier).
-// The twiddle cache is filled once per CTA instead of once per transform, and the next digit's source words are in flight while the CTA
-// waits at the barrier that ends the current digit.  Same arithmetic as the MAC kernels (fmodmul + dadd, re-centred every 8 digits and
+// accumulates them: thread j owns coefficients 16j..16j+15 of both accumulators, polynomial 0 in registers and polynomial 1 in shared
+// memory in the group layout of st_group16 (every thread touches only its own group, no extra barrier).
+// Shared memory is [work 0][work 1][acc 1][twiddle caches]: digit d's passes run in work buffer d & 1, so one block barrier per digit
+// (the all-to-all hand-off after the first pass) is all the loop needs, and warps may drift up to a digit apart.
+// The twiddle cache is filled once per CTA instead of once per transform, and a warp's next digit's source words are in flight while
+// other warps finish the current digit.  Same arithmetic as the MAC kernels (fmodmul + dadd, re-centred every 8 digits and
 // at the end), so the accumulators end at |x| <= 0.51 p, within the inverse transform's 1.25 p input bound.
-// Epilogue: the pair of CTAs is a cluster and finishes the key switch as k_behz_square_fused does: thread j holds coefficients 16j..16j+15
-// of both accumulators, exactly the group the split inverse's first four stages work on, so it runs them in registers and stores the two
-// results as consecutive half buffers (polynomial 0 over the work buffer, polynomial 1 over the polynomial-0 accumulator), then the
+// Epilogue: the pair of CTAs is a cluster and finishes the key switch as k_behz_square_fused does: thread j's group of each accumulator is
+// exactly the group the split inverse's first four stages work on, so it runs them in registers and stores the two results as
+// consecutive half buffers (polynomial 0 into work buffer 1, polynomial 1 in place over its accumulator), then the
 // remaining in-half pass of both and the cross-half stage (N^-1, canonical output, plus the base word) through DSMEM.  The base half is
 // prefetched to L2 during the last digit.  Compared with writing the accumulator and running k_ntt_inverse_ws, every (ciphertext,
 // polynomial, residue) saves an 8N-byte HBM write and read and a second kernel.  Other CTAs may still read target and base words while a
@@ -1128,7 +1131,7 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
 template <int HLOGN>
 __host__ __device__ constexpr int ks_fused_threads() { return (1 << HLOGN) / 16; }
 template <int HLOGN>
-__host__ __device__ constexpr int ks_fused_smem() { return (1 << HLOGN) * 8 * 3 + 2 * TWC * 8; } // work buffer, two accumulators, two twiddle caches
+__host__ __device__ constexpr int ks_fused_smem() { return (1 << HLOGN) * 8 * 3 + 2 * TWC * 8; } // two work buffers, polynomial-1 accumulator, two twiddle caches
 // a word below 2^48 given as its low 32 bits and bits 32..47, as an exact double (u2d of the same word)
 __device__ __forceinline__ double u48d(unsigned lo, unsigned hi16) { return __dsub_rn(__hiloint2double((int)(hi16 | 0x43300000u), (int)lo), FP_TWO52); }
 // packed copy: the 16 key words of (polynomial b, half, thread j), 48 bits each, little-endian in 24 u32: word 2m in u32 3m and the low
@@ -1160,8 +1163,8 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
     constexpr int H = 1 << HLOGN, TR = ks_fused_threads<HLOGN>(), N = 2 * H;
     constexpr int R1 = HLOGN - 8, E1 = 1 << R1, LG1 = HLOGN - R1; // first pass: stage 0 on the loads, then R1 stages; then 4 + 4
     extern __shared__ __align__(16) u64 ks_raw[];
-    double *sm = reinterpret_cast<double *>(ks_raw);           // [3][H]: work buffer, then the inverse's two half buffers
-    double2 *accv = reinterpret_cast<double2 *>(sm + H);       // [p][e/2][TR]
+    double *sm = reinterpret_cast<double *>(ks_raw);           // [3][H]: work buffers 0 and 1, polynomial-1 accumulator
+    double *acc1 = sm + 2 * H;                                 // group layout (st_group16); work 1 and acc 1 are the inverse's half buffers
     double *twc = sm + 3 * H, *twci = twc + TWC;               // forward / inverse twiddles of this half
     const int half = blockIdx.x & 1, l = (blockIdx.x >> 1) % k, c = (blockIdx.x >> 1) / k, tid = threadIdx.x;
     NttTab tb = tabs[l];
@@ -1169,8 +1172,7 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
     tb.wd = tb.wd_split + half * H;
     tb.iwd = tb.iwd_split + half * H;
     tb.fwd_recenter = tb.fwd_recenter_split;
-    const double2 *twg = reinterpret_cast<const double2 *>(tb.wd_split_grp + half * H);   // last forward pass, grouped
-    const double2 *twgi = reinterpret_cast<const double2 *>(tb.iwd_split_grp + half * H); // first inverse stages, grouped
+    const double2 *twg = reinterpret_cast<const double2 *>(tb.wd_split_grp + half * H); // last forward pass, grouped
     const double p = tb.pd, pinv = tb.pinv;
     const bool need_reduce = dm.mask >= tb.mod.p;
     const u64 *src_c = target + (size_t)c * ct_stride;
@@ -1182,14 +1184,21 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
     const u64 *key_l = key + (size_t)l * N + half * H + 16 * tid;
     load_twiddle_cache(twc, tb.wd, tid, TR);
     load_twiddle_cache(twci, tb.iwd, tid, TR);
+    double acc0[16]; // polynomial 0's accumulator: coefficients 16 tid .. 16 tid + 15
 #pragma unroll
-    for (int i = 0; i < 16; i++) accv[i * TR + tid] = make_double2(0.0, 0.0);
+    for (int e = 0; e < 16; e++) acc0[e] = 0.0;
+    st_group16(acc1, tid, acc0);
     auto cut = [&](u64 v, int shift) { // digit of a canonical word: exact below 2^50
         const double x = u2d((v >> shift) & dm.mask);
         return need_reduce ? frecenter(x, p, pinv) : x;
     };
+    __syncthreads(); // the twiddle caches are filled
 #pragma unroll 1
     for (int d = 0; d < dm.D; d++) {
+        // Digit d runs in work buffer d & 1, whose last user was digit d - 2: every thread passed the barrier after digit d - 1's first
+        // pass only once it had finished digit d - 2 (its middle- and last-pass reads included), and this thread has passed that barrier
+        // too, so the first-pass stores below need no barrier of their own.
+        double *wb = sm + (d & 1) * H;
         const u64 *src = src_c + (size_t)dm.src[d] * N;
         const int shift = dm.shift[d];
         if (d == dm.D - 1) { // the epilogue adds this half of both base polynomials: have them waiting in L2
@@ -1200,7 +1209,7 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
             }
         }
         constexpr int VT1 = (H >> R1) / TR; // first-pass virtual threads per thread
-        double xs[VT1][E1]; // stage 0 of the N-point transform, computed while other warps finish the previous digit
+        double xs[VT1][E1]; // stage 0 of the N-point transform
 #pragma unroll
         for (int v = 0; v < VT1; v++)
 #pragma unroll
@@ -1209,7 +1218,6 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
                 const double a = cut(src[idx], shift), t = fmodmul(cut(src[idx + H], shift), w0, p, pinv);
                 xs[v][e] = half ? __dsub_rn(a, t) : __dadd_rn(a, t);
             }
-        __syncthreads(); // the previous digit's last pass is done with the work buffer (d = 0: the twiddle cache is filled)
 #pragma unroll
         for (int v = 0; v < VT1; v++) {
             const int vt = tid + v * TR;
@@ -1227,86 +1235,106 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
                     x[e + h] = __dsub_rn(a, t);
                 }
             }
+            // swz only moves bits 1..3 by bits 4..6, so with LG1 >= 7 this is wb[swz(vt + (e << LG1))]: one address register and
+            // immediate offsets instead of 2^R1 swizzled offsets the compiler would keep live through the digit loop
+            static_assert(LG1 >= 7, "first-pass store offsets must not touch the swizzle's bits");
+            double *o = wb + swz(vt);
 #pragma unroll
-            for (int e = 0; e < E1; e++) sm[swz(vt + (e << LG1))] = x[e];
+            for (int e = 0; e < E1; e++) o[e << LG1] = x[e];
         }
-        __syncthreads();
+        __syncthreads(); // the first pass is all-to-all
         {
             FwdSrc unused;
             unused.src = nullptr; unused.digit = false; unused.need_reduce = false; unused.shift = 0; unused.mask = 0;
-            fwd_pass_fp<HLOGN, R1, 4, false, 1, false>(sm, twc, unused, tb, tid);
+            fwd_pass_fp<HLOGN, R1, 4, false, 1, false>(wb, twc, unused, tb, tid);
         }
         __syncwarp(); // the middle pass wrote 256-coefficient block tid >> 4, whose groups 16j..16j+15 this half warp reads next
         // last pass (stages HLOGN-4 .. HLOGN-1 on 16 consecutive coefficients), then the key product
         double x[16];
-        ld_group16(sm, tid, x);
+        // j is tid, opaque to the compiler: the 8 chunk offsets of the thread's group (work buffer and acc 1) are recomputed each digit,
+        // a few integer instructions, instead of being held in registers through the loop beside acc0, where they would spill
+        int j = tid;
+        asm volatile("" : "+r"(j));
+        double2 *acc1v = reinterpret_cast<double2 *>(acc1) + 8 * j; // pair i of the group sits at acc1v[i ^ (j & 7)] (st_group16)
+        const int xr = j & 7;
+        ld_group16(wb, j, x);
         fwd_last_stages_grp<HLOGN, 2>(x, tb, twg, tid);
         if (tb.split_out_rc) {
 #pragma unroll
             for (int e = 0; e < 16; e++) x[e] = frecenter(x[e], p, pinv);
         }
         const bool rc = (d & 7) == 7 || d == dm.D - 1;
+        // coefficient pair i (words 2i, 2i+1) of key polynomial kp into its accumulator; sums of 8 fresh products stay below 4.1 p, so
+        // they are re-centred before they could leave the exact range (and at the end)
+        auto mac = [&](int kp, int i, double k0, double k1) {
+            if (kp == 0) {
+                acc0[2 * i] = __dadd_rn(acc0[2 * i], fmodmul(x[2 * i], k0, p, pinv));
+                acc0[2 * i + 1] = __dadd_rn(acc0[2 * i + 1], fmodmul(x[2 * i + 1], k1, p, pinv));
+                if (rc) {
+                    acc0[2 * i] = frecenter(acc0[2 * i], p, pinv);
+                    acc0[2 * i + 1] = frecenter(acc0[2 * i + 1], p, pinv);
+                }
+            } else {
+                double2 a = acc1v[i ^ xr];
+                a.x = __dadd_rn(a.x, fmodmul(x[2 * i], k0, p, pinv));
+                a.y = __dadd_rn(a.y, fmodmul(x[2 * i + 1], k1, p, pinv));
+                if (rc) {
+                    a.x = frecenter(a.x, p, pinv);
+                    a.y = frecenter(a.y, p, pinv);
+                }
+                acc1v[i ^ xr] = a;
+            }
+        };
 #pragma unroll
         for (int kp = 0; kp < 2; kp++) {
-            double kd[16];
             if constexpr (PK) {
                 const uint4 *kw = keyp + ((((size_t)d * 2 + kp) * k + l) * 2 + half) * 6 * TR + tid;
-                unsigned u[24];
 #pragma unroll
-                for (int g = 0; g < 6; g++) {
-                    const uint4 v = __ldg(kw + g * TR);
-                    u[4 * g] = v.x; u[4 * g + 1] = v.y; u[4 * g + 2] = v.z; u[4 * g + 3] = v.w;
-                }
+                for (int hb = 0; hb < 2; hb++) { // 8 words from 3 groups at a time: all 24 u32 beside acc0 would not fit in 128 registers
+                    unsigned u[12];
 #pragma unroll
-                for (int m = 0; m < 8; m++) {
-                    kd[2 * m] = u48d(u[3 * m], u[3 * m + 1] & 0xffff);
-                    kd[2 * m + 1] = u48d(__funnelshift_r(u[3 * m + 1], u[3 * m + 2], 16), u[3 * m + 2] >> 16);
+                    for (int g = 0; g < 3; g++) {
+                        const uint4 v = __ldg(kw + (3 * hb + g) * TR);
+                        u[4 * g] = v.x; u[4 * g + 1] = v.y; u[4 * g + 2] = v.z; u[4 * g + 3] = v.w;
+                    }
+#pragma unroll
+                    for (int m = 0; m < 4; m++)
+                        mac(kp, 4 * hb + m, u48d(u[3 * m], u[3 * m + 1] & 0xffff),
+                            u48d(__funnelshift_r(u[3 * m + 1], u[3 * m + 2], 16), u[3 * m + 2] >> 16));
                 }
             } else {
                 const u64 *kw = key_l + (size_t)d * kstride + kp * kpoly;
 #pragma unroll
                 for (int i = 0; i < 8; i++) {
                     const ulonglong2 w = __ldg(reinterpret_cast<const ulonglong2 *>(kw) + i);
-                    kd[2 * i] = u2d(w.x);
-                    kd[2 * i + 1] = u2d(w.y);
+                    mac(kp, i, u2d(w.x), u2d(w.y));
                 }
-            }
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                double2 a = accv[(kp * 8 + i) * TR + tid];
-                a.x = __dadd_rn(a.x, fmodmul(x[2 * i], kd[2 * i], p, pinv));
-                a.y = __dadd_rn(a.y, fmodmul(x[2 * i + 1], kd[2 * i + 1], p, pinv));
-                if (rc) { // sums of 8 fresh products stay below 4.1 p; re-centre before they could leave the exact range (and at the end)
-                    a.x = frecenter(a.x, p, pinv);
-                    a.y = frecenter(a.y, p, pinv);
-                }
-                accv[(kp * 8 + i) * TR + tid] = a;
             }
         }
     }
+    // The inverse's table fields are read again here: held in registers through the digit loop beside acc0, they would spill.  The
+    // empty asm hides that the pointer is tabs + l, so the compiler cannot reuse the loads made before the loop.
+    const NttTab *tabl = tabs + l;
+    asm("" : "+l"(tabl));
+    NttTab ti = *tabl;
+    ti.iwd = ti.iwd_split + half * H;
+    const double2 *twgi = reinterpret_cast<const double2 *>(ti.iwd_split_grp + half * H); // first inverse stages, grouped
+    // Inverse stages 0..3 of both accumulators in registers, each on the thread's own group: polynomial 0 into work buffer 1 (whichever
+    // buffer the last digit used, group tid of it is read by no other thread now), polynomial 1 in place.
+    inv_first_stages_grp<HLOGN>(acc0, ti, twgi, tid);
+    st_group16(sm + H, tid, acc0);
     {
-        // inverse stages 0..3 of both accumulators in registers.  Polynomial 0 goes over the work buffer: thread j's group there is the one it
-        // read itself in the last forward pass.  Polynomial 1 goes over the polynomial-0 accumulator once every thread has read its slots.
         double x[16];
-#pragma unroll
-        for (int kp = 0; kp < 2; kp++) {
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                const double2 a = accv[(kp * 8 + i) * TR + tid];
-                x[2 * i] = a.x;
-                x[2 * i + 1] = a.y;
-            }
-            inv_first_stages_grp<HLOGN>(x, tb, twgi, tid);
-            if (kp) __syncthreads();
-            st_group16(sm + kp * H, tid, x);
-        }
+        ld_group16(acc1, tid, x);
+        inv_first_stages_grp<HLOGN>(x, ti, twgi, tid);
+        st_group16(acc1, tid, x);
     }
     __syncwarp(); // inv_pass_fp<.., 4, 4> works on 256-coefficient block tid >> 4 of each buffer: the groups this half warp just stored
 #pragma unroll 1
-    for (int r = 0; r < 2; r++) CNHE_VTN(H / 16, (inv_pass_fp<HLOGN, 4, 4, false, false>(sm + r * H, twci, nullptr, nullptr, tb, vt)));
+    for (int r = 1; r < 3; r++) CNHE_VTN(H / 16, (inv_pass_fp<HLOGN, 4, 4, false, false>(sm + r * H, twci, nullptr, nullptr, ti, vt)));
     __syncthreads();
     const size_t ol = (size_t)l * N + half * H;
-    inv_split_last<HLOGN, TR, false, 2>(sm, twci, out + (size_t)c * kstride + ol, kpoly, base + (size_t)c * base_stride + ol, tb, tid, half);
+    inv_split_last<HLOGN, TR, false, 2>(sm + H, twci, out + (size_t)c * kstride + ol, kpoly, base + (size_t)c * base_stride + ol, ti, tid, half);
 }
 
 // ================================================================ fused BEHZ square, N = 4096 / 8192

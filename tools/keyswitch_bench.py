@@ -48,14 +48,14 @@ DP_WARP_INSTR_PER_CT = (DP_PER_THREAD * D + DP_INVERSE_PER_THREAD) * (256 // 32)
 
 def l1_wavefronts_per_cta_digit(key_word, grouped):
     """128-byte L1 / shared-memory data-path wavefronts of one CTA and one digit (N = 8192: 4096-point half, 256 threads, 8 warps),
-    counted from the shapes: work buffer (pass-1 store, pass-2 load + store, last-pass load), accumulators (two polynomials, load +
-    store), twiddle-cache reads of passes 1-2 (15 distinct words per thread and pass, one wavefront per warp load), source words (both
+    counted from the shapes: work buffer (pass-1 store, pass-2 load + store, last-pass load), the polynomial-1 accumulator (load +
+    store; polynomial 0's sits in registers), twiddle-cache reads of passes 1-2 (15 distinct words per thread and pass, one wavefront per warp load), source words (both
     halves, coalesced), key words (two polynomials, coalesced) and the last pass's 15 twiddles per thread: 8 warp loads of 512
     contiguous bytes from the grouped table, or scalar loads whose lanes sit 2^u words apart at stage u (a warp load touches
     min(32, 2^(u+1)) lines, 2^u loads per stage).  A model: not measured."""
     H, T, W = 4096, 256, 8
     work = 4 * H * 8 // 128
-    acc = 2 * 2 * H * 8 // 128
+    acc = 2 * H * 8 // 128
     twc = 2 * 15 * W
     src = 2 * H * 8 // 128
     keys = int(2 * H * key_word) // 128
