@@ -86,6 +86,86 @@ __global__ void __launch_bounds__(256) k_diag_mac(const u64 *__restrict__ dhat, 
     }
 }
 
+// One term of k_diag_mac_resident: CB clients' two polynomials at a coefficient pair, x loaded as 16-byte words.
+template <int CB>
+__device__ __forceinline__ void diag_mac_pair(double (&a)[CB][2][2], const u64 *xs, size_t ct, size_t kN, int nb, double d0, double d1, double p,
+                                              double pinv) {
+#pragma unroll
+    for (int cb = 0; cb < CB; cb++) {
+        if (cb < nb) {
+            const ulonglong2 x0 = __ldg(reinterpret_cast<const ulonglong2 *>(xs + cb * ct));
+            const ulonglong2 x1 = __ldg(reinterpret_cast<const ulonglong2 *>(xs + cb * ct + kN));
+            a[cb][0][0] = __dadd_rn(a[cb][0][0], fmodmul(u2d(x0.x), d0, p, pinv));
+            a[cb][0][1] = __dadd_rn(a[cb][0][1], fmodmul(u2d(x0.y), d1, p, pinv));
+            a[cb][1][0] = __dadd_rn(a[cb][1][0], fmodmul(u2d(x1.x), d0, p, pinv));
+            a[cb][1][1] = __dadd_rn(a[cb][1][1], fmodmul(u2d(x1.y), d1, p, pinv));
+        }
+    }
+}
+
+// k_diag_mac over diagonals held resident in NTT form (cnhe_diag_prepare_ntt): nothing produced them just before, so every diagonal word
+// streams from HBM, and the kernel is built for that.  One thread per (g, l, coefficient pair): 16-byte loads of the diagonal and of the
+// baby-step words.  A full re-centring period (8 diagonals) is straight-line code in chunks of D diagonals: a chunk's D diagonal loads
+// (evict-first, so that they do not push the baby-step words the giant steps share out of L2) and baby-step indices are issued before its
+// first product, so D diagonals' loads are in flight together with the baby-step loads the compiler hoists.  D trades loads in flight
+// against registers, and so against resident warps.  CTA order as in k_diag_mac (g fastest, then the 512-coefficient tile, then l).  Per
+// (g, client, l, i) the arithmetic is k_diag_mac's in the same order: fmodmul of canonical operands, dadd, re-centred after every 8th term
+// and at the end, fsmall_u -- so the outputs are bit-identical.
+template <int CB, int D>
+__global__ void __launch_bounds__(256) k_diag_mac_resident(const u64 *__restrict__ dhat, const u64 *__restrict__ xhat, const int *__restrict__ g_start,
+                                                           const int *__restrict__ xsel, u64 *__restrict__ acc, int ng, int B, int logn,
+                                                           const __grid_constant__ BehzConstF F) {
+    static_assert(8 % D == 0, "D divides the re-centring period");
+    const int N = 1 << logn, k = F.k, tiles = N >> 9;
+    const int g = blockIdx.x % ng, tile = (blockIdx.x / ng) % tiles, l = blockIdx.x / (ng * tiles);
+    const int i = (tile << 9) + 2 * threadIdx.x;
+    const double p = F.qd[l], pinv = F.qinv[l];
+    const size_t kN = (size_t)k * N, ct = 2 * kN;
+    const int j0 = g_start[g], j1 = g_start[g + 1];
+    const u64 *dl = dhat + (size_t)l * N + i;
+    for (int b0 = 0; b0 < B; b0 += CB) {
+        const int nb = B - b0;
+        const u64 *xl = xhat + (size_t)b0 * ct + (size_t)l * N + i;
+        double a[CB][2][2]; // [client][polynomial][coefficient of the pair]
+#pragma unroll
+        for (int cb = 0; cb < CB; cb++) a[cb][0][0] = a[cb][0][1] = a[cb][1][0] = a[cb][1][1] = 0.0;
+        int jb = j0;
+        for (; jb + 8 <= j1; jb += 8) {
+#pragma unroll
+            for (int c0 = 0; c0 < 8; c0 += D) {
+                ulonglong2 dv[D];
+                int xv[D];
+#pragma unroll
+                for (int u = 0; u < D; u++) {
+                    dv[u] = __ldcs(reinterpret_cast<const ulonglong2 *>(dl + (size_t)(jb + c0 + u) * kN));
+                    xv[u] = __ldg(xsel + jb + c0 + u);
+                }
+#pragma unroll
+                for (int u = 0; u < D; u++)
+                    diag_mac_pair<CB>(a, xl + (size_t)xv[u] * B * ct, ct, kN, nb, u2d(dv[u].x), u2d(dv[u].y), p, pinv);
+            }
+#pragma unroll
+            for (int cb = 0; cb < CB; cb++) // k_diag_mac's re-centring after every 8th term
+#pragma unroll
+                for (int e = 0; e < 4; e++) a[cb][e >> 1][e & 1] = frecenter(a[cb][e >> 1][e & 1], p, pinv);
+        }
+        for (int j = jb; j < j1; j++) { // the group's last, partial period
+            const ulonglong2 d = __ldcs(reinterpret_cast<const ulonglong2 *>(dl + (size_t)j * kN));
+            diag_mac_pair<CB>(a, xl + (size_t)xsel[j] * B * ct, ct, kN, nb, u2d(d.x), u2d(d.y), p, pinv);
+        }
+#pragma unroll
+        for (int cb = 0; cb < CB; cb++) {
+            if (cb >= nb) break;
+            u64 *o = acc + ((size_t)g * B + b0 + cb) * ct + (size_t)l * N + i;
+            const u64 q = F.q_u[l];
+            *reinterpret_cast<ulonglong2 *>(o) =
+                make_ulonglong2(fsmall_u(frecenter(a[cb][0][0], p, pinv), q), fsmall_u(frecenter(a[cb][0][1], p, pinv), q));
+            *reinterpret_cast<ulonglong2 *>(o + kN) =
+                make_ulonglong2(fsmall_u(frecenter(a[cb][1][0], p, pinv), q), fsmall_u(frecenter(a[cb][1][1], p, pinv), q));
+        }
+    }
+}
+
 cudaError_t launch_diag_flags(const u64 *vals, int R, int dim, int logn, unsigned *flags, cudaStream_t s) {
     if (R <= 0) return cudaSuccess;
     k_diag_flags<<<diag_blocks((size_t)R << logn), 256, 0, s>>>(vals, R, dim, logn, flags);
@@ -104,6 +184,24 @@ cudaError_t launch_diag_mac(const u64 *dhat, const u64 *xhat, const int *g_start
     else if (B == 2) k_diag_mac<2><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
     else if (B <= 4) k_diag_mac<4><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
     else k_diag_mac<8><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
+    return cudaGetLastError();
+}
+template <int D>
+static void diag_mac_resident_cb(unsigned grid, const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B,
+                                 int logn, const BehzConstF &f, cudaStream_t s) {
+    if (B == 1) k_diag_mac_resident<1, D><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, f);
+    else if (B == 2) k_diag_mac_resident<2, D><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, f);
+    else if (B <= 4) k_diag_mac_resident<4, D><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, f);
+    else k_diag_mac_resident<8, D><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, f);
+}
+cudaError_t launch_diag_mac_resident(const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B, int k,
+                                     int logn, int depth, const BehzConstF *f, cudaStream_t s) {
+    if (ng <= 0 || B <= 0) return cudaSuccess;
+    const unsigned grid = (unsigned)ng * (unsigned)((1 << logn) >> 9) * (unsigned)k;
+    if (depth == 2) diag_mac_resident_cb<2>(grid, dhat, xhat, g_start, xsel, acc, ng, B, logn, *f, s);
+    else if (depth == 4) diag_mac_resident_cb<4>(grid, dhat, xhat, g_start, xsel, acc, ng, B, logn, *f, s);
+    else if (depth == 8) diag_mac_resident_cb<8>(grid, dhat, xhat, g_start, xsel, acc, ng, B, logn, *f, s);
+    else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 

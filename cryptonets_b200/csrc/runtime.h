@@ -126,6 +126,9 @@ struct Context {
         if (it != budget_of.end()) budget_of[dst] = it->second; else budget_of.erase(dst);
     }
     int known_budget(const u64 *p) const { auto it = budget_of.find(p); return it == budget_of.end() ? -1 : it->second; }
+    // the diagonal product's MAC over diagonals held in NTT form: k_diag_mac_resident with 2, 4 or 8 diagonals' loads issued together,
+    // or 0 for k_diag_mac (option "diag_mac_resident"; same outputs either way)
+    int diag_mac_resident = 2;
     int chunk = 1024; // ciphertexts per kernel wave (upper bound: wave() also keeps a wave's scratch under ~8 GiB)
     int wave(size_t words_per_ct) const { // ciphertexts per wave for an operation needing `words_per_ct` scratch words per ciphertext
         const size_t fit = ((size_t)1 << 30) / (words_per_ct ? words_per_ct : 1); // 2^30 words = 8 GiB

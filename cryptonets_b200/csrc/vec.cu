@@ -103,6 +103,19 @@ extern "C" int cnhe_context_set_option(cnhe_ctx *h, const char *name, int64_t va
         c.trace_noise = value != 0;
         c.trace.clear();
         if (!c.trace_noise) c.budget_of.clear();
+    } else if (n == "release_cached_memory") {
+        // give the device memory this context keeps for reuse (parked scratch blocks, the stream-ordered pool's freed blocks) back to the
+        // driver, e.g. before preparing a large resident matrix; buffers in use are untouched
+        c.sync();
+        CNHE_CUDA(cudaStreamSynchronize(c.copy_stream));
+        c.drop_recycled();
+        CNHE_CUDA(cudaDeviceSynchronize());
+        cudaMemPool_t pool;
+        CNHE_CUDA(cudaDeviceGetDefaultMemPool(&pool, c.device));
+        CNHE_CUDA(cudaMemPoolTrimTo(pool, 0));
+    } else if (n == "diag_mac_resident") {
+        if (value != 0 && value != 2 && value != 4 && value != 8) fail("diag_mac_resident must be 0, 2, 4 or 8");
+        c.diag_mac_resident = (int)value;
     } else if (n == "chunk") {
         if (value < 1 || value > 4096) fail("chunk must be in [1,4096]");
         c.chunk = (int)value;
@@ -2430,6 +2443,11 @@ struct cnhe_diag {
     int n1 = 1, n2 = 1;
     std::vector<DiagEntry> diags;
     std::vector<BufRef> plains; // per channel: [diags][N] plaintexts, coefficient form mod t
+    // cnhe_diag_prepare_ntt: the first ntt_groups giant-step groups (ntt_diags diagonals) also held lifted into every q_l and in NTT form,
+    // per channel [ntt_diags][k][N] canonical words -- what cnhe_mat_mul_diagonal would otherwise lift and transform on every call
+    int ntt_groups = 0, ntt_diags = 0;
+    std::vector<BufRef> ntt;
+    uint64_t ntt_bytes() const { return (uint64_t)ntt.size() * ntt_diags * ctx->k * ctx->N * 8; }
 };
 // key switches of rotate_rows(steps), 0 <= steps < N/2, on a context holding the Galois elements c.galois_elts: one with the step's own
 // key, else one per hop
@@ -2465,8 +2483,10 @@ static long diag_cost(const std::vector<char> &nz, const std::vector<int> &hops,
     return cost;
 }
 
-extern "C" int cnhe_diag_prepare(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int baby_steps, cnhe_diag **out) {
-    API_BEGIN(h)
+// diagonals lifted and forward transformed per wave: their NTT forms stay under 8 GiB (the product's waves, and the prepare's)
+static int diag_wave_cap(const Context &c) { return (int)std::max<size_t>(1, ((size_t)1 << 30) / ((size_t)c.k * c.N)); }
+
+static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, int baby_steps, uint64_t max_ntt_bytes, cnhe_diag **out) {
     if (!rows || !out || n_rows < 1) fail("bad arguments");
     const size_t N = c.N;
     const int half = (int)(N / 2);
@@ -2549,8 +2569,45 @@ extern "C" int cnhe_diag_prepare(cnhe_ctx *h, const cnhe_vec *const *rows, int n
             op_encode(c, ch, dv, m, (int)N, d->plains[ch]->p + (size_t)j0 * N);
         }
     }
+    // the longest prefix of whole giant-step groups whose NTT forms, over all channels, fit in max_ntt_bytes
+    const uint64_t per_diag = (uint64_t)c.P * c.k * N * 8;
+    const uint64_t fit = max_ntt_bytes / per_diag;
+    for (int j = 0; j < nd; j++) {
+        if (j + 1 < nd && d->diags[j + 1].g == d->diags[j].g) continue; // j ends its group
+        if ((uint64_t)j + 1 > fit) break;
+        d->ntt_groups++;
+        d->ntt_diags = j + 1;
+    }
+    if (d->ntt_diags) {
+        // exactly the product's words: launch_plain_lift, then the canonical forward transform
+        const size_t kN = (size_t)c.k * N;
+        const int cap = diag_wave_cap(c);
+        d->ntt.resize(c.P);
+        for (int ch = 0; ch < c.P; ch++) {
+            c.set_channel(ch);
+            d->ntt[ch] = c.alloc((size_t)d->ntt_diags * kN);
+            for (int j0 = 0; j0 < d->ntt_diags; j0 += cap) {
+                const int m = std::min(cap, d->ntt_diags - j0);
+                u64 *L = d->ntt[ch]->p + (size_t)j0 * kN;
+                c.check(launch_plain_lift(d->plains[ch]->p + (size_t)j0 * N, L, m, (int)N, c.k, c.logN, c.d_bc, c.ch[ch].pc, c.stream), "plain_lift");
+                op_ntt(c, L, L, m * c.k, 0, c.k, false);
+            }
+        }
+    }
     c.sync();
     *out = d.release();
+}
+
+extern "C" int cnhe_diag_prepare(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int baby_steps, cnhe_diag **out) {
+    API_BEGIN(h)
+    diag_prepare(c, rows, n_rows, baby_steps, 0, out);
+    API_END
+}
+
+extern "C" int cnhe_diag_prepare_ntt(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int baby_steps, uint64_t max_ntt_bytes,
+                                     cnhe_diag **out) {
+    API_BEGIN(h)
+    diag_prepare(c, rows, n_rows, baby_steps, max_ntt_bytes, out);
     API_END
 }
 
@@ -2561,7 +2618,15 @@ extern "C" int cnhe_diag_info(const cnhe_diag *d, int *n_rows, uint64_t *dim, in
     if (n1) *n1 = d->n1;
     if (n2) *n2 = d->n2;
     if (n_diags) *n_diags = (int)d->diags.size();
-    if (device_bytes) *device_bytes = (uint64_t)d->plains.size() * d->diags.size() * d->ctx->N * 8;
+    if (device_bytes) *device_bytes = (uint64_t)d->plains.size() * d->diags.size() * d->ctx->N * 8 + d->ntt_bytes();
+    return CNHE_OK;
+}
+
+extern "C" int cnhe_diag_ntt_info(const cnhe_diag *d, int *resident_giant_steps, int *resident_diags, uint64_t *ntt_bytes) {
+    if (!d) return set_err(CNHE_ERR_INVALID, "null matrix");
+    if (resident_giant_steps) *resident_giant_steps = d->ntt_groups;
+    if (resident_diags) *resident_diags = d->ntt_diags;
+    if (ntt_bytes) *ntt_bytes = d->ntt_bytes();
     return CNHE_OK;
 }
 
@@ -2583,6 +2648,18 @@ extern "C" int cnhe_diag_export(cnhe_ctx *h, const cnhe_diag *d, int channel, in
     API_END
 }
 
+extern "C" int cnhe_diag_export_ntt(cnhe_ctx *h, const cnhe_diag *d, int channel, int index, uint64_t *dst, size_t cap_words) {
+    API_BEGIN(h)
+    if (!d || d->ctx != &c) fail("matrix belongs to another context");
+    if (channel < 0 || channel >= c.P || index < 0 || index >= d->ntt_diags) fail("index outside the resident diagonals");
+    const size_t kN = (size_t)c.k * c.N;
+    if (!dst || cap_words < kN) fail("buffer too small");
+    c.set_channel(channel);
+    CNHE_CUDA(cudaMemcpyAsync(dst, d->ntt[channel]->p + (size_t)index * kN, kN * 8, cudaMemcpyDeviceToHost, c.stream));
+    CNHE_CUDA(cudaStreamSynchronize(c.stream));
+    API_END
+}
+
 extern "C" int cnhe_diag_destroy(cnhe_diag *d) {
     if (!d) return CNHE_OK;
     try {
@@ -2595,8 +2672,10 @@ extern "C" int cnhe_diag_destroy(cnhe_diag *d) {
 
 // y = sum_g rotate_rows(n1 g)( sum_{b,h} D'[g][b,h] (.) rotate_columns^b rotate_rows(h)(v) ) for B vectors at once (one per client; their key
 // slots may differ).  Per channel: the baby-step rotations of every client in one op_rotate_rows_multi (after one column rotation per
-// client when a diagonal has b = 1), their forward transforms, then waves of giant steps -- the wave's diagonals lifted and transformed,
-// every client's inner sums in the NTT domain (k_diag_mac; dyadic products and additions off the FP64 path: the same residues), the
+// client when a diagonal has b = 1), their forward transforms, then waves of giant steps -- the wave's diagonals lifted and transformed
+// (a matrix from cnhe_diag_prepare_ntt holds those words for its resident prefix of giant steps, which then takes one wave and, unless
+// the option diag_mac_resident is 0, k_diag_mac_resident), every
+// client's inner sums in the NTT domain (k_diag_mac; dyadic products and additions off the FP64 path: the same residues), the
 // inverse transforms -- and finally the giant-step rotations of every (g, client) in one op_rotate_rows_multi and each client's sum.
 // Each inner sum equals the sum of the separate multiply_plain results, since the inverse transform is linear mod q_l.
 extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe_vec *const *vs, int B, cnhe_vec **out) {
@@ -2638,8 +2717,9 @@ extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe
         outs[b]->slot = vslot[b];
         alloc_channels(outs[b].get());
     }
-    // diagonals per wave: their lifted NTT forms stay under 8 GiB (a wave always takes at least one giant step)
-    const int cap = (int)std::max<size_t>(1, ((size_t)1 << 30) / kN);
+    // diagonals per wave: their lifted NTT forms stay under 8 GiB (a wave always takes at least one giant step); the resident groups
+    // (cnhe_diag_prepare_ntt) need no such scratch and go in one wave of their own
+    const int cap = diag_wave_cap(c), nres = d->ntt_groups;
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
         WsScope scope(c);
@@ -2667,19 +2747,33 @@ extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe
         }
         for (int gi0 = 0; gi0 < ng;) {
             WsScope wave(c);
-            int gi1 = gi0 + 1;
-            while (gi1 < ng && gstart[gi1 + 1] - gstart[gi0] <= cap) gi1++;
+            const bool resident = gi0 < nres; // then gi0 = 0, and the wave is the whole resident prefix
+            int gi1 = resident ? nres : gi0 + 1;
+            while (!resident && gi1 < ng && gstart[gi1 + 1] - gstart[gi0] <= cap) gi1++;
             const int j0 = gstart[gi0], m = gstart[gi1] - j0, gw = gi1 - gi0;
-            u64 *L = c.ws_alloc((size_t)m * kN);
-            c.check(launch_plain_lift(d->plains[ch]->p + (size_t)j0 * N, L, m, (int)N, k, c.logN, c.d_bc, c.ch[ch].pc, c.stream), "plain_lift");
-            op_ntt(c, L, L, m * k, 0, k, false);
+            u64 *L;
+            if (resident) {
+                L = d->ntt[ch]->p;
+            } else {
+                L = c.ws_alloc((size_t)m * kN);
+                c.prof_begin(5, 8.0 * m * (N + kN));
+                c.check(launch_plain_lift(d->plains[ch]->p + (size_t)j0 * N, L, m, (int)N, k, c.logN, c.d_bc, c.ch[ch].pc, c.stream), "plain_lift");
+                c.prof_end();
+                op_ntt(c, L, L, m * k, 0, k, false);
+            }
             u64 *A = acc + (size_t)gi0 * B * ctw;
             if (fp) {
                 std::vector<int> st(gw + 1);
                 for (int i = 0; i <= gw; i++) st[i] = gstart[gi0 + i] - j0;
                 int *dst = reinterpret_cast<int *>(c.ws_alloc(((size_t)gw + 2) / 2));
                 c.h2d(dst, st.data(), st.size() * sizeof(int));
-                c.check(launch_diag_mac(L, X, dst, dxsel + j0, A, gw, B, k, c.logN, &c.h_bf, c.stream), "diag_mac");
+                // HBM: the wave's diagonals once per 8 clients, the baby steps once (the giant steps share them through L2), the sums once
+                c.prof_begin(4, 8.0 * ((double)((B + 7) / 8) * m * kN + (double)nx * B * ctw + (double)gw * B * ctw));
+                if (resident && c.diag_mac_resident)
+                    c.check(launch_diag_mac_resident(L, X, dst, dxsel + j0, A, gw, B, k, c.logN, c.diag_mac_resident, &c.h_bf, c.stream),
+                            "diag_mac_resident");
+                else c.check(launch_diag_mac(L, X, dst, dxsel + j0, A, gw, B, k, c.logN, &c.h_bf, c.stream), "diag_mac");
+                c.prof_end();
             } else {
                 u64 *tmp = c.ws_alloc((size_t)B * ctw);
                 for (int gi = gi0; gi < gi1; gi++) {

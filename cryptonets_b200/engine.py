@@ -134,6 +134,19 @@ class Diag:
         check(self.eng.L.cnhe_diag_export(self.eng.h, self.h, int(channel), int(index), _p(out), out.size, bgh))
         return out, (bgh[0], bgh[1], bgh[2])
 
+    def ntt_info(self):
+        """dict(giant_steps, diags, bytes): the prefix of giant-step groups held resident in NTT form (Engine.diag_prepare's ntt_bytes), its
+        diagonals and the device bytes of their NTT forms over all channels."""
+        g, nd, nb = C.c_int(), C.c_int(), C.c_uint64()
+        check(self.eng.L.cnhe_diag_ntt_info(self.h, C.byref(g), C.byref(nd), C.byref(nb)))
+        return dict(giant_steps=g.value, diags=nd.value, bytes=nb.value)
+
+    def export_ntt(self, channel, index):
+        """[k][N] words of resident diagonal `index` of a channel: lifted into every q_l and forward transformed (canonical)."""
+        out = np.zeros((len(self.eng.q), self.eng.N), np.uint64)
+        check(self.eng.L.cnhe_diag_export_ntt(self.eng.h, self.h, int(channel), int(index), _p(out), out.size))
+        return out
+
 
 class Engine:
     """One cnhe_ctx: parameters, device tables and keys for P plaintext moduli (== EncryptedSealBfvFactory)."""
@@ -611,11 +624,19 @@ class Engine:
         check(self.L.cnhe_mat_mul_rowmajor_shard(self.h, _vec_array(rows), len(rows), v.h, int(force_dense), int(first_row), int(total_rows), C.byref(out)))
         return Vec(self, out)
 
-    def diag_prepare(self, rows, baby_steps=0):
+    def diag_prepare(self, rows, baby_steps=0, ntt_bytes=0):
         """The plain row vectors of a matrix (as mat_mul_rowmajor takes them) prepared for mat_mul_diagonal; baby_steps = 0 lets the library
-        pick n1.  The rows may be disposed afterwards."""
+        pick n1.  ntt_bytes: device memory the matrix may spend on holding the longest prefix of whole giant-step groups in NTT form, so
+        that mat_mul_diagonal skips their lift and transforms (same outputs); 0 holds none, None (or 2**64 - 1) the whole matrix.  The rows
+        may be disposed afterwards."""
         out = C.c_void_p()
-        check(self.L.cnhe_diag_prepare(self.h, _vec_array(rows), len(rows), int(baby_steps), C.byref(out)))
+        if ntt_bytes == 0:
+            check(self.L.cnhe_diag_prepare(self.h, _vec_array(rows), len(rows), int(baby_steps), C.byref(out)))
+        else:
+            budget = (1 << 64) - 1 if ntt_bytes is None else int(ntt_bytes)
+            if not 0 <= budget < 1 << 64:
+                raise ValueError("ntt_bytes must be None or in [0, 2**64)")
+            check(self.L.cnhe_diag_prepare_ntt(self.h, _vec_array(rows), len(rows), int(baby_steps), budget, C.byref(out)))
         return Diag(self, out)
 
     def mat_mul_diagonal(self, diag, vs):

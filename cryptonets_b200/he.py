@@ -179,12 +179,13 @@ class B200BfvMatrix:
             raise Exception("Internal probloem: expecting the output to be dense")
         return total
 
-    def PrepareDiagonal(self, baby_steps=0):
+    def PrepareDiagonal(self, baby_steps=0, ntt_bytes=0):
         """This plain row-major matrix prepared for the diagonal (baby-step / giant-step) product, B200BfvFactory.MulDiagonalBatch; the
-        rows stay owned by this matrix.  baby_steps = 0 picks the number of baby steps with the fewest key switches."""
+        rows stay owned by this matrix.  baby_steps = 0 picks the number of baby steps with the fewest key switches.  ntt_bytes: device
+        memory to spend on holding diagonals in NTT form (Engine.diag_prepare; 0 none, None all), same products, faster."""
         if self.Format != EMatrixFormat.RowMajor:
             raise Exception("the diagonal product expects a RowMajor matrix")
-        return B200BfvDiagonalMatrix(self.factory, self.eng.diag_prepare([r.vec for r in self.vectors], baby_steps))
+        return B200BfvDiagonalMatrix(self.factory, self.eng.diag_prepare([r.vec for r in self.vectors], baby_steps, ntt_bytes))
 
     def _check(self, m):
         if m.Format != self.Format:
@@ -252,6 +253,12 @@ class B200BfvDiagonalMatrix:
 
     def Info(self):
         return self.diag.info()
+
+    def NttInfo(self):
+        return self.diag.ntt_info()
+
+    def ExportNtt(self, channel, index):
+        return self.diag.export_ntt(channel, index)
 
     RowCount = property(lambda s: s.diag.info()["n_rows"])
     ColumnCount = property(lambda s: s.diag.info()["dim"])

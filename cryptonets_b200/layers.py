@@ -544,6 +544,10 @@ class LLDenseLayer(BaseLayer):
         # backend computes M v directly either way.
         self.Method = "rows"
         self.DiagonalMatrix = None
+        # "diagonal" only: device bytes the prepared matrix may spend on holding giant-step groups of its diagonals in NTT form, so that
+        # each product skips their lift and forward transforms (bit-identical outputs); 0 holds none, None the whole matrix.  The Raw
+        # backend ignores it.
+        self.DiagonalNttBytes = 0
         self._first_row = 0
         super().__init__(**kw)
 
@@ -561,6 +565,10 @@ class LLDenseLayer(BaseLayer):
             raise Exception("the diagonal method needs ForceDenseFormat and a dense input")
         if self.Method == "diagonal" and self.Shard is not None:
             raise Exception("the diagonal method cannot be combined with Shard")
+        if self.DiagonalNttBytes != 0 and self.Method != "diagonal":
+            raise Exception("DiagonalNttBytes needs the diagonal method")
+        if self.DiagonalNttBytes is not None and not 0 <= self.DiagonalNttBytes < 1 << 64:
+            raise Exception("DiagonalNttBytes must be None or a byte count in [0, 2**64)")
         f = self.Factory
         rows = len(self.Bias)
         w = np.asarray(self.Weights, dtype=np.float64).reshape(rows, -1)
@@ -578,7 +586,7 @@ class LLDenseLayer(BaseLayer):
             self.BiasVector = f.GetPlainVector(np.asarray(self.Bias), EVectorFormat.dense, bscale)
             self.WeightsMatrix = f.GetPlainMatrix(w, EMatrixFormat.ColumnMajor, self.WeightsScale)
         if self.Method == "diagonal" and hasattr(self.WeightsMatrix, "PrepareDiagonal"):
-            self.DiagonalMatrix = self.WeightsMatrix.PrepareDiagonal()
+            self.DiagonalMatrix = self.WeightsMatrix.PrepareDiagonal(ntt_bytes=self.DiagonalNttBytes)
             self.WeightsMatrix.Dispose()  # the diagonals replace the row plaintexts
             self.WeightsMatrix = None
         self.layerPrepared = True

@@ -179,10 +179,10 @@ def synthetic_cifar(n_images, seed=20240917):
     return np.random.default_rng(seed).integers(0, 256, (n_images, 3 * 32 * 32)).astype(np.float64)
 
 
-def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows"):
+def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", diag_ntt_bytes=0):
     """LoLa-CIFAR (`CifarCryptoNet/LolaCifarCryptoNet.cs:27-131`): 3x32x32 image as an im2col matrix [196 x 192], conv 83 maps,
     square, the second convolution as a 5488 x 16268 row-major dense layer (rotate-and-sum per row), square, dense 5488 -> 10.
-    dense_method: LLDenseLayer.Method of that layer ("rows", the reference's, or "diagonal")."""
+    dense_method: LLDenseLayer.Method of that layer ("rows", the reference's, or "diagonal"); diag_ntt_bytes: its DiagonalNttBytes."""
     w = weights or cifar_weights()
     reader = LLConvReader(images, Scale=8.0, NormalizationFactor=1.0 / 256.0, InputShape=[3, 32, 32], KernelShape=[3, 8, 8], Stride=[1000, 2, 2],
                           Upperpadding=[0, 1, 1], Lowerpadding=[0, 1, 1])
@@ -197,7 +197,8 @@ def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows"):
     # shard = (rank, world, process group): the 5488 rows of the big dense layer are split over the ranks of ONE inference (SURVEY.md 8e);
     # every rank holds the same keys and input ciphertexts, the partial products are summed through cryptonets_b200/parallel.py
     dense4 = LLDenseLayer(Source=act3, WeightsScale=512.0, Weights=ce.GetDenseWeights(w["Weights_1"]), Bias=ce.GetDenseBias(w["Biases_1"]),
-                          InputFormat=EVectorFormat.dense, ForceDenseFormat=True, Shard=shard, Method=dense_method)
+                          InputFormat=EVectorFormat.dense, ForceDenseFormat=True, Shard=shard, Method=dense_method,
+                          DiagonalNttBytes=diag_ntt_bytes)
     act5 = SquareActivation(Source=dense4)
     dense6 = LLDenseLayer(Source=act5, Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512.0, InputFormat=EVectorFormat.dense)
     return dense6, reader
@@ -219,10 +220,11 @@ def lola_large_weights(seed=9, synthetic=False):
                 Biases_1=draw(163, 0.039, 0.09), Weights_2=draw(10 * 2608, 0.42, 1.63), Biases_2=draw(10, 1.6, 3.9))
 
 
-def lola_large(factory, images, weights=None, dense_method="rows"):
+def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_bytes=0):
     """Large LoLa (`LoLaCryptonets.cs:330-409`): 28x28 image as im2col [144 x 64], conv 83 maps of 8x8 stride 2 (pixels are NOT
     normalised; the weights carry the 1/256), square, the second convolution (163 maps of 83x6x6, stride 2 over 83x12x12) as a
-    2608 x 11952 row-major dense layer with ForceDenseFormat, square, dense 2608 -> 10.  dense_method: that layer's LLDenseLayer.Method."""
+    2608 x 11952 row-major dense layer with ForceDenseFormat, square, dense 2608 -> 10.  dense_method: that layer's LLDenseLayer.Method,
+    diag_ntt_bytes its DiagonalNttBytes."""
     w = weights or lola_large_weights()
     reader = LLConvReader(images, Scale=16.0, NormalizationFactor=1.0, InputShape=[1, 28, 28], KernelShape=[1, 8, 8], Stride=[1000, 2, 2],
                           Upperpadding=[0, 1, 1], Lowerpadding=[0, 1, 1])
@@ -235,7 +237,8 @@ def lola_large(factory, images, weights=None, dense_method="rows"):
     ce.InputShape, ce.KernelShape, ce.Stride, ce.MapCount = [83, 12, 12], [83, 6, 6], [83, 2, 2], [163, 1, 1]
     ce.Padding = [False, False, False]
     dense4 = LLDenseLayer(Source=act3, WeightsScale=64, Weights=ce.GetDenseWeights(w["Weights_1"]), Bias=ce.GetDenseBias(w["Biases_1"]),
-                          InputFormat=EVectorFormat.dense, ForceDenseFormat=True, Method=dense_method)
+                          InputFormat=EVectorFormat.dense, ForceDenseFormat=True, Method=dense_method,
+                          DiagonalNttBytes=diag_ntt_bytes)
     act5 = SquareActivation(Source=dense4)
     dense6 = LLDenseLayer(Source=act5, Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512, InputFormat=EVectorFormat.dense)
     return dense6, reader

@@ -62,7 +62,10 @@ int cnhe_context_bsk_moduli(const cnhe_ctx *, uint64_t *out, int *count);
 int cnhe_context_galois_elts(const cnhe_ctx *, uint64_t *out);
 /* options: "behz_centered_mtilde" (0/1), "chunk" (ciphertexts per multiply/key-switch wave), "multi_stream" (1: one CUDA
  * stream per plaintext modulus, default; 0: everything on one stream; refused while imported batches are alive),
- * "trace_noise" (1: record the invariant noise budget after every evaluator-level operation, see cnhe_trace_read) */
+ * "trace_noise" (1: record the invariant noise budget after every evaluator-level operation, see cnhe_trace_read),
+ * "diag_mac_resident" (the MAC kernel over diagonals held in NTT form: 2, default, 4 or 8 diagonals' loads issued together, or 0 for the
+ * coefficient-form path's kernel; the outputs are identical), "release_cached_memory" (any value: hand the scratch blocks the context
+ * keeps for reuse back to the driver, e.g. before preparing a large resident matrix) */
 int cnhe_context_set_option(cnhe_ctx *, const char *name, int64_t value);
 int cnhe_context_sync(cnhe_ctx *);
 /* interop with the caller's own GPU work (the NCCL all-gather of the score ciphertexts): the CUDA stream (cudaStream_t as an integer) of a
@@ -280,11 +283,24 @@ int cnhe_mat_dot_rows_batch(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows,
  * cnhe_mat_mul_diagonal: out[b] = M vs[b] for B encrypted, dense, single-block vectors of dim M's dim and one scale; their key slots may
  *   differ, out[b] keeps vs[b]'s.  out[b] is dense of dim n_rows and scale vs.scale * row scale, and decrypts to what
  *   cnhe_mat_mul_rowmajor(rows, vs[b], force_dense = 1) decrypts to (it is a different ciphertext).  A missing Galois key is CNHE_ERR_STATE.
- *   Counted as row-rotation hops, column rotations, plain multiplications, additions and one AddMany per output. */
+ *   Counted as row-rotation hops, column rotations, plain multiplications, additions and one AddMany per output.
+ * cnhe_diag_prepare_ntt: cnhe_diag_prepare (same checks, n1 and stored diagonals), and the diagonals of the longest prefix of whole
+ *   giant-step groups whose NTT forms, summed over all channels (k N 8 bytes per diagonal and channel), fit in max_ntt_bytes are also held
+ *   resident: lifted into every q_l and forward transformed, canonical, [diag][k][N] per channel -- the words cnhe_mat_mul_diagonal
+ *   otherwise computes on every call.  UINT64_MAX holds the whole matrix, 0 none (the object then behaves as cnhe_diag_prepare's).
+ *   cnhe_mat_mul_diagonal skips the lift and the transforms of the resident groups and runs a MAC kernel built to stream them from HBM
+ *   (option "diag_mac_resident"); its outputs and counts are word for word the same.
+ *   The coefficient-form diagonals stay (cnhe_diag_export is unchanged); device_bytes of cnhe_diag_info counts both forms.
+ * cnhe_diag_ntt_info: resident giant-step groups, resident diagonals and the device bytes of their NTT forms (any pointer may be NULL).
+ * cnhe_diag_export_ntt: the k N resident words of stored diagonal `index` of a channel ([k][N]); an index outside the resident prefix,
+ *   a bad channel, cap_words < k N or another context's matrix is CNHE_ERR_INVALID. */
 typedef struct cnhe_diag cnhe_diag;
 int cnhe_diag_prepare(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, int baby_steps, cnhe_diag **out);
+int cnhe_diag_prepare_ntt(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, int baby_steps, uint64_t max_ntt_bytes, cnhe_diag **out);
 int cnhe_diag_info(const cnhe_diag *, int *n_rows, uint64_t *dim, int *n1, int *n2, int *n_diags, uint64_t *device_bytes);
+int cnhe_diag_ntt_info(const cnhe_diag *, int *resident_giant_steps, int *resident_diags, uint64_t *ntt_bytes);
 int cnhe_diag_export(cnhe_ctx *, const cnhe_diag *, int channel, int index, uint64_t *dst, size_t cap_words, int *bgh);
+int cnhe_diag_export_ntt(cnhe_ctx *, const cnhe_diag *, int channel, int index, uint64_t *dst /* k*N */, size_t cap_words);
 int cnhe_diag_destroy(cnhe_diag *);
 int cnhe_mat_mul_diagonal(cnhe_ctx *, const cnhe_diag *, const cnhe_vec *const *vs, int B, cnhe_vec **out /*B*/);
 /* Whole PoolLayer.Apply with weights ("NeuralNetworks/PoolLayer.cs:149-229"): out[m] = sum_k weights[m][k] * in[gather[m*K+k]]

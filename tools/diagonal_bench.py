@@ -1,8 +1,14 @@
-"""LoLa-Large and LoLa-CIFAR with their big ForceDenseFormat dense layer (dense4) on the row method and on the diagonal method, alternated.
+"""LoLa-Large and LoLa-CIFAR with their big ForceDenseFormat dense layer (dense4) on the row method, the diagonal method and the diagonal
+method with diagonals held in NTT form (diagonal_ntt, --ntt-bytes of them; default the whole matrix), alternated.
 
-Per network and method: device time per image (every layer synchronised), the dense4 layer's time, key switches per image from the
-operation counters (row-rotation hops + column rotations + relinearisations), and for the diagonal method the prepare time, the bytes the
-prepared matrix holds and dense4 at B = 8 inputs in one call.  Then the diagonal method at the reference's SmallModulusCount: whether the
+Per network and method: device time per image (every layer synchronised), the dense4 layer's time (after one untimed dense4
+call), key switches per image from the
+operation counters (row-rotation hops + column rotations + relinearisations), and for the diagonal methods the prepare time, the
+coefficient-form and NTT-form bytes the prepared matrix holds, dense4 at B = 8 inputs in one call and the device time of one more dense4
+call per profiler family (cnhe_prof_collect; the lift is booked as "other", the MAC as "scalar_mac_layer", whose algorithmic bytes over
+its time give dense4_mac_GBps).  diagonal_ntt@D runs the NTT-form arm with the option diag_mac_resident = D (0: k_diag_mac), so the
+MAC kernels can be alternated.  held_bytes is the prepared matrix's device_bytes (both forms), coeff_bytes / ntt_bytes its parts.  Full residency takes about
+39 GB for LoLa-CIFAR and 46 GB for LoLa-Large: run one network per process.  Then the diagonal method at the reference's SmallModulusCount: whether the
 scores decrypt, and the budget entering the last layer.  Prints one JSON line per measurement (and writes them to --out if given)."""
 import argparse
 import json
@@ -16,6 +22,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from cryptonets_b200 import networks as nw  # noqa: E402
+from cryptonets_b200._lib import CnheError  # noqa: E402
 from cryptonets_b200.he import B200BfvFactory  # noqa: E402
 from cryptonets_b200.raw import RawFactory  # noqa: E402
 
@@ -43,9 +50,23 @@ def key_switches(c):
     return c["Rotation"] + c["ColumnRotation"] + c["Relinarization"]
 
 
-def run(f, name, method, imgs, batch8):
+def mem_used_mb():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=memory.used", "--format=csv,noheader,nounits"], capture_output=True, text=True)
+        return int(q.stdout.split()[0])
+    except (OSError, ValueError, IndexError):
+        return None
+
+
+def run(f, name, method, imgs, batch8, ntt_bytes=None):
+    """method: rows, diagonal, or diagonal_ntt[@D] (D = the option diag_mac_resident: 2, 4, 8, or 0 for k_diag_mac)."""
     eng = f.engine
-    net, rd = getattr(nw, name)(f, imgs, dense_method=method)
+    diag = method != "rows"
+    base, _, depth = method.partition("@")
+    eng.set_option("diag_mac_resident", int(depth) if depth else 2)
+    eng.set_option("release_cached_memory", 1)  # the previous arm's scratch goes back to the driver before this arm's matrix
+    kw = dict(diag_ntt_bytes=ntt_bytes) if base == "diagonal_ntt" else {}
+    net, rd = getattr(nw, name)(f, imgs, dense_method="diagonal" if diag else "rows", **kw)
     layers = chain(net)
     D = 5  # reader, encrypt, pool, vectorize, square, dense4, square, dense
     for L in layers[1:]:
@@ -58,11 +79,18 @@ def run(f, name, method, imgs, batch8):
     layers[D].layerPrepared = True
     eng.sync()
     prep = time.perf_counter() - t0
-    held = layers[D].DiagonalMatrix.Info()["device_bytes"] if method == "diagonal" else None
+    held = coeff_held = ntt_held = None
+    if diag:
+        ntt_held = layers[D].DiagonalMatrix.NttInfo()["bytes"]
+        held = layers[D].DiagonalMatrix.Info()["device_bytes"]
+        coeff_held = held - ntt_held
+    mem_after_prepare = mem_used_mb()
     m = rd.GetNext()
     eng.op_counts(reset=True)
     total, dense4 = 0.0, 0.0
     for i, L in enumerate(layers[1:], 1):
+        if i == D:  # one untimed dense4 first: its scratch comes from the driver once, not inside the timed call
+            L.Apply(m).Dispose()
         eng.sync()
         t0 = time.perf_counter()
         m2 = L.Apply(m)
@@ -76,8 +104,20 @@ def run(f, name, method, imgs, batch8):
             m.Dispose()
         m = m2
     ks = key_switches(eng.op_counts())
-    rec = dict(net=name, method=method, k=len(eng.q), s_per_image=total, dense4_s=dense4, key_switches=ks, prepare_s=prep, held_bytes=held)
-    if batch8 and method == "diagonal":
+    rec = dict(net=name, method=method, k=len(eng.q), s_per_image=total, dense4_s=dense4, key_switches=ks, prepare_s=prep,
+               held_bytes=held, coeff_bytes=coeff_held, ntt_bytes=ntt_held, device_mem_used_mb_after_prepare=mem_after_prepare)
+    if diag:
+        eng.sync()
+        eng.prof_enable(True)
+        y = layers[D].Apply(x4)
+        eng.sync()
+        fam = eng.prof_collect()
+        rec["dense4_families_ms"] = {k: round(v["ms"], 3) for k, v in fam.items()}
+        mac = fam["scalar_mac_layer"]  # the diagonal MAC: its algorithmic HBM bytes over its device time
+        rec["dense4_mac_GBps"] = round(mac["bytes"] / mac["ms"] / 1e6, 1) if mac["ms"] else None
+        eng.prof_enable(False)
+        y.Dispose()
+    if batch8 and diag:
         eng.sync()
         t0 = time.perf_counter()
         outs = layers[D].ApplyBatch([x4] * 8)
@@ -94,6 +134,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--nets", default="lola_large,lola_cifar")
     ap.add_argument("--reps", type=int, default=2)
+    ap.add_argument("--skip-reference-count", action="store_true", help="skip the runs at the reference's SmallModulusCount")
+    ap.add_argument("--ntt-bytes", type=int, default=None, help="diagonal_ntt's budget in bytes (default: the whole matrix; LoLa-Large "
+                    "wholly resident ran out of memory on an 80 GB H100; 34359738368 = 32 GiB works)")
+    ap.add_argument("--methods", default="rows,diagonal,diagonal_ntt")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     recs = [dict(gpu=gpu_info())]
@@ -106,13 +150,21 @@ def main():
         want = np.asarray(raw.GetNext().Decrypt()).reshape(-1)
         f = B200BfvFactory(primes, 16384, DecompositionBitCount=60, GaloisDecompositionBitCount=60, SmallModulusCount=kref + 1, seed=5)
         for rep in range(a.reps):
-            for method in ("rows", "diagonal"):
-                rec, got = run(f, name, method, imgs, batch8=rep == 0)
+            for method in a.methods.split(","):
+                try:
+                    rec, got = run(f, name, method, imgs, batch8=True, ntt_bytes=a.ntt_bytes)
+                except CnheError as e:  # e.g. a budget the card cannot hold next to the rest of the network
+                    rec = dict(net=name, method=method, rep=rep, error=str(e), device_mem_used_mb=mem_used_mb())
+                    recs.append(rec)
+                    print(json.dumps(rec), flush=True)
+                    continue
                 rec["rep"] = rep
                 rec["scores_equal_raw"] = bool(np.allclose(got, want, rtol=1e-9, atol=1e-9))
                 recs.append(rec)
                 print(json.dumps(rec), flush=True)
         f.Dispose()
+        if a.skip_reference_count:
+            continue
         # the reference's SmallModulusCount on the diagonal method: budget entering the last layer and whether the scores decrypt
         f = B200BfvFactory(primes, 16384, DecompositionBitCount=60, GaloisDecompositionBitCount=60, SmallModulusCount=kref, seed=5)
         for method in ("rows", "diagonal"):
