@@ -94,8 +94,10 @@ __global__ void __launch_bounds__(256) k_behz_tensor(const u64 *a, const u64 *b,
 }
 
 // ---- times t, fast_floor (q u Bsk -> Bsk), fastbconv_sk (Bsk -> q)
+// EPI: the FloorEpi epilogue on every output word (A v, + B x on c0 and c1, + Delta C on c0)
+template <bool EPI>
 __global__ void __launch_bounds__(256) k_behz_floor(const u64 *__restrict__ d, u64 *__restrict__ out, int n_polys, u64 t, int logn,
-                                                   const BehzConst *__restrict__ gbc) {
+                                                   const BehzConst *__restrict__ gbc, const __grid_constant__ FloorEpi E) {
     __shared__ BehzConst bc;
     load_consts(&bc, gbc);
     const int N = 1 << logn, k = bc.k, kb = bc.kb, kt = k + kb;
@@ -134,6 +136,10 @@ __global__ void __launch_bounds__(256) k_behz_floor(const u64 *__restrict__ d, u
         if (j < na) mac128(am, tmp[j], bc.bhat_mod_msk[j]);
     const u64 alpha = mulmod(barrett128(am, msk) + (msk.p - fl[na]), bc.inv_B_mod_msk, msk);
     const bool neg = alpha > (msk.p >> 1);
+    const int part = poly % 3;
+    const u64 *xs = EPI && part < 2 ? E.x[poly / 3] + (size_t)part * k * N + x : nullptr;
+    const u64 *cs = EPI && part == 0 && E.c_poly ? E.c_poly[poly / 3] : nullptr; // Delta-scaled constant plaintext (nullptr: C at x = 0)
+    if (cs) cs += x;
     for (int i = 0; i < k; i++) {
         const DMod qi = bc.q[i];
         U128 acc = {0, 0};
@@ -143,7 +149,16 @@ __global__ void __launch_bounds__(256) k_behz_floor(const u64 *__restrict__ d, u
         u64 v = barrett128(acc, qi);
         U128 c = neg ? mul64wide(bc.B_mod_q[i], msk.p - alpha) : mul64wide(qi.p - bc.B_mod_q[i], alpha);
         add128(c, v);
-        dst[(size_t)i * N] = barrett128(c, qi);
+        v = barrett128(c, qi);
+        if (EPI) {
+            v = mulmod(v, E.a[i], qi);
+            if (part < 2) {
+                v = addmod(v, mulmod(xs[(size_t)i * N], E.b[i], qi), qi.p);
+                if (cs) v = addmod(v, cs[(size_t)i * N], qi.p);
+                else if (part == 0 && x == 0) v = addmod(v, E.c[i], qi.p);
+            }
+        }
+        dst[(size_t)i * N] = v;
     }
 }
 
@@ -211,9 +226,11 @@ cudaError_t launch_behz_lift(const u64 *const *ct_ptrs, u64 *out, int n, int log
     k_behz_lift<<<blocks_for((size_t)n * 2 << logn), 256, 0, s>>>(ct_ptrs, out, n * 2, logn, bc);
     return cudaGetLastError();
 }
-cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s) {
+cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s, const FloorEpi *epi) {
     if (n <= 0) return cudaSuccess;
-    k_behz_floor<<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, t, logn, bc);
+    const FloorEpi none{};
+    if (epi) k_behz_floor<true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, t, logn, bc, *epi);
+    else k_behz_floor<false><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, t, logn, bc, none);
     return cudaGetLastError();
 }
 cudaError_t launch_behz_tensor(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConst *bc, cudaStream_t s) {

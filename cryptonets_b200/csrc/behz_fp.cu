@@ -88,9 +88,36 @@ __global__ void __launch_bounds__(256) k_behz_tensor_fp(const u64 *a, const u64 
     }
 }
 
+// The floor kernels' epilogue (FloorEpi; EPI = true instantiations only): v is residue i (any integer |v| < 2^52) of output polynomial
+// `part` of ciphertext ct at coefficient x, xs the same coefficient of the input's polynomial `part` (part < 2), cs the same coefficient
+// of ct's Delta-scaled constant plaintext (c0 only; nullptr: the constant polynomial C).  Returns A v + B x + Delta C, |r| < 2.1 p: the
+// caller's fcanon_u makes it canonical.
+__device__ __forceinline__ double floor_epi_fp(double v, const FloorEpi &E, const u64 *xs, const u64 *cs, int part, int x, int i, int N, double p,
+                                               double pinv) {
+    double r = fmodmul(frecenter(v, p, pinv), E.a_d[i], p, pinv);
+    if (part < 2) {
+        r = __dadd_rn(r, fmodmul(u2d(xs[(size_t)i * N]), E.b_d[i], p, pinv));
+        if (cs) r = __dadd_rn(r, u2d(cs[(size_t)i * N]));
+        else if (part == 0 && x == 0) r = __dadd_rn(r, E.c_d[i]);
+    }
+    return r;
+}
+// the input words the epilogue adds to output polynomial `poly` of the launch (c0, c1 of ciphertext poly / 3), or nullptr for c2
+__device__ __forceinline__ const u64 *floor_epi_src(const FloorEpi &E, size_t poly, int x, int k, int N) {
+    const int part = (int)(poly % 3);
+    return part < 2 ? E.x[poly / 3] + (size_t)part * k * N + x : nullptr;
+}
+// the Delta-scaled constant plaintext's words at coefficient x for output polynomial `poly` (c0 of a ciphertext that has one), or nullptr
+__device__ __forceinline__ const u64 *floor_epi_cpoly(const FloorEpi &E, size_t poly, int x) {
+    if (!E.c_poly || poly % 3 != 0) return nullptr;
+    const u64 *cs = E.c_poly[poly / 3];
+    return cs ? cs + x : nullptr;
+}
+
 // canonical input (the lazy input of the product takes k_behz_floor_fold_fp)
+template <bool EPI>
 __global__ void __launch_bounds__(256) k_behz_floor_fp(const u64 *__restrict__ d, u64 *__restrict__ out, int n_polys, double t, int logn,
-                                                      const __grid_constant__ BehzConstF F) {
+                                                      const __grid_constant__ BehzConstF F, const __grid_constant__ FloorEpi E) {
     const int N = 1 << logn, k = F.k, kb = F.kb, kt = k + kb, na = kb - 1;
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= (size_t)n_polys << logn) return;
@@ -131,6 +158,7 @@ __global__ void __launch_bounds__(256) k_behz_floor_fp(const u64 *__restrict__ d
     const double alpha = fcanon(fmodmul(frecenter(__dsub_rn(am, fl_sk), pm, pminv), F.inv_B_mod_msk, pm, pminv), pm, pminv);
     // centred alpha: alpha > m_sk/2 means alpha - m_sk (negative)
     const double alpha_c = alpha > F.msk_half ? __dsub_rn(alpha, pm) : alpha;
+    const u64 *xs = EPI ? floor_epi_src(E, poly, x, k, N) : nullptr, *cs = EPI ? floor_epi_cpoly(E, poly, x) : nullptr;
 #pragma unroll
     for (int i = 0; i < KMAX; i++) {
         if (i >= k) break;
@@ -140,6 +168,7 @@ __global__ void __launch_bounds__(256) k_behz_floor_fp(const u64 *__restrict__ d
         for (int j = 0; j < KBMAX; j++)
             if (j < na) v = __dadd_rn(v, fmodmul(tmp[j], F.bhat_mod_q[i][j], p, pinv));
         v = __dsub_rn(v, fmodmul(alpha_c, F.B_mod_q[i], p, pinv));
+        if (EPI) v = floor_epi_fp(v, E, xs, cs, poly % 3, x, i, N, p, pinv);
         dst[(size_t)i * N] = fcanon_u(v, p, pinv);
     }
 }
@@ -148,9 +177,9 @@ __global__ void __launch_bounds__(256) k_behz_floor_fp(const u64 *__restrict__ d
 // -12 % time for the element-wise family.  Same outputs as k_behz_floor_fp: every folded product is the same residue class and the
 // canonical representatives are formed at the same points.  ITERS > 1 walks several coefficients per thread with the next one's
 // loads issued early -- measured 60 % slower (170 registers, one CTA per SM), so only ITERS = 1 is built.
-template <int ITERS>
+template <int ITERS, bool EPI>
 __global__ void __launch_bounds__(256) k_behz_floor_fold_fp(const u64 *__restrict__ d, u64 *__restrict__ out, size_t total, int logn,
-                                                           const __grid_constant__ FloorConstF F) {
+                                                           const __grid_constant__ FloorConstF F, const __grid_constant__ FloorEpi E) {
     const int N = 1 << logn, k = F.k, kb = F.kb, kt = k + kb, na = kb - 1;
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -200,6 +229,8 @@ __global__ void __launch_bounds__(256) k_behz_floor_fold_fp(const u64 *__restric
         const double alpha = fcanon(fmodmul(frecenter(__dsub_rn(am, fl_sk), pm, pminv), F.inv_B_mod_msk, pm, pminv), pm, pminv);
         const double alpha_c = alpha > F.msk_half ? __dsub_rn(alpha, pm) : alpha;
         u64 *dst = out + (gid >> logn) * (size_t)k * N + (gid & (size_t)(N - 1));
+        const int x = (int)(gid & (size_t)(N - 1));
+        const u64 *xs = EPI ? floor_epi_src(E, gid >> logn, x, k, N) : nullptr, *cs = EPI ? floor_epi_cpoly(E, gid >> logn, x) : nullptr;
 #pragma unroll
         for (int i = 0; i < KMAX; i++) {
             if (i >= k) break;
@@ -209,6 +240,7 @@ __global__ void __launch_bounds__(256) k_behz_floor_fold_fp(const u64 *__restric
             for (int j = 0; j < KBMAX; j++)
                 if (j < na) v = __dadd_rn(v, fmodmul(tmp[j], F.bhat_mod_q[i][j], p, pinv));
             v = __dsub_rn(v, fmodmul(alpha_c, F.B_mod_q[i], p, pinv));
+            if (EPI) v = floor_epi_fp(v, E, xs, cs, (int)((gid >> logn) % 3), x, i, N, p, pinv);
             dst[(size_t)i * N] = fcanon_u(v, p, pinv);
         }
         if (more) {
@@ -410,15 +442,19 @@ cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int
     else k_behz_tensor_fp<false><<<blocks_for(((size_t)n * kt) << logn), 256, 0, s>>>(a, b, d, n, logn, *f);
     return cudaGetLastError();
 }
-cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s) {
+cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi) {
     if (n <= 0) return cudaSuccess;
-    k_behz_floor_fp<<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f);
+    const FloorEpi none{};
+    if (epi) k_behz_floor_fp<true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f, *epi);
+    else k_behz_floor_fp<false><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f, none);
     return cudaGetLastError();
 }
-cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s) {
+cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s, const FloorEpi *epi) {
     if (n <= 0) return cudaSuccess;
     const size_t total = (size_t)n * 3 << logn;
-    k_behz_floor_fold_fp<1><<<blocks_for(total), 256, 0, s>>>(d, out3, total, logn, *f);
+    const FloorEpi none{};
+    if (epi) k_behz_floor_fold_fp<1, true><<<blocks_for(total), 256, 0, s>>>(d, out3, total, logn, *f, *epi);
+    else k_behz_floor_fold_fp<1, false><<<blocks_for(total), 256, 0, s>>>(d, out3, total, logn, *f, none);
     return cudaGetLastError();
 }
 cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,

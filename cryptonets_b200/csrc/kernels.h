@@ -131,6 +131,20 @@ struct FloorConstF {
     double bhat_mod_q[KMAX][KBMAX], bhat_mod_msk[KBMAX];
     double inv_B_mod_msk, msk_half, B_mod_q[KMAX];
 };
+// Epilogue of the BEHZ floor kernels (the quadratic activation A ct^2 + B x + C, cnhe_layer_poly2): every output polynomial times A,
+// B x added to c0 and c1, Delta C added to c0, mod q_l and canonical -- the words of multiply_plain(A) on the size-3 product, then (after
+// the key switch, which is linear) multiply_plain(x, B) and add_plain(C).  x[c]: the launch's c-th input ciphertext ([2][k][N],
+// canonical coefficient form; a device pointer table).  Per residue: A and B lifted into q_l with the upper-half increment, Delta C
+// scaled as add_plain scales it; the *_d copies centred as exact doubles for the FP64 kernels.  C is the constant polynomial (every slot)
+// unless c_poly (nullptr, or a device table of one entry per ciphertext of the launch) gives the ciphertext a plaintext of its own:
+// c_poly[c] = nullptr, or [k][N] canonical words Delta m (+ q mod t where m is in the upper half) of a plaintext m, added to c0 in
+// place of Delta C at coefficient 0 (a dense vector's last, partly filled block: C in its data slots only)
+struct FloorEpi {
+    const u64 *const *x;
+    const u64 *const *c_poly;
+    u64 a[KMAX], b[KMAX], c[KMAX];
+    double a_d[KMAX], b_d[KMAX], c_d[KMAX];
+};
 // Per plaintext modulus t.
 struct PlainConst {
     u64 t, threshold;                 // (t+1)/2
@@ -188,7 +202,8 @@ cudaError_t launch_behz_lift(const u64 *const *ct_ptrs, u64 *out, int n, int log
 // d[n][3][2k+1][N] from NTT-form a,b [n][2][2k+1][N]
 cudaError_t launch_behz_tensor(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConst *bc, cudaStream_t s);
 // d (coefficient form) -> times t, fast_floor, fastbconv_sk -> out3[n][3][k][N]
-cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s);
+// epi (host copy, every floor launcher): nullptr, or the FloorEpi applied to the outputs (its x table lists the launch's n ciphertexts)
+cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s, const FloorEpi *epi = nullptr);
 // lazy = 1: the buffers exchanged with the NTT kernels (lift output, tensor input/output, digit input, accumulator output) hold lazy
 // doubles (fparith.cuh) -- pair with NTT_IN_F / NTT_OUT_F on the transforms in between
 cudaError_t launch_behz_lift_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
@@ -201,9 +216,9 @@ cudaError_t launch_behz_square_fused(const u64 *const *ct_ptrs, const u64 *lift_
                                      cudaStream_t s);
 cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
 // canonical input; lazy input takes the folded kernel below
-cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s);
+cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr);
 // folded constants + software-pipelined loads (lazy input only)
-cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s);
+cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr);
 cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,
                              const BehzConstF *f, int lazy, cudaStream_t s);
 // ---- K6: key-switch inner product. digits [n][D][k][N] (NTT), key [D][2][k][N] (NTT) -> acc [n][2][k][N] (NTT)

@@ -926,14 +926,42 @@ static bool mul_fused(const Context &c, const std::vector<const u64 *> &a, const
 }
 // scratch words per ciphertext of multiply_chunk
 static size_t mul_words(const Context &c, bool fused) { return (size_t)(fused ? 2 * c.kb + 3 * (c.k + c.kb) : 7 * (c.k + c.kb)) * c.N; }
-static void multiply_floor(Context &c, int ch, const u64 *D, int m, bool lazy, u64 *out3) {
-    PROF(2, 8.0 * c.N * m * 3 * (2 * c.k + c.kb));
-    if (c.fp_elementwise && lazy) c.check(launch_behz_floor_fold_fp(D, out3, m, c.logN, &c.ch[ch].floor_f, c.stream), "behz_floor_fold_fp");
-    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, m, c.ch[ch].t, c.logN, &c.h_bf, c.stream), "behz_floor_fp");
-    else c.check(launch_behz_floor(D, out3, m, c.ch[ch].t, c.logN, c.d_bc, c.stream), "behz_floor");
+FloorEpi floor_epi(const Context &c, int ch, u64 A, u64 B, u64 C) {
+    FloorEpi e;
+    memset(&e, 0, sizeof(e));
+    const PlainConst &pc = c.ch[ch].pc;
+    auto cen = [](u64 v, u64 p) { return v > p / 2 ? -(double)(p - v) : (double)v; };
+    for (int i = 0; i < c.k; i++) {
+        const u64 q = c.q[i];
+        auto lift = [&](u64 v) { return v >= pc.threshold ? v + (q - pc.t) : v; }; // multiply_plain's upper-half increment
+        e.a[i] = lift(A);
+        e.b[i] = lift(B);
+        e.c[i] = hm::add(hm::mul(pc.delta[i], C, q), C >= pc.threshold ? pc.q_mod_t[i] : 0, q); // add_plain: Delta C (+ q mod t)
+        e.a_d[i] = cen(e.a[i], q);
+        e.b_d[i] = cen(e.b[i], q);
+        e.c_d[i] = cen(e.c[i], q);
+    }
+    return e;
+}
+// epi: the call's FloorEpi, its x table still to be pointed at the wave's inputs (x_ptrs) and its c_poly table (one entry per ciphertext
+// of the call) at the wave's first ciphertext c0
+static void multiply_floor(Context &c, int ch, const u64 *D, int m, bool lazy, u64 *out3, const FloorEpi *epi = nullptr,
+                           const u64 *const *x_ptrs = nullptr, int c0 = 0) {
+    FloorEpi e;
+    if (epi) {
+        e = *epi;
+        e.x = x_ptrs;
+        e.c_poly = epi->c_poly ? epi->c_poly + c0 : nullptr;
+    }
+    const FloorEpi *ep = epi ? &e : nullptr;
+    // the epilogue's read of the input's c0 and c1 (8N bytes per residue and polynomial) is booked with the family
+    PROF(2, 8.0 * c.N * m * 3 * (2 * c.k + c.kb) + (epi ? 8.0 * c.N * m * 2 * c.k : 0.0));
+    if (c.fp_elementwise && lazy) c.check(launch_behz_floor_fold_fp(D, out3, m, c.logN, &c.ch[ch].floor_f, c.stream, ep), "behz_floor_fold_fp");
+    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, m, c.ch[ch].t, c.logN, &c.h_bf, c.stream, ep), "behz_floor_fp");
+    else c.check(launch_behz_floor(D, out3, m, c.ch[ch].t, c.logN, c.d_bc, c.stream, ep), "behz_floor");
 }
 static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, int c0, int m, u64 *out3,
-                           bool fused) {
+                           bool fused, const FloorEpi *epi = nullptr) {
     const int k = c.k, kt = k + c.kb;
     const size_t N = c.N;
     if (fused) {
@@ -948,20 +976,22 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
             PROF(0, 8.0 * N * m * (2 * kt + 3 * kt));
             c.check(launch_behz_square_fused(ptrs, L, D, m, k, kt, c.logN, c.d_tabs, c.stream), "behz_square_fused");
         }
-        multiply_floor(c, ch, D, m, true, out3);
+        multiply_floor(c, ch, D, m, true, out3, epi, ptrs, c0);
         return;
     }
     bool square = true;
     for (int i = 0; i < m; i++) square = square && a[c0 + i] == b[c0 + i];
+    if (epi && !square) throw Error(-1, "the activation epilogue applies to squares only");
     std::vector<const u64 *> pa(a.begin() + c0, a.begin() + c0 + m);
     u64 *A = c.ws_alloc((size_t)m * 2 * kt * N);
     const int fpt = fp_range(c, 0, kt);
     const int lazy = c.lazy && fpt ? 1 : 0;
     const int fmt = fpt | (lazy ? NTT_IN_F | NTT_OUT_F : 0);
+    const u64 *const *pa_dev = upload_ptrs(c, pa);
     {
         PROF(2, 8.0 * N * m * 2 * (k + kt));
-        if (c.fp_elementwise) c.check(launch_behz_lift_fp(upload_ptrs(c, pa), A, m, c.logN, &c.h_bf, lazy, c.stream), "behz_lift_fp");
-        else c.check(launch_behz_lift(upload_ptrs(c, pa), A, m, c.logN, c.d_bc, c.stream), "behz_lift");
+        if (c.fp_elementwise) c.check(launch_behz_lift_fp(pa_dev, A, m, c.logN, &c.h_bf, lazy, c.stream), "behz_lift_fp");
+        else c.check(launch_behz_lift(pa_dev, A, m, c.logN, c.d_bc, c.stream), "behz_lift");
     }
     {
         PROF(0, 16.0 * N * m * 2 * kt);
@@ -985,7 +1015,7 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
         PROF(1, 16.0 * N * m * 3 * kt);
         c.check(launch_ntt_inverse(D, D, m * 3 * kt, c.logN, c.d_tabs, 0, kt, fmt, c.stream), "ntt_inverse");
     }
-    multiply_floor(c, ch, D, m, lazy, out3);
+    multiply_floor(c, ch, D, m, lazy, out3, epi, pa_dev, c0);
 }
 void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3) {
     const int n = (int)a.size();
@@ -1007,7 +1037,8 @@ void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const 
     op_key_switch(c, in3 + (size_t)2 * k * N, s3, n, keys, c.dm_relin, in3, s3, out2);
     c.note(Context::OP_RELINEARIZE, ch, n, out2);
 }
-void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2, const int *slots) {
+void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2, const int *slots,
+                       const FloorEpi *epi) {
     const int n = (int)a.size(), k = c.k;
     const KsKeys keys = relin_keys(c, ch, n, slots);
     const size_t N = c.N;
@@ -1017,7 +1048,7 @@ void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, co
         WsScope scope(c); // stream-ordered frees: the next wave reuses the memory once these kernels are done
         const int m = std::min(wave, n - c0);
         u64 *ct3 = c.ws_alloc((size_t)m * 3 * k * N);
-        multiply_chunk(c, ch, a, b, c0, m, ct3, fused);
+        multiply_chunk(c, ch, a, b, c0, m, ct3, fused, epi);
         const size_t s3 = (size_t)3 * k * N;
         op_key_switch(c, ct3 + (size_t)2 * k * N, s3, m, keys.slice(c0, m), c.dm_relin, ct3, s3, out2 + (size_t)c0 * 2 * k * N);
     }

@@ -2430,6 +2430,86 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
     }
     API_END
 }
+// The constant term of cnhe_layer_poly2 on a dense vector whose last block is only partly filled: Delta times the plaintext with C in the
+// block's data slots and 0 in its padding slots ([k][N] canonical words, as add_plain scales it), so that padding stays zero as it does
+// for the square -- rotating layers (Duplicate) add whole ciphertexts.  Returns the call's table of one entry per ciphertext (nullptr: the
+// constant polynomial C, every slot a data slot), or nullptr when no ciphertext needs one.  Workspace memory of the call.
+static const u64 *const *padded_constants(Context &c, int ch, const cnhe_vec *const *in, int n, int total, u64 C) {
+    const size_t N = c.N;
+    std::vector<const u64 *> tab(total, nullptr);
+    std::map<size_t, const u64 *> by_fill; // data slots of the last block -> its Delta-scaled plaintext
+    bool any = false;
+    for (int i = 0, first = 0; i < n; first += in[i]->blocks, i++) {
+        if (in[i]->format != CNHE_DENSE || in[i]->dim % N == 0) continue;
+        const size_t fill = in[i]->dim % N;
+        const u64 *&cp = by_fill[fill];
+        if (!cp) {
+            std::vector<u64> vals(N, 0);
+            std::fill(vals.begin(), vals.begin() + fill, C);
+            u64 *dv = c.ws_alloc(N), *plain = c.ws_alloc(N), *scaled = c.ws_alloc((size_t)c.k * N);
+            c.h2d(dv, vals.data(), N * 8);
+            op_encode(c, ch, dv, 1, (int)N, plain);
+            c.check(launch_fill_zero(scaled, (size_t)c.k * N, c.stream), "fill_zero");
+            c.check(launch_ct_add_plain(scaled, scaled, 1, 1, plain, N, (int)N, c.k, c.logN, c.d_bc, c.ch[ch].pc, 0, c.stream), "ct_add_plain");
+            cp = scaled;
+        }
+        tab[first + in[i]->blocks - 1] = cp;
+        any = true;
+    }
+    return any ? upload_ptrs(c, tab) : nullptr;
+}
+// The quadratic activation a x^2 + b x + c over a whole matrix, in cnhe_layer_square's passes: the BEHZ floor kernel scales the size-3
+// product by A and adds B x and Delta C (FloorEpi), so out[i] = relinearize(A (.) in[i]^2) + B (.) in[i] + C word for word
+extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc,
+                                cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n < 1) fail("empty layer");
+    if (!a) fail("the quadratic coefficient is required");
+    for (const cnhe_vec *p : {a, b, cc}) {
+        if (!p) continue;
+        same_ctx(c, p);
+        if (p->enc) fail("the coefficients must be plain");
+        if (p->format != CNHE_SPARSE || p->dim != 1) fail("each coefficient must be a sparse vector of dimension 1");
+    }
+    std::vector<int> first(n + 1, 0);
+    for (int i = 0; i < n; i++) {
+        same_ctx(c, in[i]);
+        if (!in[i]->enc) fail("the inputs must be encrypted");
+        if (in[i]->scale != in[0]->scale) fail("Scales do not match.");
+        first[i + 1] = first[i] + in[i]->blocks;
+    }
+    const double s = in[0]->scale, out_scale = a->scale * s * s;
+    if (b && b->scale * s != out_scale) fail("Scales do not match.");
+    if (cc && cc->scale != out_scale) fail("Scales do not match.");
+    const int total = first[n];
+    const std::vector<int> vslot = vec_slots(c, in, n);
+    std::vector<int> ct_slot;
+    for (int i = 0; i < n; i++) ct_slot.insert(ct_slot.end(), in[i]->blocks, vslot[i]);
+    std::vector<BufRef> big(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        const u64 A = a->scalars[ch][0], B = b ? b->scalars[ch][0] : 0, C = cc ? cc->scalars[ch][0] : 0;
+        FloorEpi epi = floor_epi(c, ch, A, B, C);
+        if (C) epi.c_poly = padded_constants(c, ch, in, n, total, C);
+        big[ch] = c.alloc((size_t)total * c.ct_words());
+        std::vector<const u64 *> ptrs;
+        for (int i = 0; i < n; i++)
+            for (int bl = 0; bl < in[i]->blocks; bl++) ptrs.push_back(in[i]->block(ch, bl));
+        op_multiply_relin(c, ch, ptrs, ptrs, big[ch]->p, ct_slot.data(), &epi);
+        // the operations of the composition (a term that is 0 mod t is skipped in that channel)
+        if (A) c.op_count[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+        if (B) {
+            c.op_count[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+            c.op_count[Context::OP_ADD] += (uint64_t)total;
+        }
+        if (C) c.op_count[Context::OP_ADD_PLAIN] += (uint64_t)total;
+    }
+    for (int i = 0; i < n; i++) {
+        out[i] = slab_view(new_vec(c, in[i]->dim, out_scale, in[i]->format, true, in[i]->blocks), big, first[i]);
+        out[i]->slot = vslot[i];
+    }
+    API_END
+}
 
 // ---------------------------------------------------------------------------------------------------- diagonal matrix-vector product
 // A plain matrix prepared for the diagonal (Halevi-Shoup) product with baby-step / giant-step (DESIGN.md section 4.10, slot layout in

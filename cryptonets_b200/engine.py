@@ -676,6 +676,15 @@ class Engine:
         check(self.L.cnhe_layer_square(self.h, _vec_array(inputs), n, out))
         return self._wrap_many(out, n, like=inputs)
 
+    def layer_poly2(self, inputs, a, b=None, c=None):
+        """a x^2 + b x + c of every input in layer_square's passes (include/cnhe.h, cnhe_layer_poly2): a, b, c are plain sparse vectors of
+        dimension 1 at scales W, W s and W s^2 (b, c may be None); the outputs have scale W s^2."""
+        n = len(inputs)
+        out = (VECP * n)()
+        h = lambda v: None if v is None else v.h
+        check(self.L.cnhe_layer_poly2(self.h, _vec_array(inputs), n, h(a), h(b), h(c), out))
+        return self._wrap_many(out, n, like=inputs)
+
     # ---- raw device arrays (micro-benchmarks, kernel parity tests)
     def dev_alloc(self, words):
         p = C.c_uint64()

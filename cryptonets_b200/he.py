@@ -208,6 +208,12 @@ class B200BfvMatrix:
         out = [a.PointwiseMultiply(b, env) for a, b in zip(self.vectors, m.vectors)]
         return B200BfvMatrix(self.factory, out, self.Format, CopyVectors=False)
 
+    def PolyActivation(self, a, b=None, c=None, env=None):
+        """a x^2 + b x + c of every column in one wave (cnhe_layer_poly2): a, b, c plain sparse vectors of dimension 1 at scales W, W s and
+        W s^2 (b, c may be None); the result has scale W s^2."""
+        out = self.eng.layer_poly2([v.vec for v in self.vectors], a.vec, None if b is None else b.vec, None if c is None else c.vec)
+        return B200BfvMatrix(self.factory, [B200BfvVector(self.factory, o) for o in out], self.Format, CopyVectors=False)
+
     def GetColumn(self, i):
         if i >= len(self.vectors):
             raise Exception("Column does not exist")
@@ -376,6 +382,17 @@ class B200BfvFactory:
         """SquareActivation of several matrices (possibly of different clients) in one relinearisation wave."""
         vecs = [v.vec for m in matrices for v in m.vectors]
         out, i, res = self.engine.layer_square(vecs), 0, []
+        for m in matrices:
+            n = len(m.vectors)
+            res.append(B200BfvMatrix(self, [B200BfvVector(self, o) for o in out[i:i + n]], m.Format, CopyVectors=False))
+            i += n
+        return res
+
+    def PolyActivationBatch(self, matrices, a, b=None, c=None):
+        """m.PolyActivation(a, b, c) of several matrices (possibly of different clients) in one relinearisation wave."""
+        vecs = [v.vec for m in matrices for v in m.vectors]
+        out = self.engine.layer_poly2(vecs, a.vec, None if b is None else b.vec, None if c is None else c.vec)
+        i, res = 0, []
         for m in matrices:
             n = len(m.vectors)
             res.append(B200BfvMatrix(self, [B200BfvVector(self, o) for o in out[i:i + n]], m.Format, CopyVectors=False))

@@ -294,6 +294,50 @@ class SquareActivation(BaseLayer):
         return s * s
 
 
+class PolyActivation(BaseLayer):
+    """Quadratic activation a x^2 + b x + c (a learned polynomial such as a fitted ReLU or Swish) on every element.  Coefficients = (a, b,
+    c), CoefficientScale = W: the integer coefficients are A = round(a W), B = round(b W s), C = round(c W s^2) for the input scale s,
+    and the output scale is W s^2.  On a B200BfvFactory the whole layer is one call (cnhe_layer_poly2) with the square's passes; a
+    coefficient that rounds to 0 is left out.  Slots: a dense vector's padding slots (beyond its dimension) stay zero, as they do for
+    SquareActivation, so that rotating layers such as LLDuplicateLayer see only the data; each ciphertext of a sparse vector gets C in all
+    of its slots (there the slots are separate images, which no layer mixes)."""
+
+    def __init__(self, **kw):
+        self.Coefficients = (1.0, 0.0, 0.0)
+        self.CoefficientScale = 1.0
+        self.coefficientVectors = None
+        super().__init__(**kw)
+
+    def Prepare(self):
+        a, b, c = (float(x) for x in self.Coefficients)
+        W, s = self.CoefficientScale, self.Source.GetOutputScale()
+        f = self.Factory
+
+        def vec(v, scale):
+            return None if np.rint(v * scale) == 0 else f.GetPlainVector([v], EVectorFormat.sparse, scale)
+
+        self.coefficientVectors = (f.GetPlainVector([a], EVectorFormat.sparse, W), vec(b, W * s), vec(c, W * s * s))
+
+    def Apply(self, m):
+        return m.PolyActivation(*self.coefficientVectors, env=self.Factory.AllocateComputationEnv())
+
+    def ApplyBatch(self, ms):
+        batch = getattr(self.Factory, "PolyActivationBatch", None)
+        if batch is None or len(ms) < 2:
+            return super().ApplyBatch(ms)
+        return batch(ms, *self.coefficientVectors)
+
+    def GetOutputScale(self):
+        s = self.Source.GetOutputScale()
+        return self.CoefficientScale * s * s
+
+    def Dispose(self):
+        for v in self.coefficientVectors or ():
+            if v is not None and hasattr(v, "Dispose"):
+                v.Dispose()
+        self.coefficientVectors = None
+
+
 class _ConvLayerBase(BaseLayer):
     def __init__(self, **kw):
         self.ce = ConvolutionEngine()

@@ -177,6 +177,20 @@ class RawMatrix:
         r.Scale = self.Scale * m.Scale
         return r
 
+    def PolyActivation(self, a, b=None, c=None, env=None):
+        """A x^2 + B x + C on every scaled integer: a, b, c are sparse vectors of dimension 1 at scales W, W s, W s^2 (b, c may be None),
+        checked exactly as cnhe_layer_poly2 checks them."""
+        out_scale = a.Scale * self.Scale * self.Scale
+        if (b is not None and b.Scale * self.Scale != out_scale) or (c is not None and c.Scale != out_scale):
+            raise Exception("Scales do not match.")
+        r = RawMatrix(a.v[0] * self.m * self.m, 1, self.Format, self.BlockSize)
+        if b is not None:
+            r.m = r.m + b.v[0] * self.m
+        if c is not None:
+            r.m = r.m + c.v[0]
+        r.Scale = out_scale
+        return r
+
     def Add(self, m, env=None):
         self._check(m)
         if m.Scale != self.Scale:

@@ -312,6 +312,16 @@ int cnhe_layer_conv_dense(cnhe_ctx *, const cnhe_vec *const *in, int n_in, const
 /* SquareActivation.Apply over a whole matrix ("NeuralNetworks/SquareActivation.cs:10-13"): out[i] = in[i] (.) in[i].  The vectors may
  * belong to different key slots (several clients' layers in one call): each is relinearised under its own slot's keys. */
 int cnhe_layer_square(cnhe_ctx *, const cnhe_vec *const *in, int n, cnhe_vec **out /*n*/);
+/* Quadratic activation a x^2 + b x + c over a whole matrix, in the passes of cnhe_layer_square: out[i] is, word for word,
+ *   relinearize(multiply_plain(in[i] (.) in[i], a)) + multiply_plain(in[i], b) + c      (scale scale(a) s^2, s = scale of the inputs)
+ * with the terms applied inside the product's BEHZ floor kernel.  a, b, c are plain SPARSE vectors of dimension 1 (cnhe_vec_plain);
+ * b and c may be NULL.  A term that is 0 mod a plaintext prime contributes nothing in that channel.  Slots: C is added to the data slots of
+ * a dense vector only -- the last block of a vector whose dimension is not a multiple of N gets add_plain of the plaintext with C in its
+ * data slots and 0 in its padding slots, so padding stays zero as it does for cnhe_layer_square (rotations and cnhe_vec_duplicate add
+ * whole ciphertexts); every other ciphertext, and every ciphertext of a sparse vector, gets the constant plaintext C (all N slots).  (a, b, c) = (1, NULL, NULL) gives
+ * cnhe_layer_square's words.  The inputs must share one scale, and scale(b) s and scale(c) must equal scale(a) s^2 exactly; the vectors
+ * may belong to different key slots, as for cnhe_layer_square.  Operation counts are those of the composition. */
+int cnhe_layer_poly2(cnhe_ctx *, const cnhe_vec *const *in, int n, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *c, cnhe_vec **out /*n*/);
 
 /* ---- micro-benchmark / kernel-level entry points on caller-owned device memory ("raw") --------------------------- */
 int cnhe_dev_alloc(cnhe_ctx *, size_t words, uint64_t *dptr);

@@ -108,6 +108,7 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_diagonal(IntPtr a0, IntPtr diag, IntPtr[] vs, int B, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_conv_dense(IntPtr a0, IntPtr[] @in, int n_in, int[] gather, IntPtr[] weights, IntPtr[] bias, int M, int K, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_square(IntPtr a0, IntPtr[] @in, int n, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_poly2(IntPtr a0, IntPtr[] @in, int n, IntPtr a, IntPtr b, IntPtr c, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_alloc(IntPtr a0, UIntPtr words, out ulong dptr);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_free(IntPtr a0, ulong dptr);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_upload(IntPtr a0, ulong dptr, IntPtr src, UIntPtr words);
@@ -306,6 +307,15 @@ namespace HEWrapper
         }
         public IMatrix Add(IMatrix m, IComputationEnvironment env) => Zip(m, (a, b) => a.Add(b, env));                               // :123-137
         public IMatrix ElementWiseMultiply(IMatrix m, IComputationEnvironment env) => Zip(m, (a, b) => a.PointwiseMultiply(b, env)); // :140-154
+        /// a x^2 + b x + c of every column in one wave (cnhe_layer_poly2): a, b, c plain sparse vectors of dimension 1 at scales W, W s, W s^2
+        /// (b, c may be null); the result has scale W s^2
+        public IMatrix PolyActivation(IVector a, IVector b, IVector c)
+        {
+            var outs = new IntPtr[Vectors.Length];
+            Cnhe.Check(Cnhe.cnhe_layer_poly2(Ctx, Cnhe.Handles(Vectors), Vectors.Length, ((B200BfvVector)a).Handle,
+                                             b == null ? IntPtr.Zero : ((B200BfvVector)b).Handle, c == null ? IntPtr.Zero : ((B200BfvVector)c).Handle, outs));
+            return new B200BfvMatrix(Factory, outs.Select(h => (IVector)new B200BfvVector(Factory, h)).ToArray(), Format, false) { DataDisposedExternaly = false };
+        }
         public IVector GetColumn(int columnNumber)
         {
             if (Format != EMatrixFormat.ColumnMajor) throw new Exception("GetColumn is available only for ColumnMajor matrices");
