@@ -95,7 +95,9 @@ __global__ void __launch_bounds__(256) k_behz_tensor(const u64 *a, const u64 *b,
 
 // ---- times t, fast_floor (q u Bsk -> Bsk), fastbconv_sk (Bsk -> q)
 // EPI: the FloorEpi epilogue on every output word (A v, + B x on c0 and c1, + Delta C on c0)
-template <bool EPI>
+// PAIR (with EPI): output ciphertext c is the floor of product 2c minus the floor of product 2c + 1, then the epilogue.  The thread
+// floors product 2c + 1 first and parks its words in its own output words, which it reads back after flooring product 2c
+template <bool EPI, bool PAIR = false>
 __global__ void __launch_bounds__(256) k_behz_floor(const u64 *__restrict__ d, u64 *__restrict__ out, int n_polys, u64 t, int logn,
                                                    const BehzConst *__restrict__ gbc, const __grid_constant__ FloorEpi E) {
     __shared__ BehzConst bc;
@@ -104,61 +106,73 @@ __global__ void __launch_bounds__(256) k_behz_floor(const u64 *__restrict__ d, u
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= (size_t)n_polys << logn) return;
     const int x = (int)(gid & (N - 1)), poly = (int)(gid >> logn);
-    const u64 *src = d + (size_t)poly * kt * N + x;
     u64 *dst = out + (size_t)poly * k * N + x;
     const int na = kb - 1; // auxiliary primes (the base B); bsk[na] is m_sk
-    u64 tmp[KBMAX], fl[KBMAX];
+#pragma unroll 1
+    for (int h = 0; h < (PAIR ? 2 : 1); h++) {
+        // the product polynomial read: the output's own, or (PAIR) polynomial poly % 3 of product 2 (poly / 3) + 1 - h
+        const u64 *src = d + (size_t)(PAIR ? (poly / 3 * 2 + 1 - h) * 3 + poly % 3 : poly) * kt * N + x;
+        u64 tmp[KBMAX], fl[KBMAX];
 #pragma unroll
-    for (int i = 0; i < KMAX; i++)
-        if (i < k) {
-            u64 v = mulmod(src[(size_t)i * N], t, bc.q[i]); // t < q_i is enforced at context creation
-            tmp[i] = mulmod(v, bc.inv_qhat_mod_q[i], bc.q[i]);
-        }
-#pragma unroll
-    for (int j = 0; j < KBMAX; j++)
-        if (j < kb) {
-            const DMod bj = bc.bsk[j];
-            U128 acc = {0, 0};
-#pragma unroll
-            for (int i = 0; i < KMAX; i++)
-                if (i < k) mac128(acc, tmp[i], bc.qhat_mod_bsk[j][i]);
-            u64 conv = barrett128(acc, bj);
-            u64 xb = mulmod(src[(size_t)(k + j) * N], t, bj);
-            fl[j] = mulmod(xb + (bj.p - conv), bc.inv_q_mod_bsk[j], bj);
-        }
-    const DMod msk = bc.bsk[na];
-#pragma unroll
-    for (int j = 0; j < KBMAX; j++)
-        if (j < na) tmp[j] = mulmod(fl[j], bc.inv_bhat_mod_b[j], bc.bsk[j]);
-    U128 am = {0, 0};
-#pragma unroll
-    for (int j = 0; j < KBMAX; j++)
-        if (j < na) mac128(am, tmp[j], bc.bhat_mod_msk[j]);
-    const u64 alpha = mulmod(barrett128(am, msk) + (msk.p - fl[na]), bc.inv_B_mod_msk, msk);
-    const bool neg = alpha > (msk.p >> 1);
-    const int part = poly % 3;
-    const u64 *xs = EPI && part < 2 ? E.x[poly / 3] + (size_t)part * k * N + x : nullptr;
-    const u64 *cs = EPI && part == 0 && E.c_poly ? E.c_poly[poly / 3] : nullptr; // Delta-scaled constant plaintext (nullptr: C at x = 0)
-    if (cs) cs += x;
-    for (int i = 0; i < k; i++) {
-        const DMod qi = bc.q[i];
-        U128 acc = {0, 0};
+        for (int i = 0; i < KMAX; i++)
+            if (i < k) {
+                u64 v = mulmod(src[(size_t)i * N], t, bc.q[i]); // t < q_i is enforced at context creation
+                tmp[i] = mulmod(v, bc.inv_qhat_mod_q[i], bc.q[i]);
+            }
 #pragma unroll
         for (int j = 0; j < KBMAX; j++)
-            if (j < na) mac128(acc, tmp[j], bc.bhat_mod_q[i][j]);
-        u64 v = barrett128(acc, qi);
-        U128 c = neg ? mul64wide(bc.B_mod_q[i], msk.p - alpha) : mul64wide(qi.p - bc.B_mod_q[i], alpha);
-        add128(c, v);
-        v = barrett128(c, qi);
-        if (EPI) {
-            v = mulmod(v, E.a[i], qi);
-            if (part < 2) {
-                v = addmod(v, mulmod(xs[(size_t)i * N], E.b[i], qi), qi.p);
-                if (cs) v = addmod(v, cs[(size_t)i * N], qi.p);
-                else if (part == 0 && x == 0) v = addmod(v, E.c[i], qi.p);
+            if (j < kb) {
+                const DMod bj = bc.bsk[j];
+                U128 acc = {0, 0};
+#pragma unroll
+                for (int i = 0; i < KMAX; i++)
+                    if (i < k) mac128(acc, tmp[i], bc.qhat_mod_bsk[j][i]);
+                u64 conv = barrett128(acc, bj);
+                u64 xb = mulmod(src[(size_t)(k + j) * N], t, bj);
+                fl[j] = mulmod(xb + (bj.p - conv), bc.inv_q_mod_bsk[j], bj);
             }
+        const DMod msk = bc.bsk[na];
+#pragma unroll
+        for (int j = 0; j < KBMAX; j++)
+            if (j < na) tmp[j] = mulmod(fl[j], bc.inv_bhat_mod_b[j], bc.bsk[j]);
+        U128 am = {0, 0};
+#pragma unroll
+        for (int j = 0; j < KBMAX; j++)
+            if (j < na) mac128(am, tmp[j], bc.bhat_mod_msk[j]);
+        const u64 alpha = mulmod(barrett128(am, msk) + (msk.p - fl[na]), bc.inv_B_mod_msk, msk);
+        const bool neg = alpha > (msk.p >> 1);
+        const int part = poly % 3;
+        const u64 *xs = EPI && part < 2 ? E.x[poly / 3] + (size_t)part * k * N + x : nullptr;
+        const u64 *cs = EPI && part == 0 && E.c_poly ? E.c_poly[poly / 3] : nullptr; // Delta-scaled constant plaintext (nullptr: C at x = 0)
+        if (cs) cs += x;
+        for (int i = 0; i < k; i++) {
+            const DMod qi = bc.q[i];
+            U128 acc = {0, 0};
+#pragma unroll
+            for (int j = 0; j < KBMAX; j++)
+                if (j < na) mac128(acc, tmp[j], bc.bhat_mod_q[i][j]);
+            u64 v = barrett128(acc, qi);
+            U128 c = neg ? mul64wide(bc.B_mod_q[i], msk.p - alpha) : mul64wide(qi.p - bc.B_mod_q[i], alpha);
+            add128(c, v);
+            v = barrett128(c, qi);
+            if (PAIR && h == 0) {
+                dst[(size_t)i * N] = v;
+                continue;
+            }
+            if (PAIR) {
+                const u64 w = dst[(size_t)i * N];
+                v = v >= w ? v - w : v + (qi.p - w);
+            }
+            if (EPI) {
+                v = mulmod(v, E.a[i], qi);
+                if (part < 2) {
+                    v = addmod(v, mulmod(xs[(size_t)i * N], E.b[i], qi), qi.p);
+                    if (cs) v = addmod(v, cs[(size_t)i * N], qi.p);
+                    else if (part == 0 && x == 0) v = addmod(v, E.c[i], qi.p);
+                }
+            }
+            dst[(size_t)i * N] = v;
         }
-        dst[(size_t)i * N] = v;
     }
 }
 
@@ -226,10 +240,13 @@ cudaError_t launch_behz_lift(const u64 *const *ct_ptrs, u64 *out, int n, int log
     k_behz_lift<<<blocks_for((size_t)n * 2 << logn), 256, 0, s>>>(ct_ptrs, out, n * 2, logn, bc);
     return cudaGetLastError();
 }
-cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s, const FloorEpi *epi) {
+cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s, const FloorEpi *epi,
+                              bool pair) {
     if (n <= 0) return cudaSuccess;
+    if (pair && !epi) return cudaErrorInvalidValue;
     const FloorEpi none{};
-    if (epi) k_behz_floor<true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, t, logn, bc, *epi);
+    if (pair) k_behz_floor<true, true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, t, logn, bc, *epi);
+    else if (epi) k_behz_floor<true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, t, logn, bc, *epi);
     else k_behz_floor<false><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, t, logn, bc, none);
     return cudaGetLastError();
 }

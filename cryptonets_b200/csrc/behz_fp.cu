@@ -114,123 +114,58 @@ __device__ __forceinline__ const u64 *floor_epi_cpoly(const FloorEpi &E, size_t 
     return cs ? cs + x : nullptr;
 }
 
+// the product polynomial a floor thread reads for output polynomial `poly`: itself, or (PAIR) polynomial poly % 3 of product 2 (poly / 3) + sel
+__device__ __forceinline__ size_t floor_src_poly(size_t poly, bool pair, int sel) { return pair ? (poly / 3 * 2 + sel) * 3 + poly % 3 : poly; }
+
 // canonical input (the lazy input of the product takes k_behz_floor_fold_fp)
-template <bool EPI>
+// PAIR (with EPI): output ciphertext c is the floor of product 2c minus the floor of product 2c + 1, then the epilogue (FloorEpi).  The
+// thread floors product 2c + 1 first and parks its canonical words in its own output words, which it reads back after flooring product 2c
+template <bool EPI, bool PAIR = false>
 __global__ void __launch_bounds__(256) k_behz_floor_fp(const u64 *__restrict__ d, u64 *__restrict__ out, int n_polys, double t, int logn,
                                                       const __grid_constant__ BehzConstF F, const __grid_constant__ FloorEpi E) {
     const int N = 1 << logn, k = F.k, kb = F.kb, kt = k + kb, na = kb - 1;
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= (size_t)n_polys << logn) return;
     const int x = (int)(gid & (N - 1)), poly = (int)(gid >> logn);
-    const u64 *src = d + (size_t)poly * kt * N + x;
     u64 *dst = out + (size_t)poly * k * N + x;
-    double tmp[KBMAX], fl[KBMAX];
-#pragma unroll
-    for (int i = 0; i < KMAX; i++)
-        if (i < k) {
-            const double p = F.qd[i], pinv = F.qinv[i];
-            const double v = fmodmul(u2d(src[(size_t)i * N]), t, p, pinv);
-            tmp[i] = fcanon(fmodmul(v, F.inv_qhat_mod_q[i], p, pinv), p, pinv);
-        }
-#pragma unroll
-    for (int j = 0; j < KBMAX; j++)
-        if (j < kb) {
-            const double p = F.bd[j], pinv = F.binv[j];
-            double conv = 0.0;
-#pragma unroll
-            for (int i = 0; i < KMAX; i++)
-                if (i < k) conv = __dadd_rn(conv, fmodmul(tmp[i], F.qhat_mod_bsk[j][i], p, pinv));
-            const double xb = fmodmul(u2d(src[(size_t)(k + j) * N]), t, p, pinv);
-            fl[j] = fmodmul(frecenter(__dsub_rn(xb, conv), p, pinv), F.inv_q_mod_bsk[j], p, pinv);
-        }
-    const double pm = F.bd[na], pminv = F.binv[na];
-    double am = 0.0;
-#pragma unroll
-    for (int j = 0; j < KBMAX; j++)
-        if (j < na) {
-            tmp[j] = fcanon(fmodmul(fl[j], F.inv_bhat_mod_b[j], F.bd[j], F.binv[j]), F.bd[j], F.binv[j]);
-            am = __dadd_rn(am, fmodmul(tmp[j], F.bhat_mod_msk[j], pm, pminv));
-        }
-    double fl_sk = 0.0; // fl[na] without a runtime-indexed (local-memory) array access
-#pragma unroll
-    for (int j = 0; j < KBMAX; j++)
-        if (j == na) fl_sk = fl[j];
-    const double alpha = fcanon(fmodmul(frecenter(__dsub_rn(am, fl_sk), pm, pminv), F.inv_B_mod_msk, pm, pminv), pm, pminv);
-    // centred alpha: alpha > m_sk/2 means alpha - m_sk (negative)
-    const double alpha_c = alpha > F.msk_half ? __dsub_rn(alpha, pm) : alpha;
-    const u64 *xs = EPI ? floor_epi_src(E, poly, x, k, N) : nullptr, *cs = EPI ? floor_epi_cpoly(E, poly, x) : nullptr;
-#pragma unroll
-    for (int i = 0; i < KMAX; i++) {
-        if (i >= k) break;
-        const double p = F.qd[i], pinv = F.qinv[i];
-        double v = 0.0;
-#pragma unroll
-        for (int j = 0; j < KBMAX; j++)
-            if (j < na) v = __dadd_rn(v, fmodmul(tmp[j], F.bhat_mod_q[i][j], p, pinv));
-        v = __dsub_rn(v, fmodmul(alpha_c, F.B_mod_q[i], p, pinv));
-        if (EPI) v = floor_epi_fp(v, E, xs, cs, poly % 3, x, i, N, p, pinv);
-        dst[(size_t)i * N] = fcanon_u(v, p, pinv);
-    }
-}
-
-// fast_floor + fastbconv_sk with the constant factors folded into the conversion matrices (FloorConstF): -19 % FP64 instructions,
-// -12 % time for the element-wise family.  Same outputs as k_behz_floor_fp: every folded product is the same residue class and the
-// canonical representatives are formed at the same points.  ITERS > 1 walks several coefficients per thread with the next one's
-// loads issued early -- measured 60 % slower (170 registers, one CTA per SM), so only ITERS = 1 is built.
-template <int ITERS, bool EPI>
-__global__ void __launch_bounds__(256) k_behz_floor_fold_fp(const u64 *__restrict__ d, u64 *__restrict__ out, size_t total, int logn,
-                                                           const __grid_constant__ FloorConstF F, const __grid_constant__ FloorEpi E) {
-    const int N = 1 << logn, k = F.k, kb = F.kb, kt = k + kb, na = kb - 1;
-    const size_t stride = (size_t)gridDim.x * blockDim.x;
-    size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    double cq[KMAX], cb[KBMAX], nq[KMAX], nb[KBMAX]; // current / next coefficient: residues mod q_i and mod the Bsk primes
-    auto load = [&](double (&vq)[KMAX], double (&vb)[KBMAX], size_t g) {
-        const u64 *src = d + (g >> logn) * (size_t)kt * N + (g & (size_t)(N - 1));
-#pragma unroll
-        for (int i = 0; i < KMAX; i++)
-            if (i < k) vq[i] = ld_lazy(src + (size_t)i * N);
-        src += (size_t)k * N;
-#pragma unroll
-        for (int j = 0; j < KBMAX; j++)
-            if (j < kb) vb[j] = ld_lazy(src + (size_t)j * N);
-    };
-    if (gid < total) load(cq, cb, gid);
 #pragma unroll 1
-    for (int it = 0; it < ITERS; it++, gid += stride) {
-        if (gid >= total) return;
-        const bool more = ITERS > 1 && it + 1 < ITERS && gid + stride < total;
-        if (more) load(nq, nb, gid + stride);
-        double tmp[KBMAX];
-        // [x t q-hat_i^-1]_{q_i}, canonical representative (the base conversion sums these integers)
+    for (int h = 0; h < (PAIR ? 2 : 1); h++) {
+        const u64 *src = d + floor_src_poly(poly, PAIR, 1 - h) * kt * N + x;
+        double tmp[KBMAX], fl[KBMAX];
 #pragma unroll
         for (int i = 0; i < KMAX; i++)
-            if (i < k) tmp[i] = fcanon(fmodmul(cq[i], F.xq[i], F.qd[i], F.qinv[i]), F.qd[i], F.qinv[i]);
-        double fl[KBMAX];
+            if (i < k) {
+                const double p = F.qd[i], pinv = F.qinv[i];
+                const double v = fmodmul(u2d(src[(size_t)i * N]), t, p, pinv);
+                tmp[i] = fcanon(fmodmul(v, F.inv_qhat_mod_q[i], p, pinv), p, pinv);
+            }
 #pragma unroll
         for (int j = 0; j < KBMAX; j++)
             if (j < kb) {
                 const double p = F.bd[j], pinv = F.binv[j];
-                double acc = fmodmul(cb[j], F.xb[j], p, pinv);
+                double conv = 0.0;
 #pragma unroll
                 for (int i = 0; i < KMAX; i++)
-                    if (i < k) acc = __dsub_rn(acc, fmodmul(tmp[i], F.conv[j][i], p, pinv));
-                fl[j] = acc; // j < na: floor_j * B-hat_j^-1 mod p_j;  j = na: floor mod m_sk   (|acc| <= (k+1) * 0.51 p)
+                    if (i < k) conv = __dadd_rn(conv, fmodmul(tmp[i], F.qhat_mod_bsk[j][i], p, pinv));
+                const double xb = fmodmul(u2d(src[(size_t)(k + j) * N]), t, p, pinv);
+                fl[j] = fmodmul(frecenter(__dsub_rn(xb, conv), p, pinv), F.inv_q_mod_bsk[j], p, pinv);
             }
-        double pm = 0.0, pminv = 0.0, am = 0.0, fl_sk = 0.0;
-#pragma unroll
-        for (int j = 0; j < KBMAX; j++)
-            if (j == na) { pm = F.bd[j]; pminv = F.binv[j]; fl_sk = fl[j]; }
+        const double pm = F.bd[na], pminv = F.binv[na];
+        double am = 0.0;
 #pragma unroll
         for (int j = 0; j < KBMAX; j++)
             if (j < na) {
-                tmp[j] = fcanon(fl[j], F.bd[j], F.binv[j]);
+                tmp[j] = fcanon(fmodmul(fl[j], F.inv_bhat_mod_b[j], F.bd[j], F.binv[j]), F.bd[j], F.binv[j]);
                 am = __dadd_rn(am, fmodmul(tmp[j], F.bhat_mod_msk[j], pm, pminv));
             }
+        double fl_sk = 0.0; // fl[na] without a runtime-indexed (local-memory) array access
+#pragma unroll
+        for (int j = 0; j < KBMAX; j++)
+            if (j == na) fl_sk = fl[j];
         const double alpha = fcanon(fmodmul(frecenter(__dsub_rn(am, fl_sk), pm, pminv), F.inv_B_mod_msk, pm, pminv), pm, pminv);
+        // centred alpha: alpha > m_sk/2 means alpha - m_sk (negative)
         const double alpha_c = alpha > F.msk_half ? __dsub_rn(alpha, pm) : alpha;
-        u64 *dst = out + (gid >> logn) * (size_t)k * N + (gid & (size_t)(N - 1));
-        const int x = (int)(gid & (size_t)(N - 1));
-        const u64 *xs = EPI ? floor_epi_src(E, gid >> logn, x, k, N) : nullptr, *cs = EPI ? floor_epi_cpoly(E, gid >> logn, x) : nullptr;
+        const u64 *xs = EPI ? floor_epi_src(E, poly, x, k, N) : nullptr, *cs = EPI ? floor_epi_cpoly(E, poly, x) : nullptr;
 #pragma unroll
         for (int i = 0; i < KMAX; i++) {
             if (i >= k) break;
@@ -240,8 +175,97 @@ __global__ void __launch_bounds__(256) k_behz_floor_fold_fp(const u64 *__restric
             for (int j = 0; j < KBMAX; j++)
                 if (j < na) v = __dadd_rn(v, fmodmul(tmp[j], F.bhat_mod_q[i][j], p, pinv));
             v = __dsub_rn(v, fmodmul(alpha_c, F.B_mod_q[i], p, pinv));
-            if (EPI) v = floor_epi_fp(v, E, xs, cs, (int)((gid >> logn) % 3), x, i, N, p, pinv);
+            if (PAIR && h == 0) {
+                dst[(size_t)i * N] = fcanon_u(v, p, pinv);
+                continue;
+            }
+            if (PAIR) v = __dsub_rn(fcanon(v, p, pinv), u2d(dst[(size_t)i * N])); // |v| < p
+            if (EPI) v = floor_epi_fp(v, E, xs, cs, poly % 3, x, i, N, p, pinv);
             dst[(size_t)i * N] = fcanon_u(v, p, pinv);
+        }
+    }
+}
+
+// fast_floor + fastbconv_sk with the constant factors folded into the conversion matrices (FloorConstF): -19 % FP64 instructions,
+// -12 % time for the element-wise family.  Same outputs as k_behz_floor_fp: every folded product is the same residue class and the
+// canonical representatives are formed at the same points.  ITERS > 1 walks several coefficients per thread with the next one's
+// loads issued early -- measured 60 % slower (170 registers, one CTA per SM), so only ITERS = 1 is built.
+// PAIR (ITERS = 1, with EPI): as in k_behz_floor_fp
+template <int ITERS, bool EPI, bool PAIR = false>
+__global__ void __launch_bounds__(256) k_behz_floor_fold_fp(const u64 *__restrict__ d, u64 *__restrict__ out, size_t total, int logn,
+                                                           const __grid_constant__ FloorConstF F, const __grid_constant__ FloorEpi E) {
+    const int N = 1 << logn, k = F.k, kb = F.kb, kt = k + kb, na = kb - 1;
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    static_assert(!PAIR || ITERS == 1, "the pair floor walks one coefficient per thread");
+    double cq[KMAX], cb[KBMAX], nq[KMAX], nb[KBMAX]; // current / next coefficient: residues mod q_i and mod the Bsk primes
+    auto load = [&](double (&vq)[KMAX], double (&vb)[KBMAX], size_t g, int sel) {
+        const u64 *src = d + floor_src_poly(g >> logn, PAIR, sel) * (size_t)kt * N + (g & (size_t)(N - 1));
+#pragma unroll
+        for (int i = 0; i < KMAX; i++)
+            if (i < k) vq[i] = ld_lazy(src + (size_t)i * N);
+        src += (size_t)k * N;
+#pragma unroll
+        for (int j = 0; j < KBMAX; j++)
+            if (j < kb) vb[j] = ld_lazy(src + (size_t)j * N);
+    };
+    if (gid < total) load(cq, cb, gid, PAIR ? 1 : 0);
+#pragma unroll 1
+    for (int it = 0; it < ITERS; it++, gid += stride) {
+        if (gid >= total) return;
+        const bool more = ITERS > 1 && it + 1 < ITERS && gid + stride < total;
+        if (more) load(nq, nb, gid + stride, 0);
+#pragma unroll 1
+        for (int h = 0; h < (PAIR ? 2 : 1); h++) {
+            if (PAIR && h == 1) load(cq, cb, gid, 0);
+            double tmp[KBMAX];
+            // [x t q-hat_i^-1]_{q_i}, canonical representative (the base conversion sums these integers)
+#pragma unroll
+            for (int i = 0; i < KMAX; i++)
+                if (i < k) tmp[i] = fcanon(fmodmul(cq[i], F.xq[i], F.qd[i], F.qinv[i]), F.qd[i], F.qinv[i]);
+            double fl[KBMAX];
+#pragma unroll
+            for (int j = 0; j < KBMAX; j++)
+                if (j < kb) {
+                    const double p = F.bd[j], pinv = F.binv[j];
+                    double acc = fmodmul(cb[j], F.xb[j], p, pinv);
+#pragma unroll
+                    for (int i = 0; i < KMAX; i++)
+                        if (i < k) acc = __dsub_rn(acc, fmodmul(tmp[i], F.conv[j][i], p, pinv));
+                    fl[j] = acc; // j < na: floor_j * B-hat_j^-1 mod p_j;  j = na: floor mod m_sk   (|acc| <= (k+1) * 0.51 p)
+                }
+            double pm = 0.0, pminv = 0.0, am = 0.0, fl_sk = 0.0;
+#pragma unroll
+            for (int j = 0; j < KBMAX; j++)
+                if (j == na) { pm = F.bd[j]; pminv = F.binv[j]; fl_sk = fl[j]; }
+#pragma unroll
+            for (int j = 0; j < KBMAX; j++)
+                if (j < na) {
+                    tmp[j] = fcanon(fl[j], F.bd[j], F.binv[j]);
+                    am = __dadd_rn(am, fmodmul(tmp[j], F.bhat_mod_msk[j], pm, pminv));
+                }
+            const double alpha = fcanon(fmodmul(frecenter(__dsub_rn(am, fl_sk), pm, pminv), F.inv_B_mod_msk, pm, pminv), pm, pminv);
+            const double alpha_c = alpha > F.msk_half ? __dsub_rn(alpha, pm) : alpha;
+            u64 *dst = out + (gid >> logn) * (size_t)k * N + (gid & (size_t)(N - 1));
+            const int x = (int)(gid & (size_t)(N - 1));
+            const u64 *xs = EPI ? floor_epi_src(E, gid >> logn, x, k, N) : nullptr, *cs = EPI ? floor_epi_cpoly(E, gid >> logn, x) : nullptr;
+#pragma unroll
+            for (int i = 0; i < KMAX; i++) {
+                if (i >= k) break;
+                const double p = F.qd[i], pinv = F.qinv[i];
+                double v = 0.0;
+#pragma unroll
+                for (int j = 0; j < KBMAX; j++)
+                    if (j < na) v = __dadd_rn(v, fmodmul(tmp[j], F.bhat_mod_q[i][j], p, pinv));
+                v = __dsub_rn(v, fmodmul(alpha_c, F.B_mod_q[i], p, pinv));
+                if (PAIR && h == 0) {
+                    dst[(size_t)i * N] = fcanon_u(v, p, pinv);
+                    continue;
+                }
+                if (PAIR) v = __dsub_rn(fcanon(v, p, pinv), u2d(dst[(size_t)i * N])); // |v| < p
+                if (EPI) v = floor_epi_fp(v, E, xs, cs, (int)((gid >> logn) % 3), x, i, N, p, pinv);
+                dst[(size_t)i * N] = fcanon_u(v, p, pinv);
+            }
         }
         if (more) {
 #pragma unroll
@@ -442,18 +466,24 @@ cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int
     else k_behz_tensor_fp<false><<<blocks_for(((size_t)n * kt) << logn), 256, 0, s>>>(a, b, d, n, logn, *f);
     return cudaGetLastError();
 }
-cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi) {
+cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi,
+                                bool pair) {
     if (n <= 0) return cudaSuccess;
+    if (pair && !epi) return cudaErrorInvalidValue;
     const FloorEpi none{};
-    if (epi) k_behz_floor_fp<true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f, *epi);
+    if (pair) k_behz_floor_fp<true, true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f, *epi);
+    else if (epi) k_behz_floor_fp<true><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f, *epi);
     else k_behz_floor_fp<false><<<blocks_for((size_t)n * 3 << logn), 256, 0, s>>>(d, out3, n * 3, (double)t, logn, *f, none);
     return cudaGetLastError();
 }
-cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s, const FloorEpi *epi) {
+cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s, const FloorEpi *epi,
+                                     bool pair) {
     if (n <= 0) return cudaSuccess;
+    if (pair && !epi) return cudaErrorInvalidValue;
     const size_t total = (size_t)n * 3 << logn;
     const FloorEpi none{};
-    if (epi) k_behz_floor_fold_fp<1, true><<<blocks_for(total), 256, 0, s>>>(d, out3, total, logn, *f, *epi);
+    if (pair) k_behz_floor_fold_fp<1, true, true><<<blocks_for(total), 256, 0, s>>>(d, out3, total, logn, *f, *epi);
+    else if (epi) k_behz_floor_fold_fp<1, true><<<blocks_for(total), 256, 0, s>>>(d, out3, total, logn, *f, *epi);
     else k_behz_floor_fold_fp<1, false><<<blocks_for(total), 256, 0, s>>>(d, out3, total, logn, *f, none);
     return cudaGetLastError();
 }

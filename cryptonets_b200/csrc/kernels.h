@@ -133,8 +133,9 @@ struct FloorConstF {
 };
 // Epilogue of the BEHZ floor kernels (the quadratic activation A ct^2 + B x + C, cnhe_layer_poly2): every output polynomial times A,
 // B x added to c0 and c1, Delta C added to c0, mod q_l and canonical -- the words of multiply_plain(A) on the size-3 product, then (after
-// the key switch, which is linear) multiply_plain(x, B) and add_plain(C).  x[c]: the launch's c-th input ciphertext ([2][k][N],
-// canonical coefficient form; a device pointer table).  Per residue: A and B lifted into q_l with the upper-half increment, Delta C
+// the key switch, which is linear) multiply_plain(x, B) and add_plain(C).  x[c]: the ciphertext whose B multiple output c of the launch
+// gets ([2][k][N], canonical coefficient form; a device pointer table) -- the squared operand itself, or (the second level of
+// cnhe_layer_poly's quartic and cubic) the activation's original input.  Per residue: A and B lifted into q_l with the upper-half increment, Delta C
 // scaled as add_plain scales it; the *_d copies centred as exact doubles for the FP64 kernels.  C is the constant polynomial (every slot)
 // unless c_poly (nullptr, or a device table of one entry per ciphertext of the launch) gives the ciphertext a plaintext of its own:
 // c_poly[c] = nullptr, or [k][N] canonical words Delta m (+ q mod t where m is in the upper half) of a plaintext m, added to c0 in
@@ -158,6 +159,8 @@ struct PlainConst {
 // ---- elementwise over ciphertext words (words = n * size * k * N; residue of word w is (w / N) % k)
 cudaError_t launch_ct_add(const u64 *a, const u64 *b, u64 *out, size_t words, int k, int logn, const BehzConst *bc, int sub, cudaStream_t s);
 cudaError_t launch_ct_negate(const u64 *a, u64 *out, size_t words, int k, int logn, const BehzConst *bc, cudaStream_t s);
+// out[c] = a[c] + epi.x[c] + Delta C on c0 (FloorEpi's constant term; A and B unused): n size-2 ciphertexts
+cudaError_t launch_ct_add_epi(const u64 *a, u64 *out, int n, int k, int logn, const BehzConst *bc, const FloorEpi &epi, cudaStream_t s);
 // out = sum_j in_ptrs[j]  (AddMany)
 cudaError_t launch_ct_add_many(const u64 *const *in_ptrs, int n_in, u64 *out, size_t words, int k, int logn, const BehzConst *bc, cudaStream_t s);
 // ct (size polys) (+/-)= Delta*plain on c0; plain has `coeffs` coefficients mod t.  n cts, plain shared (plain_stride 0) or per ct.
@@ -203,7 +206,10 @@ cudaError_t launch_behz_lift(const u64 *const *ct_ptrs, u64 *out, int n, int log
 cudaError_t launch_behz_tensor(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConst *bc, cudaStream_t s);
 // d (coefficient form) -> times t, fast_floor, fastbconv_sk -> out3[n][3][k][N]
 // epi (host copy, every floor launcher): nullptr, or the FloorEpi applied to the outputs (its x table lists the launch's n ciphertexts)
-cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s, const FloorEpi *epi = nullptr);
+// pair (every floor launcher; needs epi): d holds 2n products [2n][3][kt][N], and output c is floor(product 2c) - floor(product 2c + 1)
+// mod q_l before the epilogue (the cubic activation's level 2, cnhe_layer_poly)
+cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s, const FloorEpi *epi = nullptr,
+                              bool pair = false);
 // lazy = 1: the buffers exchanged with the NTT kernels (lift output, tensor input/output, digit input, accumulator output) hold lazy
 // doubles (fparith.cuh) -- pair with NTT_IN_F / NTT_OUT_F on the transforms in between
 cudaError_t launch_behz_lift_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
@@ -216,9 +222,11 @@ cudaError_t launch_behz_square_fused(const u64 *const *ct_ptrs, const u64 *lift_
                                      cudaStream_t s);
 cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
 // canonical input; lazy input takes the folded kernel below
-cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr);
+cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr,
+                                bool pair = false);
 // folded constants + software-pipelined loads (lazy input only)
-cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr);
+cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr,
+                                     bool pair = false);
 cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,
                              const BehzConstF *f, int lazy, cudaStream_t s);
 // ---- K6: key-switch inner product. digits [n][D][k][N] (NTT), key [D][2][k][N] (NTT) -> acc [n][2][k][N] (NTT)

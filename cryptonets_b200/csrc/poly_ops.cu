@@ -26,6 +26,24 @@ __global__ void __launch_bounds__(256) k_ct_addsub(const u64 *a, const u64 *b, u
     const u64 p = q_of(bc, (int)((i >> logn) % k));
     out[i] = sub ? submod(a[i], b[i], p) : addmod(a[i], b[i], p);
 }
+// out[c] = a[c] + E.x[c] on both polynomials, + Delta C on c0 as the floor epilogue adds it (E.c at coefficient 0, or the ciphertext's
+// E.c_poly plaintext): n size-2 ciphertexts, the cubic activation's q1 = u + x + gamma (cnhe_layer_poly).  E.a and E.b are not used
+__global__ void __launch_bounds__(256) k_ct_add_epi(const u64 *a, u64 *out, int n, int k, int logn, const BehzConst *__restrict__ bc,
+                                                   const __grid_constant__ FloorEpi E) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t N = (size_t)1 << logn, per = 2 * (size_t)k * N;
+    if (i >= (size_t)n * per) return;
+    const size_t c = i / per, w = i % per;
+    const int l = (int)((w >> logn) % k), x = (int)(w & (N - 1));
+    const u64 p = q_of(bc, l);
+    u64 v = addmod(a[i], E.x[c][w], p);
+    if (w < (size_t)k * N) { // c0
+        const u64 *cs = E.c_poly ? E.c_poly[c] : nullptr;
+        if (cs) v = addmod(v, cs[w], p);
+        else if (x == 0) v = addmod(v, E.c[l], p);
+    }
+    out[i] = v;
+}
 __global__ void __launch_bounds__(256) k_ct_negate(const u64 *a, u64 *out, size_t words, int k, int logn, const BehzConst *__restrict__ bc) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= words) return;
@@ -419,6 +437,11 @@ cudaError_t launch_key_add_scaled(u64 *keys, const u64 *target, const u64 *facto
 cudaError_t launch_ct_add(const u64 *a, const u64 *b, u64 *out, size_t words, int k, int logn, const BehzConst *bc, int sub, cudaStream_t s) {
     if (!words) return cudaSuccess;
     k_ct_addsub<<<blocks_for(words), 256, 0, s>>>(a, b, out, words, k, logn, bc, sub);
+    return cudaGetLastError();
+}
+cudaError_t launch_ct_add_epi(const u64 *a, u64 *out, int n, int k, int logn, const BehzConst *bc, const FloorEpi &epi, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    k_ct_add_epi<<<blocks_for(((size_t)n * 2 * k) << logn), 256, 0, s>>>(a, out, n, k, logn, bc, epi);
     return cudaGetLastError();
 }
 cudaError_t launch_ct_negate(const u64 *a, u64 *out, size_t words, int k, int logn, const BehzConst *bc, cudaStream_t s) {

@@ -943,25 +943,31 @@ FloorEpi floor_epi(const Context &c, int ch, u64 A, u64 B, u64 C) {
     }
     return e;
 }
-// epi: the call's FloorEpi, its x table still to be pointed at the wave's inputs (x_ptrs) and its c_poly table (one entry per ciphertext
-// of the call) at the wave's first ciphertext c0
+// epi: the call's FloorEpi, its x table (when the caller gave none: the squared operands, x_ptrs) and its c_poly table (one entry per
+// output of the call) still to be pointed at the wave, whose first output is o0.  m products; pair: they make m / 2 outputs (2i, 2i + 1)
 static void multiply_floor(Context &c, int ch, const u64 *D, int m, bool lazy, u64 *out3, const FloorEpi *epi = nullptr,
-                           const u64 *const *x_ptrs = nullptr, int c0 = 0) {
+                           const u64 *const *x_ptrs = nullptr, int o0 = 0, bool pair = false) {
     FloorEpi e;
     if (epi) {
         e = *epi;
-        e.x = x_ptrs;
-        e.c_poly = epi->c_poly ? epi->c_poly + c0 : nullptr;
+        e.x = epi->x ? epi->x + o0 : x_ptrs;
+        e.c_poly = epi->c_poly ? epi->c_poly + o0 : nullptr;
     }
     const FloorEpi *ep = epi ? &e : nullptr;
-    // the epilogue's read of the input's c0 and c1 (8N bytes per residue and polynomial) is booked with the family
-    PROF(2, 8.0 * c.N * m * 3 * (2 * c.k + c.kb) + (epi ? 8.0 * c.N * m * 2 * c.k : 0.0));
-    if (c.fp_elementwise && lazy) c.check(launch_behz_floor_fold_fp(D, out3, m, c.logN, &c.ch[ch].floor_f, c.stream, ep), "behz_floor_fold_fp");
-    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, m, c.ch[ch].t, c.logN, &c.h_bf, c.stream, ep), "behz_floor_fp");
-    else c.check(launch_behz_floor(D, out3, m, c.ch[ch].t, c.logN, c.d_bc, c.stream, ep), "behz_floor");
+    const int n_out = pair ? m / 2 : m;
+    // the epilogue's read of the input's c0 and c1 (8N bytes per residue and polynomial) is booked with the family; the pair floor also
+    // parks the second product's floor in the output and reads it back
+    PROF(2, 8.0 * c.N * m * 3 * (c.k + c.kb) + 8.0 * c.N * n_out * 3 * c.k + (epi ? 8.0 * c.N * n_out * 2 * c.k : 0.0) +
+                (pair ? 16.0 * c.N * n_out * 3 * c.k : 0.0));
+    if (c.fp_elementwise && lazy)
+        c.check(launch_behz_floor_fold_fp(D, out3, n_out, c.logN, &c.ch[ch].floor_f, c.stream, ep, pair), "behz_floor_fold_fp");
+    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, n_out, c.ch[ch].t, c.logN, &c.h_bf, c.stream, ep, pair), "behz_floor_fp");
+    else c.check(launch_behz_floor(D, out3, n_out, c.ch[ch].t, c.logN, c.d_bc, c.stream, ep, pair), "behz_floor");
 }
+// products c0 .. c0 + m - 1 of a x b; with an epilogue, o0 is the wave's first output (c0, or c0 / 2 for pairs)
 static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, int c0, int m, u64 *out3,
-                           bool fused, const FloorEpi *epi = nullptr) {
+                           bool fused, const FloorEpi *epi = nullptr, bool pair = false) {
+    const int o0 = pair ? c0 / 2 : c0;
     const int k = c.k, kt = k + c.kb;
     const size_t N = c.N;
     if (fused) {
@@ -976,7 +982,7 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
             PROF(0, 8.0 * N * m * (2 * kt + 3 * kt));
             c.check(launch_behz_square_fused(ptrs, L, D, m, k, kt, c.logN, c.d_tabs, c.stream), "behz_square_fused");
         }
-        multiply_floor(c, ch, D, m, true, out3, epi, ptrs, c0);
+        multiply_floor(c, ch, D, m, true, out3, epi, ptrs, o0, pair);
         return;
     }
     bool square = true;
@@ -1015,7 +1021,7 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
         PROF(1, 16.0 * N * m * 3 * kt);
         c.check(launch_ntt_inverse(D, D, m * 3 * kt, c.logN, c.d_tabs, 0, kt, fmt, c.stream), "ntt_inverse");
     }
-    multiply_floor(c, ch, D, m, lazy, out3, epi, pa_dev, c0);
+    multiply_floor(c, ch, D, m, lazy, out3, epi, pa_dev, o0, pair);
 }
 void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3) {
     const int n = (int)a.size();
@@ -1038,21 +1044,22 @@ void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const 
     c.note(Context::OP_RELINEARIZE, ch, n, out2);
 }
 void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2, const int *slots,
-                       const FloorEpi *epi) {
-    const int n = (int)a.size(), k = c.k;
+                       const FloorEpi *epi, bool pair) {
+    if (pair && (!epi || !epi->x || a.size() % 2)) throw Error(-1, "the pair floor needs an epilogue with its own x table and whole pairs");
+    const int per = pair ? 2 : 1, n = (int)a.size() / per, k = c.k;
     const KsKeys keys = relin_keys(c, ch, n, slots);
     const size_t N = c.N;
     const bool fused = mul_fused(c, a, b);
-    const int wave = c.wave((ks_fused(c, n) ? 0 : (size_t)c.dm_relin.D * k * N) + mul_words(c, fused) + 5 * k * N);
+    const int wave = c.wave((ks_fused(c, n) ? 0 : (size_t)c.dm_relin.D * k * N) + per * mul_words(c, fused) + 5 * k * N);
     for (int c0 = 0; c0 < n; c0 += wave) {
         WsScope scope(c); // stream-ordered frees: the next wave reuses the memory once these kernels are done
         const int m = std::min(wave, n - c0);
         u64 *ct3 = c.ws_alloc((size_t)m * 3 * k * N);
-        multiply_chunk(c, ch, a, b, c0, m, ct3, fused, epi);
+        multiply_chunk(c, ch, a, b, c0 * per, m * per, ct3, fused, epi, pair);
         const size_t s3 = (size_t)3 * k * N;
         op_key_switch(c, ct3 + (size_t)2 * k * N, s3, m, keys.slice(c0, m), c.dm_relin, ct3, s3, out2 + (size_t)c0 * 2 * k * N);
     }
-    c.op_count[Context::OP_MULTIPLY] += (uint64_t)n;
+    c.op_count[Context::OP_MULTIPLY] += (uint64_t)a.size();
     c.note(Context::OP_RELINEARIZE, ch, n, out2, a[0], b[0]);
 }
 

@@ -218,10 +218,13 @@ void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const st
 // Key-switching operations take the keys of ciphertext i from key slot slots[i] when a per-ciphertext slot table is given (n entries,
 // host), otherwise every ciphertext uses the call's slot c.slot.  A missing key is CNHE_ERR_STATE.
 void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots = nullptr);
-// epi (squares only, a[i] == b[i]): nullptr, or the quadratic activation out2 = relin(A a^2) + B a + Delta C (floor_epi; the x table is
-// filled per wave; c_poly, when set, has one entry per ciphertext of the call) applied in the BEHZ floor kernel
+// epi (squares only, a[i] == b[i]): nullptr, or the quadratic activation out2 = relin(A a^2) + B x + Delta C (floor_epi) applied in the
+// BEHZ floor kernel.  x: epi->x, a device table of one input per output of the call (cnhe_layer_poly's second level: the activation's
+// original input), or nullptr for the squared operand itself; c_poly, when set, has one entry per output of the call.
+// pair (with epi): a holds 2n operands and output i is relin(A (a[2i]^2 - a[2i+1]^2)) + B x[i] + Delta C -- 2n squares, one floor and one
+// key switch per output (the cubic activation's second level); slots then has n entries
 void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2,
-                       const int *slots = nullptr, const FloorEpi *epi = nullptr);
+                       const int *slots = nullptr, const FloorEpi *epi = nullptr, bool pair = false);
 // the FloorEpi constants of A, B, C (residues mod the channel's t): A and B lifted into every q_l as multiply_plain lifts a constant
 // plaintext, C scaled as add_plain scales it
 FloorEpi floor_epi(const Context &c, int ch, u64 A, u64 B, u64 C);

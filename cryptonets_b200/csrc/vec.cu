@@ -2511,6 +2511,146 @@ extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, c
     API_END
 }
 
+// Quartic and cubic activations in two multiplicative levels built from squares only (DESIGN.md section 4.12).  Per plaintext prime t,
+// with the coefficients c_j of x^j reduced mod t and A the leading one:
+//   quartic (A, B, C, D, E): beta = B (2A)^-1, gamma = (C A^-1 - beta^2) 2^-1, D' = D - B gamma, E' = E - A gamma^2:
+//     q = x^2 + beta x + gamma,  P(x) = A q^2 + D' x + E'
+//   cubic (A, B, C, D): lambda = A 2^-1, gamma = (B lambda^-1 - 1) 2^-1, C' = C - A gamma, D' = D - lambda gamma^2:
+//     u = x^2, q1 = u + x + gamma,  P(x) = lambda (q1^2 - u^2) + C' x + D'
+struct PolyConsts {
+    u64 lead, b, g, lin, cst; // quartic: A, beta, gamma, D', E'   cubic: lambda, -, gamma, C', D'
+};
+static PolyConsts poly_consts(u64 t, int degree, const u64 *cf /*degree + 1 residues, cf[j] of x^j*/) {
+    const u64 inv2 = hm::inv(2, t);
+    PolyConsts k{};
+    if (degree == 4) {
+        const u64 A = cf[4], B = cf[3], C = cf[2], D = cf[1], E = cf[0];
+        k.lead = A;
+        k.b = hm::mul(B, hm::inv(hm::add(A, A, t), t), t);
+        k.g = hm::mul(hm::sub(hm::mul(C, hm::inv(A, t), t), hm::mul(k.b, k.b, t), t), inv2, t);
+        k.lin = hm::sub(D, hm::mul(B, k.g, t), t);
+        k.cst = hm::sub(E, hm::mul(A, hm::mul(k.g, k.g, t), t), t);
+    } else {
+        const u64 A = cf[3], B = cf[2], C = cf[1], D = cf[0];
+        k.lead = hm::mul(A, inv2, t);
+        k.g = hm::mul(hm::sub(hm::mul(B, hm::inv(k.lead, t), t), 1, t), inv2, t);
+        k.lin = hm::sub(C, hm::mul(A, k.g, t), t);
+        k.cst = hm::sub(D, hm::mul(k.lead, hm::mul(k.g, k.g, t), t), t);
+    }
+    return k;
+}
+// P(x) of degree 3 or 4 over a whole matrix.  Quartic: level 1 is cnhe_layer_poly2(x; 1, beta, gamma); level 2 squares q with the floor
+// epilogue (A, D', E') reading the original input x.  Cubic: level 1 squares x (u) and forms q1 = u + x + gamma; level 2 squares q1 and u
+// side by side in one wave, and the pair floor subtracts the two products and applies (lambda, C', D') before one key switch per output
+extern "C" int cnhe_layer_poly(cnhe_ctx *h, const cnhe_vec *const *in, int n, const cnhe_vec *const *coeffs, int degree, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n < 1) fail("empty layer");
+    if (degree != 3 && degree != 4) fail("the degree must be 3 or 4");
+    if (!coeffs || !coeffs[degree]) fail("the leading coefficient is required");
+    for (int j = 0; j <= degree; j++) {
+        const cnhe_vec *p = coeffs[j];
+        if (!p) continue;
+        same_ctx(c, p);
+        if (p->enc) fail("the coefficients must be plain");
+        if (p->format != CNHE_SPARSE || p->dim != 1) fail("each coefficient must be a sparse vector of dimension 1");
+    }
+    std::vector<int> first(n + 1, 0);
+    for (int i = 0; i < n; i++) {
+        same_ctx(c, in[i]);
+        if (!in[i]->enc) fail("the inputs must be encrypted");
+        if (in[i]->scale != in[0]->scale) fail("Scales do not match.");
+        first[i + 1] = first[i] + in[i]->blocks;
+    }
+    // coefficient j at scale W s^(degree - j), W the leading coefficient's scale; the powers of s multiplied up one factor at a time
+    const double s = in[0]->scale, W = coeffs[degree]->scale;
+    auto scale_at = [&](int e) {
+        double r = W;
+        for (int i = 0; i < e; i++) r *= s;
+        return r;
+    };
+    for (int j = 0; j < degree; j++)
+        if (coeffs[j] && coeffs[j]->scale != scale_at(degree - j)) fail("Scales do not match.");
+    std::vector<PolyConsts> pk(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        const u64 t = c.ch[ch].t;
+        u64 cf[5];
+        for (int j = 0; j <= degree; j++) cf[j] = coeffs[j] ? coeffs[j]->scalars[ch][0] % t : 0;
+        if (cf[degree] == 0)
+            fail(("the leading coefficient is 0 mod the plaintext prime " + std::to_string(t) + ": it has no inverse there").c_str());
+        pk[ch] = poly_consts(t, degree, cf);
+    }
+    const double out_scale = scale_at(degree);
+    const int total = first[n];
+    const size_t cw = c.ct_words();
+    const std::vector<int> vslot = vec_slots(c, in, n);
+    std::vector<int> ct_slot;
+    for (int i = 0; i < n; i++) ct_slot.insert(ct_slot.end(), in[i]->blocks, vslot[i]);
+    std::vector<BufRef> big(c.P);
+    auto &ops = c.op_count;
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        const PolyConsts &k = pk[ch];
+        big[ch] = c.alloc((size_t)total * cw);
+        std::vector<const u64 *> xs;
+        for (int i = 0; i < n; i++)
+            for (int bl = 0; bl < in[i]->blocks; bl++) xs.push_back(in[i]->block(ch, bl));
+        const u64 *const *x_tab = upload_ptrs(c, xs);
+        // the operations of the composition (a term that is 0 mod t is skipped in that channel, as in cnhe_layer_poly2)
+        auto linear_and_constant = [&](u64 lin, u64 cst) {
+            if (lin) {
+                ops[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+                ops[Context::OP_ADD] += (uint64_t)total;
+            }
+            if (cst) ops[Context::OP_ADD_PLAIN] += (uint64_t)total;
+        };
+        FloorEpi e2 = floor_epi(c, ch, k.lead, k.lin, k.cst);
+        e2.x = x_tab;
+        if (k.cst) e2.c_poly = padded_constants(c, ch, in, n, total, k.cst);
+        BufRef mid;
+        std::vector<const u64 *> sq; // the second level's squared operands
+        if (degree == 4) {
+            // level 1: q = cnhe_layer_poly2(x; 1, beta, gamma)
+            mid = c.alloc((size_t)total * cw);
+            FloorEpi e1 = floor_epi(c, ch, 1, k.b, k.g);
+            if (k.g) e1.c_poly = padded_constants(c, ch, in, n, total, k.g);
+            op_multiply_relin(c, ch, xs, xs, mid->p, ct_slot.data(), &e1);
+            ops[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+            linear_and_constant(k.b, k.g);
+            for (int i = 0; i < total; i++) sq.push_back(mid->p + (size_t)i * cw);
+            // level 2: relinearize(A (.) q^2) + D' x + E'
+            op_multiply_relin(c, ch, sq, sq, big[ch]->p, ct_slot.data(), &e2);
+            ops[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+        } else {
+            // level 1: u = relinearize(x^2) in [0, total), q1 = u + x + gamma in [total, 2 total)
+            mid = c.alloc((size_t)2 * total * cw);
+            u64 *u = mid->p, *q1 = mid->p + (size_t)total * cw;
+            op_multiply_relin(c, ch, xs, xs, u, ct_slot.data());
+            FloorEpi e1 = floor_epi(c, ch, 1, 1, k.g);
+            e1.x = x_tab;
+            if (k.g) e1.c_poly = padded_constants(c, ch, in, n, total, k.g);
+            c.prof_begin(2, 24.0 * c.N * total * 2 * c.k);
+            c.check(launch_ct_add_epi(u, q1, total, c.k, c.logN, c.d_bc, e1, c.stream), "ct_add_epi");
+            c.prof_end();
+            ops[Context::OP_ADD] += (uint64_t)total;
+            if (k.g) ops[Context::OP_ADD_PLAIN] += (uint64_t)total;
+            for (int i = 0; i < total; i++) {
+                sq.push_back(q1 + (size_t)i * cw);
+                sq.push_back(u + (size_t)i * cw);
+            }
+            // level 2: relinearize(lambda (.) (q1^2 - u^2)) + C' x + D', one key switch per output
+            op_multiply_relin(c, ch, sq, sq, big[ch]->p, ct_slot.data(), &e2, true);
+            ops[Context::OP_SUB] += (uint64_t)total;
+            ops[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+        }
+        linear_and_constant(k.lin, k.cst);
+    }
+    for (int i = 0; i < n; i++) {
+        out[i] = slab_view(new_vec(c, in[i]->dim, out_scale, in[i]->format, true, in[i]->blocks), big, first[i]);
+        out[i]->slot = vslot[i];
+    }
+    API_END
+}
+
 // ---------------------------------------------------------------------------------------------------- diagonal matrix-vector product
 // A plain matrix prepared for the diagonal (Halevi-Shoup) product with baby-step / giant-step (DESIGN.md section 4.10, slot layout in
 // diag.cu): its nonzero generalised diagonals (b, s = n1 g + h), each rotated right by n1 g and encoded, ordered by g, then b, then h.

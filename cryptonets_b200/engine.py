@@ -685,6 +685,15 @@ class Engine:
         check(self.L.cnhe_layer_poly2(self.h, _vec_array(inputs), n, h(a), h(b), h(c), out))
         return self._wrap_many(out, n, like=inputs)
 
+    def layer_poly(self, inputs, coeffs):
+        """P(x) = sum_j coeffs[j] x^j of every input, degree len(coeffs) - 1 = 3 or 4, in two levels of squares (include/cnhe.h,
+        cnhe_layer_poly): coeffs[j] is a plain sparse vector of dimension 1 at scale W s^(degree - j), or None for 0 (the leading one is
+        required); the outputs have scale W s^degree."""
+        n = len(inputs)
+        out = (VECP * n)()
+        check(self.L.cnhe_layer_poly(self.h, _vec_array(inputs), n, _vec_array(list(coeffs)), len(coeffs) - 1, out))
+        return self._wrap_many(out, n, like=inputs)
+
     # ---- raw device arrays (micro-benchmarks, kernel parity tests)
     def dev_alloc(self, words):
         p = C.c_uint64()

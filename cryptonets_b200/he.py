@@ -97,6 +97,17 @@ class B200BfvVector:
         return self._wrap(self.eng.permute(self.vec, sel, shifts, outputDim))
 
 
+
+def _poly_layer(engine, vecs, a, b, c):
+    """PolyActivation's call: the quadratic (a, b, c) through cnhe_layer_poly2, or a = 4 or 5 coefficient vectors, highest degree first,
+    through cnhe_layer_poly"""
+    v = lambda x: None if x is None else x.vec
+    if isinstance(a, (list, tuple)):
+        if b is not None or c is not None:
+            raise Exception("a list of coefficients takes no b or c")
+        return engine.layer_poly(vecs, [v(x) for x in reversed(a)])
+    return engine.layer_poly2(vecs, a.vec, v(b), v(c))
+
 class B200BfvMatrix:
     """IMatrix as an array of vectors (`HE Wrapper/EncryptedSealBfvMatrix.cs:14-231`)."""
 
@@ -210,8 +221,10 @@ class B200BfvMatrix:
 
     def PolyActivation(self, a, b=None, c=None, env=None):
         """a x^2 + b x + c of every column in one wave (cnhe_layer_poly2): a, b, c plain sparse vectors of dimension 1 at scales W, W s and
-        W s^2 (b, c may be None); the result has scale W s^2."""
-        out = self.eng.layer_poly2([v.vec for v in self.vectors], a.vec, None if b is None else b.vec, None if c is None else c.vec)
+        W s^2 (b, c may be None); the result has scale W s^2.  a may instead be a sequence of 4 or 5 such vectors, highest degree first
+        (None for 0, the first required), for the cubic or quartic of cnhe_layer_poly (b and c then None): coefficient j at scale
+        W s^(d - j), the result at scale W s^d."""
+        out = _poly_layer(self.eng, [v.vec for v in self.vectors], a, b, c)
         return B200BfvMatrix(self.factory, [B200BfvVector(self.factory, o) for o in out], self.Format, CopyVectors=False)
 
     def GetColumn(self, i):
@@ -391,7 +404,7 @@ class B200BfvFactory:
     def PolyActivationBatch(self, matrices, a, b=None, c=None):
         """m.PolyActivation(a, b, c) of several matrices (possibly of different clients) in one relinearisation wave."""
         vecs = [v.vec for m in matrices for v in m.vectors]
-        out = self.engine.layer_poly2(vecs, a.vec, None if b is None else b.vec, None if c is None else c.vec)
+        out = _poly_layer(self.engine, vecs, a, b, c)
         i, res = 0, []
         for m in matrices:
             n = len(m.vectors)

@@ -9,7 +9,7 @@ import time
 import numpy as np
 
 from .interfaces import EMatrixFormat, EVectorFormat
-from .raw import RawFactory, RawMatrix
+from .raw import RawFactory, RawMatrix, poly_scale
 
 
 class ConvolutionEngine:
@@ -300,7 +300,11 @@ class PolyActivation(BaseLayer):
     and the output scale is W s^2.  On a B200BfvFactory the whole layer is one call (cnhe_layer_poly2) with the square's passes; a
     coefficient that rounds to 0 is left out.  Slots: a dense vector's padding slots (beyond its dimension) stay zero, as they do for
     SquareActivation, so that rotating layers such as LLDuplicateLayer see only the data; each ciphertext of a sparse vector gets C in all
-    of its slots (there the slots are separate images, which no layer mixes)."""
+    of its slots (there the slots are separate images, which no layer mixes).
+
+    Coefficients of length 4 or 5, (c_d, ..., c_0) highest degree first, give the cubic or quartic of cnhe_layer_poly (two levels of
+    squares): coefficient j is round(c_j W s^(d - j)) and the output scale is W s^d.  c_d must not round to 0 mod any plaintext prime; the
+    output scale grows as s^d, so the plaintext primes must hold the largest |value| below half their product."""
 
     def __init__(self, **kw):
         self.Coefficients = (1.0, 0.0, 0.0)
@@ -309,27 +313,40 @@ class PolyActivation(BaseLayer):
         super().__init__(**kw)
 
     def Prepare(self):
-        a, b, c = (float(x) for x in self.Coefficients)
+        cs = [float(x) for x in self.Coefficients]
+        if len(cs) not in (3, 4, 5):
+            raise Exception("PolyActivation takes 3, 4 or 5 coefficients")
         W, s = self.CoefficientScale, self.Source.GetOutputScale()
         f = self.Factory
 
         def vec(v, scale):
             return None if np.rint(v * scale) == 0 else f.GetPlainVector([v], EVectorFormat.sparse, scale)
 
-        self.coefficientVectors = (f.GetPlainVector([a], EVectorFormat.sparse, W), vec(b, W * s), vec(c, W * s * s))
+        if len(cs) == 3:
+            a, b, c = cs
+            self.coefficientVectors = (f.GetPlainVector([a], EVectorFormat.sparse, W), vec(b, W * s), vec(c, W * s * s))
+        else:
+            self.coefficientVectors = tuple([f.GetPlainVector([cs[0]], EVectorFormat.sparse, W)] +
+                                            [vec(v, poly_scale(W, s, i)) for i, v in enumerate(cs[1:], 1)])
+
+    def _args(self):
+        # the quadratic's (a, b, c), or the cubic's / quartic's coefficient list
+        return self.coefficientVectors if len(self.coefficientVectors) == 3 else (list(self.coefficientVectors),)
 
     def Apply(self, m):
-        return m.PolyActivation(*self.coefficientVectors, env=self.Factory.AllocateComputationEnv())
+        return m.PolyActivation(*self._args(), env=self.Factory.AllocateComputationEnv())
 
     def ApplyBatch(self, ms):
         batch = getattr(self.Factory, "PolyActivationBatch", None)
         if batch is None or len(ms) < 2:
             return super().ApplyBatch(ms)
-        return batch(ms, *self.coefficientVectors)
+        return batch(ms, *self._args())
 
     def GetOutputScale(self):
         s = self.Source.GetOutputScale()
-        return self.CoefficientScale * s * s
+        if len(self.Coefficients) == 3:
+            return self.CoefficientScale * s * s
+        return poly_scale(self.CoefficientScale, s, len(self.Coefficients) - 1)
 
     def Dispose(self):
         for v in self.coefficientVectors or ():

@@ -135,6 +135,14 @@ class RawVector:
         return RawVector._of(res[:outputDim], self.Scale * selections[0].Scale, self.BlockSize)
 
 
+
+def poly_scale(W, s, e):
+    """W s^e with the powers of s multiplied up one factor at a time, as cnhe_layer_poly forms the scales it checks"""
+    r = W
+    for _ in range(e):
+        r *= s
+    return r
+
 class RawMatrix:
     Max = 0.0
 
@@ -179,7 +187,12 @@ class RawMatrix:
 
     def PolyActivation(self, a, b=None, c=None, env=None):
         """A x^2 + B x + C on every scaled integer: a, b, c are sparse vectors of dimension 1 at scales W, W s, W s^2 (b, c may be None),
-        checked exactly as cnhe_layer_poly2 checks them."""
+        checked exactly as cnhe_layer_poly2 checks them.  a may instead be a sequence of 4 or 5 coefficient vectors, highest degree first
+        (None for 0, the first required), checked as cnhe_layer_poly checks them: the integer polynomial, evaluated exactly."""
+        if isinstance(a, (list, tuple)):
+            if b is not None or c is not None:
+                raise Exception("a list of coefficients takes no b or c")
+            return self._poly(a)
         out_scale = a.Scale * self.Scale * self.Scale
         if (b is not None and b.Scale * self.Scale != out_scale) or (c is not None and c.Scale != out_scale):
             raise Exception("Scales do not match.")
@@ -189,6 +202,25 @@ class RawMatrix:
         if c is not None:
             r.m = r.m + c.v[0]
         r.Scale = out_scale
+        return r
+
+    def _poly(self, coeffs):
+        d = len(coeffs) - 1
+        if d not in (3, 4):
+            raise Exception("the degree must be 3 or 4")
+        if coeffs[0] is None:
+            raise Exception("the leading coefficient is required")
+        s, W = self.Scale, coeffs[0].Scale
+        for i, v in enumerate(coeffs[1:], 1):  # coefficient of x^(d - i), at scale W s^i
+            if v is not None and v.Scale != poly_scale(W, s, i):
+                raise Exception("Scales do not match.")
+        x = self.m.astype(np.int64).astype(object)  # exact integers: the polynomial's terms may pass 2^53
+        acc = np.full(x.shape, int(coeffs[0].v[0]), dtype=object)
+        for v in coeffs[1:]:
+            acc = acc * x + (0 if v is None else int(v.v[0]))
+        r = RawMatrix(np.zeros(self.m.shape), 1, self.Format, self.BlockSize)
+        r.m = np.array(acc.tolist(), dtype=np.float64).reshape(self.m.shape)
+        r.Scale = poly_scale(W, s, d)
         return r
 
     def Add(self, m, env=None):

@@ -322,6 +322,18 @@ int cnhe_layer_square(cnhe_ctx *, const cnhe_vec *const *in, int n, cnhe_vec **o
  * cnhe_layer_square's words.  The inputs must share one scale, and scale(b) s and scale(c) must equal scale(a) s^2 exactly; the vectors
  * may belong to different key slots, as for cnhe_layer_square.  Operation counts are those of the composition. */
 int cnhe_layer_poly2(cnhe_ctx *, const cnhe_vec *const *in, int n, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *c, cnhe_vec **out /*n*/);
+/* Polynomial activation P(x) = sum_j coeffs[j] x^j of degree 3 or 4 over a whole matrix, in two multiplicative levels built from squares
+ * only (DESIGN.md section 4.12).  coeffs has degree + 1 entries, coeffs[j] the coefficient of x^j: plain SPARSE vectors of dimension 1
+ * at scale W s^(degree - j), W = scale(coeffs[degree]), s = scale of the inputs; NULL means 0, except coeffs[degree], which is required
+ * and must be nonzero mod every plaintext prime.  The output scale is W s^degree.  Per plaintext prime, with the constants of DESIGN 4.12
+ * and "+ K" a constant added as cnhe_layer_poly2 adds c (data slots only on a dense vector), out[i] is, word for word,
+ *   quartic:  q = cnhe_layer_poly2(x; 1, beta, gamma);  relinearize(A (.) multiply(q, q)) + multiply_plain(x, D') + E'
+ *   cubic:    u = relinearize(multiply(x, x));  q1 = add(u, x) + gamma;
+ *             relinearize(lambda (.) (multiply(q1, q1) - multiply(u, u))) + multiply_plain(x, C') + D'
+ * where K (.) multiplies all three polynomials of a size-3 ciphertext by the constant K.  The inputs must share one scale, and the
+ * vectors may belong to different key slots, as for cnhe_layer_square.  Operation counts are those of the composition. */
+int cnhe_layer_poly(cnhe_ctx *, const cnhe_vec *const *in, int n, const cnhe_vec *const *coeffs /*degree + 1*/, int degree,
+                    cnhe_vec **out /*n*/);
 
 /* ---- micro-benchmark / kernel-level entry points on caller-owned device memory ("raw") --------------------------- */
 int cnhe_dev_alloc(cnhe_ctx *, size_t words, uint64_t *dptr);

@@ -109,6 +109,7 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_conv_dense(IntPtr a0, IntPtr[] @in, int n_in, int[] gather, IntPtr[] weights, IntPtr[] bias, int M, int K, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_square(IntPtr a0, IntPtr[] @in, int n, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_poly2(IntPtr a0, IntPtr[] @in, int n, IntPtr a, IntPtr b, IntPtr c, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_poly(IntPtr a0, IntPtr[] @in, int n, IntPtr[] coeffs, int degree, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_alloc(IntPtr a0, UIntPtr words, out ulong dptr);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_free(IntPtr a0, ulong dptr);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_upload(IntPtr a0, ulong dptr, IntPtr src, UIntPtr words);
@@ -314,6 +315,15 @@ namespace HEWrapper
             var outs = new IntPtr[Vectors.Length];
             Cnhe.Check(Cnhe.cnhe_layer_poly2(Ctx, Cnhe.Handles(Vectors), Vectors.Length, ((B200BfvVector)a).Handle,
                                              b == null ? IntPtr.Zero : ((B200BfvVector)b).Handle, c == null ? IntPtr.Zero : ((B200BfvVector)c).Handle, outs));
+            return new B200BfvMatrix(Factory, outs.Select(h => (IVector)new B200BfvVector(Factory, h)).ToArray(), Format, false) { DataDisposedExternaly = false };
+        }
+        /// the cubic or quartic of every column in two levels of squares (cnhe_layer_poly): 4 or 5 plain sparse vectors of dimension 1,
+        /// highest degree first (null for 0, the first required), coefficient j at scale W s^(d - j); the result has scale W s^d
+        public IMatrix PolyActivation(IVector[] coefficients)
+        {
+            var outs = new IntPtr[Vectors.Length];
+            var coeffs = coefficients.Reverse().Select(v => v == null ? IntPtr.Zero : ((B200BfvVector)v).Handle).ToArray();
+            Cnhe.Check(Cnhe.cnhe_layer_poly(Ctx, Cnhe.Handles(Vectors), Vectors.Length, coeffs, coeffs.Length - 1, outs));
             return new B200BfvMatrix(Factory, outs.Select(h => (IVector)new B200BfvVector(Factory, h)).ToArray(), Format, false) { DataDisposedExternaly = false };
         }
         public IVector GetColumn(int columnNumber)
