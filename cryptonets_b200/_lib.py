@@ -52,6 +52,8 @@ _SIGS = {
     "cnhe_diag_ntt_info": [C.c_void_p, C.POINTER(i32), C.POINTER(i32), U64P],
     "cnhe_diag_export_ntt": [C.c_void_p, C.c_void_p, i32, i32, U64P, sz],
     "cnhe_mat_mul_diagonal": [C.c_void_p, C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP)],
+    "cnhe_diag_prepare_folded": [C.c_void_p, C.POINTER(VECP), i32, i32, i32, u64, C.POINTER(C.c_void_p)],
+    "cnhe_diag_fold_width": [C.c_void_p, C.POINTER(i32)],
     "cnhe_vec_write": [C.c_void_p, VECP, C.c_void_p, sz, C.POINTER(sz)],
     "cnhe_vec_read": [C.c_void_p, C.c_char_p, sz, C.POINTER(VECP), C.POINTER(sz)],
     "cnhe_keys_generate_secure": [C.c_void_p],

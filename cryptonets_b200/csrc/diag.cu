@@ -23,17 +23,29 @@ __global__ void __launch_bounds__(256) k_diag_flags(const u64 *__restrict__ vals
     if (col < dim && vals[(size_t)r * N + col] != 0) flags[bs] = 1;
 }
 
+// The folded product's flags (R <= N/2): flags[d] = 1, 0 <= d < N/2, when some nonzero weight M[r, col] has col - r = d mod N/2.  Wrapped
+// diagonal j of fold width W (a power of two dividing N/2), E_j[(a, x)] = M[x mod W, a N/2 + (x + j mod N/2)], is nonzero exactly when
+// flags[d] is set for some d = j mod W, so this one pass serves every width the planner weighs.
+__global__ void __launch_bounds__(256) k_diag_flags_folded(const u64 *__restrict__ vals, int R, int dim, int logn, unsigned *__restrict__ flags) {
+    const int N = 1 << logn, half = N >> 1;
+    const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= (size_t)R << logn) return;
+    const int r = (int)(gid >> logn), col = (int)(gid & (N - 1));
+    if (col < dim && vals[gid] != 0) flags[(col - r) & (half - 1)] = 1;
+}
+
 // out[j][(a, x)] = M[(a, x - n1 g_j mod N/2), (a ^ b_j, x + h_j mod N/2)] (0 outside R x dim): the pre-rotated diagonal j, in slot order.
-// desc[j] = (b_j, n1 g_j, h_j).
+// desc[j] = (b_j, n1 g_j, h_j).  fold = W > 0 (the folded product, b_j = 0): the row is (x - n1 g_j) mod W instead, so that out[j] is
+// wrapped diagonal n1 g_j + h_j rotated right by n1 g_j.
 __global__ void __launch_bounds__(256) k_diag_gather(const u64 *__restrict__ vals, int R, int dim, const int3 *__restrict__ desc, int nd, int logn,
-                                                     u64 *__restrict__ out) {
+                                                     int fold, u64 *__restrict__ out) {
     const int N = 1 << logn, half = N >> 1;
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= (size_t)nd << logn) return;
     const int j = (int)(gid >> logn), i = (int)(gid & (N - 1));
     const int3 d = desc[j];
     const int a = i >> (logn - 1), x = i & (half - 1);
-    const int r = (a << (logn - 1)) | ((x - d.y) & (half - 1));
+    const int r = fold ? (x - d.y) & (fold - 1) : (a << (logn - 1)) | ((x - d.y) & (half - 1));
     const int col = ((a ^ d.x) << (logn - 1)) | ((x + d.z) & (half - 1));
     out[gid] = r < R && col < dim ? vals[(size_t)r * N + col] : 0;
 }
@@ -171,9 +183,14 @@ cudaError_t launch_diag_flags(const u64 *vals, int R, int dim, int logn, unsigne
     k_diag_flags<<<diag_blocks((size_t)R << logn), 256, 0, s>>>(vals, R, dim, logn, flags);
     return cudaGetLastError();
 }
-cudaError_t launch_diag_gather(const u64 *vals, int R, int dim, const int *desc, int nd, int logn, u64 *out, cudaStream_t s) {
+cudaError_t launch_diag_flags_folded(const u64 *vals, int R, int dim, int logn, unsigned *flags, cudaStream_t s) {
+    if (R <= 0) return cudaSuccess;
+    k_diag_flags_folded<<<diag_blocks((size_t)R << logn), 256, 0, s>>>(vals, R, dim, logn, flags);
+    return cudaGetLastError();
+}
+cudaError_t launch_diag_gather(const u64 *vals, int R, int dim, const int *desc, int nd, int logn, int fold, u64 *out, cudaStream_t s) {
     if (nd <= 0) return cudaSuccess;
-    k_diag_gather<<<diag_blocks((size_t)nd << logn), 256, 0, s>>>(vals, R, dim, reinterpret_cast<const int3 *>(desc), nd, logn, out);
+    k_diag_gather<<<diag_blocks((size_t)nd << logn), 256, 0, s>>>(vals, R, dim, reinterpret_cast<const int3 *>(desc), nd, logn, fold, out);
     return cudaGetLastError();
 }
 cudaError_t launch_diag_mac(const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B, int k, int logn,

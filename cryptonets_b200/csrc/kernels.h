@@ -239,8 +239,11 @@ cudaError_t launch_ks_mac(const u64 *digits, const u64 *key, const u64 *const *k
 // flags[b * N/2 + s] = 1 where diagonal (b, s) of the R x dim matrix whose rows' slot values are vals [R][N] has a nonzero weight
 // (flags is not cleared)
 cudaError_t launch_diag_flags(const u64 *vals, int R, int dim, int logn, unsigned *flags, cudaStream_t s);
-// out[j] (slot values [nd][N]) = diagonal (b, n1 g + h) rotated right by n1 g, desc[j] = (b, n1 g, h) as three ints (device)
-cudaError_t launch_diag_gather(const u64 *vals, int R, int dim, const int *desc, int nd, int logn, u64 *out, cudaStream_t s);
+// folded product (R <= N/2): flags[d] = 1, d < N/2, where a nonzero weight M[r, col] has col - r = d mod N/2 (flags is not cleared)
+cudaError_t launch_diag_flags_folded(const u64 *vals, int R, int dim, int logn, unsigned *flags, cudaStream_t s);
+// out[j] (slot values [nd][N]) = diagonal (b, n1 g + h) rotated right by n1 g, desc[j] = (b, n1 g, h) as three ints (device); fold = W > 0:
+// wrapped diagonal n1 g + h of fold width W (b = 0) rotated right by n1 g
+cudaError_t launch_diag_gather(const u64 *vals, int R, int dim, const int *desc, int nd, int logn, int fold, u64 *out, cudaStream_t s);
 // acc[g][b][p][l] = sum_{j = g_start[g]}^{g_start[g+1]-1} dhat[j][l] * xhat[xsel[j]][b][p][l]  (NTT form, canonical in and out; FP64 path)
 cudaError_t launch_diag_mac(const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B, int k, int logn,
                             const BehzConstF *f, cudaStream_t s);

@@ -1241,21 +1241,23 @@ extern "C" int cnhe_vec_pointwise_multiply(cnhe_ctx *h, const cnhe_vec *a, const
 }
 
 // The rotate-and-add ladder of SumAllSlots (AtomicSealBfvVector.cs:888-955) on n single-block ciphertexts in place, one key-switch wave per
-// step for all n; returns the summed length.  slots: per-ciphertext key slots (nullptr: the call's slot)
-static uint64_t sum_slots_batched(Context &c, int ch, u64 *cts, int n, uint64_t length, const int *slots = nullptr) {
+// step for all n; returns the summed length.  slots: per-ciphertext key slots (nullptr: the call's slot).  The folded diagonal product
+// starts the row steps at `first` (its fold width) and skips the column step when `columns` is false.
+static uint64_t sum_slots_batched(Context &c, int ch, u64 *cts, int n, uint64_t length, const int *slots = nullptr, uint64_t first = 1,
+                                  bool columns = true) {
     const size_t N = c.N, words = (size_t)n * c.ct_words();
     uint64_t len = length;
     u64 *tmp = c.ws_alloc(words);
     // every step is x += rotate(x): fused into the rotation (the permutation kernel folds x into the key switch's base) when the step
     // has its own Galois key -- it does for the powers of two the ladder walks -- else rotate, then add
     if (len >= N / 2) {
-        if (!op_rotate_add(c, ch, cts, n, 0, true, cts, slots)) {
+        if (columns && !op_rotate_add(c, ch, cts, n, 0, true, cts, slots)) {
             op_rotate_columns(c, ch, cts, n, tmp, slots);
             do_add(c, ch, cts, tmp, cts, words, 0);
         }
         len = N / 2;
     }
-    for (uint64_t steps = 1; steps < len; steps *= 2) { // RotateRowsAndAdd(sum, steps): RotateRows(c, -steps)
+    for (uint64_t steps = first; steps < len; steps *= 2) { // RotateRowsAndAdd(sum, steps): RotateRows(c, -steps)
         if (op_rotate_add(c, ch, cts, n, -(int)steps, false, cts, slots)) continue;
         op_rotate_rows(c, ch, cts, n, -(int)steps, tmp, slots);
         do_add(c, ch, cts, tmp, cts, words, 0);
@@ -2654,6 +2656,7 @@ extern "C" int cnhe_layer_poly(cnhe_ctx *h, const cnhe_vec *const *in, int n, co
 // ---------------------------------------------------------------------------------------------------- diagonal matrix-vector product
 // A plain matrix prepared for the diagonal (Halevi-Shoup) product with baby-step / giant-step (DESIGN.md section 4.10, slot layout in
 // diag.cu): its nonzero generalised diagonals (b, s = n1 g + h), each rotated right by n1 g and encoded, ordered by g, then b, then h.
+// A folded matrix (cnhe_diag_prepare_folded) holds its nonzero wrapped diagonals of fold width W instead, as (0, g, h).
 struct DiagEntry { int b, g, h; };
 struct cnhe_diag {
     Context *ctx = nullptr;
@@ -2661,6 +2664,7 @@ struct cnhe_diag {
     uint64_t dim = 0;
     double scale = 1.0;
     int n1 = 1, n2 = 1;
+    int fold = 0; // the fold width W of a folded matrix, else 0
     std::vector<DiagEntry> diags;
     std::vector<BufRef> plains; // per channel: [diags][N] plaintexts, coefficient form mod t
     // cnhe_diag_prepare_ntt: the first ntt_groups giant-step groups (ntt_diags diagonals) also held lifted into every q_l and in NTT form,
@@ -2706,7 +2710,9 @@ static long diag_cost(const std::vector<char> &nz, const std::vector<int> &hops,
 // diagonals lifted and forward transformed per wave: their NTT forms stay under 8 GiB (the product's waves, and the prepare's)
 static int diag_wave_cap(const Context &c) { return (int)std::max<size_t>(1, ((size_t)1 << 30) / ((size_t)c.k * c.N)); }
 
-static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, int baby_steps, uint64_t max_ntt_bytes, cnhe_diag **out) {
+// fold < 0: the generalised diagonals (cnhe_diag_prepare); fold >= 0: the wrapped diagonals of fold width `fold`, 0 letting the planner
+// choose it (cnhe_diag_prepare_folded)
+static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, int baby_steps, uint64_t max_ntt_bytes, int fold, cnhe_diag **out) {
     if (!rows || !out || n_rows < 1) fail("bad arguments");
     const size_t N = c.N;
     const int half = (int)(N / 2);
@@ -2720,6 +2726,13 @@ static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, in
     }
     if ((size_t)n_rows > N) fail("more rows than slots");
     if (baby_steps < 0 || (baby_steps & (baby_steps - 1)) || baby_steps > half) fail("baby_steps must be 0 or a power of two dividing N/2");
+    const bool folded = fold >= 0;
+    if (folded) {
+        if (n_rows > half) fail("the folded product takes at most N/2 rows");
+        if ((fold & (fold - 1)) || (fold && (fold < n_rows || fold > half))) fail("fold_width must be 0 or a power of two in [n_rows, N/2]");
+        if (fold && baby_steps > fold) fail("baby_steps must divide the fold width");
+        if (rows[0]->dim > N) fail("the folded product takes at most N columns");
+    }
     const int R = n_rows, dim = (int)rows[0]->dim;
     std::unique_ptr<cnhe_diag> d(new cnhe_diag());
     d->ctx = &c;
@@ -2738,7 +2751,8 @@ static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, in
         op_decode(c, ch, plain, R, vals[ch]->p);
         flags[ch] = c.alloc(N / 2); // N unsigned flags
         CNHE_CUDA(cudaMemsetAsync(flags[ch]->p, 0, N * sizeof(unsigned), c.stream));
-        c.check(launch_diag_flags(vals[ch]->p, R, dim, c.logN, reinterpret_cast<unsigned *>(flags[ch]->p), c.stream), "diag_flags");
+        if (folded) c.check(launch_diag_flags_folded(vals[ch]->p, R, dim, c.logN, reinterpret_cast<unsigned *>(flags[ch]->p), c.stream), "diag_flags");
+        else c.check(launch_diag_flags(vals[ch]->p, R, dim, c.logN, reinterpret_cast<unsigned *>(flags[ch]->p), c.stream), "diag_flags");
     }
     std::vector<char> nz(N, 0);
     {
@@ -2752,7 +2766,30 @@ static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, in
     }
     const std::vector<int> hops = rotation_hops(c);
     int n1 = baby_steps;
-    if (!n1) {
+    if (folded) {
+        // key switches per input of (W, n1): the BSGS rotations over the wrapped diagonals (b = 0 only), the column fold when the input
+        // reaches the second row, and log2(N/2 / W) row folds.  The fewest win; on a tie the smaller W, then the smaller n1.
+        int w_lo = fold, w_hi = fold;
+        if (!fold) {
+            for (w_lo = 1; w_lo < R; w_lo *= 2) {}
+            w_hi = half;
+        }
+        std::vector<char> nzw(N, 0), best_nz;
+        long best = -1;
+        for (int w = w_lo; w <= w_hi; w *= 2) {
+            std::fill(nzw.begin(), nzw.end(), 0);
+            for (int s = 0; s < half; s++)
+                if (nz[s]) nzw[s & (w - 1)] = 1;
+            long fixed = dim > half ? 1 : 0;
+            for (int v = w; v < half; v *= 2) fixed++;
+            for (int t = baby_steps ? baby_steps : 1; t <= (baby_steps ? baby_steps : w) && t <= w; t *= 2) {
+                const long cost = diag_cost(nzw, hops, t) + fixed;
+                if (best < 0 || cost < best) { best = cost; n1 = t; d->fold = w; best_nz = nzw; }
+            }
+        }
+        if (best < 0) fail("baby_steps must divide the fold width");
+        nz.swap(best_nz);
+    } else if (!n1) {
         long best = -1;
         for (int t = 1; t <= half; t *= 2) {
             const long cost = diag_cost(nz, hops, t);
@@ -2760,7 +2797,7 @@ static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, in
         }
     }
     d->n1 = n1;
-    d->n2 = half / n1;
+    d->n2 = (folded ? d->fold : half) / n1;
     for (int g = 0; g < d->n2; g++)
         for (int b = 0; b < 2; b++)
             for (int hh = 0; hh < n1; hh++)
@@ -2785,7 +2822,7 @@ static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, in
             WsScope wave(c);
             const int m = std::min(DW, nd - j0);
             u64 *dv = c.ws_alloc((size_t)m * N);
-            c.check(launch_diag_gather(vals[ch]->p, R, dim, ddesc + 3 * j0, m, c.logN, dv, c.stream), "diag_gather");
+            c.check(launch_diag_gather(vals[ch]->p, R, dim, ddesc + 3 * j0, m, c.logN, d->fold, dv, c.stream), "diag_gather");
             op_encode(c, ch, dv, m, (int)N, d->plains[ch]->p + (size_t)j0 * N);
         }
     }
@@ -2820,14 +2857,22 @@ static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, in
 
 extern "C" int cnhe_diag_prepare(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int baby_steps, cnhe_diag **out) {
     API_BEGIN(h)
-    diag_prepare(c, rows, n_rows, baby_steps, 0, out);
+    diag_prepare(c, rows, n_rows, baby_steps, 0, -1, out);
     API_END
 }
 
 extern "C" int cnhe_diag_prepare_ntt(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int baby_steps, uint64_t max_ntt_bytes,
                                      cnhe_diag **out) {
     API_BEGIN(h)
-    diag_prepare(c, rows, n_rows, baby_steps, max_ntt_bytes, out);
+    diag_prepare(c, rows, n_rows, baby_steps, max_ntt_bytes, -1, out);
+    API_END
+}
+
+extern "C" int cnhe_diag_prepare_folded(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int fold_width, int baby_steps,
+                                        uint64_t max_ntt_bytes, cnhe_diag **out) {
+    API_BEGIN(h)
+    if (fold_width < 0) fail("fold_width must be 0 or a power of two in [n_rows, N/2]");
+    diag_prepare(c, rows, n_rows, baby_steps, max_ntt_bytes, fold_width, out);
     API_END
 }
 
@@ -2839,6 +2884,12 @@ extern "C" int cnhe_diag_info(const cnhe_diag *d, int *n_rows, uint64_t *dim, in
     if (n2) *n2 = d->n2;
     if (n_diags) *n_diags = (int)d->diags.size();
     if (device_bytes) *device_bytes = (uint64_t)d->plains.size() * d->diags.size() * d->ctx->N * 8 + d->ntt_bytes();
+    return CNHE_OK;
+}
+
+extern "C" int cnhe_diag_fold_width(const cnhe_diag *d, int *width) {
+    if (!d || !width) return set_err(CNHE_ERR_INVALID, "null argument");
+    *width = d->fold;
     return CNHE_OK;
 }
 
@@ -2898,6 +2949,9 @@ extern "C" int cnhe_diag_destroy(cnhe_diag *d) {
 // client's inner sums in the NTT domain (k_diag_mac; dyadic products and additions off the FP64 path: the same residues), the
 // inverse transforms -- and finally the giant-step rotations of every (g, client) in one op_rotate_rows_multi and each client's sum.
 // Each inner sum equals the sum of the separate multiply_plain results, since the inverse transform is linear mod q_l.
+// A folded matrix then folds every client's sum in one wave per step -- rotate_columns when its input reaches the second row, then
+// rotate_rows by W, 2W, ..., N/4 (sum_slots_batched) -- so that slot i < n_rows holds row i's sum, and multiplies all B sums by one mask
+// plaintext (1 in slots 0 .. n_rows - 1, 0 elsewhere) that clears the periodic copies beyond them.
 extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe_vec *const *vs, int B, cnhe_vec **out) {
     API_BEGIN(h)
     if (!d || !vs || !out || B < 1) fail("bad arguments");
@@ -2932,10 +2986,16 @@ extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe
     for (int l = 0; l < k; l++) fp = fp && c.h_tabs[l].fp_ok;
     const int fpq = fp ? 1 : 0;
     std::vector<std::unique_ptr<cnhe_vec>> outs(B);
+    std::vector<BufRef> slab(c.P); // folded: the B outputs side by side, for the fold ladder and the mask
+    for (int ch = 0; ch < c.P && d->fold; ch++) {
+        c.set_channel(ch);
+        slab[ch] = c.alloc((size_t)B * ctw);
+    }
     for (int b = 0; b < B; b++) {
         outs[b].reset(new_vec(c, (uint64_t)d->n_rows, vs[0]->scale * d->scale, CNHE_DENSE, true, 1));
         outs[b]->slot = vslot[b];
-        alloc_channels(outs[b].get());
+        if (d->fold) slab_view(outs[b].get(), slab, (size_t)b);
+        else alloc_channels(outs[b].get());
     }
     // diagonals per wave: their lifted NTT forms stay under 8 GiB (a wave always takes at least one giant step); the resident groups
     // (cnhe_diag_prepare_ntt) need no such scratch and go in one wave of their own
@@ -3030,6 +3090,18 @@ extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe
             std::vector<const u64 *> terms;
             for (int gi = 0; gi < ng; gi++) terms.push_back(acc + ((size_t)gi * B + b) * ctw);
             do_add_many(c, ch, terms, outs[b]->ptr(ch));
+        }
+        if (d->fold) {
+            u64 *y = slab[ch]->p;
+            sum_slots_batched(c, ch, y, B, N / 2, vslot.data(), (uint64_t)d->fold, d->dim > N / 2);
+            std::vector<u64> ones(N, 0);
+            std::fill(ones.begin(), ones.begin() + d->n_rows, 1);
+            u64 *mv = c.ws_alloc(N), *mask = c.ws_alloc(N);
+            c.h2d(mv, ones.data(), N * 8);
+            op_encode(c, ch, mv, 1, (int)N, mask);
+            std::vector<const u64 *> cts(B);
+            for (int b = 0; b < B; b++) cts[b] = y + (size_t)b * ctw;
+            op_multiply_plain_dense_outer(c, ch, cts, mask, 1, y);
         }
     }
     for (int b = 0; b < B; b++) out[b] = outs[b].release();

@@ -1,7 +1,7 @@
 """Exact (mod t) numpy model of the diagonal matrix-vector product with baby-step / giant-step (cnhe_mat_mul_diagonal, DESIGN.md
 section 4.10), on a ciphertext's slot semantics: N slots as two rows of N/2, rotate_rows(s) moves column x + s of both rows to column x,
 rotate_columns swaps the rows.  It also restates the library's choice of the number of baby steps n1, so that both can be checked without
-a GPU."""
+a GPU.  The folded product for matrices with few rows (cnhe_diag_prepare_folded) is modelled the same way, with its planner."""
 import numpy as np
 
 
@@ -119,4 +119,82 @@ def product(diags, v, N, n1, t):
     y = np.zeros(N, dtype=np.int64)
     for g, acc in inner.items():
         y = (y + rotate_rows(acc, n1 * g)) % t
+    return y
+
+
+def folded_flags(M, N):
+    """nz[d], d < N/2: whether some nonzero weight M[r, col] has col - r = d mod N/2 (what the prepare's flags pass marks).  Wrapped
+    diagonal j of fold width W is nonzero exactly when nz[d] holds for some d = j mod W."""
+    half = N // 2
+    r, col = np.nonzero(np.asarray(M))
+    nz = np.zeros(half, bool)
+    nz[(col - r) % half] = True
+    return nz
+
+
+def wrapped_flags(nz, W):
+    """[2][N/2] flags in key_switch_cost's layout (b = 0 only) of the wrapped diagonals of fold width W."""
+    half = len(nz)
+    out = np.zeros((2, half), bool)
+    for d in np.nonzero(nz)[0]:
+        out[0, d % W] = True
+    return out
+
+
+def folded_cost(nz, hops, W, n1, dim):
+    """Key switches per input of the folded product: the BSGS rotations, the column fold when dim > N/2, and log2(N/2 / W) row folds."""
+    half = len(hops)
+    return key_switch_cost(wrapped_flags(nz, W), hops, n1) + (1 if dim > half else 0) + (half // W).bit_length() - 1
+
+
+def plan_folded(M, N, galois_elts, fold_width=0, baby_steps=0):
+    """The library's (W, n1, key switches): the fewest key switches over the powers of two R <= W <= N/2 (or the given W) and n1 dividing
+    W (or the given n1); on a tie the smaller W, then the smaller n1."""
+    half = N // 2
+    R, dim = np.asarray(M).shape
+    nz = folded_flags(M, N)
+    hops = rotation_hops(N, galois_elts)
+    ws = [fold_width] if fold_width else [w for w in (1 << i for i in range(half.bit_length())) if R <= w <= half]
+    best = None
+    for W in ws:
+        for n1 in ([baby_steps] if baby_steps else [1 << i for i in range(W.bit_length())]):
+            if n1 > W:
+                continue
+            cost = folded_cost(nz, hops, W, n1, dim)
+            if best is None or cost < best[2]:
+                best = (W, n1, cost)
+    return best
+
+
+def folded_diagonals(M, N, W, n1, t):
+    """{(0, g, h): slot vector} of the nonzero wrapped diagonals E_{n1 g + h}[(a, x)] = M[x mod W, a N/2 + (x + n1 g + h mod N/2)], each
+    rotated right by n1 g, mod t (what cnhe_diag_prepare_folded encodes)."""
+    half = N // 2
+    M = np.asarray(M, dtype=np.int64) % t
+    R, dim = M.shape
+    Mt = np.zeros((half, N), dtype=np.int64)
+    Mt[:R, :dim] = M
+    nz = wrapped_flags(folded_flags(M, N), W)[0]
+    i = np.arange(N)
+    a, x = i // half, i % half
+    out = {}
+    for j in range(W):
+        if nz[j]:
+            g, h = divmod(j, n1)
+            out[(0, g, h)] = Mt[(x - n1 * g) % W, a * half + (x + h) % half]
+    return out
+
+
+def folded_product(diags, v, N, W, n1, R, dim, t):
+    """The folded product: the BSGS sum over the stored diagonals, the column fold when dim > N/2, the row folds by W, 2W, ..., N/4 and the
+    mask of slots 0 .. R - 1, mod t."""
+    half = N // 2
+    y = product(diags, v, N, n1, t)
+    if dim > half:
+        y = (y + rotate_columns(y)) % t
+    s = W
+    while s < half:
+        y = (y + rotate_rows(y, s)) % t
+        s *= 2
+    y[R:] = 0
     return y

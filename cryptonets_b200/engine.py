@@ -127,6 +127,12 @@ class Diag:
         check(self.eng.L.cnhe_diag_info(self.h, C.byref(r), C.byref(dim), C.byref(n1), C.byref(n2), C.byref(nd), C.byref(nb)))
         return dict(n_rows=r.value, dim=dim.value, n1=n1.value, n2=n2.value, n_diags=nd.value, device_bytes=nb.value)
 
+    def fold_width(self):
+        """The fold width W of a matrix from Engine.diag_prepare(fold_width=...), 0 for an unfolded one."""
+        w = C.c_int()
+        check(self.eng.L.cnhe_diag_fold_width(self.h, C.byref(w)))
+        return w.value
+
     def export(self, channel, index):
         """(plaintext coefficients mod t [N], (b, g, h)) of stored diagonal `index` (stored by g, then b, then h)."""
         out = np.zeros(self.eng.N, np.uint64)
@@ -624,13 +630,20 @@ class Engine:
         check(self.L.cnhe_mat_mul_rowmajor_shard(self.h, _vec_array(rows), len(rows), v.h, int(force_dense), int(first_row), int(total_rows), C.byref(out)))
         return Vec(self, out)
 
-    def diag_prepare(self, rows, baby_steps=0, ntt_bytes=0):
+    def diag_prepare(self, rows, baby_steps=0, ntt_bytes=0, fold_width=None):
         """The plain row vectors of a matrix (as mat_mul_rowmajor takes them) prepared for mat_mul_diagonal; baby_steps = 0 lets the library
         pick n1.  ntt_bytes: device memory the matrix may spend on holding the longest prefix of whole giant-step groups in NTT form, so
         that mat_mul_diagonal skips their lift and transforms (same outputs); 0 holds none, None (or 2**64 - 1) the whole matrix.  The rows
-        may be disposed afterwards."""
+        may be disposed afterwards.  fold_width: None prepares the generalised diagonals (cnhe_diag_prepare); an int prepares the folded
+        product for few rows (cnhe_diag_prepare_folded: at most N/2 rows, a power-of-two fold width in [rows, N/2], 0 lets the library
+        choose it), whose outputs are dense of dim len(rows)."""
         out = C.c_void_p()
-        if ntt_bytes == 0:
+        if fold_width is not None:
+            budget = (1 << 64) - 1 if ntt_bytes is None else int(ntt_bytes)
+            if not 0 <= budget < 1 << 64:
+                raise ValueError("ntt_bytes must be None or in [0, 2**64)")
+            check(self.L.cnhe_diag_prepare_folded(self.h, _vec_array(rows), len(rows), int(fold_width), int(baby_steps), budget, C.byref(out)))
+        elif ntt_bytes == 0:
             check(self.L.cnhe_diag_prepare(self.h, _vec_array(rows), len(rows), int(baby_steps), C.byref(out)))
         else:
             budget = (1 << 64) - 1 if ntt_bytes is None else int(ntt_bytes)
@@ -641,7 +654,7 @@ class Engine:
 
     def mat_mul_diagonal(self, diag, vs):
         """The diagonal product of a prepared matrix with every encrypted vector of vs (one per client; their key slots may differ): each
-        output decrypts to mat_mul_rowmajor(rows, v, force_dense=True)."""
+        output decrypts to mat_mul_rowmajor(rows, v, force_dense=True) (a folded matrix: dense of dim len(rows), slot i row i's sum)."""
         B = len(vs)
         out = (VECP * B)()
         check(self.L.cnhe_mat_mul_diagonal(self.h, diag.h, _vec_array(vs), B, out))

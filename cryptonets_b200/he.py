@@ -190,13 +190,14 @@ class B200BfvMatrix:
             raise Exception("Internal probloem: expecting the output to be dense")
         return total
 
-    def PrepareDiagonal(self, baby_steps=0, ntt_bytes=0):
+    def PrepareDiagonal(self, baby_steps=0, ntt_bytes=0, fold_width=None):
         """This plain row-major matrix prepared for the diagonal (baby-step / giant-step) product, B200BfvFactory.MulDiagonalBatch; the
         rows stay owned by this matrix.  baby_steps = 0 picks the number of baby steps with the fewest key switches.  ntt_bytes: device
-        memory to spend on holding diagonals in NTT form (Engine.diag_prepare; 0 none, None all), same products, faster."""
+        memory to spend on holding diagonals in NTT form (Engine.diag_prepare; 0 none, None all), same products, faster.  fold_width: None
+        for the generalised diagonals, else the folded product for few rows (0 lets the library choose the width)."""
         if self.Format != EMatrixFormat.RowMajor:
             raise Exception("the diagonal product expects a RowMajor matrix")
-        return B200BfvDiagonalMatrix(self.factory, self.eng.diag_prepare([r.vec for r in self.vectors], baby_steps, ntt_bytes))
+        return B200BfvDiagonalMatrix(self.factory, self.eng.diag_prepare([r.vec for r in self.vectors], baby_steps, ntt_bytes, fold_width))
 
     def _check(self, m):
         if m.Format != self.Format:
@@ -275,6 +276,9 @@ class B200BfvDiagonalMatrix:
 
     def NttInfo(self):
         return self.diag.ntt_info()
+
+    def FoldWidth(self):
+        return self.diag.fold_width()
 
     def ExportNtt(self, channel, index):
         return self.diag.export_ntt(channel, index)

@@ -602,10 +602,12 @@ class LLDenseLayer(BaseLayer):
         self.Shard = None  # (rank, world, process group): split the rows of this layer over the ranks of ONE inference (SURVEY.md 8e)
         # "rows": the reference's product (per row a multiply, SumAllSlots and a one-hot mask); "diagonal": the baby-step / giant-step
         # diagonal product (DESIGN.md section 4.10), same decrypted output, ForceDenseFormat with a dense input only, no Shard.  The Raw
-        # backend computes M v directly either way.
+        # backend computes M v directly either way.  "folded": the folded diagonal product for layers with few rows (DESIGN.md section
+        # 4.10, cnhe_diag_prepare_folded), a dense input with or without ForceDenseFormat, no Shard; its output is always dense of dim
+        # len(Bias), and so is the Raw backend's.
         self.Method = "rows"
         self.DiagonalMatrix = None
-        # "diagonal" only: device bytes the prepared matrix may spend on holding giant-step groups of its diagonals in NTT form, so that
+        # "diagonal" and "folded" only: device bytes the prepared matrix may spend on holding giant-step groups of its diagonals in NTT form, so that
         # each product skips their lift and forward transforms (bit-identical outputs); 0 holds none, None the whole matrix.  The Raw
         # backend ignores it.
         self.DiagonalNttBytes = 0
@@ -620,14 +622,16 @@ class LLDenseLayer(BaseLayer):
             return
         if self.ForceDenseFormat and self.InputFormat == EVectorFormat.sparse:
             raise Exception("forcing dense format is only available when the input is dense")
-        if self.Method not in ("rows", "diagonal"):
+        if self.Method not in ("rows", "diagonal", "folded"):
             raise Exception("unknown dense layer method %r" % (self.Method,))
         if self.Method == "diagonal" and not (self.ForceDenseFormat and self.InputFormat == EVectorFormat.dense):
             raise Exception("the diagonal method needs ForceDenseFormat and a dense input")
-        if self.Method == "diagonal" and self.Shard is not None:
-            raise Exception("the diagonal method cannot be combined with Shard")
-        if self.DiagonalNttBytes != 0 and self.Method != "diagonal":
-            raise Exception("DiagonalNttBytes needs the diagonal method")
+        if self.Method == "folded" and self.InputFormat != EVectorFormat.dense:
+            raise Exception("the folded method needs a dense input")
+        if self.Method != "rows" and self.Shard is not None:
+            raise Exception("the %s method cannot be combined with Shard" % self.Method)
+        if self.DiagonalNttBytes != 0 and self.Method == "rows":
+            raise Exception("DiagonalNttBytes needs the diagonal or the folded method")
         if self.DiagonalNttBytes is not None and not 0 <= self.DiagonalNttBytes < 1 << 64:
             raise Exception("DiagonalNttBytes must be None or a byte count in [0, 2**64)")
         f = self.Factory
@@ -641,19 +645,23 @@ class LLDenseLayer(BaseLayer):
         else:
             self.Shard = None
         if self.InputFormat == EVectorFormat.dense:
-            self.BiasVector = f.GetPlainVector(np.asarray(self.Bias), EVectorFormat.dense if self.ForceDenseFormat else EVectorFormat.sparse, bscale)
+            self.BiasVector = f.GetPlainVector(np.asarray(self.Bias), EVectorFormat.dense if self._dense_out() else EVectorFormat.sparse, bscale)
             self.WeightsMatrix = f.GetPlainMatrix(w, EMatrixFormat.RowMajor, self.WeightsScale)
         else:
             self.BiasVector = f.GetPlainVector(np.asarray(self.Bias), EVectorFormat.dense, bscale)
             self.WeightsMatrix = f.GetPlainMatrix(w, EMatrixFormat.ColumnMajor, self.WeightsScale)
-        if self.Method == "diagonal" and hasattr(self.WeightsMatrix, "PrepareDiagonal"):
-            self.DiagonalMatrix = self.WeightsMatrix.PrepareDiagonal(ntt_bytes=self.DiagonalNttBytes)
+        if self.Method != "rows" and hasattr(self.WeightsMatrix, "PrepareDiagonal"):
+            fold = 0 if self.Method == "folded" else None
+            self.DiagonalMatrix = self.WeightsMatrix.PrepareDiagonal(ntt_bytes=self.DiagonalNttBytes, fold_width=fold)
             self.WeightsMatrix.Dispose()  # the diagonals replace the row plaintexts
             self.WeightsMatrix = None
         self.layerPrepared = True
 
     def OutputDimension(self):
         return len(self.Bias)
+
+    def _dense_out(self):
+        return self.ForceDenseFormat or self.Method == "folded"
 
     def Apply(self, m):
         if m.ColumnCount > 1:
@@ -673,7 +681,7 @@ class LLDenseLayer(BaseLayer):
             if mul is not part:
                 part.Dispose()
         else:
-            mul = self.WeightsMatrix.Mul(m.GetColumn(0), env, self.ForceDenseFormat)
+            mul = self.WeightsMatrix.Mul(m.GetColumn(0), env, self._dense_out())
         res = mul.Add(self.BiasVector, env)
         mul.Dispose()
         return self.Factory.GetMatrix([res], EMatrixFormat.ColumnMajor, CopyVectors=False)
@@ -694,7 +702,7 @@ class LLDenseLayer(BaseLayer):
             return super().ApplyBatch(ms)
         env = f.AllocateComputationEnv()
         out = []
-        for mul in batch(self.WeightsMatrix, [m.GetColumn(0) for m in ms], self.ForceDenseFormat):
+        for mul in batch(self.WeightsMatrix, [m.GetColumn(0) for m in ms], self._dense_out()):
             out.append(f.GetMatrix([mul.Add(self.BiasVector, env)], EMatrixFormat.ColumnMajor, CopyVectors=False))
             mul.Dispose()
         return out

@@ -76,7 +76,9 @@ def cryptonets_mnist(factory, images, batch_size=None, fused=True, weights=None,
     return net, reader
 
 
-def lola_small(factory, images, weights=None):
+def lola_small(factory, images, weights=None, dense_method="rows"):
+    """dense_method: LLDenseLayer.Method of the 10 x 845 score layer ("rows", the reference's, or "folded": dense scores in one
+    ciphertext per plaintext prime)."""
     w = weights or lola_small_weights()
     weightscale = 64
     reader = LLConvReader(images, Scale=16.0, NormalizationFactor=1.0 / 256.0, InputShape=[28, 28], KernelShape=[5, 5], Stride=[2, 2],
@@ -86,7 +88,7 @@ def lola_small(factory, images, weights=None):
                         WeightsScale=weightscale, Weights=w["Weights_0"])
     vec2 = LLVectorizeLayer(Source=conv1)
     act3 = SquareActivation(Source=vec2)
-    dense4 = LLDenseLayer(Source=act3, Bias=w["Biases_1"], Weights=w["Weights_1"], WeightsScale=weightscale)
+    dense4 = LLDenseLayer(Source=act3, Bias=w["Biases_1"], Weights=w["Weights_1"], WeightsScale=weightscale, Method=dense_method)
     return dense4, reader
 
 
@@ -179,10 +181,11 @@ def synthetic_cifar(n_images, seed=20240917):
     return np.random.default_rng(seed).integers(0, 256, (n_images, 3 * 32 * 32)).astype(np.float64)
 
 
-def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", diag_ntt_bytes=0):
+def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows"):
     """LoLa-CIFAR (`CifarCryptoNet/LolaCifarCryptoNet.cs:27-131`): 3x32x32 image as an im2col matrix [196 x 192], conv 83 maps,
     square, the second convolution as a 5488 x 16268 row-major dense layer (rotate-and-sum per row), square, dense 5488 -> 10.
-    dense_method: LLDenseLayer.Method of that layer ("rows", the reference's, or "diagonal"); diag_ntt_bytes: its DiagonalNttBytes."""
+    dense_method: LLDenseLayer.Method of that layer ("rows", the reference's, or "diagonal"); diag_ntt_bytes: its DiagonalNttBytes;
+    score_method: the Method of the score layer ("rows" or "folded")."""
     w = weights or cifar_weights()
     reader = LLConvReader(images, Scale=8.0, NormalizationFactor=1.0 / 256.0, InputShape=[3, 32, 32], KernelShape=[3, 8, 8], Stride=[1000, 2, 2],
                           Upperpadding=[0, 1, 1], Lowerpadding=[0, 1, 1])
@@ -200,7 +203,8 @@ def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", d
                           InputFormat=EVectorFormat.dense, ForceDenseFormat=True, Shard=shard, Method=dense_method,
                           DiagonalNttBytes=diag_ntt_bytes)
     act5 = SquareActivation(Source=dense4)
-    dense6 = LLDenseLayer(Source=act5, Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512.0, InputFormat=EVectorFormat.dense)
+    dense6 = LLDenseLayer(Source=act5, Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512.0, InputFormat=EVectorFormat.dense,
+                          Method=score_method)
     return dense6, reader
 
 
@@ -220,11 +224,11 @@ def lola_large_weights(seed=9, synthetic=False):
                 Biases_1=draw(163, 0.039, 0.09), Weights_2=draw(10 * 2608, 0.42, 1.63), Biases_2=draw(10, 1.6, 3.9))
 
 
-def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_bytes=0):
+def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows"):
     """Large LoLa (`LoLaCryptonets.cs:330-409`): 28x28 image as im2col [144 x 64], conv 83 maps of 8x8 stride 2 (pixels are NOT
     normalised; the weights carry the 1/256), square, the second convolution (163 maps of 83x6x6, stride 2 over 83x12x12) as a
     2608 x 11952 row-major dense layer with ForceDenseFormat, square, dense 2608 -> 10.  dense_method: that layer's LLDenseLayer.Method,
-    diag_ntt_bytes its DiagonalNttBytes."""
+    diag_ntt_bytes its DiagonalNttBytes; score_method: the Method of the score layer ("rows" or "folded")."""
     w = weights or lola_large_weights()
     reader = LLConvReader(images, Scale=16.0, NormalizationFactor=1.0, InputShape=[1, 28, 28], KernelShape=[1, 8, 8], Stride=[1000, 2, 2],
                           Upperpadding=[0, 1, 1], Lowerpadding=[0, 1, 1])
@@ -240,5 +244,6 @@ def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_byte
                           InputFormat=EVectorFormat.dense, ForceDenseFormat=True, Method=dense_method,
                           DiagonalNttBytes=diag_ntt_bytes)
     act5 = SquareActivation(Source=dense4)
-    dense6 = LLDenseLayer(Source=act5, Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512, InputFormat=EVectorFormat.dense)
+    dense6 = LLDenseLayer(Source=act5, Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512, InputFormat=EVectorFormat.dense,
+                          Method=score_method)
     return dense6, reader

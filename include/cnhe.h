@@ -1,7 +1,7 @@
 /*
  * cnhe.h -- C ABI of libcnhe.so, the H100-native BFV engine behind the CryptoNets plugin API.
  *
- * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these entry points
+ * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these 110 entry points
  * with [DllImport("cnhe")] (stub in INTEGRATION.md); the Python mirror in cryptonets_b200/ binds them with ctypes.
  * One cnhe_vec is one reference `EncryptedSealBfvVector` ("HE Wrapper/EncryptedSealBfvVector.cs:150-573"): P
  * plaintext-modulus channels, each an `AtomicSealBfvEncryptedVector` ("HE Wrapper/AtomicSealBfvVector.cs:303-1476")
@@ -293,7 +293,20 @@ int cnhe_mat_dot_rows_batch(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows,
  *   The coefficient-form diagonals stay (cnhe_diag_export is unchanged); device_bytes of cnhe_diag_info counts both forms.
  * cnhe_diag_ntt_info: resident giant-step groups, resident diagonals and the device bytes of their NTT forms (any pointer may be NULL).
  * cnhe_diag_export_ntt: the k N resident words of stored diagonal `index` of a channel ([k][N]); an index outside the resident prefix,
- *   a bad channel, cap_words < k N or another context's matrix is CNHE_ERR_INVALID. */
+ *   a bad channel, cap_words < k N or another context's matrix is CNHE_ERR_INVALID.
+ * cnhe_diag_prepare_folded: the folded (hybrid) diagonal product for matrices with few rows, R = n_rows <= N/2 and dim <= N; with
+ *   n = N/2 and fold width W (a power of two, R <= W <= n) it keeps the W wrapped diagonals
+ *     E_j[(a, x)] = M[x mod W, a n + (x + j mod n)]   (0 where the row is >= R or the column >= dim), j = n1 g + h < W,
+ *   each rotated right by n1 g and stored as (b, g, h) = (0, g, h), all-zero ones dropped.  cnhe_mat_mul_diagonal then computes
+ *     y' = sum_g rotate_rows(n1 g)( sum_h E'_{n1 g + h} (.) rotate_rows(h)(v) ),  y' += rotate_columns(y') when dim > n,
+ *     y' += rotate_rows(s)(y') for s = W, 2W, ..., n/2,  y = mask_R (.) y'   (mask_R: 1 in slots 0 .. R-1, 0 elsewhere),
+ *   so out[b] is dense of dim R (slot i = row i's sum, every other slot 0): one ciphertext per plaintext prime.  fold_width = 0 and / or
+ *   baby_steps = 0 let the library choose W and / or n1 with the fewest key switches per input (BSGS rotations counted as for
+ *   cnhe_diag_prepare, plus one when dim > n, plus log2(n / W)); on a tie the smaller W, then the smaller n1.  max_ntt_bytes as for
+ *   cnhe_diag_prepare_ntt.  R > n, dim > N, a W that is not 0 or a power of two in [R, n], an n1 that does not divide W and whatever
+ *   cnhe_diag_prepare refuses are CNHE_ERR_INVALID.  cnhe_diag_info reports n2 = W / n1; the export calls work unchanged (b = 0).
+ *   Counted as the unfolded product, plus the fold's hops, column rotations and additions and one plain multiplication per output.
+ * cnhe_diag_fold_width: W of a folded matrix, 0 for one from cnhe_diag_prepare or cnhe_diag_prepare_ntt. */
 typedef struct cnhe_diag cnhe_diag;
 int cnhe_diag_prepare(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, int baby_steps, cnhe_diag **out);
 int cnhe_diag_prepare_ntt(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, int baby_steps, uint64_t max_ntt_bytes, cnhe_diag **out);
@@ -303,6 +316,9 @@ int cnhe_diag_export(cnhe_ctx *, const cnhe_diag *, int channel, int index, uint
 int cnhe_diag_export_ntt(cnhe_ctx *, const cnhe_diag *, int channel, int index, uint64_t *dst /* k*N */, size_t cap_words);
 int cnhe_diag_destroy(cnhe_diag *);
 int cnhe_mat_mul_diagonal(cnhe_ctx *, const cnhe_diag *, const cnhe_vec *const *vs, int B, cnhe_vec **out /*B*/);
+int cnhe_diag_prepare_folded(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, int fold_width, int baby_steps, uint64_t max_ntt_bytes,
+                             cnhe_diag **out);
+int cnhe_diag_fold_width(const cnhe_diag *, int *width);
 /* Whole PoolLayer.Apply with weights ("NeuralNetworks/PoolLayer.cs:149-229"): out[m] = sum_k weights[m][k] * in[gather[m*K+k]]
  * + bias[m].  The inputs may belong to different key slots (several clients' images side by side) as long as each output's taps share
  * one; the output takes it.  weights[m] is a plain SPARSE vector of dim K, bias[m] a plain DENSE vector (or NULL); gather < 0 is a

@@ -106,6 +106,8 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_diag_ntt_info(IntPtr a0, out int resident_giant_steps, out int resident_diags, out ulong ntt_bytes);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_diag_export_ntt(IntPtr a0, IntPtr diag, int channel, int index, ulong[] dst, UIntPtr cap_words);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_diagonal(IntPtr a0, IntPtr diag, IntPtr[] vs, int B, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_diag_prepare_folded(IntPtr a0, IntPtr[] rows, int n_rows, int fold_width, int baby_steps, ulong max_ntt_bytes, out IntPtr @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_diag_fold_width(IntPtr a0, out int width);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_conv_dense(IntPtr a0, IntPtr[] @in, int n_in, int[] gather, IntPtr[] weights, IntPtr[] bias, int M, int K, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_square(IntPtr a0, IntPtr[] @in, int n, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_poly2(IntPtr a0, IntPtr[] @in, int n, IntPtr a, IntPtr b, IntPtr c, IntPtr[] @out);

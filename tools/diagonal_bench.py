@@ -9,7 +9,9 @@ call per profiler family (cnhe_prof_collect; the lift is booked as "other", the 
 its time give dense4_mac_GBps).  diagonal_ntt@D runs the NTT-form arm with the option diag_mac_resident = D (0: k_diag_mac), so the
 MAC kernels can be alternated.  held_bytes is the prepared matrix's device_bytes (both forms), coeff_bytes / ntt_bytes its parts.  Full residency takes about
 39 GB for LoLa-CIFAR and 46 GB for LoLa-Large: run one network per process.  Then the diagonal method at the reference's SmallModulusCount: whether the
-scores decrypt, and the budget entering the last layer.  Prints one JSON line per measurement (and writes them to --out if given)."""
+scores decrypt, and the budget entering the last layer.  --score-methods alternates the Method of the score layer (dense6: "rows", the
+reference's, and / or "folded") within every dense4 method; each record has dense6's time, its key switches and the bytes of the score
+ciphertexts.  Prints one JSON line per measurement (and writes them to --out if given)."""
 import argparse
 import json
 import os
@@ -58,7 +60,7 @@ def mem_used_mb():
         return None
 
 
-def run(f, name, method, imgs, batch8, ntt_bytes=None):
+def run(f, name, method, imgs, batch8, ntt_bytes=None, score_method="rows"):
     """method: rows, diagonal, or diagonal_ntt[@D] (D = the option diag_mac_resident: 2, 4, 8, or 0 for k_diag_mac)."""
     eng = f.engine
     diag = method != "rows"
@@ -66,7 +68,7 @@ def run(f, name, method, imgs, batch8, ntt_bytes=None):
     eng.set_option("diag_mac_resident", int(depth) if depth else 2)
     eng.set_option("release_cached_memory", 1)  # the previous arm's scratch goes back to the driver before this arm's matrix
     kw = dict(diag_ntt_bytes=ntt_bytes) if base == "diagonal_ntt" else {}
-    net, rd = getattr(nw, name)(f, imgs, dense_method="diagonal" if diag else "rows", **kw)
+    net, rd = getattr(nw, name)(f, imgs, dense_method="diagonal" if diag else "rows", score_method=score_method, **kw)
     layers = chain(net)
     D = 5  # reader, encrypt, pool, vectorize, square, dense4, square, dense
     for L in layers[1:]:
@@ -87,16 +89,21 @@ def run(f, name, method, imgs, batch8, ntt_bytes=None):
     mem_after_prepare = mem_used_mb()
     m = rd.GetNext()
     eng.op_counts(reset=True)
-    total, dense4 = 0.0, 0.0
+    total, dense4, dense6, ks6 = 0.0, 0.0, 0.0, 0
     for i, L in enumerate(layers[1:], 1):
         if i == D:  # one untimed dense4 first: its scratch comes from the driver once, not inside the timed call
             L.Apply(m).Dispose()
+        if i == len(layers) - 1:
+            ks6 = key_switches(eng.op_counts())
         eng.sync()
         t0 = time.perf_counter()
         m2 = L.Apply(m)
         eng.sync()
         dt = time.perf_counter() - t0
         total += dt
+        if i == len(layers) - 1:
+            dense6 = dt
+            ks6 = key_switches(eng.op_counts()) - ks6
         if i == D:
             dense4 = dt
             x4 = m  # dense4's input (kept for the batched call)
@@ -104,7 +111,9 @@ def run(f, name, method, imgs, batch8, ntt_bytes=None):
             m.Dispose()
         m = m2
     ks = key_switches(eng.op_counts())
-    rec = dict(net=name, method=method, k=len(eng.q), s_per_image=total, dense4_s=dense4, key_switches=ks, prepare_s=prep,
+    score_bytes = sum(v.vec.blocks for v in m.vectors) * eng.P * 2 * len(eng.q) * eng.N * 8
+    rec = dict(net=name, method=method, score_method=score_method, k=len(eng.q), s_per_image=total, dense4_s=dense4, dense6_s=dense6,
+               dense6_key_switches=ks6, score_bytes=score_bytes, key_switches=ks, prepare_s=prep,
                held_bytes=held, coeff_bytes=coeff_held, ntt_bytes=ntt_held, device_mem_used_mb_after_prepare=mem_after_prepare)
     if diag:
         eng.sync()
@@ -138,6 +147,7 @@ def main():
     ap.add_argument("--ntt-bytes", type=int, default=None, help="diagonal_ntt's budget in bytes (default: the whole matrix; LoLa-Large "
                     "wholly resident ran out of memory on an 80 GB H100; 34359738368 = 32 GiB works)")
     ap.add_argument("--methods", default="rows,diagonal,diagonal_ntt")
+    ap.add_argument("--score-methods", default="rows")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     recs = [dict(gpu=gpu_info())]
@@ -151,17 +161,18 @@ def main():
         f = B200BfvFactory(primes, 16384, DecompositionBitCount=60, GaloisDecompositionBitCount=60, SmallModulusCount=kref + 1, seed=5)
         for rep in range(a.reps):
             for method in a.methods.split(","):
-                try:
-                    rec, got = run(f, name, method, imgs, batch8=True, ntt_bytes=a.ntt_bytes)
-                except CnheError as e:  # e.g. a budget the card cannot hold next to the rest of the network
-                    rec = dict(net=name, method=method, rep=rep, error=str(e), device_mem_used_mb=mem_used_mb())
+                for score_method in a.score_methods.split(","):
+                    try:
+                        rec, got = run(f, name, method, imgs, batch8=True, ntt_bytes=a.ntt_bytes, score_method=score_method)
+                    except CnheError as e:  # e.g. a budget the card cannot hold next to the rest of the network
+                        rec = dict(net=name, method=method, score_method=score_method, rep=rep, error=str(e), device_mem_used_mb=mem_used_mb())
+                        recs.append(rec)
+                        print(json.dumps(rec), flush=True)
+                        continue
+                    rec["rep"] = rep
+                    rec["scores_equal_raw"] = bool(np.allclose(got, want, rtol=1e-9, atol=1e-9))
                     recs.append(rec)
                     print(json.dumps(rec), flush=True)
-                    continue
-                rec["rep"] = rep
-                rec["scores_equal_raw"] = bool(np.allclose(got, want, rtol=1e-9, atol=1e-9))
-                recs.append(rec)
-                print(json.dumps(rec), flush=True)
         f.Dispose()
         if a.skip_reference_count:
             continue
