@@ -108,6 +108,8 @@ _SIGS = {
     "cnhe_layer_square": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP)],
     "cnhe_layer_poly2": [C.c_void_p, C.POINTER(VECP), i32, VECP, VECP, VECP, C.POINTER(VECP)],
     "cnhe_layer_poly": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP), i32, C.POINTER(VECP)],
+    "cnhe_layer_activation_conv_dense": [C.c_void_p, C.POINTER(VECP), i32, VECP, VECP, VECP, C.POINTER(C.c_int32), C.POINTER(VECP),
+                                         C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_dev_alloc": [C.c_void_p, sz, U64P],
     "cnhe_dev_free": [C.c_void_p, u64],
     "cnhe_dev_upload": [C.c_void_p, u64, U64P, sz],

@@ -186,6 +186,7 @@ cudaError_t launch_galois_gather(const u64 *const *in_ptrs, u64 *out_base, u64 *
                                  cudaStream_t s);
 
 // ---- K4: out[m] = sum_k w[m][k] * in[gather[m][k]] (+ Delta*bias[m] on coefficient 0 of c0)
+// polys: polynomials per ciphertext, 2, or 3 for size-3 products (the sum is linear in each polynomial); every MAC launcher takes it
 struct MacTile {
     int n_out;       // outputs in this tile (<= 8) sharing one gather row
     int gather_row;  // row index into gather[] (K entries)
@@ -193,11 +194,12 @@ struct MacTile {
 };
 // w_ptrs[m]: K weights mod t (device); bias[m] mod t or null
 cudaError_t launch_mac_layer(const u64 *const *in_ptrs, const int *gather, const MacTile *tiles, int n_tiles, const u64 *const *w_ptrs,
-                             const u64 *bias, int K, u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
+                             const u64 *bias, int K, u64 *const *out_ptrs, int polys, int k, int logn, const BehzConst *bc, PlainConst pc,
+                             cudaStream_t s);
 
 // small-weight variant: wd[m*K + kk] = signed weight as an exact double (|w| < 2^17 and K*|w|*2^26 < 2^52, host-checked)
 cudaError_t launch_mac_layer_fp(const u64 *const *in_ptrs, const int *gather, const MacTile *tiles, int n_tiles, const double *wd, const u64 *bias,
-                                int K, u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
+                                int K, u64 *const *out_ptrs, int polys, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
 
 // ---- K5: BEHZ multiply pieces
 // in: ct pointers (each [2][k][N]); out together layout [n][2][k+kb][N] (q residues copied, then Bsk residues)
@@ -260,7 +262,7 @@ enum SampleKind { SAMPLE_TERNARY = 0, SAMPLE_NOISE = 1, SAMPLE_UNIFORM = 2 };
 // limbs = ceil(bits(q)/8); needs K*254*255 < 2^31 and every coefficient prime below 2^50 (the limb sums are joined modulo q_l in FP64:
 // (double)p must be exact and fcanon_u's input below 2^51; wider moduli belong to the 128-bit launch_mac_layer)
 cudaError_t launch_mac_dense_imma(const u64 *const *in_ptrs, const void *wfrag, const void *wfrag2, const u64 *bias, int K, int M, int limbs,
-                                  u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
+                                  u64 *const *out_ptrs, int polys, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
 // Scalar-MAC layers on wgmma (mac_umma.cu).  The layer's inputs are rows of one slab (input i at slab + i * slab_stride_words); a
 // BUNDLE is up to 128 outputs whose taps lie in a window of consecutive inputs: chunk j of the bundle multiplies the 32 inputs that start
 // at row chunk_rows[chunk0 + j] (bit 30 set: a row of the scratch slab that holds the W2 taps) with the 128 x 32 weight block at
@@ -273,7 +275,7 @@ struct UmmaLaunch {
     const u64 *slab;            // input 0
     size_t slab_stride_words;   // distance between consecutive inputs
     size_t slab_rows;           // number of inputs
-    const u64 *scratch;         // W2 taps gathered side by side (ct_words apart), or null
+    const u64 *scratch;         // W2 taps gathered side by side (polys * k * N words apart), or null
     size_t scratch_rows;
     const UmBundle *bundles;    // device
     int n_bundles;
@@ -284,7 +286,7 @@ struct UmmaLaunch {
     u64 *const *out_ptrs;       // device, bundle order
     const u64 *bias;            // device, bundle order; null = no constant bias
     int n_out_total;
-    int limbs, k, logn;
+    int limbs, polys, k, logn;  // polys: 2, or 3 for size-3 inputs (slab_stride_words >= 3kN)
     const BehzConst *bc;
     PlainConst pc;
 };

@@ -144,19 +144,19 @@ __global__ void __launch_bounds__(256, 2) k_mac_dense_imma(const u64 *const *__r
 }
 
 template <int LIMBS>
-static void imma_go(const u64 *const *in_ptrs, const uint4 *wf, const uint4 *wf2, const u64 *bias, int K, int M, u64 *const *out_ptrs, int k, int logn,
-                    const BehzConst *bc, PlainConst pc, cudaStream_t s) {
-    const size_t ct_words = (size_t)2 * k << logn;
+static void imma_go(const u64 *const *in_ptrs, const uint4 *wf, const uint4 *wf2, const u64 *bias, int K, int M, u64 *const *out_ptrs, int polys, int k,
+                    int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {
+    const size_t ct_words = (size_t)polys * k << logn;
     dim3 grid((unsigned)(ct_words / IM_TN), (unsigned)((M + 127) / 128));
     k_mac_dense_imma<LIMBS><<<grid, 256, 0, s>>>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc);
 }
 cudaError_t launch_mac_dense_imma(const u64 *const *in_ptrs, const void *wfrag, const void *wfrag2, const u64 *bias, int K, int M, int limbs,
-                                  u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {
+                                  u64 *const *out_ptrs, int polys, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {
     const uint4 *wf = reinterpret_cast<const uint4 *>(wfrag), *wf2 = reinterpret_cast<const uint4 *>(wfrag2);
     switch (limbs) {
-    case 5: imma_go<5>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
-    case 6: imma_go<6>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
-    case 7: imma_go<7>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, k, logn, bc, pc, s); break;
+    case 5: imma_go<5>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, polys, k, logn, bc, pc, s); break;
+    case 6: imma_go<6>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, polys, k, logn, bc, pc, s); break;
+    case 7: imma_go<7>(in_ptrs, wf, wf2, bias, K, M, out_ptrs, polys, k, logn, bc, pc, s); break;
     default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();

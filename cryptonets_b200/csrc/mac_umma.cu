@@ -130,8 +130,8 @@ template <int LIMBS>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1, const UmBundle *__restrict__ bundles, int n_bundles,
            const int *__restrict__ chunk_rows, int total_chunks, const unsigned char *__restrict__ wpack, int a_bytes,
-           u64 *const *__restrict__ out_ptrs, const u64 *__restrict__ bias, int n_out_total, int k, int logn, const BehzConst *__restrict__ bc,
-           PlainConst pc, unsigned long long *prof) {
+           u64 *const *__restrict__ out_ptrs, const u64 *__restrict__ bias, int n_out_total, int polys, int k, int logn,
+           const BehzConst *__restrict__ bc, PlainConst pc, unsigned long long *prof) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char *smem = smem_raw + ((1024u - (sptr(smem_raw) & 1023u)) & 1023u);
     // CNHE_UMMA_PROF=1: CTA 0 reports, per role, the cycles spent in each of its waits and in its work (prof[role * 4 + i])
@@ -151,7 +151,7 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
     static_assert((2 * UM_RAW_STAGES + 1) * 8 <= 256, "barrier block");
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int N = 1 << logn;
-    const int n_tiles = (int)(((size_t)2 * k << logn) / UM_TN);
+    const int n_tiles = (int)(((size_t)polys * k << logn) / UM_TN);
 
     if (tid == 0) {
         for (int i = 0; i < UM_RAW_STAGES; i++) { mb_init(raw_full + i, 1); mb_init(raw_empty + i, UM_CONSUMERS); }
@@ -323,7 +323,7 @@ cudaError_t umma_go(const CUtensorMap &map0, const CUtensorMap &map1, const Umma
     const UmSmem L = um_layout(a.a_bytes, a.total_chunks, a.n_out_total, a.n_bundles, LIMBS);
     cudaError_t e = cudaFuncSetAttribute(k_mac_umma<LIMBS>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total);
     if (e != cudaSuccess) return e;
-    const int n_tiles = (int)(((size_t)2 * a.k << a.logn) / UM_TN);
+    const int n_tiles = (int)(((size_t)a.polys * a.k << a.logn) / UM_TN);
     const int grid = std::min(sm_count_cached(), n_tiles);
     const bool want_prof = getenv("CNHE_UMMA_PROF") != nullptr; // read per launch: tests switch it on to see which kernel served a layer
     unsigned long long *prof = nullptr;
@@ -334,7 +334,7 @@ cudaError_t umma_go(const CUtensorMap &map0, const CUtensorMap &map1, const Umma
         prof = buf;
     }
     k_mac_umma<LIMBS><<<grid, UM_THREADS, L.total, s>>>(map0, map1, a.bundles, a.n_bundles, a.chunk_rows, a.total_chunks, a.wpack, a.a_bytes, a.out_ptrs, a.bias,
-                                                        a.n_out_total, a.k, a.logn, a.bc, a.pc, prof);
+                                                        a.n_out_total, a.polys, a.k, a.logn, a.bc, a.pc, prof);
     if (want_prof) {
         unsigned long long h[16];
         cudaMemcpyAsync(h, prof, sizeof(h), cudaMemcpyDeviceToHost, s);
@@ -365,7 +365,7 @@ void mac_umma_pack(const signed char *w, int rows, int cols, unsigned char *out)
 }
 cudaError_t launch_mac_umma(const UmmaLaunch &a, cudaStream_t s) {
     alignas(64) CUtensorMap map0, map1;
-    const size_t ctw = (size_t)2 * a.k << a.logn;
+    const size_t ctw = (size_t)a.polys * a.k << a.logn; // words per input: the maps' width and the scratch slab's row stride
     cudaError_t e = make_word_map_2d(&map0, a.slab, ctw, a.slab_rows, a.slab_stride_words * 8, UM_TN / 2, UM_CHUNK, 1);
     if (e != cudaSuccess) return e;
     if (a.scratch_rows > 0) {

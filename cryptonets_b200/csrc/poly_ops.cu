@@ -184,11 +184,11 @@ __global__ void __launch_bounds__(256) k_galois(const u64 *__restrict__ in, cons
 constexpr int MAC_TM = 8;
 __global__ void __launch_bounds__(128) k_mac_layer(const u64 *const *__restrict__ in_ptrs, const int *__restrict__ gather,
                                                   const MacTile *__restrict__ tiles, const u64 *const *__restrict__ w_ptrs,
-                                                  const u64 *__restrict__ bias, int K, u64 *const *__restrict__ out_ptrs, int k, int logn,
-                                                  const BehzConst *__restrict__ bc, PlainConst pc) {
+                                                  const u64 *__restrict__ bias, int K, u64 *const *__restrict__ out_ptrs, int polys, int k,
+                                                  int logn, const BehzConst *__restrict__ bc, PlainConst pc) {
     const int N = 1 << logn;
     const size_t word = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 2; // two words per thread (16-byte accesses)
-    const size_t ct_words = (size_t)2 * k * N;
+    const size_t ct_words = (size_t)polys * k * N;
     if (word >= ct_words) return;
     const MacTile tile = tiles[blockIdx.y];
     const int l = (int)((word >> logn) % k);
@@ -250,13 +250,13 @@ constexpr int MAC_KC = 64; // taps staged per chunk (pointers + weights in share
 constexpr int MAC_U = 8;   // loads in flight per thread
 __global__ void __launch_bounds__(128) k_mac_layer_fp(const u64 *const *__restrict__ in_ptrs, const int *__restrict__ gather,
                                                      const MacTile *__restrict__ tiles, const double *__restrict__ wd, const u64 *__restrict__ bias,
-                                                     int K, u64 *const *__restrict__ out_ptrs, int k, int logn, const BehzConst *__restrict__ bc,
-                                                     PlainConst pc) {
+                                                     int K, u64 *const *__restrict__ out_ptrs, int polys, int k, int logn,
+                                                     const BehzConst *__restrict__ bc, PlainConst pc) {
     __shared__ const u64 *sptr[MAC_KC];
     __shared__ double sw[MAC_KC][MAC_TM];
     const int N = 1 << logn;
     const size_t word = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
-    const size_t ct_words = (size_t)2 * k * N;
+    const size_t ct_words = (size_t)polys * k * N;
     const bool active = word < ct_words;
     const size_t w_off = active ? word : 0;
     const MacTile tile = tiles[blockIdx.y];
@@ -500,19 +500,20 @@ cudaError_t launch_galois_gather(const u64 *const *in_ptrs, u64 *out_base, u64 *
     return cudaGetLastError();
 }
 cudaError_t launch_mac_layer(const u64 *const *in_ptrs, const int *gather, const MacTile *tiles, int n_tiles, const u64 *const *w_ptrs,
-                             const u64 *bias, int K, u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {
+                             const u64 *bias, int K, u64 *const *out_ptrs, int polys, int k, int logn, const BehzConst *bc, PlainConst pc,
+                             cudaStream_t s) {
     if (n_tiles <= 0) return cudaSuccess;
-    const size_t pairs = ((size_t)2 * k << logn) / 2;
+    const size_t pairs = ((size_t)polys * k << logn) / 2;
     dim3 grid(blocks_for(pairs, 128), n_tiles);
-    k_mac_layer<<<grid, 128, 0, s>>>(in_ptrs, gather, tiles, w_ptrs, bias, K, out_ptrs, k, logn, bc, pc);
+    k_mac_layer<<<grid, 128, 0, s>>>(in_ptrs, gather, tiles, w_ptrs, bias, K, out_ptrs, polys, k, logn, bc, pc);
     return cudaGetLastError();
 }
 cudaError_t launch_mac_layer_fp(const u64 *const *in_ptrs, const int *gather, const MacTile *tiles, int n_tiles, const double *wd, const u64 *bias,
-                                int K, u64 *const *out_ptrs, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {
+                                int K, u64 *const *out_ptrs, int polys, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {
     if (n_tiles <= 0) return cudaSuccess;
-    const size_t pairs = ((size_t)2 * k << logn) / 2;
+    const size_t pairs = ((size_t)polys * k << logn) / 2;
     dim3 grid(blocks_for(pairs, 128), n_tiles);
-    k_mac_layer_fp<<<grid, 128, 0, s>>>(in_ptrs, gather, tiles, wd, bias, K, out_ptrs, k, logn, bc, pc);
+    k_mac_layer_fp<<<grid, 128, 0, s>>>(in_ptrs, gather, tiles, wd, bias, K, out_ptrs, polys, k, logn, bc, pc);
     return cudaGetLastError();
 }
 cudaError_t launch_sample(u64 *out, int n, int kind, const RngKey &seed, u64 stream0, u64 stream_step, int k, int logn, const BehzConst *bc, cudaStream_t s) {

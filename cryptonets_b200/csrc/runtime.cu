@@ -1023,14 +1023,14 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
     }
     multiply_floor(c, ch, D, m, lazy, out3, epi, pa_dev, o0, pair);
 }
-void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3) {
+void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3, const FloorEpi *epi) {
     const int n = (int)a.size();
     const bool fused = mul_fused(c, a, b);
     const int wave = c.wave(mul_words(c, fused));
     for (int c0 = 0; c0 < n; c0 += wave) {
         WsScope scope(c);
         const int m = std::min(wave, n - c0);
-        multiply_chunk(c, ch, a, b, c0, m, out3 + (size_t)c0 * 3 * c.k * c.N, fused);
+        multiply_chunk(c, ch, a, b, c0, m, out3 + (size_t)c0 * 3 * c.k * c.N, fused, epi);
     }
     c.note(Context::OP_MULTIPLY, ch, n);
 }

@@ -214,7 +214,8 @@ u64 *const *upload_ptrs_mut(Context &c, const std::vector<u64 *> &ptrs);
 
 void op_ntt(Context &c, const u64 *src, u64 *dst, int n_polys, int mod_base, int mod_count, bool inverse);
 // out3[n][3][k][N] = a[i] * b[i]  (BEHZ).  a_ptrs/b_ptrs: host vectors of device ciphertext pointers.
-void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3);
+// epi (squares only): nullptr, or op_multiply_relin's floor epilogue applied to the size-3 products, A (.) a^2 + (B x0 + Delta C, B x1, 0)
+void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3, const FloorEpi *epi = nullptr);
 // Key-switching operations take the keys of ciphertext i from key slot slots[i] when a per-ciphertext slot table is given (n entries,
 // host), otherwise every ciphertext uses the call's slot c.slot.  A missing key is CNHE_ERR_STATE.
 void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots = nullptr);

@@ -1957,18 +1957,31 @@ static std::shared_ptr<UmmaPlan> umma_plan(Context &c, int ch, const std::vector
     c.umma_plans[key] = best;
     return best;
 }
-// Shared body of DenseMatrixBySparseVectorMultiply (ciphertext columns x plain constants) and of the fused PoolLayer.
-// in[n_in] encrypted dense vectors (same block count), weights[m] plain sparse of dim K, bias[m] plain dense or null.
-static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int32_t *gather, const cnhe_vec *const *weights, const cnhe_vec *const *bias,
-                      int M, int K, cnhe_vec **out) {
+// A validated scalar-MAC layer: outputs that share a gather row in tiles of 8, and the key slot of every output.  The inputs are
+// encrypted dense vectors (same block count), weights[m] plain sparse of dim K, bias[m] plain dense or null.
+struct MacLayer {
+    int n_in, M, K, bl, maxbits;
+    const int32_t *gather;
+    const cnhe_vec *const *weights, *const *bias;
+    bool const_bias;
+    std::vector<int> grows, out_slot;
+    std::vector<MacTile> tiles;
+    std::vector<std::vector<int>> row_outs; // outputs of every distinct gather row, in the order of `grows`
+};
+// in_scale: the scale of the ciphertexts the MAC sums (the inputs', or the activation's output scale when they are squared first); the
+// bias must be at in_scale times the weights' scale
+static MacLayer mac_prepare(Context &c, const cnhe_vec *const *in, int n_in, double in_scale, const int32_t *gather, const cnhe_vec *const *weights,
+                            const cnhe_vec *const *bias, int M, int K) {
     if (n_in < 1 || M < 1 || K < 1) fail("bad layer shape");
-    const int bl = in[0]->blocks;
+    MacLayer L;
+    L.n_in = n_in; L.M = M; L.K = K; L.gather = gather; L.weights = weights; L.bias = bias;
+    L.bl = in[0]->blocks;
     for (int i = 0; i < n_in; i++) {
         same_ctx(c, in[i]);
         if (!in[i]->enc || in[i]->format != CNHE_DENSE) fail("layer inputs must be encrypted dense vectors");
-        if (in[i]->blocks != bl || in[i]->dim != in[0]->dim || in[i]->scale != in[0]->scale) fail("all layer inputs must share dimension and scale");
+        if (in[i]->blocks != L.bl || in[i]->dim != in[0]->dim || in[i]->scale != in[0]->scale) fail("all layer inputs must share dimension and scale");
     }
-    bool const_bias = bias != nullptr;
+    L.const_bias = bias != nullptr;
     for (int m = 0; m < M; m++) {
         same_ctx(c, weights[m]);
         if (weights[m]->enc || weights[m]->format != CNHE_SPARSE) fail("expecting a sparse vector");
@@ -1978,73 +1991,242 @@ static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int
             if (!bias[m]) fail("null bias");
             same_ctx(c, bias[m]);
             if (bias[m]->enc || bias[m]->format != CNHE_DENSE || bias[m]->dim != in[0]->dim) fail("bias must be a plain dense vector of the input dimension");
-            if (bias[m]->scale != in[0]->scale * weights[0]->scale) fail("Scales do not match.");
-            const_bias = const_bias && bias[m]->is_const;
+            if (bias[m]->scale != in_scale * weights[0]->scale) fail("Scales do not match.");
+            L.const_bias = L.const_bias && bias[m]->is_const;
         }
     }
     // The scalar MAC is key-independent, so one call may serve several clients (their images' columns side by side, each output's
     // gather row inside one client's columns): every output takes the key slot its taps share; taps of two slots in one output are refused
     const std::vector<int> in_slot = vec_slots(c, in, n_in);
-    std::vector<int> out_slot(M, -1);
+    L.out_slot.assign(M, -1);
     for (int m = 0; m < M; m++) {
         for (int kk = 0; kk < (gather ? K : n_in); kk++) {
             const int g = gather ? gather[(size_t)m * K + kk] : kk;
             if (g < 0) continue;
             if (g >= n_in) fail("gather index out of range");
-            if (out_slot[m] >= 0 && out_slot[m] != in_slot[g]) fail("encrypted operands belong to different key slots");
-            out_slot[m] = in_slot[g];
+            if (L.out_slot[m] >= 0 && L.out_slot[m] != in_slot[g]) fail("encrypted operands belong to different key slots");
+            L.out_slot[m] = in_slot[g];
         }
-        if (out_slot[m] < 0) out_slot[m] = in_slot[0];
+        if (L.out_slot[m] < 0) L.out_slot[m] = in_slot[0];
     }
     // 128-bit accumulator bound: K products of (q_l - 1)^2
-    int maxbits = 0;
-    for (u64 q : c.q) maxbits = std::max(maxbits, hm::bit_length(q));
-    if (2 * maxbits + hm::bit_length((u64)K) > 127) fail("layer too wide for the 128-bit accumulator with these coefficient moduli");
+    L.maxbits = 0;
+    for (u64 q : c.q) L.maxbits = std::max(L.maxbits, hm::bit_length(q));
+    if (2 * L.maxbits + hm::bit_length((u64)K) > 127) fail("layer too wide for the 128-bit accumulator with these coefficient moduli");
     // tiles: outputs that share a gather row, 8 at a time
-    std::vector<int> grows;
-    std::vector<MacTile> tiles;
-    std::vector<std::vector<int>> row_outs; // outputs of every distinct gather row, in the order of `grows`
-    {
-        std::unordered_map<std::vector<int>, std::vector<int>, RowHash> groups;
-        std::vector<std::vector<int>> order;
-        for (int m = 0; m < M; m++) {
-            std::vector<int> row(K);
-            bool any = false;
-            for (int kk = 0; kk < K; kk++) {
-                row[kk] = gather ? gather[(size_t)m * K + kk] : kk;
-                if (row[kk] >= n_in) fail("gather index out of range");
-            }
-            // The reference skips zero plaintexts per plaintext modulus (IsZero, AtomicSealBfvVector.cs:468) and sums what is left, so an
-            // output whose taps are all = 0 modulo one of the t_c has an empty sum in that channel.  (Deviation, documented in DESIGN.md:
-            // padded taps are skipped here, while the reference multiplies a fresh encryption of zero by their weight.)
-            for (int ch = 0; ch < c.P; ch++) {
-                bool any_ch = false;
-                for (int kk = 0; kk < K; kk++) any_ch = any_ch || (row[kk] >= 0 && weights[m]->scalars[ch][kk] != 0);
-                any = any || any_ch;
-                if (!any_ch) fail("an output has no non-zero tap modulo one of the plaintext primes (the reference would sum an empty list)");
-            }
-            if (!any) fail("an output has no non-zero tap (the reference would sum an empty list)");
-            auto it = groups.find(row);
-            if (it == groups.end()) { order.push_back(row); groups[row] = {m}; }
-            else it->second.push_back(m);
+    std::unordered_map<std::vector<int>, std::vector<int>, RowHash> groups;
+    std::vector<std::vector<int>> order;
+    for (int m = 0; m < M; m++) {
+        std::vector<int> row(K);
+        bool any = false;
+        for (int kk = 0; kk < K; kk++) {
+            row[kk] = gather ? gather[(size_t)m * K + kk] : kk;
+            if (row[kk] >= n_in) fail("gather index out of range");
         }
-        for (auto &row : order) {
-            const int row_index = (int)(grows.size() / K);
-            grows.insert(grows.end(), row.begin(), row.end());
-            const std::vector<int> &ms = groups[row];
-            row_outs.push_back(ms);
-            for (size_t s = 0; s < ms.size(); s += 8) {
-                MacTile t;
-                memset(&t, 0, sizeof(t));
-                t.gather_row = row_index;
-                t.n_out = (int)std::min<size_t>(8, ms.size() - s);
-                for (int j = 0; j < t.n_out; j++) t.out_index[j] = ms[s + j];
-                tiles.push_back(t);
-            }
+        // The reference skips zero plaintexts per plaintext modulus (IsZero, AtomicSealBfvVector.cs:468) and sums what is left, so an
+        // output whose taps are all = 0 modulo one of the t_c has an empty sum in that channel.  (Deviation, documented in DESIGN.md:
+        // padded taps are skipped here, while the reference multiplies a fresh encryption of zero by their weight.)
+        for (int ch = 0; ch < c.P; ch++) {
+            bool any_ch = false;
+            for (int kk = 0; kk < K; kk++) any_ch = any_ch || (row[kk] >= 0 && weights[m]->scalars[ch][kk] != 0);
+            any = any || any_ch;
+            if (!any_ch) fail("an output has no non-zero tap modulo one of the plaintext primes (the reference would sum an empty list)");
+        }
+        if (!any) fail("an output has no non-zero tap (the reference would sum an empty list)");
+        auto it = groups.find(row);
+        if (it == groups.end()) { order.push_back(row); groups[row] = {m}; }
+        else it->second.push_back(m);
+    }
+    for (auto &row : order) {
+        const int row_index = (int)(L.grows.size() / K);
+        L.grows.insert(L.grows.end(), row.begin(), row.end());
+        const std::vector<int> &ms = groups[row];
+        L.row_outs.push_back(ms);
+        for (size_t s = 0; s < ms.size(); s += 8) {
+            MacTile t;
+            memset(&t, 0, sizeof(t));
+            t.gather_row = row_index;
+            t.n_out = (int)std::min<size_t>(8, ms.size() - s);
+            for (int j = 0; j < t.n_out; j++) t.out_index[j] = ms[s + j];
+            L.tiles.push_back(t);
         }
     }
+    return L;
+}
+// One channel of a prepared layer on ciphertexts of `polys` polynomials (2, or 3 for size-3 products: the sum is linear in each
+// polynomial): ip[b * n_in + i] is block b of input i, op[m * bl + b] block b of output m; the blocks of one output lie consecutively,
+// polys * k * N words apart.  The bias goes to c0.
+static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector<const u64 *> &ip_all, const std::vector<u64 *> &op_all, int polys) {
+    const int n_in = L.n_in, M = L.M, K = L.K, bl = L.bl, maxbits = L.maxbits;
+    const int32_t *gather = L.gather;
+    const cnhe_vec *const *weights = L.weights, *const *bias = L.bias;
+    const std::vector<int> &grows = L.grows;
+    const std::vector<MacTile> &tiles = L.tiles;
     const int order_rows = (int)(grows.size() / K);
-    const double out_scale = in[0]->scale * weights[0]->scale;
+    const size_t ctw = (size_t)polys * c.k * c.N;
+    // every temporary lives on this channel's stream (stream-ordered frees must not overtake another channel's kernels)
+    int *d_gather = (int *)c.ws_alloc((grows.size() + 1) / 2 + 1);
+    c.h2d(d_gather, grows.data(), grows.size() * sizeof(int));
+    MacTile *d_tiles = (MacTile *)c.ws_alloc((tiles.size() * sizeof(MacTile) + 7) / 8);
+    c.h2d(d_tiles, tiles.data(), tiles.size() * sizeof(MacTile));
+    std::vector<const u64 *> wp(M);
+    for (int m = 0; m < M; m++) wp[m] = weights[m]->ptr(ch);
+    const u64 *const *d_w = upload_ptrs(c, wp);
+    // signed weights as doubles for the FP64 accumulate path, when they are small enough for it to be exact
+    const u64 t = c.t[ch], thr = (t + 1) >> 1;
+    std::vector<double> wdh((size_t)M * K);
+    double wmax = 0;
+    for (int m = 0; m < M; m++)
+        for (int kk = 0; kk < K; kk++) {
+            const u64 w = weights[m]->scalars[ch][kk];
+            const double d = w >= thr ? -(double)(t - w) : (double)w;
+            wdh[(size_t)m * K + kk] = d;
+            wmax = std::max(wmax, std::fabs(d));
+        }
+    const bool fp_mac = maxbits <= 50 && wmax < 131072.0 && (double)K * wmax * 67108864.0 < 4503599627370496.0 && !getenv("CNHE_MAC_INT");
+    // dense layer (one gather row shared by every output, 8-bit weights): exact integer GEMM on the tensor cores (mac_imma.cu).  Both
+    // tensor-core kernels join the limb sums in an FP64 epilogue that is exact only for moduli below 2^50 ((double)p, fcanon_u's
+    // |x| < 2^51); wider moduli (N = 2048's 54-bit default, custom ones) take the 128-bit k_mac_layer
+    const int limbs = (maxbits + 7) / 8;
+    const bool imma = order_rows == 1 && wmax <= 254.0 && K >= 32 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 &&
+                      (double)K * 254.0 * 255.0 < 2147483648.0 && !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
+    // ... or, for any layer whose inputs are evenly spaced rows of one slab (the previous layer's output, an imported batch) and whose
+    // weights stay within +-254: wgmma (mac_umma.cu), dense and convolution alike, under the same modulus bound
+    std::shared_ptr<UmmaPlan> plan;
+    long long tap_stride = 0;
+    {
+        // (M >= 8: LoLa's per-map products come one output at a time -- a 128-row MMA per tile would be 99 % padding and the kernel's
+        // per-tile latency more than the whole scalar-MAC launch)
+        bool slab = bl == 1 && n_in >= 2 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 && wmax <= 254.0 && !getenv("CNHE_MAC_NO_UMMA") &&
+                    !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
+        if (slab) {
+            tap_stride = ip_all[1] - ip_all[0];
+            slab = tap_stride >= (long long)ctw && tap_stride % 2 == 0;
+            for (int i = 0; i < n_in && slab; i++) slab = ip_all[i] == ip_all[0] + (long long)i * tap_stride;
+        }
+        if (slab) plan = umma_plan(c, ch, grows, L.row_outs, wdh, M, K, limbs);
+    }
+    const bool umma = plan && plan->ok && (double)plan->total_chunks * 32.0 * 127.0 * 255.0 < 2147483648.0;
+    const void *d_wfrag = nullptr, *d_wfrag2 = nullptr;
+    if (!umma && imma) {
+        const int mtiles = (M + 15) / 16, chunks = (K + 31) / 32;
+        const size_t fwords = (size_t)mtiles * chunks * 32 * 4;
+        std::vector<uint32_t> frag(2 * fwords, 0); // W1 = clamp(W, +-127) then the residual W2 = W - W1
+        bool any2 = false;
+        auto wq = [&](int m, int kk, int part) -> uint32_t { // signed weight of output m, tap kk (0 outside the matrix / on padded taps)
+            if (m >= M || kk >= K || grows[kk] < 0) return 0;
+            const int w = (int)wdh[(size_t)m * K + kk], w1 = std::max(-127, std::min(127, w));
+            const int v = part ? w - w1 : w1;
+            if (part && v) any2 = true;
+            return (uint32_t)(uint8_t)(int8_t)v;
+        };
+        for (int part = 0; part < 2; part++)
+            for (int mt = 0; mt < mtiles; mt++)
+                for (int cch = 0; cch < chunks; cch++)
+                    for (int lane = 0; lane < 32; lane++) {
+                        const int g = lane >> 2, tig = lane & 3;
+                        uint32_t *dst = &frag[part * fwords + (((size_t)mt * chunks + cch) * 32 + lane) * 4];
+                        for (int r = 0; r < 4; r++) { // r: 0 (row g, k 0..15) 1 (row g+8) 2 (row g, k 16..31) 3 (row g+8, k 16..31)
+                            const int row = mt * 16 + g + (r & 1) * 8, k0 = cch * 32 + tig * 4 + (r >> 1) * 16;
+                            dst[r] = wq(row, k0, part) | (wq(row, k0 + 1, part) << 8) | (wq(row, k0 + 2, part) << 16) | (wq(row, k0 + 3, part) << 24);
+                        }
+                    }
+        u64 *buf = c.ws_alloc((frag.size() * 4 + 7) / 8);
+        c.h2d(buf, frag.data(), (any2 ? 2 : 1) * fwords * 4);
+        d_wfrag = buf;
+        if (any2) d_wfrag2 = reinterpret_cast<const uint32_t *>(buf) + fwords;
+    }
+    const double *d_wd = nullptr;
+    if (fp_mac) {
+        u64 *buf = c.ws_alloc(wdh.size());
+        c.h2d(buf, wdh.data(), wdh.size() * 8);
+        d_wd = reinterpret_cast<const double *>(buf);
+    }
+    const u64 *d_bias = nullptr;
+    if (bias && L.const_bias) {
+        std::vector<u64> bv(M);
+        for (int m = 0; m < M; m++) bv[m] = bias[m]->const_val[ch];
+        u64 *db = c.ws_alloc(M);
+        c.h2d(db, bv.data(), (size_t)M * 8);
+        d_bias = db;
+    }
+    for (int b = 0; b < bl; b++) {
+        std::vector<const u64 *> ip(ip_all.begin() + (size_t)b * n_in, ip_all.begin() + (size_t)(b + 1) * n_in);
+        std::vector<u64 *> op(M);
+        for (int m = 0; m < M; m++) op[m] = op_all[(size_t)m * bl + b];
+        double used = 0;
+        for (auto &t : tiles) { int kk = 0; for (int j = 0; j < K; j++) kk += grows[(size_t)t.gather_row * K + j] >= 0; used += kk + t.n_out; }
+        c.prof_begin(4, used * 8.0 * ctw);
+        if (umma) {
+            UmmaLaunch a;
+            memset(&a, 0, sizeof(a));
+            a.slab = ip[0];
+            a.slab_stride_words = (size_t)tap_stride;
+            a.slab_rows = (size_t)n_in;
+            if (!plan->extra_taps.empty()) { // the taps that need the W2 part, side by side
+                u64 *scratch = c.ws_alloc(plan->extra_taps.size() * ctw);
+                for (size_t j = 0; j < plan->extra_taps.size(); j++)
+                    CNHE_CUDA(cudaMemcpyAsync(scratch + j * ctw, ip[plan->extra_taps[j]], ctw * 8, cudaMemcpyDeviceToDevice, c.stream));
+                a.scratch = scratch;
+                a.scratch_rows = plan->extra_taps.size();
+            }
+            std::vector<u64 *> opo(M);
+            for (int i = 0; i < M; i++) opo[i] = op[plan->out_order[i]];
+            const u64 *d_bias_o = nullptr;
+            if (d_bias) {
+                std::vector<u64> bo(M);
+                for (int i = 0; i < M; i++) bo[i] = bias[plan->out_order[i]]->const_val[ch];
+                u64 *db = c.ws_alloc(M);
+                c.h2d(db, bo.data(), (size_t)M * 8);
+                d_bias_o = db;
+            }
+            a.bundles = plan->d_bundles; a.n_bundles = (int)plan->bundles.size();
+            a.chunk_rows = plan->d_rows; a.total_chunks = plan->total_chunks;
+            a.wpack = plan->d_wpack; a.a_bytes = (int)plan->wpack.size();
+            a.out_ptrs = upload_ptrs_mut(c, opo); a.bias = d_bias_o; a.n_out_total = M;
+            a.limbs = limbs; a.polys = polys; a.k = c.k; a.logn = c.logN; a.bc = c.d_bc; a.pc = c.ch[ch].pc;
+            c.check(launch_mac_umma(a, c.stream), "mac_umma");
+        } else if (imma) {
+            std::vector<const u64 *> ipg(K);
+            for (int kk = 0; kk < K; kk++) ipg[kk] = ip[grows[kk] < 0 ? 0 : grows[kk]]; // padded taps carry weight 0
+            c.check(launch_mac_dense_imma(upload_ptrs(c, ipg), d_wfrag, d_wfrag2, d_bias, K, M, limbs, upload_ptrs_mut(c, op), polys, c.k, c.logN, c.d_bc,
+                                          c.ch[ch].pc, c.stream),
+                    "mac_dense_imma");
+        } else if (fp_mac)
+            c.check(launch_mac_layer_fp(upload_ptrs(c, ip), d_gather, d_tiles, (int)tiles.size(), d_wd, d_bias, K, upload_ptrs_mut(c, op), polys, c.k,
+                                        c.logN, c.d_bc, c.ch[ch].pc, c.stream),
+                    "mac_layer_fp");
+        else
+            c.check(launch_mac_layer(upload_ptrs(c, ip), d_gather, d_tiles, (int)tiles.size(), d_w, d_bias, K, upload_ptrs_mut(c, op), polys, c.k, c.logN,
+                                     c.d_bc, c.ch[ch].pc, c.stream),
+                    "mac_layer");
+        c.prof_end();
+    }
+    { // what the reference issues for this layer (AtomicSealBfvVector.cs:466-475, 497-505): MultiplyPlain per non-zero tap, AddMany per output
+        uint64_t taps = 0;
+        for (int m = 0; m < M; m++)
+            for (int kk = 0; kk < K; kk++) taps += (!gather || gather[(size_t)m * K + kk] >= 0) && weights[m]->scalars[ch][kk] != 0;
+        c.op_count[Context::OP_MULTIPLY_SCALAR] += taps * bl;
+        c.op_count[Context::OP_ADD_MANY_ITEMS] += taps * bl;
+        if (bias) c.op_count[Context::OP_ADD_PLAIN] += (uint64_t)M * bl;
+        double ss = 0; // output 0: root-sum-square of its centred weights (the noise gain of the scalar MAC under independent inputs)
+        for (int kk = 0; kk < K; kk++)
+            if (!gather || gather[kk] >= 0) ss += wdh[kk] * wdh[kk];
+        // (a size-3 sum has no noise budget of its own: its relinearised outputs are measured)
+        c.note(Context::OP_ADD_MANY, ch, M * bl, polys == 2 ? op_all[0] : nullptr, ip_all[gather ? std::max(gather[0], 0) : 0], nullptr,
+               ss > 0 ? 0.5 * std::log2(ss) : 0);
+    }
+    if (bias && !L.const_bias) // generic AddPlain per output, on c0 of each of its blocks
+        for (int m = 0; m < M; m++) {
+            u64 *o = op_all[(size_t)m * bl];
+            c.check(launch_ct_add_plain(o, o, bl, polys, bias[m]->ptr(ch), c.N, (int)c.N, c.k, c.logN, c.d_bc, c.ch[ch].pc, 0, c.stream), "ct_add_plain");
+        }
+}
+// Shared body of DenseMatrixBySparseVectorMultiply (ciphertext columns x plain constants) and of the fused PoolLayer.
+static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int32_t *gather, const cnhe_vec *const *weights, const cnhe_vec *const *bias,
+                      int M, int K, cnhe_vec **out) {
+    const MacLayer L = mac_prepare(c, in, n_in, n_in > 0 ? in[0]->scale : 0.0, gather, weights, bias, M, K);
+    const int bl = L.bl;
     std::vector<BufRef> big(c.P);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
@@ -2052,166 +2234,17 @@ static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int
     }
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
-        // every temporary lives on this channel's stream (stream-ordered frees must not overtake another channel's kernels)
-        int *d_gather = (int *)c.ws_alloc((grows.size() + 1) / 2 + 1);
-        c.h2d(d_gather, grows.data(), grows.size() * sizeof(int));
-        MacTile *d_tiles = (MacTile *)c.ws_alloc((tiles.size() * sizeof(MacTile) + 7) / 8);
-        c.h2d(d_tiles, tiles.data(), tiles.size() * sizeof(MacTile));
-        std::vector<const u64 *> wp(M);
-        for (int m = 0; m < M; m++) wp[m] = weights[m]->ptr(ch);
-        const u64 *const *d_w = upload_ptrs(c, wp);
-        // signed weights as doubles for the FP64 accumulate path, when they are small enough for it to be exact
-        const u64 t = c.t[ch], thr = (t + 1) >> 1;
-        std::vector<double> wdh((size_t)M * K);
-        double wmax = 0;
-        for (int m = 0; m < M; m++)
-            for (int kk = 0; kk < K; kk++) {
-                const u64 w = weights[m]->scalars[ch][kk];
-                const double d = w >= thr ? -(double)(t - w) : (double)w;
-                wdh[(size_t)m * K + kk] = d;
-                wmax = std::max(wmax, std::fabs(d));
-            }
-        const bool fp_mac = maxbits <= 50 && wmax < 131072.0 && (double)K * wmax * 67108864.0 < 4503599627370496.0 && !getenv("CNHE_MAC_INT");
-        // dense layer (one gather row shared by every output, 8-bit weights): exact integer GEMM on the tensor cores (mac_imma.cu).  Both
-        // tensor-core kernels join the limb sums in an FP64 epilogue that is exact only for moduli below 2^50 ((double)p, fcanon_u's
-        // |x| < 2^51); wider moduli (N = 2048's 54-bit default, custom ones) take the 128-bit k_mac_layer
-        const int limbs = (maxbits + 7) / 8;
-        const bool imma = order_rows == 1 && wmax <= 254.0 && K >= 32 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 &&
-                          (double)K * 254.0 * 255.0 < 2147483648.0 && !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
-        // ... or, for any layer whose inputs are evenly spaced rows of one slab (the previous layer's output, an imported batch) and whose
-        // weights stay within +-254: wgmma (mac_umma.cu), dense and convolution alike, under the same modulus bound
-        std::shared_ptr<UmmaPlan> plan;
-        long long tap_stride = 0;
-        {
-            // (M >= 8: LoLa's per-map products come one output at a time -- a 128-row MMA per tile would be 99 % padding and the kernel's
-            // per-tile latency more than the whole scalar-MAC launch)
-            bool slab = bl == 1 && n_in >= 2 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 && wmax <= 254.0 && !getenv("CNHE_MAC_NO_UMMA") &&
-                        !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
-            if (slab) {
-                tap_stride = in[1]->block(ch, 0) - in[0]->block(ch, 0);
-                slab = tap_stride >= (long long)c.ct_words() && tap_stride % 2 == 0;
-                for (int i = 0; i < n_in && slab; i++) slab = in[i]->block(ch, 0) == in[0]->block(ch, 0) + (long long)i * tap_stride;
-            }
-            if (slab) plan = umma_plan(c, ch, grows, row_outs, wdh, M, K, limbs);
-        }
-        const bool umma = plan && plan->ok && (double)plan->total_chunks * 32.0 * 127.0 * 255.0 < 2147483648.0;
-        const void *d_wfrag = nullptr, *d_wfrag2 = nullptr;
-        if (!umma && imma) {
-            const int mtiles = (M + 15) / 16, chunks = (K + 31) / 32;
-            const size_t fwords = (size_t)mtiles * chunks * 32 * 4;
-            std::vector<uint32_t> frag(2 * fwords, 0); // W1 = clamp(W, +-127) then the residual W2 = W - W1
-            bool any2 = false;
-            auto wq = [&](int m, int kk, int part) -> uint32_t { // signed weight of output m, tap kk (0 outside the matrix / on padded taps)
-                if (m >= M || kk >= K || grows[kk] < 0) return 0;
-                const int w = (int)wdh[(size_t)m * K + kk], w1 = std::max(-127, std::min(127, w));
-                const int v = part ? w - w1 : w1;
-                if (part && v) any2 = true;
-                return (uint32_t)(uint8_t)(int8_t)v;
-            };
-            for (int part = 0; part < 2; part++)
-                for (int mt = 0; mt < mtiles; mt++)
-                    for (int cch = 0; cch < chunks; cch++)
-                        for (int lane = 0; lane < 32; lane++) {
-                            const int g = lane >> 2, tig = lane & 3;
-                            uint32_t *dst = &frag[part * fwords + (((size_t)mt * chunks + cch) * 32 + lane) * 4];
-                            for (int r = 0; r < 4; r++) { // r: 0 (row g, k 0..15) 1 (row g+8) 2 (row g, k 16..31) 3 (row g+8, k 16..31)
-                                const int row = mt * 16 + g + (r & 1) * 8, k0 = cch * 32 + tig * 4 + (r >> 1) * 16;
-                                dst[r] = wq(row, k0, part) | (wq(row, k0 + 1, part) << 8) | (wq(row, k0 + 2, part) << 16) | (wq(row, k0 + 3, part) << 24);
-                            }
-                        }
-            u64 *buf = c.ws_alloc((frag.size() * 4 + 7) / 8);
-            c.h2d(buf, frag.data(), (any2 ? 2 : 1) * fwords * 4);
-            d_wfrag = buf;
-            if (any2) d_wfrag2 = reinterpret_cast<const uint32_t *>(buf) + fwords;
-        }
-        const double *d_wd = nullptr;
-        if (fp_mac) {
-            u64 *buf = c.ws_alloc(wdh.size());
-            c.h2d(buf, wdh.data(), wdh.size() * 8);
-            d_wd = reinterpret_cast<const double *>(buf);
-        }
-        const u64 *d_bias = nullptr;
-        if (bias && const_bias) {
-            std::vector<u64> bv(M);
-            for (int m = 0; m < M; m++) bv[m] = bias[m]->const_val[ch];
-            u64 *db = c.ws_alloc(M);
-            c.h2d(db, bv.data(), (size_t)M * 8);
-            d_bias = db;
-        }
-        for (int b = 0; b < bl; b++) {
-            std::vector<const u64 *> ip(n_in);
-            for (int i = 0; i < n_in; i++) ip[i] = in[i]->block(ch, b);
-            std::vector<u64 *> op(M);
-            for (int m = 0; m < M; m++) op[m] = big[ch]->p + ((size_t)m * bl + b) * c.ct_words();
-            double used = 0;
-            for (auto &t : tiles) { int kk = 0; for (int j = 0; j < K; j++) kk += grows[(size_t)t.gather_row * K + j] >= 0; used += kk + t.n_out; }
-            c.prof_begin(4, used * 8.0 * c.ct_words());
-            if (umma) {
-                UmmaLaunch a;
-                memset(&a, 0, sizeof(a));
-                a.slab = in[0]->block(ch, 0);
-                a.slab_stride_words = (size_t)tap_stride;
-                a.slab_rows = (size_t)n_in;
-                if (!plan->extra_taps.empty()) { // the taps that need the W2 part, side by side
-                    u64 *scratch = c.ws_alloc(plan->extra_taps.size() * c.ct_words());
-                    for (size_t j = 0; j < plan->extra_taps.size(); j++)
-                        CNHE_CUDA(cudaMemcpyAsync(scratch + j * c.ct_words(), ip[plan->extra_taps[j]], c.ct_words() * 8, cudaMemcpyDeviceToDevice, c.stream));
-                    a.scratch = scratch;
-                    a.scratch_rows = plan->extra_taps.size();
-                }
-                std::vector<u64 *> opo(M);
-                for (int i = 0; i < M; i++) opo[i] = op[plan->out_order[i]];
-                const u64 *d_bias_o = nullptr;
-                if (d_bias) {
-                    std::vector<u64> bo(M);
-                    for (int i = 0; i < M; i++) bo[i] = bias[plan->out_order[i]]->const_val[ch];
-                    u64 *db = c.ws_alloc(M);
-                    c.h2d(db, bo.data(), (size_t)M * 8);
-                    d_bias_o = db;
-                }
-                a.bundles = plan->d_bundles; a.n_bundles = (int)plan->bundles.size();
-                a.chunk_rows = plan->d_rows; a.total_chunks = plan->total_chunks;
-                a.wpack = plan->d_wpack; a.a_bytes = (int)plan->wpack.size();
-                a.out_ptrs = upload_ptrs_mut(c, opo); a.bias = d_bias_o; a.n_out_total = M;
-                a.limbs = limbs; a.k = c.k; a.logn = c.logN; a.bc = c.d_bc; a.pc = c.ch[ch].pc;
-                c.check(launch_mac_umma(a, c.stream), "mac_umma");
-            } else if (imma) {
-                std::vector<const u64 *> ipg(K);
-                for (int kk = 0; kk < K; kk++) ipg[kk] = ip[grows[kk] < 0 ? 0 : grows[kk]]; // padded taps carry weight 0
-                c.check(launch_mac_dense_imma(upload_ptrs(c, ipg), d_wfrag, d_wfrag2, d_bias, K, M, limbs, upload_ptrs_mut(c, op), c.k, c.logN, c.d_bc, c.ch[ch].pc,
-                                              c.stream),
-                        "mac_dense_imma");
-            } else if (fp_mac)
-                c.check(launch_mac_layer_fp(upload_ptrs(c, ip), d_gather, d_tiles, (int)tiles.size(), d_wd, d_bias, K, upload_ptrs_mut(c, op), c.k, c.logN,
-                                            c.d_bc, c.ch[ch].pc, c.stream),
-                        "mac_layer_fp");
-            else
-                c.check(launch_mac_layer(upload_ptrs(c, ip), d_gather, d_tiles, (int)tiles.size(), d_w, d_bias, K, upload_ptrs_mut(c, op), c.k, c.logN,
-                                         c.d_bc, c.ch[ch].pc, c.stream),
-                        "mac_layer");
-            c.prof_end();
-        }
-        { // what the reference issues for this layer (AtomicSealBfvVector.cs:466-475, 497-505): MultiplyPlain per non-zero tap, AddMany per output
-            uint64_t taps = 0;
-            for (int m = 0; m < M; m++)
-                for (int kk = 0; kk < K; kk++) taps += (!gather || gather[(size_t)m * K + kk] >= 0) && weights[m]->scalars[ch][kk] != 0;
-            c.op_count[Context::OP_MULTIPLY_SCALAR] += taps * bl;
-            c.op_count[Context::OP_ADD_MANY_ITEMS] += taps * bl;
-            if (bias) c.op_count[Context::OP_ADD_PLAIN] += (uint64_t)M * bl;
-            double ss = 0; // output 0: root-sum-square of its centred weights (the noise gain of the scalar MAC under independent inputs)
-            for (int kk = 0; kk < K; kk++)
-                if (!gather || gather[kk] >= 0) ss += wdh[kk] * wdh[kk];
-            c.note(Context::OP_ADD_MANY, ch, M * bl, big[ch]->p, in[gather ? std::max(gather[0], 0) : 0]->block(ch, 0), nullptr, ss > 0 ? 0.5 * std::log2(ss) : 0);
-        }
-        if (bias && !const_bias) // generic AddPlain per output
-            for (int m = 0; m < M; m++) {
-                u64 *o = big[ch]->p + (size_t)m * bl * c.ct_words();
-                c.check(launch_ct_add_plain(o, o, bl, 2, bias[m]->ptr(ch), c.N, (int)c.N, c.k, c.logN, c.d_bc, c.ch[ch].pc, 0, c.stream), "ct_add_plain");
-            }
+        std::vector<const u64 *> ip((size_t)bl * n_in);
+        for (int b = 0; b < bl; b++)
+            for (int i = 0; i < n_in; i++) ip[(size_t)b * n_in + i] = in[i]->block(ch, b);
+        std::vector<u64 *> op((size_t)M * bl);
+        for (size_t j = 0; j < op.size(); j++) op[j] = big[ch]->p + j * c.ct_words();
+        mac_channel(c, L, ch, ip, op, 2);
     }
+    const double out_scale = in[0]->scale * weights[0]->scale;
     for (int m = 0; m < M; m++) {
         out[m] = slab_view(new_vec(c, in[0]->dim, out_scale, CNHE_DENSE, true, bl), big, (size_t)m * bl);
-        out[m]->slot = out_slot[m];
+        out[m]->slot = L.out_slot[m];
     }
 }
 extern "C" int cnhe_layer_conv_dense(cnhe_ctx *h, const cnhe_vec *const *in, int n_in, const int32_t *gather, const cnhe_vec *const *weights,
@@ -2460,12 +2493,8 @@ static const u64 *const *padded_constants(Context &c, int ch, const cnhe_vec *co
     }
     return any ? upload_ptrs(c, tab) : nullptr;
 }
-// The quadratic activation a x^2 + b x + c over a whole matrix, in cnhe_layer_square's passes: the BEHZ floor kernel scales the size-3
-// product by A and adds B x and Delta C (FloorEpi), so out[i] = relinearize(A (.) in[i]^2) + B (.) in[i] + C word for word
-extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc,
-                                cnhe_vec **out) {
-    API_BEGIN(h)
-    if (n < 1) fail("empty layer");
+// cnhe_layer_poly2's coefficients: a required, each one a plain sparse vector of dimension 1
+static void poly2_check_coeffs(Context &c, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc) {
     if (!a) fail("the quadratic coefficient is required");
     for (const cnhe_vec *p : {a, b, cc}) {
         if (!p) continue;
@@ -2473,6 +2502,30 @@ extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, c
         if (p->enc) fail("the coefficients must be plain");
         if (p->format != CNHE_SPARSE || p->dim != 1) fail("each coefficient must be a sparse vector of dimension 1");
     }
+}
+// the output scale scale(a) s^2 of inputs at scale s; scale(b) s and scale(c) must equal it
+static double poly2_out_scale(double s, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc) {
+    const double out_scale = a->scale * s * s;
+    if (b && b->scale * s != out_scale) fail("Scales do not match.");
+    if (cc && cc->scale != out_scale) fail("Scales do not match.");
+    return out_scale;
+}
+// the operations of a x^2 + b x + c on `total` ciphertexts of one channel beyond the product (a term that is 0 mod t is skipped there)
+static void poly2_count(Context &c, u64 A, u64 B, u64 C, int total) {
+    if (A) c.op_count[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+    if (B) {
+        c.op_count[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+        c.op_count[Context::OP_ADD] += (uint64_t)total;
+    }
+    if (C) c.op_count[Context::OP_ADD_PLAIN] += (uint64_t)total;
+}
+// The quadratic activation a x^2 + b x + c over a whole matrix, in cnhe_layer_square's passes: the BEHZ floor kernel scales the size-3
+// product by A and adds B x and Delta C (FloorEpi), so out[i] = relinearize(A (.) in[i]^2) + B (.) in[i] + C word for word
+extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc,
+                                cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n < 1) fail("empty layer");
+    poly2_check_coeffs(c, a, b, cc);
     std::vector<int> first(n + 1, 0);
     for (int i = 0; i < n; i++) {
         same_ctx(c, in[i]);
@@ -2480,9 +2533,7 @@ extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, c
         if (in[i]->scale != in[0]->scale) fail("Scales do not match.");
         first[i + 1] = first[i] + in[i]->blocks;
     }
-    const double s = in[0]->scale, out_scale = a->scale * s * s;
-    if (b && b->scale * s != out_scale) fail("Scales do not match.");
-    if (cc && cc->scale != out_scale) fail("Scales do not match.");
+    const double out_scale = poly2_out_scale(in[0]->scale, a, b, cc);
     const int total = first[n];
     const std::vector<int> vslot = vec_slots(c, in, n);
     std::vector<int> ct_slot;
@@ -2498,17 +2549,67 @@ extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, c
         for (int i = 0; i < n; i++)
             for (int bl = 0; bl < in[i]->blocks; bl++) ptrs.push_back(in[i]->block(ch, bl));
         op_multiply_relin(c, ch, ptrs, ptrs, big[ch]->p, ct_slot.data(), &epi);
-        // the operations of the composition (a term that is 0 mod t is skipped in that channel)
-        if (A) c.op_count[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
-        if (B) {
-            c.op_count[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
-            c.op_count[Context::OP_ADD] += (uint64_t)total;
-        }
-        if (C) c.op_count[Context::OP_ADD_PLAIN] += (uint64_t)total;
+        poly2_count(c, A, B, C, total); // the operations of the composition
     }
     for (int i = 0; i < n; i++) {
         out[i] = slab_view(new_vec(c, in[i]->dim, out_scale, in[i]->format, true, in[i]->blocks), big, first[i]);
         out[i]->slot = vslot[i];
+    }
+    API_END
+}
+// The square (a == NULL) or quadratic activation followed by a scalar-MAC layer, relinearising the layer's outputs instead of its squared
+// inputs: the scalar MAC is linear in each polynomial of a size-3 ciphertext, so per plaintext prime
+//   P3(x)  = A (.) multiply(x, x) + (B x0 + Delta C, B x1, 0)       (cnhe_layer_poly2's floor epilogue on the unrelinearised product)
+//   out[m] = relinearize(sum_k w[m][k] (.) P3(in[gather[m K + k]]) + add_plain(bias[m]))
+// word for word, with M key switches per block instead of n_in.  All n_in size-3 products of a channel are held at once.
+extern "C" int cnhe_layer_activation_conv_dense(cnhe_ctx *h, const cnhe_vec *const *in, int n_in, const cnhe_vec *a, const cnhe_vec *b,
+                                                const cnhe_vec *cc, const int32_t *gather, const cnhe_vec *const *weights,
+                                                const cnhe_vec *const *bias, int M, int K, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n_in < 1) fail("empty layer");
+    if (a) poly2_check_coeffs(c, a, b, cc);
+    else if (b || cc) fail("the quadratic coefficient is required");
+    same_ctx(c, in[0]);
+    const double s = in[0]->scale, act_scale = a ? poly2_out_scale(s, a, b, cc) : s * s;
+    const MacLayer L = mac_prepare(c, in, n_in, act_scale, gather, weights, bias, M, K);
+    const int bl = L.bl, total = n_in * bl;
+    const size_t w3 = (size_t)3 * c.k * c.N;
+    if ((size_t)total * w3 > ((size_t)1 << 30)) fail("the size-3 products of the layer's inputs exceed the 8 GiB scratch limit");
+    std::vector<int> ct_slot; // relinearisation: every output under the key slot its taps share
+    for (int m = 0; m < M; m++) ct_slot.insert(ct_slot.end(), bl, L.out_slot[m]);
+    std::vector<BufRef> big(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        big[ch] = c.alloc((size_t)M * bl * c.ct_words());
+    }
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        WsScope scope(c); // the size-3 slabs of this channel go back to its stream when its key switch is done
+        u64 *x3 = c.ws_alloc((size_t)total * w3), *y3 = c.ws_alloc((size_t)M * bl * w3);
+        std::vector<const u64 *> ptrs;
+        for (int i = 0; i < n_in; i++)
+            for (int bb = 0; bb < bl; bb++) ptrs.push_back(in[i]->block(ch, bb));
+        FloorEpi epi;
+        const FloorEpi *ep = nullptr;
+        if (a) {
+            const u64 A = a->scalars[ch][0], B = b ? b->scalars[ch][0] : 0, C = cc ? cc->scalars[ch][0] : 0;
+            epi = floor_epi(c, ch, A, B, C);
+            if (C) epi.c_poly = padded_constants(c, ch, in, n_in, total, C);
+            ep = &epi;
+            poly2_count(c, A, B, C, total);
+        }
+        op_multiply(c, ch, ptrs, ptrs, x3, ep);
+        std::vector<const u64 *> ip((size_t)bl * n_in);
+        for (int bb = 0; bb < bl; bb++)
+            for (int i = 0; i < n_in; i++) ip[(size_t)bb * n_in + i] = x3 + ((size_t)i * bl + bb) * w3;
+        std::vector<u64 *> op((size_t)M * bl);
+        for (size_t j = 0; j < op.size(); j++) op[j] = y3 + j * w3;
+        mac_channel(c, L, ch, ip, op, 3);
+        op_relinearize(c, ch, y3, M * bl, big[ch]->p, ct_slot.data());
+    }
+    for (int m = 0; m < M; m++) {
+        out[m] = slab_view(new_vec(c, in[0]->dim, act_scale * weights[0]->scale, CNHE_DENSE, true, bl), big, (size_t)m * bl);
+        out[m]->slot = L.out_slot[m];
     }
     API_END
 }

@@ -671,6 +671,21 @@ class Engine:
             None if bias is None else _vec_array(bias), M, K, out))
         return self._wrap_many(out, M)
 
+    def layer_activation_conv_dense(self, inputs, a, b, c, gather, weights, bias, M, K):
+        """The activation a x^2 + b x + c (a, b, c None: the square) followed by layer_conv_dense, with one relinearisation per output
+        instead of one per input (include/cnhe.h, cnhe_layer_activation_conv_dense).  a, b, c as for layer_poly2; the outputs have scale
+        scale(a) s^2 scale(w), which the bias must share."""
+        g = None
+        if gather is not None:
+            g = np.ascontiguousarray(gather, dtype=np.int32)
+            assert g.size == M * K
+        out = (VECP * M)()
+        h = lambda v: None if v is None else v.h
+        check(self.L.cnhe_layer_activation_conv_dense(
+            self.h, _vec_array(inputs), len(inputs), h(a), h(b), h(c), None if g is None else g.ctypes.data_as(C.POINTER(C.c_int32)),
+            _vec_array(weights), None if bias is None else _vec_array(bias), M, K, out))
+        return self._wrap_many(out, M)
+
     def _wrap_many(self, out, n, like=None):
         """Vec handles for the n outputs of one batched call: they share dim/scale/format/blocks, so the metadata is queried once.
         like: the inputs of a call whose outputs follow their own input's shape -- shared only when those inputs share theirs."""

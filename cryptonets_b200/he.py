@@ -526,5 +526,13 @@ class B200BfvFactory:
                                            None if bias is None else [b.vec for b in bias], M, K)
         return [B200BfvVector(self, o) for o in out]
 
+    def ActivationConvDenseLayer(self, inputs, a, b, c, gather, weights, bias, M, K):
+        """PoolLayer(DeferRelinearization=True) over its activation's input: the activation (a, b, c None: the square; else PolyActivation's
+        quadratic) and ConvDenseLayer in one call, relinearising the M outputs instead of every squared input."""
+        v = lambda x: None if x is None else x.vec
+        out = self.engine.layer_activation_conv_dense([x.vec for x in inputs], v(a), v(b), v(c), gather, [w.vec for w in weights],
+                                                      None if bias is None else [x.vec for x in bias], M, K)
+        return [B200BfvVector(self, o) for o in out]
+
     def Dispose(self):
         self.engine.close()

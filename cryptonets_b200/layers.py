@@ -410,13 +410,29 @@ class _ConvLayerBase(BaseLayer):
 
 
 class PoolLayer(_ConvLayerBase):
-    """Convolution / dense / mean-pool over per-pixel ciphertexts (`NeuralNetworks/PoolLayer.cs:13-245`)."""
+    """Convolution / dense / mean-pool over per-pixel ciphertexts (`NeuralNetworks/PoolLayer.cs:13-245`).
 
-    def __init__(self, Fused=True, **kw):
+    DeferRelinearization=True (with Fused, weights, and a SquareActivation or 3-coefficient PolyActivation as Source): GetNext takes the
+    activation's input and makes one factory call (ActivationConvDenseLayer) that squares, sums the unrelinearised products and
+    relinearises only this layer's outputs -- the same decryption with one key switch per output instead of one per input.  Apply and
+    ApplyBatch are unchanged, and a factory without that call (the Raw backend) applies the activation, then this layer."""
+
+    def __init__(self, Fused=True, DeferRelinearization=False, **kw):
         self.Fused = Fused
+        self.DeferRelinearization = DeferRelinearization
         super().__init__(**kw)
 
     def Prepare(self):
+        if self.DeferRelinearization:
+            src = self.Source
+            if not self.Fused:
+                raise Exception("DeferRelinearization needs the fused layer (Fused=True)")
+            if self.Weights is None:
+                raise Exception("DeferRelinearization needs a layer with weights")
+            if not isinstance(src, (SquareActivation, PolyActivation)):
+                raise Exception("DeferRelinearization needs a SquareActivation or PolyActivation as Source")
+            if isinstance(src, PolyActivation) and len(src.Coefficients) != 3:
+                raise Exception("DeferRelinearization takes a quadratic PolyActivation (3 coefficients)")
         if self.layerPrepared:
             return
         self.ce.Prepare()
@@ -429,6 +445,47 @@ class PoolLayer(_ConvLayerBase):
 
     def _gather_row(self, corner):
         return [self.ce.Location(corner, off, self.InputShape) for off in self.Offsets]
+
+    def GetNext(self):
+        f = self.Factory
+        if not (self.DeferRelinearization and hasattr(f, "ActivationConvDenseLayer")):
+            return super().GetNext()
+        act = self.Source
+        for layer in (self, act):
+            if not layer.layerPrepared:
+                layer.Prepare()
+                layer.layerPrepared = True
+        m = act.Source.GetNext()
+        start = time.time()
+        a, b, c = act.coefficientVectors if isinstance(act, PolyActivation) else (None, None, None)
+        res = self._fused(m, lambda inputs, *layer: f.ActivationConvDenseLayer(inputs, a, b, c, *layer))
+        self.LastSeconds = time.time() - start
+        if self.Verbose:
+            print("Layer %s (deferred relinearisation) computed in %.4f seconds layer width (%d,%d)"
+                  % (type(self).__name__, self.LastSeconds, m.RowCount, m.ColumnCount))
+        m.Dispose()
+        return res
+
+    def _prepare_bias(self, m):
+        if self.biasVectors is None or self.biasVectors[0].Dim != m.RowCount:
+            if self.biasVectors:
+                for b in self.biasVectors:
+                    b.Dispose()
+            scale = self.Source.GetOutputScale() * self.WeightsScale
+            f = self.Factory
+            self.biasVectors = [f.GetPlainVector(np.full(m.RowCount, self._bias_value(k)), EVectorFormat.dense, scale) for k in range(self.maps())]
+
+    def _fused(self, m, call):
+        """call(inputs, gather, weights, bias, M, K) over the columns of m: the whole layer in one factory call."""
+        self._prepare_bias(m)
+        K = len(self.Offsets)
+        M = self.maps() * len(self.Corners)
+        if getattr(self, "_gather", None) is None:  # the topology is static: index table built once
+            self._gather = np.array([self._gather_row(c) for c in self.Corners] * self.maps(), dtype=np.int32)  # k = map*corners + corner
+        inputs = [m.GetColumn(i) for i in range(m.ColumnCount)]
+        weights = [self.weightWindows[k // len(self.Corners)] for k in range(M)]
+        bias = [self.biasVectors[k // len(self.Corners)] for k in range(M)]
+        return self.Factory.GetMatrix(call(inputs, self._gather, weights, bias, M, K), EMatrixFormat.ColumnMajor, CopyVectors=False)
 
     def Apply(self, m):
         f = self.Factory
@@ -450,24 +507,10 @@ class PoolLayer(_ConvLayerBase):
                 agg.RegisterScale(agg.Scale * len(self.Offsets))
                 outs.append(agg)
             return f.GetMatrix(outs, EMatrixFormat.ColumnMajor, CopyVectors=False)
-        maps = self.maps()
-        if self.biasVectors is None or self.biasVectors[0].Dim != m.RowCount:
-            if self.biasVectors:
-                for b in self.biasVectors:
-                    b.Dispose()
-            scale = self.Source.GetOutputScale() * self.WeightsScale
-            self.biasVectors = [f.GetPlainVector(np.full(m.RowCount, self._bias_value(k)), EVectorFormat.dense, scale) for k in range(maps)]
-        K = len(self.Offsets)
-        M = maps * len(self.Corners)
         if self.Fused and hasattr(f, "ConvDenseLayer"):
-            if getattr(self, "_gather", None) is None:  # the topology is static: index table built once
-                self._gather = np.array([self._gather_row(c) for c in self.Corners] * maps, dtype=np.int32)  # k = map*corners + corner
-            gather = self._gather
-            inputs = [m.GetColumn(i) for i in range(m.ColumnCount)]
-            weights = [self.weightWindows[k // len(self.Corners)] for k in range(M)]
-            bias = [self.biasVectors[k // len(self.Corners)] for k in range(M)]
-            res = f.ConvDenseLayer(inputs, gather, weights, bias, M, K)
-            return f.GetMatrix(res, EMatrixFormat.ColumnMajor, CopyVectors=False)
+            return self._fused(m, f.ConvDenseLayer)
+        self._prepare_bias(m)
+        M = self.maps() * len(self.Corners)
         res, temps = [], []
         for k in range(M):  # the reference's per-output path (PoolLayer.cs:113-121, 214-223)
             mapIndex, cornerIndex = divmod(k, len(self.Corners))

@@ -57,8 +57,10 @@ def synthetic_mnist(n_images, seed=20240917):
     return px.astype(np.float64)
 
 
-def cryptonets_mnist(factory, images, batch_size=None, fused=True, weights=None, timing=True):
-    """Returns (network, reader).  network.GetNext() yields the 10-column score matrix of one batch."""
+def cryptonets_mnist(factory, images, batch_size=None, fused=True, weights=None, timing=True, defer_relinearization=False):
+    """Returns (network, reader).  network.GetNext() yields the 10-column score matrix of one batch.  defer_relinearization: both dense
+    layers square their input and relinearise only their outputs (PoolLayer.DeferRelinearization): same scores, 110 relinearisations per
+    plaintext prime instead of 945."""
     w = weights or cryptonets_weights()
     weightscale = 32
     reader = MatrixSource(images, Scale=16.0, NormalizationFactor=1.0 / 256.0, MaxSlots=batch_size or len(images))
@@ -68,10 +70,11 @@ def cryptonets_mnist(factory, images, batch_size=None, fused=True, weights=None,
                       WeightsScale=weightscale, Weights=w["Weights_0"], Fused=fused)
     act2 = SquareActivation(Source=conv1)
     dense3 = PoolLayer(Source=act2, InputShape=[5 * 13 * 13], KernelShape=[5 * 13 * 13], Stride=[1000], MapCount=[100],
-                       Weights=transpose(w["Weights_1"], 5 * 13 * 13, 100), Bias=w["Biases_2"], WeightsScale=weightscale * weightscale, Fused=fused)
+                       Weights=transpose(w["Weights_1"], 5 * 13 * 13, 100), Bias=w["Biases_2"], WeightsScale=weightscale * weightscale, Fused=fused,
+                       DeferRelinearization=defer_relinearization)
     act4 = SquareActivation(Source=dense3)
     dense5 = PoolLayer(Source=act4, InputShape=[100], KernelShape=[100], Stride=[1000], MapCount=[10], Weights=w["Weights_3"],
-                       Bias=w["Biases_3"], WeightsScale=weightscale, Fused=fused)
+                       Bias=w["Biases_3"], WeightsScale=weightscale, Fused=fused, DeferRelinearization=defer_relinearization)
     net = TimingLayer(Source=dense5, StopCounters=["Batch-Time"]) if timing else dense5
     return net, reader
 

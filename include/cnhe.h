@@ -1,7 +1,7 @@
 /*
  * cnhe.h -- C ABI of libcnhe.so, the H100-native BFV engine behind the CryptoNets plugin API.
  *
- * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these 110 entry points
+ * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these 111 entry points
  * with [DllImport("cnhe")] (stub in INTEGRATION.md); the Python mirror in cryptonets_b200/ binds them with ctypes.
  * One cnhe_vec is one reference `EncryptedSealBfvVector` ("HE Wrapper/EncryptedSealBfvVector.cs:150-573"): P
  * plaintext-modulus channels, each an `AtomicSealBfvEncryptedVector` ("HE Wrapper/AtomicSealBfvVector.cs:303-1476")
@@ -350,6 +350,20 @@ int cnhe_layer_poly2(cnhe_ctx *, const cnhe_vec *const *in, int n, const cnhe_ve
  * vectors may belong to different key slots, as for cnhe_layer_square.  Operation counts are those of the composition. */
 int cnhe_layer_poly(cnhe_ctx *, const cnhe_vec *const *in, int n, const cnhe_vec *const *coeffs /*degree + 1*/, int degree,
                     cnhe_vec **out /*n*/);
+/* The square (a, b, c all NULL) or the quadratic activation of cnhe_layer_poly2, followed by the layer of cnhe_layer_conv_dense, with the
+ * relinearisation deferred to the layer's outputs: M key switches per block instead of n_in.  Per plaintext prime, out[m] is, word for word,
+ *   P3(x)  = A (.) multiply(x, x) + (B x0 + Delta C, B x1, 0)      (size 3; (A, B, C) = (1, 0, 0) when a is NULL)
+ *   out[m] = relinearize(sum_k w[m][k] (.) P3(in[gather[m*K+k]]) + add_plain(bias[m]))
+ * where w (.) multiplies all three polynomials by the weight, lifted as the scalar MAC lifts it, and the bias goes to c0.  The same
+ * decryption as cnhe_layer_conv_dense over cnhe_layer_poly2's (or cnhe_layer_square's) outputs, with one key-switch noise term per output
+ * instead of a weighted sum of them.  a, b, c follow cnhe_layer_poly2 (C in the data slots of a dense vector only); in, gather, weights,
+ * bias and the key slots follow cnhe_layer_conv_dense.  The output scale is scale(a) s^2 scale(w) (s^2 scale(w) for the square), which the
+ * bias must share.  Operation counts are those of the composition: n_in * blocks multiplications, the activation's terms, the scalar MAC's
+ * counts and M * blocks relinearisations.  All n_in * blocks size-3 products of a plaintext prime are held at once: a call that needs
+ * more than 8 GiB for them is refused (CNHE_ERR_INVALID). */
+int cnhe_layer_activation_conv_dense(cnhe_ctx *, const cnhe_vec *const *in, int n_in, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *c,
+                                     const int32_t *gather, const cnhe_vec *const *weights, const cnhe_vec *const *bias, int M, int K,
+                                     cnhe_vec **out /*M*/);
 
 /* ---- micro-benchmark / kernel-level entry points on caller-owned device memory ("raw") --------------------------- */
 int cnhe_dev_alloc(cnhe_ctx *, size_t words, uint64_t *dptr);

@@ -112,6 +112,7 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_square(IntPtr a0, IntPtr[] @in, int n, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_poly2(IntPtr a0, IntPtr[] @in, int n, IntPtr a, IntPtr b, IntPtr c, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_poly(IntPtr a0, IntPtr[] @in, int n, IntPtr[] coeffs, int degree, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_layer_activation_conv_dense(IntPtr a0, IntPtr[] @in, int n_in, IntPtr a, IntPtr b, IntPtr c, int[] gather, IntPtr[] weights, IntPtr[] bias, int M, int K, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_alloc(IntPtr a0, UIntPtr words, out ulong dptr);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_free(IntPtr a0, ulong dptr);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_upload(IntPtr a0, ulong dptr, IntPtr src, UIntPtr words);
@@ -327,6 +328,16 @@ namespace HEWrapper
             var coeffs = coefficients.Reverse().Select(v => v == null ? IntPtr.Zero : ((B200BfvVector)v).Handle).ToArray();
             Cnhe.Check(Cnhe.cnhe_layer_poly(Ctx, Cnhe.Handles(Vectors), Vectors.Length, coeffs, coeffs.Length - 1, outs));
             return new B200BfvMatrix(Factory, outs.Select(h => (IVector)new B200BfvVector(Factory, h)).ToArray(), Format, false) { DataDisposedExternaly = false };
+        }
+        /// the square (a, b, c null) or a x^2 + b x + c of every column followed by the scalar-MAC layer of ConvDenseLayer, relinearising only
+        /// the M outputs (cnhe_layer_activation_conv_dense); the outputs have scale scale(a) s^2 scale(w), which the bias must share
+        public IVector[] ActivationConvDense(IVector a, IVector b, IVector c, int[] gather, IVector[] weights, IVector[] bias, int M, int K)
+        {
+            IntPtr H(IVector v) => v == null ? IntPtr.Zero : ((B200BfvVector)v).Handle;
+            var outs = new IntPtr[M];
+            Cnhe.Check(Cnhe.cnhe_layer_activation_conv_dense(Ctx, Cnhe.Handles(Vectors), Vectors.Length, H(a), H(b), H(c), gather, Cnhe.Handles(weights),
+                                                             bias == null ? null : Cnhe.Handles(bias), M, K, outs));
+            return outs.Select(h => (IVector)new B200BfvVector(Factory, h)).ToArray();
         }
         public IVector GetColumn(int columnNumber)
         {
