@@ -21,6 +21,7 @@ _SIGS = {
     "cnhe_context_coeff_moduli": [C.c_void_p, U64P],
     "cnhe_context_plain_moduli": [C.c_void_p, U64P],
     "cnhe_context_bsk_moduli": [C.c_void_p, U64P, C.POINTER(i32)],
+    "cnhe_context_product_sum_terms": [C.c_void_p, C.POINTER(i32)],
     "cnhe_context_galois_elts": [C.c_void_p, U64P],
     "cnhe_context_set_option": [C.c_void_p, C.c_char_p, i64],
     "cnhe_context_sync": [C.c_void_p],
@@ -101,6 +102,7 @@ _SIGS = {
     "cnhe_vecs_stack": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP)],
     "cnhe_vecs_generate_sparse_of_array": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP)],
     "cnhe_mat_mul_colmajor_sparse": [C.c_void_p, C.POINTER(VECP), i32, VECP, C.POINTER(VECP)],
+    "cnhe_mat_mul_colmajor_sparse_deferred": [C.c_void_p, C.POINTER(VECP), i32, VECP, C.POINTER(VECP)],
     "cnhe_mat_mul_rowmajor": [C.c_void_p, C.POINTER(VECP), i32, VECP, i32, C.POINTER(VECP)],
     "cnhe_mat_mul_rowmajor_shard": [C.c_void_p, C.POINTER(VECP), i32, VECP, i32, i32, i32, C.POINTER(VECP)],
     "cnhe_layer_conv_dense": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(C.c_int32), C.POINTER(VECP), C.POINTER(VECP), i32, i32,

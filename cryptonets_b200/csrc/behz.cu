@@ -93,6 +93,42 @@ __global__ void __launch_bounds__(256) k_behz_tensor(const u64 *a, const u64 *b,
     d[o + (size_t)2 * kt * N] = d2;
 }
 
+// ---- sum of T tensor products per output (op_multiply_sum; the FP64 twin is k_behz_tensor_mac_fp): d[o] = sum_j a[o T + j] (x) b[j],
+// a [n_out T][2][kt][N], b [T][2][kt][N], d [n_out][3][kt][N], canonical words.  One thread per (output, residue, coefficient), CTAs ordered
+// output fastest as in the FP64 kernel.  128-bit sums of at most 8 products of 62-bit words (4 terms: d1 takes two per term) between
+// Barrett reductions, as in k_ks_mac.
+__global__ void __launch_bounds__(256) k_behz_tensor_mac(const u64 *__restrict__ a, const u64 *__restrict__ b, u64 *__restrict__ d, int n_out, int T,
+                                                        int logn, const BehzConst *__restrict__ gbc) {
+    __shared__ BehzConst bc;
+    load_consts(&bc, gbc);
+    const int N = 1 << logn, k = bc.k, kt = k + bc.kb, tiles = N >> 8;
+    const int o = blockIdx.x % n_out, tile = (blockIdx.x / n_out) % tiles, l = blockIdx.x / (n_out * tiles);
+    const int x = (tile << 8) + threadIdx.x;
+    const DMod m = l < k ? bc.q[l] : bc.bsk[l - k];
+    const size_t ktN = (size_t)kt * N, ct = 2 * ktN;
+    const u64 *ap = a + (size_t)o * T * ct + (size_t)l * N + x, *bp = b + (size_t)l * N + x;
+    U128 r0 = {0, 0}, r1 = {0, 0}, r2 = {0, 0};
+    for (int j0 = 0; j0 < T; j0 += 4) {
+        U128 s0 = {0, 0}, s1 = {0, 0}, s2 = {0, 0};
+        const int j1 = min(T, j0 + 4);
+        for (int j = j0; j < j1; j++) {
+            const u64 a0 = __ldcs(ap + (size_t)j * ct), a1 = __ldcs(ap + (size_t)j * ct + ktN);
+            const u64 b0 = __ldg(bp + (size_t)j * ct), b1 = __ldg(bp + (size_t)j * ct + ktN);
+            mac128(s0, a0, b0);
+            mac128(s1, a0, b1);
+            mac128(s1, a1, b0);
+            mac128(s2, a1, b1);
+        }
+        add128(r0, barrett128(s0, m));
+        add128(r1, barrett128(s1, m));
+        add128(r2, barrett128(s2, m));
+    }
+    u64 *dp = d + (size_t)o * 3 * ktN + (size_t)l * N + x;
+    dp[0] = barrett128(r0, m);
+    dp[ktN] = barrett128(r1, m);
+    dp[2 * ktN] = barrett128(r2, m);
+}
+
 // ---- times t, fast_floor (q u Bsk -> Bsk), fastbconv_sk (Bsk -> q)
 // EPI: the FloorEpi epilogue on every output word (A v, + B x on c0 and c1, + Delta C on c0)
 // PAIR (with EPI): output ciphertext c is the floor of product 2c minus the floor of product 2c + 1, then the epilogue.  The thread
@@ -253,6 +289,12 @@ cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, c
 cudaError_t launch_behz_tensor(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConst *bc, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     k_behz_tensor<<<blocks_for(((size_t)n * kt) << logn), 256, 0, s>>>(a, b, d, n, logn, bc);
+    return cudaGetLastError();
+}
+cudaError_t launch_behz_tensor_mac(const u64 *a, const u64 *b, u64 *d, int n_out, int T, int kt, int logn, const BehzConst *bc, cudaStream_t s) {
+    if (n_out <= 0) return cudaSuccess;
+    if (logn < 8) return cudaErrorInvalidValue;
+    k_behz_tensor_mac<<<(unsigned)((size_t)n_out * ((size_t)1 << (logn - 8)) * kt), 256, 0, s>>>(a, b, d, n_out, T, logn, bc);
     return cudaGetLastError();
 }
 cudaError_t launch_ks_mac(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn, const BehzConst *bc,

@@ -88,6 +88,52 @@ __global__ void __launch_bounds__(256) k_behz_tensor_fp(const u64 *a, const u64 
     }
 }
 
+// Sum of T tensor products per output in the NTT domain (op_multiply_sum): d[o] = sum_j a[o T + j] (x) b[j], i.e. per residue l of q u Bsk
+//   d0 = sum a0 b0,   d1 = sum (a0 b1 + a1 b0),   d2 = sum a1 b1
+// a [n_out T][2][kt][N] (the column operands, streamed once), b [T][2][kt][N] (shared by every output), d [n_out][3][kt][N] in
+// k_behz_tensor_fp's layout.  One thread per (output, residue, coefficient pair) keeps the six sums in registers.  CTA order: output
+// fastest, then the 512-coefficient tile, then the residue -- the CTAs of one (l, tile) run together and read the shared b words through
+// L2, as k_diag_mac orders its giant steps.  Arithmetic as in k_ks_mac_fp: fmodmul of canonical or lazy operands (the lazy forward output's
+// A^2 p < 2^51 bound of fp_schedule), dadd, re-centred after every 8th term (d1 gains two fresh products, <= 1.02 p, per term: 8.7 p at
+// most between re-centrings) and at the end, so the outputs are within the inverse transform's input bound (|.| <= 0.51 p < 1.25 p).
+template <bool LAZY>
+__global__ void __launch_bounds__(256) k_behz_tensor_mac_fp(const u64 *__restrict__ a, const u64 *__restrict__ b, u64 *__restrict__ d, int n_out,
+                                                           int T, int logn, const __grid_constant__ BehzConstF F) {
+    const int N = 1 << logn, k = F.k, kt = k + F.kb, tiles = N >> 9;
+    const int o = blockIdx.x % n_out, tile = (blockIdx.x / n_out) % tiles, l = blockIdx.x / (n_out * tiles);
+    const int x = (tile << 9) + 2 * threadIdx.x;
+    const double p = l < k ? F.qd[l] : F.bd[l - k], pinv = l < k ? F.qinv[l] : F.binv[l - k];
+    const size_t ktN = (size_t)kt * N, ct = 2 * ktN;
+    const u64 *ap = a + (size_t)o * T * ct + (size_t)l * N + x, *bp = b + (size_t)l * N + x;
+    auto ld = [](const u64 *q, bool stream) {
+        const ulonglong2 v = stream ? __ldcs(reinterpret_cast<const ulonglong2 *>(q)) : __ldg(reinterpret_cast<const ulonglong2 *>(q));
+        return LAZY ? make_double2(__longlong_as_double((long long)v.x), __longlong_as_double((long long)v.y)) : make_double2(u2d(v.x), u2d(v.y));
+    };
+    double s[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}}; // [polynomial][coefficient of the pair]
+    for (int j = 0; j < T; j++) {
+        const double2 a0 = ld(ap + (size_t)j * ct, true), a1 = ld(ap + (size_t)j * ct + ktN, true); // each column word is read once
+        const double2 b0 = ld(bp + (size_t)j * ct, false), b1 = ld(bp + (size_t)j * ct + ktN, false);
+        s[0][0] = __dadd_rn(s[0][0], fmodmul(a0.x, b0.x, p, pinv));
+        s[0][1] = __dadd_rn(s[0][1], fmodmul(a0.y, b0.y, p, pinv));
+        s[1][0] = __dadd_rn(s[1][0], __dadd_rn(fmodmul(a0.x, b1.x, p, pinv), fmodmul(a1.x, b0.x, p, pinv)));
+        s[1][1] = __dadd_rn(s[1][1], __dadd_rn(fmodmul(a0.y, b1.y, p, pinv), fmodmul(a1.y, b0.y, p, pinv)));
+        s[2][0] = __dadd_rn(s[2][0], fmodmul(a1.x, b1.x, p, pinv));
+        s[2][1] = __dadd_rn(s[2][1], fmodmul(a1.y, b1.y, p, pinv));
+        if ((j & 7) == 7) {
+#pragma unroll
+            for (int u = 0; u < 3; u++) { s[u][0] = frecenter(s[u][0], p, pinv); s[u][1] = frecenter(s[u][1], p, pinv); }
+        }
+    }
+    u64 *dp = d + (size_t)o * 3 * ktN + (size_t)l * N + x;
+#pragma unroll
+    for (int u = 0; u < 3; u++) {
+        const double v0 = frecenter(s[u][0], p, pinv), v1 = frecenter(s[u][1], p, pinv);
+        const u64 pu = (u64)p;
+        *reinterpret_cast<ulonglong2 *>(dp + (size_t)u * ktN) =
+            LAZY ? make_ulonglong2(lazy_bits(v0), lazy_bits(v1)) : make_ulonglong2(fsmall_u(v0, pu), fsmall_u(v1, pu));
+    }
+}
+
 // The floor kernels' epilogue (FloorEpi; EPI = true instantiations only): v is residue i (any integer |v| < 2^52) of output polynomial
 // `part` of ciphertext ct at coefficient x, xs the same coefficient of the input's polynomial `part` (part < 2), cs the same coefficient
 // of ct's Delta-scaled constant plaintext (c0 only; nullptr: the constant polynomial C).  Returns A v + B x + Delta C, |r| < 2.1 p: the
@@ -464,6 +510,15 @@ cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int
     if (n <= 0) return cudaSuccess;
     if (lazy) k_behz_tensor_fp<true><<<blocks_for(((size_t)n * kt) << logn), 256, 0, s>>>(a, b, d, n, logn, *f);
     else k_behz_tensor_fp<false><<<blocks_for(((size_t)n * kt) << logn), 256, 0, s>>>(a, b, d, n, logn, *f);
+    return cudaGetLastError();
+}
+cudaError_t launch_behz_tensor_mac_fp(const u64 *a, const u64 *b, u64 *d, int n_out, int T, int kt, int logn, const BehzConstF *f, int lazy,
+                                      cudaStream_t s) {
+    if (n_out <= 0) return cudaSuccess;
+    if (logn < 9) return cudaErrorInvalidValue; // whole 512-coefficient tiles
+    const unsigned grid = (unsigned)((size_t)n_out * ((size_t)1 << (logn - 9)) * kt);
+    if (lazy) k_behz_tensor_mac_fp<true><<<grid, 256, 0, s>>>(a, b, d, n_out, T, logn, *f);
+    else k_behz_tensor_mac_fp<false><<<grid, 256, 0, s>>>(a, b, d, n_out, T, logn, *f);
     return cudaGetLastError();
 }
 cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi,

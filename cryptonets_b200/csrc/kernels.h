@@ -223,6 +223,11 @@ cudaError_t launch_behz_lift_bsk_fp(const u64 *const *ct_ptrs, u64 *out, int n, 
 cudaError_t launch_behz_square_fused(const u64 *const *ct_ptrs, const u64 *lift_bsk, u64 *d, int n_ct, int k, int kt, int logn, const NttTab *tabs,
                                      cudaStream_t s);
 cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
+// sums of T tensor products per output: d[o] = sum_j a[o T + j] (x) b[j], a [n_out T][2][kt][N] and b [T][2][kt][N] in NTT form, d
+// [n_out][3][kt][N] as launch_behz_tensor writes one product (lazy: lazy doubles in and out, else canonical words)
+cudaError_t launch_behz_tensor_mac_fp(const u64 *a, const u64 *b, u64 *d, int n_out, int T, int kt, int logn, const BehzConstF *f, int lazy,
+                                      cudaStream_t s);
+cudaError_t launch_behz_tensor_mac(const u64 *a, const u64 *b, u64 *d, int n_out, int T, int kt, int logn, const BehzConst *bc, cudaStream_t s);
 // canonical input; lazy input takes the folded kernel below
 cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr,
                                 bool pair = false);

@@ -412,6 +412,65 @@ std::vector<u64> standard_galois_elts(uint32_t N) {
     return out;
 }
 
+// ---- K_c (DESIGN 4.14).  A lifted word is x + c Q with |x + c Q| < Q (1 + k / m~) (c in {0, 1}; the centred m~ halves it), so a coefficient
+// of a sum of K tensor products is below 2 K N Q^2 (1 + k / m~)^2 (d1 adds two negacyclic products of N terms each).  fast_floor returns
+// y = floor(t X / Q) - e with 0 <= e < k, so |y| < 2 K N t Q (1 + k / m~)^2 + k + 1, and fastbconv_sk recovers y exactly while its alpha,
+// which lies in (-|y| / B, na + |y| / B), stays inside the centred range of m_sk: |y| < B ((m_sk - 1) / 2 - na).  K_c is the largest K
+// meeting both for the largest t, at least 1 (one product per floor is what op_multiply does) and at most INT32_MAX.
+namespace {
+typedef std::vector<u64> Big; // little-endian 64-bit limbs
+Big big_of(u64 v) { return Big{v}; }
+Big big_mul(const Big &a, u64 m) {
+    Big r(a.size() + 1, 0);
+    unsigned __int128 carry = 0;
+    for (size_t i = 0; i < a.size(); i++) {
+        const unsigned __int128 v = (unsigned __int128)a[i] * m + carry;
+        r[i] = (u64)v;
+        carry = v >> 64;
+    }
+    r[a.size()] = (u64)carry;
+    while (r.size() > 1 && r.back() == 0) r.pop_back();
+    return r;
+}
+Big big_sub(Big a, u64 v) { // a >= v
+    for (size_t i = 0; i < a.size() && v; i++) {
+        const u64 before = a[i];
+        a[i] -= v;
+        v = a[i] > before ? 1 : 0;
+    }
+    while (a.size() > 1 && a.back() == 0) a.pop_back();
+    return a;
+}
+int big_cmp(const Big &a, const Big &b) {
+    if (a.size() != b.size()) return a.size() < b.size() ? -1 : 1;
+    for (size_t i = a.size(); i-- > 0;)
+        if (a[i] != b[i]) return a[i] < b[i] ? -1 : 1;
+    return 0;
+}
+double big_log2(const Big &a) { return 64.0 * (double)(a.size() - 1) + std::log2((double)a.back()); }
+} // namespace
+static int product_sum_terms(const std::vector<u64> &q, const std::vector<u64> &bsk, const std::vector<u64> &t, uint32_t N) {
+    const int k = (int)q.size(), na = (int)bsk.size() - 1;
+    const u64 msk = bsk[na], MT = 1ULL << 32;
+    u64 tmax = 0;
+    for (u64 v : t) tmax = std::max(tmax, v);
+    // limit = (B ((m_sk - 1) / 2 - na) - k - 1) m~^2,   per term = 2 N t Q (m~ + k)^2:   K_c = the largest K with K * per term < limit
+    Big limit = big_of((msk - 1) / 2 - (u64)na);
+    for (int j = 0; j < na; j++) limit = big_mul(limit, bsk[j]);
+    limit = big_mul(big_mul(big_sub(limit, (u64)k + 1), MT), MT);
+    Big per = big_of(2ULL * N);
+    per = big_mul(big_mul(big_mul(per, tmax), MT + (u64)k), MT + (u64)k);
+    for (u64 p : q) per = big_mul(per, p);
+    if (big_log2(limit) - big_log2(per) > 32.0) return INT32_MAX;
+    u64 lo = 0, hi = 1ULL << 33; // K * per < limit holds at lo and fails at hi
+    while (hi - lo > 1) {
+        const u64 mid = (lo + hi) / 2;
+        if (big_cmp(big_mul(per, mid), limit) < 0) lo = mid;
+        else hi = mid;
+    }
+    return (int)std::max<u64>(1, std::min<u64>(lo, INT32_MAX));
+}
+
 Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *coeff, int k, int dbc_relin, int dbc_galois, int device) {
     if (P < 1 || P > 16) throw Error(-1, "need 1..16 plaintext primes");
     int logN = 0;
@@ -480,6 +539,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     const int kb = (int)c.bsk.size();
     const u64 M_SK = c.bsk[kb - 1];
     c.kb = kb;
+    c.sum_terms = product_sum_terms(c.q, c.bsk, c.t, N);
     c.streams.resize(P);
     for (int i = 0; i < P; i++) CNHE_CUDA(cudaStreamCreateWithFlags(&c.streams[i], cudaStreamNonBlocking));
     c.stream = c.streams[0];
@@ -1033,6 +1093,75 @@ void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const st
         multiply_chunk(c, ch, a, b, c0, m, out3 + (size_t)c0 * 3 * c.k * c.N, fused, epi);
     }
     c.note(Context::OP_MULTIPLY, ch, n);
+}
+int multiply_sum_wave(const Context &c, int T) {
+    const size_t N = c.N, kt = (size_t)c.k + c.kb, lifted = 2 * kt * N;
+    // resident for the chunk: its T shared operands; per output: T lifted columns, the summed product and its floor
+    const size_t fixed = (size_t)T * lifted, per = (size_t)T * lifted + 3 * kt * N + 3 * (size_t)c.k * N, cap = (size_t)1 << 30; // 8 GiB
+    if (fixed + per > cap) return 0;
+    return (int)std::min<size_t>((cap - fixed) / per, (size_t)INT32_MAX);
+}
+void op_multiply_sum(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, int T, int n_out, u64 *out2,
+                     const int *slots) {
+    if (T < 1 || n_out < 1 || a.size() != (size_t)n_out * T || b.size() != (size_t)T) throw Error(-1, "bad product-sum shape");
+    const int Tc = std::min(T, c.sum_terms);
+    const int wave = multiply_sum_wave(c, Tc);
+    if (wave < 1) throw Error(-1, "a chunk of the product sum needs more than 8 GiB of scratch next to one output");
+    (void)relin_keys(c, ch, n_out, slots); // a missing key fails before any launch
+    const int k = c.k, kt = k + c.kb;
+    const size_t N = c.N, lifted = (size_t)2 * kt * N, s3 = (size_t)3 * k * N;
+    const int fpt = fp_range(c, 0, kt);
+    const int lazy = c.lazy && fpt ? 1 : 0;
+    const int fmt = fpt | (lazy ? NTT_IN_F | NTT_OUT_F : 0);
+    // BEHZ lift and forward transforms of n ciphertexts into [n][2][kt][N] (as multiply_chunk lifts its operands)
+    auto lift = [&](const std::vector<const u64 *> &cts, u64 *dst) {
+        const int n = (int)cts.size();
+        const u64 *const *dev = upload_ptrs(c, cts);
+        {
+            PROF(2, 8.0 * N * n * 2 * (k + kt));
+            if (c.fp_elementwise) c.check(launch_behz_lift_fp(dev, dst, n, c.logN, &c.h_bf, lazy, c.stream), "behz_lift_fp");
+            else c.check(launch_behz_lift(dev, dst, n, c.logN, c.d_bc, c.stream), "behz_lift");
+        }
+        PROF(0, 16.0 * N * n * 2 * kt);
+        c.check(launch_ntt_forward(dst, dst, n * 2 * kt, c.logN, c.d_tabs, 0, kt, fmt, c.stream), "ntt_forward");
+    };
+    WsScope scope(c);
+    u64 *Y = c.ws_alloc((size_t)n_out * s3); // the floors of the chunks, summed
+    for (int j0 = 0; j0 < T; j0 += Tc) {
+        WsScope chunk(c);
+        const int nt = std::min(Tc, T - j0);
+        u64 *S = c.ws_alloc((size_t)nt * lifted);
+        lift(std::vector<const u64 *>(b.begin() + j0, b.begin() + j0 + nt), S);
+        for (int o0 = 0; o0 < n_out; o0 += wave) {
+            WsScope w(c);
+            const int m = std::min(wave, n_out - o0);
+            std::vector<const u64 *> pa;
+            for (int o = o0; o < o0 + m; o++) pa.insert(pa.end(), a.begin() + (size_t)o * T + j0, a.begin() + (size_t)o * T + j0 + nt);
+            u64 *A = c.ws_alloc((size_t)m * nt * lifted), *D = c.ws_alloc((size_t)m * 3 * kt * N);
+            lift(pa, A);
+            {
+                // HBM: every column word once, the shared words once (the outputs' CTAs of one tile read them out of L2), the sums written once
+                PROF(2, 8.0 * N * ((double)m * nt * 2 * kt + (double)nt * 2 * kt + (double)m * 3 * kt));
+                if (c.fp_elementwise) c.check(launch_behz_tensor_mac_fp(A, S, D, m, nt, kt, c.logN, &c.h_bf, lazy, c.stream), "behz_tensor_mac_fp");
+                else c.check(launch_behz_tensor_mac(A, S, D, m, nt, kt, c.logN, c.d_bc, c.stream), "behz_tensor_mac");
+            }
+            {
+                PROF(1, 16.0 * N * m * 3 * kt);
+                c.check(launch_ntt_inverse(D, D, m * 3 * kt, c.logN, c.d_tabs, 0, kt, fmt, c.stream), "ntt_inverse");
+            }
+            u64 *dst = Y + (size_t)o0 * s3;
+            if (j0 == 0) {
+                multiply_floor(c, ch, D, m, lazy, dst);
+            } else { // the chunk's floor added mod q to the earlier chunks' (the add kernel over the three polynomials)
+                u64 *F = c.ws_alloc((size_t)m * s3);
+                multiply_floor(c, ch, D, m, lazy, F);
+                c.check(launch_ct_add(dst, F, dst, (size_t)m * s3, k, c.logN, c.d_bc, 0, c.stream), "ct_add");
+            }
+        }
+    }
+    c.op_count[Context::OP_MULTIPLY] += (uint64_t)n_out * T;
+    c.op_count[Context::OP_ADD] += (uint64_t)n_out * (T - 1);
+    op_relinearize(c, ch, Y, n_out, out2, slots);
 }
 void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots) {
     const KsKeys keys = relin_keys(c, ch, n, slots);

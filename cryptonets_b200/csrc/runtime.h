@@ -129,6 +129,8 @@ struct Context {
     // the diagonal product's MAC over diagonals held in NTT form: k_diag_mac_resident with 2, 4 or 8 diagonals' loads issued together,
     // or 0 for k_diag_mac (option "diag_mac_resident"; same outputs either way)
     int diag_mac_resident = 2;
+    // K_c of op_multiply_sum: the most tensor products whose sum the BEHZ floor still rounds exactly in this context's base Bsk (DESIGN 4.14)
+    int sum_terms = 1;
     int chunk = 1024; // ciphertexts per kernel wave (upper bound: wave() also keeps a wave's scratch under ~8 GiB)
     int wave(size_t words_per_ct) const { // ciphertexts per wave for an operation needing `words_per_ct` scratch words per ciphertext
         const size_t fit = ((size_t)1 << 30) / (words_per_ct ? words_per_ct : 1); // 2^30 words = 8 GiB
@@ -226,6 +228,15 @@ void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const 
 // key switch per output (the cubic activation's second level); slots then has n entries
 void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2,
                        const int *slots = nullptr, const FloorEpi *epi = nullptr, bool pair = false);
+// Sums of products with one floor per chunk and one relinearisation per output (DESIGN 4.14): out2[o] = relinearize(sum over the chunks of
+// floor(sum_{j in chunk} a[o T + j] (x) b[j])), the chunks T terms split into runs of at most c.sum_terms in index order, their floors added
+// mod q.  a: n_out * T ciphertexts (output o's terms at o T + j), b: T ciphertexts shared by every output.  Each ciphertext is lifted and
+// transformed once.  Counted as n_out T multiplications, n_out (T - 1) additions and n_out relinearisations.  CNHE_ERR_INVALID when a
+// chunk and one output's operands need more than 8 GiB of scratch (multiply_sum_wave == 0); slots as in op_relinearize (n_out entries)
+void op_multiply_sum(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, int T, int n_out, u64 *out2,
+                     const int *slots = nullptr);
+// outputs per wave of op_multiply_sum next to a chunk of T terms, or 0 when not even one fits under the 8 GiB scratch cap
+int multiply_sum_wave(const Context &c, int T);
 // the FloorEpi constants of A, B, C (residues mod the channel's t): A and B lifted into every q_l as multiply_plain lifts a constant
 // plaintext, C scaled as add_plain scales it
 FloorEpi floor_epi(const Context &c, int ch, u64 A, u64 B, u64 C);

@@ -2302,6 +2302,49 @@ extern "C" int cnhe_mat_mul_colmajor_sparse(cnhe_ctx *h, const cnhe_vec *const *
     }
     API_END
 }
+// cnhe_mat_mul_colmajor_sparse with both operands encrypted, the products' relinearisation deferred past their sum (DESIGN 4.14): per
+// channel one op_multiply_sum over the K terms of every output block, which lifts and transforms each column block and each sparse element
+// once, floors each chunk of at most K_c summed products once and relinearises each output block once
+extern "C" int cnhe_mat_mul_colmajor_sparse_deferred(cnhe_ctx *h, const cnhe_vec *const *cols, int K, const cnhe_vec *sparse, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (!cols || !out) fail("bad arguments");
+    if (K < 1) fail("empty matrix");
+    same_ctx(c, sparse);
+    for (int i = 0; i < K; i++) same_ctx(c, cols[i]);
+    if ((uint64_t)K != sparse->dim) fail("dimensions do not match");
+    if (sparse->format != CNHE_SPARSE) fail("expecting a sparse vector");
+    if (!cols[0]->enc && !sparse->enc) fail("at least one parameter has to be encrypted");
+    for (int i = 0; i < K; i++)
+        if (!cols[i]->enc || !sparse->enc)
+            fail("the deferred product needs encrypted columns and an encrypted sparse vector (cnhe_mat_mul_colmajor_sparse serves the rest)");
+    for (int i = 1; i < K; i++)
+        if (cols[i]->dim != cols[0]->dim || cols[i]->blocks != cols[0]->blocks) fail("dimensions do not match");
+    {
+        std::vector<const cnhe_vec *> all(cols, cols + K);
+        all.push_back(sparse);
+        use_slot(c, all.data(), K + 1);
+    }
+    const int bl = cols[0]->blocks;
+    cnhe_vec *o = new_vec(c, cols[0]->dim, cols[0]->scale * sparse->scale, CNHE_DENSE, true, bl);
+    std::unique_ptr<cnhe_vec> guard(o);
+    alloc_channels(o);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        std::vector<const u64 *> a, b;
+        for (int i = 0; i < bl; i++)
+            for (int kk = 0; kk < K; kk++) a.push_back(cols[kk]->block(ch, i));
+        for (int kk = 0; kk < K; kk++) b.push_back(sparse->block(ch, kk));
+        op_multiply_sum(c, ch, a, b, K, bl, o->block(ch, 0));
+        c.op_count[Context::OP_ADD_MANY_ITEMS] += (uint64_t)K * bl; // the sums, booked as the existing call books its AddMany items
+    }
+    *out = guard.release();
+    API_END
+}
+extern "C" int cnhe_context_product_sum_terms(const cnhe_ctx *h, int *terms) {
+    if (!h || !terms) return set_err(CNHE_ERR_INVALID, "null argument");
+    *terms = h->c->sum_terms;
+    return CNHE_OK;
+}
 // RowMajor matrix x vector (EncryptedSealBfvMatrix.cs:79-120): per row DotProduct(row, v) = PointwiseMultiply + SumAllSlots, then
 // GenerateSparseOfArray, or (ForceDenseFormat) a one-hot mask per row and the sum of all rows.  All rows go through each stage
 // together instead of one DotProduct per row.

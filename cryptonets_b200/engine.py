@@ -570,6 +570,19 @@ class Engine:
         check(self.L.cnhe_mat_mul_colmajor_sparse(self.h, _vec_array(cols), len(cols), sparse.h, C.byref(out)))
         return Vec(self, out)
 
+    def mat_mul_colmajor_sparse_deferred(self, cols, sparse):
+        """mat_mul_colmajor_sparse with encrypted columns and an encrypted sparse vector, one relinearisation per output block: the products
+        of each chunk of at most product_sum_terms() columns are summed before one BEHZ floor (cnhe.h, DESIGN.md 4.14)"""
+        out = VECP()
+        check(self.L.cnhe_mat_mul_colmajor_sparse_deferred(self.h, _vec_array(cols), len(cols), sparse.h, C.byref(out)))
+        return Vec(self, out)
+
+    def product_sum_terms(self):
+        """K_c: the most products one floor of mat_mul_colmajor_sparse_deferred sums in this context"""
+        n = C.c_int()
+        check(self.L.cnhe_context_product_sum_terms(self.h, C.byref(n)))
+        return n.value
+
     def mat_mul_rowmajor(self, rows, v, force_dense=False):
         out = VECP()
         check(self.L.cnhe_mat_mul_rowmajor(self.h, _vec_array(rows), len(rows), v.h, int(force_dense), C.byref(out)))

@@ -7,7 +7,7 @@ Errors surface as Python exceptions carrying the reference's message (the refere
 import numpy as np
 
 from .engine import ALL_SLOTS, Engine, Vec
-from .interfaces import EMatrixFormat, EVectorFormat
+from .interfaces import EMatrixFormat, EVectorFormat, check_deferred_mul
 
 
 class B200BfvEnvironment:
@@ -160,8 +160,13 @@ class B200BfvMatrix:
             raise Exception("MulRows expects a RowMajor matrix")
         return B200BfvVector(self.factory, self.eng.mat_mul_rowmajor_shard([r.vec for r in self.vectors], v.vec, ForceDenseFormat, first_row, total_rows))
 
-    def Mul(self, v, env=None, ForceDenseFormat=False):
+    def Mul(self, v, env=None, ForceDenseFormat=False, DeferRelinearization=False):
+        """DeferRelinearization (B200-specific, column-major encrypted matrix times an encrypted sparse vector only): sum the products
+        before relinearising, one relinearisation per output block (Engine.mat_mul_colmajor_sparse_deferred); same decrypted values"""
         f = self.factory
+        if DeferRelinearization:
+            check_deferred_mul(self, v, ForceDenseFormat)
+            return B200BfvVector(f, self.eng.mat_mul_colmajor_sparse_deferred([c.vec for c in self.vectors], v.vec))
         if self.Format == EMatrixFormat.ColumnMajor:
             if ForceDenseFormat:
                 raise Exception("Forcing dense format is available only in RowMajor mode")

@@ -5,7 +5,7 @@ it as the source of EncryptLayer's input matrices, as the mock for layer tests, 
 result is compared with; it plays the same three roles here.  It is not a fallback of the encrypted path."""
 import numpy as np
 
-from .interfaces import EMatrixFormat, EVectorFormat
+from .interfaces import EMatrixFormat, EVectorFormat, check_deferred_mul
 
 
 def _round(a):
@@ -168,7 +168,10 @@ class RawMatrix:
     def Decrypt(self, env=None):
         return self.m / self.Scale
 
-    def Mul(self, v, env=None, ForceDenseFormat=False):
+    def Mul(self, v, env=None, ForceDenseFormat=False, DeferRelinearization=False):
+        """DeferRelinearization changes nothing in exact arithmetic; the shapes the encrypted backend refuses with it are refused here too"""
+        if DeferRelinearization:
+            check_deferred_mul(self, v, ForceDenseFormat, encrypted=False)
         return RawVector._of(self.m @ v.v, self.Scale * v.Scale, v.BlockSize)
 
     def _check(self, m):

@@ -59,6 +59,9 @@ int cnhe_context_plain_moduli(const cnhe_ctx *, uint64_t *out_P);
 /* the BEHZ auxiliary base Bsk (auxiliary primes, m_sk last); out may be NULL to query the count.  NTT modulus ids:
  * 0..k-1 coefficient primes, k..k+count-1 Bsk, k+count+c plaintext modulus c */
 int cnhe_context_bsk_moduli(const cnhe_ctx *, uint64_t *out, int *count);
+/* K_c of cnhe_mat_mul_colmajor_sparse_deferred: the most ciphertext products whose sum one BEHZ floor rounds exactly in this context's
+ * Bsk, derived at context creation (DESIGN.md 4.14); at least 1, at most INT32_MAX */
+int cnhe_context_product_sum_terms(const cnhe_ctx *, int *terms);
 int cnhe_context_galois_elts(const cnhe_ctx *, uint64_t *out);
 /* options: "behz_centered_mtilde" (0/1), "chunk" (ciphertexts per multiply/key-switch wave), "multi_stream" (1: one CUDA
  * stream per plaintext modulus, default; 0: everything on one stream; refused while imported batches are alive),
@@ -251,6 +254,18 @@ int cnhe_vecs_rotate(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int amount,
 /* ---- IMatrix.Mul and the fused layer entry points ------------------------------------------------------------------ */
 /* ColumnMajor matrix x sparse vector ("EncryptedSealBfvMatrix.cs:70-78" -> "AtomicSealBfvVector.cs:434-521") */
 int cnhe_mat_mul_colmajor_sparse(cnhe_ctx *, const cnhe_vec *const *cols, int K, const cnhe_vec *sparse, cnhe_vec **out);
+/* The same product with encrypted columns and an encrypted sparse vector, relinearised once per output block instead of once per product
+ * (DESIGN.md 4.14).  Per plaintext prime and output block i:
+ *   X_i = sum_k lift(cols[k]_i) (x) lift(sparse_k)   (size 3, base q u Bsk, summed in NTT form)
+ *   Y_i = sum over chunks of floor_BEHZ(INTT(X_i restricted to the chunk's terms))   (mod q)
+ *   out_i = relinearize(Y_i)
+ * The K terms are cut into chunks of at most K_c (cnhe_context_product_sum_terms) in index order; each chunk is floored once.  The output
+ * decrypts to cnhe_mat_mul_colmajor_sparse's values, dense, at scale(cols) scale(sparse), with the columns' dimension and blocks, but its
+ * words differ: one floor-rounding term per chunk and one key-switch term per output instead of K of each.  Argument checks and messages are
+ * cnhe_mat_mul_colmajor_sparse's; the columns must share dimension and blocks, every operand must be encrypted and in one key slot
+ * (CNHE_ERR_INVALID otherwise, naming the existing call), and a chunk whose lifted operands and one output's sums need more than 8 GiB of
+ * scratch is refused.  Counted as K bl Multiply, bl (K - 1) Addition, bl Relinearize and K bl AddMany items. */
+int cnhe_mat_mul_colmajor_sparse_deferred(cnhe_ctx *, const cnhe_vec *const *cols, int K, const cnhe_vec *sparse, cnhe_vec **out);
 /* RowMajor plain matrix x encrypted dense vector ("EncryptedSealBfvMatrix.cs:79-120" -> DotProduct per row = MultiplyPlain +
  * SumAllSlots, "AtomicSealBfvVector.cs:964-977,888-955"); force_dense: one-hot mask per row, rows summed into one dense vector */
 int cnhe_mat_mul_rowmajor(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows, const cnhe_vec *v, int force_dense, cnhe_vec **out);

@@ -31,6 +31,7 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_coeff_moduli(IntPtr a0, ulong[] out_k);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_plain_moduli(IntPtr a0, ulong[] out_P);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_bsk_moduli(IntPtr a0, ulong[] @out, out int count);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_product_sum_terms(IntPtr a0, out int terms);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_galois_elts(IntPtr a0, ulong[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_set_option(IntPtr a0, string name, long value);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_sync(IntPtr a0);
@@ -90,6 +91,7 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_rotate(IntPtr a0, IntPtr[] vecs, int n, int amount, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_stack_batch(IntPtr a0, IntPtr[] vecs, int n, int B, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_colmajor_sparse(IntPtr a0, IntPtr[] cols, int K, IntPtr sparse, out IntPtr @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_colmajor_sparse_deferred(IntPtr a0, IntPtr[] cols, int K, IntPtr sparse, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_rowmajor(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr v, int force_dense, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_mul_rowmajor_batch(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr[] vs, int B, int force_dense, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_mat_dot_rows_batch(IntPtr a0, IntPtr[] rows, int n_rows, IntPtr[] vs, int B, ulong length, IntPtr[] @out);
@@ -269,6 +271,16 @@ namespace HEWrapper
             foreach (var v in Vectors) v.Write(str);
             str.WriteLine("<End LargeEncryptedMatrix>");
             str.Flush();
+        }
+        // B200-specific: an encrypted column-major matrix times an encrypted sparse vector with one relinearisation per output block
+        // (cnhe_mat_mul_colmajor_sparse_deferred; decrypts to Mul's values)
+        public IVector MulDeferred(IVector v)
+        {
+            if (!(v is B200BfvVector bv)) throw new Exception("expecting B200BfvVector");
+            if (Format != EMatrixFormat.ColumnMajor || !IsEncrypted || !bv.IsEncrypted)
+                throw new Exception("MulDeferred serves an encrypted column-major matrix times an encrypted sparse vector; use Mul");
+            Cnhe.Check(Cnhe.cnhe_mat_mul_colmajor_sparse_deferred(Ctx, Cnhe.Handles(Vectors), Vectors.Length, bv.Handle, out IntPtr r));
+            return new B200BfvVector(Factory, r);
         }
         public IVector Mul(IVector v, IComputationEnvironment env, bool ForceDenseFormat = false)
         {   // EncryptedSealBfvMatrix.cs:70-121
