@@ -74,6 +74,10 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
 cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab,
                                     const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn,
                                     const NttTab *tabs, cudaStream_t s);
+// The fused key switch with its digits read from int32 planes: digit d of ciphertext c is planes[(c * D + d) * N + i], |value| < min q_l
+// (the digit sums of a scalar-MAC layer over unrelinearised products, DESIGN 4.15); keys, base, out and key_tab as above
+cudaError_t launch_key_switch_planes(const int *planes, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab, const u64 *base,
+                                     size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s);
 // the fused key switch's packed key copy: n_polys canonical N-word polynomials (words < 2^48) -> 6N bytes each, thread-interleaved (ntt.cu)
 cudaError_t launch_pack_keys48(const u64 *key, uint4 *out, int n_polys, int logn, cudaStream_t s);
 // dst[b] = INTT(src[b]) + base[(b / base_group) * base_stride + (b % base_group) * N]  (mod p)
@@ -276,6 +280,13 @@ cudaError_t launch_mac_dense_imma(const u64 *const *in_ptrs, const void *wfrag, 
 struct UmBundle {
     int chunk0, n_chunks, a_off, n_out, out0;
 };
+// Digit mode of the wgmma MAC (size-3 inputs): the c2 digit sums of every output into int32 planes [D][N] instead of a reduced c2
+struct UmDigits {
+    int *const *planes;          // device, bundle order: each output's planes; null = no digit mode
+    int w, groups;               // digit width; digit groups of limbs / 2 digits per residue
+    unsigned mask;               // 2^w - 1
+    unsigned char first[KMAX], count[KMAX]; // per residue: its first digit and its number of digits (DigitMap order)
+};
 struct UmmaLaunch {
     const u64 *slab;            // input 0
     size_t slab_stride_words;   // distance between consecutive inputs
@@ -294,6 +305,7 @@ struct UmmaLaunch {
     int limbs, polys, k, logn;  // polys: 2, or 3 for size-3 inputs (slab_stride_words >= 3kN)
     const BehzConst *bc;
     PlainConst pc;
+    UmDigits dig;               // digit mode (polys == 3): outputs get c0 and c1 only (2kN words), c2 goes to the digit planes
 };
 bool mac_umma_fits(int a_bytes, int total_chunks, int n_out_total, int n_bundles, int limbs);
 void mac_umma_pack(const signed char *w, int rows, int cols, unsigned char *out); // cols a multiple of 32; out: cols / 32 * 4096 bytes

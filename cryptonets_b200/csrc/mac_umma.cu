@@ -126,12 +126,16 @@ __host__ __device__ inline UmSmem um_layout(int a_bytes, int total_chunks, int n
 }
 
 // wpack: per chunk 4096 bytes, weight (row r, tap kb of the chunk) at (r >> 3) * 256 + (kb >> 4) * 128 + (r & 7) * 16 + (kb & 15)
-template <int LIMBS>
+// DIG (digit mode, size-3 inputs, DESIGN 4.15): the tiles of c0 and c1 as above into 2kN-word outputs, then every tile of c2 once per
+// group of LIMBS / 2 key-switch digits.  A digit tile cuts each word at the digit boundaries instead of the byte boundaries, two limbs
+// per digit (bits [i w, i w + 8) and [i w + 8, (i + 1) w)), and its epilogue writes S = P_lo + 256 P_hi, the exact integer digit sum,
+// into the output's int32 plane of that digit (|S| < 2^31 is host-checked).  Same ring, same MMAs, same weights.
+template <int LIMBS, bool DIG>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1, const UmBundle *__restrict__ bundles, int n_bundles,
            const int *__restrict__ chunk_rows, int total_chunks, const unsigned char *__restrict__ wpack, int a_bytes,
            u64 *const *__restrict__ out_ptrs, const u64 *__restrict__ bias, int n_out_total, int polys, int k, int logn,
-           const BehzConst *__restrict__ bc, PlainConst pc, unsigned long long *prof) {
+           const BehzConst *__restrict__ bc, PlainConst pc, const __grid_constant__ UmDigits dg, unsigned long long *prof) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char *smem = smem_raw + ((1024u - (sptr(smem_raw) & 1023u)) & 1023u);
     // CNHE_UMMA_PROF=1: CTA 0 reports, per role, the cycles spent in each of its waits and in its work (prof[role * 4 + i])
@@ -151,7 +155,9 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
     static_assert((2 * UM_RAW_STAGES + 1) * 8 <= 256, "barrier block");
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int N = 1 << logn;
-    const int n_tiles = (int)(((size_t)polys * k << logn) / UM_TN);
+    // DIG: main tiles over c0 and c1, then dg.groups passes over the kN / 32 tiles of c2
+    const int n_main = (int)(((size_t)(DIG ? 2 : polys) * k << logn) / UM_TN), c2_tiles = (int)(((size_t)k << logn) / UM_TN);
+    const int n_tiles = DIG ? n_main + dg.groups * c2_tiles : n_main;
 
     if (tid == 0) {
         for (int i = 0; i < UM_RAW_STAGES; i++) { mb_init(raw_full + i, 1); mb_init(raw_empty + i, UM_CONSUMERS); }
@@ -177,7 +183,7 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
             for (int o = 0; o < a_bytes; o += UM_A_CHUNK) bulk_g2s(sw + o, wpack + o, UM_A_CHUNK, w_full);
             unsigned it = 0;
             for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const int col0 = tile * UM_TN;
+                const int col0 = (!DIG || tile < n_main) ? tile * UM_TN : (2 * c2_tiles + (tile - n_main) % c2_tiles) * UM_TN;
                 for (int b = 0; b < n_bundles; b++) {
                     const UmBundle bn = sbun[b];
                     for (int c = 0; c < bn.n_chunks; c++, it++) {
@@ -214,7 +220,9 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
     unsigned it = 0;
     long long t_d = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const size_t col0 = (size_t)tile * UM_TN;
+        const bool dig = DIG && tile >= n_main;
+        const int dgrp = dig ? (tile - n_main) / c2_tiles : 0; // digit tile: its group, and the coefficients it covers in its residue
+        const size_t col0 = dig ? (size_t)(2 * c2_tiles + (tile - n_main) % c2_tiles) * UM_TN : (size_t)tile * UM_TN;
         const int l = (int)((col0 >> logn) % k);
         const double p = smod[l * 8], pinv = smod[l * 8 + 1];
         const double c24 = smod[l * 8 + 2], c48 = smod[l * 8 + 5]; // 2^24, 2^48 mod p
@@ -240,6 +248,22 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
                     hi[j] = t.y;
                 }
                 mb_arrive(raw_empty + rs);
+                if (DIG && dig) { // limb a: half a & 1 of digit dgrp * LIMBS / 2 + a / 2 of the four words (0 past the residue's digits)
+                    const int nd = dg.count[l];
+#pragma unroll
+                    for (int a = 0; a < LIMBS; a++) {
+                        const int i = dgrp * (LIMBS / 2) + (a >> 1);
+                        unsigned w = 0;
+                        if (a < 2 * (LIMBS / 2) && i < nd) {
+                            const int sh = i * dg.w + 8 * (a & 1);
+                            const unsigned m = (a & 1) ? (dg.mask >> 8) : (dg.mask & 0xFFu);
+#pragma unroll
+                            for (int j = 0; j < 4; j++) w |= ((unsigned)((((u64)hi[j] << 32) | lo[j]) >> sh) & m) << (8 * j);
+                        }
+                        const int row = a * UM_TN + n;
+                        *reinterpret_cast<unsigned *>(bst + (row >> 3) * 256 + qh * 128 + (row & 7) * 16 + (lane & 3) * 4) = w;
+                    }
+                } else {
 #pragma unroll
                 for (int a = 0; a < LIMBS; a++) { // byte a of the four words -> one 32-bit word, three byte permutes
                     const unsigned sel = (a & 3) | (((a & 3) + 4) << 4);
@@ -248,6 +272,7 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
                     const unsigned w = __byte_perm(t01, t23, 0x5410);
                     const int row = a * UM_TN + n;
                     *reinterpret_cast<unsigned *>(bst + (row >> 3) * 256 + qh * 128 + (row & 7) * 16 + (lane & 3) * 4) = w;
+                }
                 }
                 fence_async_smem(); // generic-proxy stores -> visible to the tensor core's (async proxy) reads
                 consumers_sync();
@@ -271,6 +296,32 @@ k_mac_umma(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CU
             wgmma_wait<0>();
 #pragma unroll
             for (int a = 0; a < LIMBS; a++) acc_fence(acc[a]);
+            if (DIG && dig) {
+                if (active && (warp & 3) * 16 + wg * 64 < bn.n_out) {
+                    const int nd = dg.count[l], nc = (int)(col0 & (size_t)(N - 1)) + c0;
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const int m = r0 + 8 * h;
+                        if (m >= bn.n_out) continue;
+                        int *prow = dg.planes[bn.out0 + m] + nc;
+#pragma unroll
+                        for (int ii = 0; ii < LIMBS / 2; ii++) {
+                            const int i = dgrp * (LIMBS / 2) + ii;
+                            if (i >= nd) continue;
+                            int *o = prow + (size_t)(dg.first[l] + i) * N;
+#pragma unroll
+                            for (int j = 0; j < 4; j++) {
+                                const int e0 = 4 * j + 2 * h;
+                                const int v0 = acc[2 * ii][e0] + (int)((unsigned)acc[2 * ii + 1][e0] << 8);
+                                const int v1 = acc[2 * ii][e0 + 1] + (int)((unsigned)acc[2 * ii + 1][e0 + 1] << 8);
+                                asm volatile("st.global.v2.b32 [%0], {%1,%2};" ::"l"(o + 8 * j), "r"(v0), "r"(v1) : "memory");
+                            }
+                        }
+                    }
+                }
+                UM_ACC(t_d);
+                continue;
+            }
             if (active && (warp & 3) * 16 + wg * 64 < bn.n_out) { // warps whose 16 rows are all padding skip the arithmetic (uniform per warp)
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
@@ -318,12 +369,12 @@ int sm_count_cached() {
     return n;
 }
 
-template <int LIMBS>
+template <int LIMBS, bool DIG>
 cudaError_t umma_go(const CUtensorMap &map0, const CUtensorMap &map1, const UmmaLaunch &a, cudaStream_t s) {
     const UmSmem L = um_layout(a.a_bytes, a.total_chunks, a.n_out_total, a.n_bundles, LIMBS);
-    cudaError_t e = cudaFuncSetAttribute(k_mac_umma<LIMBS>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total);
+    cudaError_t e = cudaFuncSetAttribute(k_mac_umma<LIMBS, DIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total);
     if (e != cudaSuccess) return e;
-    const int n_tiles = (int)(((size_t)a.polys * a.k << a.logn) / UM_TN);
+    const int n_tiles = (int)((((size_t)(DIG ? 2 + a.dig.groups : a.polys)) * a.k << a.logn) / UM_TN);
     const int grid = std::min(sm_count_cached(), n_tiles);
     const bool want_prof = getenv("CNHE_UMMA_PROF") != nullptr; // read per launch: tests switch it on to see which kernel served a layer
     unsigned long long *prof = nullptr;
@@ -333,15 +384,15 @@ cudaError_t umma_go(const CUtensorMap &map0, const CUtensorMap &map1, const Umma
         cudaMemsetAsync(buf, 0, 16 * sizeof(unsigned long long), s);
         prof = buf;
     }
-    k_mac_umma<LIMBS><<<grid, UM_THREADS, L.total, s>>>(map0, map1, a.bundles, a.n_bundles, a.chunk_rows, a.total_chunks, a.wpack, a.a_bytes, a.out_ptrs, a.bias,
-                                                        a.n_out_total, a.polys, a.k, a.logn, a.bc, a.pc, prof);
+    k_mac_umma<LIMBS, DIG><<<grid, UM_THREADS, L.total, s>>>(map0, map1, a.bundles, a.n_bundles, a.chunk_rows, a.total_chunks, a.wpack, a.a_bytes,
+                                                             a.out_ptrs, a.bias, a.n_out_total, a.polys, a.k, a.logn, a.bc, a.pc, a.dig, prof);
     if (want_prof) {
         unsigned long long h[16];
         cudaMemcpyAsync(h, prof, sizeof(h), cudaMemcpyDeviceToHost, s);
         cudaStreamSynchronize(s);
-        fprintf(stderr, "[umma bundles=%d chunks/tile=%d outputs=%d weights=%d KB tiles/cta=%.1f] producer: wait_empty %llu issue %llu | "
+        fprintf(stderr, "[umma%s bundles=%d chunks/tile=%d outputs=%d weights=%d KB tiles/cta=%.1f] producer: wait_empty %llu issue %llu | "
                         "consumers: wait_raw %llu cut %llu mma %llu epilogue %llu (cycles, CTA 0)\n",
-                a.n_bundles, a.total_chunks, a.n_out_total, a.a_bytes / 1024, (double)n_tiles / grid, h[0], h[1], h[8], h[9], h[10], h[12]);
+                DIG ? " digits" : "", a.n_bundles, a.total_chunks, a.n_out_total, a.a_bytes / 1024, (double)n_tiles / grid, h[0], h[1], h[8], h[9], h[10], h[12]);
     }
     return cudaGetLastError();
 }
@@ -373,10 +424,19 @@ cudaError_t launch_mac_umma(const UmmaLaunch &a, cudaStream_t s) {
         if (e != cudaSuccess) return e;
     } else
         map1 = map0;
+    if (a.dig.planes) {
+        if (a.polys != 3) return cudaErrorInvalidValue;
+        switch (a.limbs) {
+        case 5: return umma_go<5, true>(map0, map1, a, s);
+        case 6: return umma_go<6, true>(map0, map1, a, s);
+        case 7: return umma_go<7, true>(map0, map1, a, s);
+        default: return cudaErrorInvalidValue;
+        }
+    }
     switch (a.limbs) {
-    case 5: return umma_go<5>(map0, map1, a, s);
-    case 6: return umma_go<6>(map0, map1, a, s);
-    case 7: return umma_go<7>(map0, map1, a, s);
+    case 5: return umma_go<5, false>(map0, map1, a, s);
+    case 6: return umma_go<6, false>(map0, map1, a, s);
+    case 7: return umma_go<7, false>(map0, map1, a, s);
     default: return cudaErrorInvalidValue;
     }
 }

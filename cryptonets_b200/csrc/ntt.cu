@@ -1155,11 +1155,14 @@ __global__ void __launch_bounds__(256) k_pack_keys48(const u64 *__restrict__ key
 #pragma unroll
     for (int g = 0; g < 6; g++) o[g * TR] = make_uint4(u[4 * g], u[4 * g + 1], u[4 * g + 2], u[4 * g + 3]);
 }
-template <int HLOGN, bool PK>
+// Plane source (PL): digit d of ciphertext c is int32 plane d of planes + c * D * N instead of a cut of the target words -- the digit
+// sums S = sum_j W_j digit_d(c2_j) of a scalar-MAC layer over unrelinearised squares (DESIGN 4.15).  |S| < min q_l (host-checked),
+// the same input bound as a canonical digit, so nothing after the loads changes; `target` and `ct_stride` are unused.
+template <int HLOGN, bool PK, bool PL>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(ks_fused_threads<HLOGN>(), HLOGN == 12 ? 2 : 4)
-k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *__restrict__ key, const uint4 *__restrict__ keyp,
-                   const u64 *const *__restrict__ key_tab, const u64 *__restrict__ base, size_t base_stride, u64 *__restrict__ out,
-                   const NttTab *__restrict__ tabs, int k, DigitMap dm) {
+k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const int *__restrict__ planes, const u64 *__restrict__ key,
+                   const uint4 *__restrict__ keyp, const u64 *const *__restrict__ key_tab, const u64 *__restrict__ base, size_t base_stride,
+                   u64 *__restrict__ out, const NttTab *__restrict__ tabs, int k, DigitMap dm) {
     constexpr int H = 1 << HLOGN, TR = ks_fused_threads<HLOGN>(), N = 2 * H;
     constexpr int R1 = HLOGN - 8, E1 = 1 << R1, LG1 = HLOGN - R1; // first pass: stage 0 on the loads, then R1 stages; then 4 + 4
     extern __shared__ __align__(16) u64 ks_raw[];
@@ -1215,7 +1218,15 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const u64 *
 #pragma unroll
             for (int e = 0; e < E1; e++) {
                 const int idx = tid + v * TR + (e << LG1);
-                const double a = cut(src[idx], shift), t = fmodmul(cut(src[idx + H], shift), w0, p, pinv);
+                double a, t;
+                if constexpr (PL) {
+                    const int *pl = planes + ((size_t)c * dm.D + d) * N;
+                    a = (double)pl[idx];
+                    t = fmodmul((double)pl[idx + H], w0, p, pinv);
+                } else {
+                    a = cut(src[idx], shift);
+                    t = fmodmul(cut(src[idx + H], shift), w0, p, pinv);
+                }
                 xs[v][e] = half ? __dsub_rn(a, t) : __dadd_rn(a, t);
             }
 #pragma unroll
@@ -1822,29 +1833,36 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
     });
     return cudaGetLastError();
 }
-template <int HL, bool PK>
-static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, const u64 *const *key_tab,
-                                   const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, const NttTab *tabs,
-                                   cudaStream_t s) {
-    cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL, PK>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
+template <int HL, bool PK, bool PL>
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const int *planes, const u64 *key, const uint4 *keyp,
+                                   const u64 *const *key_tab, const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm,
+                                   const NttTab *tabs, cudaStream_t s) {
+    cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL, PK, PL>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
     if (e != cudaSuccess) return e;
-    k_key_switch_fused<HL, PK><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, key, keyp, key_tab, base,
-                                                                                               base_stride, out, tabs, k, dm);
+    k_key_switch_fused<HL, PK, PL><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, planes, key, keyp, key_tab,
+                                                                                                   base, base_stride, out, tabs, k, dm);
     return cudaGetLastError();
 }
-template <int HL>
-static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *keyp, const u64 *const *key_tab,
-                                   const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, const NttTab *tabs,
-                                   cudaStream_t s) {
-    return keyp ? launch_ks_fused<HL, true>(target, ct_stride, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s)
-                : launch_ks_fused<HL, false>(target, ct_stride, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+template <int HL, bool PL>
+static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const int *planes, const u64 *key, const uint4 *keyp,
+                                   const u64 *const *key_tab, const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm,
+                                   const NttTab *tabs, cudaStream_t s) {
+    return keyp ? launch_ks_fused<HL, true, PL>(target, ct_stride, planes, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s)
+                : launch_ks_fused<HL, false, PL>(target, ct_stride, planes, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
 }
 cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab,
                                     const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn,
                                     const NttTab *tabs, cudaStream_t s) {
     if (n_ct <= 0) return cudaSuccess;
-    if (logn == 13) return launch_ks_fused<12>(target, ct_stride, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
-    if (logn == 12) return launch_ks_fused<11>(target, ct_stride, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+    if (logn == 13) return launch_ks_fused<12, false>(target, ct_stride, nullptr, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+    if (logn == 12) return launch_ks_fused<11, false>(target, ct_stride, nullptr, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+    return cudaErrorInvalidValue;
+}
+cudaError_t launch_key_switch_planes(const int *planes, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab, const u64 *base,
+                                     size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s) {
+    if (n_ct <= 0) return cudaSuccess;
+    if (logn == 13) return launch_ks_fused<12, true>(nullptr, 0, planes, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+    if (logn == 12) return launch_ks_fused<11, true>(nullptr, 0, planes, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
     return cudaErrorInvalidValue;
 }
 template <int HL>

@@ -1163,14 +1163,31 @@ void op_multiply_sum(Context &c, int ch, const std::vector<const u64 *> &a, cons
     c.op_count[Context::OP_ADD] += (uint64_t)n_out * (T - 1);
     op_relinearize(c, ch, Y, n_out, out2, slots);
 }
-void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots) {
+void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots, bool book) {
     const KsKeys keys = relin_keys(c, ch, n, slots);
     const int k = c.k;
     const size_t N = c.N;
     // the size-3 layout [c0 c1 c2] is consumed in place: c2 is the key-switch target, (c0, c1) the base it is added to
     const size_t s3 = (size_t)3 * k * N;
     op_key_switch(c, in3 + (size_t)2 * k * N, s3, n, keys, c.dm_relin, in3, s3, out2);
-    c.note(Context::OP_RELINEARIZE, ch, n, out2);
+    if (book) c.note(Context::OP_RELINEARIZE, ch, n, out2);
+}
+bool relin_planes_built(const Context &c) { return ks_fused_built(c); }
+void op_relinearize_planes(Context &c, int ch, const int *planes, int n, const u64 *base, u64 *out2, const int *slots) {
+    if (!ks_fused_built(c)) throw Error(-1, "the plane-source key switch needs the fused key switch (N = 4096 / 8192, lazy FP64 path)");
+    const KsKeys keys = relin_keys(c, ch, n, slots);
+    const int k = c.k;
+    const size_t N = c.N;
+    const DigitMap &dm = c.dm_relin;
+    const u64 *key_packed = keys.per_ct() ? (keys.packs.empty() ? nullptr : keys.packs[0]) : keys.packed;
+    WsScope scope(c);
+    const u64 *const *key_tab = nullptr;
+    if (keys.per_ct()) key_tab = upload_ptrs(c, key_packed ? keys.packs : keys.keys);
+    // HBM: the digit planes once (every residue's CTAs of a ciphertext share them through L2), the keys once, the output
+    PROF(3, 4.0 * N * n * dm.D + 8.0 * N * n * 2 * k + (key_packed ? 6.0 : 8.0) * N * dm.D * 2 * k);
+    c.check(launch_key_switch_planes(planes, keys.key, reinterpret_cast<const uint4 *>(key_packed), key_tab, base, (size_t)2 * k * N, out2, n, k, dm,
+                                     c.logN, c.d_tabs, c.stream),
+            "key_switch_planes");
 }
 void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2, const int *slots,
                        const FloorEpi *epi, bool pair) {

@@ -220,12 +220,18 @@ void op_ntt(Context &c, const u64 *src, u64 *dst, int n_polys, int mod_base, int
 void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3, const FloorEpi *epi = nullptr);
 // Key-switching operations take the keys of ciphertext i from key slot slots[i] when a per-ciphertext slot table is given (n entries,
 // host), otherwise every ciphertext uses the call's slot c.slot.  A missing key is CNHE_ERR_STATE.
-void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots = nullptr);
+// book: count the relinearisations (false: the caller booked them, as a deferred square does when it is made)
+void op_relinearize(Context &c, int ch, const u64 *in3, int n, u64 *out2, const int *slots = nullptr, bool book = true);
 // epi (squares only, a[i] == b[i]): nullptr, or the quadratic activation out2 = relin(A a^2) + B x + Delta C (floor_epi) applied in the
 // BEHZ floor kernel.  x: epi->x, a device table of one input per output of the call (cnhe_layer_poly's second level: the activation's
 // original input), or nullptr for the squared operand itself; c_poly, when set, has one entry per output of the call.
 // pair (with epi): a holds 2n operands and output i is relin(A (a[2i]^2 - a[2i+1]^2)) + B x[i] + Delta C -- 2n squares, one floor and one
 // key switch per output (the cubic activation's second level); slots then has n entries
+// Relinearisation whose key-switch digits arrive as int32 planes (DESIGN 4.15): out2[i] = base_i + sum_d planes_i[d] * rlk_d, base and
+// out2 packed [n][2][k][N], planes [n][D][N] with |value| < min q_l; slots as in op_relinearize.  Counts nothing (the caller booked the
+// relinearisations).  relin_planes_built: whether the context has the fused key switch this needs.
+bool relin_planes_built(const Context &c);
+void op_relinearize_planes(Context &c, int ch, const int *planes, int n, const u64 *base, u64 *out2, const int *slots);
 void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2,
                        const int *slots = nullptr, const FloorEpi *epi = nullptr, bool pair = false);
 // Sums of products with one floor per chunk and one relinearisation per output (DESIGN 4.14): out2[o] = relinearize(sum over the chunks of

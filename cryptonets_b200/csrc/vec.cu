@@ -4,6 +4,7 @@
 // one per plaintext modulus, each carrying what AtomicSealBfvEncryptedVector ("HE Wrapper/AtomicSealBfvVector.cs:303-326")
 // keeps in `Ciphertext[] encData` / `Plaintext[] plainData` -- here blocks of HBM.  The functions below restate that
 // class method by method (cited inline); the arithmetic itself is in the CUDA kernels.
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <climits>
@@ -366,13 +367,47 @@ static cnhe_vec *slab_view(cnhe_vec *v, const std::vector<BufRef> &slab, size_t 
     return v;
 }
 static cnhe_vec *alias_of(const cnhe_vec *a) { return new cnhe_vec(*a); } // shares the reference-counted buffers
+cnhe_vec::cnhe_vec(const cnhe_vec &o)
+    : ctx(o.ctx), dim(o.dim), scale(o.scale), format(o.format), enc(o.enc), slot(o.slot), blocks(o.blocks), buf(o.buf), off(o.off),
+      scalars(o.scalars), is_const(o.is_const), const_val(o.const_val), pend(o.pend), pend_ct(o.pend_ct) {
+    if (pend) pend->members.push_back(this);
+}
+cnhe_vec::~cnhe_vec() {
+    if (!pend) return;
+    auto &m = pend->members;
+    m.erase(std::remove(m.begin(), m.end(), this), m.end());
+}
+// Relinearises v's pending group, if it has one: one op_relinearize per channel over all the group's products (the eager square's call,
+// run later), then every member points at its ciphertexts in the result
+void materialise(Context &c, const cnhe_vec *v) {
+    if (!v || !v->pend) return;
+    const std::shared_ptr<PendingGroup> g = v->pend;
+    const cudaStream_t s0 = c.stream;
+    const size_t ctw = c.ct_words();
+    std::vector<BufRef> slab2(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        slab2[ch] = c.alloc((size_t)g->total * ctw);
+        op_relinearize(c, ch, g->slab3[ch]->p, g->total, slab2[ch]->p, g->ct_slot.data(), false); // booked by the square
+    }
+    c.stream = s0;
+    for (cnhe_vec *m : g->members) {
+        m->buf = slab2;
+        for (int ch = 0; ch < c.P; ch++) m->off[ch] = m->pend_ct * ctw;
+        m->pend.reset();
+    }
+    g->members.clear();
+    g->slab3.clear();
+}
 void same_ctx(Context &c, const cnhe_vec *v) {
     if (!v) fail("null vector");
     if (v->ctx != &c) fail("vector belongs to another context");
+    materialise(c, v);
 }
 int use_slot(Context &c, const cnhe_vec *const *vs, int n) {
     int s = -1;
     for (int i = 0; i < n; i++) {
+        if (vs[i] && vs[i]->ctx == &c) materialise(c, vs[i]);
         if (!vs[i] || !vs[i]->enc) continue;
         if (s >= 0 && vs[i]->slot != s) fail("encrypted operands belong to different key slots");
         s = vs[i]->slot;
@@ -383,10 +418,12 @@ int use_slot(Context &c, const cnhe_vec *const *vs, int n) {
     c.foreign = s != 0;
     return s;
 }
-// key slot of each encrypted vector, checked against the context (layer entry points that serve several clients in one call)
-static std::vector<int> vec_slots(Context &c, const cnhe_vec *const *vs, int n) {
+// key slot of each encrypted vector, checked against the context (layer entry points that serve several clients in one call); keep_pending:
+// leave pending vectors as they are (the scalar-MAC layer's exact path reads them unrelinearised)
+static std::vector<int> vec_slots(Context &c, const cnhe_vec *const *vs, int n, bool keep_pending = false) {
     std::vector<int> s(n);
     for (int i = 0; i < n; i++) {
+        if (!keep_pending && vs[i]->ctx == &c) materialise(c, vs[i]);
         s[i] = vs[i]->slot;
         if (!c.slot_live(s[i])) fail("the vector's key slot was removed");
         if (s[i] != 0) c.foreign = true;
@@ -1090,6 +1127,16 @@ extern "C" int cnhe_export_wait(cnhe_ctx *h, int ticket) {
 }
 extern "C" int cnhe_vec_device_ptr(const cnhe_vec *v, int channel, uint64_t *dptr, size_t *words) {
     if (!v || channel < 0 || channel >= v->ctx->P) return set_err(CNHE_ERR_INVALID, "bad arguments");
+    if (v->pend) { // the caller reads the words: relinearise them first
+        cnhe_ctx h{v->ctx};
+        const int r = [&]() -> int {
+            API_BEGIN(&h)
+            materialise(c, v);
+            c.sync();
+            API_END
+        }();
+        if (r != CNHE_OK) return r;
+    }
     *dptr = (uint64_t)v->ptr(channel);
     if (words) *words = (size_t)v->blocks * v->unit();
     return CNHE_OK;
@@ -1970,14 +2017,16 @@ struct MacLayer {
 };
 // in_scale: the scale of the ciphertexts the MAC sums (the inputs', or the activation's output scale when they are squared first); the
 // bias must be at in_scale times the weights' scale
+// keep_pending: leave pending inputs unrelinearised (the exact path of mac_layer)
 static MacLayer mac_prepare(Context &c, const cnhe_vec *const *in, int n_in, double in_scale, const int32_t *gather, const cnhe_vec *const *weights,
-                            const cnhe_vec *const *bias, int M, int K) {
+                            const cnhe_vec *const *bias, int M, int K, bool keep_pending = false) {
     if (n_in < 1 || M < 1 || K < 1) fail("bad layer shape");
     MacLayer L;
     L.n_in = n_in; L.M = M; L.K = K; L.gather = gather; L.weights = weights; L.bias = bias;
     L.bl = in[0]->blocks;
     for (int i = 0; i < n_in; i++) {
-        same_ctx(c, in[i]);
+        if (!keep_pending) same_ctx(c, in[i]);
+        else if (!in[i] || in[i]->ctx != &c) fail(!in[i] ? "null vector" : "vector belongs to another context");
         if (!in[i]->enc || in[i]->format != CNHE_DENSE) fail("layer inputs must be encrypted dense vectors");
         if (in[i]->blocks != L.bl || in[i]->dim != in[0]->dim || in[i]->scale != in[0]->scale) fail("all layer inputs must share dimension and scale");
     }
@@ -1997,7 +2046,7 @@ static MacLayer mac_prepare(Context &c, const cnhe_vec *const *in, int n_in, dou
     }
     // The scalar MAC is key-independent, so one call may serve several clients (their images' columns side by side, each output's
     // gather row inside one client's columns): every output takes the key slot its taps share; taps of two slots in one output are refused
-    const std::vector<int> in_slot = vec_slots(c, in, n_in);
+    const std::vector<int> in_slot = vec_slots(c, in, n_in, keep_pending);
     L.out_slot.assign(M, -1);
     for (int m = 0; m < M; m++) {
         for (int kk = 0; kk < (gather ? K : n_in); kk++) {
@@ -2053,10 +2102,46 @@ static MacLayer mac_prepare(Context &c, const cnhe_vec *const *in, int n_in, dou
     }
     return L;
 }
+// the layer's weights in channel ch as signed integers (centred mod t), and their largest magnitude
+static std::vector<double> mac_weights(Context &c, const MacLayer &L, int ch, double &wmax) {
+    const u64 t = c.t[ch], thr = (t + 1) >> 1;
+    std::vector<double> wdh((size_t)L.M * L.K);
+    wmax = 0;
+    for (int m = 0; m < L.M; m++)
+        for (int kk = 0; kk < L.K; kk++) {
+            const u64 w = L.weights[m]->scalars[ch][kk];
+            const double d = w >= thr ? -(double)(t - w) : (double)w;
+            wdh[(size_t)m * L.K + kk] = d;
+            wmax = std::max(wmax, std::fabs(d));
+        }
+    return wdh;
+}
+// the wgmma plan of channel ch, or null when the wgmma kernel cannot serve the layer: any layer whose inputs are evenly spaced rows of one
+// slab (the previous layer's output, an imported batch) and whose weights stay within +-254; tap_stride: the rows' distance in words
+static std::shared_ptr<UmmaPlan> mac_umma_plan(Context &c, const MacLayer &L, int ch, const std::vector<const u64 *> &ip_all, size_t ctw,
+                                               const std::vector<double> &wdh, double wmax, long long &tap_stride) {
+    const int n_in = L.n_in, M = L.M, maxbits = L.maxbits, limbs = (maxbits + 7) / 8;
+    // (M >= 8: LoLa's per-map products come one output at a time -- a 128-row MMA per tile would be 99 % padding and the kernel's
+    // per-tile latency more than the whole scalar-MAC launch)
+    bool slab = L.bl == 1 && n_in >= 2 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 && wmax <= 254.0 && !getenv("CNHE_MAC_NO_UMMA") &&
+                !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
+    tap_stride = 0;
+    if (slab) {
+        tap_stride = ip_all[1] - ip_all[0];
+        slab = tap_stride >= (long long)ctw && tap_stride % 2 == 0;
+        for (int i = 0; i < n_in && slab; i++) slab = ip_all[i] == ip_all[0] + (long long)i * tap_stride;
+    }
+    if (!slab) return nullptr;
+    std::shared_ptr<UmmaPlan> plan = umma_plan(c, ch, L.grows, L.row_outs, wdh, M, L.K, limbs);
+    return plan->ok && (double)plan->total_chunks * 32.0 * 127.0 * 255.0 < 2147483648.0 ? plan : nullptr;
+}
 // One channel of a prepared layer on ciphertexts of `polys` polynomials (2, or 3 for size-3 products: the sum is linear in each
 // polynomial): ip[b * n_in + i] is block b of input i, op[m * bl + b] block b of output m; the blocks of one output lie consecutively,
 // polys * k * N words apart.  The bias goes to c0.
-static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector<const u64 *> &ip_all, const std::vector<u64 *> &op_all, int polys) {
+// planes (exact path, DESIGN 4.15; size-3 inputs on the wgmma kernel only): the outputs get c0 and c1 alone (2kN words) and the digit
+// sums of c2 go to planes[m][D][N] (int32) for the plane-source key switch
+static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector<const u64 *> &ip_all, const std::vector<u64 *> &op_all, int polys,
+                        int *planes = nullptr) {
     const int n_in = L.n_in, M = L.M, K = L.K, bl = L.bl, maxbits = L.maxbits;
     const int32_t *gather = L.gather;
     const cnhe_vec *const *weights = L.weights, *const *bias = L.bias;
@@ -2073,16 +2158,8 @@ static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector
     for (int m = 0; m < M; m++) wp[m] = weights[m]->ptr(ch);
     const u64 *const *d_w = upload_ptrs(c, wp);
     // signed weights as doubles for the FP64 accumulate path, when they are small enough for it to be exact
-    const u64 t = c.t[ch], thr = (t + 1) >> 1;
-    std::vector<double> wdh((size_t)M * K);
     double wmax = 0;
-    for (int m = 0; m < M; m++)
-        for (int kk = 0; kk < K; kk++) {
-            const u64 w = weights[m]->scalars[ch][kk];
-            const double d = w >= thr ? -(double)(t - w) : (double)w;
-            wdh[(size_t)m * K + kk] = d;
-            wmax = std::max(wmax, std::fabs(d));
-        }
+    const std::vector<double> wdh = mac_weights(c, L, ch, wmax);
     const bool fp_mac = maxbits <= 50 && wmax < 131072.0 && (double)K * wmax * 67108864.0 < 4503599627370496.0 && !getenv("CNHE_MAC_INT");
     // dense layer (one gather row shared by every output, 8-bit weights): exact integer GEMM on the tensor cores (mac_imma.cu).  Both
     // tensor-core kernels join the limb sums in an FP64 epilogue that is exact only for moduli below 2^50 ((double)p, fcanon_u's
@@ -2090,23 +2167,11 @@ static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector
     const int limbs = (maxbits + 7) / 8;
     const bool imma = order_rows == 1 && wmax <= 254.0 && K >= 32 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 &&
                       (double)K * 254.0 * 255.0 < 2147483648.0 && !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
-    // ... or, for any layer whose inputs are evenly spaced rows of one slab (the previous layer's output, an imported batch) and whose
-    // weights stay within +-254: wgmma (mac_umma.cu), dense and convolution alike, under the same modulus bound
-    std::shared_ptr<UmmaPlan> plan;
+    // ... or wgmma (mac_umma.cu), dense and convolution alike, under the same modulus bound
     long long tap_stride = 0;
-    {
-        // (M >= 8: LoLa's per-map products come one output at a time -- a 128-row MMA per tile would be 99 % padding and the kernel's
-        // per-tile latency more than the whole scalar-MAC launch)
-        bool slab = bl == 1 && n_in >= 2 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 && wmax <= 254.0 && !getenv("CNHE_MAC_NO_UMMA") &&
-                    !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
-        if (slab) {
-            tap_stride = ip_all[1] - ip_all[0];
-            slab = tap_stride >= (long long)ctw && tap_stride % 2 == 0;
-            for (int i = 0; i < n_in && slab; i++) slab = ip_all[i] == ip_all[0] + (long long)i * tap_stride;
-        }
-        if (slab) plan = umma_plan(c, ch, grows, L.row_outs, wdh, M, K, limbs);
-    }
-    const bool umma = plan && plan->ok && (double)plan->total_chunks * 32.0 * 127.0 * 255.0 < 2147483648.0;
+    const std::shared_ptr<UmmaPlan> plan = mac_umma_plan(c, L, ch, ip_all, ctw, wdh, wmax, tap_stride);
+    const bool umma = plan != nullptr;
+    if (planes && !umma) throw Error(CNHE_ERR_INVALID, "internal error: the exact scalar-MAC path needs the wgmma kernel");
     const void *d_wfrag = nullptr, *d_wfrag2 = nullptr;
     if (!umma && imma) {
         const int mtiles = (M + 15) / 16, chunks = (K + 31) / 32;
@@ -2185,6 +2250,22 @@ static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector
             a.wpack = plan->d_wpack; a.a_bytes = (int)plan->wpack.size();
             a.out_ptrs = upload_ptrs_mut(c, opo); a.bias = d_bias_o; a.n_out_total = M;
             a.limbs = limbs; a.polys = polys; a.k = c.k; a.logn = c.logN; a.bc = c.d_bc; a.pc = c.ch[ch].pc;
+            if (planes) { // digit planes in the key order of the relinearisation keys: digit d of residue src[d], bits shift[d] ..
+                const DigitMap &dm = c.dm_relin;
+                std::vector<int *> pp(M);
+                for (int i = 0; i < M; i++) pp[i] = planes + (size_t)plan->out_order[i] * dm.D * c.N;
+                u64 *dpp = c.ws_alloc(M);
+                c.h2d(dpp, pp.data(), (size_t)M * 8);
+                a.dig.planes = reinterpret_cast<int *const *>(dpp);
+                a.dig.mask = (unsigned)dm.mask;
+                a.dig.w = hm::bit_length(dm.mask);
+                int most = 0;
+                for (int d = 0; d < dm.D; d++) {
+                    if (a.dig.count[dm.src[d]]++ == 0) a.dig.first[dm.src[d]] = (unsigned char)d;
+                    most = std::max(most, (int)a.dig.count[dm.src[d]]);
+                }
+                a.dig.groups = (most + limbs / 2 - 1) / (limbs / 2);
+            }
             c.check(launch_mac_umma(a, c.stream), "mac_umma");
         } else if (imma) {
             std::vector<const u64 *> ipg(K);
@@ -2213,18 +2294,78 @@ static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector
         for (int kk = 0; kk < K; kk++)
             if (!gather || gather[kk] >= 0) ss += wdh[kk] * wdh[kk];
         // (a size-3 sum has no noise budget of its own: its relinearised outputs are measured)
-        c.note(Context::OP_ADD_MANY, ch, M * bl, polys == 2 ? op_all[0] : nullptr, ip_all[gather ? std::max(gather[0], 0) : 0], nullptr,
+        c.note(Context::OP_ADD_MANY, ch, M * bl, polys == 2 && !planes ? op_all[0] : nullptr, ip_all[gather ? std::max(gather[0], 0) : 0], nullptr,
                ss > 0 ? 0.5 * std::log2(ss) : 0);
     }
     if (bias && !L.const_bias) // generic AddPlain per output, on c0 of each of its blocks
         for (int m = 0; m < M; m++) {
             u64 *o = op_all[(size_t)m * bl];
-            c.check(launch_ct_add_plain(o, o, bl, polys, bias[m]->ptr(ch), c.N, (int)c.N, c.k, c.logN, c.d_bc, c.ch[ch].pc, 0, c.stream), "ct_add_plain");
+            c.check(launch_ct_add_plain(o, o, bl, planes ? 2 : polys, bias[m]->ptr(ch), c.N, (int)c.N, c.k, c.logN, c.d_bc, c.ch[ch].pc, 0, c.stream),
+                    "ct_add_plain");
         }
+}
+// The exact path of mac_layer over pending squares (DESIGN 4.15): relinearising a size-3 product adds sum_d digit_d(c2) * rlk_d to
+// (c0, c1), so the layer's output m is (sum_j W_mj (c0_j, c1_j) + bias) + sum_d S_md * rlk_d with the integer digit sums
+// S_md = sum_j W_mj digit_d(c2_j) -- the same element of R_q, written canonical, as the layer over the relinearised squares: the same
+// words and noise, for M key switches instead of one per input.  Taken when every input is pending, the context has the plane-source key
+// switch, the wgmma kernel serves the layer in every channel and every |S| stays below min(2^31, min_l q_l); returns false (nothing
+// done) otherwise.
+static bool mac_layer_exact(Context &c, const cnhe_vec *const *in, int n_in, const int32_t *gather, const cnhe_vec *const *weights,
+                            const cnhe_vec *const *bias, int M, int K, cnhe_vec **out) {
+    if (n_in < 2 || !in || c.trace_noise || !relin_planes_built(c)) return false;
+    const DigitMap &dm = c.dm_relin;
+    const int w = hm::bit_length(dm.mask);
+    if (w > 16) return false;
+    for (int i = 0; i < n_in; i++) {
+        if (!in[i] || in[i]->ctx != &c || !in[i]->pend) return false;
+        for (int b = 0; b < in[i]->blocks; b++) // the square's key slot is the one its relinearisation would use
+            if (in[i]->pend->ct_slot[in[i]->pend_ct + b] != in[i]->slot) return false;
+    }
+    const MacLayer L = mac_prepare(c, in, n_in, in[0]->scale, gather, weights, bias, M, K, true);
+    if (L.bl != 1) return false;
+    double bound = 2147483648.0;
+    for (u64 q : c.q) bound = std::min(bound, (double)q);
+    std::vector<std::vector<const u64 *>> ips(c.P);
+    const size_t s3 = (size_t)3 * c.k * c.N, ctw = c.ct_words();
+    for (int ch = 0; ch < c.P; ch++) {
+        for (int i = 0; i < n_in; i++) ips[ch].push_back(in[i]->pending_block(ch, 0));
+        double wmax = 0;
+        const std::vector<double> wdh = mac_weights(c, L, ch, wmax);
+        long long tap_stride = 0;
+        if (!mac_umma_plan(c, L, ch, ips[ch], s3, wdh, wmax, tap_stride)) return false;
+        for (int m = 0; m < M; m++) {
+            double sum = 0;
+            for (int kk = 0; kk < K; kk++)
+                if (!gather || gather[(size_t)m * K + kk] >= 0) sum += std::fabs(wdh[(size_t)m * K + kk]);
+            if (sum * (double)dm.mask >= bound) return false;
+        }
+    }
+    std::vector<BufRef> big(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        big[ch] = c.alloc((size_t)M * ctw);
+    }
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        WsScope scope(c);
+        u64 *y = c.ws_alloc((size_t)M * ctw);
+        int *planes = reinterpret_cast<int *>(c.ws_alloc(((size_t)M * dm.D * c.N + 1) / 2));
+        std::vector<u64 *> op(M);
+        for (int m = 0; m < M; m++) op[m] = y + (size_t)m * ctw;
+        mac_channel(c, L, ch, ips[ch], op, 3, planes);
+        op_relinearize_planes(c, ch, planes, M, y, big[ch]->p, L.out_slot.data());
+    }
+    const double out_scale = in[0]->scale * weights[0]->scale;
+    for (int m = 0; m < M; m++) {
+        out[m] = slab_view(new_vec(c, in[0]->dim, out_scale, CNHE_DENSE, true, 1), big, (size_t)m);
+        out[m]->slot = L.out_slot[m];
+    }
+    return true;
 }
 // Shared body of DenseMatrixBySparseVectorMultiply (ciphertext columns x plain constants) and of the fused PoolLayer.
 static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int32_t *gather, const cnhe_vec *const *weights, const cnhe_vec *const *bias,
                       int M, int K, cnhe_vec **out) {
+    if (mac_layer_exact(c, in, n_in, gather, weights, bias, M, K, out)) return;
     const MacLayer L = mac_prepare(c, in, n_in, n_in > 0 ? in[0]->scale : 0.0, gather, weights, bias, M, K);
     const int bl = L.bl;
     std::vector<BufRef> big(c.P);
@@ -2483,6 +2624,8 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
     API_BEGIN(h)
     if (n < 1) fail("empty layer");
     std::vector<int> first(n + 1, 0);
+    bool chained = false; // a square of a pending square: a polynomial chain (x^4), not an activation that feeds a scalar-MAC layer
+    for (int i = 0; i < n; i++) chained = chained || (in[i] && in[i]->pend);
     for (int i = 0; i < n; i++) {
         same_ctx(c, in[i]);
         if (!in[i]->enc) fail("multiplying two plaintexts is not implemented");
@@ -2493,6 +2636,35 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
     const std::vector<int> vslot = vec_slots(c, in, n);
     std::vector<int> ct_slot;
     for (int i = 0; i < n; i++) ct_slot.insert(ct_slot.end(), in[i]->blocks, vslot[i]);
+    // The products stay unrelinearised until something reads them (DESIGN 4.15): a scalar-MAC layer then key-switches its outputs instead
+    // of these, with the same words.  Eager where that path can never run: with the noise trace (it measures every relinearised square),
+    // without the plane-source key switch or with digits wider than 16 bits, when the size-3 slab would pass 8 GiB, and for a square of
+    // squares, whose next consumer is another product rather than a scalar-MAC layer.
+    const size_t s3 = (size_t)3 * c.k * c.N;
+    if (!chained && !c.trace_noise && relin_planes_built(c) && hm::bit_length(c.dm_relin.mask) <= 16 && (size_t)total * s3 <= ((size_t)1 << 30)) {
+        auto g = std::make_shared<PendingGroup>();
+        g->total = total;
+        g->ct_slot = ct_slot;
+        g->slab3.resize(c.P);
+        for (int ch = 0; ch < c.P; ch++) {
+            c.set_channel(ch);
+            (void)relin_keys(c, ch, total, ct_slot.data()); // a missing key fails here, as it does for the eager square
+            g->slab3[ch] = c.alloc((size_t)total * s3);
+            std::vector<const u64 *> ptrs;
+            for (int i = 0; i < n; i++)
+                for (int b = 0; b < in[i]->blocks; b++) ptrs.push_back(in[i]->block(ch, b));
+            op_multiply(c, ch, ptrs, ptrs, g->slab3[ch]->p);
+            c.op_count[Context::OP_RELINEARIZE] += (uint64_t)total; // booked here, as the eager square books it
+        }
+        for (int i = 0; i < n; i++) {
+            out[i] = new_vec(c, in[i]->dim, in[i]->scale * in[i]->scale, in[i]->format, true, in[i]->blocks);
+            out[i]->slot = vslot[i];
+            out[i]->pend = g;
+            out[i]->pend_ct = (size_t)first[i];
+            g->members.push_back(out[i]);
+        }
+        return CNHE_OK;
+    }
     std::vector<BufRef> big(c.P);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);

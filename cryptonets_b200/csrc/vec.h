@@ -14,7 +14,21 @@ struct cnhe_ctx {
     Context *c;
 };
 
+struct cnhe_vec;
+// The outputs of one cnhe_layer_square call before their relinearisation (DESIGN 4.15): the size-3 products of every ciphertext in one
+// slab per channel.  A scalar-MAC layer that can key-switch its own outputs instead reads them as they are; any other use relinearises
+// the whole group (materialise, vec.cu) and re-points every member at the result, which is the eager square's words.
+struct PendingGroup {
+    std::vector<BufRef> slab3;       // per channel: [total][3][k][N]
+    std::vector<int> ct_slot;        // key slot of every ciphertext, as the square recorded it
+    int total = 0;
+    std::vector<cnhe_vec *> members; // the live vectors that still point into slab3
+};
 struct cnhe_vec {
+    cnhe_vec() = default;
+    cnhe_vec(const cnhe_vec &o); // an alias of a pending vector joins its group
+    cnhe_vec &operator=(const cnhe_vec &) = delete;
+    ~cnhe_vec();
     Context *ctx = nullptr;
     uint64_t dim = 0;
     double scale = 1.0;
@@ -28,7 +42,14 @@ struct cnhe_vec {
     bool is_const = false;                 // plain dense whose every plaintext is a constant polynomial
     std::vector<u64> const_val;            // per channel constant (mod t) when is_const
 
-    u64 *ptr(int ch) const { return buf[ch]->p + off[ch]; }
+    std::shared_ptr<PendingGroup> pend; // set while this vector's ciphertexts are unrelinearised products in pend->slab3
+    size_t pend_ct = 0;                 // ... starting at ciphertext pend_ct of the group
+
+    u64 *ptr(int ch) const {
+        if (pend) throw Error(CNHE_ERR_INVALID, "internal error: a squared vector was read before its relinearisation");
+        return buf[ch]->p + off[ch];
+    }
+    const u64 *pending_block(int ch, int b) const { return pend->slab3[ch]->p + (pend_ct + (size_t)b) * 3 * ctx->k * ctx->N; }
     size_t unit() const { return enc ? ctx->ct_words() : (format == CNHE_DENSE ? (size_t)ctx->N : 1); }
     u64 *block(int ch, int b) const { return ptr(ch) + (size_t)b * unit(); }
 };
@@ -57,5 +78,6 @@ cnhe_vec *new_vec(Context &c, uint64_t dim, double scale, int format, bool enc, 
 int use_slot(Context &c, const cnhe_vec *const *vs, int n);
 static inline int use_slot(Context &c, std::initializer_list<const cnhe_vec *> vs) { return use_slot(c, vs.begin(), (int)vs.size()); }
 void alloc_channels(cnhe_vec *v);
-void same_ctx(Context &c, const cnhe_vec *v);
+void same_ctx(Context &c, const cnhe_vec *v); // also relinearises v's pending group (as use_slot and the layers' slot checks do)
+void materialise(Context &c, const cnhe_vec *v);
 
