@@ -5,10 +5,12 @@
 // keeps in `Ciphertext[] encData` / `Plaintext[] plainData` -- here blocks of HBM.  The functions below restate that
 // class method by method (cited inline); the arithmetic itself is in the CUDA kernels.
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdlib>
 #include <climits>
 #include <cstring>
+#include <optional>
 #include <unordered_map>
 
 #include "hostmath.h"
@@ -364,6 +366,13 @@ static cnhe_vec *slab_view(cnhe_vec *v, const std::vector<BufRef> &slab, size_t 
         v->buf[ch] = slab[ch];
         v->off[ch] = ct * v->ctx->ct_words();
     }
+    return v;
+}
+// An output of a batched call: an encrypted vector shaped like `like` (dimension, format, blocks) at `scale` and in key slot `slot`,
+// viewing the call's slab from ciphertext `ct` on
+static cnhe_vec *slab_output(Context &c, const std::vector<BufRef> &slab, size_t ct, const cnhe_vec *like, double scale, int slot) {
+    cnhe_vec *v = slab_view(new_vec(c, like->dim, scale, like->format, true, like->blocks), slab, ct);
+    v->slot = slot;
     return v;
 }
 static cnhe_vec *alias_of(const cnhe_vec *a) { return new cnhe_vec(*a); } // shares the reference-counted buffers
@@ -2355,11 +2364,7 @@ static bool mac_layer_exact(Context &c, const cnhe_vec *const *in, int n_in, con
         mac_channel(c, L, ch, ips[ch], op, 3, planes);
         op_relinearize_planes(c, ch, planes, M, y, big[ch]->p, L.out_slot.data());
     }
-    const double out_scale = in[0]->scale * weights[0]->scale;
-    for (int m = 0; m < M; m++) {
-        out[m] = slab_view(new_vec(c, in[0]->dim, out_scale, CNHE_DENSE, true, 1), big, (size_t)m);
-        out[m]->slot = L.out_slot[m];
-    }
+    for (int m = 0; m < M; m++) out[m] = slab_output(c, big, (size_t)m, in[0], in[0]->scale * weights[0]->scale, L.out_slot[m]);
     return true;
 }
 // Shared body of DenseMatrixBySparseVectorMultiply (ciphertext columns x plain constants) and of the fused PoolLayer.
@@ -2382,11 +2387,7 @@ static void mac_layer(Context &c, const cnhe_vec *const *in, int n_in, const int
         for (size_t j = 0; j < op.size(); j++) op[j] = big[ch]->p + j * c.ct_words();
         mac_channel(c, L, ch, ip, op, 2);
     }
-    const double out_scale = in[0]->scale * weights[0]->scale;
-    for (int m = 0; m < M; m++) {
-        out[m] = slab_view(new_vec(c, in[0]->dim, out_scale, CNHE_DENSE, true, bl), big, (size_t)m * bl);
-        out[m]->slot = L.out_slot[m];
-    }
+    for (int m = 0; m < M; m++) out[m] = slab_output(c, big, (size_t)m * bl, in[0], in[0]->scale * weights[0]->scale, L.out_slot[m]);
 }
 extern "C" int cnhe_layer_conv_dense(cnhe_ctx *h, const cnhe_vec *const *in, int n_in, const int32_t *gather, const cnhe_vec *const *weights,
                                      const cnhe_vec *const *bias, int M, int K, cnhe_vec **out) {
@@ -2619,79 +2620,93 @@ extern "C" int cnhe_mat_dot_rows_batch(cnhe_ctx *h, const cnhe_vec *const *rows,
     mat_mul_rowmajor(c, rows, n_rows, vs, B, false, 0, n_rows, out, length, true);
     API_END
 }
-// SquareActivation over a whole matrix: every column PointwiseMultiply'd with itself in one wave per channel
-extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, cnhe_vec **out) {
-    API_BEGIN(h)
-    if (n < 1) fail("empty layer");
-    std::vector<int> first(n + 1, 0);
-    bool chained = false; // a square of a pending square: a polynomial chain (x^4), not an activation that feeds a scalar-MAC layer
-    for (int i = 0; i < n; i++) chained = chained || (in[i] && in[i]->pend);
+// The inputs of an activation layer: n encrypted vectors whose ciphertexts the layer takes as one flat batch, in[i]'s blocks from first[i]
+// on (first[n]: the batch's size)
+struct ActInputs {
+    const cnhe_vec *const *in;
+    int n;
+    std::vector<int> first;
+    std::vector<int> vslot, ct_slot; // the key slot of every vector and of every ciphertext (act_inputs)
+    ActInputs(const cnhe_vec *const *in, int n) : in(in), n(n), first(n + 1, 0) {
+        for (int i = 0; i < n; i++) first[i + 1] = first[i] + in[i]->blocks;
+    }
+    int total() const { return first[n]; }
+    std::vector<const u64 *> blocks(int ch) const { // the batch's ciphertexts in channel ch
+        std::vector<const u64 *> p;
+        for (int i = 0; i < n; i++)
+            for (int b = 0; b < in[i]->blocks; b++) p.push_back(in[i]->block(ch, b));
+        return p;
+    }
+};
+// The coefficients of an activation polynomial of degree 2, 3 or 4: cf[j] the coefficient of x^j (nullptr: 0), each a plain sparse vector
+// of dimension 1; the leading one is required
+struct ActCoeffs {
+    int degree;
+    const cnhe_vec *cf[5] = {};
+    double out_scale = 0;                // W s^degree (read)
+    std::vector<std::array<u64, 5>> res; // per channel the residues of cf[j] (read)
+    ActCoeffs(Context &c, const cnhe_vec *const *coeffs, int degree, const char *lead_missing) : degree(degree) {
+        if (!coeffs || !coeffs[degree]) fail(lead_missing);
+        for (int j = 0; j <= degree; j++) {
+            const cnhe_vec *p = cf[j] = coeffs[j];
+            if (!p) continue;
+            same_ctx(c, p);
+            if (p->enc) fail("the coefficients must be plain");
+            if (p->format != CNHE_SPARSE || p->dim != 1) fail("each coefficient must be a sparse vector of dimension 1");
+        }
+    }
+    // for inputs at scale s: coefficient j at scale W s^(degree - j), W the leading coefficient's scale, the powers of s multiplied up one
+    // factor at a time.  A leading coefficient that is 0 mod a plaintext prime only drops the square term of a quadratic there; degrees 3
+    // and 4 divide by it
+    void read(Context &c, double s) {
+        double at[5];
+        at[degree] = cf[degree]->scale;
+        for (int j = degree - 1; j >= 0; j--) at[j] = at[j + 1] * s;
+        for (int j = 0; j < degree; j++)
+            if (cf[j] && cf[j]->scale != at[j]) fail("Scales do not match.");
+        out_scale = at[0];
+        res.assign(c.P, std::array<u64, 5>{});
+        for (int ch = 0; ch < c.P; ch++) {
+            const u64 t = c.ch[ch].t;
+            for (int j = 0; j <= degree; j++) res[ch][j] = cf[j] ? cf[j]->scalars[ch][0] % t : 0;
+            if (degree > 2 && res[ch][degree] == 0)
+                fail(("the leading coefficient is 0 mod the plaintext prime " + std::to_string(t) + ": it has no inverse there").c_str());
+        }
+    }
+};
+// cnhe_layer_poly2's a x^2 + b x + c (b, c may be null)
+static ActCoeffs quad_coeffs(Context &c, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc) {
+    const cnhe_vec *cf[3] = {cc, b, a};
+    return ActCoeffs(c, cf, 2, "the quadratic coefficient is required");
+}
+// Validates an activation layer's inputs -- encrypted (else plain_msg), and at one scale when the layer has coefficients, which are then
+// read at that scale -- and records their key slots: the vectors may belong to different key slots (several clients' layers in one
+// call), each ciphertext is relinearised under its own
+static ActInputs act_inputs(Context &c, const cnhe_vec *const *in, int n, const char *plain_msg, ActCoeffs *cf = nullptr) {
     for (int i = 0; i < n; i++) {
         same_ctx(c, in[i]);
-        if (!in[i]->enc) fail("multiplying two plaintexts is not implemented");
-        first[i + 1] = first[i] + in[i]->blocks;
+        if (!in[i]->enc) fail(plain_msg);
+        if (cf && in[i]->scale != in[0]->scale) fail("Scales do not match.");
     }
-    const int total = first[n];
-    // the vectors may belong to different key slots (several clients' layers in one call): each ciphertext is relinearised under its own
-    const std::vector<int> vslot = vec_slots(c, in, n);
-    std::vector<int> ct_slot;
-    for (int i = 0; i < n; i++) ct_slot.insert(ct_slot.end(), in[i]->blocks, vslot[i]);
-    // The products stay unrelinearised until something reads them (DESIGN 4.15): a scalar-MAC layer then key-switches its outputs instead
-    // of these, with the same words.  Eager where that path can never run: with the noise trace (it measures every relinearised square),
-    // without the plane-source key switch or with digits wider than 16 bits, when the size-3 slab would pass 8 GiB, and for a square of
-    // squares, whose next consumer is another product rather than a scalar-MAC layer.
-    const size_t s3 = (size_t)3 * c.k * c.N;
-    if (!chained && !c.trace_noise && relin_planes_built(c) && hm::bit_length(c.dm_relin.mask) <= 16 && (size_t)total * s3 <= ((size_t)1 << 30)) {
-        auto g = std::make_shared<PendingGroup>();
-        g->total = total;
-        g->ct_slot = ct_slot;
-        g->slab3.resize(c.P);
-        for (int ch = 0; ch < c.P; ch++) {
-            c.set_channel(ch);
-            (void)relin_keys(c, ch, total, ct_slot.data()); // a missing key fails here, as it does for the eager square
-            g->slab3[ch] = c.alloc((size_t)total * s3);
-            std::vector<const u64 *> ptrs;
-            for (int i = 0; i < n; i++)
-                for (int b = 0; b < in[i]->blocks; b++) ptrs.push_back(in[i]->block(ch, b));
-            op_multiply(c, ch, ptrs, ptrs, g->slab3[ch]->p);
-            c.op_count[Context::OP_RELINEARIZE] += (uint64_t)total; // booked here, as the eager square books it
-        }
-        for (int i = 0; i < n; i++) {
-            out[i] = new_vec(c, in[i]->dim, in[i]->scale * in[i]->scale, in[i]->format, true, in[i]->blocks);
-            out[i]->slot = vslot[i];
-            out[i]->pend = g;
-            out[i]->pend_ct = (size_t)first[i];
-            g->members.push_back(out[i]);
-        }
-        return CNHE_OK;
-    }
-    std::vector<BufRef> big(c.P);
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        big[ch] = c.alloc((size_t)total * c.ct_words());
-        std::vector<const u64 *> ptrs;
-        for (int i = 0; i < n; i++)
-            for (int b = 0; b < in[i]->blocks; b++) ptrs.push_back(in[i]->block(ch, b));
-        op_multiply_relin(c, ch, ptrs, ptrs, big[ch]->p, ct_slot.data());
-    }
-    for (int i = 0; i < n; i++) {
-        out[i] = slab_view(new_vec(c, in[i]->dim, in[i]->scale * in[i]->scale, in[i]->format, true, in[i]->blocks), big, first[i]);
-        out[i]->slot = vslot[i];
-    }
-    API_END
+    if (cf) cf->read(c, in[0]->scale);
+    ActInputs X(in, n);
+    X.vslot = vec_slots(c, in, n);
+    for (int i = 0; i < n; i++) X.ct_slot.insert(X.ct_slot.end(), in[i]->blocks, X.vslot[i]);
+    return X;
 }
-// The constant term of cnhe_layer_poly2 on a dense vector whose last block is only partly filled: Delta times the plaintext with C in the
+// The constant term of an activation on a dense vector whose last block is only partly filled: Delta times the plaintext with C in the
 // block's data slots and 0 in its padding slots ([k][N] canonical words, as add_plain scales it), so that padding stays zero as it does
 // for the square -- rotating layers (Duplicate) add whole ciphertexts.  Returns the call's table of one entry per ciphertext (nullptr: the
 // constant polynomial C, every slot a data slot), or nullptr when no ciphertext needs one.  Workspace memory of the call.
-static const u64 *const *padded_constants(Context &c, int ch, const cnhe_vec *const *in, int n, int total, u64 C) {
+static const u64 *const *padded_constants(Context &c, int ch, const ActInputs &X, u64 C) {
     const size_t N = c.N;
-    std::vector<const u64 *> tab(total, nullptr);
+    std::vector<const u64 *> tab(X.total(), nullptr);
     std::map<size_t, const u64 *> by_fill; // data slots of the last block -> its Delta-scaled plaintext
     bool any = false;
-    for (int i = 0, first = 0; i < n; first += in[i]->blocks, i++) {
-        if (in[i]->format != CNHE_DENSE || in[i]->dim % N == 0) continue;
-        const size_t fill = in[i]->dim % N;
+    for (int i = 0; i < X.n; i++) {
+        const cnhe_vec *v = X.in[i];
+        if (v->format != CNHE_DENSE || v->dim % N == 0) continue;
+        const size_t fill = v->dim % N;
         const u64 *&cp = by_fill[fill];
         if (!cp) {
             std::vector<u64> vals(N, 0);
@@ -2703,36 +2718,84 @@ static const u64 *const *padded_constants(Context &c, int ch, const cnhe_vec *co
             c.check(launch_ct_add_plain(scaled, scaled, 1, 1, plain, N, (int)N, c.k, c.logN, c.d_bc, c.ch[ch].pc, 0, c.stream), "ct_add_plain");
             cp = scaled;
         }
-        tab[first + in[i]->blocks - 1] = cp;
+        tab[X.first[i + 1] - 1] = cp;
         any = true;
     }
     return any ? upload_ptrs(c, tab) : nullptr;
 }
-// cnhe_layer_poly2's coefficients: a required, each one a plain sparse vector of dimension 1
-static void poly2_check_coeffs(Context &c, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc) {
-    if (!a) fail("the quadratic coefficient is required");
-    for (const cnhe_vec *p : {a, b, cc}) {
-        if (!p) continue;
-        same_ctx(c, p);
-        if (p->enc) fail("the coefficients must be plain");
-        if (p->format != CNHE_SPARSE || p->dim != 1) fail("each coefficient must be a sparse vector of dimension 1");
+// The floor epilogue of one channel's activation wave over X (floor_epi): relinearize(A y^2) + B x + Delta C for the squared operand y,
+// x read from the table x (nullptr: y itself), the constant padded where a dense vector's last block is partly filled.  book: count the
+// terms' operations beyond the product (a term that is 0 mod t is skipped in that channel)
+static FloorEpi act_epilogue(Context &c, int ch, const ActInputs &X, u64 A, u64 B, u64 C, const u64 *const *x = nullptr, bool book = true) {
+    FloorEpi e = floor_epi(c, ch, A, B, C);
+    e.x = x;
+    if (C) e.c_poly = padded_constants(c, ch, X, C);
+    if (book) {
+        auto &ops = c.op_count;
+        const uint64_t n = (uint64_t)X.total();
+        if (A) ops[Context::OP_MULTIPLY_SCALAR] += n;
+        if (B) {
+            ops[Context::OP_MULTIPLY_SCALAR] += n;
+            ops[Context::OP_ADD] += n;
+        }
+        if (C) ops[Context::OP_ADD_PLAIN] += n;
+    }
+    return e;
+}
+// cnhe_layer_square (cf == nullptr) and cnhe_layer_poly2 over validated inputs, in one wave per channel: relinearize(x^2), or with the
+// quadratic's floor epilogue relinearize(A x^2) + B x + Delta C word for word
+static void square_layer(Context &c, const ActInputs &X, const ActCoeffs *cf, cnhe_vec **out) {
+    std::vector<BufRef> big(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        FloorEpi epi;
+        if (cf) epi = act_epilogue(c, ch, X, cf->res[ch][2], cf->res[ch][1], cf->res[ch][0]);
+        big[ch] = c.alloc((size_t)X.total() * c.ct_words());
+        const std::vector<const u64 *> xs = X.blocks(ch);
+        op_multiply_relin(c, ch, xs, xs, big[ch]->p, X.ct_slot.data(), cf ? &epi : nullptr);
+    }
+    for (int i = 0; i < X.n; i++) {
+        const double s = X.in[i]->scale;
+        out[i] = slab_output(c, big, X.first[i], X.in[i], cf ? cf->out_scale : s * s, X.vslot[i]);
     }
 }
-// the output scale scale(a) s^2 of inputs at scale s; scale(b) s and scale(c) must equal it
-static double poly2_out_scale(double s, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc) {
-    const double out_scale = a->scale * s * s;
-    if (b && b->scale * s != out_scale) fail("Scales do not match.");
-    if (cc && cc->scale != out_scale) fail("Scales do not match.");
-    return out_scale;
-}
-// the operations of a x^2 + b x + c on `total` ciphertexts of one channel beyond the product (a term that is 0 mod t is skipped there)
-static void poly2_count(Context &c, u64 A, u64 B, u64 C, int total) {
-    if (A) c.op_count[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
-    if (B) {
-        c.op_count[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
-        c.op_count[Context::OP_ADD] += (uint64_t)total;
+// SquareActivation over a whole matrix: every column PointwiseMultiply'd with itself in one wave per channel; inputs of any scales
+extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n < 1) fail("empty layer");
+    bool chained = false; // a square of a pending square: a polynomial chain (x^4), not an activation that feeds a scalar-MAC layer
+    for (int i = 0; i < n; i++) chained = chained || (in[i] && in[i]->pend);
+    const ActInputs X = act_inputs(c, in, n, "multiplying two plaintexts is not implemented");
+    const int total = X.total();
+    // The products stay unrelinearised until something reads them (DESIGN 4.15): a scalar-MAC layer then key-switches its outputs instead
+    // of these, with the same words.  Eager where that path can never run: with the noise trace (it measures every relinearised square),
+    // without the plane-source key switch or with digits wider than 16 bits, when the size-3 slab would pass 8 GiB, and for a square of
+    // squares, whose next consumer is another product rather than a scalar-MAC layer.
+    const size_t s3 = (size_t)3 * c.k * c.N;
+    if (!chained && !c.trace_noise && relin_planes_built(c) && hm::bit_length(c.dm_relin.mask) <= 16 && (size_t)total * s3 <= ((size_t)1 << 30)) {
+        auto g = std::make_shared<PendingGroup>();
+        g->total = total;
+        g->ct_slot = X.ct_slot;
+        g->slab3.resize(c.P);
+        for (int ch = 0; ch < c.P; ch++) {
+            c.set_channel(ch);
+            (void)relin_keys(c, ch, total, X.ct_slot.data()); // a missing key fails here, as it does for the eager square
+            g->slab3[ch] = c.alloc((size_t)total * s3);
+            const std::vector<const u64 *> xs = X.blocks(ch);
+            op_multiply(c, ch, xs, xs, g->slab3[ch]->p);
+            c.op_count[Context::OP_RELINEARIZE] += (uint64_t)total; // booked here, as the eager square books it
+        }
+        for (int i = 0; i < n; i++) {
+            out[i] = new_vec(c, in[i]->dim, in[i]->scale * in[i]->scale, in[i]->format, true, in[i]->blocks);
+            out[i]->slot = X.vslot[i];
+            out[i]->pend = g;
+            out[i]->pend_ct = (size_t)X.first[i];
+            g->members.push_back(out[i]);
+        }
+        return CNHE_OK;
     }
-    if (C) c.op_count[Context::OP_ADD_PLAIN] += (uint64_t)total;
+    square_layer(c, X, nullptr, out);
+    API_END
 }
 // The quadratic activation a x^2 + b x + c over a whole matrix, in cnhe_layer_square's passes: the BEHZ floor kernel scales the size-3
 // product by A and adds B x and Delta C (FloorEpi), so out[i] = relinearize(A (.) in[i]^2) + B (.) in[i] + C word for word
@@ -2740,36 +2803,8 @@ extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, c
                                 cnhe_vec **out) {
     API_BEGIN(h)
     if (n < 1) fail("empty layer");
-    poly2_check_coeffs(c, a, b, cc);
-    std::vector<int> first(n + 1, 0);
-    for (int i = 0; i < n; i++) {
-        same_ctx(c, in[i]);
-        if (!in[i]->enc) fail("the inputs must be encrypted");
-        if (in[i]->scale != in[0]->scale) fail("Scales do not match.");
-        first[i + 1] = first[i] + in[i]->blocks;
-    }
-    const double out_scale = poly2_out_scale(in[0]->scale, a, b, cc);
-    const int total = first[n];
-    const std::vector<int> vslot = vec_slots(c, in, n);
-    std::vector<int> ct_slot;
-    for (int i = 0; i < n; i++) ct_slot.insert(ct_slot.end(), in[i]->blocks, vslot[i]);
-    std::vector<BufRef> big(c.P);
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        const u64 A = a->scalars[ch][0], B = b ? b->scalars[ch][0] : 0, C = cc ? cc->scalars[ch][0] : 0;
-        FloorEpi epi = floor_epi(c, ch, A, B, C);
-        if (C) epi.c_poly = padded_constants(c, ch, in, n, total, C);
-        big[ch] = c.alloc((size_t)total * c.ct_words());
-        std::vector<const u64 *> ptrs;
-        for (int i = 0; i < n; i++)
-            for (int bl = 0; bl < in[i]->blocks; bl++) ptrs.push_back(in[i]->block(ch, bl));
-        op_multiply_relin(c, ch, ptrs, ptrs, big[ch]->p, ct_slot.data(), &epi);
-        poly2_count(c, A, B, C, total); // the operations of the composition
-    }
-    for (int i = 0; i < n; i++) {
-        out[i] = slab_view(new_vec(c, in[i]->dim, out_scale, in[i]->format, true, in[i]->blocks), big, first[i]);
-        out[i]->slot = vslot[i];
-    }
+    ActCoeffs cf = quad_coeffs(c, a, b, cc);
+    square_layer(c, act_inputs(c, in, n, "the inputs must be encrypted", &cf), &cf, out);
     API_END
 }
 // The square (a == NULL) or quadratic activation followed by a scalar-MAC layer, relinearising the layer's outputs instead of its squared
@@ -2782,12 +2817,14 @@ extern "C" int cnhe_layer_activation_conv_dense(cnhe_ctx *h, const cnhe_vec *con
                                                 const cnhe_vec *const *bias, int M, int K, cnhe_vec **out) {
     API_BEGIN(h)
     if (n_in < 1) fail("empty layer");
-    if (a) poly2_check_coeffs(c, a, b, cc);
-    else if (b || cc) fail("the quadratic coefficient is required");
+    std::optional<ActCoeffs> cf; // none: the square
+    if (a || b || cc) cf = quad_coeffs(c, a, b, cc);
     same_ctx(c, in[0]);
-    const double s = in[0]->scale, act_scale = a ? poly2_out_scale(s, a, b, cc) : s * s;
+    if (cf) cf->read(c, in[0]->scale);
+    const double act_scale = cf ? cf->out_scale : in[0]->scale * in[0]->scale;
     const MacLayer L = mac_prepare(c, in, n_in, act_scale, gather, weights, bias, M, K);
-    const int bl = L.bl, total = n_in * bl;
+    const ActInputs X(in, n_in);
+    const int bl = L.bl, total = X.total();
     const size_t w3 = (size_t)3 * c.k * c.N;
     if ((size_t)total * w3 > ((size_t)1 << 30)) fail("the size-3 products of the layer's inputs exceed the 8 GiB scratch limit");
     std::vector<int> ct_slot; // relinearisation: every output under the key slot its taps share
@@ -2801,19 +2838,10 @@ extern "C" int cnhe_layer_activation_conv_dense(cnhe_ctx *h, const cnhe_vec *con
         c.set_channel(ch);
         WsScope scope(c); // the size-3 slabs of this channel go back to its stream when its key switch is done
         u64 *x3 = c.ws_alloc((size_t)total * w3), *y3 = c.ws_alloc((size_t)M * bl * w3);
-        std::vector<const u64 *> ptrs;
-        for (int i = 0; i < n_in; i++)
-            for (int bb = 0; bb < bl; bb++) ptrs.push_back(in[i]->block(ch, bb));
         FloorEpi epi;
-        const FloorEpi *ep = nullptr;
-        if (a) {
-            const u64 A = a->scalars[ch][0], B = b ? b->scalars[ch][0] : 0, C = cc ? cc->scalars[ch][0] : 0;
-            epi = floor_epi(c, ch, A, B, C);
-            if (C) epi.c_poly = padded_constants(c, ch, in, n_in, total, C);
-            ep = &epi;
-            poly2_count(c, A, B, C, total);
-        }
-        op_multiply(c, ch, ptrs, ptrs, x3, ep);
+        if (cf) epi = act_epilogue(c, ch, X, cf->res[ch][2], cf->res[ch][1], cf->res[ch][0]);
+        const std::vector<const u64 *> xs = X.blocks(ch);
+        op_multiply(c, ch, xs, xs, x3, cf ? &epi : nullptr);
         std::vector<const u64 *> ip((size_t)bl * n_in);
         for (int bb = 0; bb < bl; bb++)
             for (int i = 0; i < n_in; i++) ip[(size_t)bb * n_in + i] = x3 + ((size_t)i * bl + bb) * w3;
@@ -2822,13 +2850,9 @@ extern "C" int cnhe_layer_activation_conv_dense(cnhe_ctx *h, const cnhe_vec *con
         mac_channel(c, L, ch, ip, op, 3);
         op_relinearize(c, ch, y3, M * bl, big[ch]->p, ct_slot.data());
     }
-    for (int m = 0; m < M; m++) {
-        out[m] = slab_view(new_vec(c, in[0]->dim, act_scale * weights[0]->scale, CNHE_DENSE, true, bl), big, (size_t)m * bl);
-        out[m]->slot = L.out_slot[m];
-    }
+    for (int m = 0; m < M; m++) out[m] = slab_output(c, big, (size_t)m * bl, in[0], act_scale * weights[0]->scale, L.out_slot[m]);
     API_END
 }
-
 // Quartic and cubic activations in two multiplicative levels built from squares only (DESIGN.md section 4.12).  Per plaintext prime t,
 // with the coefficients c_j of x^j reduced mod t and A the leading one:
 //   quartic (A, B, C, D, E): beta = B (2A)^-1, gamma = (C A^-1 - beta^2) 2^-1, D' = D - B gamma, E' = E - A gamma^2:
@@ -2864,88 +2888,35 @@ extern "C" int cnhe_layer_poly(cnhe_ctx *h, const cnhe_vec *const *in, int n, co
     API_BEGIN(h)
     if (n < 1) fail("empty layer");
     if (degree != 3 && degree != 4) fail("the degree must be 3 or 4");
-    if (!coeffs || !coeffs[degree]) fail("the leading coefficient is required");
-    for (int j = 0; j <= degree; j++) {
-        const cnhe_vec *p = coeffs[j];
-        if (!p) continue;
-        same_ctx(c, p);
-        if (p->enc) fail("the coefficients must be plain");
-        if (p->format != CNHE_SPARSE || p->dim != 1) fail("each coefficient must be a sparse vector of dimension 1");
-    }
-    std::vector<int> first(n + 1, 0);
-    for (int i = 0; i < n; i++) {
-        same_ctx(c, in[i]);
-        if (!in[i]->enc) fail("the inputs must be encrypted");
-        if (in[i]->scale != in[0]->scale) fail("Scales do not match.");
-        first[i + 1] = first[i] + in[i]->blocks;
-    }
-    // coefficient j at scale W s^(degree - j), W the leading coefficient's scale; the powers of s multiplied up one factor at a time
-    const double s = in[0]->scale, W = coeffs[degree]->scale;
-    auto scale_at = [&](int e) {
-        double r = W;
-        for (int i = 0; i < e; i++) r *= s;
-        return r;
-    };
-    for (int j = 0; j < degree; j++)
-        if (coeffs[j] && coeffs[j]->scale != scale_at(degree - j)) fail("Scales do not match.");
-    std::vector<PolyConsts> pk(c.P);
-    for (int ch = 0; ch < c.P; ch++) {
-        const u64 t = c.ch[ch].t;
-        u64 cf[5];
-        for (int j = 0; j <= degree; j++) cf[j] = coeffs[j] ? coeffs[j]->scalars[ch][0] % t : 0;
-        if (cf[degree] == 0)
-            fail(("the leading coefficient is 0 mod the plaintext prime " + std::to_string(t) + ": it has no inverse there").c_str());
-        pk[ch] = poly_consts(t, degree, cf);
-    }
-    const double out_scale = scale_at(degree);
-    const int total = first[n];
+    ActCoeffs cf(c, coeffs, degree, "the leading coefficient is required");
+    const ActInputs X = act_inputs(c, in, n, "the inputs must be encrypted", &cf);
+    const int total = X.total();
     const size_t cw = c.ct_words();
-    const std::vector<int> vslot = vec_slots(c, in, n);
-    std::vector<int> ct_slot;
-    for (int i = 0; i < n; i++) ct_slot.insert(ct_slot.end(), in[i]->blocks, vslot[i]);
     std::vector<BufRef> big(c.P);
     auto &ops = c.op_count;
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
-        const PolyConsts &k = pk[ch];
+        const PolyConsts k = poly_consts(c.ch[ch].t, degree, cf.res[ch].data());
         big[ch] = c.alloc((size_t)total * cw);
-        std::vector<const u64 *> xs;
-        for (int i = 0; i < n; i++)
-            for (int bl = 0; bl < in[i]->blocks; bl++) xs.push_back(in[i]->block(ch, bl));
+        const std::vector<const u64 *> xs = X.blocks(ch);
         const u64 *const *x_tab = upload_ptrs(c, xs);
-        // the operations of the composition (a term that is 0 mod t is skipped in that channel, as in cnhe_layer_poly2)
-        auto linear_and_constant = [&](u64 lin, u64 cst) {
-            if (lin) {
-                ops[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
-                ops[Context::OP_ADD] += (uint64_t)total;
-            }
-            if (cst) ops[Context::OP_ADD_PLAIN] += (uint64_t)total;
-        };
-        FloorEpi e2 = floor_epi(c, ch, k.lead, k.lin, k.cst);
-        e2.x = x_tab;
-        if (k.cst) e2.c_poly = padded_constants(c, ch, in, n, total, k.cst);
+        FloorEpi e2 = act_epilogue(c, ch, X, k.lead, k.lin, k.cst, x_tab);
         BufRef mid;
         std::vector<const u64 *> sq; // the second level's squared operands
         if (degree == 4) {
             // level 1: q = cnhe_layer_poly2(x; 1, beta, gamma)
             mid = c.alloc((size_t)total * cw);
-            FloorEpi e1 = floor_epi(c, ch, 1, k.b, k.g);
-            if (k.g) e1.c_poly = padded_constants(c, ch, in, n, total, k.g);
-            op_multiply_relin(c, ch, xs, xs, mid->p, ct_slot.data(), &e1);
-            ops[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
-            linear_and_constant(k.b, k.g);
+            FloorEpi e1 = act_epilogue(c, ch, X, 1, k.b, k.g);
+            op_multiply_relin(c, ch, xs, xs, mid->p, X.ct_slot.data(), &e1);
             for (int i = 0; i < total; i++) sq.push_back(mid->p + (size_t)i * cw);
             // level 2: relinearize(A (.) q^2) + D' x + E'
-            op_multiply_relin(c, ch, sq, sq, big[ch]->p, ct_slot.data(), &e2);
-            ops[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
+            op_multiply_relin(c, ch, sq, sq, big[ch]->p, X.ct_slot.data(), &e2);
         } else {
-            // level 1: u = relinearize(x^2) in [0, total), q1 = u + x + gamma in [total, 2 total)
+            // level 1: u = relinearize(x^2) in [0, total), q1 = u + x + gamma in [total, 2 total): an addition, not a floor epilogue
             mid = c.alloc((size_t)2 * total * cw);
             u64 *u = mid->p, *q1 = mid->p + (size_t)total * cw;
-            op_multiply_relin(c, ch, xs, xs, u, ct_slot.data());
-            FloorEpi e1 = floor_epi(c, ch, 1, 1, k.g);
-            e1.x = x_tab;
-            if (k.g) e1.c_poly = padded_constants(c, ch, in, n, total, k.g);
+            op_multiply_relin(c, ch, xs, xs, u, X.ct_slot.data());
+            FloorEpi e1 = act_epilogue(c, ch, X, 1, 1, k.g, x_tab, false);
             c.prof_begin(2, 24.0 * c.N * total * 2 * c.k);
             c.check(launch_ct_add_epi(u, q1, total, c.k, c.logN, c.d_bc, e1, c.stream), "ct_add_epi");
             c.prof_end();
@@ -2956,16 +2927,11 @@ extern "C" int cnhe_layer_poly(cnhe_ctx *h, const cnhe_vec *const *in, int n, co
                 sq.push_back(u + (size_t)i * cw);
             }
             // level 2: relinearize(lambda (.) (q1^2 - u^2)) + C' x + D', one key switch per output
-            op_multiply_relin(c, ch, sq, sq, big[ch]->p, ct_slot.data(), &e2, true);
+            op_multiply_relin(c, ch, sq, sq, big[ch]->p, X.ct_slot.data(), &e2, true);
             ops[Context::OP_SUB] += (uint64_t)total;
-            ops[Context::OP_MULTIPLY_SCALAR] += (uint64_t)total;
         }
-        linear_and_constant(k.lin, k.cst);
     }
-    for (int i = 0; i < n; i++) {
-        out[i] = slab_view(new_vec(c, in[i]->dim, out_scale, in[i]->format, true, in[i]->blocks), big, first[i]);
-        out[i]->slot = vslot[i];
-    }
+    for (int i = 0; i < n; i++) out[i] = slab_output(c, big, X.first[i], in[i], cf.out_scale, X.vslot[i]);
     API_END
 }
 
