@@ -124,6 +124,7 @@ _SIGS = {
     "cnhe_raw_rotate_rows": [C.c_void_p, i32, u64, i32, i32, u64],
     "cnhe_raw_behz_lift": [C.c_void_p, u64, i32, u64],
     "cnhe_raw_behz_floor": [C.c_void_p, i32, u64, i32, u64],
+    "cnhe_raw_import_products": [C.c_void_p, U64P, i32, u64, C.c_double, i32, C.POINTER(VECP)],
     "cnhe_raw_event_timing": [C.c_void_p, i32],
     "cnhe_raw_elapsed_ms": [C.c_void_p, C.POINTER(C.c_float)],
     "cnhe_kernel_launch_count": [C.c_void_p],

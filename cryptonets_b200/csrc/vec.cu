@@ -2797,6 +2797,42 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
     square_layer(c, X, nullptr, out);
     API_END
 }
+// Chosen size-3 words as pending squares: n one-block vectors sharing one group in key slot `slot`, as cnhe_layer_square returns them, so
+// that a test can place any digit in any plane of the exact scalar-MAC path.  Refused where the square would be eager, and for words that
+// are not canonical residues.
+extern "C" int cnhe_raw_import_products(cnhe_ctx *h, const uint64_t *words, int n, uint64_t dim, double scale, int slot, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (!words || n < 1 || !out || dim < 1 || dim > c.N) fail("bad arguments");
+    if (!c.slot_live(slot)) fail("no such key slot");
+    const size_t s3 = (size_t)3 * c.k * c.N;
+    if (c.trace_noise || !relin_planes_built(c) || hm::bit_length(c.dm_relin.mask) > 16 || (size_t)n * s3 > ((size_t)1 << 30))
+        fail("the context keeps no products pending (noise trace, no plane-source key switch, digits wider than 16 bits or over 8 GiB)");
+    for (int ch = 0; ch < c.P; ch++)
+        for (size_t j = 0; j < (size_t)n * 3 * c.k; j++) {
+            const uint64_t *r = words + ((size_t)ch * n * 3 * c.k + j) * c.N, q = c.q[j % c.k];
+            for (size_t i = 0; i < c.N; i++)
+                if (r[i] >= q) fail("the words are not canonical residues");
+        }
+    auto g = std::make_shared<PendingGroup>();
+    g->total = n;
+    g->ct_slot.assign(n, slot);
+    g->slab3.resize(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        (void)relin_keys(c, ch, n, g->ct_slot.data()); // a missing key fails here, as it does for the square
+        g->slab3[ch] = c.alloc((size_t)n * s3);
+        CNHE_CUDA(cudaMemcpyAsync(g->slab3[ch]->p, words + (size_t)ch * n * s3, (size_t)n * s3 * 8, cudaMemcpyHostToDevice, c.stream));
+    }
+    c.sync();
+    for (int i = 0; i < n; i++) {
+        out[i] = new_vec(c, dim, scale, CNHE_DENSE, true, 1);
+        out[i]->slot = slot;
+        out[i]->pend = g;
+        out[i]->pend_ct = (size_t)i;
+        g->members.push_back(out[i]);
+    }
+    API_END
+}
 // The quadratic activation a x^2 + b x + c over a whole matrix, in cnhe_layer_square's passes: the BEHZ floor kernel scales the size-3
 // product by A and adds B x and Delta C (FloorEpi), so out[i] = relinearize(A (.) in[i]^2) + B (.) in[i] + C word for word
 extern "C" int cnhe_layer_poly2(cnhe_ctx *h, const cnhe_vec *const *in, int n, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *cc,

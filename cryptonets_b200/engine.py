@@ -783,6 +783,15 @@ class Engine:
     def raw_behz_floor(self, ch, d, n, out3):
         check(self.L.cnhe_raw_behz_floor(self.h, ch, int(d), int(n), int(out3)))
 
+    def raw_import_products(self, words, n, dim=None, scale=1.0, slot=0):
+        """n size-3 products (words [P][n][3][k][N]) as pending squares of one group in key slot `slot` (include/cnhe.h,
+        cnhe_raw_import_products): a scalar-MAC layer over them takes the exact path, any other read relinearises them."""
+        a = _u64(words).ravel()
+        assert a.size == self.P * n * 3 * self.k * self.N
+        out = (VECP * n)()
+        check(self.L.cnhe_raw_import_products(self.h, _p(a), int(n), int(self.N if dim is None else dim), float(scale), int(slot), out))
+        return self._wrap_many(out, n)
+
     def timer_start(self):
         check(self.L.cnhe_raw_event_timing(self.h, 1))
 

@@ -396,6 +396,12 @@ int cnhe_raw_rotate_rows(cnhe_ctx *, int channel, uint64_t in, int n, int steps,
 int cnhe_raw_behz_lift(cnhe_ctx *, uint64_t in_cts, int n, uint64_t out_together);
 int cnhe_raw_behz_floor(cnhe_ctx *, int channel, uint64_t d_together, int n, uint64_t out3);
 int cnhe_dev_copy(cnhe_ctx *, uint64_t dst, uint64_t src, size_t words); /* device to device, on the context stream */
+/* n size-3 products from host words [P][n][3][k][N] as n one-block dense vectors of dimension dim (<= N) in key slot `slot`, left
+ * unrelinearised in one group exactly as cnhe_layer_square leaves its squares: a scalar-MAC layer over all of them takes the exact
+ * path (DESIGN 4.15), any other read relinearises the group.  For parity tests of that path with chosen digits.  CNHE_ERR_INVALID where
+ * cnhe_layer_square would relinearise at once (noise trace, no plane-source key switch, digits wider than 16 bits, more than 8 GiB of
+ * products) and for words that are not canonical residues. */
+int cnhe_raw_import_products(cnhe_ctx *, const uint64_t *words, int n, uint64_t dim, double scale, int slot, cnhe_vec **out);
 /* per-kernel-family device timing (CUDA events around the launches on the context stream): enable, run, collect.
  * family: 0 ntt forward (incl. digit variant), 1 ntt inverse, 2 behz element-wise, 3 key-switch mac, 4 scalar mac layer, 5 other */
 int cnhe_prof_enable(cnhe_ctx *, int on);

@@ -128,6 +128,7 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_raw_behz_lift(IntPtr a0, ulong in_cts, int n, ulong out_together);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_raw_behz_floor(IntPtr a0, int channel, ulong d_together, int n, ulong out3);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_dev_copy(IntPtr a0, ulong dst, ulong src, UIntPtr words);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_raw_import_products(IntPtr a0, ulong[] words, int n, ulong dim, double scale, int slot, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_prof_enable(IntPtr a0, int on);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_prof_collect(IntPtr a0, int family, out double total_ms, out ulong launches, out double algorithmic_bytes);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_raw_event_timing(IntPtr a0, int start);

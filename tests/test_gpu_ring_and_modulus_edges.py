@@ -17,38 +17,7 @@ import worst_case_inputs as W
 pytestmark = pytest.mark.gpu
 
 
-def _is_prime(n):
-    if n < 2:
-        return False
-    for sp in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37):
-        if n % sp == 0:
-            return n == sp
-    d, s = n - 1, 0
-    while d % 2 == 0:
-        d, s = d // 2, s + 1
-    for a in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37):  # deterministic below 3.3e24
-        x = pow(a, d, n)
-        if x in (1, n - 1):
-            continue
-        for _ in range(s - 1):
-            x = x * x % n
-            if x == n - 1:
-                break
-        else:
-            return False
-    return True
-
-
-def _primes(bits, N, count=1):
-    """the `count` largest `bits`-bit primes = 1 mod 2N, descending (none of them 48-bit, so none is a fast Bsk prime)"""
-    assert bits != 48
-    out, c = [], ((1 << bits) - 1) // (2 * N) * (2 * N) + 1
-    while len(out) < count:
-        if _is_prime(c):
-            out.append(c)
-        c -= 2 * N
-    assert all(p.bit_length() == bits for p in out)
-    return out
+_primes = W.primes
 
 
 # name: t, N, q (None: the default coefficient modulus, cut to `count` primes); fp: FP64 transforms on every q prime; umma: the wgmma

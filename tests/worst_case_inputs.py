@@ -155,6 +155,8 @@ def _solve(w, p, sign, limit=None):
     goal = sign * int(TARGET * p)
     if limit is None or limit >= p:
         return goal * pow(w, -1, p) % p
+    if limit > 1 << 16 and limit < p >> 16:
+        return _near_class(w, p, goal, limit)
     if limit > 1 << 16:  # walk the classes outwards from the goal until one has a small enough preimage
         wi = pow(w, -1, p)
         for off in range(1 << 20):
@@ -166,16 +168,51 @@ def _solve(w, p, sign, limit=None):
     return int(ys[int(np.argmin([abs(int(v) - goal) for v in prods]))])
 
 
-def forward_worst_case(p, wd, out_index, digit_bits=None, negative=False):
+def _near_class(w, p, goal, limit):
+    """y in [0, limit) whose centred product with w is near goal, for preimage ranges too sparse to walk (limit / p below 2^-16): the
+    lattice {(s y, w y + p z)}, s = p // limit, weighs both coordinates alike; Babai rounding on its Lagrange-reduced basis gives a
+    vector near (s limit / 2, goal), so y is near limit / 2 and the product within about p / sqrt(limit) of goal"""
+    from fractions import Fraction
+    s = max(1, p // limit)
+    b1, b2 = (s, w % p), (0, p)
+    n2 = lambda v: v[0] * v[0] + v[1] * v[1]
+    if n2(b1) > n2(b2):
+        b1, b2 = b2, b1
+    while True:
+        mu = round(Fraction(b1[0] * b2[0] + b1[1] * b2[1], n2(b1)))
+        b2 = (b2[0] - mu * b1[0], b2[1] - mu * b1[1])
+        if n2(b2) >= n2(b1):
+            break
+        b1, b2 = b2, b1
+    tx, ty = s * (limit // 2), goal
+    det = b1[0] * b2[1] - b1[1] * b2[0]
+    c1, c2 = Fraction(tx * b2[1] - ty * b2[0], det), Fraction(b1[0] * ty - b1[1] * tx, det)
+    best = None
+    for d1 in (-1, 0, 1, 2):
+        for d2 in (-1, 0, 1, 2):
+            a1, a2 = c1.__floor__() + d1, c2.__floor__() + d2
+            y = (a1 * b1[0] + a2 * b2[0]) // s
+            if 0 <= y < limit:
+                err = abs(centred(w * y, p) - goal)
+                if best is None or err < best[0]:
+                    best = (err, y)
+    if best is None:
+        raise ValueError("no preimage below %d" % limit)
+    return best[1]
+
+
+def forward_worst_case(p, wd, out_index, digit_bits=None, negative=False, limit=None):
     """Canonical input whose lazy value on the path from input 0 to output `out_index` grows by TARGET*p at every stage.
 
     a[0] is maximal.  On that path the path value is always the upper operand of its butterfly; the partner at stage s is input
     N >> (s+1) on its own (its subtree holds nothing else), so one coefficient per stage is solved to make w*y = +-TARGET p, with the
-    sign that adds to the path on the branch the output takes.  digit_bits: every coefficient below 2^digit_bits (a digit plane).
-    negative: every product subtracts instead, so the output ends near -(logN TARGET - 1) p."""
+    sign that adds to the path on the branch the output takes.  digit_bits: every coefficient below 2^digit_bits (a digit plane);
+    limit: every coefficient below limit (<= p) instead.  negative: every product subtracts instead, so the output ends near
+    -(logN TARGET - 1) p."""
     N = len(wd)
     logN = N.bit_length() - 1
-    limit = None if digit_bits is None else min(1 << digit_bits, p)
+    if limit is None:
+        limit = None if digit_bits is None else min(1 << digit_bits, p)
     a = [0] * N
     a[0] = (p - 1) if limit is None else limit - 1
     pos = 0
@@ -230,6 +267,41 @@ def square_root_near_target(p, seed=0):
 def key_constant(p, v):
     """K with K*v = TARGET p (mod p): the NTT-domain key word that turns the digit constant v into the worst product"""
     return int(TARGET * p) * pow(v % p, -1, p) % p
+
+
+# ---------------------------------------------------------------- NTT-friendly primes of a chosen width
+def is_prime(n):
+    if n < 2:
+        return False
+    for sp in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37):
+        if n % sp == 0:
+            return n == sp
+    d, s = n - 1, 0
+    while d % 2 == 0:
+        d, s = d // 2, s + 1
+    for a in (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37):  # deterministic below 3.3e24
+        x = pow(a, d, n)
+        if x in (1, n - 1):
+            continue
+        for _ in range(s - 1):
+            x = x * x % n
+            if x == n - 1:
+                break
+        else:
+            return False
+    return True
+
+
+def primes(bits, N, count=1):
+    """the `count` largest `bits`-bit primes = 1 mod 2N, descending (none of them 48-bit, so none is a fast Bsk prime)"""
+    assert bits != 48
+    out, c = [], ((1 << bits) - 1) // (2 * N) * (2 * N) + 1
+    while len(out) < count:
+        if is_prime(c):
+            out.append(c)
+        c -= 2 * N
+    assert all(p.bit_length() == bits for p in out)
+    return out
 
 
 # ---------------------------------------------------------------- digit decomposition (make_digit_map, runtime.cu)
@@ -317,18 +389,24 @@ def behz_extreme_cts(q, N, fresh):
 
 
 # ---------------------------------------------------------------- closed-form key switch
-def key_switch_reference(orc, target, keys, dbc):
+def key_switch_reference(orc, target, keys, dbc, planes=None):
     """(2 x k x N) INTT(sum_d NTT(digit_d) * K_d) mod q_l for target residues (k x N) and NTT-domain keys (D x 2 x k x N), from the
-    oracle's transforms: the part a key switch adds to its base"""
+    oracle's transforms: the part a key switch adds to its base.  planes: signed integer digit planes (D x N) in place of the digits
+    of a target (the plane-source key switch; target is then unused), taken modulo each q_l."""
     q, N = orc.q, orc.N
     k = len(q)
     dm = digit_map(q, dbc)
     keys = np.asarray(keys, dtype=np.uint64).reshape(len(dm), 2, k, N)
     out = np.zeros((2, k, N), np.uint64)
+    if planes is not None:
+        planes = np.asarray(planes, dtype=np.int64).reshape(len(dm), N)
     for l in range(k):
         ql = q[l]
-        digits = np.stack([((np.asarray(target[i], dtype=np.uint64) >> np.uint64(sh)) & np.uint64((1 << dbc) - 1)).astype(object) % ql
-                           for i, sh in dm]).astype(np.uint64)
+        if planes is not None:
+            digits = (planes % ql).astype(np.uint64)  # numpy's % takes the divisor's sign: canonical residues
+        else:
+            digits = np.stack([((np.asarray(target[i], dtype=np.uint64) >> np.uint64(sh)) & np.uint64((1 << dbc) - 1)).astype(object) % ql
+                               for i, sh in dm]).astype(np.uint64)
         nt = orc.ntt_batch(l, digits).astype(object)
         for part in range(2):
             acc = (nt * keys[:, part, l, :].astype(object)).sum(axis=0) % ql
