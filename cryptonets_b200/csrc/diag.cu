@@ -117,17 +117,17 @@ __device__ __forceinline__ void diag_mac_pair(double (&a)[CB][2][2], const u64 *
 
 // k_diag_mac over diagonals held resident in NTT form (cnhe_diag_prepare_ntt): nothing produced them just before, so every diagonal word
 // streams from HBM, and the kernel is built for that.  One thread per (g, l, coefficient pair): 16-byte loads of the diagonal and of the
-// baby-step words.  A full re-centring period (8 diagonals) is straight-line code in chunks of D diagonals: a chunk's D diagonal loads
-// (evict-first, so that they do not push the baby-step words the giant steps share out of L2) and baby-step indices are issued before its
-// first product, so D diagonals' loads are in flight together with the baby-step loads the compiler hoists.  D trades loads in flight
-// against registers, and so against resident warps.  CTA order as in k_diag_mac (g fastest, then the 512-coefficient tile, then l).  Per
+// baby-step words.  A full re-centring period (8 diagonals) is straight-line code in chunks of D = 2 diagonals: a chunk's two diagonal
+// loads (evict-first, so that they do not push the baby-step words the giant steps share out of L2) and baby-step indices are issued
+// before its first product, so they are in flight together with the baby-step loads the compiler hoists (4 and 8 took more registers
+// and were no faster, DESIGN.md 4.10).  CTA order as in k_diag_mac (g fastest, then the 512-coefficient tile, then l).  Per
 // (g, client, l, i) the arithmetic is k_diag_mac's in the same order: fmodmul of canonical operands, dadd, re-centred after every 8th term
 // and at the end, fsmall_u -- so the outputs are bit-identical.
-template <int CB, int D>
+template <int CB>
 __global__ void __launch_bounds__(256) k_diag_mac_resident(const u64 *__restrict__ dhat, const u64 *__restrict__ xhat, const int *__restrict__ g_start,
                                                            const int *__restrict__ xsel, u64 *__restrict__ acc, int ng, int B, int logn,
                                                            const __grid_constant__ BehzConstF F) {
-    static_assert(8 % D == 0, "D divides the re-centring period");
+    constexpr int D = 2;
     const int N = 1 << logn, k = F.k, tiles = N >> 9;
     const int g = blockIdx.x % ng, tile = (blockIdx.x / ng) % tiles, l = blockIdx.x / (ng * tiles);
     const int i = (tile << 9) + 2 * threadIdx.x;
@@ -203,22 +203,14 @@ cudaError_t launch_diag_mac(const u64 *dhat, const u64 *xhat, const int *g_start
     else k_diag_mac<8><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
     return cudaGetLastError();
 }
-template <int D>
-static void diag_mac_resident_cb(unsigned grid, const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B,
-                                 int logn, const BehzConstF &f, cudaStream_t s) {
-    if (B == 1) k_diag_mac_resident<1, D><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, f);
-    else if (B == 2) k_diag_mac_resident<2, D><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, f);
-    else if (B <= 4) k_diag_mac_resident<4, D><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, f);
-    else k_diag_mac_resident<8, D><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, f);
-}
 cudaError_t launch_diag_mac_resident(const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B, int k,
-                                     int logn, int depth, const BehzConstF *f, cudaStream_t s) {
+                                     int logn, const BehzConstF *f, cudaStream_t s) {
     if (ng <= 0 || B <= 0) return cudaSuccess;
     const unsigned grid = (unsigned)ng * (unsigned)((1 << logn) >> 9) * (unsigned)k;
-    if (depth == 2) diag_mac_resident_cb<2>(grid, dhat, xhat, g_start, xsel, acc, ng, B, logn, *f, s);
-    else if (depth == 4) diag_mac_resident_cb<4>(grid, dhat, xhat, g_start, xsel, acc, ng, B, logn, *f, s);
-    else if (depth == 8) diag_mac_resident_cb<8>(grid, dhat, xhat, g_start, xsel, acc, ng, B, logn, *f, s);
-    else return cudaErrorInvalidValue;
+    if (B == 1) k_diag_mac_resident<1><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
+    else if (B == 2) k_diag_mac_resident<2><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
+    else if (B <= 4) k_diag_mac_resident<4><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
+    else k_diag_mac_resident<8><<<grid, 256, 0, s>>>(dhat, xhat, g_start, xsel, acc, ng, B, logn, *f);
     return cudaGetLastError();
 }
 

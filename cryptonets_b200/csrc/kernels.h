@@ -258,10 +258,10 @@ cudaError_t launch_diag_gather(const u64 *vals, int R, int dim, const int *desc,
 // acc[g][b][p][l] = sum_{j = g_start[g]}^{g_start[g+1]-1} dhat[j][l] * xhat[xsel[j]][b][p][l]  (NTT form, canonical in and out; FP64 path)
 cudaError_t launch_diag_mac(const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B, int k, int logn,
                             const BehzConstF *f, cudaStream_t s);
-// the same sums, bit-identical, over diagonals held resident in NTT form (streamed from HBM: 16-byte loads, `depth` = 2, 4 or 8 diagonals'
-// loads issued together)
+// the same sums, bit-identical, over diagonals held resident in NTT form (streamed from HBM: 16-byte loads, two diagonals' loads issued
+// together)
 cudaError_t launch_diag_mac_resident(const u64 *dhat, const u64 *xhat, const int *g_start, const int *xsel, u64 *acc, int ng, int B, int k,
-                                     int logn, int depth, const BehzConstF *f, cudaStream_t s);
+                                     int logn, const BehzConstF *f, cudaStream_t s);
 
 // ---- sampling / encode / encrypt / decrypt
 enum SampleKind { SAMPLE_TERNARY = 0, SAMPLE_NOISE = 1, SAMPLE_UNIFORM = 2 };

@@ -126,9 +126,6 @@ struct Context {
         if (it != budget_of.end()) budget_of[dst] = it->second; else budget_of.erase(dst);
     }
     int known_budget(const u64 *p) const { auto it = budget_of.find(p); return it == budget_of.end() ? -1 : it->second; }
-    // the diagonal product's MAC over diagonals held in NTT form: k_diag_mac_resident with 2, 4 or 8 diagonals' loads issued together,
-    // or 0 for k_diag_mac (option "diag_mac_resident"; same outputs either way)
-    int diag_mac_resident = 2;
     // K_c of op_multiply_sum: the most tensor products whose sum the BEHZ floor still rounds exactly in this context's base Bsk (DESIGN 4.14)
     int sum_terms = 1;
     int chunk = 1024; // ciphertexts per kernel wave (upper bound: wave() also keeps a wave's scratch under ~8 GiB)

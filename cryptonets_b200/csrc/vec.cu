@@ -116,9 +116,6 @@ extern "C" int cnhe_context_set_option(cnhe_ctx *h, const char *name, int64_t va
         cudaMemPool_t pool;
         CNHE_CUDA(cudaDeviceGetDefaultMemPool(&pool, c.device));
         CNHE_CUDA(cudaMemPoolTrimTo(pool, 0));
-    } else if (n == "diag_mac_resident") {
-        if (value != 0 && value != 2 && value != 4 && value != 8) fail("diag_mac_resident must be 0, 2, 4 or 8");
-        c.diag_mac_resident = (int)value;
     } else if (n == "chunk") {
         if (value < 1 || value > 4096) fail("chunk must be in [1,4096]");
         c.chunk = (int)value;
@@ -3262,10 +3259,10 @@ extern "C" int cnhe_diag_destroy(cnhe_diag *d) {
 // y = sum_g rotate_rows(n1 g)( sum_{b,h} D'[g][b,h] (.) rotate_columns^b rotate_rows(h)(v) ) for B vectors at once (one per client; their key
 // slots may differ).  Per channel: the baby-step rotations of every client in one op_rotate_rows_multi (after one column rotation per
 // client when a diagonal has b = 1), their forward transforms, then waves of giant steps -- the wave's diagonals lifted and transformed
-// (a matrix from cnhe_diag_prepare_ntt holds those words for its resident prefix of giant steps, which then takes one wave and, unless
-// the option diag_mac_resident is 0, k_diag_mac_resident), every
-// client's inner sums in the NTT domain (k_diag_mac; dyadic products and additions off the FP64 path: the same residues), the
-// inverse transforms -- and finally the giant-step rotations of every (g, client) in one op_rotate_rows_multi and each client's sum.
+// (a matrix from cnhe_diag_prepare_ntt holds those words for its resident prefix of giant steps, which then takes one wave and
+// k_diag_mac_resident), every client's inner sums in the NTT domain (k_diag_mac; dyadic products and additions off the FP64 path: the
+// same residues), the inverse transforms -- and finally the giant-step rotations of every (g, client) in one op_rotate_rows_multi and
+// each client's sum.
 // Each inner sum equals the sum of the separate multiply_plain results, since the inverse transform is linear mod q_l.
 // A folded matrix then folds every client's sum in one wave per step -- rotate_columns when its input reaches the second row, then
 // rotate_rows by W, 2W, ..., N/4 (sum_slots_batched) -- so that slot i < n_rows holds row i's sum, and multiplies all B sums by one mask
@@ -3367,9 +3364,8 @@ extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe
                 c.h2d(dst, st.data(), st.size() * sizeof(int));
                 // HBM: the wave's diagonals once per 8 clients, the baby steps once (the giant steps share them through L2), the sums once
                 c.prof_begin(4, 8.0 * ((double)((B + 7) / 8) * m * kN + (double)nx * B * ctw + (double)gw * B * ctw));
-                if (resident && c.diag_mac_resident)
-                    c.check(launch_diag_mac_resident(L, X, dst, dxsel + j0, A, gw, B, k, c.logN, c.diag_mac_resident, &c.h_bf, c.stream),
-                            "diag_mac_resident");
+                if (resident)
+                    c.check(launch_diag_mac_resident(L, X, dst, dxsel + j0, A, gw, B, k, c.logN, &c.h_bf, c.stream), "diag_mac_resident");
                 else c.check(launch_diag_mac(L, X, dst, dxsel + j0, A, gw, B, k, c.logN, &c.h_bf, c.stream), "diag_mac");
                 c.prof_end();
             } else {

@@ -66,9 +66,8 @@ int cnhe_context_galois_elts(const cnhe_ctx *, uint64_t *out);
 /* options: "behz_centered_mtilde" (0/1), "chunk" (ciphertexts per multiply/key-switch wave), "multi_stream" (1: one CUDA
  * stream per plaintext modulus, default; 0: everything on one stream; refused while imported batches are alive),
  * "trace_noise" (1: record the invariant noise budget after every evaluator-level operation, see cnhe_trace_read),
- * "diag_mac_resident" (the MAC kernel over diagonals held in NTT form: 2, default, 4 or 8 diagonals' loads issued together, or 0 for the
- * coefficient-form path's kernel; the outputs are identical), "release_cached_memory" (any value: hand the scratch blocks the context
- * keeps for reuse back to the driver, e.g. before preparing a large resident matrix) */
+ * "release_cached_memory" (any value: hand the scratch blocks the context keeps for reuse back to the driver, e.g. before preparing a
+ * large resident matrix) */
 int cnhe_context_set_option(cnhe_ctx *, const char *name, int64_t value);
 int cnhe_context_sync(cnhe_ctx *);
 /* interop with the caller's own GPU work (the NCCL all-gather of the score ciphertexts): the CUDA stream (cudaStream_t as an integer) of a
@@ -303,8 +302,8 @@ int cnhe_mat_dot_rows_batch(cnhe_ctx *, const cnhe_vec *const *rows, int n_rows,
  *   giant-step groups whose NTT forms, summed over all channels (k N 8 bytes per diagonal and channel), fit in max_ntt_bytes are also held
  *   resident: lifted into every q_l and forward transformed, canonical, [diag][k][N] per channel -- the words cnhe_mat_mul_diagonal
  *   otherwise computes on every call.  UINT64_MAX holds the whole matrix, 0 none (the object then behaves as cnhe_diag_prepare's).
- *   cnhe_mat_mul_diagonal skips the lift and the transforms of the resident groups and runs a MAC kernel built to stream them from HBM
- *   (option "diag_mac_resident"); its outputs and counts are word for word the same.
+ *   cnhe_mat_mul_diagonal skips the lift and the transforms of the resident groups and runs a MAC kernel built to stream them from HBM;
+ *   its outputs and counts are word for word the same.
  *   The coefficient-form diagonals stay (cnhe_diag_export is unchanged); device_bytes of cnhe_diag_info counts both forms.
  * cnhe_diag_ntt_info: resident giant-step groups, resident diagonals and the device bytes of their NTT forms (any pointer may be NULL).
  * cnhe_diag_export_ntt: the k N resident words of stored diagonal `index` of a channel ([k][N]); an index outside the resident prefix,

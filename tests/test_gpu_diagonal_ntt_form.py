@@ -1,6 +1,7 @@
 """Diagonal matrices held in NTT form (cnhe_diag_prepare_ntt): the resident words against the oracle's lift and forward transform, the
 product word for word against the coefficient-form matrix of the same rows for every budget, client count, key-slot mix and the integer
-path, the budget bookkeeping, the refusals, and LoLa-Large / LoLa-CIFAR with a partial budget."""
+path, the budget bookkeeping, the refusals (the removed MAC option among them), and LoLa-Large / LoLa-CIFAR with a partial
+budget."""
 import os
 
 import numpy as np
@@ -143,24 +144,29 @@ def test_product_is_word_for_word_the_coefficient_forms(eng, budget, B):
     assert ni["giant_steps"] == groups and ni["diags"] == sum(sizes[:groups])
 
 
-@pytest.mark.parametrize("depth", [0, 2, 4, 8])
-def test_every_resident_mac_variant(eng, depth):
-    """The option diag_mac_resident picks the MAC over resident words (k_diag_mac_resident with 2 / 4 / 8 diagonals' loads together, or
-    k_diag_mac): every choice gives the coefficient form's words, for every client-count instantiation and partial periods."""
-    rng = np.random.default_rng(200 + depth)
+@pytest.mark.parametrize("B", [1, 2, 3, 5, 9])
+def test_resident_mac(eng, B):
+    """The MAC over the wholly resident matrix gives the coefficient form's words, for every client-count instantiation (B = 9: two
+    passes of 8), with groups whose lengths are not multiples of the 8-term re-centring period."""
+    rng = np.random.default_rng(200 + B)
     M = rng.integers(-1, 2, (37, 2100)).astype(np.float64) * (rng.random((37, 2100)) < 0.7)
-    eng.set_option("diag_mac_resident", depth)
-    try:
-        for B in (1, 2, 3, 5, 9):
-            xs = [eng.encrypt(rng.integers(-3, 4, 2100).astype(np.float64), 1.0) for _ in range(B)]
-            _compare(eng, M, 16, ALL, xs)
-    finally:
-        eng.set_option("diag_mac_resident", 2)
+    assert any(s % 8 for s in _group_sizes(M, N, 16))
+    xs = [eng.encrypt(rng.integers(-3, 4, 2100).astype(np.float64), 1.0) for _ in range(B)]
+    _compare(eng, M, 16, ALL, xs)
 
 
 def test_resident_mac_option_refusals(eng):
-    for bad in (1, 3, 16, -1):
-        assert _code(lambda: eng.set_option("diag_mac_resident", bad)) == ERR_INVALID
+    """diag_mac_resident, which once picked the resident MAC kernel, is an unknown option now, for the values it used to accept."""
+    for old in (0, 2, 8):
+        assert _code(lambda: eng.set_option("diag_mac_resident", old)) == ERR_INVALID
+    rng = np.random.default_rng(81)
+    M = rng.integers(-1, 2, (20, 100)).astype(np.float64)
+    d = _prepare(eng, M, 0, ALL)
+    v = rng.integers(-2, 3, 100).astype(np.float64)
+    y = eng.mat_mul_diagonal(d, [eng.encrypt(v, 1.0)])[0]
+    assert np.array_equal(eng.decrypt(y), M @ v)
+    y.dispose()
+    d.dispose()
 
 
 def test_giant_steps_with_gaps(eng):

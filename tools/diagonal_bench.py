@@ -5,11 +5,10 @@ Per network and method: device time per image (every layer synchronised), the de
 call), key switches per image from the
 operation counters (row-rotation hops + column rotations + relinearisations), and for the diagonal methods the prepare time, the
 coefficient-form and NTT-form bytes the prepared matrix holds, dense4 at B = 8 inputs in one call and the device time of one more dense4
-call per profiler family (cnhe_prof_collect; the lift is booked as "other", the MAC as "scalar_mac_layer", whose algorithmic bytes over
-its time give dense4_mac_GBps).  diagonal_ntt@D runs the NTT-form arm with the option diag_mac_resident = D (0: k_diag_mac), so the
-MAC kernels can be alternated.  held_bytes is the prepared matrix's device_bytes (both forms), coeff_bytes / ntt_bytes its parts.  Full residency takes about
-39 GB for LoLa-CIFAR and 46 GB for LoLa-Large: run one network per process.  Then the diagonal method at the reference's SmallModulusCount: whether the
-scores decrypt, and the budget entering the last layer.  --score-methods alternates the Method of the score layer (dense6: "rows", the
+call per profiler family at B = 1 and at B = 8 (cnhe_prof_collect; the lift is booked as "other", the MAC as "scalar_mac_layer", whose
+algorithmic bytes over its time give dense4_mac_GBps and dense4_B8_mac_GBps).  held_bytes is the prepared matrix's device_bytes (both
+forms), coeff_bytes / ntt_bytes its parts.  Full residency takes about 39 GB for LoLa-CIFAR and 46 GB for LoLa-Large: run one network
+per process.  Then the diagonal method at the reference's SmallModulusCount: whether the scores decrypt, and the budget entering the last layer.  --score-methods alternates the Method of the score layer (dense6: "rows", the
 reference's, and / or "folded") within every dense4 method; each record has dense6's time, its key switches and the bytes of the score
 ciphertexts.  Prints one JSON line per measurement (and writes them to --out if given)."""
 import argparse
@@ -60,14 +59,27 @@ def mem_used_mb():
         return None
 
 
+def profile(eng, call):
+    """Device time per profiler family of one call that returns a list of outputs (cnhe_prof_collect), and the diagonal MAC's
+    ("scalar_mac_layer") algorithmic HBM bytes over its device time."""
+    eng.sync()
+    eng.prof_enable(True)
+    outs = call()
+    eng.sync()
+    fam = eng.prof_collect()
+    eng.prof_enable(False)
+    for o in outs:
+        o.Dispose()
+    mac = fam["scalar_mac_layer"]
+    return {k: round(v["ms"], 3) for k, v in fam.items()}, (round(mac["bytes"] / mac["ms"] / 1e6, 1) if mac["ms"] else None)
+
+
 def run(f, name, method, imgs, batch8, ntt_bytes=None, score_method="rows"):
-    """method: rows, diagonal, or diagonal_ntt[@D] (D = the option diag_mac_resident: 2, 4, 8, or 0 for k_diag_mac)."""
+    """method: rows, diagonal or diagonal_ntt."""
     eng = f.engine
     diag = method != "rows"
-    base, _, depth = method.partition("@")
-    eng.set_option("diag_mac_resident", int(depth) if depth else 2)
     eng.set_option("release_cached_memory", 1)  # the previous arm's scratch goes back to the driver before this arm's matrix
-    kw = dict(diag_ntt_bytes=ntt_bytes) if base == "diagonal_ntt" else {}
+    kw = dict(diag_ntt_bytes=ntt_bytes) if method == "diagonal_ntt" else {}
     net, rd = getattr(nw, name)(f, imgs, dense_method="diagonal" if diag else "rows", score_method=score_method, **kw)
     layers = chain(net)
     D = 5  # reader, encrypt, pool, vectorize, square, dense4, square, dense
@@ -116,16 +128,7 @@ def run(f, name, method, imgs, batch8, ntt_bytes=None, score_method="rows"):
                dense6_key_switches=ks6, score_bytes=score_bytes, key_switches=ks, prepare_s=prep,
                held_bytes=held, coeff_bytes=coeff_held, ntt_bytes=ntt_held, device_mem_used_mb_after_prepare=mem_after_prepare)
     if diag:
-        eng.sync()
-        eng.prof_enable(True)
-        y = layers[D].Apply(x4)
-        eng.sync()
-        fam = eng.prof_collect()
-        rec["dense4_families_ms"] = {k: round(v["ms"], 3) for k, v in fam.items()}
-        mac = fam["scalar_mac_layer"]  # the diagonal MAC: its algorithmic HBM bytes over its device time
-        rec["dense4_mac_GBps"] = round(mac["bytes"] / mac["ms"] / 1e6, 1) if mac["ms"] else None
-        eng.prof_enable(False)
-        y.Dispose()
+        rec["dense4_families_ms"], rec["dense4_mac_GBps"] = profile(eng, lambda: [layers[D].Apply(x4)])
     if batch8 and diag:
         eng.sync()
         t0 = time.perf_counter()
@@ -134,6 +137,7 @@ def run(f, name, method, imgs, batch8, ntt_bytes=None, score_method="rows"):
         rec["dense4_B8_s"] = time.perf_counter() - t0
         for o in outs:
             o.Dispose()
+        rec["dense4_B8_families_ms"], rec["dense4_B8_mac_GBps"] = profile(eng, lambda: layers[D].ApplyBatch([x4] * 8))
     scores = np.asarray(m.Decrypt()).reshape(-1)
     net.DisposeNetwork()
     return rec, scores
