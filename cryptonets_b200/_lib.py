@@ -128,6 +128,13 @@ _SIGS = {
     "cnhe_raw_event_timing": [C.c_void_p, i32],
     "cnhe_raw_elapsed_ms": [C.c_void_p, C.POINTER(C.c_float)],
     "cnhe_kernel_launch_count": [C.c_void_p],
+    "cnhe_capture_begin": [C.c_void_p],
+    "cnhe_capture_end": [C.c_void_p, C.POINTER(C.c_void_p)],
+    "cnhe_capture_abort": [C.c_void_p],
+    "cnhe_graph_launch": [C.c_void_p],
+    "cnhe_graph_info": [C.c_void_p, U64P, U64P],
+    "cnhe_graph_destroy": [C.c_void_p],
+    "cnhe_vecs_assign": [C.c_void_p, C.POINTER(VECP), C.POINTER(VECP), i32],
     "cnhe_last_error": [],
     "cnhe_version": [],
 }

@@ -77,6 +77,16 @@ constexpr size_t RECYCLE_MIN_WORDS = (size_t)1 << 19;        // 4 MB
 constexpr size_t RECYCLE_CAP_WORDS = (size_t)16 << 27;       // 16 GiB parked at most (a fifth of an 80 GB H100)
 DevBuf::DevBuf(size_t w, cudaStream_t s, Context *ctx) : words(w), stream(s), owner(ctx) {
     if (!w) return;
+    if (ctx && ctx->rec) { // recording: the graph's own memory
+        arena = ctx->rec->arena;
+        size_t got = 0;
+        p = arena->take(w, s, got);
+        if (p) words = got;
+        else if (!(p = static_cast<u64 *>(arena->fresh(w * sizeof(u64)))))
+            ctx->refuse("needs more device memory than a graph can own (recorded blocks are reused only by later allocations of a "
+                        "similar size on the same stream)");
+        return;
+    }
     if (ctx && w >= RECYCLE_MIN_WORDS) {
         size_t got = 0;
         p = ctx->take_recycled(w, s, got);
@@ -166,9 +176,92 @@ void Context::release_upload(int slot, cudaStream_t s) {
 }
 DevBuf::~DevBuf() {
     if (!p) return;
+    if (arena) { arena->give(p, words, stream); return; }
+    if (owner && owner->rec) { // a stream-ordered free now would be recorded into the graph: release it once the recording ends
+        owner->rec->deferred.push_back({p, words, stream, upload_slot});
+        return;
+    }
     if (upload_slot >= 0) { owner->release_upload(upload_slot, stream); return; }
     if (owner && owner->give_recycled(p, words, stream)) return;
     cudaFreeAsync(p, stream);
+}
+
+u64 *GraphArena::take(size_t words, cudaStream_t s, size_t &got_words) { // the recycle list's fit rule
+    int best = -1;
+    for (int i = 0; i < (int)free.size(); i++) {
+        const Free &f = free[i];
+        if (f.stream != s || f.words < words || f.words > words + words / 2) continue;
+        if (best < 0 || f.words < free[best].words) best = i;
+    }
+    if (best < 0) return nullptr;
+    u64 *p = free[best].p;
+    got_words = free[best].words;
+    free.erase(free.begin() + best);
+    return p;
+}
+void *GraphArena::fresh(size_t n) {
+    void *p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, n); // not stream ordered: the block exists before the graph that uses it does
+    if (e == cudaErrorMemoryAllocation) { (void)cudaGetLastError(); return nullptr; }
+    CNHE_CUDA(e);
+    blocks.push_back(p);
+    bytes += n;
+    return p;
+}
+const void *GraphArena::constant(const void *src, size_t n, cudaStream_t s) {
+    const size_t need = (n + 255) & ~(size_t)255;
+    if (const_off + need > const_cap) { // constants are small (pointer tables, masks, scalars): packed into 1 MB blocks
+        const_cap = std::max<size_t>(need, (size_t)1 << 20);
+        const_block = static_cast<unsigned char *>(fresh(const_cap));
+        const_off = 0;
+        if (!const_block) { const_cap = 0; throw Error(-3 /* CNHE_ERR_STATE */, "no device memory left for a graph's constants"); }
+    }
+    unsigned char *d = const_block + const_off;
+    const_off += need;
+    CNHE_CUDA(cudaMemcpyAsync(d, src, n, cudaMemcpyHostToDevice, s));
+    CNHE_CUDA(cudaStreamSynchronize(s));
+    return d;
+}
+GraphArena::~GraphArena() {
+    for (void *p : blocks) cudaFree(p);
+}
+void release_deferred(Context &c, const std::vector<Recording::Deferred> &d) {
+    for (const Recording::Deferred &x : d) {
+        DevBuf b(0, x.stream, &c);
+        b.p = x.p;
+        b.words = x.words;
+        b.upload_slot = x.upload_slot;
+    }
+}
+cudaGraph_t end_recording(Context &c, bool keep, std::vector<Recording::Deferred> *hold) {
+    std::unique_ptr<Recording> r = std::move(c.rec);
+    // every channel stream joins the capturing stream 0 again (a capture cannot end with a stream left out); errors here only mean the
+    // capture was already invalidated, which cudaStreamEndCapture reports
+    for (size_t i = 1; i < c.streams.size(); i++) {
+        cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+        if (cudaStreamIsCapturing(c.streams[i], &st) == cudaSuccess && st == cudaStreamCaptureStatusActive &&
+            cudaEventRecord(c.ev_join, c.streams[i]) == cudaSuccess)
+            cudaStreamWaitEvent(c.streams[0], c.ev_join, 0);
+    }
+    cudaGraph_t g = nullptr;
+    if (cudaStreamEndCapture(c.streams[0], &g) != cudaSuccess) g = nullptr;
+    for (cudaStream_t s : c.streams) { // a stream of an invalidated capture may still be in it
+        cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+        if (cudaStreamIsCapturing(s, &st) == cudaSuccess && st != cudaStreamCaptureStatusNone) {
+            cudaGraph_t stray = nullptr;
+            if (cudaStreamEndCapture(s, &stray) == cudaSuccess && stray) cudaGraphDestroy(stray);
+        }
+    }
+    (void)cudaGetLastError();
+    if (g && !keep) { cudaGraphDestroy(g); g = nullptr; }
+    for (int i = 0; i < Context::OP_COUNT; i++) c.op_count[i] = r->op0[i]; // recording runs nothing
+    c.launches = r->launches0;
+    r->arena->recording = false;
+    r->arena->free.clear();
+    ws_release_all(c); // the last recorded call's temporaries go back to the graph's memory, not to the driver
+    if (hold && g) *hold = std::move(r->deferred);
+    else release_deferred(c, r->deferred);
+    return g;
 }
 
 static std::vector<BufRef> &temps_of(Context &c) { return c.temps; } // per context, guarded by the context mutex
@@ -180,6 +273,7 @@ u64 *Context::ws_alloc(size_t words) {
     return b->p;
 }
 void Context::sync() {
+    if (rec) refuse("waits for the device");
     for (cudaStream_t s : streams) CNHE_CUDA(cudaStreamSynchronize(s));
 }
 void Context::join_streams() {
@@ -193,8 +287,17 @@ void Context::fork_streams() {
     CNHE_CUDA(cudaEventRecord(ev_join, streams[0]));
     for (size_t i = 1; i < streams.size(); i++) CNHE_CUDA(cudaStreamWaitEvent(streams[i], ev_join, 0));
 }
+void Context::refuse(const char *why) const {
+    throw Error(-3 /* CNHE_ERR_STATE */, std::string(api) + " " + why + ": refused while the context records a graph");
+}
+void Context::upload(void *dst, const void *src, size_t bytes) {
+    if (!bytes) return;
+    if (rec) CNHE_CUDA(cudaMemcpyAsync(dst, rec->arena->constant(src, bytes, copy_stream), bytes, cudaMemcpyDeviceToDevice, stream));
+    else CNHE_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream));
+}
 void Context::h2d(void *dst, const void *src, size_t bytes) {
     if (!bytes) return;
+    if (rec) { upload(dst, src, bytes); return; } // the staging ring is overwritten by later calls: constants of a graph live in its memory
     if (!stage_buf) {
         stage_size = 64u << 20;
         CNHE_CUDA(cudaHostAlloc((void **)&stage_buf, stage_size, cudaHostAllocDefault));
@@ -261,6 +364,7 @@ struct ProfScope {
 #define PROF(family, bytes) ProfScope prof_scope_##__LINE__(c, family, bytes)
 Context::~Context() {
     cudaSetDevice(device);
+    if (rec) end_recording(*this, false);
     for (cudaStream_t s : streams) cudaStreamSynchronize(s);
     if (copy_stream) cudaStreamSynchronize(copy_stream);
     recycle_on = false; // buffers released from here on go straight back to the driver
@@ -864,6 +968,10 @@ static bool spans_overlap(const u64 *a, size_t a_words, const u64 *b, size_t b_w
 // target + i * target_stride, its base (2 polynomials) at base + i * base_stride; out is packed [n][2][k][N]
 const KeySet &Context::keys(int channel, int s) const {
     if (!slot_live(s)) throw Error(-1, "no such key slot");
+    if (rec) {
+        const auto g = key_gen.find(s);
+        rec->slots[s] = g == key_gen.end() ? 0 : g->second;
+    }
     return s == 0 ? ch[channel] : clients[s - 1][channel];
 }
 KsKeys KsKeys::slice(int c0, int m) const {
@@ -1422,6 +1530,7 @@ void op_decode(Context &c, int ch, const u64 *plain, int n, u64 *values) {
     c.check(launch_decode_gather(tmp, values, n, c.d_index_map, c.logN, c.stream), "decode_gather");
 }
 u64 take_nonces(Context &c, int chi, u64 n) {
+    if (c.rec) c.refuse("samples encryption randomness (a replay would reuse it for every input)");
     Channel &ch = c.ch[chi];
     if (n >= (1ULL << 31)) throw Error(-1, "too many encryptions in one call");
     if (ch.nonce + n >= (1ULL << 32)) { // the stream id carries 32 bits of the counter

@@ -10,6 +10,7 @@
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "kernels.h"
@@ -23,6 +24,27 @@ struct Error : std::runtime_error {
 void cuda_check(cudaError_t e, const char *what);
 #define CNHE_CUDA(x) ::cnhe::cuda_check((x), #x)
 
+// Device memory of one recorded graph (cnhe_capture_begin .. cnhe_capture_end): every allocation made while recording comes from here, never
+// from the stream-ordered pool or the context's recycle list, so no eager call can be handed a block a replay writes.  A block released
+// while recording goes to a per-stream free list that later recorded allocations on the same stream take from (stream order inside the
+// graph makes that safe, as it does for the recycle list); once the recording ends nothing is reused.  Host-built constants get blocks of
+// their own that are never released.  The memory goes back to the driver when the graph and every buffer cut from it are gone.
+struct GraphArena {
+    std::vector<void *> blocks;
+    size_t bytes = 0;
+    bool recording = true;
+    struct Free { u64 *p; size_t words; cudaStream_t stream; };
+    std::vector<Free> free;
+    unsigned char *const_block = nullptr;
+    size_t const_off = 0, const_cap = 0;
+    u64 *take(size_t words, cudaStream_t s, size_t &got_words);
+    void give(u64 *p, size_t words, cudaStream_t s) { if (recording) free.push_back({p, words, s}); }
+    void *fresh(size_t bytes); // nullptr when the device is out of memory
+    // a device copy of `bytes` host bytes, complete on return (copied on `s`, a stream outside the recording)
+    const void *constant(const void *src, size_t bytes, cudaStream_t s);
+    ~GraphArena();
+};
+
 // Reference-counted device allocation (stream-ordered pool).
 struct DevBuf {
     u64 *p = nullptr;
@@ -32,10 +54,25 @@ struct DevBuf {
     DevBuf(size_t w, cudaStream_t s);
     DevBuf(size_t w, cudaStream_t s, struct Context *owner);
     int upload_slot = -1; // >= 0: the block is one of the context's persistent upload slots (returned, not freed)
+    std::shared_ptr<GraphArena> arena; // set: allocated while recording a graph, from that graph's memory
     ~DevBuf();
     DevBuf(const DevBuf &) = delete;
 };
 typedef std::shared_ptr<DevBuf> BufRef;
+
+// State of a context while it records its calls into a CUDA graph (stream capture of the channel streams, vec.cu cnhe_capture_*)
+struct Recording {
+    std::thread::id thread;             // the recording thread: calls from any other thread are refused
+    std::shared_ptr<GraphArena> arena;
+    std::vector<uint64_t> op0;          // operation counters and kernel count when the recording began: restored when it ends, the
+    uint64_t launches0 = 0;             // difference is what every launch of the graph adds
+    std::map<int, uint64_t> slots;      // key slot -> its key generation, for every slot whose keys a recorded key switch reads
+    std::vector<std::shared_ptr<void>> keep; // cached host-built device tables (scalar-MAC plans) the recorded kernels read
+    // buffers allocated before the recording and released during it: the graph may read them, so they are freed (or recycled) outside
+    // it, when the graph is destroyed (at once when the recording is aborted)
+    struct Deferred { u64 *p; size_t words; cudaStream_t stream; int upload_slot; };
+    std::vector<Deferred> deferred;
+};
 
 // the evaluation keys of one client under one plaintext modulus
 struct KeySet {
@@ -80,7 +117,20 @@ struct Context {
     int slot = 0; // key slot of the ciphertexts the current public call works on (reset to 0 by every call; vec.cu sets it from the operands)
     bool foreign = false; // the current call touches ciphertexts of a slot other than 0: the noise trace cannot measure them (no secret key)
     bool slot_live(int s) const { return s == 0 || (s > 0 && (size_t)s <= clients.size() && !clients[s - 1].empty()); }
-    const KeySet &keys(int channel, int s) const;
+    const KeySet &keys(int channel, int s) const; // while recording, also notes the slot and its key generation
+    // key generation of a slot: bumped whenever its keys are replaced or removed, so that a graph recorded against them refuses to launch
+    std::map<int, uint64_t> key_gen;
+    void keys_changed(int s) { key_gen[s]++; }
+
+    // ---- graph recording (vec.cu, cnhe_capture_*).  `api`: the public call in progress, named in refusals
+    std::unique_ptr<Recording> rec;
+    const char *api = "";
+    [[noreturn]] void refuse(const char *why) const; // CNHE_ERR_STATE: the call cannot be recorded
+    // host -> device copy of `bytes` on `stream`.  While recording, the bytes are copied once into a constant block of the graph's memory
+    // and the graph copies them from there on every launch (a host buffer may be gone by then, and pageable copies cannot be recorded)
+    void upload(void *dst, const void *src, size_t bytes);
+    // waits until the host buffers handed to upload / h2d have been read; while recording they were read at once, so nothing waits
+    void host_fence() { if (!rec) sync(); }
     // one CUDA stream per plaintext-modulus channel (the reference runs one Task per prime, EncryptedSealBfvVector.cs:225-236):
     // channels are independent until decryption, so their kernels and host<->device copies overlap.  `stream` is the stream of the
     // channel currently being issued (set_channel).
@@ -181,8 +231,13 @@ struct Context {
     std::unordered_map<u64, std::shared_ptr<void>> umma_plans; // wgmma layer plans (vec.cu), keyed by a hash of the layer's weights and gather table
     double trace_ms = 0; // CNHE_TRACE_SLOW: report host-side gaps between consecutive launches longer than this
     void trace_gap(const char *what);
-    void sync();
+    void sync(); // waits for every channel stream; refused while recording
 };
+// ends the context's recording and returns the captured graph (nullptr when the capture failed; keep: false destroys it) and restores the
+// operation counters.  The buffers from before the recording that were released during it may still be read by the graph: they move to
+// *hold (the graph releases them when it is destroyed), or are released at once when hold is nullptr (an aborted recording)
+cudaGraph_t end_recording(Context &c, bool keep, std::vector<Recording::Deferred> *hold = nullptr);
+void release_deferred(Context &c, const std::vector<Recording::Deferred> &d); // as their DevBufs would have released them
 
 void ws_release_all(Context &c); // drop every workspace temporary (call at the start of a public operation)
 struct WsScope {                  // temporaries allocated inside the scope are released when it ends

@@ -24,6 +24,15 @@ int set_err(int code, const std::string &m) {
     return code;
 }
 extern "C" const char *cnhe_last_error(void) { return g_err.c_str(); }
+void api_enter(Context &c, const char *name) {
+    c.api = name;
+    if (c.rec && c.rec->thread != std::this_thread::get_id()) c.refuse("was called from another thread than the recording one");
+}
+int api_fail(Context &c, int code, const std::string &m) {
+    std::lock_guard<std::recursive_mutex> lock(c.mu);
+    if (c.rec) end_recording(c, false);
+    return set_err(code, m);
+}
 extern "C" const char *cnhe_version(void) { return "cnhe-b200 0.3 (sm_90a)"; }
 
 // ---------------------------------------------------------------------------------------------------- context & keys
@@ -86,6 +95,7 @@ extern "C" int cnhe_context_galois_elts(const cnhe_ctx *h, uint64_t *out) {
 }
 extern "C" int cnhe_context_set_option(cnhe_ctx *h, const char *name, int64_t value) {
     API_BEGIN(h)
+    not_recorded(c, "changes the context's options");
     std::string n(name ? name : "");
     if (n == "behz_centered_mtilde") {
         c.h_bc.centered_mtilde = value ? 1 : 0;
@@ -147,13 +157,119 @@ extern "C" int cnhe_context_sync(cnhe_ctx *h) {
     API_END
 }
 extern "C" uint64_t cnhe_kernel_launch_count(const cnhe_ctx *h) { return h ? h->c->launches : 0; }
+
+// ---------------------------------------------------------------------------------------------------- graph recording and replay
+// The context's calls are captured from its channel streams into one CUDA graph (stream capture, relaxed mode: the record-time copies of
+// host constants and the allocations of the graph's memory happen outside the captured streams).  Channel streams fork from stream 0 when
+// the recording begins and join it before it ends, as fork_streams / join_streams order them for eager calls.
+struct cnhe_graph {
+    cnhe_ctx *h = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    std::shared_ptr<GraphArena> arena;
+    std::vector<uint64_t> ops; // operation counts one launch adds
+    uint64_t launches = 0;     // kernel launches one launch adds (what the recorded calls counted)
+    uint64_t kernel_nodes = 0;
+    std::map<int, uint64_t> slots;
+    std::vector<std::shared_ptr<void>> keep;
+    std::vector<Recording::Deferred> held; // buffers from before the recording, released during it: the graph may read them
+};
+extern "C" int cnhe_capture_begin(cnhe_ctx *h) {
+    API_BEGIN(h)
+    if (c.rec) c.refuse("cannot start a second recording");
+    if (c.prof) fail("cnhe_capture_begin: profiling is on (cnhe_prof_enable)");
+    if (c.trace_noise) fail("cnhe_capture_begin: the noise trace is on (option trace_noise)");
+    auto r = std::make_unique<Recording>();
+    r->thread = std::this_thread::get_id();
+    r->arena = std::make_shared<GraphArena>();
+    r->op0.assign(c.op_count, c.op_count + Context::OP_COUNT);
+    r->launches0 = c.launches;
+    CNHE_CUDA(cudaStreamBeginCapture(c.streams[0], cudaStreamCaptureModeRelaxed));
+    c.rec = std::move(r);
+    c.fork_streams(); // the channel streams join the capture
+    API_END
+}
+extern "C" int cnhe_capture_abort(cnhe_ctx *h) {
+    API_BEGIN(h)
+    if (c.rec) end_recording(c, false);
+    API_END
+}
+extern "C" int cnhe_capture_end(cnhe_ctx *h, cnhe_graph **out) {
+    API_BEGIN(h)
+    if (!c.rec) throw Error(CNHE_ERR_STATE, "cnhe_capture_end: the context is not recording (was the recording aborted by a refused call?)");
+    if (!out) fail("null argument");
+    std::unique_ptr<cnhe_graph> g(new cnhe_graph);
+    g->h = h;
+    g->arena = c.rec->arena;
+    g->slots = c.rec->slots;
+    g->keep = c.rec->keep;
+    for (int i = 0; i < Context::OP_COUNT; i++) g->ops.push_back(c.op_count[i] - c.rec->op0[i]);
+    g->launches = c.launches - c.rec->launches0;
+    cudaGraph_t graph = end_recording(c, true, &g->held);
+    if (!graph) throw Error(CNHE_ERR_CUDA, "cnhe_capture_end: the CUDA stream capture failed");
+    size_t n = 0;
+    cudaError_t e = cudaGraphGetNodes(graph, nullptr, &n);
+    std::vector<cudaGraphNode_t> nodes(n);
+    if (e == cudaSuccess && n) e = cudaGraphGetNodes(graph, nodes.data(), &n);
+    for (size_t i = 0; i < n && e == cudaSuccess; i++) {
+        cudaGraphNodeType t;
+        e = cudaGraphNodeGetType(nodes[i], &t);
+        g->kernel_nodes += e == cudaSuccess && t == cudaGraphNodeTypeKernel;
+    }
+    if (e == cudaSuccess) e = cudaGraphInstantiate(&g->exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (e != cudaSuccess) release_deferred(c, g->held);
+    CNHE_CUDA(e);
+    *out = g.release();
+    API_END
+}
+extern "C" int cnhe_graph_launch(cnhe_graph *g) {
+    if (!g) return set_err(CNHE_ERR_INVALID, "null graph");
+    API_BEGIN(g->h)
+    not_recorded(c, "launches a recorded graph");
+    for (const auto &s : g->slots) {
+        const auto it = c.key_gen.find(s.first);
+        if (!c.slot_live(s.first) || (it == c.key_gen.end() ? 0 : it->second) != s.second)
+            throw Error(CNHE_ERR_STATE, "cnhe_graph_launch: the keys of key slot " + std::to_string(s.first) +
+                                            " were removed or replaced after the graph was recorded");
+    }
+    c.join_streams(); // after every call queued before, on any channel
+    CNHE_CUDA(cudaGraphLaunch(g->exec, c.streams[0]));
+    c.fork_streams(); // before every call queued after
+    for (int i = 0; i < Context::OP_COUNT; i++) c.op_count[i] += g->ops[i];
+    c.launches += g->launches;
+    API_END
+}
+extern "C" int cnhe_graph_info(const cnhe_graph *g, uint64_t *kernel_nodes, uint64_t *device_bytes) {
+    if (!g) return set_err(CNHE_ERR_INVALID, "null graph");
+    if (kernel_nodes) *kernel_nodes = g->kernel_nodes;
+    if (device_bytes) *device_bytes = g->arena->bytes;
+    return CNHE_OK;
+}
+extern "C" int cnhe_graph_destroy(cnhe_graph *g) {
+    if (!g) return CNHE_OK;
+    Context &c = *g->h->c;
+    try {
+        std::lock_guard<std::recursive_mutex> lock(c.mu);
+        if (c.rec) return set_err(CNHE_ERR_STATE, "cnhe_graph_destroy: refused while the context records a graph");
+        CNHE_CUDA(cudaSetDevice(c.device));
+        c.sync(); // no launch still runs in the memory about to be freed
+        CNHE_CUDA(cudaGraphExecDestroy(g->exec));
+        release_deferred(c, g->held);
+        delete g;
+    } catch (const Error &e) { return set_err(e.code, e.what()); }
+    return CNHE_OK;
+}
 extern "C" int cnhe_keys_generate(cnhe_ctx *h, uint64_t seed) {
     API_BEGIN(h)
+    not_recorded(c, "replaces keys");
+    c.keys_changed(0);
     keys_generate(c, seed);
     API_END
 }
 extern "C" int cnhe_keys_generate_secure(cnhe_ctx *h) {
     API_BEGIN(h)
+    not_recorded(c, "replaces keys");
+    c.keys_changed(0);
     keys_generate_secure(c);
     API_END
 }
@@ -161,6 +277,7 @@ extern "C" int cnhe_keys_generate_secure(cnhe_ctx *h) {
 extern "C" int cnhe_op_counts(cnhe_ctx *h, uint64_t *out, int cap, int reset) {
     API_BEGIN(h)
     if (!out || cap < Context::OP_COUNT) fail("need room for CNHE_OP_COUNT counters");
+    if (reset) not_recorded(c, "resets the operation counters");
     for (int i = 0; i < Context::OP_COUNT; i++) out[i] = c.op_count[i];
     if (reset) for (int i = 0; i < Context::OP_COUNT; i++) c.op_count[i] = 0;
     API_END
@@ -168,6 +285,7 @@ extern "C" int cnhe_op_counts(cnhe_ctx *h, uint64_t *out, int cap, int reset) {
 extern "C" const char *cnhe_op_name(int kind) { return op_kind_name(kind); }
 extern "C" int cnhe_trace_read(cnhe_ctx *h, int32_t *out, size_t cap_records, size_t *n_records, int clear) {
     API_BEGIN(h)
+    not_recorded(c, "reads the noise trace");
     if (n_records) *n_records = c.trace.size();
     if (out) {
         const size_t n = std::min(cap_records, c.trace.size());
@@ -179,6 +297,7 @@ extern "C" int cnhe_trace_read(cnhe_ctx *h, int32_t *out, size_t cap_records, si
 }
 extern "C" int cnhe_keys_set_seed(cnhe_ctx *h, int channel, uint64_t seed) {
     API_BEGIN(h)
+    not_recorded(c, "changes a channel's sampler");
     if (channel < 0 || channel >= c.P) fail("bad channel");
     memset(&c.ch[channel].rng, 0, sizeof(RngKey)); // deterministic sampler (tests): see cnhe.h
     c.ch[channel].rng.seed = seed;
@@ -186,6 +305,7 @@ extern "C" int cnhe_keys_set_seed(cnhe_ctx *h, int channel, uint64_t seed) {
 }
 extern "C" int cnhe_keys_export(cnhe_ctx *h, int channel, int what, uint64_t arg, uint64_t *dst, size_t cap) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     size_t words;
     BufRef &b = key_slot(c, channel, what, arg, words, false);
     if (cap < words) fail("destination too small");
@@ -195,6 +315,8 @@ extern "C" int cnhe_keys_export(cnhe_ctx *h, int channel, int what, uint64_t arg
 }
 extern "C" int cnhe_keys_import(cnhe_ctx *h, int channel, int what, uint64_t arg, const uint64_t *src, size_t nwords) {
     API_BEGIN(h)
+    not_recorded(c, "replaces keys");
+    c.keys_changed(0);
     size_t words;
     BufRef &b = key_slot(c, channel, what, arg, words, true);
     if (nwords != words) fail("wrong key size");
@@ -223,12 +345,14 @@ extern "C" int cnhe_dev_free(cnhe_ctx *h, uint64_t dptr) {
 }
 extern "C" int cnhe_dev_upload(cnhe_ctx *h, uint64_t dptr, const uint64_t *src, size_t words) {
     API_BEGIN(h)
+    not_recorded(c, "uploads host words");
     CNHE_CUDA(cudaMemcpyAsync((void *)dptr, src, words * 8, cudaMemcpyHostToDevice, c.stream));
     c.sync();
     API_END
 }
 extern "C" int cnhe_dev_download(cnhe_ctx *h, uint64_t *dst, uint64_t dptr, size_t words) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     CNHE_CUDA(cudaMemcpyAsync(dst, (void *)dptr, words * 8, cudaMemcpyDeviceToHost, c.stream));
     c.sync();
     API_END
@@ -304,6 +428,7 @@ extern "C" int cnhe_dev_copy(cnhe_ctx *h, uint64_t dst, uint64_t src, size_t wor
 }
 extern "C" int cnhe_prof_enable(cnhe_ctx *h, int on) {
     API_BEGIN(h)
+    not_recorded(c, "profiles");
     c.prof_flush();
     c.prof = on != 0;
     if (on) for (int i = 0; i < 6; i++) { c.prof_ms[i] = 0; c.prof_bytes[i] = 0; c.prof_n[i] = 0; }
@@ -311,6 +436,7 @@ extern "C" int cnhe_prof_enable(cnhe_ctx *h, int on) {
 }
 extern "C" int cnhe_prof_collect(cnhe_ctx *h, int family, double *total_ms, uint64_t *launches, double *bytes) {
     API_BEGIN(h)
+    not_recorded(c, "profiles");
     if (family < 0 || family > 5) fail("bad family");
     c.prof_flush();
     if (total_ms) *total_ms = c.prof_ms[family];
@@ -320,6 +446,7 @@ extern "C" int cnhe_prof_collect(cnhe_ctx *h, int family, double *total_ms, uint
 }
 extern "C" int cnhe_raw_event_timing(cnhe_ctx *h, int start) {
     API_BEGIN(h)
+    not_recorded(c, "profiles");
     if (start) {
         c.join_streams();
         CNHE_CUDA(cudaEventRecord(c.ev0, c.streams[0]));
@@ -332,6 +459,7 @@ extern "C" int cnhe_raw_event_timing(cnhe_ctx *h, int start) {
 }
 extern "C" int cnhe_raw_elapsed_ms(cnhe_ctx *h, float *ms) {
     API_BEGIN(h)
+    not_recorded(c, "profiles");
     CNHE_CUDA(cudaEventSynchronize(c.ev1));
     CNHE_CUDA(cudaEventElapsedTime(ms, c.ev0, c.ev1));
     API_END
@@ -388,6 +516,8 @@ cnhe_vec::~cnhe_vec() {
 void materialise(Context &c, const cnhe_vec *v) {
     if (!v || !v->pend) return;
     const std::shared_ptr<PendingGroup> g = v->pend;
+    // a group made before the recording would be re-pointed at graph memory that holds no words until a launch: read it first
+    if (c.rec && g->slab3[0]->arena != c.rec->arena) c.refuse("relinearises squares made before the recording (read them once first)");
     const cudaStream_t s0 = c.stream;
     const size_t ctw = c.ct_words();
     std::vector<BufRef> slab2(c.P);
@@ -497,9 +627,9 @@ static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64
         for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
             out->buf[ch] = c.alloc(dim);
-            CNHE_CUDA(cudaMemcpyAsync(out->buf[ch]->p, split[ch].data(), dim * 8, cudaMemcpyHostToDevice, c.stream));
+            c.upload(out->buf[ch]->p, split[ch].data(), dim * 8);
         }
-        c.sync();
+        c.host_fence();
         return guard.release();
     }
     alloc_channels(out);
@@ -510,7 +640,7 @@ static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64
             std::vector<u64> padded((size_t)blocks * N, 0);
             memcpy(padded.data(), split[ch].data(), dim * 8);
             u64 *dvals = c.ws_alloc((size_t)blocks * N);
-            CNHE_CUDA(cudaMemcpyAsync(dvals, padded.data(), padded.size() * 8, cudaMemcpyHostToDevice, c.stream));
+            c.upload(dvals, padded.data(), padded.size() * 8);
             u64 *plain = encrypt ? c.ws_alloc((size_t)blocks * N) : out->ptr(ch);
             op_encode(c, ch, dvals, blocks, (int)N, plain);
             if (encrypt) {
@@ -518,10 +648,10 @@ static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64
             }
         } else { // sparse encrypted: one constant-polynomial plaintext per element (AtomicSealBfvVector.cs:1135-1138)
             u64 *dvals = c.ws_alloc(dim);
-            CNHE_CUDA(cudaMemcpyAsync(dvals, split[ch].data(), dim * 8, cudaMemcpyHostToDevice, c.stream));
+            c.upload(dvals, split[ch].data(), dim * 8);
             op_encrypt(c, ch, dvals, 1, blocks, 1, take_nonces(c, ch, blocks), out->ptr(ch));
         }
-        c.sync(); // host staging buffers go out of scope
+        c.host_fence(); // host staging buffers go out of scope
     }
     if (v && !encrypt && format == CNHE_DENSE && dim % N == 0) { // every slot equal => every plaintext is the constant polynomial
         bool all_eq = true;
@@ -536,6 +666,7 @@ static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64
 
 extern "C" int cnhe_vec_encrypt(cnhe_ctx *h, const double *v, uint64_t dim, double scale, int format, cnhe_vec **out) {
     API_BEGIN(h)
+    not_recorded(c, "samples encryption randomness (a replay would reuse it for every input)");
     *out = make_vector(c, v, dim, scale, format, true);
     API_END
 }
@@ -545,6 +676,7 @@ extern "C" int cnhe_vec_from_residues(cnhe_ctx *h, const uint64_t *residues, uin
     API_BEGIN(h)
     if (!residues || !out || dim < 1) fail("bad arguments");
     if (format != CNHE_DENSE && format != CNHE_SPARSE) fail("bad format");
+    if (encrypt) not_recorded(c, "samples encryption randomness (a replay would reuse it for every input)");
     std::vector<std::vector<u64>> split(c.P, std::vector<u64>(dim));
     for (int ch = 0; ch < c.P; ch++)
         for (uint64_t j = 0; j < dim; j++) {
@@ -562,6 +694,7 @@ extern "C" int cnhe_vec_plain(cnhe_ctx *h, const double *v, uint64_t dim, double
 // n dense single-block-or-more vectors encrypted in one wave per channel (GetEncryptedMatrix, IFactory.cs:353-380)
 extern "C" int cnhe_vecs_encrypt(cnhe_ctx *h, const double *v, int n, uint64_t dim, double scale, cnhe_vec **out) {
     API_BEGIN(h)
+    not_recorded(c, "samples encryption randomness (a replay would reuse it for every input)");
     if (n < 1 || !v || !out) fail("bad arguments");
     if (scale == 0) scale = 1;
     const size_t N = c.N;
@@ -613,6 +746,7 @@ static void decrypt_channel(Context &c, const cnhe_vec *v, int ch, std::vector<u
 }
 extern "C" int cnhe_vec_decrypt(cnhe_ctx *h, const cnhe_vec *v, double *out, uint64_t cap) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     same_ctx(c, v);
     if (cap < v->dim) fail("destination too small");
     std::vector<std::vector<u64>> split(c.P);
@@ -627,6 +761,7 @@ extern "C" int cnhe_vec_decrypt(cnhe_ctx *h, const cnhe_vec *v, double *out, uin
 // (JoinSplitNumbers, ":397-411"); out is [P][dim]
 extern "C" int cnhe_vec_decrypt_residues(cnhe_ctx *h, const cnhe_vec *v, uint64_t *out, uint64_t cap) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     same_ctx(c, v);
     if (!out || cap < v->dim * (uint64_t)c.P) fail("destination too small");
     for (int ch = 0; ch < c.P; ch++) {
@@ -639,6 +774,7 @@ extern "C" int cnhe_vec_decrypt_residues(cnhe_ctx *h, const cnhe_vec *v, uint64_
 }
 extern "C" int cnhe_vecs_decrypt(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, double *out, uint64_t dim) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     for (int i = 0; i < n; i++) {
         same_ctx(c, vecs[i]);
         if (vecs[i]->dim != dim) fail("all vectors must have the same dimension");
@@ -648,6 +784,61 @@ extern "C" int cnhe_vecs_decrypt(cnhe_ctx *h, const cnhe_vec *const *vecs, int n
             decrypt_channel(c, vecs[i], ch, split[ch]);
         }
         join_values(c, split, dim, vecs[i]->scale, out + (size_t)i * dim);
+    }
+    API_END
+}
+// New words for existing encrypted vectors (a graph's recorded inputs): dst[i] takes src[i]'s ciphertexts, device to device on each
+// channel's stream.  Host-side attributes a recording may have acted on (dimension, blocks, format, scale, key slot) must match.
+extern "C" int cnhe_vecs_assign(cnhe_ctx *h, cnhe_vec *const *dst, const cnhe_vec *const *src, int n) {
+    API_BEGIN(h)
+    if (!dst || !src || n < 1) fail("bad arguments");
+    for (int i = 0; i < n; i++) {
+        if (!dst[i] || !src[i]) fail("null vector");
+        if (dst[i]->ctx != &c || src[i]->ctx != &c) fail("vector belongs to another context");
+    }
+    vec_slots(c, src, n); // the sources' key slots are live; pending sources are relinearised
+    vec_slots(c, dst, n, true);
+    for (int i = 0; i < n; i++) {
+        const cnhe_vec *d = dst[i], *s = src[i];
+        if (!d->enc || !s->enc) fail("cnhe_vecs_assign copies encrypted vectors only");
+        if (d->pend) fail("the destination's squares are not relinearised (it was made by a square layer and never read)");
+        if (d->dim != s->dim || d->blocks != s->blocks || d->format != s->format) fail("source and destination differ in shape");
+        if (d->scale != s->scale) fail("source and destination differ in scale");
+        if (d->slot != s->slot) fail("source and destination belong to different key slots");
+    }
+    // a destination may be its own source (nothing to copy) but may not overlap any other source: the copies (coalesced below) would
+    // read words they, or an earlier copy, overwrite
+    const size_t ctw = c.ct_words();
+    for (int ch = 0; ch < c.P; ch++) {
+        std::vector<std::pair<const u64 *, int>> by_start(n);
+        for (int i = 0; i < n; i++) by_start[i] = {src[i]->ptr(ch), i};
+        std::sort(by_start.begin(), by_start.end());
+        std::vector<const u64 *> reach(n); // reach[k]: the furthest end of the sources sorted up to k
+        for (int k = 0; k < n; k++) {
+            const u64 *e = by_start[k].first + src[by_start[k].second]->blocks * ctw;
+            reach[k] = k && reach[k - 1] > e ? reach[k - 1] : e;
+        }
+        for (int i = 0; i < n; i++) {
+            const u64 *a = dst[i]->ptr(ch), *a_end = a + dst[i]->blocks * ctw;
+            for (int k = (int)(std::lower_bound(by_start.begin(), by_start.end(), std::make_pair(a_end, -1)) - by_start.begin()) - 1;
+                 k >= 0 && reach[k] > a; k--) {
+                const int j = by_start[k].second;
+                if (by_start[k].first + src[j]->blocks * ctw > a && !(j == i && by_start[k].first == a))
+                    fail("a destination overlaps a source other than its own");
+            }
+        }
+    }
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        for (int i = 0, j; i < n; i = j) { // one copy per run of vectors that lie back to back in one slab on both sides
+            size_t words = dst[i]->blocks * ctw;
+            for (j = i + 1; j < n && dst[j]->buf[ch] == dst[i]->buf[ch] && src[j]->buf[ch] == src[i]->buf[ch] &&
+                            dst[j]->ptr(ch) == dst[i]->ptr(ch) + words && src[j]->ptr(ch) == src[i]->ptr(ch) + words;
+                 j++)
+                words += dst[j]->blocks * ctw;
+            if (dst[i]->ptr(ch) != src[i]->ptr(ch))
+                CNHE_CUDA(cudaMemcpyAsync(dst[i]->ptr(ch), src[i]->ptr(ch), words * 8, cudaMemcpyDeviceToDevice, c.stream));
+        }
     }
     API_END
 }
@@ -713,6 +904,7 @@ extern "C" int cnhe_vec_register_dim(cnhe_vec *v, uint64_t dim) {
 }
 extern "C" int cnhe_vec_export_raw(cnhe_ctx *h, const cnhe_vec *v, int channel, int block, uint64_t *dst, size_t cap) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     same_ctx(c, v);
     if (!v->enc) fail("vector is not encrypted");
     if (channel < 0 || channel >= c.P || block < 0 || block >= v->blocks) fail("bad channel/block");
@@ -723,6 +915,7 @@ extern "C" int cnhe_vec_export_raw(cnhe_ctx *h, const cnhe_vec *v, int channel, 
 }
 extern "C" int cnhe_vec_import_raw(cnhe_ctx *h, const uint64_t *src, int blocks, uint64_t dim, double scale, int format, cnhe_vec **out) {
     API_BEGIN(h)
+    not_recorded(c, "uploads host words");
     if (!src || blocks < 1) fail("bad arguments");
     cnhe_vec *o = new_vec(c, dim, scale, format, true, blocks);
     alloc_channels(o);
@@ -737,6 +930,7 @@ extern "C" int cnhe_vec_import_raw(cnhe_ctx *h, const uint64_t *src, int blocks,
 }
 extern "C" int cnhe_vecs_import_raw(cnhe_ctx *h, const uint64_t *src, int n, int blocks, uint64_t dim, double scale, int format, cnhe_vec **out) {
     API_BEGIN(h)
+    not_recorded(c, "uploads host words");
     if (!src || n < 1 || blocks < 1 || !out) fail("bad arguments");
     const size_t per = (size_t)blocks * c.ct_words(), words = (size_t)n * per;
     std::vector<BufRef> big(c.P);
@@ -796,6 +990,7 @@ static CompactHeader parse_compact(const Context &c, const uint8_t *src, size_t 
 }
 extern "C" int cnhe_vecs_encrypt_compact(cnhe_ctx *h, const double *v, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap, size_t *needed) {
     API_BEGIN(h)
+    not_recorded(c, "samples encryption randomness (a replay would reuse it for every input)");
     if (n < 1 || dim < 1 || !v || (!dst && !needed)) fail("bad arguments");
     if (scale == 0) scale = 1;
     const size_t N = c.N;
@@ -844,6 +1039,7 @@ extern "C" int cnhe_vecs_encrypt_compact(cnhe_ctx *h, const double *v, int n, ui
 // into a persistent upload slot on the same stream, and the channel's stream waits for it -- the call returns at once.
 extern "C" int cnhe_vecs_import_compact(cnhe_ctx *h, const uint8_t *src, size_t len, cnhe_vec **out, int cap, int *n) {
     API_BEGIN(h)
+    not_recorded(c, "uploads host words");
     if (!src || !out || !n) fail("bad arguments");
     const CompactHeader hd = parse_compact(c, src, len);
     *n = (int)hd.n;
@@ -883,6 +1079,7 @@ static std::vector<u64> select_galois(const Context &c, const uint64_t *elts, in
 }
 extern "C" int cnhe_keys_save_compact(cnhe_ctx *h, int sets, const uint64_t *galois_elts, int n_galois, uint8_t *dst, size_t cap, size_t *needed) {
     API_BEGIN(h)
+    not_recorded(c, "generates keys");
     if (!dst && !needed) fail("bad arguments");
     if (sets & ~3) fail("unknown key sets (bit 0 public key, bit 1 relinearization keys)");
     const std::vector<u64> elts = select_galois(c, galois_elts, n_galois);
@@ -1008,6 +1205,7 @@ extern "C" int cnhe_context_load_compact(const uint8_t *blob, size_t len, int de
 // ---------------------------------------------------------------------------------------------------- key slots (several clients)
 extern "C" int cnhe_context_add_client_compact(cnhe_ctx *h, const uint8_t *blob, size_t len, int *slot) {
     API_BEGIN(h)
+    not_recorded(c, "adds a client's keys");
     if (!blob || !slot) fail("null argument");
     const KeyBlob kb = parse_compact_keys(blob, len); // every header field and the exact length, before anything is allocated
     bool same = kb.N == c.N && (int)kb.k == c.k && (int)kb.P == c.P && (int)kb.dbc_relin == c.dbc_relin && (int)kb.dbc_galois == c.dbc_galois;
@@ -1033,9 +1231,11 @@ extern "C" int cnhe_context_add_client_compact(cnhe_ctx *h, const uint8_t *blob,
 }
 extern "C" int cnhe_context_remove_client(cnhe_ctx *h, int slot) {
     API_BEGIN(h)
+    not_recorded(c, "removes a client's keys");
     if (slot < 1 || !c.slot_live(slot)) fail("no such key slot");
     c.sync(); // no queued key switch still reads the keys
     c.clients[slot - 1].clear();
+    c.keys_changed(slot);
     API_END
 }
 extern "C" int cnhe_vec_set_key_slot(cnhe_vec *v, int slot) {
@@ -1078,6 +1278,7 @@ extern "C" int cnhe_vecs_rotate(cnhe_ctx *h, const cnhe_vec *const *vecs, int n,
 }
 extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     if (n < 1 || !dst) fail("bad arguments");
     const int blocks = vecs[0]->blocks;
     const size_t per = (size_t)blocks * c.ct_words();
@@ -1095,6 +1296,7 @@ extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, in
 }
 extern "C" int cnhe_vecs_export_raw_async(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap, int *ticket) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     if (n < 1 || !dst || !ticket) fail("bad arguments");
     const int blocks = vecs[0]->blocks;
     const size_t per = (size_t)blocks * c.ct_words();
@@ -1133,22 +1335,20 @@ extern "C" int cnhe_export_wait(cnhe_ctx *h, int ticket) {
 }
 extern "C" int cnhe_vec_device_ptr(const cnhe_vec *v, int channel, uint64_t *dptr, size_t *words) {
     if (!v || channel < 0 || channel >= v->ctx->P) return set_err(CNHE_ERR_INVALID, "bad arguments");
+    cnhe_ctx h{v->ctx};
+    API_BEGIN(&h)
+    not_recorded(c, "hands device words to the caller");
     if (v->pend) { // the caller reads the words: relinearise them first
-        cnhe_ctx h{v->ctx};
-        const int r = [&]() -> int {
-            API_BEGIN(&h)
-            materialise(c, v);
-            c.sync();
-            API_END
-        }();
-        if (r != CNHE_OK) return r;
+        materialise(c, v);
+        c.sync();
     }
     *dptr = (uint64_t)v->ptr(channel);
     if (words) *words = (size_t)v->blocks * v->unit();
-    return CNHE_OK;
+    API_END
 }
 extern "C" int cnhe_noise_budget(cnhe_ctx *h, const cnhe_vec *v, int channel, int block, int *bits) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     same_ctx(c, v);
     if (!v->enc || channel < 0 || channel >= c.P || block < 0 || block >= v->blocks) fail("bad arguments");
     if (v->slot != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
@@ -1245,10 +1445,10 @@ static cnhe_vec *mul_sparse_dim_one(Context &c, const cnhe_vec *self, const cnhe
             std::vector<u64> sc(self->blocks, s->scalars[ch][0]);
             if (sc[0] == 0) fail("plain cannot be zero (the result would be a transparent ciphertext)");
             u64 *d = c.ws_alloc(sc.size());
-            CNHE_CUDA(cudaMemcpyAsync(d, sc.data(), sc.size() * 8, cudaMemcpyHostToDevice, c.stream));
+            c.upload(d, sc.data(), sc.size() * 8);
             c.check(launch_ct_scale(self->ptr(ch), o->ptr(ch), self->blocks, 2, d, c.k, c.logN, c.d_bc, c.ch[ch].pc, c.stream), "ct_scale");
             c.note(Context::OP_MULTIPLY_SCALAR, ch, self->blocks, o->ptr(ch), self->ptr(ch), nullptr, log2_centred(sc[0], c.t[ch]));
-            c.sync();
+            c.host_fence();
         } else { // plain blocks times the single ciphertext of s
             if (self->format != CNHE_DENSE) fail("unsupported plain format");
             u64 *rep = c.ws_alloc((size_t)self->blocks * c.ct_words());
@@ -1344,10 +1544,10 @@ static cnhe_vec *sum_all_slots(Context &c, const cnhe_vec *a, uint64_t length, i
             std::vector<u64> onehot(N, 0);
             onehot[force_column] = 1;
             u64 *dv = c.ws_alloc(N), *pl = c.ws_alloc(N);
-            CNHE_CUDA(cudaMemcpyAsync(dv, onehot.data(), N * 8, cudaMemcpyHostToDevice, c.stream));
+            c.upload(dv, onehot.data(), N * 8);
             op_encode(c, ch, dv, 1, (int)N, pl);
             op_multiply_plain_dense(c, ch, sum, 1, pl, false, sum);
-            c.sync();
+            c.host_fence();
             len = 1;
         }
     }
@@ -1539,9 +1739,9 @@ static void interleave_finish(Context &c, int ch, const std::vector<const cnhe_v
         std::vector<u64> v(block_size, 0);
         for (int i = 0; i < count; i++) v[i] = 1;
         u64 *dv = c.ws_alloc(block_size), *pl = c.ws_alloc(block_size);
-        CNHE_CUDA(cudaMemcpyAsync(dv, v.data(), (size_t)block_size * 8, cudaMemcpyHostToDevice, c.stream));
+        c.upload(dv, v.data(), (size_t)block_size * 8);
         op_encode(c, ch, dv, 1, block_size, pl);
-        c.sync();
+        c.host_fence();
         return pl;
     };
     // split the vectors that straddle a half / block boundary with a one-hot-prefix mask (":640-672") and file every piece
@@ -1994,7 +2194,10 @@ static std::shared_ptr<UmmaPlan> umma_plan(Context &c, int ch, const std::vector
         mix(shape.data(), shape.size() / 2 * 8);
     }
     auto hit = c.umma_plans.find(key);
-    if (hit != c.umma_plans.end()) return std::static_pointer_cast<UmmaPlan>(hit->second);
+    if (hit != c.umma_plans.end()) {
+        if (c.rec) c.rec->keep.push_back(hit->second); // the cache may drop it; a graph that reads it keeps it
+        return std::static_pointer_cast<UmmaPlan>(hit->second);
+    }
     std::shared_ptr<UmmaPlan> best = umma_search(grows, row_outs, wdh, M, K, limbs);
     if (!best) best = std::make_shared<UmmaPlan>();
     else {
@@ -2002,12 +2205,17 @@ static std::shared_ptr<UmmaPlan> umma_plan(Context &c, int ch, const std::vector
         CNHE_CUDA(cudaMalloc((void **)&best->d_bundles, best->bundles.size() * sizeof(UmBundle)));
         CNHE_CUDA(cudaMalloc((void **)&best->d_rows, best->chunk_rows.size() * sizeof(int)));
         CNHE_CUDA(cudaMalloc((void **)&best->d_wpack, best->wpack.size()));
-        CNHE_CUDA(cudaMemcpy(best->d_bundles, best->bundles.data(), best->bundles.size() * sizeof(UmBundle), cudaMemcpyHostToDevice));
-        CNHE_CUDA(cudaMemcpy(best->d_rows, best->chunk_rows.data(), best->chunk_rows.size() * sizeof(int), cudaMemcpyHostToDevice));
-        CNHE_CUDA(cudaMemcpy(best->d_wpack, best->wpack.data(), best->wpack.size(), cudaMemcpyHostToDevice));
+        // complete on return, on the upload stream: a plan built while recording must not touch the captured streams
+        CNHE_CUDA(cudaMemcpyAsync(best->d_bundles, best->bundles.data(), best->bundles.size() * sizeof(UmBundle), cudaMemcpyHostToDevice,
+                                  c.copy_stream));
+        CNHE_CUDA(cudaMemcpyAsync(best->d_rows, best->chunk_rows.data(), best->chunk_rows.size() * sizeof(int), cudaMemcpyHostToDevice,
+                                  c.copy_stream));
+        CNHE_CUDA(cudaMemcpyAsync(best->d_wpack, best->wpack.data(), best->wpack.size(), cudaMemcpyHostToDevice, c.copy_stream));
+        CNHE_CUDA(cudaStreamSynchronize(c.copy_stream));
     }
     if (c.umma_plans.size() > 64) c.umma_plans.clear();
     c.umma_plans[key] = best;
+    if (c.rec) c.rec->keep.push_back(best);
     return best;
 }
 // A validated scalar-MAC layer: outputs that share a gather row in tiles of 8, and the key slot of every output.  The inputs are
@@ -2435,7 +2643,7 @@ extern "C" int cnhe_mat_mul_colmajor_sparse(cnhe_ctx *h, const cnhe_vec *const *
                 for (int kk = 0; kk < K; kk++) terms.push_back(prod + ((size_t)kk * bl + i) * ctw);
                 do_add_many(c, ch, terms, o->block(ch, i));
             }
-            c.sync();
+            c.host_fence();
         }
         *out = guard.release();
     }
@@ -2573,7 +2781,7 @@ static void mat_mul_rowmajor(Context &c, const cnhe_vec *const *rows, int n_rows
                     do_add_many(c, ch, terms, outs[b]->ptr(ch));
                     first[b] = 0;
                 }
-                c.sync();
+                c.host_fence();
             }
         }
     }
@@ -2799,6 +3007,7 @@ extern "C" int cnhe_layer_square(cnhe_ctx *h, const cnhe_vec *const *in, int n, 
 // are not canonical residues.
 extern "C" int cnhe_raw_import_products(cnhe_ctx *h, const uint64_t *words, int n, uint64_t dim, double scale, int slot, cnhe_vec **out) {
     API_BEGIN(h)
+    not_recorded(c, "uploads host words");
     if (!words || n < 1 || !out || dim < 1 || dim > c.N) fail("bad arguments");
     if (!c.slot_live(slot)) fail("no such key slot");
     const size_t s3 = (size_t)3 * c.k * c.N;
@@ -3172,6 +3381,7 @@ static void diag_prepare(Context &c, const cnhe_vec *const *rows, int n_rows, in
 
 extern "C" int cnhe_diag_prepare(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int baby_steps, cnhe_diag **out) {
     API_BEGIN(h)
+    not_recorded(c, "prepares a matrix (it reads device words back)");
     diag_prepare(c, rows, n_rows, baby_steps, 0, -1, out);
     API_END
 }
@@ -3179,6 +3389,7 @@ extern "C" int cnhe_diag_prepare(cnhe_ctx *h, const cnhe_vec *const *rows, int n
 extern "C" int cnhe_diag_prepare_ntt(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int baby_steps, uint64_t max_ntt_bytes,
                                      cnhe_diag **out) {
     API_BEGIN(h)
+    not_recorded(c, "prepares a matrix (it reads device words back)");
     diag_prepare(c, rows, n_rows, baby_steps, max_ntt_bytes, -1, out);
     API_END
 }
@@ -3186,6 +3397,7 @@ extern "C" int cnhe_diag_prepare_ntt(cnhe_ctx *h, const cnhe_vec *const *rows, i
 extern "C" int cnhe_diag_prepare_folded(cnhe_ctx *h, const cnhe_vec *const *rows, int n_rows, int fold_width, int baby_steps,
                                         uint64_t max_ntt_bytes, cnhe_diag **out) {
     API_BEGIN(h)
+    not_recorded(c, "prepares a matrix (it reads device words back)");
     if (fold_width < 0) fail("fold_width must be 0 or a power of two in [n_rows, N/2]");
     diag_prepare(c, rows, n_rows, baby_steps, max_ntt_bytes, fold_width, out);
     API_END
@@ -3218,6 +3430,7 @@ extern "C" int cnhe_diag_ntt_info(const cnhe_diag *d, int *resident_giant_steps,
 
 extern "C" int cnhe_diag_export(cnhe_ctx *h, const cnhe_diag *d, int channel, int index, uint64_t *dst, size_t cap_words, int *bgh) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     if (!d || d->ctx != &c) fail("matrix belongs to another context");
     if (channel < 0 || channel >= c.P || index < 0 || index >= (int)d->diags.size()) fail("index out of range");
     if (dst) {
@@ -3236,6 +3449,7 @@ extern "C" int cnhe_diag_export(cnhe_ctx *h, const cnhe_diag *d, int channel, in
 
 extern "C" int cnhe_diag_export_ntt(cnhe_ctx *h, const cnhe_diag *d, int channel, int index, uint64_t *dst, size_t cap_words) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     if (!d || d->ctx != &c) fail("matrix belongs to another context");
     if (channel < 0 || channel >= c.P || index < 0 || index >= d->ntt_diags) fail("index outside the resident diagonals");
     const size_t kN = (size_t)c.k * c.N;

@@ -55,12 +55,19 @@ struct cnhe_vec {
 };
 
 int set_err(int code, const std::string &m); // thread-local last error (vec.cu)
+// Graph recording (vec.cu).  api_enter: start of a public call on a context -- names the call for refusals and refuses calls from another
+// thread than the recording one.  api_fail: a call failed; a failure while recording aborts the recording (the context stays usable).
+// not_recorded: refuses the call while recording, saying why it cannot be part of a graph.
+void api_enter(Context &c, const char *name);
+int api_fail(Context &c, int code, const std::string &m);
+static inline void not_recorded(Context &c, const char *why) { if (c.rec) c.refuse(why); }
 
 #define API_BEGIN(CTX)                                                                                                 \
     if (!(CTX)) return set_err(CNHE_ERR_INVALID, "null context");                                                      \
     Context &c = *(CTX)->c;                                                                                            \
     try {                                                                                                              \
         std::lock_guard<std::recursive_mutex> lock(c.mu);                                                              \
+        api_enter(c, __func__);                                                                                        \
         CNHE_CUDA(cudaSetDevice(c.device));                                                                            \
         c.set_channel(0);                                                                                              \
         c.slot = 0;                                                                                                    \
@@ -68,8 +75,8 @@ int set_err(int code, const std::string &m); // thread-local last error (vec.cu)
         ws_release_all(c);
 #define API_END                                                                                                        \
     }                                                                                                                  \
-    catch (const Error &e) { return set_err(e.code, e.what()); }                                                      \
-    catch (const std::exception &e) { return set_err(CNHE_ERR_INVALID, e.what()); }                                   \
+    catch (const Error &e) { return api_fail(c, e.code, e.what()); }                                                  \
+    catch (const std::exception &e) { return api_fail(c, CNHE_ERR_INVALID, e.what()); }                               \
     return CNHE_OK;
 static inline void fail(const char *m) { throw Error(CNHE_ERR_INVALID, m); }
 cnhe_vec *new_vec(Context &c, uint64_t dim, double scale, int format, bool enc, int blocks); // bound to the call's key slot c.slot

@@ -321,6 +321,7 @@ const char *NL = "\r\n"; // StreamWriter.WriteLine on the reference's platform
 // ==================================================================================================== key archive
 extern "C" int cnhe_keys_save(cnhe_ctx *h, int with_private_keys, uint8_t *dst, size_t cap, size_t *needed) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     if (!needed) fail("null argument");
     const uint64_t N = c.N, k = (uint64_t)c.k, kN = k * N;
     std::vector<ZipEntry> entries;
@@ -497,6 +498,7 @@ extern "C" int cnhe_context_load(const uint8_t *archive, size_t len, int device,
 // ==================================================================================================== vector text
 extern "C" int cnhe_vec_write(cnhe_ctx *h, const cnhe_vec *v, char *dst, size_t cap, size_t *needed) {
     API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
     same_ctx(c, v);
     if (!needed) fail("null argument");
     const uint64_t N = c.N, k = (uint64_t)c.k;
@@ -547,6 +549,7 @@ extern "C" int cnhe_vec_write(cnhe_ctx *h, const cnhe_vec *v, char *dst, size_t 
 
 extern "C" int cnhe_vec_read(cnhe_ctx *h, const char *text, size_t len, cnhe_vec **out, size_t *consumed) {
     API_BEGIN(h)
+    not_recorded(c, "uploads host words");
     if (!text || !out) fail("null argument");
     const uint64_t N = c.N, k = (uint64_t)c.k;
     Lines L(text, len);

@@ -154,6 +154,39 @@ class Diag:
         return out
 
 
+class Graph:
+    """Owning handle of a cnhe_graph: a recorded chain of calls, replayed by launch() (include/cnhe.h, cnhe_capture_begin)."""
+
+    __slots__ = ("eng", "h", "__weakref__")
+
+    def __init__(self, eng, handle):
+        self.eng = eng
+        self.h = C.c_void_p(handle) if not isinstance(handle, C.c_void_p) else handle
+        eng._live.add(self)
+
+    def launch(self):
+        """Enqueue one replay (asynchronous, ordered with the engine's other calls)."""
+        check(self.eng.L.cnhe_graph_launch(self.h))
+
+    def info(self):
+        """dict(kernel_nodes, device_bytes): the graph's kernel nodes and the device memory it owns."""
+        kn, nb = C.c_uint64(), C.c_uint64()
+        check(self.eng.L.cnhe_graph_info(self.h, C.byref(kn), C.byref(nb)))
+        return dict(kernel_nodes=kn.value, device_bytes=nb.value)
+
+    def dispose(self):
+        if self.h:
+            if self.eng.h:
+                check(self.eng.L.cnhe_graph_destroy(self.h))
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.dispose()
+        except Exception:
+            pass
+
+
 class Engine:
     """One cnhe_ctx: parameters, device tables and keys for P plaintext moduli (== EncryptedSealBfvFactory)."""
 
@@ -206,7 +239,9 @@ class Engine:
 
     def close(self):
         if self.h:
-            for v in list(self._live):  # vectors hold device buffers of this context: release them first
+            self.L.cnhe_capture_abort(self.h)
+            live = list(self._live)  # graphs, vectors and matrices hold device buffers of this context: release them first
+            for v in sorted(live, key=lambda o: not isinstance(o, Graph)):
                 v.dispose()
             self.L.cnhe_context_destroy(self.h)
             self.h = C.c_void_p()
@@ -341,6 +376,26 @@ class Engine:
 
     def launch_count(self):
         return int(self.L.cnhe_kernel_launch_count(self.h))
+
+    # ---- graph recording (include/cnhe.h, cnhe_capture_begin)
+    def capture_begin(self):
+        """From now on the context records its calls into a graph instead of running them."""
+        check(self.L.cnhe_capture_begin(self.h))
+
+    def capture_end(self):
+        """The recorded calls as a Graph (launch() replays them)."""
+        g = C.c_void_p()
+        check(self.L.cnhe_capture_end(self.h, C.byref(g)))
+        return Graph(self, g)
+
+    def capture_abort(self):
+        check(self.L.cnhe_capture_abort(self.h))
+
+    def vecs_assign(self, dst, src):
+        """dst[i] takes src[i]'s ciphertext words (same dimension, blocks, format, scale and key slot): new inputs of a recorded graph."""
+        if len(dst) != len(src):
+            raise ValueError("dst and src differ in length")
+        check(self.L.cnhe_vecs_assign(self.h, _vec_array(dst), _vec_array(src), len(dst)))
 
     # ---- vectors
     def _new(self, fn, v, scale, fmt):

@@ -539,5 +539,96 @@ class B200BfvFactory:
                                                       None if bias is None else [x.vec for x in bias], M, K)
         return [B200BfvVector(self, o) for o in out]
 
+    def CaptureInference(self, net, example_inputs):
+        """Records the layers of `net` after its EncryptLayer once, on example_inputs, as one CUDA graph (include/cnhe.h,
+        cnhe_capture_begin): a CapturedInference whose Run(inputs) replays the whole chain with one launch.  example_inputs is one encrypted
+        input matrix (the network's GetNext path, Apply per layer) or a list of them, one per client, each bound to its client's key slot
+        (the serve_batch path, ApplyBatch per layer).  The chain runs once eagerly on the examples first, so that the layers build their
+        long-lived state outside the graph.  Runs must use the same shapes, scales and key slots; the network's prepared weights
+        and the factory's keys are read in place and must outlive the capture.  The example matrices become the graph's inputs: every Run
+        writes its inputs' words into them, so they belong to the capture until it is disposed."""
+        return CapturedInference(self, net, example_inputs)
+
     def Dispose(self):
         self.engine.close()
+
+
+class CapturedInference:
+    """One inference of a network recorded as a CUDA graph (B200BfvFactory.CaptureInference).  The example input matrices are the graph's
+    inputs (Run overwrites them with its inputs' words, one device copy per matrix and plaintext prime when each matrix's vectors lie in
+    one slab, as encrypted and imported matrices do); the output matrices the recording made are graph-owned: their words are those of
+    the latest Run and valid until the next one.  TimingLayers are left out: they time and synchronise the host, which a replay does
+    not do."""
+
+    def __init__(self, factory, net, example_inputs):
+        from .layers import EncryptLayer, TimingLayer
+        self.factory, self.graph, self.outputs = factory, None, None
+        self.batch = isinstance(example_inputs, (list, tuple))
+        examples = list(example_inputs) if self.batch else [example_inputs]
+        chain, layer = [], net
+        while not isinstance(layer, EncryptLayer):
+            if not isinstance(layer, TimingLayer):
+                chain.append(layer)
+            layer = layer.Source
+        chain.reverse()
+        for layer in chain:
+            if not layer.layerPrepared:
+                layer.Prepare()
+                layer.layerPrepared = True
+        self.inputs = examples
+        eng = factory.engine
+        # One eager pass first: layers build long-lived state (bias vectors, scalar-MAC plans) on their first Apply.  Built while recording,
+        # it would sit in graph memory that holds no words until a launch -- and never, if the recording is refused -- and later eager
+        # inferences of the network would read it.
+        for m in self._apply(chain, examples):
+            m.Dispose()
+        eng.capture_begin()
+        try:
+            ms = self._apply(chain, examples)
+            self.graph = eng.capture_end()
+        except BaseException:
+            eng.capture_abort()
+            raise
+        self.outputs = ms
+
+    def _apply(self, chain, inputs):
+        """the layers on the input matrices, each intermediate disposed once read (as serve_batch and GetNext do: while recording, later
+        recorded allocations reuse its memory); the inputs are kept"""
+        ms = list(inputs)
+        try:
+            for layer in chain:
+                out = layer.ApplyBatch(ms) if self.batch else [layer.Apply(ms[0])]
+                for m, o in zip(ms, out):
+                    if o is not m and not any(m is i for i in inputs):
+                        m.Dispose()
+                ms = out
+        except BaseException:
+            for m in ms:
+                if not any(m is i for i in inputs):
+                    m.Dispose()
+            raise
+        return ms
+
+    def Info(self):
+        """dict(kernel_nodes, device_bytes) of the recorded graph."""
+        return self.graph.info()
+
+    def Run(self, inputs):
+        """Assigns `inputs` (shaped as the example inputs: one matrix, or a list of one per client) to the recorded inputs, launches the
+        graph and returns the output matrix (or list of them).  Asynchronous like any other call; reading the outputs orders after it."""
+        ms = list(inputs) if self.batch else [inputs]
+        if len(ms) != len(self.inputs) or any(len(m.vectors) != len(i.vectors) for m, i in zip(ms, self.inputs)):
+            raise Exception("the inputs are not shaped as the recorded ones")
+        eng = self.factory.engine
+        eng.vecs_assign([v.vec for m in self.inputs for v in m.vectors], [v.vec for m in ms for v in m.vectors])
+        self.graph.launch()
+        return list(self.outputs) if self.batch else self.outputs[0]
+
+    def Dispose(self):
+        """Releases the outputs and the graph; the example input matrices stay the caller's."""
+        for m in self.outputs or []:
+            m.Dispose()
+        self.outputs = None
+        if self.graph is not None:
+            self.graph.dispose()
+            self.graph = None

@@ -1,7 +1,7 @@
 /*
  * cnhe.h -- C ABI of libcnhe.so, the H100-native BFV engine behind the CryptoNets plugin API.
  *
- * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these 111 entry points
+ * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these 121 entry points
  * with [DllImport("cnhe")] (stub in INTEGRATION.md); the Python mirror in cryptonets_b200/ binds them with ctypes.
  * One cnhe_vec is one reference `EncryptedSealBfvVector` ("HE Wrapper/EncryptedSealBfvVector.cs:150-573"): P
  * plaintext-modulus channels, each an `AtomicSealBfvEncryptedVector` ("HE Wrapper/AtomicSealBfvVector.cs:303-1476")
@@ -378,6 +378,55 @@ int cnhe_layer_poly(cnhe_ctx *, const cnhe_vec *const *in, int n, const cnhe_vec
 int cnhe_layer_activation_conv_dense(cnhe_ctx *, const cnhe_vec *const *in, int n_in, const cnhe_vec *a, const cnhe_vec *b, const cnhe_vec *c,
                                      const int32_t *gather, const cnhe_vec *const *weights, const cnhe_vec *const *bias, int M, int K,
                                      cnhe_vec **out /*M*/);
+
+/* ---- recording and replaying a chain of calls as one CUDA graph -------------------------------------------------- */
+/* A latency-bound inference (one LoLa image) spends its time launching hundreds of small kernels and preparing their arguments on the
+ * host.  Recorded once, for fixed shapes, key slots and prepared weights, the same chain replays as one graph launch per input: the same
+ * sm_90a kernels in the same order with the same arguments, and no host work between them.
+ * cnhe_capture_begin: from now on the context records its calls instead of running them (CNHE_ERR_STATE while already recording, and
+ *   CNHE_ERR_INVALID while profiling or the noise trace is on).  Works with "multi_stream" 0 and 1: the channel streams fork from the
+ *   capturing stream and join it through events, as cnhe_context_fork_streams / cnhe_context_join_streams order them.
+ * cnhe_capture_end: instantiates what was recorded into *out.  cnhe_capture_abort: drops the recording (a no-op when not recording); the
+ *   context stays usable.
+ * cnhe_graph_launch: enqueues one replay on the context's streams -- asynchronous and ordered with the calls before and after it, like any
+ *   other call.  CNHE_ERR_STATE when a key slot a recorded key switch reads has since been removed or had its keys replaced (key generation
+ *   or import), and while the context records.  Each launch adds the recorded operation counts to cnhe_op_counts and the recorded kernel
+ *   count to cnhe_kernel_launch_count: per-inference figures match the eager calls'.  Recording itself counts nothing.
+ * cnhe_graph_info: the graph's kernel nodes and the device bytes it owns (either pointer may be NULL).
+ * cnhe_graph_destroy: waits for the context's queued work and releases the graph (CNHE_ERR_STATE while the context records).  Destroy every
+ *   graph before its context.
+ * cnhe_vecs_assign: copies each src[i]'s ciphertext words into dst[i], device to device, ordered like any call: how a new input enters a
+ *   graph's recorded input vectors.  Both must be encrypted and match in dimension, blocks, format, scale and key slot (the recording acted
+ *   on those); the slots must be live, as for the calls that take several vectors, and a destination may not partly overlap its source
+ *   (CNHE_ERR_INVALID otherwise).  May be recorded.
+ * What a recording means:
+ *   Outputs: vectors created while recording belong to the graph.  Their words are defined once a launch completes and are overwritten by
+ *     the next launch.  Destroying an intermediate while recording lets later recorded allocations reuse its memory inside the graph; it
+ *     frees nothing outside the graph.  Vectors made by an aborted recording hold no defined words.
+ *   Memory: recorded allocations come from device memory the graph owns, never from the context's scratch recycling or upload slots, so
+ *     no eager call is handed a block a replay writes.  It returns to the driver once the graph and every vector made while recording are
+ *     destroyed.  Vectors, keys and prepared matrices created before the recording are read in place by every launch and must outlive the
+ *     graph; a buffer of theirs that is released while recording stays allocated until the graph is destroyed.
+ *   Constants: pointer tables, masks, scalar tables and every other host-built argument are copied once, at record time, into the graph's
+ *     memory; a launch reads nothing from the host.
+ *   Host decisions (which key-switch path, whether a square stays unrelinearised for the next layer, wave sizes) are taken at record time
+ *     and replay as recorded.
+ *   Refused while recording, with CNHE_ERR_STATE naming the call: every call that returns words or decisions to the host (decryption,
+ *     exports, cnhe_vec_device_ptr, noise budgets, cnhe_context_sync, preparing a diagonal matrix), every call that samples randomness
+ *     (encryption, including the fresh encryptions of zero an unfused layer makes: a replay would reuse it for every input), uploads,
+ *     profiling, the noise trace, key generation, import and export, adding or removing clients, cnhe_context_set_option, resetting the
+ *     operation counters, reading squares a cnhe_layer_square made before the recording and left unrelinearised (read them once
+ *     first: relinearised inside the graph they would hold no words until a launch), and any call on the context from another thread
+ *     than the recording one.  Any call that fails while recording
+ *     aborts the recording, as cnhe_capture_abort does; cnhe_capture_end then reports CNHE_ERR_STATE. */
+typedef struct cnhe_graph cnhe_graph;
+int cnhe_capture_begin(cnhe_ctx *);
+int cnhe_capture_end(cnhe_ctx *, cnhe_graph **out);
+int cnhe_capture_abort(cnhe_ctx *);
+int cnhe_graph_launch(cnhe_graph *);
+int cnhe_graph_info(const cnhe_graph *, uint64_t *kernel_nodes, uint64_t *device_bytes);
+int cnhe_graph_destroy(cnhe_graph *);
+int cnhe_vecs_assign(cnhe_ctx *, cnhe_vec *const *dst, const cnhe_vec *const *src, int n);
 
 /* ---- micro-benchmark / kernel-level entry points on caller-owned device memory ("raw") --------------------------- */
 int cnhe_dev_alloc(cnhe_ctx *, size_t words, uint64_t *dptr);

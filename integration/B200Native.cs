@@ -134,6 +134,13 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_raw_event_timing(IntPtr a0, int start);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_raw_elapsed_ms(IntPtr a0, out float ms);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern ulong cnhe_kernel_launch_count(IntPtr a0);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_begin(IntPtr a0);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_end(IntPtr a0, out IntPtr @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_abort(IntPtr a0);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_launch(IntPtr a0);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_info(IntPtr a0, out ulong kernel_nodes, out ulong device_bytes);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_destroy(IntPtr a0);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_assign(IntPtr a0, IntPtr[] dst, IntPtr[] src, int n);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_from_residues(IntPtr a0, ulong[] residues, ulong dim, double scale, int format, int encrypt, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_decrypt_residues(IntPtr a0, IntPtr a1, ulong[] @out, ulong cap_words);
 
@@ -578,6 +585,26 @@ namespace HEWrapper
             Cnhe.Check(Cnhe.cnhe_layer_square(Ctx, Cnhe.Handles(inputs), inputs.Length, outs));
             return outs.Select(h => (IVector)new B200BfvVector(this, h)).ToArray();
         }
+        /// Records the library calls `record` makes (one inference through the layers after the EncryptLayer, on example inputs) as one CUDA
+        /// graph instead of running them (include/cnhe.h, cnhe_capture_begin).  Returns the graph; the vectors `record` created belong to it.
+        /// A call that cannot be recorded (decryption, encryption, a synchronising timer) throws and aborts the recording.
+        public IntPtr Capture(Action record)
+        {
+            Cnhe.Check(Cnhe.cnhe_capture_begin(Ctx));
+            try { record(); }
+            catch { Cnhe.cnhe_capture_abort(Ctx); throw; }
+            Cnhe.Check(Cnhe.cnhe_capture_end(Ctx, out var graph));
+            return graph;
+        }
+        /// One replay of a Capture graph: `inputs` are copied into the vectors the recording read as its inputs (same shapes, scales and
+        /// key slots), then the graph is launched.  The recorded outputs hold this run's words until the next Run.
+        public void Run(IntPtr graph, IVector[] recordedInputs, IVector[] inputs)
+        {
+            if (recordedInputs.Length != inputs.Length) throw new Exception("the inputs are not shaped as the recorded ones");
+            Cnhe.Check(Cnhe.cnhe_vecs_assign(Ctx, Cnhe.Handles(recordedInputs), Cnhe.Handles(inputs), inputs.Length));
+            Cnhe.Check(Cnhe.cnhe_graph_launch(graph));
+        }
+        public void DisposeCapture(IntPtr graph) => Cnhe.Check(Cnhe.cnhe_graph_destroy(graph));
         /// CryptoTracker.TestBudget (CryptoTracker.cs:41-52)
         public int NoiseBudget(IVector v, int channel = 0, int block = 0)
         {
