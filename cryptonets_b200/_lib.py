@@ -132,6 +132,8 @@ _SIGS = {
     "cnhe_capture_end": [C.c_void_p, C.POINTER(C.c_void_p)],
     "cnhe_capture_abort": [C.c_void_p],
     "cnhe_graph_launch": [C.c_void_p],
+    "cnhe_graph_slots": [C.c_void_p, C.POINTER(C.c_int32), i32, C.POINTER(C.c_int32)],
+    "cnhe_graph_bind": [C.c_void_p, C.POINTER(C.c_int32), i32],
     "cnhe_graph_info": [C.c_void_p, U64P, U64P],
     "cnhe_graph_destroy": [C.c_void_p],
     "cnhe_vecs_assign": [C.c_void_p, C.POINTER(VECP), C.POINTER(VECP), i32],

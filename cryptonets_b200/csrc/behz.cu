@@ -213,7 +213,9 @@ __global__ void __launch_bounds__(256) k_behz_floor(const u64 *__restrict__ d, u
 }
 
 // ---- key-switch inner product: acc{0,1}[c][l][x] = sum_d digits[c][l][d][x] * key[d][{0,1}][l][x]
-// key_tab: nullptr, or one key base per ciphertext (calls whose ciphertexts belong to different key slots)
+// key_tab: nullptr, or one key base per ciphertext (calls whose ciphertexts belong to different key slots); REF: key and the key_tab
+// entries are key references (kernels.h key_base), the form a recorded graph's key switches take
+template <bool REF = false>
 __global__ void __launch_bounds__(256) k_ks_mac(const u64 *__restrict__ digits, const u64 *__restrict__ key, const u64 *const *__restrict__ key_tab,
                                                u64 *__restrict__ acc, int n, int D, int logn, const BehzConst *__restrict__ gbc) {
     __shared__ BehzConst bc;
@@ -225,7 +227,7 @@ __global__ void __launch_bounds__(256) k_ks_mac(const u64 *__restrict__ digits, 
     const int l = (int)((gid >> logn) % k), c = (int)((gid >> logn) / k);
     const DMod m = bc.q[l];
     const u64 *dg = digits + ((size_t)c * k + l) * D * N + x;
-    const u64 *k0 = (key_tab ? key_tab[c] : key) + (size_t)l * N + x;
+    const u64 *k0 = key_base<REF>(key_tab ? key_tab[c] : key) + (size_t)l * N + x;
     const size_t dstride = (size_t)N, kpoly = (size_t)k * N, kstride = (size_t)2 * k * N;
     U128 a0 = {0, 0}, a1 = {0, 0};
     for (int d0 = 0; d0 < D; d0 += 8) { // at most 8 products of 62x62 bits between reductions
@@ -298,9 +300,10 @@ cudaError_t launch_behz_tensor_mac(const u64 *a, const u64 *b, u64 *d, int n_out
     return cudaGetLastError();
 }
 cudaError_t launch_ks_mac(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn, const BehzConst *bc,
-                          cudaStream_t s) {
+                          cudaStream_t s, bool ref) {
     if (n <= 0) return cudaSuccess;
-    k_ks_mac<<<blocks_for(((size_t)n * k) << logn), 256, 0, s>>>(digits, key, key_tab, acc, n, D, logn, bc);
+    if (ref) k_ks_mac<true><<<blocks_for(((size_t)n * k) << logn), 256, 0, s>>>(digits, key, key_tab, acc, n, D, logn, bc);
+    else k_ks_mac<<<blocks_for(((size_t)n * k) << logn), 256, 0, s>>>(digits, key, key_tab, acc, n, D, logn, bc);
     return cudaGetLastError();
 }
 cudaError_t launch_decrypt_round(const u64 *x, u64 *plain, int n, int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s) {

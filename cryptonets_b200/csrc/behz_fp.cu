@@ -334,8 +334,9 @@ __device__ __forceinline__ ulonglong2 ldcs2(const u64 *p) { // streaming (evict-
 // them.  With one ciphertext per thread the kernel moved 48 bytes through L2 for every 16 bytes of the digit stream and sat on the L2
 // bandwidth (3.9 TB/s of HBM reads = 11.7 TB/s out of L2); with four it is 24 bytes.
 // TAB (CT == 1 only): ciphertext c0 reads its keys at key_tab[c0] instead of key (calls whose ciphertexts belong to different key slots);
-// a template argument so that the single-key instantiations stay exactly as they were (the table read costs the lazy one 12 registers)
-template <bool LAZY, int UNR, int CT, bool TAB = false>
+// a template argument so that the single-key instantiations stay exactly as they were (the table read costs the lazy one 12 registers).
+// REF: key and the key_tab entries are key references (kernels.h key_base), the form a recorded graph's key switches take
+template <bool LAZY, int UNR, int CT, bool TAB = false, bool REF = false>
 __global__ void __launch_bounds__(256) k_ks_mac_fp(const u64 *__restrict__ digits, const u64 *__restrict__ key, const u64 *const *__restrict__ key_tab,
                                                   u64 *__restrict__ acc, int n, int D, int logn, const __grid_constant__ BehzConstF F) {
     const int N = 1 << logn, k = F.k;
@@ -347,7 +348,7 @@ __global__ void __launch_bounds__(256) k_ks_mac_fp(const u64 *__restrict__ digit
     const double p = F.qd[l], pinv = F.qinv[l];
     const size_t kpoly = (size_t)k * N, kstride = (size_t)2 * k * N, cstride = (size_t)k * D * N;
     const u64 *dg = digits + ((size_t)c0 * k + l) * D * N + x;
-    const u64 *k0 = (TAB ? key_tab[c0] : key) + (size_t)l * N + x;
+    const u64 *k0 = key_base<REF>(TAB ? key_tab[c0] : key) + (size_t)l * N + x;
     double a[CT][4]; // [ciphertext][key poly * 2 + coefficient]
 #pragma unroll
     for (int ci = 0; ci < CT; ci++) a[ci][0] = a[ci][1] = a[ci][2] = a[ci][3] = 0.0;
@@ -407,7 +408,7 @@ __device__ __forceinline__ void kt_wait(unsigned long long *bar, unsigned parity
         if (!done && spin > (1u << 28)) __trap(); // a protocol error fails the launch instead of hanging the GPU
     }
 }
-template <int CT>
+template <int CT, bool REF = false>
 __global__ void __launch_bounds__(KT_THREADS, 2) k_ks_mac_tma(const u64 *__restrict__ digits, const u64 *__restrict__ key, u64 *__restrict__ acc, int n, int D,
                                                              int logn, const __grid_constant__ BehzConstF F) {
     extern __shared__ __align__(128) unsigned char kt_smem[];
@@ -431,7 +432,7 @@ __global__ void __launch_bounds__(KT_THREADS, 2) k_ks_mac_tma(const u64 *__restr
     if (tid >= KT_CONSUMERS) {
         if (tid == KT_CONSUMERS) { // producer
             const u64 *dg = digits + ((size_t)c0 * k + l) * D * N + x0;
-            const u64 *k0 = key + (size_t)l * N + x0;
+            const u64 *k0 = key_base<REF>(key) + (size_t)l * N + x0;
             for (int dd = 0; dd < D; dd++) {
                 const int s = dd % KT_STAGES;
                 kt_wait(empty + s, (((unsigned)dd / KT_STAGES) & 1) ^ 1);
@@ -542,29 +543,35 @@ cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, 
     else k_behz_floor_fold_fp<1, false><<<blocks_for(total), 256, 0, s>>>(d, out3, total, logn, *f, none);
     return cudaGetLastError();
 }
-cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,
+// REF: the recorded form (key references); the same kernel, grid and arithmetic as the pointer form for every n
+template <bool REF>
+static cudaError_t ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,
                              const BehzConstF *f, int lazy, cudaStream_t s) {
-    if (n <= 0) return cudaSuccess;
     // key reuse pays once the launch fills the GPU anyway: with few ciphertexts (LoLa: 1-32 per call) four per thread leaves SMs idle.
     // Per-ciphertext keys share nothing: one ciphertext per thread, and the copy-engine kernel (one key stream per CTA) is not used
     const int ct = n < 64 || key_tab ? 1 : 4;
     static_assert(1024 % KT_X == 0, "every ring (N >= 1024) is a whole number of tiles");
     if (lazy && ct == 4) { // full waves of lazy digits: the copy-engine-staged kernel
         constexpr int smem = KT_STAGES * (4 + 2) * KT_X * 8 + 2 * KT_STAGES * 8;
-        cudaError_t e = cudaFuncSetAttribute(k_ks_mac_tma<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        cudaError_t e = cudaFuncSetAttribute(k_ks_mac_tma<4, REF>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return e;
         const unsigned grid = (unsigned)(((1 << logn) / KT_X) * k * ((n + 3) / 4));
-        k_ks_mac_tma<4><<<grid, KT_THREADS, smem, s>>>(digits, key, acc, n, D, logn, *f);
+        k_ks_mac_tma<4, REF><<<grid, KT_THREADS, smem, s>>>(digits, key, acc, n, D, logn, *f);
         return cudaGetLastError();
     }
     const unsigned blocks = blocks_for(((size_t)((n + ct - 1) / ct) * k) << (logn - 1));
     if (key_tab) {
-        if (lazy) k_ks_mac_fp<true, 1, 1, true><<<blocks, 256, 0, s>>>(digits, key, key_tab, acc, n, D, logn, *f);
-        else k_ks_mac_fp<false, 4, 1, true><<<blocks, 256, 0, s>>>(digits, key, key_tab, acc, n, D, logn, *f);
-    } else if (lazy) k_ks_mac_fp<true, 1, 1><<<blocks, 256, 0, s>>>(digits, key, nullptr, acc, n, D, logn, *f);
-    else if (ct == 4) k_ks_mac_fp<false, 1, 4><<<blocks, 256, 0, s>>>(digits, key, nullptr, acc, n, D, logn, *f);
-    else k_ks_mac_fp<false, 4, 1><<<blocks, 256, 0, s>>>(digits, key, nullptr, acc, n, D, logn, *f);
+        if (lazy) k_ks_mac_fp<true, 1, 1, true, REF><<<blocks, 256, 0, s>>>(digits, key, key_tab, acc, n, D, logn, *f);
+        else k_ks_mac_fp<false, 4, 1, true, REF><<<blocks, 256, 0, s>>>(digits, key, key_tab, acc, n, D, logn, *f);
+    } else if (lazy) k_ks_mac_fp<true, 1, 1, false, REF><<<blocks, 256, 0, s>>>(digits, key, nullptr, acc, n, D, logn, *f);
+    else if (ct == 4) k_ks_mac_fp<false, 1, 4, false, REF><<<blocks, 256, 0, s>>>(digits, key, nullptr, acc, n, D, logn, *f);
+    else k_ks_mac_fp<false, 4, 1, false, REF><<<blocks, 256, 0, s>>>(digits, key, nullptr, acc, n, D, logn, *f);
     return cudaGetLastError();
+}
+cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,
+                             const BehzConstF *f, int lazy, cudaStream_t s, bool ref) {
+    if (n <= 0) return cudaSuccess;
+    return ref ? ks_mac_fp<true>(digits, key, key_tab, acc, n, D, k, logn, f, lazy, s) : ks_mac_fp<false>(digits, key, key_tab, acc, n, D, k, logn, f, lazy, s);
 }
 
 } // namespace cnhe

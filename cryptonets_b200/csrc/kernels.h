@@ -49,6 +49,15 @@ struct DigitMap {
     u64 mask;
 };
 
+// Key references (DESIGN 4.16).  A key switch recorded into a graph is given, in place of each key base, the address of a device word
+// that holds the base: the graph's key binding, which the host rewrites between launches so that one recording reads any client's keys.
+// With REF, a launcher's key, key_packed and key_tab entries are such addresses; the kernel loads the base through them once.
+template <bool REF, class T>
+__device__ __forceinline__ const T *key_base(const T *p) {
+    if constexpr (REF) return *reinterpret_cast<const T *const *>(p);
+    else return p;
+}
+
 // `fp` argument of the NTT launchers
 enum NttFormat { NTT_FP = 1, NTT_IN_F = 2, NTT_OUT_F = 4 };
 enum NttLoad { NTT_LOAD_PLAIN = 0, NTT_LOAD_DIGIT = 1 };
@@ -71,13 +80,15 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
 // buffer and no accumulator.  out must overlap neither the target nor the base words: other CTAs still read them while one writes.
 // key_packed: nullptr, or the copy of `key` made by launch_pack_keys48 (every q_l < 2^48), which the kernel then reads instead.
 // key_tab: nullptr, or a device table of n_ct key bases (ciphertext c reads key_tab[c] in place of key, or of key_packed when that is set)
+// ref: key, key_packed and the key_tab entries are key references (key_base above), not bases
 cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab,
                                     const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn,
-                                    const NttTab *tabs, cudaStream_t s);
+                                    const NttTab *tabs, cudaStream_t s, bool ref = false);
 // The fused key switch with its digits read from int32 planes: digit d of ciphertext c is planes[(c * D + d) * N + i], |value| < min q_l
-// (the digit sums of a scalar-MAC layer over unrelinearised products, DESIGN 4.15); keys, base, out and key_tab as above
+// (the digit sums of a scalar-MAC layer over unrelinearised products, DESIGN 4.15); keys, base, out, key_tab and ref as above
 cudaError_t launch_key_switch_planes(const int *planes, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab, const u64 *base,
-                                     size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s);
+                                     size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s,
+                                     bool ref = false);
 // the fused key switch's packed key copy: n_polys canonical N-word polynomials (words < 2^48) -> 6N bytes each, thread-interleaved (ntt.cu)
 cudaError_t launch_pack_keys48(const u64 *key, uint4 *out, int n_polys, int logn, cudaStream_t s);
 // dst[b] = INTT(src[b]) + base[(b / base_group) * base_stride + (b % base_group) * N]  (mod p)
@@ -239,11 +250,12 @@ cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn
 cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr,
                                      bool pair = false);
 cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,
-                             const BehzConstF *f, int lazy, cudaStream_t s);
+                             const BehzConstF *f, int lazy, cudaStream_t s, bool ref = false);
 // ---- K6: key-switch inner product. digits [n][D][k][N] (NTT), key [D][2][k][N] (NTT) -> acc [n][2][k][N] (NTT)
-// key_tab: nullptr, or a device table of n key bases (ciphertext c reads key_tab[c] in place of key)
+// key_tab: nullptr, or a device table of n key bases (ciphertext c reads key_tab[c] in place of key); ref: key and the key_tab entries
+// are key references (key_base), as for the fused key switch
 cudaError_t launch_ks_mac(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn, const BehzConst *bc,
-                          cudaStream_t s);
+                          cudaStream_t s, bool ref = false);
 // split a size-3 array [n][3][k][N] view: base[n][2][k][N] = (c0,c1), c2[n][k][N]
 
 // ---- diagonal matrix-vector product (diag.cu; slot layout and indices there)

@@ -1128,6 +1128,8 @@ k_ntt_inverse_split(const u64 *src, const u64 *base_add, int base_group, size_t 
 // bytes and a thread reads 96 B instead of 128.
 // key_tab: nullptr (every ciphertext uses key / keyp), or a device table of one key base per ciphertext -- packed copies with PK, u64
 // keys without -- for calls whose ciphertexts belong to different key slots.  Same grid, same arithmetic either way.
+// REF: key, keyp and the key_tab entries are key references (kernels.h key_base), the form a recorded graph's key switches take; the
+// base a CTA reads is loaded once, before the digit loop.
 template <int HLOGN>
 __host__ __device__ constexpr int ks_fused_threads() { return (1 << HLOGN) / 16; }
 template <int HLOGN>
@@ -1158,7 +1160,7 @@ __global__ void __launch_bounds__(256) k_pack_keys48(const u64 *__restrict__ key
 // Plane source (PL): digit d of ciphertext c is int32 plane d of planes + c * D * N instead of a cut of the target words -- the digit
 // sums S = sum_j W_j digit_d(c2_j) of a scalar-MAC layer over unrelinearised squares (DESIGN 4.15).  |S| < min q_l (host-checked),
 // the same input bound as a canonical digit, so nothing after the loads changes; `target` and `ct_stride` are unused.
-template <int HLOGN, bool PK, bool PL>
+template <int HLOGN, bool PK, bool PL, bool REF = false>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(ks_fused_threads<HLOGN>(), HLOGN == 12 ? 2 : 4)
 k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const int *__restrict__ planes, const u64 *__restrict__ key,
                    const uint4 *__restrict__ keyp, const u64 *const *__restrict__ key_tab, const u64 *__restrict__ base, size_t base_stride,
@@ -1181,8 +1183,11 @@ k_key_switch_fused(const u64 *__restrict__ target, size_t ct_stride, const int *
     const u64 *src_c = target + (size_t)c * ct_stride;
     const size_t kpoly = (size_t)k * N, kstride = 2 * kpoly;
     if (key_tab) { // per-ciphertext keys (several clients' key slots in one call): the table holds the form this instantiation reads
-        if constexpr (PK) keyp = reinterpret_cast<const uint4 *>(key_tab[c]);
-        else key = key_tab[c];
+        if constexpr (PK) keyp = key_base<REF>(reinterpret_cast<const uint4 *>(key_tab[c]));
+        else key = key_base<REF>(key_tab[c]);
+    } else if constexpr (REF) {
+        if constexpr (PK) keyp = key_base<REF>(keyp);
+        else key = key_base<REF>(key);
     }
     const u64 *key_l = key + (size_t)l * N + half * H + 16 * tid;
     load_twiddle_cache(twc, tb.wd, tid, TR);
@@ -1833,36 +1838,40 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
     });
     return cudaGetLastError();
 }
-template <int HL, bool PK, bool PL>
+template <int HL, bool PK, bool PL, bool REF>
 static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const int *planes, const u64 *key, const uint4 *keyp,
                                    const u64 *const *key_tab, const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm,
                                    const NttTab *tabs, cudaStream_t s) {
-    cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL, PK, PL>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
+    cudaError_t e = cudaFuncSetAttribute(k_key_switch_fused<HL, PK, PL, REF>, cudaFuncAttributeMaxDynamicSharedMemorySize, ks_fused_smem<HL>());
     if (e != cudaSuccess) return e;
-    k_key_switch_fused<HL, PK, PL><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, planes, key, keyp, key_tab,
-                                                                                                   base, base_stride, out, tabs, k, dm);
+    k_key_switch_fused<HL, PK, PL, REF><<<2 * n_ct * k, ks_fused_threads<HL>(), ks_fused_smem<HL>(), s>>>(target, ct_stride, planes, key, keyp,
+                                                                                                        key_tab, base, base_stride, out, tabs, k, dm);
     return cudaGetLastError();
 }
 template <int HL, bool PL>
 static cudaError_t launch_ks_fused(const u64 *target, size_t ct_stride, const int *planes, const u64 *key, const uint4 *keyp,
                                    const u64 *const *key_tab, const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm,
-                                   const NttTab *tabs, cudaStream_t s) {
-    return keyp ? launch_ks_fused<HL, true, PL>(target, ct_stride, planes, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s)
-                : launch_ks_fused<HL, false, PL>(target, ct_stride, planes, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+                                   const NttTab *tabs, cudaStream_t s, bool ref) {
+    if (ref)
+        return keyp ? launch_ks_fused<HL, true, PL, true>(target, ct_stride, planes, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s)
+                    : launch_ks_fused<HL, false, PL, true>(target, ct_stride, planes, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+    return keyp ? launch_ks_fused<HL, true, PL, false>(target, ct_stride, planes, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s)
+                : launch_ks_fused<HL, false, PL, false>(target, ct_stride, planes, key, keyp, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
 }
 cudaError_t launch_key_switch_fused(const u64 *target, size_t ct_stride, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab,
                                     const u64 *base, size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn,
-                                    const NttTab *tabs, cudaStream_t s) {
+                                    const NttTab *tabs, cudaStream_t s, bool ref) {
     if (n_ct <= 0) return cudaSuccess;
-    if (logn == 13) return launch_ks_fused<12, false>(target, ct_stride, nullptr, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
-    if (logn == 12) return launch_ks_fused<11, false>(target, ct_stride, nullptr, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+    if (logn == 13) return launch_ks_fused<12, false>(target, ct_stride, nullptr, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s, ref);
+    if (logn == 12) return launch_ks_fused<11, false>(target, ct_stride, nullptr, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s, ref);
     return cudaErrorInvalidValue;
 }
 cudaError_t launch_key_switch_planes(const int *planes, const u64 *key, const uint4 *key_packed, const u64 *const *key_tab, const u64 *base,
-                                     size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s) {
+                                     size_t base_stride, u64 *out, int n_ct, int k, const DigitMap &dm, int logn, const NttTab *tabs, cudaStream_t s,
+                                     bool ref) {
     if (n_ct <= 0) return cudaSuccess;
-    if (logn == 13) return launch_ks_fused<12, true>(nullptr, 0, planes, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
-    if (logn == 12) return launch_ks_fused<11, true>(nullptr, 0, planes, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s);
+    if (logn == 13) return launch_ks_fused<12, true>(nullptr, 0, planes, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s, ref);
+    if (logn == 12) return launch_ks_fused<11, true>(nullptr, 0, planes, key, key_packed, key_tab, base, base_stride, out, n_ct, k, dm, tabs, s, ref);
     return cudaErrorInvalidValue;
 }
 template <int HL>

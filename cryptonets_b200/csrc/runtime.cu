@@ -968,11 +968,26 @@ static bool spans_overlap(const u64 *a, size_t a_words, const u64 *b, size_t b_w
 // target + i * target_stride, its base (2 polynomials) at base + i * base_stride; out is packed [n][2][k][N]
 const KeySet &Context::keys(int channel, int s) const {
     if (!slot_live(s)) throw Error(-1, "no such key slot");
-    if (rec) {
-        const auto g = key_gen.find(s);
-        rec->slots[s] = g == key_gen.end() ? 0 : g->second;
-    }
     return s == 0 ? ch[channel] : clients[s - 1][channel];
+}
+const u64 *KeyBinding::ref(const u64 *base) {
+    auto w = word.find(base);
+    if (w == word.end()) {
+        const auto k = seen.find(base);
+        if (k == seen.end()) throw Error(-1, "internal error: a recorded key switch was given a key that no key slot holds");
+        if (words.size() >= cap) throw Error(-1, "internal error: a recording read more keys than its key slots hold");
+        w = word.emplace(base, words.size()).first;
+        words.push_back(k->second);
+    }
+    return reinterpret_cast<const u64 *>(table + w->second);
+}
+// the pointer a kernel is given for key base p: while recording, its key reference (the graph reads the key through its binding)
+static const u64 *key_arg(Context &c, const u64 *p) { return c.rec && p ? c.rec->keys->ref(p) : p; }
+// ciphertexts c0 .. c0 + m of a per-ciphertext key table, as key_arg passes them, in workspace memory
+static const u64 *const *key_table(Context &c, const std::vector<const u64 *> &tab, int c0, int m) {
+    std::vector<const u64 *> part(tab.begin() + c0, tab.begin() + c0 + m);
+    for (const u64 *&p : part) p = key_arg(c, p);
+    return upload_ptrs(c, part);
 }
 KsKeys KsKeys::slice(int c0, int m) const {
     KsKeys r = *this;
@@ -982,9 +997,16 @@ KsKeys KsKeys::slice(int c0, int m) const {
     return r;
 }
 // collects each ciphertext's key set (per-ciphertext table or the call's slot) into KsKeys; a call of one slot stays uniform
+// (kind, elt: which key pick takes, as a recording notes it)
 template <class Pick>
-static KsKeys pick_keys(Context &c, int ch, int n, const int *slots, Pick pick) {
+static KsKeys pick_keys(Context &c, int ch, int n, const int *slots, int kind, u64 elt, Pick pick) {
     KsKeys r;
+    auto take = [&](int s, const u64 *&key, const u64 *&pk) {
+        pick(c.keys(ch, s), key, pk);
+        if (!c.rec) return;
+        c.rec->keys->seen[key] = {s, ch, kind, elt};
+        if (pk) c.rec->keys->seen[pk] = {s, ch, KeyBinding::RLK_PACKED, 0};
+    };
     if (slots) {
         bool uniform = true;
         for (int i = 0; i < n; i++) uniform = uniform && slots[i] == slots[0];
@@ -992,7 +1014,7 @@ static KsKeys pick_keys(Context &c, int ch, int n, const int *slots, Pick pick) 
             bool packed = true;
             for (int i = 0; i < n; i++) {
                 const u64 *key, *pk;
-                pick(c.keys(ch, slots[i]), key, pk);
+                take(slots[i], key, pk);
                 r.keys.push_back(key);
                 r.packs.push_back(pk);
                 packed = packed && pk;
@@ -1001,18 +1023,18 @@ static KsKeys pick_keys(Context &c, int ch, int n, const int *slots, Pick pick) 
             return r;
         }
     }
-    pick(c.keys(ch, slots && n ? slots[0] : c.slot), r.key, r.packed);
+    take(slots && n ? slots[0] : c.slot, r.key, r.packed);
     return r;
 }
 KsKeys relin_keys(Context &c, int ch, int n, const int *slots) {
-    return pick_keys(c, ch, n, slots, [](const KeySet &ks, const u64 *&key, const u64 *&pk) {
+    return pick_keys(c, ch, n, slots, KeyBinding::RLK, 0, [](const KeySet &ks, const u64 *&key, const u64 *&pk) {
         if (!ks.have_rlk) throw Error(-3, "relinearization keys are missing");
         key = ks.rlk->p;
         pk = ks.rlk_packed ? ks.rlk_packed->p : nullptr;
     });
 }
 KsKeys galois_keys(Context &c, int ch, int n, const int *slots, u64 elt) {
-    return pick_keys(c, ch, n, slots, [elt](const KeySet &ks, const u64 *&key, const u64 *&pk) {
+    return pick_keys(c, ch, n, slots, KeyBinding::GALOIS, elt, [elt](const KeySet &ks, const u64 *&key, const u64 *&pk) {
         auto it = ks.glk.find(elt);
         if (it == ks.glk.end()) throw Error(-3, "Galois key not present");
         key = it->second->p;
@@ -1044,17 +1066,15 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
         const int m = std::min(wave, n - c0);
         // a call of several key slots passes one key base per ciphertext (the packed copies when every slot has one)
         const u64 *const *key_tab = nullptr;
-        if (keys.per_ct()) {
-            const std::vector<const u64 *> &tab = fused && key_packed ? keys.packs : keys.keys;
-            key_tab = upload_ptrs(c, std::vector<const u64 *>(tab.begin() + c0, tab.begin() + c0 + m));
-        }
+        if (keys.per_ct()) key_tab = key_table(c, fused && key_packed ? keys.packs : keys.keys, c0, m);
         if (fused) {
             // HBM: the target residues once (the pair and the other residues' CTAs share them through L2), the keys once, the output.  The
             // base words the epilogue adds (another 8N bytes per output polynomial, mostly prefetched) are not booked: the figure keeps the
             // meaning it had when the kernel wrote an accumulator of the output's size
             PROF(3, 8.0 * N * ((double)m * k + (double)m * 2 * k) + (key_packed ? 6.0 : 8.0) * N * dm.D * 2 * k);
-            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, keys.key, reinterpret_cast<const uint4 *>(key_packed),
-                                            key_tab, base + (size_t)c0 * base_stride, base_stride, out + (size_t)c0 * 2 * k * N, m, k, dm, c.logN, c.d_tabs, c.stream),
+            c.check(launch_key_switch_fused(target + (size_t)c0 * target_stride, target_stride, key_arg(c, keys.key),
+                                            reinterpret_cast<const uint4 *>(key_arg(c, key_packed)), key_tab, base + (size_t)c0 * base_stride, base_stride,
+                                            out + (size_t)c0 * 2 * k * N, m, k, dm, c.logN, c.d_tabs, c.stream, c.rec != nullptr),
                     "key_switch_fused");
             continue;
         }
@@ -1068,8 +1088,9 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
                         "ntt_forward_digits");
             }
             PROF(3, 8.0 * N * ((double)m * dm.D * k + (double)dm.D * 2 * k + (double)m * 2 * k));
-            if (c.fp_elementwise) c.check(launch_ks_mac_fp(digits, keys.key, key_tab, acc, m, dm.D, k, c.logN, &c.h_bf, lazy, c.stream), "ks_mac_fp");
-            else c.check(launch_ks_mac(digits, keys.key, key_tab, acc, m, dm.D, k, c.logN, c.d_bc, c.stream), "ks_mac");
+            const u64 *key = key_arg(c, keys.key);
+            if (c.fp_elementwise) c.check(launch_ks_mac_fp(digits, key, key_tab, acc, m, dm.D, k, c.logN, &c.h_bf, lazy, c.stream, c.rec != nullptr), "ks_mac_fp");
+            else c.check(launch_ks_mac(digits, key, key_tab, acc, m, dm.D, k, c.logN, c.d_bc, c.stream, c.rec != nullptr), "ks_mac");
         }
         PROF(1, 24.0 * N * m * 2 * k);
         c.check(launch_ntt_inverse_add(acc, base + (size_t)c0 * base_stride, 2 * k, base_stride, out + (size_t)c0 * 2 * k * N, m * 2 * k, c.logN,
@@ -1290,11 +1311,11 @@ void op_relinearize_planes(Context &c, int ch, const int *planes, int n, const u
     const u64 *key_packed = keys.per_ct() ? (keys.packs.empty() ? nullptr : keys.packs[0]) : keys.packed;
     WsScope scope(c);
     const u64 *const *key_tab = nullptr;
-    if (keys.per_ct()) key_tab = upload_ptrs(c, key_packed ? keys.packs : keys.keys);
+    if (keys.per_ct()) key_tab = key_table(c, key_packed ? keys.packs : keys.keys, 0, n);
     // HBM: the digit planes once (every residue's CTAs of a ciphertext share them through L2), the keys once, the output
     PROF(3, 4.0 * N * n * dm.D + 8.0 * N * n * 2 * k + (key_packed ? 6.0 : 8.0) * N * dm.D * 2 * k);
-    c.check(launch_key_switch_planes(planes, keys.key, reinterpret_cast<const uint4 *>(key_packed), key_tab, base, (size_t)2 * k * N, out2, n, k, dm,
-                                     c.logN, c.d_tabs, c.stream),
+    c.check(launch_key_switch_planes(planes, key_arg(c, keys.key), reinterpret_cast<const uint4 *>(key_arg(c, key_packed)), key_tab, base,
+                                     (size_t)2 * k * N, out2, n, k, dm, c.logN, c.d_tabs, c.stream, c.rec != nullptr),
             "key_switch_planes");
 }
 void op_multiply_relin(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out2, const int *slots,

@@ -60,13 +60,31 @@ struct DevBuf {
 };
 typedef std::shared_ptr<DevBuf> BufRef;
 
+// The key binding of a recorded graph (DESIGN 4.16).  While recording, every key base a key switch hands a kernel is replaced by a key
+// reference: the address of one word of `table`, a small device array the graph owns, that stands for one key of one key slot and
+// channel -- the relinearisation keys, their packed copy, or the keys of one Galois element.  The graph's key positions are the distinct
+// slots its references name, in ascending order.  Binding (cnhe_graph_bind) points every word of a position at another slot's key of
+// the same kind, and the next launch copies the words into the table before the recorded kernels read them.
+struct KeyBinding {
+    enum Kind { RLK, RLK_PACKED, GALOIS };
+    struct Key { int slot, channel, kind; u64 elt; };
+    std::map<const u64 *, Key> seen;      // while recording: every key base picked for a key switch, and which key it is
+    std::map<const u64 *, size_t> word;   // key base -> its table word
+    std::vector<Key> words;               // the key each table word stands for, in the order they were handed out
+    const u64 **table = nullptr;          // device, `cap` words (graph memory)
+    size_t cap = 0;
+    std::map<int, int> to;                // recorded slot -> the slot it is bound to (identity until the first bind)
+    int slot(int s) const { const auto it = to.find(s); return it == to.end() ? s : it->second; }
+    const u64 *ref(const u64 *base);      // the key reference of a key base picked while recording
+};
+
 // State of a context while it records its calls into a CUDA graph (stream capture of the channel streams, vec.cu cnhe_capture_*)
 struct Recording {
     std::thread::id thread;             // the recording thread: calls from any other thread are refused
     std::shared_ptr<GraphArena> arena;
     std::vector<uint64_t> op0;          // operation counters and kernel count when the recording began: restored when it ends, the
     uint64_t launches0 = 0;             // difference is what every launch of the graph adds
-    std::map<int, uint64_t> slots;      // key slot -> its key generation, for every slot whose keys a recorded key switch reads
+    std::shared_ptr<KeyBinding> keys;   // the references the recorded key switches read their keys through
     std::vector<std::shared_ptr<void>> keep; // cached host-built device tables (scalar-MAC plans) the recorded kernels read
     // buffers allocated before the recording and released during it: the graph may read them, so they are freed (or recycled) outside
     // it, when the graph is destroyed (at once when the recording is aborted)
@@ -117,7 +135,7 @@ struct Context {
     int slot = 0; // key slot of the ciphertexts the current public call works on (reset to 0 by every call; vec.cu sets it from the operands)
     bool foreign = false; // the current call touches ciphertexts of a slot other than 0: the noise trace cannot measure them (no secret key)
     bool slot_live(int s) const { return s == 0 || (s > 0 && (size_t)s <= clients.size() && !clients[s - 1].empty()); }
-    const KeySet &keys(int channel, int s) const; // while recording, also notes the slot and its key generation
+    const KeySet &keys(int channel, int s) const;
     // key generation of a slot: bumped whenever its keys are replaced or removed, so that a graph recorded against them refuses to launch
     std::map<int, uint64_t> key_gen;
     void keys_changed(int s) { key_gen[s]++; }
@@ -302,6 +320,7 @@ FloorEpi floor_epi(const Context &c, int ch, u64 A, u64 B, u64 C);
 struct KsKeys {
     const u64 *key = nullptr, *packed = nullptr; // uniform call; packed: the 48-bit copy for the fused kernel (nullptr: u64 keys)
     std::vector<const u64 *> keys, packs;        // per ciphertext (empty: uniform); packs empty when some key has no packed copy
+    // Key bases, also while recording: op_key_switch and op_relinearize_planes turn the ones they pass into key references (KeyBinding)
     bool per_ct() const { return !keys.empty(); }
     KsKeys slice(int c0, int m) const;
 };

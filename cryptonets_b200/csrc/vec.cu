@@ -11,6 +11,7 @@
 #include <climits>
 #include <cstring>
 #include <optional>
+#include <set>
 #include <unordered_map>
 
 #include "hostmath.h"
@@ -169,10 +170,53 @@ struct cnhe_graph {
     std::vector<uint64_t> ops; // operation counts one launch adds
     uint64_t launches = 0;     // kernel launches one launch adds (what the recorded calls counted)
     uint64_t kernel_nodes = 0;
-    std::map<int, uint64_t> slots;
+    // key binding (cnhe_graph_bind): the key positions (recorded slots, ascending), the slot each is bound to and that slot's key
+    // generation when it was bound, and the words of the device table under that binding
+    std::shared_ptr<KeyBinding> keys;
+    std::vector<int> positions, bound;
+    std::vector<uint64_t> bound_gen;
+    std::vector<const u64 *> words;
+    bool words_sent = false; // the device table holds `words` (or will, once the copy queued by the last launch has run)
     std::vector<std::shared_ptr<void>> keep;
     std::vector<Recording::Deferred> held; // buffers from before the recording, released during it: the graph may read them
 };
+static uint64_t key_gen(const Context &c, int s) {
+    const auto it = c.key_gen.find(s);
+    return it == c.key_gen.end() ? 0 : it->second;
+}
+// Binds key position i of g to slots[i]: checks that every slot is live and holds every key its position's references stand for, in the
+// recorded form, then (and only then) takes the binding.  The device table is rewritten by the next launch.
+static void bind_graph(Context &c, cnhe_graph &g, const int *slots) {
+    const size_t np = g.positions.size();
+    for (size_t i = 0; i < np; i++)
+        if (!c.slot_live(slots[i])) fail(("cnhe_graph_bind: no such key slot " + std::to_string(slots[i])).c_str());
+    std::vector<const u64 *> words;
+    for (const KeyBinding::Key &k : g.keys->words) {
+        const int s = slots[std::lower_bound(g.positions.begin(), g.positions.end(), k.slot) - g.positions.begin()];
+        const KeySet &ks = c.keys(k.channel, s);
+        auto missing = [&](const std::string &what) {
+            throw Error(CNHE_ERR_STATE, "cnhe_graph_bind: key slot " + std::to_string(s) + " (plaintext channel " + std::to_string(k.channel) +
+                                            ") holds no " + what + ", which the graph reads");
+        };
+        if (k.kind == KeyBinding::GALOIS) {
+            const auto it = ks.glk.find(k.elt);
+            if (it == ks.glk.end()) missing("Galois key of element " + std::to_string(k.elt));
+            words.push_back(it->second->p);
+        } else if (!ks.have_rlk || (k.kind == KeyBinding::RLK_PACKED && !ks.rlk_packed)) {
+            missing(k.kind == KeyBinding::RLK ? "relinearization keys" : "packed relinearization keys");
+        } else words.push_back(k.kind == KeyBinding::RLK ? ks.rlk->p : ks.rlk_packed->p);
+    }
+    g.bound.assign(slots, slots + np);
+    g.bound_gen.clear();
+    for (size_t i = 0; i < np; i++) {
+        g.bound_gen.push_back(key_gen(c, slots[i]));
+        g.keys->to[g.positions[i]] = slots[i];
+    }
+    if (words != g.words) {
+        g.words = std::move(words);
+        g.words_sent = false;
+    }
+}
 extern "C" int cnhe_capture_begin(cnhe_ctx *h) {
     API_BEGIN(h)
     if (c.rec) c.refuse("cannot start a second recording");
@@ -183,6 +227,13 @@ extern "C" int cnhe_capture_begin(cnhe_ctx *h) {
     r->arena = std::make_shared<GraphArena>();
     r->op0.assign(c.op_count, c.op_count + Context::OP_COUNT);
     r->launches0 = c.launches;
+    // the key binding's device table: one word for every key the context's slots hold (a recording reads each at most once)
+    r->keys = std::make_shared<KeyBinding>();
+    for (int s = 0; s <= (int)c.clients.size(); s++)
+        if (c.slot_live(s))
+            for (int ch = 0; ch < c.P; ch++) r->keys->cap += 2 + c.keys(ch, s).glk.size();
+    const std::vector<const u64 *> zeros(r->keys->cap);
+    r->keys->table = static_cast<const u64 **>(const_cast<void *>(r->arena->constant(zeros.data(), zeros.size() * sizeof(u64 *), c.copy_stream)));
     CNHE_CUDA(cudaStreamBeginCapture(c.streams[0], cudaStreamCaptureModeRelaxed));
     c.rec = std::move(r);
     c.fork_streams(); // the channel streams join the capture
@@ -200,7 +251,7 @@ extern "C" int cnhe_capture_end(cnhe_ctx *h, cnhe_graph **out) {
     std::unique_ptr<cnhe_graph> g(new cnhe_graph);
     g->h = h;
     g->arena = c.rec->arena;
-    g->slots = c.rec->slots;
+    g->keys = c.rec->keys;
     g->keep = c.rec->keep;
     for (int i = 0; i < Context::OP_COUNT; i++) g->ops.push_back(c.op_count[i] - c.rec->op0[i]);
     g->launches = c.launches - c.rec->launches0;
@@ -219,20 +270,48 @@ extern "C" int cnhe_capture_end(cnhe_ctx *h, cnhe_graph **out) {
     cudaGraphDestroy(graph);
     if (e != cudaSuccess) release_deferred(c, g->held);
     CNHE_CUDA(e);
+    // the recording is the first binding: every position bound to itself
+    g->keys->seen.clear();
+    g->keys->word.clear();
+    std::set<int> pos;
+    for (const KeyBinding::Key &k : g->keys->words) pos.insert(k.slot);
+    g->positions.assign(pos.begin(), pos.end());
+    bind_graph(c, *g, g->positions.data());
     *out = g.release();
+    API_END
+}
+extern "C" int cnhe_graph_slots(const cnhe_graph *g, int *slots, int cap, int *n) {
+    if (!g || !n) return set_err(CNHE_ERR_INVALID, "null argument");
+    *n = (int)g->positions.size();
+    if (slots)
+        for (int i = 0; i < *n && i < cap; i++) slots[i] = g->positions[i];
+    return CNHE_OK;
+}
+extern "C" int cnhe_graph_bind(cnhe_graph *g, const int *slots, int n) {
+    if (!g) return set_err(CNHE_ERR_INVALID, "null graph");
+    API_BEGIN(g->h)
+    not_recorded(c, "binds a recorded graph to key slots");
+    if (n != (int)g->positions.size() || (n > 0 && !slots))
+        fail(("cnhe_graph_bind: the graph has " + std::to_string(g->positions.size()) + " key positions (cnhe_graph_slots), " +
+              std::to_string(n) + " slots were given").c_str());
+    bind_graph(c, *g, slots);
     API_END
 }
 extern "C" int cnhe_graph_launch(cnhe_graph *g) {
     if (!g) return set_err(CNHE_ERR_INVALID, "null graph");
     API_BEGIN(g->h)
     not_recorded(c, "launches a recorded graph");
-    for (const auto &s : g->slots) {
-        const auto it = c.key_gen.find(s.first);
-        if (!c.slot_live(s.first) || (it == c.key_gen.end() ? 0 : it->second) != s.second)
-            throw Error(CNHE_ERR_STATE, "cnhe_graph_launch: the keys of key slot " + std::to_string(s.first) +
-                                            " were removed or replaced after the graph was recorded");
+    for (size_t i = 0; i < g->bound.size(); i++) {
+        const int s = g->bound[i];
+        if (!c.slot_live(s) || key_gen(c, s) != g->bound_gen[i])
+            throw Error(CNHE_ERR_STATE, "cnhe_graph_launch: the keys of key slot " + std::to_string(s) +
+                                            " were removed or replaced after the graph was recorded or bound to it (cnhe_graph_bind)");
     }
     c.join_streams(); // after every call queued before, on any channel
+    if (!g->words_sent) { // a new binding: stream 0 orders the copy after the previous launch's kernels and before this one's
+        c.h2d(g->keys->table, g->words.data(), g->words.size() * sizeof(u64 *));
+        g->words_sent = true;
+    }
     CNHE_CUDA(cudaGraphLaunch(g->exec, c.streams[0]));
     c.fork_streams(); // before every call queued after
     for (int i = 0; i < Context::OP_COUNT; i++) c.op_count[i] += g->ops[i];
@@ -474,6 +553,7 @@ cnhe_vec *new_vec(Context &c, uint64_t dim, double scale, int format, bool enc, 
     v->format = format;
     v->enc = enc;
     v->slot = c.slot;
+    if (c.rec) v->binding = c.rec->keys;
     v->blocks = blocks;
     v->buf.resize(c.P);
     v->off.assign(c.P, 0);
@@ -502,7 +582,7 @@ static cnhe_vec *slab_output(Context &c, const std::vector<BufRef> &slab, size_t
 }
 static cnhe_vec *alias_of(const cnhe_vec *a) { return new cnhe_vec(*a); } // shares the reference-counted buffers
 cnhe_vec::cnhe_vec(const cnhe_vec &o)
-    : ctx(o.ctx), dim(o.dim), scale(o.scale), format(o.format), enc(o.enc), slot(o.slot), blocks(o.blocks), buf(o.buf), off(o.off),
+    : ctx(o.ctx), dim(o.dim), scale(o.scale), format(o.format), enc(o.enc), slot(o.slot), binding(o.binding), blocks(o.blocks), buf(o.buf), off(o.off),
       scalars(o.scalars), is_const(o.is_const), const_val(o.const_val), pend(o.pend), pend_ct(o.pend_ct) {
     if (pend) pend->members.push_back(this);
 }
@@ -520,11 +600,14 @@ void materialise(Context &c, const cnhe_vec *v) {
     if (c.rec && g->slab3[0]->arena != c.rec->arena) c.refuse("relinearises squares made before the recording (read them once first)");
     const cudaStream_t s0 = c.stream;
     const size_t ctw = c.ct_words();
+    std::vector<int> slots = g->ct_slot; // squares recorded into a graph: under the slots the graph is bound to
+    if (v->binding)
+        for (int &s : slots) s = v->binding->slot(s);
     std::vector<BufRef> slab2(c.P);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
         slab2[ch] = c.alloc((size_t)g->total * ctw);
-        op_relinearize(c, ch, g->slab3[ch]->p, g->total, slab2[ch]->p, g->ct_slot.data(), false); // booked by the square
+        op_relinearize(c, ch, g->slab3[ch]->p, g->total, slab2[ch]->p, slots.data(), false); // booked by the square
     }
     c.stream = s0;
     for (cnhe_vec *m : g->members) {
@@ -545,8 +628,8 @@ int use_slot(Context &c, const cnhe_vec *const *vs, int n) {
     for (int i = 0; i < n; i++) {
         if (vs[i] && vs[i]->ctx == &c) materialise(c, vs[i]);
         if (!vs[i] || !vs[i]->enc) continue;
-        if (s >= 0 && vs[i]->slot != s) fail("encrypted operands belong to different key slots");
-        s = vs[i]->slot;
+        if (s >= 0 && vs[i]->key_slot() != s) fail("encrypted operands belong to different key slots");
+        s = vs[i]->key_slot();
     }
     if (s < 0) s = 0;
     if (!c.slot_live(s)) fail("the vector's key slot was removed");
@@ -560,7 +643,7 @@ static std::vector<int> vec_slots(Context &c, const cnhe_vec *const *vs, int n, 
     std::vector<int> s(n);
     for (int i = 0; i < n; i++) {
         if (!keep_pending && vs[i]->ctx == &c) materialise(c, vs[i]);
-        s[i] = vs[i]->slot;
+        s[i] = vs[i]->key_slot();
         if (!c.slot_live(s[i])) fail("the vector's key slot was removed");
         if (s[i] != 0) c.foreign = true;
     }
@@ -724,7 +807,7 @@ static void decrypt_channel(Context &c, const cnhe_vec *v, int ch, std::vector<u
     if (!v->enc && v->format == CNHE_SPARSE) { res = v->scalars[ch]; return; }
     u64 *plain;
     if (v->enc) {
-        if (v->slot != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
+        if (v->key_slot() != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
         plain = c.ws_alloc((size_t)v->blocks * N);
         op_decrypt(c, ch, v->ptr(ch), v->blocks, plain);
     } else plain = v->ptr(ch);
@@ -804,7 +887,7 @@ extern "C" int cnhe_vecs_assign(cnhe_ctx *h, cnhe_vec *const *dst, const cnhe_ve
         if (d->pend) fail("the destination's squares are not relinearised (it was made by a square layer and never read)");
         if (d->dim != s->dim || d->blocks != s->blocks || d->format != s->format) fail("source and destination differ in shape");
         if (d->scale != s->scale) fail("source and destination differ in scale");
-        if (d->slot != s->slot) fail("source and destination belong to different key slots");
+        if (d->key_slot() != s->key_slot()) fail("source and destination belong to different key slots");
     }
     // a destination may be its own source (nothing to copy) but may not overlap any other source: the copies (coalesced below) would
     // read words they, or an earlier copy, overwrite
@@ -1244,11 +1327,12 @@ extern "C" int cnhe_vec_set_key_slot(cnhe_vec *v, int slot) {
     if (!v->enc) return set_err(CNHE_ERR_INVALID, "plain vectors have no key slot");
     if (!v->ctx->slot_live(slot)) return set_err(CNHE_ERR_INVALID, "no such key slot");
     v->slot = slot;
+    v->binding.reset();
     return CNHE_OK;
 }
 extern "C" int cnhe_vec_key_slot(const cnhe_vec *v, int *slot) {
     if (!v || !slot) return set_err(CNHE_ERR_INVALID, "null argument");
-    *slot = v->enc ? v->slot : -1;
+    *slot = v->enc ? v->key_slot() : -1;
     return CNHE_OK;
 }
 // Rotate (first block) of n vectors by the same amount, their key slots may differ: the hops of all vectors share each key-switch wave
@@ -1351,7 +1435,7 @@ extern "C" int cnhe_noise_budget(cnhe_ctx *h, const cnhe_vec *v, int channel, in
     not_recorded(c, "returns words to the host");
     same_ctx(c, v);
     if (!v->enc || channel < 0 || channel >= c.P || block < 0 || block >= v->blocks) fail("bad arguments");
-    if (v->slot != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
+    if (v->key_slot() != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
     *bits = op_noise_budget(c, channel, v->block(channel, block));
     API_END
 }

@@ -35,6 +35,9 @@ struct cnhe_vec {
     int format = CNHE_DENSE;
     bool enc = false;
     int slot = 0;   // encrypted: the key slot whose evaluation keys its key switches use (plain vectors ignore it)
+    // made while recording a graph: that graph's key binding, which maps `slot` to the slot the graph is bound to (key_slot)
+    std::shared_ptr<const KeyBinding> binding;
+    int key_slot() const { return binding ? binding->slot(slot) : slot; }
     int blocks = 0; // ciphertexts / plaintexts per channel
     std::vector<BufRef> buf; // per channel: enc -> blocks*2kN words, plain dense -> blocks*N words, plain sparse -> `blocks` scalars
     std::vector<size_t> off;

@@ -168,6 +168,19 @@ class Graph:
         """Enqueue one replay (asynchronous, ordered with the engine's other calls)."""
         check(self.eng.L.cnhe_graph_launch(self.h))
 
+    def slots(self):
+        """The graph's key positions: the distinct key slots its recorded key switches read, ascending (include/cnhe.h, cnhe_graph_slots)."""
+        n = C.c_int32()
+        check(self.eng.L.cnhe_graph_slots(self.h, None, 0, C.byref(n)))
+        out = (C.c_int32 * max(n.value, 1))()
+        check(self.eng.L.cnhe_graph_slots(self.h, out, n.value, C.byref(n)))
+        return list(out[:n.value])
+
+    def bind(self, slots):
+        """From the next launch on, key position i (slots()[i]) reads key slot slots[i]'s keys (include/cnhe.h, cnhe_graph_bind)."""
+        arr = (C.c_int32 * max(len(slots), 1))(*[int(s) for s in slots])
+        check(self.eng.L.cnhe_graph_bind(self.h, arr, len(slots)))
+
     def info(self):
         """dict(kernel_nodes, device_bytes): the graph's kernel nodes and the device memory it owns."""
         kn, nb = C.c_uint64(), C.c_uint64()

@@ -546,11 +546,23 @@ class B200BfvFactory:
         (the serve_batch path, ApplyBatch per layer).  The chain runs once eagerly on the examples first, so that the layers build their
         long-lived state outside the graph.  Runs must use the same shapes, scales and key slots; the network's prepared weights
         and the factory's keys are read in place and must outlive the capture.  The example matrices become the graph's inputs: every Run
-        writes its inputs' words into them, so they belong to the capture until it is disposed."""
+        writes its inputs' words into them, so they belong to the capture until it is disposed.  Run serves any client of the factory: it
+        binds the graph's key switches to the key slots its inputs carry (include/cnhe.h, cnhe_graph_bind)."""
         return CapturedInference(self, net, example_inputs)
 
     def Dispose(self):
         self.engine.close()
+
+
+def graph_binding(positions, recorded, current):
+    """The slots to bind a recorded graph's key positions to (include/cnhe.h, cnhe_graph_bind): input vector j was recorded in key slot
+    recorded[j] and its replacement belongs to slot current[j], so position recorded[j] is bound to current[j].  A position no input was
+    recorded in keeps its own slot.  Raises when one recorded slot would be bound to two slots."""
+    to = {}
+    for r, c in zip(recorded, current):
+        if to.setdefault(r, c) != c:
+            raise Exception("the inputs bind recorded key slot %d to two key slots (%d and %d)" % (r, to[r], c))
+    return [to.get(p, p) for p in positions]
 
 
 class CapturedInference:
@@ -576,6 +588,8 @@ class CapturedInference:
                 layer.Prepare()
                 layer.layerPrepared = True
         self.inputs = examples
+        # the key slot of every example vector as recorded: Run binds each to the slot of the input vector that takes its place
+        self.recorded_slots = [v.vec.key_slot for m in examples for v in m.vectors]
         eng = factory.engine
         # One eager pass first: layers build long-lived state (bias vectors, scalar-MAC plans) on their first Apply.  Built while recording,
         # it would sit in graph memory that holds no words until a launch -- and never, if the recording is refused -- and later eager
@@ -590,6 +604,8 @@ class CapturedInference:
             eng.capture_abort()
             raise
         self.outputs = ms
+        self.positions = self.graph.slots()  # the graph's key positions, and the slots they are bound to
+        self.bound = list(self.positions)
 
     def _apply(self, chain, inputs):
         """the layers on the input matrices, each intermediate disposed once read (as serve_batch and GetNext do: while recording, later
@@ -615,12 +631,37 @@ class CapturedInference:
 
     def Run(self, inputs):
         """Assigns `inputs` (shaped as the example inputs: one matrix, or a list of one per client) to the recorded inputs, launches the
-        graph and returns the output matrix (or list of them).  Asynchronous like any other call; reading the outputs orders after it."""
+        graph and returns the output matrix (or list of them).  Asynchronous like any other call; reading the outputs orders after it.
+        The inputs may belong to other clients than the examples did: the graph is bound to their key slots (graph_binding) and the outputs
+        report them.  Inputs that would bind one recorded key slot to two clients, or that a bind or the assignment refuses, leave the
+        graph's binding and the recorded inputs' key slots as they were."""
         ms = list(inputs) if self.batch else [inputs]
         if len(ms) != len(self.inputs) or any(len(m.vectors) != len(i.vectors) for m, i in zip(ms, self.inputs)):
             raise Exception("the inputs are not shaped as the recorded ones")
         eng = self.factory.engine
-        eng.vecs_assign([v.vec for m in self.inputs for v in m.vectors], [v.vec for m in ms for v in m.vectors])
+        src = [v.vec for m in ms for v in m.vectors]
+        dst = [v.vec for m in self.inputs for v in m.vectors]
+        slots = [v.key_slot for v in src]
+        binding = graph_binding(self.positions, self.recorded_slots, slots)
+        tags = [d.key_slot for d in dst]
+        self.graph.bind(binding)
+        try:
+            for d, s in zip(dst, slots):
+                if d.key_slot != s:
+                    d.set_key_slot(s)
+            eng.vecs_assign(dst, src)
+        except BaseException:
+            # a refused assignment leaves the graph's binding and the recorded inputs' key slots as they were (as far as the slots they
+            # were bound to still exist)
+            try:
+                self.graph.bind(self.bound)
+                for d, t in zip(dst, tags):
+                    if d.key_slot != t:
+                        d.set_key_slot(t)
+            except Exception:  # noqa: BLE001 -- the assignment's error is the one to report
+                pass
+            raise
+        self.bound = binding
         self.graph.launch()
         return list(self.outputs) if self.batch else self.outputs[0]
 

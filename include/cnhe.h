@@ -381,17 +381,34 @@ int cnhe_layer_activation_conv_dense(cnhe_ctx *, const cnhe_vec *const *in, int 
 
 /* ---- recording and replaying a chain of calls as one CUDA graph -------------------------------------------------- */
 /* A latency-bound inference (one LoLa image) spends its time launching hundreds of small kernels and preparing their arguments on the
- * host.  Recorded once, for fixed shapes, key slots and prepared weights, the same chain replays as one graph launch per input: the same
- * sm_90a kernels in the same order with the same arguments, and no host work between them.
+ * host.  Recorded once, for fixed shapes and prepared weights, the same chain replays as one graph launch per input: the same sm_90a
+ * kernels in the same order with the same arguments, and no host work between them.  Its key switches read their keys through the
+ * graph's key binding, so one recording serves every client of the context (cnhe_graph_bind).
  * cnhe_capture_begin: from now on the context records its calls instead of running them (CNHE_ERR_STATE while already recording, and
  *   CNHE_ERR_INVALID while profiling or the noise trace is on).  Works with "multi_stream" 0 and 1: the channel streams fork from the
  *   capturing stream and join it through events, as cnhe_context_fork_streams / cnhe_context_join_streams order them.
  * cnhe_capture_end: instantiates what was recorded into *out.  cnhe_capture_abort: drops the recording (a no-op when not recording); the
  *   context stays usable.
  * cnhe_graph_launch: enqueues one replay on the context's streams -- asynchronous and ordered with the calls before and after it, like any
- *   other call.  CNHE_ERR_STATE when a key slot a recorded key switch reads has since been removed or had its keys replaced (key generation
- *   or import), and while the context records.  Each launch adds the recorded operation counts to cnhe_op_counts and the recorded kernel
+ *   other call.  CNHE_ERR_STATE when a key slot the graph is bound to has since been removed or had its keys replaced (key generation
+ *   or import) -- binding it again reads the new keys -- and while the context records.  Each launch adds the recorded operation counts to cnhe_op_counts and the recorded kernel
  *   count to cnhe_kernel_launch_count: per-inference figures match the eager calls'.  Recording itself counts nothing.
+ * cnhe_graph_slots: the graph's key positions -- the distinct key slots its recorded key switches read, in ascending slot number -- into
+ *   slots[0 .. min(cap, *n)), their number into *n (slots may be NULL).
+ * cnhe_graph_bind: binds key position i to key slot slots[i] (n = the number of positions, CNHE_ERR_INVALID otherwise): from the next
+ *   launch on, every recorded key switch that read position i's keys -- relinearisation keys (u64 or 48-bit packed) and Galois keys -- reads
+ *   slot slots[i]'s keys of the same kind instead.  Several positions may be bound to one slot.  The recording is the first binding (every
+ *   position bound to itself), so a graph never bound behaves as recorded.  Before changing anything the call checks that each slot is live
+ *   (CNHE_ERR_INVALID) and holds every key its position's key switches read, per plaintext channel: the relinearisation keys in the form
+ *   recorded and each recorded Galois element (CNHE_ERR_STATE naming the slot and the element otherwise).  A refused bind leaves the
+ *   previous binding in force; refused while the context records.  A launch reads the bound slots' keys as they were when bound.  Binds and
+ *   launches are ordered like any call: launches bound to different clients may be enqueued back to back without a host synchronisation,
+ *   and each reads its own binding.  A bind allocates no device memory.
+ *   Vectors created while recording report, and are key-switched and decrypted under, the slot their slot's position is bound to
+ *   (cnhe_vec_key_slot).  The recorded input vectors predate the recording: retag them (cnhe_vec_set_key_slot) before cnhe_vecs_assign.
+ *   Rotation hop plans and the choice of key-switch path stay as recorded: a client holding the recording client's Galois elements gets,
+ *   word for word, its eager inference's ciphertexts; a client holding more elements follows the recorded (possibly longer) hop plan, whose
+ *   results decrypt to the same values but whose words can differ from an eager run, which plans from that client's own elements.
  * cnhe_graph_info: the graph's kernel nodes and the device bytes it owns (either pointer may be NULL).
  * cnhe_graph_destroy: waits for the context's queued work and releases the graph (CNHE_ERR_STATE while the context records).  Destroy every
  *   graph before its context.
@@ -424,6 +441,8 @@ int cnhe_capture_begin(cnhe_ctx *);
 int cnhe_capture_end(cnhe_ctx *, cnhe_graph **out);
 int cnhe_capture_abort(cnhe_ctx *);
 int cnhe_graph_launch(cnhe_graph *);
+int cnhe_graph_slots(const cnhe_graph *, int *slots, int cap, int *n);
+int cnhe_graph_bind(cnhe_graph *, const int *slots, int n);
 int cnhe_graph_info(const cnhe_graph *, uint64_t *kernel_nodes, uint64_t *device_bytes);
 int cnhe_graph_destroy(cnhe_graph *);
 int cnhe_vecs_assign(cnhe_ctx *, cnhe_vec *const *dst, const cnhe_vec *const *src, int n);

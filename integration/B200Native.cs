@@ -138,6 +138,8 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_end(IntPtr a0, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_abort(IntPtr a0);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_launch(IntPtr a0);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_slots(IntPtr a0, int[] slots, int cap, out int n);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_bind(IntPtr a0, int[] slots, int n);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_info(IntPtr a0, out ulong kernel_nodes, out ulong device_bytes);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_destroy(IntPtr a0);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_assign(IntPtr a0, IntPtr[] dst, IntPtr[] src, int n);
@@ -596,15 +598,52 @@ namespace HEWrapper
             Cnhe.Check(Cnhe.cnhe_capture_end(Ctx, out var graph));
             return graph;
         }
-        /// One replay of a Capture graph: `inputs` are copied into the vectors the recording read as its inputs (same shapes, scales and
-        /// key slots), then the graph is launched.  The recorded outputs hold this run's words until the next Run.
+        /// One replay of a Capture graph: `inputs` are copied into the vectors the recording read as its inputs (same shapes and scales),
+        /// then the graph is launched.  The inputs may belong to other clients (key slots) than the recorded ones: the graph is bound to
+        /// their slots first (include/cnhe.h, cnhe_graph_bind), and the recorded inputs and outputs report them.  The slots the recorded
+        /// inputs carry at a graph's first Run are taken as the ones it was recorded in.  The recorded outputs hold this run's words until
+        /// the next Run.
         public void Run(IntPtr graph, IVector[] recordedInputs, IVector[] inputs)
         {
             if (recordedInputs.Length != inputs.Length) throw new Exception("the inputs are not shaped as the recorded ones");
-            Cnhe.Check(Cnhe.cnhe_vecs_assign(Ctx, Cnhe.Handles(recordedInputs), Cnhe.Handles(inputs), inputs.Length));
+            IntPtr[] dst = Cnhe.Handles(recordedInputs), src = Cnhe.Handles(inputs);
+            if (!recordedSlots.TryGetValue(graph, out var recorded))
+                recordedSlots[graph] = recorded = dst.Select(KeySlot).ToArray();
+            int[] current = src.Select(KeySlot).ToArray();
+            Cnhe.Check(Cnhe.cnhe_graph_bind(graph, GraphBinding(graph, recorded, current), GraphSlots(graph).Length));
+            for (int i = 0; i < dst.Length; i++)
+                if (KeySlot(dst[i]) != current[i]) Cnhe.Check(Cnhe.cnhe_vec_set_key_slot(dst[i], current[i]));
+            Cnhe.Check(Cnhe.cnhe_vecs_assign(Ctx, dst, src, inputs.Length));
             Cnhe.Check(Cnhe.cnhe_graph_launch(graph));
         }
-        public void DisposeCapture(IntPtr graph) => Cnhe.Check(Cnhe.cnhe_graph_destroy(graph));
+        readonly Dictionary<IntPtr, int[]> recordedSlots = new Dictionary<IntPtr, int[]>();
+        static int KeySlot(IntPtr v) { Cnhe.Check(Cnhe.cnhe_vec_key_slot(v, out int s)); return s; }
+        static int[] GraphSlots(IntPtr graph)
+        {
+            Cnhe.Check(Cnhe.cnhe_graph_slots(graph, null, 0, out int n));
+            var slots = new int[n];
+            Cnhe.Check(Cnhe.cnhe_graph_slots(graph, slots, n, out n));
+            return slots;
+        }
+        /// The slot each key position of `graph` is bound to when recorded input j (recorded in slot recorded[j]) takes an input of slot
+        /// current[j]; a position no input was recorded in keeps its own slot.  Throws, before anything changes, when one recorded slot would
+        /// be bound to two slots.
+        static int[] GraphBinding(IntPtr graph, int[] recorded, int[] current)
+        {
+            var to = new Dictionary<int, int>();
+            for (int j = 0; j < recorded.Length; j++)
+            {
+                if (to.TryGetValue(recorded[j], out int c) && c != current[j])
+                    throw new Exception($"the inputs bind recorded key slot {recorded[j]} to two key slots ({c} and {current[j]})");
+                to[recorded[j]] = current[j];
+            }
+            return GraphSlots(graph).Select(p => to.TryGetValue(p, out int s) ? s : p).ToArray();
+        }
+        public void DisposeCapture(IntPtr graph)
+        {
+            recordedSlots.Remove(graph);
+            Cnhe.Check(Cnhe.cnhe_graph_destroy(graph));
+        }
         /// CryptoTracker.TestBudget (CryptoTracker.cs:41-52)
         public int NoiseBudget(IVector v, int channel = 0, int block = 0)
         {
