@@ -93,9 +93,11 @@ __global__ void __launch_bounds__(256) k_behz_tensor_fp(const u64 *a, const u64 
 // a [n_out T][2][kt][N] (the column operands, streamed once), b [T][2][kt][N] (shared by every output), d [n_out][3][kt][N] in
 // k_behz_tensor_fp's layout.  One thread per (output, residue, coefficient pair) keeps the six sums in registers.  CTA order: output
 // fastest, then the 512-coefficient tile, then the residue -- the CTAs of one (l, tile) run together and read the shared b words through
-// L2, as k_diag_mac orders its giant steps.  Arithmetic as in k_ks_mac_fp: fmodmul of canonical or lazy operands (the lazy forward output's
-// A^2 p < 2^51 bound of fp_schedule), dadd, re-centred after every 8th term (d1 gains two fresh products, <= 1.02 p, per term: 8.7 p at
-// most between re-centrings) and at the end, so the outputs are within the inverse transform's input bound (|.| <= 0.51 p < 1.25 p).
+// L2, as k_diag_mac orders its giant steps.  Arithmetic: fmodmul of canonical or lazy operands, |r| <= p/2 + |a b| 2^-52 (the rounding of
+// h pinv): below 0.625 p for canonical operands (p < 2^49), below 0.95 p for the lazy forward output (A^2 p < 0.9 * 2^51, fp_schedule
+// re-centres the output otherwise).  dadd, re-centred after every 8th term and at the end: d1 gains two products per term, so a carry
+// (<= p/2 + 1) and 8 terms stay below 15.7 p < 2^53 (10.5 p on canonical operands); without the in-loop re-centre 17 coherent terms of
+// about p pass 2^53 (tests/fp64_accumulators.py).  The outputs are re-centred, within the inverse transform's input bound (1.25 p).
 template <bool LAZY>
 __global__ void __launch_bounds__(256) k_behz_tensor_mac_fp(const u64 *__restrict__ a, const u64 *__restrict__ b, u64 *__restrict__ d, int n_out,
                                                            int T, int logn, const __grid_constant__ BehzConstF F) {

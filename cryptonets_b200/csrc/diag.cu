@@ -54,8 +54,10 @@ __global__ void __launch_bounds__(256) k_diag_gather(const u64 *__restrict__ val
 // dhat: the wave's lifted diagonals in NTT form [nd][k][N]; xhat: the baby-step ciphertexts in NTT form [2 n1][B][2][k][N], canonical.
 // One thread per (g, l, i) keeps CB clients' two accumulators in registers, so a diagonal word is loaded once for CB clients and both
 // polynomials (B > CB: once per CB clients).  The CTAs of one (l, coefficient tile) are consecutive over g: the giant steps of a wave read
-// the same baby-step words at about the same time, and those reads are served by L2.  Arithmetic as in k_ks_mac_fp: fmodmul products of
-// canonical operands (|.| <= 0.51 q), summed with dadd and re-centred every 8 terms.
+// the same baby-step words at about the same time, and those reads are served by L2.  Arithmetic: fmodmul products of canonical operands
+// a, w < q < 2^49, |r| <= q/2 + a w 2^-52 < 0.625 q (the rounding of h pinv moves r past q/2), summed with dadd and re-centred after
+// every 8th term and at the end.  A re-centred carry (<= q/2 + 1) and 8 products stay below 5.5 q < 2^52, inside the 2^53 range of exact
+// double sums; without the in-loop re-centre 33 coherent products of about q/2 pass 2^53 (tests/fp64_accumulators.py models the sum).
 template <int CB>
 __global__ void __launch_bounds__(256) k_diag_mac(const u64 *__restrict__ dhat, const u64 *__restrict__ xhat, const int *__restrict__ g_start,
                                                   const int *__restrict__ xsel, u64 *__restrict__ acc, int ng, int B, int logn,
@@ -80,7 +82,7 @@ __global__ void __launch_bounds__(256) k_diag_mac(const u64 *__restrict__ dhat, 
                     a[cb][1] = __dadd_rn(a[cb][1], fmodmul(u2d(xs[cb * ct + kN]), d, p, pinv));
                 }
             }
-            if (((j - j0) & 7) == 7) { // sums of 8 fresh products stay below 4.1 q; re-centre before they could leave the exact range
+            if (((j - j0) & 7) == 7) { // a carry and 8 fresh products stay below 5.5 q; re-centre before they could leave the exact range
 #pragma unroll
                 for (int cb = 0; cb < CB; cb++) {
                     a[cb][0] = frecenter(a[cb][0], p, pinv);
@@ -122,7 +124,7 @@ __device__ __forceinline__ void diag_mac_pair(double (&a)[CB][2][2], const u64 *
 // before its first product, so they are in flight together with the baby-step loads the compiler hoists (4 and 8 took more registers
 // and were no faster, DESIGN.md 4.10).  CTA order as in k_diag_mac (g fastest, then the 512-coefficient tile, then l).  Per
 // (g, client, l, i) the arithmetic is k_diag_mac's in the same order: fmodmul of canonical operands, dadd, re-centred after every 8th term
-// and at the end, fsmall_u -- so the outputs are bit-identical.
+// and at the end (below 5.5 q < 2^52 in between, as there), fsmall_u -- so the outputs are bit-identical.
 template <int CB>
 __global__ void __launch_bounds__(256) k_diag_mac_resident(const u64 *__restrict__ dhat, const u64 *__restrict__ xhat, const int *__restrict__ g_start,
                                                            const int *__restrict__ xsel, u64 *__restrict__ acc, int ng, int B, int logn,
