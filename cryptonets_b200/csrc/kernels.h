@@ -200,6 +200,18 @@ cudaError_t launch_galois(const u64 *in, u64 *out_base, u64 *perm_c1, int n, u64
 cudaError_t launch_galois_gather(const u64 *const *in_ptrs, u64 *out_base, u64 *perm_c1, int n, u64 elt_inv, int k, int logn, const BehzConst *bc,
                                  cudaStream_t s);
 
+// ---- modulus switch (BFV mod_switch_to_next, applied k - k_out times): out [n][2][k_out][N] from in[c] [2][k][N], coefficient form,
+// canonical words.  Dropping prime j maps every residue i < j to (x_i - (r mod q_i) + (floor(q_j / 2) mod q_i)) q_j^-1 mod q_i with
+// r = (x_j + floor(q_j / 2)) mod q_j: round(x / q_j) on the representative x of [0, q).  Any order of widths, q_l < 2^61.
+struct ModSwitchConst {
+    int k, k_out;
+    DMod q[KMAX];
+    u64 half[KMAX];               // floor(q_j / 2)
+    u64 half_mod[KMAX][KMAX];     // [j][i]: floor(q_j / 2) mod q_i
+    u64 inv[KMAX][KMAX], inv_s[KMAX][KMAX]; // [j][i]: q_j^-1 mod q_i and its Shoup quotient
+};
+cudaError_t launch_mod_switch(const u64 *const *in, u64 *out, int n, int logn, const ModSwitchConst &M, cudaStream_t s);
+
 // ---- K4: out[m] = sum_k w[m][k] * in[gather[m][k]] (+ Delta*bias[m] on coefficient 0 of c0)
 // polys: polynomials per ciphertext, 2, or 3 for size-3 products (the sum is linear in each polynomial); every MAC launcher takes it
 struct MacTile {

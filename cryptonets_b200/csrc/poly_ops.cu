@@ -554,4 +554,42 @@ cudaError_t launch_fill_zero(u64 *p, size_t words, cudaStream_t s) {
     return cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- modulus switch (Evaluator::mod_switch_scale_to_next, BFV)
+// One thread per coefficient of one polynomial: its k words are read once, the primes k-1 .. k_out are dropped in registers, and its
+// k_out words are written once.  Every index into x is a compile-time constant after unrolling, so x stays in registers.
+__global__ void __launch_bounds__(256) k_mod_switch(const u64 *const *__restrict__ in, u64 *out, int n, int logn,
+                                                   const __grid_constant__ ModSwitchConst M) {
+    const size_t N = (size_t)1 << logn;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)n * 2 * N) return;
+    const size_t poly = i >> logn, x = i & (N - 1), c = poly >> 1, part = poly & 1;
+    const u64 *src = in[c] + part * M.k * N + x;
+    u64 v[KMAX];
+#pragma unroll
+    for (int l = 0; l < KMAX; l++) v[l] = l < M.k ? src[(size_t)l * N] : 0;
+#pragma unroll
+    for (int j = KMAX - 1; j >= 1; j--) {
+        if (j >= M.k || j < M.k_out) continue;
+        u64 r = v[j] + M.half[j]; // (x_j + floor(q_j / 2)) mod q_j: both terms below q_j < 2^61
+        if (r >= M.q[j].p) r -= M.q[j].p;
+#pragma unroll
+        for (int l = 0; l < KMAX - 1; l++) {
+            if (l >= j) continue;
+            const u64 p = M.q[l].p;
+            const u64 d = addmod(submod(v[l], reduce64(r, M.q[l]), p), M.half_mod[j][l], p);
+            const u64 y = mul_shoup_lazy(d, M.inv[j][l], M.inv_s[j][l], p);
+            v[l] = y >= p ? y - p : y;
+        }
+    }
+    u64 *dst = out + (c * 2 + part) * M.k_out * N + x;
+#pragma unroll
+    for (int l = 0; l < KMAX; l++)
+        if (l < M.k_out) dst[(size_t)l * N] = v[l];
+}
+cudaError_t launch_mod_switch(const u64 *const *in, u64 *out, int n, int logn, const ModSwitchConst &M, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    k_mod_switch<<<blocks_for(((size_t)n * 2) << logn), 256, 0, s>>>(in, out, n, logn, M);
+    return cudaGetLastError();
+}
+
 } // namespace cnhe

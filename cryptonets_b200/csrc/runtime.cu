@@ -1,5 +1,6 @@
 // Host runtime of libcnhe (see runtime.h).  Product code: builds every table with hostmath.h, never touches oracle/.
 #include "runtime.h"
+#include <atomic>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -588,6 +589,8 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     if (device < 0 || device >= ndev) throw Error(-1, "bad device ordinal");
     std::unique_ptr<Context> cp(new Context());
     Context &c = *cp;
+    static std::atomic<uint64_t> serials{0};
+    c.serial = c.root = ++serials;
     c.device = device;
     CNHE_CUDA(cudaSetDevice(device));
     c.N = N; c.logN = logN; c.k = k; c.P = P; c.dbc_relin = dbc_relin; c.dbc_galois = dbc_galois;
@@ -1954,5 +1957,106 @@ void op_keys_load_compact(Context &c, KeySet &dst, int sets, const std::vector<u
 
 void keys_generate(Context &c, u64 seed) { keys_generate_impl(c, false, seed); }
 void keys_generate_secure(Context &c) { keys_generate_impl(c, true, 0); }
+
+// ---------------------------------------------------------------- levels (DESIGN 4.17)
+Context *context_derive(Context &p, int k) {
+    if (k < 1 || k >= p.k) throw Error(-1, "a derived level needs 1 <= k < the parent's coefficient prime count");
+    std::unique_ptr<Context> cp(context_create(p.t.data(), p.P, p.N, p.q.data(), k, p.dbc_relin, p.dbc_galois, p.device));
+    Context &c = *cp;
+    c.root = p.root;
+    c.h_bc.centered_mtilde = c.h_bf.centered_mtilde = p.h_bc.centered_mtilde;
+    CNHE_CUDA(cudaMemcpy(c.d_bc, &c.h_bc, sizeof(BehzConst), cudaMemcpyHostToDevice));
+    CNHE_CUDA(cudaMemcpy(c.d_bf, &c.h_bf, sizeof(BehzConstF), cudaMemcpyHostToDevice));
+    c.chunk = p.chunk;
+    c.multi_stream = p.multi_stream;
+    c.galois_elts = p.galois_elts;
+    // a seeded (test) sampler is inherited, so that the child encrypts as a seeded context on q[:k] would; a secure channel keeps the
+    // fresh OS key context_create drew, so parent and child never share encryption randomness
+    for (int ci = 0; ci < p.P; ci++)
+        if (!p.ch[ci].rng.secure) c.ch[ci].rng = p.ch[ci].rng;
+    c.clients.resize(p.clients.size());
+    for (int s = 0; s <= (int)p.clients.size(); s++) restrict_keys(c, p, s);
+    return cp.release();
+}
+// Key (i, j) of a key-switching key is an encryption of 2^{jw} target on residue i only; its rows < k encrypt the same under q[:k], and the
+// digits of residues < k are the first D' (residue-major): [D][2][k_src][N] -> [D'][2][k][N] is one strided copy
+void restrict_keys(Context &dst, const Context &src, int s) {
+    const size_t N = dst.N, kN = (size_t)dst.k * N, skN = (size_t)src.k * N;
+    dst.keys_changed(s); // a graph recorded in dst against the slot's previous keys refuses to launch
+    if (s > 0) {
+        if ((size_t)s > dst.clients.size()) dst.clients.resize(s);
+        dst.clients[s - 1].clear();
+        if (!src.slot_live(s)) {
+            dst.origin[s] = src.key_origin(s);
+            return;
+        }
+        dst.clients[s - 1].resize(dst.P);
+    }
+    auto cut = [&](const BufRef &from, size_t rows) { // rows of k_src N words -> rows of k N words
+        BufRef to = dst.alloc(rows * kN);
+        CNHE_CUDA(cudaMemcpy2DAsync(to->p, kN * 8, from->p, skN * 8, kN * 8, rows, cudaMemcpyDeviceToDevice, dst.stream));
+        return to;
+    };
+    for (int ci = 0; ci < dst.P; ci++) {
+        dst.set_channel(ci);
+        const KeySet &from = src.keys(ci, s);
+        KeySet &to = s == 0 ? static_cast<KeySet &>(dst.ch[ci]) : dst.clients[s - 1][ci];
+        to.have_rlk = false;
+        to.rlk.reset();
+        to.rlk_packed.reset();
+        to.glk.clear();
+        if (s == 0) {
+            const Channel &fc = src.ch[ci];
+            Channel &tc = dst.ch[ci];
+            tc.have_sk = fc.have_sk && fc.sk;
+            tc.have_pk = fc.have_pk && fc.pk;
+            tc.sk = tc.have_sk ? cut(fc.sk, 1) : nullptr;
+            tc.pk = tc.have_pk ? cut(fc.pk, 2) : nullptr;
+        }
+        for (const auto &g : from.glk) to.glk[g.first] = cut(g.second, (size_t)dst.dm_galois.D * 2);
+        if (from.have_rlk && from.rlk) {
+            to.rlk = cut(from.rlk, (size_t)dst.dm_relin.D * 2);
+            rlk_ready(dst, to); // synchronises the stream
+        }
+        CNHE_CUDA(cudaStreamSynchronize(dst.stream));
+    }
+    dst.set_channel(0);
+    dst.origin[s] = src.key_origin(s);
+}
+void op_mod_switch(Context &src, Context &dst, int ch, const std::vector<const u64 *> &in, u64 *out) {
+    ModSwitchConst M;
+    memset(&M, 0, sizeof(M));
+    M.k = src.k;
+    M.k_out = dst.k;
+    for (int l = 0; l < src.k; l++) {
+        M.q[l] = make_dmod(src.q[l]);
+        M.half[l] = src.q[l] >> 1;
+    }
+    for (int j = dst.k; j < src.k; j++)
+        for (int i = 0; i < j; i++) {
+            const u64 qi = src.q[i];
+            M.half_mod[j][i] = M.half[j] % qi;
+            M.inv[j][i] = hm::inv(src.q[j] % qi, qi);
+            M.inv_s[j][i] = hm::shoup(M.inv[j][i], qi);
+        }
+    const cudaStream_t ss = src.streams[src.multi_stream ? ch : 0];
+    dst.set_channel(ch);
+    cudaEvent_t ready, done;
+    CNHE_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+    CNHE_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+    CNHE_CUDA(cudaEventRecord(ready, ss)); // the inputs are complete on the source's stream
+    CNHE_CUDA(cudaStreamWaitEvent(dst.stream, ready, 0));
+    const size_t in_words = (size_t)2 * src.k * dst.N, out_words = (size_t)2 * dst.k * dst.N;
+    const int wave = dst.wave(in_words + out_words);
+    for (int c0 = 0; c0 < (int)in.size(); c0 += wave) {
+        const int m = std::min<int>(wave, (int)in.size() - c0);
+        const std::vector<const u64 *> part(in.begin() + c0, in.begin() + c0 + m);
+        dst.check(launch_mod_switch(upload_ptrs(dst, part), out + (size_t)c0 * out_words, m, dst.logN, M, dst.stream), "mod_switch");
+    }
+    CNHE_CUDA(cudaEventRecord(done, dst.stream)); // the source's later use (and release) of the inputs waits for the kernel
+    CNHE_CUDA(cudaStreamWaitEvent(ss, done, 0));
+    cudaEventDestroy(ready);
+    cudaEventDestroy(done);
+}
 
 } // namespace cnhe

@@ -138,7 +138,19 @@ struct Context {
     const KeySet &keys(int channel, int s) const;
     // key generation of a slot: bumped whenever its keys are replaced or removed, so that a graph recorded against them refuses to launch
     std::map<int, uint64_t> key_gen;
-    void keys_changed(int s) { key_gen[s]++; }
+    void keys_changed(int s) { key_gen[s]++; origin.erase(s); }
+
+    // ---- levels (DESIGN 4.17).  A context made by context_derive holds the first k' of its parent's coefficient primes; every context
+    // of one family shares `root`, the serial of the context created from parameters.  The keys of a slot are named by their origin:
+    // (serial, key generation) of the context whose own keys they are, carried along when they are restricted into a derived context
+    uint64_t serial = 0, root = 0;
+    std::map<int, std::pair<uint64_t, uint64_t>> origin; // slots whose keys were restricted from another context of the family
+    std::pair<uint64_t, uint64_t> key_origin(int s) const {
+        const auto it = origin.find(s);
+        if (it != origin.end()) return it->second;
+        const auto g = key_gen.find(s);
+        return {serial, g == key_gen.end() ? 0 : g->second};
+    }
 
     // ---- graph recording (vec.cu, cnhe_capture_*).  `api`: the public call in progress, named in refusals
     std::unique_ptr<Recording> rec;
@@ -266,6 +278,16 @@ struct WsScope {                  // temporaries allocated inside the scope are 
 };
 
 Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *coeff, int k, int dbc_relin, int dbc_galois, int device);
+// A context on the first k of parent's coefficient primes (1 <= k < parent.k), created as context_create creates one on them, that starts
+// with the parent's options and the restriction of every key slot's keys (restrict_keys)
+Context *context_derive(Context &parent, int k);
+// Makes slot s of dst (fewer primes, same family) hold the restriction of src's slot s keys: the secret key and each key-switching key
+// cut to its rows and digits of residues < dst.k, the public key to its rows; a slot src does not hold is emptied.  Returns once the copies
+// and the packed relinearisation keys are complete.
+void restrict_keys(Context &dst, const Context &src, int s);
+// out [n][2][dst.k][N] (dst's memory) = the n ciphertexts in[c] of src ([2][src.k][N], coefficient form) with primes src.k-1 .. dst.k
+// dropped (launch_mod_switch), on dst's stream `ch`: that stream first waits for src's stream `ch`, and src's stream waits for the kernel
+void op_mod_switch(Context &src, Context &dst, int ch, const std::vector<const u64 *> &in, u64 *out);
 std::vector<u64> default_coeff_modulus(uint32_t N);
 
 // ---- keys

@@ -385,6 +385,16 @@ extern "C" int cnhe_keys_set_seed(cnhe_ctx *h, int channel, uint64_t seed) {
 extern "C" int cnhe_keys_export(cnhe_ctx *h, int channel, int what, uint64_t arg, uint64_t *dst, size_t cap) {
     API_BEGIN(h)
     not_recorded(c, "returns words to the host");
+    if (what == 4) { // the packed relinearisation keys the fused key switch reads
+        if (channel < 0 || channel >= c.P) fail("bad channel");
+        const BufRef &pk = c.ch[channel].rlk_packed;
+        if (!pk) throw Error(CNHE_ERR_STATE, "the channel holds no packed relinearization keys");
+        const size_t words = (size_t)c.dm_relin.D * 2 * c.k * c.N * 6 / 8;
+        if (cap < words) fail("destination too small");
+        CNHE_CUDA(cudaMemcpyAsync(dst, pk->p, words * 8, cudaMemcpyDeviceToHost, c.stream));
+        c.sync();
+        return CNHE_OK;
+    }
     size_t words;
     BufRef &b = key_slot(c, channel, what, arg, words, false);
     if (cap < words) fail("destination too small");
@@ -1319,6 +1329,62 @@ extern "C" int cnhe_context_remove_client(cnhe_ctx *h, int slot) {
     c.sync(); // no queued key switch still reads the keys
     c.clients[slot - 1].clear();
     c.keys_changed(slot);
+    API_END
+}
+// ---------------------------------------------------------------------------------------------------- levels (DESIGN 4.17)
+extern "C" int cnhe_context_derive_level(cnhe_ctx *h, int k, cnhe_ctx **out) {
+    API_BEGIN(h)
+    not_recorded(c, "creates a context");
+    if (!out) fail("null argument");
+    if (k < 1 || k >= c.k) fail("cnhe_context_derive_level: need 1 <= k < the context's coefficient prime count");
+    c.sync(); // the parent's keys are complete
+    std::unique_ptr<Context> child(context_derive(c, k));
+    *out = new cnhe_ctx{child.release()};
+    API_END
+}
+extern "C" int cnhe_vecs_mod_switch(cnhe_ctx *h, const cnhe_vec *const *in, int n, cnhe_ctx *to, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (!to || to == h || !in || !out || n < 1) fail("bad arguments");
+    Context &d = *to->c;
+    // root and k never change after creation: checked before the second lock, so every call that takes it locks the context with more
+    // primes first, and two switches of one family cannot wait on each other's locks
+    if (d.root != c.root || d.k >= c.k) fail("cnhe_vecs_mod_switch: the destination must be a level of the same context family with fewer primes");
+    std::lock_guard<std::recursive_mutex> lock_to(d.mu);
+    // the switch spans two contexts' streams and key slots: it cannot be part of either context's graph
+    not_recorded(c, "switches vectors to another context's level");
+    if (d.rec) {
+        end_recording(d, false);
+        throw Error(CNHE_ERR_STATE, "cnhe_vecs_mod_switch: the destination context records a graph; a switch between levels cannot be recorded "
+                                    "(the recording was aborted)");
+    }
+    for (int i = 0; i < n; i++) {
+        same_ctx(c, in[i]); // a pending vector is relinearised here
+        if (!in[i]->enc) fail("cnhe_vecs_mod_switch: only encrypted vectors switch levels");
+    }
+    const std::vector<int> slots = vec_slots(c, in, n);
+    CNHE_CUDA(cudaSetDevice(d.device));
+    d.set_channel(0);
+    d.slot = 0;
+    ws_release_all(d);
+    for (int s : std::set<int>(slots.begin(), slots.end()))
+        if (d.key_origin(s) != c.key_origin(s)) restrict_keys(d, c, s);
+    size_t total = 0;
+    for (int i = 0; i < n; i++) total += in[i]->blocks;
+    std::vector<BufRef> slab(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        d.set_channel(ch);
+        slab[ch] = d.alloc(total * d.ct_words());
+        std::vector<const u64 *> ptrs;
+        for (int i = 0; i < n; i++)
+            for (int b = 0; b < in[i]->blocks; b++) ptrs.push_back(in[i]->block(ch, b));
+        op_mod_switch(c, d, ch, ptrs, slab[ch]->p);
+    }
+    d.set_channel(0);
+    size_t ct = 0;
+    for (int i = 0; i < n; i++) {
+        out[i] = slab_output(d, slab, ct, in[i], in[i]->scale, slots[i]);
+        ct += in[i]->blocks;
+    }
     API_END
 }
 extern "C" int cnhe_vec_set_key_slot(cnhe_vec *v, int slot) {

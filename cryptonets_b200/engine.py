@@ -233,6 +233,10 @@ class Engine:
             cm = _u64(coeff_moduli)
             check(self.L.cnhe_context_create_custom(_p(pp), len(pp), N, _p(cm), len(cm), dbc_relin, dbc_galois, device, C.byref(h)))
         self.h = h
+        self._describe(pp)
+
+    def _describe(self, pp):
+        """Reads the context's parameters into attributes (pp: its plaintext primes)."""
         n, k, P, rd, gd, ge = C.c_uint32(), C.c_int(), C.c_int(), C.c_int(), C.c_int(), C.c_int()
         check(self.L.cnhe_context_info(self.h, C.byref(n), C.byref(k), C.byref(P), C.byref(rd), C.byref(gd), C.byref(ge)))
         self.N, self.k, self.P = n.value, k.value, P.value
@@ -351,6 +355,27 @@ class Engine:
     def remove_client(self, slot):
         check(self.L.cnhe_context_remove_client(self.h, int(slot)))
 
+    # ---- levels (include/cnhe.h, cnhe_context_derive_level; DESIGN 4.17)
+    def derive_level(self, k):
+        """A new Engine on the first k coefficient primes of this one, holding the restriction of its keys and of every key slot's.  The
+        two engines are independent afterwards; vectors move down with mod_switch."""
+        h = C.c_void_p()
+        check(self.L.cnhe_context_derive_level(self.h, int(k), C.byref(h)))
+        child = Engine.__new__(Engine)
+        child.L = self.L
+        child._live = weakref.WeakSet()
+        child.h = h
+        child._describe(np.array(self.primes, np.uint64))
+        return child
+
+    def mod_switch(self, vecs, to):
+        """The encrypted vectors `vecs` of this engine switched to engine `to` (a level of the same family with fewer primes): every
+        ciphertext drops the primes it has beyond to.k.  Outputs keep dimension, scale, format and key slot."""
+        n = len(vecs)
+        out = (VECP * n)()
+        check(self.L.cnhe_vecs_mod_switch(self.h, _vec_array(vecs), n, to.h, out))
+        return to._wrap_many(out, n, like=vecs)
+
     def write_vector(self, vec):
         """EncryptedSealBfvVector.Write: the text form of one vector."""
         n = C.c_size_t()
@@ -373,7 +398,7 @@ class Engine:
 
     def _key_words(self, what):
         kN = self.k * self.N
-        return {0: kN, 1: 2 * kN, 2: self.relin_digits * 2 * kN, 3: self.galois_digits * 2 * kN}[what]
+        return {0: kN, 1: 2 * kN, 2: self.relin_digits * 2 * kN, 3: self.galois_digits * 2 * kN, 4: self.relin_digits * 2 * kN * 6 // 8}[what]
 
     def export_key(self, channel, what, arg=0):
         a = np.zeros(self._key_words(what), np.uint64)

@@ -476,6 +476,41 @@ class B200BfvFactory:
     def GetMatrix(self, vectors, fmt, CopyVectors=True):
         return B200BfvMatrix(self, vectors, fmt, CopyVectors=CopyVectors)
 
+    # ---- levels (include/cnhe.h, cnhe_context_derive_level; DESIGN 4.17)
+    CoeffModulusCount = property(lambda s: s.engine.k)
+
+    def AtLevel(self, k):
+        """The factory of this one's level on its first k coefficient primes (the restriction of its keys and key slots), made once and
+        cached; k equal to this factory's count is the factory itself."""
+        if k == self.engine.k:
+            return self
+        levels = self.__dict__.setdefault("_levels", {})
+        if k not in levels:
+            f = B200BfvFactory.__new__(B200BfvFactory)
+            f.engine = self.engine.derive_level(k)
+            f._env = B200BfvEnvironment(f)
+            f.bigFactor, f.preComputedCoefficients = self.bigFactor, self.preComputedCoefficients
+            levels[k] = f
+        return levels[k]
+
+    def ModSwitch(self, m, level_factory):
+        """An encrypted matrix or vector of this factory switched to level_factory (AtLevel), every ciphertext on fewer primes."""
+        return self.ModSwitchBatch([m], level_factory)[0]
+
+    def ModSwitchBatch(self, items, level_factory):
+        """ModSwitch of several matrices or vectors (possibly of different clients) in one pass."""
+        vecs = [v.vec for it in items for v in (it.vectors if isinstance(it, B200BfvMatrix) else [it])]
+        out, i, res = self.engine.mod_switch(vecs, level_factory.engine), 0, []
+        for it in items:
+            if isinstance(it, B200BfvMatrix):
+                n = len(it.vectors)
+                res.append(B200BfvMatrix(level_factory, [B200BfvVector(level_factory, o) for o in out[i:i + n]], it.Format, CopyVectors=False))
+            else:
+                n = 1
+                res.append(B200BfvVector(level_factory, out[i]))
+            i += n
+        return res
+
     # ---- wire formats (IFactory.cs:474-495; SEAL streams unpinned, see csrc/wire.cu)
     def Save(self, target, withPrivateKeys=False):
         """IFactory.Save(stream | fileName, withPrivateKeys): the ZIP key archive."""
@@ -551,6 +586,8 @@ class B200BfvFactory:
         return CapturedInference(self, net, example_inputs)
 
     def Dispose(self):
+        for f in self.__dict__.get("_levels", {}).values():
+            f.Dispose()
         self.engine.close()
 
 

@@ -277,6 +277,35 @@ class TimingLayer(BaseLayer):
         return m
 
 
+class ModSwitchLayer(BaseLayer):
+    """Switches the ciphertexts to the first CoeffModulusCount coefficient primes (BFV modulus switching, DESIGN 4.17): every later layer
+    prepares and runs on the level factory Source.Factory.AtLevel(CoeffModulusCount), whose key switches and products cost less.  The
+    values are unchanged as long as the noise budget left clears the level's floors (tools/level_plan.py).  A factory without levels
+    (RawFactory) passes the matrix through."""
+
+    def __init__(self, **kw):
+        self.CoeffModulusCount = None
+        super().__init__(**kw)
+
+    @property
+    def Factory(self):
+        f = BaseLayer.Factory.fget(self)
+        return f.AtLevel(self.CoeffModulusCount) if hasattr(f, "AtLevel") else f
+
+    @Factory.setter
+    def Factory(self, f):
+        self._factory = f
+
+    def Apply(self, m):
+        return self.ApplyBatch([m])[0]
+
+    def ApplyBatch(self, ms):
+        f = BaseLayer.Factory.fget(self)
+        if not hasattr(f, "ModSwitchBatch"):
+            return list(ms)
+        return f.ModSwitchBatch(ms, self.Factory)
+
+
 class SquareActivation(BaseLayer):
     """`NeuralNetworks/SquareActivation.cs:8-20`"""
 

@@ -11,7 +11,7 @@ import numpy as np
 
 from .interfaces import EVectorFormat
 from .layers import (ConvolutionEngine, EncryptLayer, LLConvReader, LLDenseLayer, LLDuplicateLayer, LLInterleavedDenseLayer, LLInterleaveLayer,
-                     LLPackedDenseLayer, LLPoolLayer, LLPreConvLayer, LLSingleLineReader, LLVectorizeLayer, MatrixSource, PoolLayer,
+                     LLPackedDenseLayer, LLPoolLayer, LLPreConvLayer, LLSingleLineReader, LLVectorizeLayer, MatrixSource, ModSwitchLayer, PoolLayer,
                      SquareActivation, TimingLayer)
 
 _MODELS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "models")
@@ -79,9 +79,10 @@ def cryptonets_mnist(factory, images, batch_size=None, fused=True, weights=None,
     return net, reader
 
 
-def lola_small(factory, images, weights=None, dense_method="rows"):
+def lola_small(factory, images, weights=None, dense_method="rows", levels=None):
     """dense_method: LLDenseLayer.Method of the 10 x 845 score layer ("rows", the reference's, or "folded": dense scores in one
-    ciphertext per plaintext prime)."""
+    ciphertext per plaintext prime).  levels: {layer: k'} switches to k' coefficient primes after the named layers (conv1, vec2, act3)."""
+    lv = _Levels(levels, ["conv1", "vec2", "act3"])
     w = weights or lola_small_weights()
     weightscale = 64
     reader = LLConvReader(images, Scale=16.0, NormalizationFactor=1.0 / 256.0, InputShape=[28, 28], KernelShape=[5, 5], Stride=[2, 2],
@@ -89,10 +90,37 @@ def lola_small(factory, images, weights=None, dense_method="rows"):
     enc = EncryptLayer(Source=reader, Factory=factory)
     conv1 = LLPoolLayer(Source=enc, InputShape=[28, 28], KernelShape=[5, 5], Upperpadding=[1, 1], Stride=[2, 2], MapCount=[5, 1],
                         WeightsScale=weightscale, Weights=w["Weights_0"])
-    vec2 = LLVectorizeLayer(Source=conv1)
-    act3 = SquareActivation(Source=vec2)
-    dense4 = LLDenseLayer(Source=act3, Bias=w["Biases_1"], Weights=w["Weights_1"], WeightsScale=weightscale, Method=dense_method)
+    vec2 = LLVectorizeLayer(Source=lv("conv1", conv1))
+    act3 = SquareActivation(Source=lv("vec2", vec2))
+    dense4 = LLDenseLayer(Source=lv("act3", act3), Bias=w["Biases_1"], Weights=w["Weights_1"], WeightsScale=weightscale, Method=dense_method)
     return dense4, reader
+
+
+# Level schedules ({layer: k'}) for the parameters of each network's end-to-end GPU test (tools/level_bench.py NETS): the output of
+# `python tools/level_bench.py trace` on an H100 80GB HBM3 (700 W): budgets of one seeded inference at the full level, planned by
+# tools/level_plan.py with its 7-bit margin.  lola_small (k = 4, budgets 123 / 99 / 61 after conv1 / vec2 / act3) has nothing to drop:
+# its floors at 3 primes sit below every budget plus the margin.  CryptoNets-MNIST takes no levels.
+LEVEL_SCHEDULES = {
+    "lola": {"dense5": 4, "act7": 3},                               # k = 5; budgets after dense5, act7: 92, 39 bits
+    "lola_dense": {"act4": 7, "dense6": 6, "act7": 5, "inter8": 4},  # k = 8; 221, 169, 125, 85
+    "lola_large": {"act3": 7, "dense4": 5, "act5": 4},              # k = 8; 210, 123, 79
+    "lola_cifar": {"act3": 8, "dense4": 5, "act5": 4},              # k = 9; 232, 127, 73
+}
+
+
+class _Levels:
+    """The `levels` argument of a network: {local layer name: k'} inserts a ModSwitchLayer to k' coefficient primes after that layer."""
+
+    def __init__(self, levels, names):
+        self.levels = dict(levels or {})
+        unknown = sorted(set(self.levels) - set(names))
+        if unknown:
+            raise ValueError("levels names layers the network does not have: %s (its layers: %s)" % (unknown, ", ".join(names)))
+
+    def __call__(self, name, layer):
+        layer.LevelName = name  # the name a schedule gives this layer (tools/level_bench.py traces budgets under it)
+        k = self.levels.get(name)
+        return layer if k is None else ModSwitchLayer(Source=layer, CoeffModulusCount=k)
 
 
 def serve_batch(net, inputs):
@@ -119,8 +147,10 @@ def serve_batch(net, inputs):
     return ms
 
 
-def lola(factory, images, weights=None):
-    """LoLa (`LowLatencyCryptoNets/LoLaCryptonets.cs:203-276`): im2col input, 8-way packed dense layer, interleave, square, dense."""
+def lola(factory, images, weights=None, levels=None):
+    """LoLa (`LowLatencyCryptoNets/LoLaCryptonets.cs:203-276`): im2col input, 8-way packed dense layer, interleave, square, dense.
+    levels: {layer: k'} switches to k' coefficient primes after the named layers (conv1 .. act7)."""
+    lv = _Levels(levels, ["conv1", "vec2", "act3", "dup4", "dense5", "inter6", "act7"])
     w = weights or cryptonets_weights()
     weightscale = 32
     reader = LLConvReader(images, Scale=16.0, NormalizationFactor=1.0 / 256.0, InputShape=[28, 28], KernelShape=[5, 5], Stride=[2, 2],
@@ -128,38 +158,40 @@ def lola(factory, images, weights=None):
     enc = EncryptLayer(Source=reader, Factory=factory)
     conv1 = LLPoolLayer(Source=enc, InputShape=[28, 28], KernelShape=[5, 5], Upperpadding=[1, 1], Stride=[2, 2], MapCount=[5, 1],
                         WeightsScale=weightscale, Weights=w["Weights_0"])
-    vec2 = LLVectorizeLayer(Source=conv1)
-    act3 = SquareActivation(Source=vec2)
-    dup4 = LLDuplicateLayer(Source=act3, Count=8)
-    dense5 = LLPackedDenseLayer(Source=dup4, Weights=transpose(w["Weights_1"], 5 * 13 * 13, 100), Bias=w["Biases_2"],
+    vec2 = LLVectorizeLayer(Source=lv("conv1", conv1))
+    act3 = SquareActivation(Source=lv("vec2", vec2))
+    dup4 = LLDuplicateLayer(Source=lv("act3", act3), Count=8)
+    dense5 = LLPackedDenseLayer(Source=lv("dup4", dup4), Weights=transpose(w["Weights_1"], 5 * 13 * 13, 100), Bias=w["Biases_2"],
                                 WeightsScale=weightscale * weightscale, PackingCount=8, PackingShift=1024)
     sel = [1023 + i * 1024 for i in range(8)]
-    inter6 = LLInterleaveLayer(Source=dense5, Shift=-1, SelectedIndices=sel)
-    act7 = SquareActivation(Source=inter6)
-    dense8 = LLInterleavedDenseLayer(Source=act7, Weights=w["Weights_3"], Bias=w["Biases_3"], WeightsScale=weightscale, Shift=-1,
+    inter6 = LLInterleaveLayer(Source=lv("dense5", dense5), Shift=-1, SelectedIndices=sel)
+    act7 = SquareActivation(Source=lv("inter6", inter6))
+    dense8 = LLInterleavedDenseLayer(Source=lv("act7", act7), Weights=w["Weights_3"], Bias=w["Biases_3"], WeightsScale=weightscale, Shift=-1,
                                      SelectedIndices=sel)
     return dense8, reader
 
 
-def lola_dense(factory, images, weights=None):
+def lola_dense(factory, images, weights=None, levels=None):
     """LoLa-Dense (`LoLaCryptonets.cs:116-201`): the image arrives as ONE ciphertext; the im2col columns are built homomorphically
-    (LLPreConvLayer), 16-way packed dense layer, square, interleave, dense."""
+    (LLPreConvLayer), 16-way packed dense layer, square, interleave, dense.  levels: {layer: k'} switches to k' coefficient primes after
+    the named layers (pre1 .. inter8)."""
+    lv = _Levels(levels, ["pre1", "conv2", "vec3", "act4", "dup5", "dense6", "act7", "inter8"])
     w = weights or cryptonets_weights()
     weightscale = 32
     reader = LLSingleLineReader(images, Scale=16.0, NormalizationFactor=1.0 / 256.0)
     enc = EncryptLayer(Source=reader, Factory=factory)
     pre1 = LLPreConvLayer(Source=enc, InputShape=[28, 28], KernelShape=[5, 5], Upperpadding=[1, 1], Stride=[2, 2], UseAxisForBlocks=[True, True])
-    conv2 = LLPoolLayer(Source=pre1, InputShape=[28, 28], KernelShape=[5, 5], Upperpadding=[1, 1], Stride=[2, 2], MapCount=[5, 1],
+    conv2 = LLPoolLayer(Source=lv("pre1", pre1), InputShape=[28, 28], KernelShape=[5, 5], Upperpadding=[1, 1], Stride=[2, 2], MapCount=[5, 1],
                         WeightsScale=weightscale, Weights=w["Weights_0"], HotIndices=pre1.HotIndices)
-    vec3 = LLVectorizeLayer(Source=conv2)
-    act4 = SquareActivation(Source=vec3)
-    dup5 = LLDuplicateLayer(Source=act4, Count=16)
-    dense6 = LLPackedDenseLayer(Source=dup5, Weights=pre1.RearrangeWeights(transpose(w["Weights_1"], 5 * 13 * 13, 100)), Bias=w["Biases_2"],
+    vec3 = LLVectorizeLayer(Source=lv("conv2", conv2))
+    act4 = SquareActivation(Source=lv("vec3", vec3))
+    dup5 = LLDuplicateLayer(Source=lv("act4", act4), Count=16)
+    dense6 = LLPackedDenseLayer(Source=lv("dup5", dup5), Weights=pre1.RearrangeWeights(transpose(w["Weights_1"], 5 * 13 * 13, 100)), Bias=w["Biases_2"],
                                 WeightsScale=weightscale * weightscale, PackingCount=16, PackingShift=1024)
-    act7 = SquareActivation(Source=dense6)
+    act7 = SquareActivation(Source=lv("dense6", dense6))
     sel = [1023 + i * 1024 for i in range(16)]
-    inter8 = LLInterleaveLayer(Source=act7, Shift=-1, SelectedIndices=sel)
-    dense9 = LLInterleavedDenseLayer(Source=inter8, Weights=w["Weights_3"], Bias=w["Biases_3"], WeightsScale=weightscale, Shift=-1,
+    inter8 = LLInterleaveLayer(Source=lv("act7", act7), Shift=-1, SelectedIndices=sel)
+    dense9 = LLInterleavedDenseLayer(Source=lv("inter8", inter8), Weights=w["Weights_3"], Bias=w["Biases_3"], WeightsScale=weightscale, Shift=-1,
                                      SelectedIndices=sel)
     return dense9, reader
 
@@ -184,29 +216,31 @@ def synthetic_cifar(n_images, seed=20240917):
     return np.random.default_rng(seed).integers(0, 256, (n_images, 3 * 32 * 32)).astype(np.float64)
 
 
-def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows"):
+def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows", levels=None):
     """LoLa-CIFAR (`CifarCryptoNet/LolaCifarCryptoNet.cs:27-131`): 3x32x32 image as an im2col matrix [196 x 192], conv 83 maps,
     square, the second convolution as a 5488 x 16268 row-major dense layer (rotate-and-sum per row), square, dense 5488 -> 10.
     dense_method: LLDenseLayer.Method of that layer ("rows", the reference's, or "diagonal"); diag_ntt_bytes: its DiagonalNttBytes;
-    score_method: the Method of the score layer ("rows" or "folded")."""
+    score_method: the Method of the score layer ("rows" or "folded").  levels: {layer: k'} switches to k' coefficient primes after the
+    named layers (conv1 .. act5)."""
+    lv = _Levels(levels, ["conv1", "vec2", "act3", "dense4", "act5"])
     w = weights or cifar_weights()
     reader = LLConvReader(images, Scale=8.0, NormalizationFactor=1.0 / 256.0, InputShape=[3, 32, 32], KernelShape=[3, 8, 8], Stride=[1000, 2, 2],
                           Upperpadding=[0, 1, 1], Lowerpadding=[0, 1, 1])
     enc = EncryptLayer(Source=reader, Factory=factory)
     conv1 = LLPoolLayer(Source=enc, InputShape=[3, 32, 32], KernelShape=[3, 8, 8], Upperpadding=[0, 1, 1], Lowerpadding=[0, 1, 1],
                         Stride=[1000, 2, 2], MapCount=[83, 1, 1], WeightsScale=256.0, Weights=w["Weights_0"], Bias=w["Biases_0"])
-    vec2 = LLVectorizeLayer(Source=conv1)
-    act3 = SquareActivation(Source=vec2)
+    vec2 = LLVectorizeLayer(Source=lv("conv1", conv1))
+    act3 = SquareActivation(Source=lv("vec2", vec2))
     ce = ConvolutionEngine()
     ce.InputShape, ce.KernelShape, ce.Stride, ce.MapCount = [83, 14, 14], [83, 10, 10], [83, 2, 2], [112, 1, 1]
     ce.Upperpadding, ce.Lowerpadding = [0, 4, 4], [0, 4, 4]
     # shard = (rank, world, process group): the 5488 rows of the big dense layer are split over the ranks of ONE inference (SURVEY.md 8e);
     # every rank holds the same keys and input ciphertexts, the partial products are summed through cryptonets_b200/parallel.py
-    dense4 = LLDenseLayer(Source=act3, WeightsScale=512.0, Weights=ce.GetDenseWeights(w["Weights_1"]), Bias=ce.GetDenseBias(w["Biases_1"]),
+    dense4 = LLDenseLayer(Source=lv("act3", act3), WeightsScale=512.0, Weights=ce.GetDenseWeights(w["Weights_1"]), Bias=ce.GetDenseBias(w["Biases_1"]),
                           InputFormat=EVectorFormat.dense, ForceDenseFormat=True, Shard=shard, Method=dense_method,
                           DiagonalNttBytes=diag_ntt_bytes)
-    act5 = SquareActivation(Source=dense4)
-    dense6 = LLDenseLayer(Source=act5, Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512.0, InputFormat=EVectorFormat.dense,
+    act5 = SquareActivation(Source=lv("dense4", dense4))
+    dense6 = LLDenseLayer(Source=lv("act5", act5), Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512.0, InputFormat=EVectorFormat.dense,
                           Method=score_method)
     return dense6, reader
 
@@ -227,26 +261,28 @@ def lola_large_weights(seed=9, synthetic=False):
                 Biases_1=draw(163, 0.039, 0.09), Weights_2=draw(10 * 2608, 0.42, 1.63), Biases_2=draw(10, 1.6, 3.9))
 
 
-def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows"):
+def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows", levels=None):
     """Large LoLa (`LoLaCryptonets.cs:330-409`): 28x28 image as im2col [144 x 64], conv 83 maps of 8x8 stride 2 (pixels are NOT
     normalised; the weights carry the 1/256), square, the second convolution (163 maps of 83x6x6, stride 2 over 83x12x12) as a
     2608 x 11952 row-major dense layer with ForceDenseFormat, square, dense 2608 -> 10.  dense_method: that layer's LLDenseLayer.Method,
-    diag_ntt_bytes its DiagonalNttBytes; score_method: the Method of the score layer ("rows" or "folded")."""
+    diag_ntt_bytes its DiagonalNttBytes; score_method: the Method of the score layer ("rows" or "folded").  levels: {layer: k'} switches
+    to k' coefficient primes after the named layers (conv1 .. act5)."""
+    lv = _Levels(levels, ["conv1", "vec2", "act3", "dense4", "act5"])
     w = weights or lola_large_weights()
     reader = LLConvReader(images, Scale=16.0, NormalizationFactor=1.0, InputShape=[1, 28, 28], KernelShape=[1, 8, 8], Stride=[1000, 2, 2],
                           Upperpadding=[0, 1, 1], Lowerpadding=[0, 1, 1])
     enc = EncryptLayer(Source=reader, Factory=factory)
     conv1 = LLPoolLayer(Source=enc, InputShape=[1, 28, 28], KernelShape=[1, 8, 8], Upperpadding=[0, 1, 1], Lowerpadding=[0, 1, 1],
                         Stride=[1000, 2, 2], MapCount=[83, 1, 1], WeightsScale=4096, Weights=np.asarray(w["Weights_0"]) / 256.0, Bias=w["Biases_0"])
-    vec2 = LLVectorizeLayer(Source=conv1)
-    act3 = SquareActivation(Source=vec2)
+    vec2 = LLVectorizeLayer(Source=lv("conv1", conv1))
+    act3 = SquareActivation(Source=lv("vec2", vec2))
     ce = ConvolutionEngine()
     ce.InputShape, ce.KernelShape, ce.Stride, ce.MapCount = [83, 12, 12], [83, 6, 6], [83, 2, 2], [163, 1, 1]
     ce.Padding = [False, False, False]
-    dense4 = LLDenseLayer(Source=act3, WeightsScale=64, Weights=ce.GetDenseWeights(w["Weights_1"]), Bias=ce.GetDenseBias(w["Biases_1"]),
+    dense4 = LLDenseLayer(Source=lv("act3", act3), WeightsScale=64, Weights=ce.GetDenseWeights(w["Weights_1"]), Bias=ce.GetDenseBias(w["Biases_1"]),
                           InputFormat=EVectorFormat.dense, ForceDenseFormat=True, Method=dense_method,
                           DiagonalNttBytes=diag_ntt_bytes)
-    act5 = SquareActivation(Source=dense4)
-    dense6 = LLDenseLayer(Source=act5, Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512, InputFormat=EVectorFormat.dense,
+    act5 = SquareActivation(Source=lv("dense4", dense4))
+    dense6 = LLDenseLayer(Source=lv("act5", act5), Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512, InputFormat=EVectorFormat.dense,
                           Method=score_method)
     return dense6, reader

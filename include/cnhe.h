@@ -87,7 +87,9 @@ int cnhe_context_fork_streams(cnhe_ctx *);
 int cnhe_keys_generate_secure(cnhe_ctx *);
 int cnhe_keys_generate(cnhe_ctx *, uint64_t seed);
 /* what: 0 secret key [k][N] (NTT form), 1 public key [2][k][N], 2 relin keys [D][2][k][N], 3 Galois key of element
- * `arg` [D][2][k][N].  Stand-in for the SEAL key streams of SaveToStream/LoadFromStream ("AtomicSealBfvVector.cs:93-130"). */
+ * `arg` [D][2][k][N]; export only: 4 the relin keys' packed copy the fused key switch reads (48-bit words, D 2 k N 6 / 8 words;
+ * CNHE_ERR_STATE where the context keeps none: the fused key switch does not run or some q_l >= 2^48).  Stand-in for the SEAL key
+ * streams of SaveToStream/LoadFromStream ("AtomicSealBfvVector.cs:93-130"). */
 int cnhe_keys_export(cnhe_ctx *, int channel, int what, uint64_t arg, uint64_t *dst, size_t cap_words);
 int cnhe_keys_import(cnhe_ctx *, int channel, int what, uint64_t arg, const uint64_t *src, size_t words);
 int cnhe_keys_set_seed(cnhe_ctx *, int channel, uint64_t seed); /* TESTS ONLY: later encryptions of that channel use the deterministic sampler */
@@ -154,6 +156,23 @@ int cnhe_context_add_client_compact(cnhe_ctx *, const uint8_t *blob, size_t len,
 int cnhe_context_remove_client(cnhe_ctx *, int slot);
 int cnhe_vec_set_key_slot(cnhe_vec *, int slot);
 int cnhe_vec_key_slot(const cnhe_vec *, int *slot);
+/* Levels (modulus switching, SEAL's mod_switch_to_next for BFV; DESIGN 4.17).  cnhe_context_derive_level creates in *out a context on
+ * the first k coefficient primes of this one (1 <= k < its k, else CNHE_ERR_INVALID): the same plaintext primes, N, decomposition bit
+ * counts, device and Galois element list, with the tables, BEHZ base and options a context created on q_0..q_{k-1} would have, and the
+ * options behz_centered_mtilde, chunk and multi_stream copied.  Its keys are the restriction of this context's: the secret and public
+ * keys' rows l < k, and of every key-switching key the digits of residues l < k with their rows l < k -- word for word the keys a seeded
+ * context on q_0..q_{k-1} generates.  Every live key slot is restricted too; a context without a secret key (cnhe_context_load_compact)
+ * derives as well.  A seeded channel sampler is inherited.  The two contexts are independent afterwards: either may be destroyed first.
+ * cnhe_vecs_mod_switch writes in out[i] vector in[i] of context `from` switched to context `to`, which must be a level of the same
+ * family (derived from the same created context, directly or through other levels) with fewer primes: every ciphertext drops the primes
+ * q_{k-1} .. q_{k'} one at a time, x -> round(x / q_j) mod q_0..q_{j-1}, in one pass over its words.  Encrypted vectors only; a
+ * pending (deferred-relinearisation) vector is relinearised first.  Outputs keep dimension, scale, format and key slot, one slab per
+ * channel; a slot whose keys in `from` were added or replaced since `to` was derived is restricted into `to` first, under the same
+ * number.  Counts no operation.  `to`'s streams wait for the inputs and `from`'s streams for the switch.  CNHE_ERR_INVALID for vectors
+ * of another context, plain vectors or an unrelated / not smaller `to`; CNHE_ERR_STATE while either context records a graph (the
+ * recording is aborted). */
+int cnhe_context_derive_level(cnhe_ctx *, int k, cnhe_ctx **out);
+int cnhe_vecs_mod_switch(cnhe_ctx *from, const cnhe_vec *const *in, int n, cnhe_ctx *to, cnhe_vec **out /*n*/);
 int cnhe_vec_write(cnhe_ctx *, const cnhe_vec *, char *dst, size_t cap, size_t *needed);
 int cnhe_vec_read(cnhe_ctx *, const char *text, size_t len, cnhe_vec **out, size_t *consumed);
 

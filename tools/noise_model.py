@@ -42,9 +42,10 @@ class Model:
         self.ks_relin = self.ks_peak(rec["dbc"])
         self.ks_gal = self.ks_peak(rec["dbc_galois"])
 
-    def ks_peak(self, w):  # log2 of the peak of the key-switching noise (invariant, i.e. times t/q)
+    def ks_peak(self, w, q=None):  # log2 of the peak of the key-switching noise (invariant, i.e. times t/q), at q or a prefix of it
+        q = self.q if q is None else q
         ss = 0.0
-        for p in self.q:
+        for p in q:
             bits = p.bit_length()
             sh = 0
             while sh < bits:
@@ -52,7 +53,12 @@ class Model:
                 ss += 4.0 ** b / 3.0
                 sh += w
         rms = SIGMA * math.sqrt(self.N * ss)
-        return math.log2(self.c * rms) + math.log2(self.t) - self.logq
+        return math.log2(self.c * rms) + math.log2(self.t) - math.log2(prod(q))
+
+    def switch_peak(self, logq_prime):
+        """log2 of the peak invariant noise a modulus switch to q' adds: t/q' times the rounding r0 + r1 s, |r_i| <= 1/2 uniform, whose
+        coefficients have rms sqrt(1/12 + N (2/3) / 12) ~ sqrt(N / 18)"""
+        return math.log2(self.c * math.sqrt(self.N / 18.0)) + math.log2(self.t) - logq_prime
 
     @staticmethod
     def peak(budget):  # log2 peak from a budget
