@@ -131,6 +131,7 @@ _SIGS = {
     "cnhe_raw_elapsed_ms": [C.c_void_p, C.POINTER(C.c_float)],
     "cnhe_kernel_launch_count": [C.c_void_p],
     "cnhe_capture_begin": [C.c_void_p],
+    "cnhe_capture_begin_levels": [C.c_void_p, C.POINTER(C.c_void_p), C.c_int],
     "cnhe_capture_end": [C.c_void_p, C.POINTER(C.c_void_p)],
     "cnhe_capture_abort": [C.c_void_p],
     "cnhe_graph_launch": [C.c_void_p],

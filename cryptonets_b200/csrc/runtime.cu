@@ -234,35 +234,60 @@ void release_deferred(Context &c, const std::vector<Recording::Deferred> &d) {
         b.upload_slot = x.upload_slot;
     }
 }
-cudaGraph_t end_recording(Context &c, bool keep, std::vector<Recording::Deferred> *hold) {
-    std::unique_ptr<Recording> r = std::move(c.rec);
-    // every channel stream joins the capturing stream 0 again (a capture cannot end with a stream left out); errors here only mean the
-    // capture was already invalidated, which cudaStreamEndCapture reports
-    for (size_t i = 1; i < c.streams.size(); i++) {
-        cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
-        if (cudaStreamIsCapturing(c.streams[i], &st) == cudaSuccess && st == cudaStreamCaptureStatusActive &&
-            cudaEventRecord(c.ev_join, c.streams[i]) == cudaSuccess)
-            cudaStreamWaitEvent(c.streams[0], c.ev_join, 0);
-    }
-    cudaGraph_t g = nullptr;
-    if (cudaStreamEndCapture(c.streams[0], &g) != cudaSuccess) g = nullptr;
-    for (cudaStream_t s : c.streams) { // a stream of an invalidated capture may still be in it
-        cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
-        if (cudaStreamIsCapturing(s, &st) == cudaSuccess && st != cudaStreamCaptureStatusNone) {
-            cudaGraph_t stray = nullptr;
-            if (cudaStreamEndCapture(s, &stray) == cudaSuccess && stray) cudaGraphDestroy(stray);
+cudaGraph_t end_capture(RecGroup &grp, bool keep) {
+    const cudaStream_t s0 = grp.members[0]->streams[0];
+    // every channel stream of every member joins the capturing stream 0 again (a capture cannot end with a stream left out); errors here
+    // only mean the capture was already invalidated, which cudaStreamEndCapture reports
+    for (Context *m : grp.members) {
+        cudaSetDevice(m->device);
+        for (cudaStream_t s : m->streams) {
+            cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+            if (s != s0 && cudaStreamIsCapturing(s, &st) == cudaSuccess && st == cudaStreamCaptureStatusActive &&
+                cudaEventRecord(m->ev_join, s) == cudaSuccess)
+                cudaStreamWaitEvent(s0, m->ev_join, 0);
         }
     }
+    cudaSetDevice(grp.members[0]->device);
+    cudaGraph_t g = nullptr;
+    if (cudaStreamEndCapture(s0, &g) != cudaSuccess) g = nullptr;
+    for (Context *m : grp.members)
+        for (cudaStream_t s : m->streams) { // a stream of an invalidated capture may still be in it
+            cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+            if (cudaStreamIsCapturing(s, &st) == cudaSuccess && st != cudaStreamCaptureStatusNone) {
+                cudaGraph_t stray = nullptr;
+                if (cudaStreamEndCapture(s, &stray) == cudaSuccess && stray) cudaGraphDestroy(stray);
+            }
+        }
     (void)cudaGetLastError();
     if (g && !keep) { cudaGraphDestroy(g); g = nullptr; }
+    return g;
+}
+void end_part(Context &c, std::vector<Recording::Deferred> *hold) {
+    std::unique_ptr<Recording> r = std::move(c.rec);
+    cudaSetDevice(c.device);
     for (int i = 0; i < Context::OP_COUNT; i++) c.op_count[i] = r->op0[i]; // recording runs nothing
     c.launches = r->launches0;
     r->arena->recording = false;
     r->arena->free.clear();
     ws_release_all(c); // the last recorded call's temporaries go back to the graph's memory, not to the driver
-    if (hold && g) *hold = std::move(r->deferred);
+    if (hold) *hold = std::move(r->deferred);
     else release_deferred(c, r->deferred);
-    return g;
+}
+void abort_recording(Context &c) {
+    const std::shared_ptr<RecGroup> grp = c.rec->group;
+    std::vector<Context *> locked;
+    bool all = true;
+    for (Context *m : grp->members) {
+        if (m == &c) continue;
+        if (!m->mu.try_lock()) { all = false; break; }
+        locked.push_back(m);
+    }
+    if (all) {
+        end_capture(*grp, false);
+        for (Context *m : grp->members) end_part(*m);
+    } else grp->abort_requested = true;
+    for (Context *m : locked) m->mu.unlock();
+    cudaSetDevice(c.device);
 }
 
 static std::vector<BufRef> &temps_of(Context &c) { return c.temps; } // per context, guarded by the context mutex
@@ -365,7 +390,7 @@ struct ProfScope {
 #define PROF(family, bytes) ProfScope prof_scope_##__LINE__(c, family, bytes)
 Context::~Context() {
     cudaSetDevice(device);
-    if (rec) end_recording(*this, false);
+    if (rec) abort_recording(*this);
     for (cudaStream_t s : streams) cudaStreamSynchronize(s);
     if (copy_stream) cudaStreamSynchronize(copy_stream);
     recycle_on = false; // buffers released from here on go straight back to the driver
@@ -1007,8 +1032,8 @@ static KsKeys pick_keys(Context &c, int ch, int n, const int *slots, int kind, u
     auto take = [&](int s, const u64 *&key, const u64 *&pk) {
         pick(c.keys(ch, s), key, pk);
         if (!c.rec) return;
-        c.rec->keys->seen[key] = {s, ch, kind, elt};
-        if (pk) c.rec->keys->seen[pk] = {s, ch, KeyBinding::RLK_PACKED, 0};
+        c.rec->keys->seen[key] = {s, ch, kind, elt, c.rec->member};
+        if (pk) c.rec->keys->seen[pk] = {s, ch, KeyBinding::RLK_PACKED, 0, c.rec->member};
     };
     if (slots) {
         bool uniform = true;

@@ -4,6 +4,7 @@
 #pragma once
 #include <cstdint>
 #include <algorithm>
+#include <atomic>
 #include <map>
 #include <unordered_map>
 #include <memory>
@@ -67,7 +68,7 @@ typedef std::shared_ptr<DevBuf> BufRef;
 // the same kind, and the next launch copies the words into the table before the recorded kernels read them.
 struct KeyBinding {
     enum Kind { RLK, RLK_PACKED, GALOIS };
-    struct Key { int slot, channel, kind; u64 elt; };
+    struct Key { int slot, channel, kind; u64 elt; int member; }; // member: the enlisted context whose key pick took it (RecGroup)
     std::map<const u64 *, Key> seen;      // while recording: every key base picked for a key switch, and which key it is
     std::map<const u64 *, size_t> word;   // key base -> its table word
     std::vector<Key> words;               // the key each table word stands for, in the order they were handed out
@@ -78,13 +79,24 @@ struct KeyBinding {
     const u64 *ref(const u64 *base);      // the key reference of a key base picked while recording
 };
 
+// The contexts one recording spans (cnhe_capture_begin_levels; one context for cnhe_capture_begin): the capture runs on members[0]'s
+// stream 0, and every channel stream of every member forks from it.  Members are ordered by descending prime count, the order their
+// locks are taken in.  abort_requested: a refused call found another member's lock taken (a call in flight on another thread), so the
+// recording could not end at once; the recording thread's next call on any member ends it.
+struct RecGroup {
+    std::vector<struct Context *> members;
+    std::atomic<bool> abort_requested{false};
+};
+
 // State of a context while it records its calls into a CUDA graph (stream capture of the channel streams, vec.cu cnhe_capture_*)
 struct Recording {
     std::thread::id thread;             // the recording thread: calls from any other thread are refused
-    std::shared_ptr<GraphArena> arena;
+    std::shared_ptr<RecGroup> group;    // the contexts of the recording, shared by every member's Recording
+    int member = 0;                     // this context's index in group->members
+    std::shared_ptr<GraphArena> arena;  // shared by every member
     std::vector<uint64_t> op0;          // operation counters and kernel count when the recording began: restored when it ends, the
     uint64_t launches0 = 0;             // difference is what every launch of the graph adds
-    std::shared_ptr<KeyBinding> keys;   // the references the recorded key switches read their keys through
+    std::shared_ptr<KeyBinding> keys;   // the references the recorded key switches read their keys through (shared by every member)
     std::vector<std::shared_ptr<void>> keep; // cached host-built device tables (scalar-MAC plans) the recorded kernels read
     // buffers allocated before the recording and released during it: the graph may read them, so they are freed (or recycled) outside
     // it, when the graph is destroyed (at once when the recording is aborted)
@@ -263,10 +275,16 @@ struct Context {
     void trace_gap(const char *what);
     void sync(); // waits for every channel stream; refused while recording
 };
-// ends the context's recording and returns the captured graph (nullptr when the capture failed; keep: false destroys it) and restores the
-// operation counters.  The buffers from before the recording that were released during it may still be read by the graph: they move to
-// *hold (the graph releases them when it is destroyed), or are released at once when hold is nullptr (an aborted recording)
-cudaGraph_t end_recording(Context &c, bool keep, std::vector<Recording::Deferred> *hold = nullptr);
+// ends the capture of a recording group (every member's lock held): every member's capturing streams join members[0]'s stream 0, whose
+// capture ends; returns the captured graph (nullptr when the capture failed; keep: false destroys it)
+cudaGraph_t end_capture(RecGroup &g, bool keep);
+// ends c's part of its recording once the capture has ended, and restores its operation counters.  The buffers from before the recording
+// that were released during it may still be read by the graph: they move to *hold (the graph releases them when it is destroyed), or are
+// released at once when hold is nullptr (an aborted recording)
+void end_part(Context &c, std::vector<Recording::Deferred> *hold = nullptr);
+// aborts the recording c takes part in (c's lock held), for every member: at once when every member's lock can be taken without waiting,
+// else by setting abort_requested (another thread is inside a call on a member; a capture must not end under a call that issues into it)
+void abort_recording(Context &c);
 void release_deferred(Context &c, const std::vector<Recording::Deferred> &d); // as their DevBufs would have released them
 
 void ws_release_all(Context &c); // drop every workspace temporary (call at the start of a public operation)

@@ -27,11 +27,13 @@ int set_err(int code, const std::string &m) {
 extern "C" const char *cnhe_last_error(void) { return g_err.c_str(); }
 void api_enter(Context &c, const char *name) {
     c.api = name;
-    if (c.rec && c.rec->thread != std::this_thread::get_id()) c.refuse("was called from another thread than the recording one");
+    if (!c.rec) return;
+    if (c.rec->thread != std::this_thread::get_id()) c.refuse("was called from another thread than the recording one");
+    if (c.rec->group->abort_requested) abort_recording(c); // a call refused on another thread while this one was inside a call
 }
 int api_fail(Context &c, int code, const std::string &m) {
     std::lock_guard<std::recursive_mutex> lock(c.mu);
-    if (c.rec) end_recording(c, false);
+    if (c.rec) abort_recording(c);
     return set_err(code, m);
 }
 extern "C" const char *cnhe_version(void) { return "cnhe-b200 0.3 (sm_90a)"; }
@@ -162,41 +164,75 @@ extern "C" uint64_t cnhe_kernel_launch_count(const cnhe_ctx *h) { return h ? h->
 // ---------------------------------------------------------------------------------------------------- graph recording and replay
 // The context's calls are captured from its channel streams into one CUDA graph (stream capture, relaxed mode: the record-time copies of
 // host constants and the allocations of the graph's memory happen outside the captured streams).  Channel streams fork from stream 0 when
-// the recording begins and join it before it ends, as fork_streams / join_streams order them for eager calls.
+// the recording begins and join it before it ends, as fork_streams / join_streams order them for eager calls.  A recording that enlists
+// levels (cnhe_capture_begin_levels) forks every channel stream of every level from the same stream 0, so the mod switches' event
+// hand-offs between the contexts' streams are captured like any other cross-stream order.
 struct cnhe_graph {
     cnhe_ctx *h = nullptr;
+    std::vector<Context *> members; // the contexts the recording spanned: members[0] is h's, the rest its enlisted levels (lock order)
     cudaGraphExec_t exec = nullptr;
     std::shared_ptr<GraphArena> arena;
-    std::vector<uint64_t> ops; // operation counts one launch adds
-    uint64_t launches = 0;     // kernel launches one launch adds (what the recorded calls counted)
+    std::vector<std::vector<uint64_t>> ops; // per member: the operation counts one launch adds
+    std::vector<uint64_t> launches;         // per member: the kernel launches one launch adds (what the recorded calls counted)
     uint64_t kernel_nodes = 0;
-    // key binding (cnhe_graph_bind): the key positions (recorded slots, ascending), the slot each is bound to and that slot's key
-    // generation when it was bound, and the words of the device table under that binding
+    // key binding (cnhe_graph_bind): the key positions (recorded slots, ascending), the slot each is bound to and, per member, that slot's
+    // key generation when it was bound, and the words of the device table under that binding
     std::shared_ptr<KeyBinding> keys;
     std::vector<int> positions, bound;
-    std::vector<uint64_t> bound_gen;
+    std::vector<std::vector<uint64_t>> bound_gen;
     std::vector<const u64 *> words;
     bool words_sent = false; // the device table holds `words` (or will, once the copy queued by the last launch has run)
     std::vector<std::shared_ptr<void>> keep;
-    std::vector<Recording::Deferred> held; // buffers from before the recording, released during it: the graph may read them
+    std::vector<std::vector<Recording::Deferred>> held; // per member: buffers from before the recording, released during it (the graph may read them)
 };
 static uint64_t key_gen(const Context &c, int s) {
     const auto it = c.key_gen.find(s);
     return it == c.key_gen.end() ? 0 : it->second;
 }
-// Binds key position i of g to slots[i]: checks that every slot is live and holds every key its position's references stand for, in the
-// recorded form, then (and only then) takes the binding.  The device table is rewritten by the next launch.
-static void bind_graph(Context &c, cnhe_graph &g, const int *slots) {
+typedef std::vector<std::unique_lock<std::recursive_mutex>> Locks;
+// the locks of members[1..] (the caller holds members[0]'s), taken in member order
+static Locks lock_members(const std::vector<Context *> &members) {
+    Locks l;
+    for (size_t i = 1; i < members.size(); i++) l.emplace_back(members[i]->mu);
+    return l;
+}
+// a graph call on the levels a graph spans: each is locked and entered like a public call; while one records, the call is refused and
+// that recording aborted, as a refused call on the graph's own context aborts its recording
+static Locks enter_levels(cnhe_graph &g, const char *name, const char *why) {
+    Locks l = lock_members(g.members);
+    for (size_t i = 1; i < g.members.size(); i++) {
+        Context &m = *g.members[i];
+        m.api = name;
+        if (m.rec) {
+            abort_recording(m);
+            throw Error(CNHE_ERR_STATE, std::string(name) + " " + why + ": refused while a level the graph spans records a graph (the recording was aborted)");
+        }
+        m.set_channel(0);
+        m.slot = 0;
+        ws_release_all(m);
+    }
+    return l;
+}
+// Binds key position i of g to slots[i]: checks that every slot is live, restricts into each level a slot whose keys there are not the
+// graph's context's (as the eager switch would), checks that every slot holds every key its position's references stand for in the
+// recorded form, in the context that read it, then (and only then) takes the binding.  The device table is rewritten by the next launch.
+static void bind_graph(cnhe_graph &g, const int *slots) {
+    Context &top = *g.members[0];
     const size_t np = g.positions.size();
     for (size_t i = 0; i < np; i++)
-        if (!c.slot_live(slots[i])) fail(("cnhe_graph_bind: no such key slot " + std::to_string(slots[i])).c_str());
+        if (!top.slot_live(slots[i])) fail(("cnhe_graph_bind: no such key slot " + std::to_string(slots[i])).c_str());
+    for (size_t mi = 1; mi < g.members.size(); mi++)
+        for (size_t i = 0; i < np; i++)
+            if (g.members[mi]->key_origin(slots[i]) != top.key_origin(slots[i])) restrict_keys(*g.members[mi], top, slots[i]);
     std::vector<const u64 *> words;
     for (const KeyBinding::Key &k : g.keys->words) {
         const int s = slots[std::lower_bound(g.positions.begin(), g.positions.end(), k.slot) - g.positions.begin()];
-        const KeySet &ks = c.keys(k.channel, s);
+        const Context &m = *g.members[k.member];
+        const KeySet &ks = m.keys(k.channel, s);
         auto missing = [&](const std::string &what) {
             throw Error(CNHE_ERR_STATE, "cnhe_graph_bind: key slot " + std::to_string(s) + " (plaintext channel " + std::to_string(k.channel) +
-                                            ") holds no " + what + ", which the graph reads");
+                                            (k.member ? ", level of " + std::to_string(m.k) + " primes" : std::string()) + ") holds no " + what +
+                                            ", which the graph reads");
         };
         if (k.kind == KeyBinding::GALOIS) {
             const auto it = ks.glk.find(k.elt);
@@ -207,56 +243,118 @@ static void bind_graph(Context &c, cnhe_graph &g, const int *slots) {
         } else words.push_back(k.kind == KeyBinding::RLK ? ks.rlk->p : ks.rlk_packed->p);
     }
     g.bound.assign(slots, slots + np);
-    g.bound_gen.clear();
-    for (size_t i = 0; i < np; i++) {
-        g.bound_gen.push_back(key_gen(c, slots[i]));
-        g.keys->to[g.positions[i]] = slots[i];
-    }
+    g.bound_gen.assign(g.members.size(), {});
+    for (size_t mi = 0; mi < g.members.size(); mi++)
+        for (size_t i = 0; i < np; i++) g.bound_gen[mi].push_back(key_gen(*g.members[mi], slots[i]));
+    for (size_t i = 0; i < np; i++) g.keys->to[g.positions[i]] = slots[i];
     if (words != g.words) {
         g.words = std::move(words);
         g.words_sent = false;
     }
 }
+// starts a recording on members[0] that enlists the rest (every member locked, none recording)
+static void start_recording(const std::vector<Context *> &members) {
+    Context &c = *members[0];
+    for (Context *m : members) {
+        if (m->prof) fail("cnhe_capture_begin: profiling is on (cnhe_prof_enable)");
+        if (m->trace_noise) fail("cnhe_capture_begin: the noise trace is on (option trace_noise)");
+    }
+    auto grp = std::make_shared<RecGroup>();
+    grp->members = members;
+    auto arena = std::make_shared<GraphArena>();
+    // the key binding's device table: one word for every key the members' slots hold (a recording reads each at most once)
+    auto keys = std::make_shared<KeyBinding>();
+    for (Context *m : members)
+        for (int s = 0; s <= (int)m->clients.size(); s++)
+            if (m->slot_live(s))
+                for (int ch = 0; ch < m->P; ch++) keys->cap += 2 + m->keys(ch, s).glk.size();
+    const std::vector<const u64 *> zeros(keys->cap);
+    keys->table = static_cast<const u64 **>(const_cast<void *>(arena->constant(zeros.data(), zeros.size() * sizeof(u64 *), c.copy_stream)));
+    CNHE_CUDA(cudaStreamBeginCapture(c.streams[0], cudaStreamCaptureModeRelaxed));
+    for (size_t i = 0; i < members.size(); i++) {
+        Context &m = *members[i];
+        auto r = std::make_unique<Recording>();
+        r->thread = std::this_thread::get_id();
+        r->group = grp;
+        r->member = (int)i;
+        r->arena = arena;
+        r->op0.assign(m.op_count, m.op_count + Context::OP_COUNT);
+        r->launches0 = m.launches;
+        r->keys = keys;
+        m.rec = std::move(r);
+    }
+    // every channel stream of every member joins the capture before any call: a stream left out would run its work once, now
+    CNHE_CUDA(cudaEventRecord(c.ev_join, c.streams[0]));
+    for (Context *m : members)
+        for (cudaStream_t s : m->streams)
+            if (s != c.streams[0]) CNHE_CUDA(cudaStreamWaitEvent(s, c.ev_join, 0));
+}
 extern "C" int cnhe_capture_begin(cnhe_ctx *h) {
     API_BEGIN(h)
     if (c.rec) c.refuse("cannot start a second recording");
-    if (c.prof) fail("cnhe_capture_begin: profiling is on (cnhe_prof_enable)");
-    if (c.trace_noise) fail("cnhe_capture_begin: the noise trace is on (option trace_noise)");
-    auto r = std::make_unique<Recording>();
-    r->thread = std::this_thread::get_id();
-    r->arena = std::make_shared<GraphArena>();
-    r->op0.assign(c.op_count, c.op_count + Context::OP_COUNT);
-    r->launches0 = c.launches;
-    // the key binding's device table: one word for every key the context's slots hold (a recording reads each at most once)
-    r->keys = std::make_shared<KeyBinding>();
-    for (int s = 0; s <= (int)c.clients.size(); s++)
-        if (c.slot_live(s))
-            for (int ch = 0; ch < c.P; ch++) r->keys->cap += 2 + c.keys(ch, s).glk.size();
-    const std::vector<const u64 *> zeros(r->keys->cap);
-    r->keys->table = static_cast<const u64 **>(const_cast<void *>(r->arena->constant(zeros.data(), zeros.size() * sizeof(u64 *), c.copy_stream)));
-    CNHE_CUDA(cudaStreamBeginCapture(c.streams[0], cudaStreamCaptureModeRelaxed));
-    c.rec = std::move(r);
-    c.fork_streams(); // the channel streams join the capture
+    start_recording({&c});
+    API_END
+}
+extern "C" int cnhe_capture_begin_levels(cnhe_ctx *h, cnhe_ctx *const *levels, int n) {
+    API_BEGIN(h)
+    if (n < 0 || (n > 0 && !levels)) fail("cnhe_capture_begin_levels: null argument");
+    std::vector<Context *> members{&c};
+    for (int i = 0; i < n; i++) {
+        if (!levels[i]) fail("cnhe_capture_begin_levels: null level");
+        Context *m = levels[i]->c;
+        if (m == &c) fail("cnhe_capture_begin_levels: the recording context cannot enlist itself");
+        if (std::find(members.begin(), members.end(), m) != members.end()) fail("cnhe_capture_begin_levels: a level is listed twice");
+        if (m->root != c.root) fail("cnhe_capture_begin_levels: a level of another context family");
+        if (m->k >= c.k) fail("cnhe_capture_begin_levels: a level needs fewer coefficient primes than the recording context");
+        members.push_back(m);
+    }
+    // lock order: more primes first, as cnhe_vecs_mod_switch takes them (ties by address)
+    std::sort(members.begin() + 1, members.end(), [](const Context *a, const Context *b) { return a->k != b->k ? a->k > b->k : a < b; });
+    const Locks locks = lock_members(members);
+    if (c.rec) c.refuse("cannot start a second recording");
+    for (size_t i = 1; i < members.size(); i++)
+        if (members[i]->rec) throw Error(CNHE_ERR_STATE, "cnhe_capture_begin_levels: an enlisted level already records a graph");
+    start_recording(members);
     API_END
 }
 extern "C" int cnhe_capture_abort(cnhe_ctx *h) {
     API_BEGIN(h)
-    if (c.rec) end_recording(c, false);
+    if (c.rec) abort_recording(c);
     API_END
 }
 extern "C" int cnhe_capture_end(cnhe_ctx *h, cnhe_graph **out) {
     API_BEGIN(h)
     if (!c.rec) throw Error(CNHE_ERR_STATE, "cnhe_capture_end: the context is not recording (was the recording aborted by a refused call?)");
+    if (c.rec->member != 0) c.refuse("ends a recording that began on another context (end it there)");
     if (!out) fail("null argument");
+    const std::shared_ptr<RecGroup> grp = c.rec->group;
+    const Locks locks = lock_members(grp->members);
+    if (grp->abort_requested) {
+        abort_recording(c);
+        throw Error(CNHE_ERR_STATE, "cnhe_capture_end: the recording was aborted by a call refused on another thread");
+    }
     std::unique_ptr<cnhe_graph> g(new cnhe_graph);
     g->h = h;
+    g->members = grp->members;
     g->arena = c.rec->arena;
     g->keys = c.rec->keys;
-    g->keep = c.rec->keep;
-    for (int i = 0; i < Context::OP_COUNT; i++) g->ops.push_back(c.op_count[i] - c.rec->op0[i]);
-    g->launches = c.launches - c.rec->launches0;
-    cudaGraph_t graph = end_recording(c, true, &g->held);
-    if (!graph) throw Error(CNHE_ERR_CUDA, "cnhe_capture_end: the CUDA stream capture failed");
+    for (Context *m : g->members) {
+        g->keep.insert(g->keep.end(), m->rec->keep.begin(), m->rec->keep.end());
+        std::vector<uint64_t> ops;
+        for (int i = 0; i < Context::OP_COUNT; i++) ops.push_back(m->op_count[i] - m->rec->op0[i]);
+        g->ops.push_back(std::move(ops));
+        g->launches.push_back(m->launches - m->rec->launches0);
+    }
+    cudaGraph_t graph = end_capture(*grp, true);
+    g->held.resize(g->members.size());
+    for (size_t i = 0; i < g->members.size(); i++) end_part(*g->members[i], &g->held[i]);
+    auto release_held = [&] {
+        for (size_t i = 0; i < g->members.size(); i++) release_deferred(*g->members[i], g->held[i]);
+    };
+    if (!graph) {
+        release_held();
+        throw Error(CNHE_ERR_CUDA, "cnhe_capture_end: the CUDA stream capture failed");
+    }
     size_t n = 0;
     cudaError_t e = cudaGraphGetNodes(graph, nullptr, &n);
     std::vector<cudaGraphNode_t> nodes(n);
@@ -268,7 +366,7 @@ extern "C" int cnhe_capture_end(cnhe_ctx *h, cnhe_graph **out) {
     }
     if (e == cudaSuccess) e = cudaGraphInstantiate(&g->exec, graph, 0);
     cudaGraphDestroy(graph);
-    if (e != cudaSuccess) release_deferred(c, g->held);
+    if (e != cudaSuccess) release_held();
     CNHE_CUDA(e);
     // the recording is the first binding: every position bound to itself
     g->keys->seen.clear();
@@ -276,7 +374,7 @@ extern "C" int cnhe_capture_end(cnhe_ctx *h, cnhe_graph **out) {
     std::set<int> pos;
     for (const KeyBinding::Key &k : g->keys->words) pos.insert(k.slot);
     g->positions.assign(pos.begin(), pos.end());
-    bind_graph(c, *g, g->positions.data());
+    bind_graph(*g, g->positions.data());
     *out = g.release();
     API_END
 }
@@ -291,31 +389,54 @@ extern "C" int cnhe_graph_bind(cnhe_graph *g, const int *slots, int n) {
     if (!g) return set_err(CNHE_ERR_INVALID, "null graph");
     API_BEGIN(g->h)
     not_recorded(c, "binds a recorded graph to key slots");
+    const Locks locks = enter_levels(*g, "cnhe_graph_bind", "binds a recorded graph to key slots");
     if (n != (int)g->positions.size() || (n > 0 && !slots))
         fail(("cnhe_graph_bind: the graph has " + std::to_string(g->positions.size()) + " key positions (cnhe_graph_slots), " +
               std::to_string(n) + " slots were given").c_str());
-    bind_graph(c, *g, slots);
+    bind_graph(*g, slots);
     API_END
 }
 extern "C" int cnhe_graph_launch(cnhe_graph *g) {
     if (!g) return set_err(CNHE_ERR_INVALID, "null graph");
     API_BEGIN(g->h)
     not_recorded(c, "launches a recorded graph");
-    for (size_t i = 0; i < g->bound.size(); i++) {
-        const int s = g->bound[i];
-        if (!c.slot_live(s) || key_gen(c, s) != g->bound_gen[i])
-            throw Error(CNHE_ERR_STATE, "cnhe_graph_launch: the keys of key slot " + std::to_string(s) +
-                                            " were removed or replaced after the graph was recorded or bound to it (cnhe_graph_bind)");
+    const Locks locks = enter_levels(*g, "cnhe_graph_launch", "launches a recorded graph");
+    for (size_t mi = 0; mi < g->members.size(); mi++) {
+        const Context &m = *g->members[mi];
+        for (size_t i = 0; i < g->bound.size(); i++) {
+            const int s = g->bound[i];
+            if (!m.slot_live(s) || key_gen(m, s) != g->bound_gen[mi][i])
+                throw Error(CNHE_ERR_STATE, "cnhe_graph_launch: the keys of key slot " + std::to_string(s) +
+                                                (mi ? " in the level of " + std::to_string(m.k) + " primes" : std::string()) +
+                                                " were removed or replaced after the graph was recorded or bound to it (cnhe_graph_bind)");
+        }
     }
-    c.join_streams(); // after every call queued before, on any channel
+    // after every call queued before, on any channel of any context the graph spans
+    c.join_streams();
+    for (size_t mi = 1; mi < g->members.size(); mi++) {
+        Context &m = *g->members[mi];
+        for (cudaStream_t s : m.streams) {
+            CNHE_CUDA(cudaEventRecord(m.ev_join, s));
+            CNHE_CUDA(cudaStreamWaitEvent(c.streams[0], m.ev_join, 0));
+        }
+    }
     if (!g->words_sent) { // a new binding: stream 0 orders the copy after the previous launch's kernels and before this one's
         c.h2d(g->keys->table, g->words.data(), g->words.size() * sizeof(u64 *));
         g->words_sent = true;
     }
     CNHE_CUDA(cudaGraphLaunch(g->exec, c.streams[0]));
-    c.fork_streams(); // before every call queued after
-    for (int i = 0; i < Context::OP_COUNT; i++) c.op_count[i] += g->ops[i];
-    c.launches += g->launches;
+    // before every call queued after (a level's decryption of the scores, say)
+    c.fork_streams();
+    if (g->members.size() > 1) {
+        CNHE_CUDA(cudaEventRecord(c.ev_join, c.streams[0]));
+        for (size_t mi = 1; mi < g->members.size(); mi++)
+            for (cudaStream_t s : g->members[mi]->streams) CNHE_CUDA(cudaStreamWaitEvent(s, c.ev_join, 0));
+    }
+    for (size_t mi = 0; mi < g->members.size(); mi++) {
+        Context &m = *g->members[mi];
+        for (int i = 0; i < Context::OP_COUNT; i++) m.op_count[i] += g->ops[mi][i];
+        m.launches += g->launches[mi];
+    }
     API_END
 }
 extern "C" int cnhe_graph_info(const cnhe_graph *g, uint64_t *kernel_nodes, uint64_t *device_bytes) {
@@ -329,11 +450,13 @@ extern "C" int cnhe_graph_destroy(cnhe_graph *g) {
     Context &c = *g->h->c;
     try {
         std::lock_guard<std::recursive_mutex> lock(c.mu);
-        if (c.rec) return set_err(CNHE_ERR_STATE, "cnhe_graph_destroy: refused while the context records a graph");
+        const Locks locks = lock_members(g->members);
+        for (Context *m : g->members)
+            if (m->rec) return set_err(CNHE_ERR_STATE, "cnhe_graph_destroy: refused while a context the graph spans records a graph");
         CNHE_CUDA(cudaSetDevice(c.device));
-        c.sync(); // no launch still runs in the memory about to be freed
+        for (Context *m : g->members) m->sync(); // no launch still runs in the memory about to be freed
         CNHE_CUDA(cudaGraphExecDestroy(g->exec));
-        release_deferred(c, g->held);
+        for (size_t i = 0; i < g->members.size(); i++) release_deferred(*g->members[i], g->held[i]);
         delete g;
     } catch (const Error &e) { return set_err(e.code, e.what()); }
     return CNHE_OK;
@@ -1350,12 +1473,17 @@ extern "C" int cnhe_vecs_mod_switch(cnhe_ctx *h, const cnhe_vec *const *in, int 
     // primes first, and two switches of one family cannot wait on each other's locks
     if (d.root != c.root || d.k >= c.k) fail("cnhe_vecs_mod_switch: the destination must be a level of the same context family with fewer primes");
     std::lock_guard<std::recursive_mutex> lock_to(d.mu);
-    // the switch spans two contexts' streams and key slots: it cannot be part of either context's graph
-    not_recorded(c, "switches vectors to another context's level");
-    if (d.rec) {
-        end_recording(d, false);
-        throw Error(CNHE_ERR_STATE, "cnhe_vecs_mod_switch: the destination context records a graph; a switch between levels cannot be recorded "
-                                    "(the recording was aborted)");
+    // the switch spans two contexts' streams and key slots: it is part of a graph only when both contexts are enlisted in one recording
+    // (cnhe_capture_begin_levels), whose capture holds both contexts' streams
+    if (d.rec) api_enter(d, __func__); // a call on another thread than the recording one is refused
+    const bool recorded = c.rec && d.rec && c.rec->group == d.rec->group;
+    if (!recorded) {
+        not_recorded(c, "switches vectors to a level that is not enlisted in the same recording (cnhe_capture_begin_levels)");
+        if (d.rec) {
+            abort_recording(d);
+            throw Error(CNHE_ERR_STATE, "cnhe_vecs_mod_switch: the destination context records a graph that does not enlist the source; the "
+                                        "switch cannot be recorded (the recording was aborted)");
+        }
     }
     for (int i = 0; i < n; i++) {
         same_ctx(c, in[i]); // a pending vector is relinearised here
@@ -1367,7 +1495,11 @@ extern "C" int cnhe_vecs_mod_switch(cnhe_ctx *h, const cnhe_vec *const *in, int 
     d.slot = 0;
     ws_release_all(d);
     for (int s : std::set<int>(slots.begin(), slots.end()))
-        if (d.key_origin(s) != c.key_origin(s)) restrict_keys(d, c, s);
+        if (d.key_origin(s) != c.key_origin(s)) {
+            // restrict_keys synchronises; an eager run of the same chain restricts first, and a graph's bind restricts for later clients
+            if (recorded) c.refuse("would restrict a key slot's keys into the level (run the switch once eagerly first)");
+            restrict_keys(d, c, s);
+        }
     size_t total = 0;
     for (int i = 0; i < n; i++) total += in[i]->blocks;
     std::vector<BufRef> slab(c.P);

@@ -416,15 +416,26 @@ class Engine:
         return int(self.L.cnhe_kernel_launch_count(self.h))
 
     # ---- graph recording (include/cnhe.h, cnhe_capture_begin)
-    def capture_begin(self):
-        """From now on the context records its calls into a graph instead of running them."""
-        check(self.L.cnhe_capture_begin(self.h))
+    def capture_begin(self, levels=None):
+        """From now on the context records its calls into a graph instead of running them.  levels: engines of this one's family with
+        fewer primes (derive_level) to enlist: their calls and the mod_switch calls between them go into the same graph
+        (include/cnhe.h, cnhe_capture_begin_levels)."""
+        if levels is None:
+            check(self.L.cnhe_capture_begin(self.h))
+            self._capture_levels = []
+            return
+        arr = (C.c_void_p * max(len(levels), 1))(*[e.h.value for e in levels])
+        check(self.L.cnhe_capture_begin_levels(self.h, arr, len(levels)))
+        self._capture_levels = list(levels)
 
     def capture_end(self):
-        """The recorded calls as a Graph (launch() replays them)."""
+        """The recorded calls as a Graph (launch() replays them).  A graph that spans levels is also released when one of them closes."""
         g = C.c_void_p()
         check(self.L.cnhe_capture_end(self.h, C.byref(g)))
-        return Graph(self, g)
+        graph = Graph(self, g)
+        for e in self.__dict__.pop("_capture_levels", []):
+            e._live.add(graph)
+        return graph
 
     def capture_abort(self):
         check(self.L.cnhe_capture_abort(self.h))

@@ -574,7 +574,7 @@ class B200BfvFactory:
                                                       None if bias is None else [x.vec for x in bias], M, K)
         return [B200BfvVector(self, o) for o in out]
 
-    def CaptureInference(self, net, example_inputs):
+    def CaptureInference(self, net, example_inputs, SpanLevels=False):
         """Records the layers of `net` after its EncryptLayer once, on example_inputs, as one CUDA graph (include/cnhe.h,
         cnhe_capture_begin): a CapturedInference whose Run(inputs) replays the whole chain with one launch.  example_inputs is one encrypted
         input matrix (the network's GetNext path, Apply per layer) or a list of them, one per client, each bound to its client's key slot
@@ -582,13 +582,30 @@ class B200BfvFactory:
         long-lived state outside the graph.  Runs must use the same shapes, scales and key slots; the network's prepared weights
         and the factory's keys are read in place and must outlive the capture.  The example matrices become the graph's inputs: every Run
         writes its inputs' words into them, so they belong to the capture until it is disposed.  Run serves any client of the factory: it
-        binds the graph's key switches to the key slots its inputs carry (include/cnhe.h, cnhe_graph_bind)."""
-        return CapturedInference(self, net, example_inputs)
+        binds the graph's key switches to the key slots its inputs carry (include/cnhe.h, cnhe_graph_bind).
+        SpanLevels: a network built with levels= records across the level factories its ModSwitchLayers run on (level_factories,
+        include/cnhe.h cnhe_capture_begin_levels); the outputs are then matrices of the lowest level.  Without it, a chain that switches
+        levels is refused (CNHE_ERR_STATE)."""
+        return CapturedInference(self, net, example_inputs, SpanLevels)
 
     def Dispose(self):
         for f in self.__dict__.get("_levels", {}).values():
             f.Dispose()
         self.engine.close()
+
+
+def level_factories(chain):
+    """The level factories the ModSwitchLayers of `chain` (a network's layers after its EncryptLayer) run on, in chain order, each once:
+    the contexts a recording of the chain enlists (CaptureInference(SpanLevels=True)).  A switch on a factory without levels (RawFactory)
+    passes its matrix through and names none."""
+    from .layers import BaseLayer, ModSwitchLayer
+    out = []
+    for layer in chain:
+        if isinstance(layer, ModSwitchLayer):
+            f = layer.Factory
+            if f is not BaseLayer.Factory.fget(layer) and not any(f is g for g in out):
+                out.append(f)
+    return out
 
 
 def graph_binding(positions, recorded, current):
@@ -609,7 +626,7 @@ class CapturedInference:
     the latest Run and valid until the next one.  TimingLayers are left out: they time and synchronise the host, which a replay does
     not do."""
 
-    def __init__(self, factory, net, example_inputs):
+    def __init__(self, factory, net, example_inputs, SpanLevels=False):
         from .layers import EncryptLayer, TimingLayer
         self.factory, self.graph, self.outputs = factory, None, None
         self.batch = isinstance(example_inputs, (list, tuple))
@@ -633,7 +650,8 @@ class CapturedInference:
         # inferences of the network would read it.
         for m in self._apply(chain, examples):
             m.Dispose()
-        eng.capture_begin()
+        # the level factories exist after the eager pass, and hold the restriction of every key slot the examples carry
+        eng.capture_begin(levels=[f.engine for f in level_factories(chain)] if SpanLevels else None)
         try:
             ms = self._apply(chain, examples)
             self.graph = eng.capture_end()

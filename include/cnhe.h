@@ -169,8 +169,11 @@ int cnhe_vec_key_slot(const cnhe_vec *, int *slot);
  * pending (deferred-relinearisation) vector is relinearised first.  Outputs keep dimension, scale, format and key slot, one slab per
  * channel; a slot whose keys in `from` were added or replaced since `to` was derived is restricted into `to` first, under the same
  * number.  Counts no operation.  `to`'s streams wait for the inputs and `from`'s streams for the switch.  CNHE_ERR_INVALID for vectors
- * of another context, plain vectors or an unrelated / not smaller `to`; CNHE_ERR_STATE while either context records a graph (the
- * recording is aborted). */
+ * of another context, plain vectors or an unrelated / not smaller `to`.  The switch is recorded when both contexts are enlisted in one
+ * recording (cnhe_capture_begin_levels): its pointer table goes to the graph's memory and the event hand-off between the two contexts'
+ * streams becomes an edge of the graph.  CNHE_ERR_STATE, the recording aborted, while one context records alone or the two record
+ * different graphs, and while recording a switch that would have to restrict a slot's keys into `to` (the restriction synchronises: run
+ * the chain once eagerly first, as CaptureInference does, or bind the graph to the slot, cnhe_graph_bind). */
 int cnhe_context_derive_level(cnhe_ctx *, int k, cnhe_ctx **out);
 int cnhe_vecs_mod_switch(cnhe_ctx *from, const cnhe_vec *const *in, int n, cnhe_ctx *to, cnhe_vec **out /*n*/);
 int cnhe_vec_write(cnhe_ctx *, const cnhe_vec *, char *dst, size_t cap, size_t *needed);
@@ -422,7 +425,10 @@ int cnhe_layer_activation_conv_dense(cnhe_ctx *, const cnhe_vec *const *in, int 
  *   recorded and each recorded Galois element (CNHE_ERR_STATE naming the slot and the element otherwise).  A refused bind leaves the
  *   previous binding in force; refused while the context records.  A launch reads the bound slots' keys as they were when bound.  Binds and
  *   launches are ordered like any call: launches bound to different clients may be enqueued back to back without a host synchronisation,
- *   and each reads its own binding.  A bind allocates no device memory.
+ *   and each reads its own binding.  A bind allocates no device memory, with one exception for a graph that spans levels: a bound slot
+ *   whose keys in an enlisted level are not those of the graph's context (a client added to, replaced in or removed from the context since
+ *   the level was derived or last switched to) is first restricted into that level, as the eager switch would (that allocates the level's
+ *   copy of the keys and synchronises).  Slots are numbered alike in every context of a family, so positions are slot numbers there too.
  *   Vectors created while recording report, and are key-switched and decrypted under, the slot their slot's position is bound to
  *   (cnhe_vec_key_slot).  The recorded input vectors predate the recording: retag them (cnhe_vec_set_key_slot) before cnhe_vecs_assign.
  *   Rotation hop plans and the choice of key-switch path stay as recorded: a client holding the recording client's Galois elements gets,
@@ -430,7 +436,27 @@ int cnhe_layer_activation_conv_dense(cnhe_ctx *, const cnhe_vec *const *in, int 
  *   results decrypt to the same values but whose words can differ from an eager run, which plans from that client's own elements.
  * cnhe_graph_info: the graph's kernel nodes and the device bytes it owns (either pointer may be NULL).
  * cnhe_graph_destroy: waits for the context's queued work and releases the graph (CNHE_ERR_STATE while the context records).  Destroy every
- *   graph before its context.
+ *   graph before any context it spans.
+ * cnhe_capture_begin_levels: a recording on `ctx` that also enlists the n contexts levels[0..n) -- levels of ctx's family with fewer
+ *   primes (cnhe_context_derive_level), typically the ones a levelled network switches to.  Calls on any enlisted context, and the
+ *   cnhe_vecs_mod_switch calls between them, are captured into the one graph cnhe_capture_end(ctx) returns; it is launched, bound and
+ *   destroyed like any other.  CNHE_ERR_INVALID for a null argument, a level listed twice, ctx itself, a context of another family or one
+ *   with no fewer primes than ctx, and, as for cnhe_capture_begin, while any of the contexts profiles or traces noise; CNHE_ERR_STATE while
+ *   any of them records (ctx's own recording is then aborted, an enlisted level's is left running).
+ *   Streams: the capture runs on ctx's channel stream 0, and at begin every channel stream of every enlisted context forks from it (an
+ *     event on that stream, a wait on each of theirs), before any call: a stream left out would run its work (a bias upload, a plain
+ *     vector) once, at record time, and never in a replay.  cnhe_capture_end joins every enlisted stream back into ctx's stream 0 first.
+ *     A launch joins every stream of every enlisted context into ctx's stream 0, launches there, then forks them all again, so a later
+ *     eager call on a level (decrypting the scores) is ordered after the replay.
+ *   One recording: the enlisted contexts share the graph's memory, its key binding and its fate.  A call refused or failing on any of
+ *     them -- another thread's call included -- aborts the recording of every one, after which each computes eagerly;
+ *     cnhe_capture_abort on any of them does the same.  cnhe_capture_end must be called on ctx (on a level it is refused, and aborts).
+ *     Buffers from before the recording that a level releases during it stay allocated until the graph is destroyed.
+ *   Counts: each context's operation counters and kernel count are restored when the recording ends, and each launch adds to every
+ *     context what was recorded on it: after a launch every context's counts equal those of one eager levelled inference.
+ *   Key binding: a recorded key switch on a level reads that level's keys of the bound slot (see the restriction under cnhe_graph_bind).
+ *     A launch is refused (CNHE_ERR_STATE) when a bound slot's keys changed since the bind in any enlisted context.
+ *   cnhe_graph_destroy synchronises every enlisted context, and is refused while any of them records.
  * cnhe_vecs_assign: copies each src[i]'s ciphertext words into dst[i], device to device, ordered like any call: how a new input enters a
  *   graph's recorded input vectors.  Both must be encrypted and match in dimension, blocks, format, scale and key slot (the recording acted
  *   on those); the slots must be live, as for the calls that take several vectors, and a destination may not partly overlap its source
@@ -457,6 +483,7 @@ int cnhe_layer_activation_conv_dense(cnhe_ctx *, const cnhe_vec *const *in, int 
  *     aborts the recording, as cnhe_capture_abort does; cnhe_capture_end then reports CNHE_ERR_STATE. */
 typedef struct cnhe_graph cnhe_graph;
 int cnhe_capture_begin(cnhe_ctx *);
+int cnhe_capture_begin_levels(cnhe_ctx *ctx, cnhe_ctx *const *levels, int n);
 int cnhe_capture_end(cnhe_ctx *, cnhe_graph **out);
 int cnhe_capture_abort(cnhe_ctx *);
 int cnhe_graph_launch(cnhe_graph *);

@@ -137,6 +137,7 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_raw_elapsed_ms(IntPtr a0, out float ms);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern ulong cnhe_kernel_launch_count(IntPtr a0);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_begin(IntPtr a0);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_begin_levels(IntPtr ctx, IntPtr[] levels, int n);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_end(IntPtr a0, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_capture_abort(IntPtr a0);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_graph_launch(IntPtr a0);
@@ -595,6 +596,17 @@ namespace HEWrapper
         public IntPtr Capture(Action record)
         {
             Cnhe.Check(Cnhe.cnhe_capture_begin(Ctx));
+            try { record(); }
+            catch { Cnhe.cnhe_capture_abort(Ctx); throw; }
+            Cnhe.Check(Cnhe.cnhe_capture_end(Ctx, out var graph));
+            return graph;
+        }
+        /// Capture of a levelled inference: `levels` are the contexts (cnhe_context_derive_level of this factory's) its mod switches go to.
+        /// Their calls and the switches between them are recorded into the same graph (include/cnhe.h, cnhe_capture_begin_levels); the
+        /// graph must be disposed before any of those contexts.
+        public IntPtr CaptureLevels(IntPtr[] levels, Action record)
+        {
+            Cnhe.Check(Cnhe.cnhe_capture_begin_levels(Ctx, levels, levels.Length));
             try { record(); }
             catch { Cnhe.cnhe_capture_abort(Ctx); throw; }
             Cnhe.Check(Cnhe.cnhe_capture_end(Ctx, out var graph));

@@ -18,7 +18,7 @@ ALLOWED = {
     "cnhe_ctx *": {"IntPtr"}, "const cnhe_ctx *": {"IntPtr"}, "cnhe_vec *": {"IntPtr"}, "const cnhe_vec *": {"IntPtr"},
     "cnhe_diag *": {"IntPtr"}, "const cnhe_diag *": {"IntPtr"}, "cnhe_diag **": {"out IntPtr"},
     "cnhe_graph *": {"IntPtr"}, "const cnhe_graph *": {"IntPtr"}, "cnhe_graph **": {"out IntPtr"},
-    "cnhe_ctx **": {"out IntPtr"}, "cnhe_vec **": {"out IntPtr", "IntPtr[]"},
+    "cnhe_ctx **": {"out IntPtr"}, "cnhe_ctx *const *": {"IntPtr[]"}, "cnhe_vec **": {"out IntPtr", "IntPtr[]"},
     "const cnhe_vec *const *": {"IntPtr[]"}, "cnhe_vec *const *": {"IntPtr[]"},
     "const uint64_t *": {"ulong[]", "IntPtr"}, "uint64_t *": {"ulong[]", "IntPtr", "out ulong"},
     "const double *": {"double[]"}, "double *": {"double[]", "out double"},
