@@ -668,6 +668,18 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
             std::reverse(c.bsk.begin(), c.bsk.end()); // m_sk (last) = the largest
         }
     }
+    // Decryption divides by q mod gamma and BEHZ by q mod each Bsk prime: a q holding one of them makes that inverse 0 and every result
+    // garbage, with no error.  gamma and SEAL's base (61-bit, = 1 mod 2^18) are valid coefficient primes for every N; SEAL caps user
+    // primes at 60 bits and never meets this, this library takes 61, so it refuses the collision.  (The fast base avoids q by choice.)
+    for (u64 p : c.q) {
+        if (p == GAMMA) throw Error(-1, "coefficient moduli must not contain gamma = 0x1fffffffffc80001, the decryption's auxiliary prime");
+        for (u64 b : c.bsk)
+            if (p == b) {
+                char m[112];
+                snprintf(m, sizeof(m), "coefficient moduli must not contain a prime of the BEHZ base Bsk (0x%llx)", (unsigned long long)b);
+                throw Error(-1, m);
+            }
+    }
     const int kb = (int)c.bsk.size();
     const u64 M_SK = c.bsk[kb - 1];
     c.kb = kb;

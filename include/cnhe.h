@@ -49,7 +49,10 @@ const char *cnhe_version(void);
  * DefaultParams.CoeffModulus128(N) ("AtomicSealBfvVector.cs:140-151").  Builds every device table; no keys yet. */
 int cnhe_context_create(const uint64_t *plain_primes, int P, uint32_t N, int dbc_relin, int dbc_galois,
                         int small_modulus_count, int device, cnhe_ctx **out);
-/* same with explicit coefficient moduli (AtomicSealBfvVector.cs:152-161 Parms(t, n, coefModulus)) */
+/* same with explicit coefficient moduli (AtomicSealBfvVector.cs:152-161 Parms(t, n, coefModulus)): 1..9 primes = 1 mod 2N below
+ * 2^61, each larger than every plaintext prime.  CNHE_ERR_INVALID for a q holding gamma = 0x1fffffffffc80001 (decryption's auxiliary
+ * prime) or a prime of the BEHZ base (under CNHE_AUX_BASE=seal: m_sk = 0x1fffffffffe00001 and SEAL's first k auxiliary primes), which
+ * would make decryption or the multiply silently wrong, and for a q whose auxiliary base would need more than 12 primes. */
 int cnhe_context_create_custom(const uint64_t *plain_primes, int P, uint32_t N, const uint64_t *coeff_moduli, int k,
                                int dbc_relin, int dbc_galois, int device, cnhe_ctx **out);
 int cnhe_context_destroy(cnhe_ctx *);

@@ -261,6 +261,7 @@ struct orc_ctx {
     u64 neg_inv_q_mod_t = 0, neg_inv_q_mod_gamma = 0, inv_gamma_mod_t = 0;
     /* keys */
     bool have_keys = false;
+    const char *refuse_decrypt = nullptr, *refuse_behz = nullptr; /* q holds gamma / a Bsk prime (build_ctx) */
     std::vector<u64> sk_ntt, sk_coeff, pk; /* sk_coeff: k*N lifted ternary */
     KSKey rlk;
     std::vector<u64> galois_elts;
@@ -377,11 +378,19 @@ static orc_ctx *build_ctx(u64 t, uint32_t N, const std::vector<u64> &qv, int dbc
         if (!is_prime(p) || (p - 1) % (2ULL * N)) { fail("coefficient modulus must be prime and = 1 mod 2N"); return nullptr; }
     if (!is_prime(t) || (t - 1) % (2ULL * N)) { fail("plain modulus must be prime and = 1 mod 2N (batching)"); return nullptr; }
     orc_ctx *c = new orc_ctx();
+    /* gamma, m_sk and the auxiliary primes are 61-bit primes = 1 mod 2^18: a q holding one makes the inverse of q modulo it 0, so the
+     * decryption (gamma) or the BEHZ multiply (Bsk) built on it would be silently wrong.  The context stays usable for what does not
+     * divide by q there (tables, transforms, keys, encryption, key switches); those operations refuse. */
+    std::vector<u64> aux = aux_primes((int)qv.size());
+    for (u64 p : qv) {
+        if (p == GAMMA) c->refuse_decrypt = "coefficient moduli must not contain gamma = 0x1fffffffffc80001";
+        if (p == M_SK || std::find(aux.begin(), aux.end(), p) != aux.end())
+            c->refuse_behz = "coefficient moduli must not contain a prime of the BEHZ base Bsk";
+    }
     c->t = t; c->N = N; c->logN = logN; c->k = (int)qv.size();
     c->dbc_relin = dbc_relin; c->dbc_galois = dbc_galois;
     int k = c->k;
     for (u64 p : qv) c->q.push_back(make_mod(p));
-    std::vector<u64> aux = aux_primes(k);
     for (u64 p : aux) c->bsk.push_back(make_mod(p));
     c->bsk.push_back(make_mod(M_SK));
     c->tmod = make_mod(t);
@@ -670,6 +679,7 @@ static void dot_with_secret(const orc_ctx *c, const u64 *ct, int size, u64 *out)
 }
 /* Decryptor::decrypt (BFV): scale-and-round through {t, gamma} (AtomicSealBfvVector.cs:1042,1085) */
 extern "C" int orc_decrypt(const orc_ctx *c, const u64 *ct, int size, u64 *plain) {
+    if (c->refuse_decrypt) return fail(c->refuse_decrypt);
     if (!c->have_keys) return fail("no keys");
     if (size < 2 || size > 3) return fail("ciphertext size must be 2 or 3");
     const int k = c->k;
@@ -814,7 +824,8 @@ extern "C" int orc_multiply_plain(const orc_ctx *c, const u64 *ct, int size, con
 /* ------------------------------------------------------------------ BEHZ multiply (SEAL evaluator.cpp bfv_multiply,
  * util/baseconverter.cpp fastbconv_mtilde / mont_rq / fast_floor / fastbconv_sk)
  * reached from AtomicSealBfvVector.cs:461,546,786,839,1457 */
-extern "C" void orc_behz_lift(const orc_ctx *c, const u64 *in, u64 *out) {
+extern "C" int orc_behz_lift(const orc_ctx *c, const u64 *in, u64 *out) {
+    if (c->refuse_behz) return fail(c->refuse_behz);
     const int k = c->k;
     const size_t N = c->N;
     u64 tmp[16];
@@ -839,9 +850,11 @@ extern "C" void orc_behz_lift(const orc_ctx *c, const u64 *in, u64 *out) {
             out[j * N + n] = mulmod(v, c->inv_mtilde_mod_bsk[j], bj);
         }
     }
+    return 0;
 }
 /* in: [k q-residues | k+1 Bsk residues] of t*d ; out: k q-residues of floor-ish(t*d/q) */
-extern "C" void orc_behz_floor(const orc_ctx *c, const u64 *in, u64 *out) {
+extern "C" int orc_behz_floor(const orc_ctx *c, const u64 *in, u64 *out) {
+    if (c->refuse_behz) return fail(c->refuse_behz);
     const int k = c->k;
     const size_t N = c->N;
     const Mod &msk = c->bsk[k];
@@ -872,8 +885,10 @@ extern "C" void orc_behz_floor(const orc_ctx *c, const u64 *in, u64 *out) {
             out[i * N + n] = v;
         }
     }
+    return 0;
 }
 extern "C" int orc_multiply(const orc_ctx *c, const u64 *a, const u64 *b, u64 *out) {
+    if (c->refuse_behz) return fail(c->refuse_behz);
     const int k = c->k, kb = k + 1;
     const size_t N = c->N;
     /* steps 0-1: both operands into Bsk, then NTT everything */
@@ -1097,6 +1112,7 @@ extern "C" int orc_mac_layer(const orc_ctx *c, const u64 *in, int n_in, const in
     return 0;
 }
 extern "C" int orc_square_layer(const orc_ctx *c, const u64 *in, int n, u64 *out, int threads, int begin, int step) {
+    if (c->refuse_behz) return fail(c->refuse_behz);
     const size_t ctw = (size_t)2 * c->k * c->N;
     if (step < 1) step = 1;
     std::vector<int> is;

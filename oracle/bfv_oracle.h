@@ -28,7 +28,9 @@ typedef struct orc_ctx orc_ctx;
 /* coeff_count: number of default coefficient primes to keep (prefix of DefaultParams.CoeffModulus128(N)),
  * <=0 = all  (AtomicSealBfvVector.cs:140-151).  dbc_*: decomposition bit counts (IFactory.cs:244-245). */
 orc_ctx *orc_create(uint64_t plain_modulus, uint32_t N, int coeff_count, int dbc_relin, int dbc_galois);
-/* explicit coefficient moduli (used by small-N cross checks) */
+/* explicit coefficient moduli (used by small-N cross checks, and as transform tables of any NTT primes).  A q holding gamma makes
+ * orc_decrypt fail; a q holding a prime of the Bsk base (m_sk or the first k auxiliary primes) makes orc_multiply, orc_square_layer
+ * and the BEHZ stages fail: their constants divide by q modulo that prime, which is 0. */
 orc_ctx *orc_create_custom(uint64_t plain_modulus, uint32_t N, const uint64_t *q, int k, int dbc_relin, int dbc_galois);
 void orc_destroy(orc_ctx *);
 const char *orc_last_error(void);
@@ -85,8 +87,8 @@ int orc_rotate_columns(const orc_ctx *, const uint64_t *ct, uint64_t *out);
 uint64_t orc_galois_elt_from_step(const orc_ctx *, int steps);
 
 /* individual BEHZ stages (exposed so each GPU kernel can be checked on its own) */
-void orc_behz_lift(const orc_ctx *, const uint64_t *poly_q /*kN*/, uint64_t *poly_bsk /*(k+1)N*/); /* fastbconv_mtilde + mont_rq */
-void orc_behz_floor(const orc_ctx *, const uint64_t *poly_q_bsk /*(2k+1)N, already *t */, uint64_t *poly_q /*kN*/); /* fast_floor + fastbconv_sk */
+int orc_behz_lift(const orc_ctx *, const uint64_t *poly_q /*kN*/, uint64_t *poly_bsk /*(k+1)N*/); /* fastbconv_mtilde + mont_rq */
+int orc_behz_floor(const orc_ctx *, const uint64_t *poly_q_bsk /*(2k+1)N, already *t */, uint64_t *poly_q /*kN*/); /* fast_floor + fastbconv_sk */
 
 /* Multi-threaded layer-level drivers = the timed CPU baseline (mirrors Utils.ParallelProcessInEnv,
  * "HE Wrapper/Utils.cs:46-88": `threads` workers pulling output indices from an atomic counter). */

@@ -247,13 +247,13 @@ class Oracle:
     def behz_lift(self, poly_q):
         a = _u64(poly_q).ravel()
         out = np.zeros((self.k + 1) * self.N, np.uint64)
-        self.L.orc_behz_lift(self.h, _p(a), _p(out))
+        self._chk(self.L.orc_behz_lift(self.h, _p(a), _p(out)))
         return out
 
     def behz_floor(self, poly_q_bsk):
         a = _u64(poly_q_bsk).ravel()
         out = np.zeros(self.k * self.N, np.uint64)
-        self.L.orc_behz_floor(self.h, _p(a), _p(out))
+        self._chk(self.L.orc_behz_floor(self.h, _p(a), _p(out)))
         return out
 
     # layer drivers (CPU baseline)

@@ -304,6 +304,68 @@ def primes(bits, N, count=1):
     return out
 
 
+GAMMA = 0x1fffffffffc80001  # the decryption's auxiliary prime (SEAL small_mods)
+M_SK = 0x1fffffffffe00001   # SEAL's m_sk; SEAL's auxiliary base primes are the next 61-bit primes = 1 mod 2^18
+
+
+def clear_primes(bits, N, count=1):
+    """the `count` largest `bits`-bit primes = 1 mod 2N that are neither gamma, nor m_sk, nor = 1 mod 2^18 (so no SEAL auxiliary base
+    prime at any k): coefficient moduli every context and the oracle accept"""
+    assert bits != 48
+    out, c = [], ((1 << bits) - 1) // (2 * N) * (2 * N) + 1
+    while len(out) < count:
+        if (c - 1) % (1 << 18) and is_prime(c):
+            out.append(c)
+        c -= 2 * N
+    assert all(p.bit_length() == bits for p in out) and GAMMA not in out and M_SK not in out
+    return out
+
+
+# ---------------------------------------------------------------- decryption on big integers (no gamma, no oracle)
+def ternary_secret(sk_coeff, q):
+    """the secret key's coefficients in {-1, 0, 1} from its residues [k][N] in coefficient form; every residue must say the same"""
+    sk = np.asarray(sk_coeff, np.uint64).reshape(len(q), -1)
+    s = np.where(sk[0] == 1, 1, np.where(sk[0] == q[0] - 1, -1, 0)).astype(np.int64)
+    for l, p in enumerate(q):
+        assert np.array_equal(sk[l], np.where(s < 0, p - 1, s).astype(np.uint64)), "not one ternary polynomial"
+    return s
+
+
+def _kron(a):
+    """Kronecker substitution: coefficients below 2^64 as one integer, 128 bits apart"""
+    w = np.zeros((len(a), 2), np.uint64)
+    w[:, 0] = a
+    return int.from_bytes(w.tobytes(), "little")
+
+
+def _unkron(x, n):
+    w = np.frombuffer(x.to_bytes(16 * n, "little"), np.uint64).reshape(n, 2)
+    return w[:, 0].astype(object) + (w[:, 1].astype(object) << 64)
+
+
+def times_ternary(c, s, p):
+    """c(x) s(x) mod (x^N + 1, p), c in [0, p)^N, s in {-1, 0, 1}^N, exactly (every product coefficient stays below 2^128)"""
+    N = len(c)
+    C = _kron(np.asarray(c, np.uint64))
+    full = _unkron(C * _kron((s == 1).astype(np.uint64)), 2 * N) - _unkron(C * _kron((s == -1).astype(np.uint64)), 2 * N)
+    return (full[:N] - full[N:]) % p
+
+
+def exact_decrypt(ct, s, q, t):
+    """the plaintext round(t [c0 + c1 s]_Q / Q) mod t of a size-2 ciphertext [2][k][N] (coefficient form), on Python integers"""
+    k = len(q)
+    ct = np.asarray(ct, np.uint64).reshape(2, k, -1)
+    Q = 1
+    for p in q:
+        Q *= p
+    x = 0
+    for l, p in enumerate(q):
+        r = (ct[0, l].astype(object) + times_ternary(ct[1, l], s, p)) % p
+        x = x + r * ((Q // p) * pow(Q // p % p, -1, p))
+    x = x % Q
+    return ((2 * t * x + Q) // (2 * Q) % t).astype(np.uint64)
+
+
 # ---------------------------------------------------------------- digit decomposition (make_digit_map, runtime.cu)
 def digit_map(q, w):
     """[(residue index, shift)] in digit order; more than 64 digits is refused"""
