@@ -960,17 +960,21 @@ static void decrypt_channel(Context &c, const cnhe_vec *v, int ch, std::vector<u
         memcpy(res.data(), hostv.data(), take * 8);
     }
 }
-extern "C" int cnhe_vec_decrypt(cnhe_ctx *h, const cnhe_vec *v, double *out, uint64_t cap) {
-    API_BEGIN(h)
-    not_recorded(c, "returns words to the host");
-    same_ctx(c, v);
-    if (cap < v->dim) fail("destination too small");
+// Decrypt of v's `dim` values: every channel's residues, joined
+static void decrypt_values(Context &c, const cnhe_vec *v, double *out) {
     std::vector<std::vector<u64>> split(c.P);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
         decrypt_channel(c, v, ch, split[ch]);
     }
     join_values(c, split, v->dim, v->scale, out);
+}
+extern "C" int cnhe_vec_decrypt(cnhe_ctx *h, const cnhe_vec *v, double *out, uint64_t cap) {
+    API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
+    same_ctx(c, v);
+    if (cap < v->dim) fail("destination too small");
+    decrypt_values(c, v, out);
     API_END
 }
 // DecryptFullPrecision ("EncryptedSealBfvVector.cs:343-348"): the residues of every channel, for the caller's BigInteger CRT join
@@ -994,12 +998,7 @@ extern "C" int cnhe_vecs_decrypt(cnhe_ctx *h, const cnhe_vec *const *vecs, int n
     for (int i = 0; i < n; i++) {
         same_ctx(c, vecs[i]);
         if (vecs[i]->dim != dim) fail("all vectors must have the same dimension");
-        std::vector<std::vector<u64>> split(c.P);
-        for (int ch = 0; ch < c.P; ch++) {
-            c.set_channel(ch);
-            decrypt_channel(c, vecs[i], ch, split[ch]);
-        }
-        join_values(c, split, dim, vecs[i]->scale, out + (size_t)i * dim);
+        decrypt_values(c, vecs[i], out + (size_t)i * dim);
     }
     API_END
 }
@@ -1533,9 +1532,9 @@ extern "C" int cnhe_vec_key_slot(const cnhe_vec *v, int *slot) {
     *slot = v->enc ? v->key_slot() : -1;
     return CNHE_OK;
 }
-// Rotate (first block) of n vectors by the same amount, their key slots may differ: the hops of all vectors share each key-switch wave
-extern "C" int cnhe_vecs_rotate(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int amount, cnhe_vec **out) {
-    API_BEGIN(h)
+// Rotate (AtomicSealBfvVector.cs:1414-1430, first block only) of n vectors by the same amount, their key slots may differ: the hops of
+// all vectors share each key-switch wave
+static void rotate_vecs(Context &c, const cnhe_vec *const *vecs, int n, int amount, cnhe_vec **out) {
     if (n < 1 || !vecs || !out) fail("bad arguments");
     for (int i = 0; i < n; i++) {
         same_ctx(c, vecs[i]);
@@ -1556,6 +1555,15 @@ extern "C" int cnhe_vecs_rotate(cnhe_ctx *h, const cnhe_vec *const *vecs, int n,
         op_rotate_rows_multi(c, ch, jobs);
     }
     for (int i = 0; i < n; i++) out[i] = outs[i].release();
+}
+extern "C" int cnhe_vec_rotate(cnhe_ctx *h, const cnhe_vec *a, int amount, cnhe_vec **out) {
+    API_BEGIN(h)
+    rotate_vecs(c, &a, 1, amount, out);
+    API_END
+}
+extern "C" int cnhe_vecs_rotate(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, int amount, cnhe_vec **out) {
+    API_BEGIN(h)
+    rotate_vecs(c, vecs, n, amount, out);
     API_END
 }
 extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap) {
@@ -1852,107 +1860,6 @@ extern "C" int cnhe_vec_dot_product(cnhe_ctx *h, const cnhe_vec *a, const cnhe_v
     *out = sum_all_slots(c, mul.get(), length, force_column);
     API_END
 }
-// Rotate (AtomicSealBfvVector.cs:1414-1430): first block only
-extern "C" int cnhe_vec_rotate(cnhe_ctx *h, const cnhe_vec *a, int amount, cnhe_vec **out) {
-    API_BEGIN(h)
-    same_ctx(c, a);
-    use_slot(c, {a});
-    if (!a->enc) fail("Rotate operates only on encrypted data");
-    if (a->format == CNHE_SPARSE) fail("Rotate operates only on dense vectors");
-    cnhe_vec *o = new_vec(c, a->dim, a->scale, CNHE_DENSE, true, 1);
-    std::unique_ptr<cnhe_vec> guard(o);
-    alloc_channels(o);
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        op_rotate_rows(c, ch, a->ptr(ch), 1, amount, o->ptr(ch));
-    }
-    *out = guard.release();
-    API_END
-}
-// Duplicate (AtomicSealBfvVector.cs:1370-1408)
-extern "C" int cnhe_vec_duplicate(cnhe_ctx *h, const cnhe_vec *a, uint64_t count, cnhe_vec **out) {
-    API_BEGIN(h)
-    same_ctx(c, a);
-    use_slot(c, {a});
-    uint64_t shift = 1;
-    while (shift < a->dim) shift *= 2;
-    if (!a->enc) fail("Duplicate operates only on encrypted data");
-    if (a->format == CNHE_SPARSE) fail("Duplicate operates only on dense vectors");
-    const size_t N = c.N, ctw = c.ct_words();
-    if (shift * count > N) fail("Packed vector must fit in a single ciphertext");
-    cnhe_vec *o = new_vec(c, count * shift, a->scale, CNHE_DENSE, true, 1);
-    std::unique_ptr<cnhe_vec> guard(o);
-    alloc_channels(o);
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        u64 *res = o->ptr(ch), *rotator = c.ws_alloc(ctw);
-        CNHE_CUDA(cudaMemcpyAsync(res, a->ptr(ch), ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(res, a->ptr(ch));
-        const u64 *rot_src = a->ptr(ch);
-        bool column_rotated = false;
-        // the count-1 rotations of the original (or of its column-rotated copy) are independent: queue them, execute them together
-        // (hops with the same Galois element share a key-switch wave), then add them in the reference's order (":1385-1402")
-        std::vector<RotateJob> jobs;
-        std::vector<u64 *> pieces;
-        for (uint64_t i = 1; i < count; i++) {
-            long long target = (long long)(i * shift);
-            if (target * 2 >= (long long)N) {
-                if (!column_rotated) {
-                    column_rotated = true;
-                    op_rotate_columns(c, ch, a->ptr(ch), 1, rotator);
-                    rot_src = rotator;
-                }
-                target -= (long long)N / 2;
-            }
-            u64 *tmp = c.ws_alloc(ctw);
-            jobs.push_back({rot_src, -(int)target, tmp}); // RotateRowsAndAdd(rotator, target, ...)
-            pieces.push_back(tmp);
-        }
-        op_rotate_rows_multi(c, ch, jobs);
-        for (u64 *tmp : pieces) do_add(c, ch, res, tmp, res, ctw, 0);
-    }
-    *out = guard.release();
-    API_END
-}
-// Permute (AtomicSealBfvVector.cs:1436-1475)
-extern "C" int cnhe_vec_permute(cnhe_ctx *h, const cnhe_vec *a, const cnhe_vec *const *selections, const int *shifts, int n, uint64_t output_dim,
-                                cnhe_vec **out) {
-    API_BEGIN(h)
-    same_ctx(c, a);
-    use_slot(c, {a});
-    if (a->format != CNHE_DENSE) fail("Permute works only on dense vectors");
-    if (!a->enc) fail("can permute only encrypted vectors");
-    if (a->blocks > 1) fail("can permute only a single block");
-    int first = -1;
-    for (int i = 0; i < n; i++) {
-        if (!selections[i]) continue;
-        same_ctx(c, selections[i]);
-        if (first < 0) first = i;
-        if (selections[i]->dim != a->dim) fail("dimension of selection vector does not match dimension of data vector");
-        if (selections[i]->scale != selections[first]->scale) fail("scales of all selection vectors should be the same");
-        if (selections[i]->enc) fail("encrypted size must be 2 (rotating the size-3 product of an encrypted selection is rejected by SEAL)");
-        if (selections[i]->format != CNHE_DENSE) fail("selection vectors must be dense");
-    }
-    if (first < 0) fail("permuting with no selected values is illigal");
-    const size_t ctw = c.ct_words();
-    cnhe_vec *o = new_vec(c, output_dim, a->scale * selections[first]->scale, CNHE_DENSE, true, 1);
-    std::unique_ptr<cnhe_vec> guard(o);
-    alloc_channels(o);
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        u64 *t = c.ws_alloc(ctw), *r = c.ws_alloc(ctw);
-        bool have = false;
-        for (int i = 0; i < n; i++) {
-            if (!selections[i]) continue;
-            op_multiply_plain_dense(c, ch, a->ptr(ch), 1, selections[i]->ptr(ch), false, t);
-            op_rotate_rows(c, ch, t, 1, shifts[i], r);
-            if (!have) { CNHE_CUDA(cudaMemcpyAsync(o->ptr(ch), r, ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(o->ptr(ch), r); }
-            else do_add(c, ch, o->ptr(ch), r, o->ptr(ch), ctw, 0);
-            have = true;
-        }
-    }
-    *out = guard.release();
-    API_END
-}
 // GenerateSparseOfArray (AtomicSealBfvVector.cs:1347-1359)
 extern "C" int cnhe_vecs_generate_sparse_of_array(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, cnhe_vec **out) {
     API_BEGIN(h)
@@ -2160,10 +2067,9 @@ static std::vector<std::unique_ptr<cnhe_vec>> batch_outputs(Context &c, int n, c
     }
     return outs;
 }
-// cnhe_vec_duplicate of B vectors (one per client; key slots may differ): the column rotations in one call, every client's count - 1 row
-// rotations in one op_rotate_rows_multi, then each client's additions in the reference's order.  out[b] is bit-identical to the single call.
-extern "C" int cnhe_vecs_duplicate_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int B, uint64_t count, cnhe_vec **out) {
-    API_BEGIN(h)
+// Duplicate (AtomicSealBfvVector.cs:1370-1408) of B vectors (one per client; key slots may differ): the column rotations in one call,
+// every client's count - 1 row rotations in one op_rotate_rows_multi, then each client's additions in the reference's order
+static void duplicate_vecs(Context &c, const cnhe_vec *const *vecs, int B, uint64_t count, cnhe_vec **out) {
     const std::vector<int> slots = batch_inputs(c, vecs, B, out);
     const cnhe_vec *a = vecs[0];
     uint64_t shift = 1;
@@ -2178,11 +2084,15 @@ extern "C" int cnhe_vecs_duplicate_batch(cnhe_ctx *h, const cnhe_vec *const *vec
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
         u64 *rotator = nullptr;
-        if (column) { // rotate_columns of every input (":1387-1394"), gathered so that one call serves all
-            u64 *in = c.ws_alloc((size_t)B * ctw);
+        if (column) { // rotate_columns of every input (":1387-1394"); several are gathered so that one call serves all, one is read in place
+            const u64 *in = vecs[0]->ptr(ch);
+            if (B > 1) {
+                u64 *g = c.ws_alloc((size_t)B * ctw);
+                for (int b = 0; b < B; b++)
+                    { CNHE_CUDA(cudaMemcpyAsync(g + (size_t)b * ctw, vecs[b]->ptr(ch), ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(g + (size_t)b * ctw, vecs[b]->ptr(ch)); }
+                in = g;
+            }
             rotator = c.ws_alloc((size_t)B * ctw);
-            for (int b = 0; b < B; b++)
-                { CNHE_CUDA(cudaMemcpyAsync(in + (size_t)b * ctw, vecs[b]->ptr(ch), ctw * 8, cudaMemcpyDeviceToDevice, c.stream)); c.note_copy(in + (size_t)b * ctw, vecs[b]->ptr(ch)); }
             op_rotate_columns(c, ch, in, B, rotator, slots.data());
         }
         std::vector<RotateJob> jobs;
@@ -2208,15 +2118,23 @@ extern "C" int cnhe_vecs_duplicate_batch(cnhe_ctx *h, const cnhe_vec *const *vec
             for (size_t i = 0; i < per; i++) do_add(c, ch, outs[b]->ptr(ch), pieces[b * per + i], outs[b]->ptr(ch), ctw, 0);
     }
     for (int b = 0; b < B; b++) out[b] = outs[b].release();
+}
+extern "C" int cnhe_vec_duplicate(cnhe_ctx *h, const cnhe_vec *a, uint64_t count, cnhe_vec **out) {
+    API_BEGIN(h)
+    duplicate_vecs(c, &a, 1, count, out);
     API_END
 }
-// cnhe_vec_permute of B vectors (one per client) with the same n_perm permutations of n_sel selections each: out[b * n_perm + j] is
-// bit-identical to cnhe_vec_permute(vecs[b], selections + j * n_sel, shifts + j * n_sel, n_sel, output_dim).  Per wave of clients the
-// mask products are one outer product of the clients and the distinct selections, and every (client, permutation, selection) rotation
-// goes into one op_rotate_rows_multi; then each output's sum in the reference's order (":1446-1461").
-extern "C" int cnhe_vecs_permute_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int B, const cnhe_vec *const *selections, const int *shifts,
-                                       int n_perm, int n_sel, uint64_t output_dim, cnhe_vec **out) {
+extern "C" int cnhe_vecs_duplicate_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int B, uint64_t count, cnhe_vec **out) {
     API_BEGIN(h)
+    duplicate_vecs(c, vecs, B, count, out);
+    API_END
+}
+// Permute (AtomicSealBfvVector.cs:1436-1475) of B vectors (one per client) with the same n_perm permutations of n_sel selections each:
+// out[b * n_perm + j] permutes vecs[b] with selections + j * n_sel and shifts + j * n_sel.  Per wave of clients the mask products are one
+// outer product of the clients and the distinct selections, and every (client, permutation, selection) rotation goes into one
+// op_rotate_rows_multi; then each output's sum in the reference's order (":1446-1461").
+static void permute_vecs(Context &c, const cnhe_vec *const *vecs, int B, const cnhe_vec *const *selections, const int *shifts, int n_perm,
+                         int n_sel, uint64_t output_dim, cnhe_vec **out) {
     const std::vector<int> slots = batch_inputs(c, vecs, B, out);
     if (!selections || !shifts || n_perm < 1 || n_sel < 1) fail("bad arguments");
     const cnhe_vec *a = vecs[0];
@@ -2265,6 +2183,7 @@ extern "C" int cnhe_vecs_permute_batch(cnhe_ctx *h, const cnhe_vec *const *vecs,
             std::vector<const u64 *> cts(nb);
             for (int j = 0; j < nb; j++) cts[j] = vecs[b0 + j]->ptr(ch);
             op_multiply_plain_dense_outer(c, ch, cts, plains, S, prod);
+            c.op_count[Context::OP_MULTIPLY_PLAIN] += (uint64_t)nb * (terms - S); // one per term, as the reference issues them
             std::vector<RotateJob> jobs; // (client, permutation, selection) in that order: the terms of an output are consecutive
             for (int bb = 0; bb < nb; bb++)
                 for (size_t q = 0; q < sel_index.size(); q++)
@@ -2286,6 +2205,17 @@ extern "C" int cnhe_vecs_permute_batch(cnhe_ctx *h, const cnhe_vec *const *vecs,
         }
     }
     for (size_t o = 0; o < outs.size(); o++) out[o] = outs[o].release();
+}
+extern "C" int cnhe_vec_permute(cnhe_ctx *h, const cnhe_vec *a, const cnhe_vec *const *selections, const int *shifts, int n, uint64_t output_dim,
+                                cnhe_vec **out) {
+    API_BEGIN(h)
+    permute_vecs(c, &a, 1, selections, shifts, 1, n, output_dim, out);
+    API_END
+}
+extern "C" int cnhe_vecs_permute_batch(cnhe_ctx *h, const cnhe_vec *const *vecs, int B, const cnhe_vec *const *selections, const int *shifts,
+                                       int n_perm, int n_sel, uint64_t output_dim, cnhe_vec **out) {
+    API_BEGIN(h)
+    permute_vecs(c, vecs, B, selections, shifts, n_perm, n_sel, output_dim, out);
     API_END
 }
 // cnhe_vec_pointwise_multiply(vecs[i], plain) of n encrypted vectors and one plain dense vector, one outer product per channel and block:

@@ -261,9 +261,10 @@ int cnhe_vecs_generate_sparse_of_array(cnhe_ctx *, const cnhe_vec *const *vecs, 
  * differ).  Each output is bit-identical to the single call named; every key-switching stage runs as one wave over all clients, and the
  * plain products of several clients with the same plaintexts transform each plaintext once.  The inputs must share dimension, scale,
  * format, block count and encryption (CNHE_ERR_INVALID otherwise, as for B < 1); other refusals are the single call's.
- * cnhe_vecs_duplicate_batch: out[b] = cnhe_vec_duplicate(vecs[b], count).
+ * cnhe_vecs_duplicate_batch: out[b] = cnhe_vec_duplicate(vecs[b], count); cnhe_vec_duplicate is the case B = 1.
  * cnhe_vecs_permute_batch: out[b * n_perm + j] = cnhe_vec_permute(vecs[b], selections + j * n_sel, shifts + j * n_sel, n_sel, output_dim)
- *   (selections [n_perm][n_sel], NULL entries skipped; LLPreConvLayer's permutations of one image).
+ *   (selections [n_perm][n_sel], NULL entries skipped; LLPreConvLayer's permutations of one image); cnhe_vec_permute is the case B = 1,
+ *   n_perm = 1.  Both count one PlainMultiplication per non-NULL selection of every output, a selection listed twice included.
  * cnhe_vecs_interleave_batch: out[b] = cnhe_vecs_interleave(vecs + b * n, n, shift), vecs [B][n].
  * cnhe_vecs_multiply_plain: out[i] = cnhe_vec_pointwise_multiply(vecs[i], plain) for n encrypted vectors and one plain dense vector. */
 int cnhe_vecs_duplicate_batch(cnhe_ctx *, const cnhe_vec *const *vecs, int B, uint64_t count, cnhe_vec **out /*B*/);
@@ -272,7 +273,7 @@ int cnhe_vecs_permute_batch(cnhe_ctx *, const cnhe_vec *const *vecs, int B, cons
 int cnhe_vecs_interleave_batch(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int B, int shift, cnhe_vec **out /*B*/);
 int cnhe_vecs_multiply_plain(cnhe_ctx *, const cnhe_vec *const *vecs, int n, const cnhe_vec *plain, cnhe_vec **out /*n*/);
 /* cnhe_vec_rotate of n vectors by the same amount in one pass (out[i] = rotation of vecs[i]); the vectors may belong to different key
- * slots.  Bit-identical to n cnhe_vec_rotate calls. */
+ * slots.  Bit-identical to n cnhe_vec_rotate calls; cnhe_vec_rotate is the case n = 1. */
 int cnhe_vecs_rotate(cnhe_ctx *, const cnhe_vec *const *vecs, int n, int amount, cnhe_vec **out /*n*/);
 
 /* ---- IMatrix.Mul and the fused layer entry points ------------------------------------------------------------------ */

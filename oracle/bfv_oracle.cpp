@@ -616,6 +616,12 @@ extern "C" int orc_get_galois_key(const orc_ctx *c, u64 elt, u64 *out) {
     memcpy(out, it->second.data.data(), it->second.data.size() * 8);
     return 0;
 }
+extern "C" int orc_set_galois_key(orc_ctx *c, u64 elt, const u64 *in) {
+    auto it = c->glk.find(elt);
+    if (it == c->glk.end()) return fail("Galois key not present");
+    memcpy(it->second.data.data(), in, it->second.data.size() * 8);
+    return 0;
+}
 
 /* ------------------------------------------------------------------ BatchEncoder (SEAL batchencoder.cpp) */
 extern "C" void orc_encode(const orc_ctx *c, const u64 *values, size_t n, u64 *plain) {

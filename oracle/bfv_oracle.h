@@ -62,6 +62,8 @@ int orc_galois_elt_count(const orc_ctx *);
 void orc_get_galois_elts(const orc_ctx *, uint64_t *out);
 int orc_galois_key_count(const orc_ctx *); /* digits per element */
 int orc_get_galois_key(const orc_ctx *, uint64_t elt, uint64_t *out /*count*2*k*N*/);
+/* replaces the key of an element the context holds: the rotations of a server's client key slot, whose keys are not keygen's */
+int orc_set_galois_key(orc_ctx *, uint64_t elt, const uint64_t *in /*count*2*k*N*/);
 
 /* BatchEncoder */
 void orc_encode(const orc_ctx *, const uint64_t *values, size_t n, uint64_t *plain /*N*/);

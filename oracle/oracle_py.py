@@ -148,6 +148,13 @@ class Oracle:
         self._chk(self.L.orc_get_galois_key(self.h, C.c_uint64(elt), _p(a)))
         return a.reshape(n, 2, self.k, self.N)
 
+    def set_galois_key(self, elt, key):
+        """Replaces the key of an element this context holds with `key` [count][2][k][N] (another key set's, e.g. a client key slot's)."""
+        a = _u64(key).ravel()
+        if a.size != self.L.orc_galois_key_count(self.h) * self.ct_words:
+            raise ValueError("wrong Galois key size")
+        self._chk(self.L.orc_set_galois_key(self.h, C.c_uint64(elt), _p(a)))
+
     # encoder
     def encode(self, values):
         v = _u64(values)
