@@ -39,6 +39,7 @@ _SIGS = {
     "cnhe_vec_key_slot": [VECP, C.POINTER(i32)],
     "cnhe_context_derive_level": [C.c_void_p, i32, C.POINTER(C.c_void_p)],
     "cnhe_vecs_mod_switch": [C.c_void_p, C.POINTER(VECP), i32, C.c_void_p, C.POINTER(VECP)],
+    "cnhe_vecs_sanitize": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_vecs_rotate": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_vecs_stack_batch": [C.c_void_p, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],
     "cnhe_mat_mul_rowmajor_batch": [C.c_void_p, C.POINTER(VECP), i32, C.POINTER(VECP), i32, i32, C.POINTER(VECP)],

@@ -350,6 +350,30 @@ cudaError_t launch_encrypt_finish(u64 *ct, const u64 *plain, size_t plain_stride
 cudaError_t launch_encrypt_finish_sk(u64 *ct, const u64 *as, const u64 *plain, size_t plain_stride, int n, int coeffs, const RngKey &seed, u64 nonce0,
                                      int k, int logn, const BehzConst *bc, PlainConst pc, cudaStream_t s);
 
+// ---- sanitisation (circuit privacy, DESIGN 4.18).  Ciphertext i of a call draws under nonce v = *base + i (base: the word the
+// one-thread take kernel wrote) on the streams stream_id(purpose, v mod 2^32, v >> 32) of these purposes: u, e0, e1 and the flood f
+constexpr u64 PURPOSE_SAN_U = 16, PURPOSE_SAN_E0 = 17, PURPOSE_SAN_E1 = 18, PURPOSE_SAN_F = 19;
+constexpr u64 SANITIZE_NONCES = 1ULL << 48; // nonces per channel key: 32 bits in the stream id's middle field, 16 in its low field
+__host__ __device__ __forceinline__ u64 sanitize_stream(u64 purpose, u64 nonce) { return stream_id(purpose, nonce & 0xffffffffULL, nonce >> 32); }
+// the flood f of one coefficient: words w_j = rng64(stream(PURPOSE_SAN_F), x W + j), j < W = ceil((b + 1) / 64), read as one
+// little-endian integer F of b + 1 bits (the top word masked); f = F - 2^b
+struct SanitizeConst {
+    int k, words;        // W
+    u64 top_mask;        // mask of word W - 1
+    DMod q[KMAX];
+    u64 pow2b[KMAX];     // 2^b mod q_l
+};
+// *base = *counter, *counter += n (one thread)
+cudaError_t launch_sanitize_take(u64 *counter, u64 n, u64 *base, cudaStream_t s);
+// u[i][l][x] = ternary of ciphertext i, lifted into every q_l, i < n
+cudaError_t launch_sanitize_u(u64 *u, int n, const u64 *base, const RngKey &rk, int k, int logn, const BehzConst *bc, cudaStream_t s);
+// out[i][p][l] = pk_tab[i][p][l] * u[i][l] (NTT form); ref: the pk_tab entries are key references (key_base)
+cudaError_t launch_sanitize_upk(const u64 *const *pk_tab, const u64 *u, u64 *out, int n, int k, int logn, const BehzConst *bc, bool ref,
+                                cudaStream_t s);
+// out[i] = in[i] + out[i] + (e0 + f, e1) (coefficient form; out holds u pk): one thread per coefficient of a ciphertext
+cudaError_t launch_sanitize_finish(const u64 *const *in, u64 *out, int n, const u64 *base, const RngKey &rk, const SanitizeConst &S, int logn,
+                                   cudaStream_t s);
+
 // ---- compact ciphertext upload (compact.cu; format in its header comment)
 // stream-id purposes no other sampler call uses: the expanded c1, the noise e of a secret-key encryption, a test-seeded expansion key;
 // the expanded a and the noise e of a compact key set's pairs

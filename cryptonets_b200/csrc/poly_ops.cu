@@ -412,6 +412,92 @@ __global__ void __launch_bounds__(256) k_encrypt_finish_sk(u64 *ct, const u64 *_
     }
     ct[c * 2 * kN + r] = v;
 }
+// ---------------------------------------------------------------- sanitisation (DESIGN 4.18)
+__global__ void k_sanitize_take(u64 *counter, u64 n, u64 *base) {
+    const u64 v = *counter;
+    *base = v;
+    *counter = v + n;
+}
+// one thread per coefficient: the ternary draw once, written into every residue
+__global__ void __launch_bounds__(256) k_sanitize_u(u64 *__restrict__ u, int n, const u64 *__restrict__ base, RngKey rk, int k, int logn,
+                                                   const BehzConst *__restrict__ bc) {
+    const int N = 1 << logn;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)n << logn) return;
+    const size_t c = i >> logn;
+    const int x = (int)(i & (N - 1));
+    const int v = draw_ternary(rng64(rk, sanitize_stream(PURPOSE_SAN_U, *base + c), (u64)x));
+    u64 *dst = u + c * k * N + x;
+    for (int l = 0; l < k; l++) dst[(size_t)l * N] = lift_small(v, bc->q[l].p);
+}
+template <bool REF>
+__global__ void __launch_bounds__(256) k_sanitize_upk(const u64 *const *__restrict__ pk_tab, const u64 *__restrict__ u, u64 *__restrict__ out, int n,
+                                                     int k, int logn, const BehzConst *__restrict__ bc) {
+    const size_t kN = (size_t)k << logn;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)n * 2 * kN) return;
+    const size_t c = i / (2 * kN), r = i % (2 * kN), w = r % kN;
+    const u64 *pk = key_base<REF>(pk_tab[c]);
+    out[i] = mulmod(pk[r], u[c * kN + w], bc->q[w >> logn]);
+}
+// One thread per coefficient x of ciphertext c: e0, e1 and the W flood words are drawn once, F is reduced into each q_l by Horner over the
+// words (barrett128 of r 2^64 + w_j), and the 2k words of the coefficient are read from in and out and written to out once
+__global__ void __launch_bounds__(256) k_sanitize_finish(const u64 *const *__restrict__ in, u64 *__restrict__ out, int n, const u64 *__restrict__ base,
+                                                        RngKey rk, const __grid_constant__ SanitizeConst S, int logn) {
+    const int N = 1 << logn, k = S.k, W = S.words;
+    const size_t kN = (size_t)k * N;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)n << logn) return;
+    const size_t c = i >> logn;
+    const int x = (int)(i & (N - 1));
+    const u64 nonce = *base + c;
+    const int e0 = draw_noise(rng64(rk, sanitize_stream(PURPOSE_SAN_E0, nonce), (u64)x));
+    const int e1 = draw_noise(rng64(rk, sanitize_stream(PURPOSE_SAN_E1, nonce), (u64)x));
+    const u64 sf = sanitize_stream(PURPOSE_SAN_F, nonce);
+    u64 w[KMAX];
+#pragma unroll
+    for (int j = 0; j < KMAX; j++)
+        if (j < W) w[j] = rng64(rk, sf, (u64)x * W + j) & (j == W - 1 ? S.top_mask : ~0ULL); // constant indices: w stays in registers
+    const u64 *src = in[c] + x;
+    u64 *dst = out + c * 2 * kN + x;
+    for (int l = 0; l < k; l++) {
+        const DMod q = S.q[l];
+        u64 F = 0;
+#pragma unroll
+        for (int j = KMAX - 1; j >= 0; j--)
+            if (j < W) F = barrett128(U128{w[j], F}, q);
+        const u64 f = submod(F, S.pow2b[l], q.p);
+        const size_t o0 = (size_t)l * N, o1 = kN + o0;
+        const u64 v0 = addmod(addmod(src[o0], dst[o0], q.p), addmod(lift_small(e0, q.p), f, q.p), q.p);
+        const u64 v1 = addmod(addmod(src[o1], dst[o1], q.p), lift_small(e1, q.p), q.p);
+        dst[o0] = v0;
+        dst[o1] = v1;
+    }
+}
+cudaError_t launch_sanitize_take(u64 *counter, u64 n, u64 *base, cudaStream_t s) {
+    k_sanitize_take<<<1, 1, 0, s>>>(counter, n, base);
+    return cudaGetLastError();
+}
+cudaError_t launch_sanitize_u(u64 *u, int n, const u64 *base, const RngKey &rk, int k, int logn, const BehzConst *bc, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    k_sanitize_u<<<blocks_for((size_t)n << logn), 256, 0, s>>>(u, n, base, rk, k, logn, bc);
+    return cudaGetLastError();
+}
+cudaError_t launch_sanitize_upk(const u64 *const *pk_tab, const u64 *u, u64 *out, int n, int k, int logn, const BehzConst *bc, bool ref,
+                                cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    const unsigned g = blocks_for(((size_t)n * 2 * k) << logn);
+    if (ref) k_sanitize_upk<true><<<g, 256, 0, s>>>(pk_tab, u, out, n, k, logn, bc);
+    else k_sanitize_upk<false><<<g, 256, 0, s>>>(pk_tab, u, out, n, k, logn, bc);
+    return cudaGetLastError();
+}
+cudaError_t launch_sanitize_finish(const u64 *const *in, u64 *out, int n, const u64 *base, const RngKey &rk, const SanitizeConst &S, int logn,
+                                   cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    k_sanitize_finish<<<blocks_for((size_t)n << logn), 256, 0, s>>>(in, out, n, base, rk, S, logn);
+    return cudaGetLastError();
+}
+
 __global__ void __launch_bounds__(256) k_fill_zero(u64 *p, size_t words) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < words) p[i] = 0;

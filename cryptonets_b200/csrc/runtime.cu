@@ -266,6 +266,7 @@ void end_part(Context &c, std::vector<Recording::Deferred> *hold) {
     std::unique_ptr<Recording> r = std::move(c.rec);
     cudaSetDevice(c.device);
     for (int i = 0; i < Context::OP_COUNT; i++) c.op_count[i] = r->op0[i]; // recording runs nothing
+    for (int i = 0; i < c.P; i++) c.ch[i].sanitized = r->sanitized0[i];
     c.launches = r->launches0;
     r->arena->recording = false;
     r->arena->free.clear();
@@ -403,6 +404,7 @@ Context::~Context() {
     if (d_tabs) cudaFree(d_tabs);
     if (d_table_mem) cudaFree(d_table_mem);
     if (d_index_map) cudaFree(d_index_map);
+    if (d_sanitize_nonce) cudaFree(d_sanitize_nonce);
     for (auto &r : prof_recs) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
     for (auto e : prof_pool) cudaEventDestroy(e);
     if (stage_buf) cudaFreeHost(stage_buf);
@@ -953,6 +955,8 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
             c.crt_coeff.push_back(minor * y);
         }
     }
+    CNHE_CUDA(cudaMalloc((void **)&c.d_sanitize_nonce, (size_t)P * 8));
+    CNHE_CUDA(cudaMemset(c.d_sanitize_nonce, 0, (size_t)P * 8));
     CNHE_CUDA(cudaDeviceSynchronize());
     return cp.release();
 }
@@ -1078,6 +1082,13 @@ KsKeys galois_keys(Context &c, int ch, int n, const int *slots, u64 elt) {
         auto it = ks.glk.find(elt);
         if (it == ks.glk.end()) throw Error(-3, "Galois key not present");
         key = it->second->p;
+        pk = nullptr;
+    });
+}
+static KsKeys public_keys(Context &c, int ch, int n, const int *slots) {
+    return pick_keys(c, ch, n, slots, KeyBinding::PK, 0, [](const KeySet &ks, const u64 *&key, const u64 *&pk) {
+        if (!ks.have_pk || !ks.pk) throw Error(-3, "public key is missing");
+        key = ks.pk->p;
         pk = nullptr;
     });
 }
@@ -1622,6 +1633,61 @@ void op_encrypt(Context &c, int chi, const u64 *plain, size_t plain_stride, int 
     }
     c.note(Context::OP_ENCRYPT, chi, n, ct);
 }
+// ---------------------------------------------------------------- sanitisation (DESIGN 4.18)
+int sanitize_max_bits(const Context &c) {
+    int best = 1 << 30;
+    for (u64 t : c.t) {
+        std::vector<u64> quot;
+        u64 rem;
+        hm::div_product(c.q, t, quot, rem); // floor(q / t): its bit length less one is floor(log2(q / t))
+        int bits = 0;
+        for (size_t i = quot.size(); i-- > 0;)
+            if (quot[i]) { bits = 64 * (int)i + hm::bit_length(quot[i]); break; }
+        best = std::min(best, bits - 1 - 2);
+    }
+    return best;
+}
+void sanitize_reserve(Context &c, int chi, u64 n) {
+    Channel &ch = c.ch[chi];
+    if (n > SANITIZE_NONCES - ch.sanitized)
+        throw Error(-3, "the channel's sampler key has handed out its 2^48 sanitisation nonces (cnhe_keys_generate_secure re-keys it)");
+    ch.sanitized += n;
+}
+void op_sanitize(Context &c, int chi, const std::vector<const u64 *> &in, const int *slots, int flood_bits, u64 *out) {
+    Channel &ch = c.ch[chi];
+    const int n = (int)in.size(), k = c.k;
+    const size_t N = c.N, kN = (size_t)k * N;
+    const KsKeys pks = public_keys(c, chi, n, slots);
+    SanitizeConst S;
+    memset(&S, 0, sizeof(S));
+    S.k = k;
+    S.words = flood_bits / 64 + 1; // ceil((b + 1) / 64)
+    S.top_mask = (flood_bits + 1) % 64 ? (1ULL << ((flood_bits + 1) % 64)) - 1 : ~0ULL;
+    for (int l = 0; l < k; l++) {
+        S.q[l] = c.h_bc.q[l];
+        S.pow2b[l] = hm::pw(2, (u64)flood_bits, c.q[l]);
+    }
+    sanitize_reserve(c, chi, (u64)n);
+    const int wave = c.wave(3 * kN);
+    for (int c0 = 0; c0 < n; c0 += wave) {
+        WsScope scope(c);
+        const int m = std::min(wave, n - c0);
+        u64 *base = c.ws_alloc(1), *u = c.ws_alloc((size_t)m * kN), *dst = out + (size_t)c0 * 2 * kN;
+        c.check(launch_sanitize_take(c.d_sanitize_nonce + chi, (u64)m, base, c.stream), "sanitize_take");
+        c.check(launch_sanitize_u(u, m, base, ch.rng, k, c.logN, c.d_bc, c.stream), "sanitize_u");
+        c.check(launch_ntt_forward(u, u, m * k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_forward");
+        std::vector<const u64 *> tab(m);
+        for (int i = 0; i < m; i++) tab[i] = pks.per_ct() ? pks.keys[c0 + i] : pks.key;
+        c.check(launch_sanitize_upk(key_table(c, tab, 0, m), u, dst, m, k, c.logN, c.d_bc, c.rec != nullptr, c.stream), "sanitize_upk");
+        c.check(launch_ntt_inverse(dst, dst, m * 2 * k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_inverse");
+        const std::vector<const u64 *> part(in.begin() + c0, in.begin() + c0 + m);
+        const u64 *const *in_tab = upload_ptrs(c, part);
+        PROF(6, (double)m * 3 * 2 * kN * 8); // in and u pk read, out written: 48 k N bytes per ciphertext
+        c.check(launch_sanitize_finish(in_tab, dst, m, base, ch.rng, S, c.logN, c.stream), "sanitize_finish");
+    }
+    c.note(Context::OP_ENCRYPT, chi, n, out);
+    c.note(Context::OP_ADD, chi, n, out);
+}
 CompactShape compact_shape(const Context &c) {
     CompactShape sh;
     memset(&sh, 0, sizeof(sh));
@@ -1881,6 +1947,8 @@ static void keys_generate_impl(Context &c, bool secure, u64 seed) {
         if (secure) rng_from_os(ch.rng);
         else { memset(&ch.rng, 0, sizeof(ch.rng)); ch.rng.seed = seed + (u64)ci; }
         ch.nonce = 1;
+        ch.sanitized = 0; // a new sampler key: its sanitisation nonces start again from 0
+        CNHE_CUDA(cudaMemsetAsync(c.d_sanitize_nonce + ci, 0, 8, c.stream));
         size_t words;
         // secret key: ternary, kept in NTT form (and a coefficient-form copy for the Galois keys)
         BufRef &sk = key_slot(c, ci, 0, 0, words, true);
@@ -1959,8 +2027,7 @@ void op_keys_save_compact(Context &c, int chi, int sets, const std::vector<u64> 
 }
 // pairs of one blob channel in order: public key, relinearisation digits, Galois digits of each element; `slot_of` gives each set's key buffer
 template <class SlotOf>
-static void keys_load_compact(Context &c, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key, SlotOf slot_of,
-                              bool skip_pk = false) {
+static void keys_load_compact(Context &c, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key, SlotOf slot_of) {
     const CompactShape sh = compact_shape(c);
     u64 kappa = 0;
     auto expand = [&](int what, u64 arg) {
@@ -1970,10 +2037,7 @@ static void keys_load_compact(Context &c, int sets, const std::vector<u64> &elts
         c.check(launch_compact_expand(slot->p, packed + kappa * sh.off[c.k], key, PURPOSE_KEYS_A, kappa, D, sh, c.d_bc, c.stream), "compact_expand");
         kappa += D;
     };
-    if (sets & 1) {
-        if (skip_pk) kappa += 1; // a key slot evaluates only: the public key pair is left in the blob
-        else expand(1, 0);
-    }
+    if (sets & 1) expand(1, 0);
     if (sets & 2) expand(2, 0);
     for (u64 elt : elts) expand(3, elt);
 }
@@ -1984,11 +2048,12 @@ void op_keys_load_compact(Context &c, int chi, int sets, const std::vector<u64> 
 }
 void op_keys_load_compact(Context &c, KeySet &dst, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key) {
     keys_load_compact(c, sets, elts, packed, key, [&](int what, u64 arg, size_t &words) -> BufRef & {
-        BufRef &b = what == 2 ? dst.rlk : dst.glk[arg];
-        words = (size_t)(what == 2 ? c.dm_relin.D : c.dm_galois.D) * c.ct_words();
+        BufRef &b = what == 1 ? dst.pk : what == 2 ? dst.rlk : dst.glk[arg];
+        words = (size_t)(what == 1 ? 1 : what == 2 ? c.dm_relin.D : c.dm_galois.D) * c.ct_words();
         if (!b) b = c.alloc(words);
         return b;
-    }, true);
+    });
+    if (sets & 1) dst.have_pk = true; // the key slot's sanitisation encrypts zero under it
     if (sets & 2) rlk_ready(c, dst); // synchronises the stream
 }
 
@@ -2042,13 +2107,13 @@ void restrict_keys(Context &dst, const Context &src, int s) {
         to.rlk.reset();
         to.rlk_packed.reset();
         to.glk.clear();
+        to.have_pk = from.have_pk && from.pk;
+        to.pk = to.have_pk ? cut(from.pk, 2) : nullptr;
         if (s == 0) {
             const Channel &fc = src.ch[ci];
             Channel &tc = dst.ch[ci];
             tc.have_sk = fc.have_sk && fc.sk;
-            tc.have_pk = fc.have_pk && fc.pk;
             tc.sk = tc.have_sk ? cut(fc.sk, 1) : nullptr;
-            tc.pk = tc.have_pk ? cut(fc.pk, 2) : nullptr;
         }
         for (const auto &g : from.glk) to.glk[g.first] = cut(g.second, (size_t)dst.dm_galois.D * 2);
         if (from.have_rlk && from.rlk) {

@@ -63,11 +63,11 @@ typedef std::shared_ptr<DevBuf> BufRef;
 
 // The key binding of a recorded graph (DESIGN 4.16).  While recording, every key base a key switch hands a kernel is replaced by a key
 // reference: the address of one word of `table`, a small device array the graph owns, that stands for one key of one key slot and
-// channel -- the relinearisation keys, their packed copy, or the keys of one Galois element.  The graph's key positions are the distinct
+// channel -- the relinearisation keys, their packed copy, the keys of one Galois element, or the public key (sanitisation).  The graph's key positions are the distinct
 // slots its references name, in ascending order.  Binding (cnhe_graph_bind) points every word of a position at another slot's key of
 // the same kind, and the next launch copies the words into the table before the recorded kernels read them.
 struct KeyBinding {
-    enum Kind { RLK, RLK_PACKED, GALOIS };
+    enum Kind { RLK, RLK_PACKED, GALOIS, PK };
     struct Key { int slot, channel, kind; u64 elt; int member; }; // member: the enlisted context whose key pick took it (RecGroup)
     std::map<const u64 *, Key> seen;      // while recording: every key base picked for a key switch, and which key it is
     std::map<const u64 *, size_t> word;   // key base -> its table word
@@ -96,6 +96,7 @@ struct Recording {
     std::shared_ptr<GraphArena> arena;  // shared by every member
     std::vector<uint64_t> op0;          // operation counters and kernel count when the recording began: restored when it ends, the
     uint64_t launches0 = 0;             // difference is what every launch of the graph adds
+    std::vector<uint64_t> sanitized0;   // the same for the channels' sanitisation nonces (Channel::sanitized)
     std::shared_ptr<KeyBinding> keys;   // the references the recorded key switches read their keys through (shared by every member)
     std::vector<std::shared_ptr<void>> keep; // cached host-built device tables (scalar-MAC plans) the recorded kernels read
     // buffers allocated before the recording and released during it: the graph may read them, so they are freed (or recycled) outside
@@ -104,10 +105,10 @@ struct Recording {
     std::vector<Deferred> deferred;
 };
 
-// the evaluation keys of one client under one plaintext modulus
+// the keys of one client under one plaintext modulus: evaluation keys, and the public key that sanitisation encrypts zero under
 struct KeySet {
-    bool have_rlk = false;
-    BufRef rlk;
+    bool have_rlk = false, have_pk = false;
+    BufRef rlk, pk;   // pk: [2][k][N] NTT form
     BufRef rlk_packed; // rlk with 48-bit words for the fused key switch (set by rlk_ready when that kernel can run and every q_l < 2^48)
     std::map<u64, BufRef> glk;
 };
@@ -115,10 +116,14 @@ struct Channel : KeySet { // one plaintext modulus (one AtomicSealBfvEncryptedEn
     u64 t = 0;
     PlainConst pc;
     int mod_id = 0; // NTT table id of t
-    bool have_sk = false, have_pk = false;
-    BufRef sk, pk;
+    bool have_sk = false;
+    BufRef sk;
     RngKey rng;    // secure (ChaCha20 keyed from the OS) unless a deterministic test seed was requested explicitly
     u64 nonce = 1; // running encryption counter (32 bits enter the stream id; a secure channel re-keys before it wraps)
+    // Sanitisation nonces (DESIGN 4.18) come from a device counter, d_sanitize_nonce[channel], that the call's first kernel reads and
+    // advances, so that every replay of a recorded graph draws fresh randomness; `sanitized` is the host's count of the nonces handed out
+    // (eager calls and graph launches), which keeps the counter below SANITIZE_NONCES
+    u64 sanitized = 0;
     FloorConstF floor_f; // folded fast_floor constants for this t (valid when the context's fp_elementwise is set)
 };
 
@@ -147,6 +152,7 @@ struct Context {
     int slot = 0; // key slot of the ciphertexts the current public call works on (reset to 0 by every call; vec.cu sets it from the operands)
     bool foreign = false; // the current call touches ciphertexts of a slot other than 0: the noise trace cannot measure them (no secret key)
     bool slot_live(int s) const { return s == 0 || (s > 0 && (size_t)s <= clients.size() && !clients[s - 1].empty()); }
+    u64 *d_sanitize_nonce = nullptr; // [P] device counters of the channels' sanitisation nonces (Channel::sanitized)
     const KeySet &keys(int channel, int s) const;
     // key generation of a slot: bumped whenever its keys are replaced or removed, so that a graph recorded against them refuses to launch
     std::map<int, uint64_t> key_gen;
@@ -234,8 +240,9 @@ struct Context {
     struct ProfRec { int family; double bytes; cudaEvent_t e0, e1; };
     std::vector<ProfRec> prof_recs;
     std::vector<cudaEvent_t> prof_pool;
-    double prof_ms[6] = {0, 0, 0, 0, 0, 0}, prof_bytes[6] = {0, 0, 0, 0, 0, 0};
-    uint64_t prof_n[6] = {0, 0, 0, 0, 0, 0};
+    static constexpr int PROF_FAMILIES = 7; // cnhe_prof_collect's families; 6: the sanitisation finish kernel
+    double prof_ms[PROF_FAMILIES] = {0}, prof_bytes[PROF_FAMILIES] = {0};
+    uint64_t prof_n[PROF_FAMILIES] = {0};
     void prof_begin(int family, double bytes);
     void prof_end();
     void prof_flush();
@@ -419,5 +426,14 @@ void op_keys_load_compact(Context &c, int ch, int sets, const std::vector<u64> &
 // the same into a key slot's key set (relinearisation and Galois keys; a public key pair in the blob is skipped)
 void op_keys_load_compact(Context &c, KeySet &dst, int sets, const std::vector<u64> &elts, const u64 *packed, const CompactKey &key);
 int op_noise_budget(Context &c, int ch, const u64 *ct);
+// ---- sanitisation (circuit privacy, DESIGN 4.18; kernels in sanitize.cu)
+// the widest flood the context allows: floor(log2(q / t)) - 2 for the smallest such value over its plaintext moduli
+int sanitize_max_bits(const Context &c);
+// takes n sanitisation nonces of a channel on the host's count: CNHE_ERR_STATE when the count would pass SANITIZE_NONCES
+void sanitize_reserve(Context &c, int ch, u64 n);
+// out[i] = in[i] + (pk0 u + e0 + f, pk1 u + e1) under the public key of key slot slots[i] (n entries); u ternary, e0, e1 clipped normal,
+// f uniform in [-2^b, 2^b), drawn under the nonces the device counter hands out; out packed [n][2][k][N], coefficient form.  Counted as n
+// encryptions and n additions.  A slot without a public key is CNHE_ERR_STATE (-3)
+void op_sanitize(Context &c, int ch, const std::vector<const u64 *> &in, const int *slots, int flood_bits, u64 *out);
 
 } // namespace cnhe

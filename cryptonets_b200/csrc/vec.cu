@@ -174,6 +174,7 @@ struct cnhe_graph {
     std::shared_ptr<GraphArena> arena;
     std::vector<std::vector<uint64_t>> ops; // per member: the operation counts one launch adds
     std::vector<uint64_t> launches;         // per member: the kernel launches one launch adds (what the recorded calls counted)
+    std::vector<std::vector<uint64_t>> sanitized; // per member and channel: the sanitisation nonces one launch takes from the device counter
     uint64_t kernel_nodes = 0;
     // key binding (cnhe_graph_bind): the key positions (recorded slots, ascending), the slot each is bound to and, per member, that slot's
     // key generation when it was bound, and the words of the device table under that binding
@@ -238,6 +239,9 @@ static void bind_graph(cnhe_graph &g, const int *slots) {
             const auto it = ks.glk.find(k.elt);
             if (it == ks.glk.end()) missing("Galois key of element " + std::to_string(k.elt));
             words.push_back(it->second->p);
+        } else if (k.kind == KeyBinding::PK) {
+            if (!ks.have_pk || !ks.pk) missing("public key");
+            words.push_back(ks.pk->p);
         } else if (!ks.have_rlk || (k.kind == KeyBinding::RLK_PACKED && !ks.rlk_packed)) {
             missing(k.kind == KeyBinding::RLK ? "relinearization keys" : "packed relinearization keys");
         } else words.push_back(k.kind == KeyBinding::RLK ? ks.rlk->p : ks.rlk_packed->p);
@@ -267,7 +271,7 @@ static void start_recording(const std::vector<Context *> &members) {
     for (Context *m : members)
         for (int s = 0; s <= (int)m->clients.size(); s++)
             if (m->slot_live(s))
-                for (int ch = 0; ch < m->P; ch++) keys->cap += 2 + m->keys(ch, s).glk.size();
+                for (int ch = 0; ch < m->P; ch++) keys->cap += 3 + m->keys(ch, s).glk.size();
     const std::vector<const u64 *> zeros(keys->cap);
     keys->table = static_cast<const u64 **>(const_cast<void *>(arena->constant(zeros.data(), zeros.size() * sizeof(u64 *), c.copy_stream)));
     CNHE_CUDA(cudaStreamBeginCapture(c.streams[0], cudaStreamCaptureModeRelaxed));
@@ -280,6 +284,7 @@ static void start_recording(const std::vector<Context *> &members) {
         r->arena = arena;
         r->op0.assign(m.op_count, m.op_count + Context::OP_COUNT);
         r->launches0 = m.launches;
+        for (int ch = 0; ch < m.P; ch++) r->sanitized0.push_back(m.ch[ch].sanitized);
         r->keys = keys;
         m.rec = std::move(r);
     }
@@ -344,6 +349,9 @@ extern "C" int cnhe_capture_end(cnhe_ctx *h, cnhe_graph **out) {
         for (int i = 0; i < Context::OP_COUNT; i++) ops.push_back(m->op_count[i] - m->rec->op0[i]);
         g->ops.push_back(std::move(ops));
         g->launches.push_back(m->launches - m->rec->launches0);
+        std::vector<uint64_t> san;
+        for (int ch = 0; ch < m->P; ch++) san.push_back(m->ch[ch].sanitized - m->rec->sanitized0[ch]);
+        g->sanitized.push_back(std::move(san));
     }
     cudaGraph_t graph = end_capture(*grp, true);
     g->held.resize(g->members.size());
@@ -411,6 +419,16 @@ extern "C" int cnhe_graph_launch(cnhe_graph *g) {
                                                 " were removed or replaced after the graph was recorded or bound to it (cnhe_graph_bind)");
         }
     }
+    // a launch takes as many sanitisation nonces from each channel's device counter as the recording did: refused before it would pass
+    // the key's range, as the eager call is
+    for (size_t mi = 0; mi < g->members.size(); mi++) {
+        const Context &m = *g->members[mi];
+        for (int ch = 0; ch < m.P; ch++)
+            if (g->sanitized[mi][ch] > SANITIZE_NONCES - m.ch[ch].sanitized)
+                throw Error(CNHE_ERR_STATE, "cnhe_graph_launch: a channel's sampler key has handed out its 2^48 sanitisation nonces");
+    }
+    for (size_t mi = 0; mi < g->members.size(); mi++)
+        for (int ch = 0; ch < g->members[mi]->P; ch++) g->members[mi]->ch[ch].sanitized += g->sanitized[mi][ch];
     // after every call queued before, on any channel of any context the graph spans
     c.join_streams();
     for (size_t mi = 1; mi < g->members.size(); mi++) {
@@ -643,13 +661,13 @@ extern "C" int cnhe_prof_enable(cnhe_ctx *h, int on) {
     not_recorded(c, "profiles");
     c.prof_flush();
     c.prof = on != 0;
-    if (on) for (int i = 0; i < 6; i++) { c.prof_ms[i] = 0; c.prof_bytes[i] = 0; c.prof_n[i] = 0; }
+    if (on) for (int i = 0; i < Context::PROF_FAMILIES; i++) { c.prof_ms[i] = 0; c.prof_bytes[i] = 0; c.prof_n[i] = 0; }
     API_END
 }
 extern "C" int cnhe_prof_collect(cnhe_ctx *h, int family, double *total_ms, uint64_t *launches, double *bytes) {
     API_BEGIN(h)
     not_recorded(c, "profiles");
-    if (family < 0 || family > 5) fail("bad family");
+    if (family < 0 || family >= Context::PROF_FAMILIES) fail("bad family");
     c.prof_flush();
     if (total_ms) *total_ms = c.prof_ms[family];
     if (launches) *launches = c.prof_n[family];
@@ -1514,6 +1532,42 @@ extern "C" int cnhe_vecs_mod_switch(cnhe_ctx *h, const cnhe_vec *const *in, int 
     size_t ct = 0;
     for (int i = 0; i < n; i++) {
         out[i] = slab_output(d, slab, ct, in[i], in[i]->scale, slots[i]);
+        ct += in[i]->blocks;
+    }
+    API_END
+}
+// ---------------------------------------------------------------------------------------------------- sanitisation (DESIGN 4.18)
+extern "C" int cnhe_vecs_sanitize(cnhe_ctx *h, const cnhe_vec *const *in, int n, int flood_bits, cnhe_vec **out) {
+    API_BEGIN(h)
+    if (n < 1 || !in || !out) fail("bad arguments");
+    const int max_bits = sanitize_max_bits(c);
+    if (flood_bits < 0 || flood_bits > max_bits)
+        fail(("cnhe_vecs_sanitize: the flood width must be in [0, " + std::to_string(max_bits) + "] bits (floor(log2(q/t)) - 2)").c_str());
+    for (int i = 0; i < n; i++) {
+        same_ctx(c, in[i]); // a pending vector is relinearised here
+        if (!in[i]->enc) fail("cnhe_vecs_sanitize: only encrypted vectors are sanitised");
+    }
+    const std::vector<int> slots = vec_slots(c, in, n);
+    std::vector<int> ct_slot;
+    size_t total = 0;
+    for (int i = 0; i < n; i++) {
+        total += in[i]->blocks;
+        ct_slot.insert(ct_slot.end(), in[i]->blocks, slots[i]);
+    }
+    if (total > (size_t)INT_MAX) fail("cnhe_vecs_sanitize: too many ciphertexts");
+    std::vector<BufRef> slab(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        slab[ch] = c.alloc(total * c.ct_words());
+        std::vector<const u64 *> ptrs;
+        for (int i = 0; i < n; i++)
+            for (int b = 0; b < in[i]->blocks; b++) ptrs.push_back(in[i]->block(ch, b));
+        op_sanitize(c, ch, ptrs, ct_slot.data(), flood_bits, slab[ch]->p);
+    }
+    c.set_channel(0);
+    size_t ct = 0;
+    for (int i = 0; i < n; i++) {
+        out[i] = slab_output(c, slab, ct, in[i], in[i]->scale, slots[i]);
         ct += in[i]->blocks;
     }
     API_END

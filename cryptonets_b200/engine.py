@@ -376,6 +376,23 @@ class Engine:
         check(self.L.cnhe_vecs_mod_switch(self.h, _vec_array(vecs), n, to.h, out))
         return to._wrap_many(out, n, like=vecs)
 
+    # ---- sanitisation (include/cnhe.h, cnhe_vecs_sanitize; DESIGN 4.18)
+    def sanitize_max_bits(self):
+        """The widest flood sanitize accepts: floor(log2(q / t)) - 2 for the largest plaintext prime t."""
+        q = 1
+        for x in self.q:
+            q *= x
+        return min((q // t).bit_length() - 1 for t in self.primes) - 2
+
+    def sanitize(self, vecs, flood_bits):
+        """The encrypted vectors `vecs` (key slots may differ) re-randomised under their slots' public keys, with a uniform flood of
+        flood_bits bits in their noise: the results decrypt as the inputs do and reveal nothing else about how they were computed as long
+        as flood_bits covers the inputs' noise (DESIGN 4.18).  Outputs keep dimension, scale, format and key slot."""
+        n = len(vecs)
+        out = (VECP * n)()
+        check(self.L.cnhe_vecs_sanitize(self.h, _vec_array(vecs), n, int(flood_bits), out))
+        return self._wrap_many(out, n, like=vecs)
+
     def write_vector(self, vec):
         """EncryptedSealBfvVector.Write: the text form of one vector."""
         n = C.c_size_t()
@@ -580,7 +597,7 @@ class Engine:
         check(self.L.cnhe_prof_enable(self.h, int(on)))
 
     def prof_collect(self):
-        names = ["ntt_forward", "ntt_inverse", "behz_elementwise", "keyswitch_mac", "scalar_mac_layer", "other"]
+        names = ["ntt_forward", "ntt_inverse", "behz_elementwise", "keyswitch_mac", "scalar_mac_layer", "other", "sanitize_finish"]
         out = {}
         for i, nm in enumerate(names):
             ms, n, b = C.c_double(), C.c_uint64(), C.c_double()

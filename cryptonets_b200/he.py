@@ -511,6 +511,30 @@ class B200BfvFactory:
             i += n
         return res
 
+    # ---- sanitisation (include/cnhe.h, cnhe_vecs_sanitize; DESIGN 4.18)
+    def SanitizeMaxBits(self):
+        """The widest flood width Sanitize accepts, floor(log2(q/t)) - 2."""
+        return self.engine.sanitize_max_bits()
+
+    def Sanitize(self, m, flood_bits):
+        """An encrypted matrix or vector re-randomised under its key slot's public key with a flood of flood_bits bits in its noise: what
+        a result should be before it goes back to its client."""
+        return self.SanitizeBatch([m], flood_bits)[0]
+
+    def SanitizeBatch(self, items, flood_bits):
+        """Sanitize of several matrices or vectors (possibly of different clients) in one pass."""
+        vecs = [v.vec for it in items for v in (it.vectors if isinstance(it, B200BfvMatrix) else [it])]
+        out, i, res = self.engine.sanitize(vecs, flood_bits), 0, []
+        for it in items:
+            if isinstance(it, B200BfvMatrix):
+                n = len(it.vectors)
+                res.append(B200BfvMatrix(self, [B200BfvVector(self, o) for o in out[i:i + n]], it.Format, CopyVectors=False))
+            else:
+                n = 1
+                res.append(B200BfvVector(self, out[i]))
+            i += n
+        return res
+
     # ---- wire formats (IFactory.cs:474-495; SEAL streams unpinned, see csrc/wire.cu)
     def Save(self, target, withPrivateKeys=False):
         """IFactory.Save(stream | fileName, withPrivateKeys): the ZIP key archive."""

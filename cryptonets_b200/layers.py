@@ -306,6 +306,32 @@ class ModSwitchLayer(BaseLayer):
         return f.ModSwitchBatch(ms, self.Factory)
 
 
+class SanitizeLayer(BaseLayer):
+    """Sanitises the network's output before it goes back to its client (circuit privacy, DESIGN 4.18): every ciphertext gets a fresh
+    public-key encryption of zero under its client's key and a uniform flood in its noise, FloodBits = NoiseBits + StatisticalBits +
+    log2 N bits wide, so that for an output noise of at most 2^NoiseBits (infinity norm) the decrypted noise is within statistical
+    distance 2^-StatisticalBits of one independent of the weights and of the client's input noise.  NoiseBits is a stated bound
+    (networks.OUTPUT_NOISE_BITS): the server cannot measure the noise.  The values are unchanged while the output's noise budget exceeds
+    about FloodBits + 2 bits.  A factory without sanitisation (RawFactory) passes the matrix through."""
+
+    def __init__(self, **kw):
+        self.NoiseBits = None
+        self.StatisticalBits = 40
+        super().__init__(**kw)
+
+    def FloodBits(self, N):
+        return int(self.NoiseBits) + int(self.StatisticalBits) + int(N).bit_length() - 1
+
+    def Apply(self, m):
+        return self.ApplyBatch([m])[0]
+
+    def ApplyBatch(self, ms):
+        f = self.Factory
+        if not hasattr(f, "SanitizeBatch"):
+            return list(ms)
+        return f.SanitizeBatch(ms, self.FloodBits(f.engine.N))
+
+
 class SquareActivation(BaseLayer):
     """`NeuralNetworks/SquareActivation.cs:8-20`"""
 

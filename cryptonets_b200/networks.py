@@ -12,7 +12,7 @@ import numpy as np
 from .interfaces import EVectorFormat
 from .layers import (ConvolutionEngine, EncryptLayer, LLConvReader, LLDenseLayer, LLDuplicateLayer, LLInterleavedDenseLayer, LLInterleaveLayer,
                      LLPackedDenseLayer, LLPoolLayer, LLPreConvLayer, LLSingleLineReader, LLVectorizeLayer, MatrixSource, ModSwitchLayer, PoolLayer,
-                     SquareActivation, TimingLayer)
+                     SanitizeLayer, SquareActivation, TimingLayer)
 
 _MODELS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "models")
 CRYPTONETS_PRIMES = [549764251649, 549764284417]  # CryptoNets.cs:17
@@ -57,10 +57,10 @@ def synthetic_mnist(n_images, seed=20240917):
     return px.astype(np.float64)
 
 
-def cryptonets_mnist(factory, images, batch_size=None, fused=True, weights=None, timing=True, defer_relinearization=False):
+def cryptonets_mnist(factory, images, batch_size=None, fused=True, weights=None, timing=True, defer_relinearization=False, sanitize=False):
     """Returns (network, reader).  network.GetNext() yields the 10-column score matrix of one batch.  defer_relinearization: both dense
     layers square their input and relinearise only their outputs (PoolLayer.DeferRelinearization): same scores, 110 relinearisations per
-    plaintext prime instead of 945."""
+    plaintext prime instead of 945.  sanitize: end in a SanitizeLayer under OUTPUT_NOISE_BITS (circuit privacy, DESIGN 4.18)."""
     w = weights or cryptonets_weights()
     weightscale = 32
     reader = MatrixSource(images, Scale=16.0, NormalizationFactor=1.0 / 256.0, MaxSlots=batch_size or len(images))
@@ -75,11 +75,12 @@ def cryptonets_mnist(factory, images, batch_size=None, fused=True, weights=None,
     act4 = SquareActivation(Source=dense3)
     dense5 = PoolLayer(Source=act4, InputShape=[100], KernelShape=[100], Stride=[1000], MapCount=[10], Weights=w["Weights_3"],
                        Bias=w["Biases_3"], WeightsScale=weightscale, Fused=fused, DeferRelinearization=defer_relinearization)
-    net = TimingLayer(Source=dense5, StopCounters=["Batch-Time"]) if timing else dense5
+    out = _sanitized("cryptonets_mnist", dense5, sanitize)
+    net = TimingLayer(Source=out, StopCounters=["Batch-Time"]) if timing else out
     return net, reader
 
 
-def lola_small(factory, images, weights=None, dense_method="rows", levels=None):
+def lola_small(factory, images, weights=None, dense_method="rows", levels=None, sanitize=False):
     """dense_method: LLDenseLayer.Method of the 10 x 845 score layer ("rows", the reference's, or "folded": dense scores in one
     ciphertext per plaintext prime).  levels: {layer: k'} switches to k' coefficient primes after the named layers (conv1, vec2, act3)."""
     lv = _Levels(levels, ["conv1", "vec2", "act3"])
@@ -93,7 +94,7 @@ def lola_small(factory, images, weights=None, dense_method="rows", levels=None):
     vec2 = LLVectorizeLayer(Source=lv("conv1", conv1))
     act3 = SquareActivation(Source=lv("vec2", vec2))
     dense4 = LLDenseLayer(Source=lv("act3", act3), Bias=w["Biases_1"], Weights=w["Weights_1"], WeightsScale=weightscale, Method=dense_method)
-    return dense4, reader
+    return _sanitized("lola_small", dense4, sanitize), reader
 
 
 # Level schedules ({layer: k'}) for the parameters of each network's end-to-end GPU test (tools/level_bench.py NETS): the output of
@@ -106,6 +107,22 @@ LEVEL_SCHEDULES = {
     "lola_large": {"act3": 7, "dense4": 5, "act5": 4},              # k = 8; 210, 123, 79
     "lola_cifar": {"act3": 8, "dense4": 5, "act5": 4},              # k = 9; 232, 127, 73
 }
+
+
+# Output-noise bounds ({network: e}) for the parameters of each network's end-to-end GPU test (tools/level_bench.py NETS; CryptoNets-MNIST
+# at N = 8192 and its reference q): the largest infinity norm of the output noise, log2, measured exactly with the secret key over several
+# seeded inferences by `python tools/output_noise.py`, plus a margin of OUTPUT_NOISE_MARGIN bits.  SanitizeLayer floods e + 40 + log2 N bits.
+OUTPUT_NOISE_MARGIN = 4
+OUTPUT_NOISE_BITS = {"lola_small": 134, "lola": 198, "lola_dense": 327, "lola_large": 332, "lola_cifar": 386, "cryptonets_mnist": 170}
+
+
+def _sanitized(name, layer, sanitize):
+    """layer, or a SanitizeLayer after it under the network's committed output-noise bound"""
+    if not sanitize:
+        return layer
+    if name not in OUTPUT_NOISE_BITS:
+        raise ValueError("no output-noise bound is committed for %s (tools/output_noise.py)" % name)
+    return SanitizeLayer(Source=layer, NoiseBits=OUTPUT_NOISE_BITS[name])
 
 
 class _Levels:
@@ -147,7 +164,7 @@ def serve_batch(net, inputs):
     return ms
 
 
-def lola(factory, images, weights=None, levels=None):
+def lola(factory, images, weights=None, levels=None, sanitize=False):
     """LoLa (`LowLatencyCryptoNets/LoLaCryptonets.cs:203-276`): im2col input, 8-way packed dense layer, interleave, square, dense.
     levels: {layer: k'} switches to k' coefficient primes after the named layers (conv1 .. act7)."""
     lv = _Levels(levels, ["conv1", "vec2", "act3", "dup4", "dense5", "inter6", "act7"])
@@ -168,10 +185,10 @@ def lola(factory, images, weights=None, levels=None):
     act7 = SquareActivation(Source=lv("inter6", inter6))
     dense8 = LLInterleavedDenseLayer(Source=lv("act7", act7), Weights=w["Weights_3"], Bias=w["Biases_3"], WeightsScale=weightscale, Shift=-1,
                                      SelectedIndices=sel)
-    return dense8, reader
+    return _sanitized("lola", dense8, sanitize), reader
 
 
-def lola_dense(factory, images, weights=None, levels=None):
+def lola_dense(factory, images, weights=None, levels=None, sanitize=False):
     """LoLa-Dense (`LoLaCryptonets.cs:116-201`): the image arrives as ONE ciphertext; the im2col columns are built homomorphically
     (LLPreConvLayer), 16-way packed dense layer, square, interleave, dense.  levels: {layer: k'} switches to k' coefficient primes after
     the named layers (pre1 .. inter8)."""
@@ -193,7 +210,7 @@ def lola_dense(factory, images, weights=None, levels=None):
     inter8 = LLInterleaveLayer(Source=lv("act7", act7), Shift=-1, SelectedIndices=sel)
     dense9 = LLInterleavedDenseLayer(Source=lv("inter8", inter8), Weights=w["Weights_3"], Bias=w["Biases_3"], WeightsScale=weightscale, Shift=-1,
                                      SelectedIndices=sel)
-    return dense9, reader
+    return _sanitized("lola_dense", dense9, sanitize), reader
 
 
 def cifar_weights(seed=7, synthetic=False):
@@ -216,7 +233,8 @@ def synthetic_cifar(n_images, seed=20240917):
     return np.random.default_rng(seed).integers(0, 256, (n_images, 3 * 32 * 32)).astype(np.float64)
 
 
-def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows", levels=None):
+def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows", levels=None,
+               sanitize=False):
     """LoLa-CIFAR (`CifarCryptoNet/LolaCifarCryptoNet.cs:27-131`): 3x32x32 image as an im2col matrix [196 x 192], conv 83 maps,
     square, the second convolution as a 5488 x 16268 row-major dense layer (rotate-and-sum per row), square, dense 5488 -> 10.
     dense_method: LLDenseLayer.Method of that layer ("rows", the reference's, or "diagonal"); diag_ntt_bytes: its DiagonalNttBytes;
@@ -242,7 +260,7 @@ def lola_cifar(factory, images, weights=None, shard=None, dense_method="rows", d
     act5 = SquareActivation(Source=lv("dense4", dense4))
     dense6 = LLDenseLayer(Source=lv("act5", act5), Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512.0, InputFormat=EVectorFormat.dense,
                           Method=score_method)
-    return dense6, reader
+    return _sanitized("lola_cifar", dense6, sanitize), reader
 
 
 def lola_large_weights(seed=9, synthetic=False):
@@ -261,7 +279,8 @@ def lola_large_weights(seed=9, synthetic=False):
                 Biases_1=draw(163, 0.039, 0.09), Weights_2=draw(10 * 2608, 0.42, 1.63), Biases_2=draw(10, 1.6, 3.9))
 
 
-def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows", levels=None):
+def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_bytes=0, score_method="rows", levels=None,
+               sanitize=False):
     """Large LoLa (`LoLaCryptonets.cs:330-409`): 28x28 image as im2col [144 x 64], conv 83 maps of 8x8 stride 2 (pixels are NOT
     normalised; the weights carry the 1/256), square, the second convolution (163 maps of 83x6x6, stride 2 over 83x12x12) as a
     2608 x 11952 row-major dense layer with ForceDenseFormat, square, dense 2608 -> 10.  dense_method: that layer's LLDenseLayer.Method,
@@ -285,4 +304,4 @@ def lola_large(factory, images, weights=None, dense_method="rows", diag_ntt_byte
     act5 = SquareActivation(Source=lv("dense4", dense4))
     dense6 = LLDenseLayer(Source=lv("act5", act5), Weights=w["Weights_2"], Bias=w["Biases_2"], WeightsScale=512, InputFormat=EVectorFormat.dense,
                           Method=score_method)
-    return dense6, reader
+    return _sanitized("lola_large", dense6, sanitize), reader

@@ -1,7 +1,7 @@
 /*
  * cnhe.h -- C ABI of libcnhe.so, the H100-native BFV engine behind the CryptoNets plugin API.
  *
- * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these 121 entry points
+ * This is the drop-in boundary (SURVEY.md section 8b).  A C# `B200BfvFactory : IFactory` binds these 127 entry points
  * with [DllImport("cnhe")] (stub in INTEGRATION.md); the Python mirror in cryptonets_b200/ binds them with ctypes.
  * One cnhe_vec is one reference `EncryptedSealBfvVector` ("HE Wrapper/EncryptedSealBfvVector.cs:150-573"): P
  * plaintext-modulus channels, each an `AtomicSealBfvEncryptedVector` ("HE Wrapper/AtomicSealBfvVector.cs:303-1476")
@@ -179,6 +179,23 @@ int cnhe_vec_key_slot(const cnhe_vec *, int *slot);
  * the chain once eagerly first, as CaptureInference does, or bind the graph to the slot, cnhe_graph_bind). */
 int cnhe_context_derive_level(cnhe_ctx *, int k, cnhe_ctx **out);
 int cnhe_vecs_mod_switch(cnhe_ctx *from, const cnhe_vec *const *in, int n, cnhe_ctx *to, cnhe_vec **out /*n*/);
+/* Sanitisation (circuit privacy, DESIGN 4.18): out[i] = in[i] + a fresh public-key encryption of zero under the public key of in[i]'s
+ * key slot, whose c0 also carries a flood f, per coefficient one integer uniform in [-2^b, 2^b) (b = flood_bits) reduced into every q_l:
+ * out = in + (pk0 u + e0 + f, pk1 u + e1), u ternary, e0 and e1 as an encryption draws them.  The result decrypts as in did while in's
+ * noise budget exceeds about b + 2 bits; its noise is then about 2^b, so its budget about log2(q/t) - b - 2 bits.  With b = e + lambda +
+ * log2 N for an input noise of at most 2^e (infinity norm) the output's noise is within statistical distance 2^-lambda of one that does
+ * not depend on in's noise, and c1 is a fresh RLWE sample: what a client decrypts tells it the plaintext and nothing about the circuit.
+ * Encrypted vectors of any format and block count; a pending (deferred-relinearisation) vector is relinearised first; the vectors may
+ * belong to different key slots.  Outputs keep dimension, scale, format and key slot, one slab per channel.  Counted as one Encryption
+ * and one Addition per ciphertext.  Randomness: per channel a device counter hands each ciphertext a nonce (the call's first kernel
+ * reads and advances it), so every launch of a recorded graph draws fresh u, e0, e1 and f; a seeded channel draws the same words in its
+ * i-th call whether that call is eager or the i-th launch of a graph recorded on a context seeded alike.  cnhe_keys_generate and
+ * cnhe_keys_generate_secure restart the counter.  CNHE_ERR_INVALID for flood_bits outside [0, floor(log2(q/t)) - 2] (the smallest over
+ * the plaintext moduli), plain vectors or vectors of another context; CNHE_ERR_STATE when a ciphertext's key slot holds no public key
+ * (a slot's compact key blob carries it when its sets include bit 0) or when a channel's sampler key has handed out 2^48 sanitisation
+ * nonces (cnhe_keys_generate_secure re-keys it).  Recordable, also across levels; a recorded call reads the public keys through the
+ * graph's key binding, so cnhe_graph_bind to another slot sanitises under that client's public key. */
+int cnhe_vecs_sanitize(cnhe_ctx *, const cnhe_vec *const *in, int n, int flood_bits, cnhe_vec **out /*n*/);
 int cnhe_vec_write(cnhe_ctx *, const cnhe_vec *, char *dst, size_t cap, size_t *needed);
 int cnhe_vec_read(cnhe_ctx *, const char *text, size_t len, cnhe_vec **out, size_t *consumed);
 
@@ -520,7 +537,8 @@ int cnhe_dev_copy(cnhe_ctx *, uint64_t dst, uint64_t src, size_t words); /* devi
  * products) and for words that are not canonical residues. */
 int cnhe_raw_import_products(cnhe_ctx *, const uint64_t *words, int n, uint64_t dim, double scale, int slot, cnhe_vec **out);
 /* per-kernel-family device timing (CUDA events around the launches on the context stream): enable, run, collect.
- * family: 0 ntt forward (incl. digit variant), 1 ntt inverse, 2 behz element-wise, 3 key-switch mac, 4 scalar mac layer, 5 other */
+ * family: 0 ntt forward (incl. digit variant), 1 ntt inverse, 2 behz element-wise, 3 key-switch mac, 4 scalar mac layer, 5 other,
+ * 6 the sanitisation finish kernel (cnhe_vecs_sanitize) */
 int cnhe_prof_enable(cnhe_ctx *, int on);
 int cnhe_prof_collect(cnhe_ctx *, int family, double *total_ms, uint64_t *launches, double *algorithmic_bytes);
 int cnhe_raw_event_timing(cnhe_ctx *, int start); /* start=1: record start event; start=0: record stop, return via cnhe_raw_elapsed_ms */

@@ -56,6 +56,7 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_key_slot(IntPtr a0, out int slot);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_context_derive_level(IntPtr a0, int k, out IntPtr @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_mod_switch(IntPtr from, IntPtr[] @in, int n, IntPtr to, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_sanitize(IntPtr ctx, IntPtr[] @in, int n, int flood_bits, IntPtr[] @out);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_write(IntPtr a0, IntPtr a1, byte[] dst, UIntPtr cap, out UIntPtr needed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_read(IntPtr a0, byte[] text, UIntPtr len, out IntPtr @out, out UIntPtr consumed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_encrypt(IntPtr a0, double[] v, ulong dim, double scale, int format, out IntPtr @out);

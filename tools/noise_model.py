@@ -79,6 +79,25 @@ class Model:
         p_gauss = math.log2(self.c * SIGMA * math.sqrt(4.0 * self.N / 3.0 + 1.0)) + math.log2(self.t) - self.logq
         return self.budget(math.log2(2.0 ** p_round + 2.0 ** p_gauss)), self.budget(p_round), self.budget(p_gauss)
 
+    def flood_bits(self, noise_bits, statistical_bits=40):
+        """The flood width b of a sanitisation (DESIGN 4.18) that hides an output noise of at most 2^noise_bits (infinity norm) within
+        statistical distance 2^-statistical_bits over all N coefficients: b = e + lambda + log2 N"""
+        return int(noise_bits) + int(statistical_bits) + int(round(math.log2(self.N)))
+
+    def max_flood_bits(self):
+        """the widest flood cnhe_vecs_sanitize accepts for this plaintext modulus: floor(log2(q / t)) - 2"""
+        return (self.Q // self.t).bit_length() - 1 - 2
+
+    def sanitize(self, b, budget_in):
+        """The budget after a sanitisation of flood width b of a ciphertext with budget budget_in, or None when the sum may change the
+        plaintext: the input noise, the flood (peak 2^b, uniform) and a fresh encryption's noise add, so the budget is about
+        log2(q/t) - b - 1 once the flood dominates.  An input noise of 2^e leaves a budget of about log2(q/t) - e - 1, so the flood of
+        flood_bits(e, lambda) fits only while budget_in exceeds about lambda + log2 N + 2 bits."""
+        p_flood = b + math.log2(self.t) - self.logq
+        p_fresh = math.log2(self.c * SIGMA * math.sqrt(4.0 * self.N / 3.0 + 1.0)) + math.log2(self.t) - self.logq
+        out = self.budget(self.rss(self.peak(budget_in), p_flood, p_fresh))
+        return out if out > 0 else None
+
     def plain_gain(self):
         return math.log2(self.t / math.sqrt(12.0)) + 0.5 * math.log2(self.N)
 
