@@ -2615,6 +2615,29 @@ static std::shared_ptr<UmmaPlan> mac_umma_plan(Context &c, const MacLayer &L, in
     std::shared_ptr<UmmaPlan> plan = umma_plan(c, ch, L.grows, L.row_outs, wdh, M, L.K, limbs);
     return plan->ok && (double)plan->total_chunks * 32.0 * 127.0 * 255.0 < 2147483648.0 ? plan : nullptr;
 }
+// The kernel that serves channel ch of a prepared layer, the first whose accumulator bound holds: wgmma (a plan, above), mma.sync (one
+// gather row), FP64 (26-bit halves of each word), else the 128-bit integer MAC, whose bound mac_prepare enforces.  wdh / wmax: the
+// channel's signed weights and their largest magnitude; plan and tap_stride are set for wgmma.
+enum class MacRoute { UMMA, IMMA, FP64, INT128 };
+static MacRoute mac_route(Context &c, const MacLayer &L, int ch, const std::vector<const u64 *> &ip_all, size_t ctw, const std::vector<double> &wdh,
+                          double wmax, std::shared_ptr<UmmaPlan> &plan, long long &tap_stride) {
+    const int K = L.K, M = L.M, maxbits = L.maxbits;
+    // FP64: K * |w| * 2^26 < 2^52 keeps every sum of w * x_lo exact in a double
+    const bool fp_mac = maxbits <= 50 && wmax < 131072.0 && (double)K * wmax * 67108864.0 < 4503599627370496.0 && !getenv("CNHE_MAC_INT");
+    // dense layer (one gather row shared by every output, 8-bit weights): exact integer GEMM on the tensor cores (mac_imma.cu).  Both
+    // tensor-core kernels join the limb sums in an FP64 epilogue that is exact only for moduli below 2^50 ((double)p, fcanon_u's
+    // |x| < 2^51); wider moduli (N = 2048's 54-bit default, custom ones) take the 128-bit k_mac_layer
+    const int limbs = (maxbits + 7) / 8;
+    const bool imma = L.grows.size() / K == 1 && wmax <= 254.0 && K >= 32 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 &&
+                      (double)K * 254.0 * 255.0 < 2147483648.0 && !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
+    // ... or wgmma (mac_umma.cu), dense and convolution alike, under the same modulus bound
+    plan = mac_umma_plan(c, L, ch, ip_all, ctw, wdh, wmax, tap_stride);
+    const MacRoute r = plan ? MacRoute::UMMA : imma ? MacRoute::IMMA : fp_mac ? MacRoute::FP64 : MacRoute::INT128;
+    static const char *const name[] = {"umma", "imma", "fp64", "int128"};
+    if (getenv("CNHE_MAC_ROUTE")) // read per call, like CNHE_UMMA_PROF: tests switch it on to see which kernel served each channel
+        fprintf(stderr, "[mac route ch=%d kernel=%s K=%d M=%d]\n", ch, name[(int)r], K, M);
+    return r;
+}
 // One channel of a prepared layer on ciphertexts of `polys` polynomials (2, or 3 for size-3 products: the sum is linear in each
 // polynomial): ip[b * n_in + i] is block b of input i, op[m * bl + b] block b of output m; the blocks of one output lie consecutively,
 // polys * k * N words apart.  The bias goes to c0.
@@ -2627,7 +2650,6 @@ static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector
     const cnhe_vec *const *weights = L.weights, *const *bias = L.bias;
     const std::vector<int> &grows = L.grows;
     const std::vector<MacTile> &tiles = L.tiles;
-    const int order_rows = (int)(grows.size() / K);
     const size_t ctw = (size_t)polys * c.k * c.N;
     // every temporary lives on this channel's stream (stream-ordered frees must not overtake another channel's kernels)
     int *d_gather = (int *)c.ws_alloc((grows.size() + 1) / 2 + 1);
@@ -2637,23 +2659,17 @@ static void mac_channel(Context &c, const MacLayer &L, int ch, const std::vector
     std::vector<const u64 *> wp(M);
     for (int m = 0; m < M; m++) wp[m] = weights[m]->ptr(ch);
     const u64 *const *d_w = upload_ptrs(c, wp);
-    // signed weights as doubles for the FP64 accumulate path, when they are small enough for it to be exact
+    // signed weights as doubles (the FP64 path takes them as they are)
     double wmax = 0;
     const std::vector<double> wdh = mac_weights(c, L, ch, wmax);
-    const bool fp_mac = maxbits <= 50 && wmax < 131072.0 && (double)K * wmax * 67108864.0 < 4503599627370496.0 && !getenv("CNHE_MAC_INT");
-    // dense layer (one gather row shared by every output, 8-bit weights): exact integer GEMM on the tensor cores (mac_imma.cu).  Both
-    // tensor-core kernels join the limb sums in an FP64 epilogue that is exact only for moduli below 2^50 ((double)p, fcanon_u's
-    // |x| < 2^51); wider moduli (N = 2048's 54-bit default, custom ones) take the 128-bit k_mac_layer
     const int limbs = (maxbits + 7) / 8;
-    const bool imma = order_rows == 1 && wmax <= 254.0 && K >= 32 && M >= 8 && maxbits <= 50 && limbs >= 5 && limbs <= 7 &&
-                      (double)K * 254.0 * 255.0 < 2147483648.0 && !getenv("CNHE_MAC_NO_IMMA") && !getenv("CNHE_MAC_INT");
-    // ... or wgmma (mac_umma.cu), dense and convolution alike, under the same modulus bound
     long long tap_stride = 0;
-    const std::shared_ptr<UmmaPlan> plan = mac_umma_plan(c, L, ch, ip_all, ctw, wdh, wmax, tap_stride);
-    const bool umma = plan != nullptr;
+    std::shared_ptr<UmmaPlan> plan;
+    const MacRoute route = mac_route(c, L, ch, ip_all, ctw, wdh, wmax, plan, tap_stride);
+    const bool umma = route == MacRoute::UMMA, imma = route == MacRoute::IMMA, fp_mac = route == MacRoute::FP64;
     if (planes && !umma) throw Error(CNHE_ERR_INVALID, "internal error: the exact scalar-MAC path needs the wgmma kernel");
     const void *d_wfrag = nullptr, *d_wfrag2 = nullptr;
-    if (!umma && imma) {
+    if (imma) {
         const int mtiles = (M + 15) / 16, chunks = (K + 31) / 32;
         const size_t fwords = (size_t)mtiles * chunks * 32 * 4;
         std::vector<uint32_t> frag(2 * fwords, 0); // W1 = clamp(W, +-127) then the residual W2 = W - W1
