@@ -5,7 +5,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["ntt.cu", "poly_ops.cu", "mac_imma.cu", "mac_umma.cu", "behz.cu", "behz_fp.cu", "runtime.cu", "vec.cu", "wire.cu", "compact.cu", "diag.cu"]
+SOURCES = ["ntt.cu", "poly_ops.cu", "mac_imma.cu", "mac_umma.cu", "behz.cu", "behz_fp.cu", "runtime.cu", "vec.cu", "wire.cu", "compact.cu", "diag.cu", "values.cu"]
 OUT = os.path.join(HERE, "libcnhe.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-O2"]

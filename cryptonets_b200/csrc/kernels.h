@@ -343,6 +343,29 @@ cudaError_t launch_encode_scatter(const u64 *values, u64 *plain, int n, int coun
 // plain[i][index_map[first_col + i]] = 1, zero elsewhere (one-hot slot masks, encoded form before the inverse transform)
 cudaError_t launch_onehot_scatter(u64 *plain, int n, int first_col, const u32 *index_map, int logn, cudaStream_t s);
 cudaError_t launch_decode_gather(const u64 *plain_ntt, u64 *values, int n, const u32 *index_map, int logn, cudaStream_t s);
+// ---- values in and out of the channels (values.cu, DESIGN 4.19)
+// dense (index_map set): plain[c][index_map[j]] = the residue mod t of value (c % bl) N + j of vector c / bl of values [n][dim] (zero past
+// dim), c < n_ct; sparse (index_map null): plain[j] = the residue of values[j], j < dim.  Residue: w = rint(v scale), |w| mod big, made
+// big - |w| mod big when w < 0.  A value with !(|w| < 1.5e38) sets *bad and writes 0.
+cudaError_t launch_split_scatter(const double *values, u64 *plain, int n_ct, int bl, u64 dim, double scale, unsigned __int128 big, u64 t,
+                                 const u32 *index_map, int logn, int *bad, cudaStream_t s);
+// c0[i], c1[i] ([kN] each) = the two parts of ciphertext ct_tab[i] ([2][kN])
+cudaError_t launch_split_parts(const u64 *const *ct_tab, u64 *c0, u64 *c1, int n, size_t kN, cudaStream_t s);
+// where the join finds one vector's residues of one channel: value j at p[j stride] for j < count, zero past it; scale: the vector's
+// (read from the channel-0 entries)
+struct JoinSrc {
+    const u64 *p;
+    u64 stride, count;
+    double scale;
+};
+struct JoinConst {
+    int P;
+    u64 big_lo, big_hi;                 // B, the product of the plaintext moduli (< 2^126)
+    u64 coeff_lo[16], coeff_hi[16];     // the CRT coefficients mod B
+};
+// out[i][j] = centred sum over the channels of coeff_ch r_ch mod B, as a double rounded to nearest even, over the vector's scale;
+// src [P][n]
+cudaError_t launch_crt_join(const JoinSrc *src, double *out, int n, u64 dim, const JoinConst &jc, cudaStream_t s);
 // ct[i] (already u*pk, coefficient form) += (e0 + Delta*m_i, e1)
 cudaError_t launch_encrypt_finish(u64 *ct, const u64 *plain, size_t plain_stride, int n, int coeffs, const RngKey &seed, u64 nonce0, int k, int logn,
                                   const BehzConst *bc, PlainConst pc, cudaStream_t s);

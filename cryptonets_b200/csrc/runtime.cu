@@ -1592,6 +1592,15 @@ void op_encode(Context &c, int ch, const u64 *values, int n, int count, u64 *pla
     c.check(launch_encode_scatter(values, plain, n, count, c.d_index_map, c.logN, c.stream), "encode_scatter");
     c.check(launch_ntt_inverse(plain, plain, n, c.logN, c.d_tabs, c.ch[ch].mod_id, 1, fp_range(c, c.ch[ch].mod_id, 1), c.stream), "ntt_inverse(t)");
 }
+void op_encode_values(Context &c, int ch, const double *values, int n, uint64_t dim, double scale, bool dense, u64 *plain, int *bad) {
+    const int bl = dense ? (int)((dim + c.N - 1) / c.N) : 0;
+    c.check(launch_split_scatter(values, plain, n * bl, bl, dim, scale, c.big_factor, c.t[ch], dense ? c.d_index_map : nullptr, c.logN, bad,
+                                 c.stream),
+            "split_scatter");
+    if (dense)
+        c.check(launch_ntt_inverse(plain, plain, n * bl, c.logN, c.d_tabs, c.ch[ch].mod_id, 1, fp_range(c, c.ch[ch].mod_id, 1), c.stream),
+                "ntt_inverse(t)");
+}
 void op_encode_onehot(Context &c, int ch, int n, int first_col, u64 *plain) {
     c.check(launch_onehot_scatter(plain, n, first_col, c.d_index_map, c.logN, c.stream), "onehot_scatter");
     c.check(launch_ntt_inverse(plain, plain, n, c.logN, c.d_tabs, c.ch[ch].mod_id, 1, fp_range(c, c.ch[ch].mod_id, 1), c.stream), "ntt_inverse(t)");
@@ -1747,22 +1756,42 @@ void op_compact_expand(Context &c, const u64 *packed, const CompactKey &key, int
     }
     c.stream = keep;
 }
-static void dot_with_secret(Context &c, int chi, const u64 *ct, int n, u64 *x) {
+// x = c0 + c1 s (coefficient form) of the n ciphertexts whose parts are c0, c1 [n][kN]; c1 is overwritten
+static void dot_parts(Context &c, int chi, const u64 *c0, u64 *c1, int n, u64 *x) {
     Channel &ch = c.ch[chi];
     if (!ch.have_sk) throw Error(-3, "secret key is missing");
     const int k = c.k;
-    const size_t N = c.N, kN = (size_t)k * N;
-    u64 *c0 = c.ws_alloc((size_t)n * kN), *c1 = c.ws_alloc((size_t)n * kN);
-    CNHE_CUDA(cudaMemcpy2DAsync(c0, kN * 8, ct, 2 * kN * 8, kN * 8, n, cudaMemcpyDeviceToDevice, c.stream));
-    CNHE_CUDA(cudaMemcpy2DAsync(c1, kN * 8, ct + kN, 2 * kN * 8, kN * 8, n, cudaMemcpyDeviceToDevice, c.stream));
+    const size_t N = c.N;
     c.check(launch_ntt_forward(c1, c1, n * k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_forward");
     c.check(launch_dyadic_bcast(c1, ch.sk->p, c1, n, 1, 1, 0, k, c.logN, c.d_bc, c.stream), "dyadic");
     c.check(launch_ntt_inverse_add(c1, c0, 1, N, x, n * k, c.logN, c.d_tabs, 0, k, fp_range(c, 0, k), c.stream), "ntt_inverse_add");
+}
+static void dot_with_secret(Context &c, int chi, const u64 *ct, int n, u64 *x) {
+    const size_t kN = (size_t)c.k * c.N;
+    u64 *c0 = c.ws_alloc((size_t)n * kN), *c1 = c.ws_alloc((size_t)n * kN);
+    CNHE_CUDA(cudaMemcpy2DAsync(c0, kN * 8, ct, 2 * kN * 8, kN * 8, n, cudaMemcpyDeviceToDevice, c.stream));
+    CNHE_CUDA(cudaMemcpy2DAsync(c1, kN * 8, ct + kN, 2 * kN * 8, kN * 8, n, cudaMemcpyDeviceToDevice, c.stream));
+    dot_parts(c, chi, c0, c1, n, x);
 }
 void op_decrypt(Context &c, int chi, const u64 *ct, int n, u64 *plain) {
     u64 *x = c.ws_alloc((size_t)n * c.k * c.N);
     dot_with_secret(c, chi, ct, n, x);
     c.check(launch_decrypt_round(x, plain, n, c.k, c.logN, c.d_bc, c.ch[chi].pc, c.stream), "decrypt_round");
+    c.op_count[Context::OP_DECRYPT] += (uint64_t)n;
+}
+void op_decrypt_many(Context &c, int chi, const std::vector<const u64 *> &cts, u64 *plain) {
+    const int n = (int)cts.size();
+    const size_t kN = (size_t)c.k * c.N;
+    const int wave = c.wave(3 * kN);
+    for (int c0 = 0; c0 < n; c0 += wave) {
+        WsScope scope(c);
+        const int m = std::min(wave, n - c0);
+        u64 *p0 = c.ws_alloc((size_t)m * kN), *p1 = c.ws_alloc((size_t)m * kN), *x = c.ws_alloc((size_t)m * kN);
+        const std::vector<const u64 *> part(cts.begin() + c0, cts.begin() + c0 + m);
+        c.check(launch_split_parts(upload_ptrs(c, part), p0, p1, m, kN, c.stream), "split_parts");
+        dot_parts(c, chi, p0, p1, m, x);
+        c.check(launch_decrypt_round(x, plain + (size_t)c0 * c.N, m, c.k, c.logN, c.d_bc, c.ch[chi].pc, c.stream), "decrypt_round");
+    }
     c.op_count[Context::OP_DECRYPT] += (uint64_t)n;
 }
 // Decryptor::invariant_noise_budget: bits(q) - bits(|t * (c0 + c1 s) mod q|_centred) - 1, composed on the host

@@ -407,6 +407,11 @@ void op_encode_onehot(Context &c, int ch, int n, int first_col, u64 *plain);
 u64 take_nonces(Context &c, int ch, u64 n);
 void op_encrypt(Context &c, int ch, const u64 *plain, size_t plain_stride, int n, int coeffs, u64 nonce0, u64 *ct);
 void op_decrypt(Context &c, int ch, const u64 *ct, int n, u64 *plain);
+// plain [n][N] = decryptions of the ciphertexts at cts[i] (any addresses), one wave of kernels per c.wave(3kN) ciphertexts
+void op_decrypt_many(Context &c, int ch, const std::vector<const u64 *> &cts, u64 *plain);
+// values [n][dim] doubles (device) -> plain: dense [n][bl][N] coefficient form (bl = ceil(dim / N), the split fused into the encode scatter,
+// a short last block zero padded); sparse (n = 1) [dim] residues.  Out-of-range values set *bad (DESIGN 4.19)
+void op_encode_values(Context &c, int ch, const double *values, int n, uint64_t dim, double scale, bool dense, u64 *plain, int *bad);
 // ---- compact ciphertext upload (format: compact.cu)
 CompactShape compact_shape(const Context &c); // bit lengths of the q_l and the packed word offsets of one ciphertext
 // expansion key K_c of one blob: a fresh OS draw on a secure channel; four words of the seeded sampler on a test channel (reproducible)

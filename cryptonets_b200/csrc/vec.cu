@@ -813,30 +813,6 @@ static void split_values(Context &c, const double *v, uint64_t n, double scale, 
         for (int i = 0; i < c.P; i++) res[i][j] = (u64)(z % c.t[i]);
     }
 }
-static u128 mulmod_u128(u128 a, u64 b, u128 m) { // a < m < 2^126
-    u128 r = 0;
-    while (b) {
-        if (b & 1) { r += a; if (r >= m) r -= m; }
-        a += a; if (a >= m) a -= m;
-        b >>= 1;
-    }
-    return r;
-}
-// JoinSplitNumbers ("EncryptedSealBfvVector.cs:381-395")
-static void join_values(Context &c, const std::vector<std::vector<u64>> &split, uint64_t n, double scale, double *out) {
-    for (uint64_t j = 0; j < n; j++) {
-        u128 acc = 0;
-        for (int i = 0; i < c.P; i++) {
-            acc += mulmod_u128(c.crt_coeff[i] % c.big_factor, split[i][j], c.big_factor);
-            if (acc >= c.big_factor) acc -= c.big_factor;
-        }
-        double val;
-        if (acc * 2 > c.big_factor) val = -(double)(c.big_factor - acc);
-        else val = (double)acc;
-        out[j] = val / scale;
-    }
-}
-
 static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64>> &split, const double *v, uint64_t dim, double scale, int format,
                                    bool encrypt);
 static cnhe_vec *make_vector(Context &c, const double *v, uint64_t dim, double scale, int format, bool encrypt) {
@@ -898,10 +874,83 @@ static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64
     return guard.release();
 }
 
+// ---- values in and out of the channels on the GPU (DESIGN 4.19).  Every encryption and decryption of doubles runs through these: the
+// host entry points copy the doubles to the device, or the result back, once.
+static const char *const ENCRYPT_WHY = "samples encryption randomness (a replay would reuse it for every input)";
+// the n vectors [n][dim] of doubles at device address `values`, split and encoded per channel: plain[ch] dense [n][bl][N] coefficient form,
+// sparse (n = 1) [dim] residues.  The channels read `values` after the work already queued on stream 0.  An out-of-range value is
+// CNHE_ERR_INVALID once every channel's split has run, before any nonce is taken or output allocated.
+static std::vector<u64 *> encode_values(Context &c, const double *values, int n, uint64_t dim, double scale, bool dense) {
+    const size_t N = c.N, words = dense ? (size_t)n * ((dim + N - 1) / N) * N : dim;
+    int *bad = (int *)c.ws_alloc(1);
+    CNHE_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), c.stream));
+    c.fork_streams();
+    std::vector<u64 *> plain(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        plain[ch] = c.ws_alloc(words);
+        op_encode_values(c, ch, values, n, dim, scale, dense, plain[ch], bad);
+    }
+    c.join_streams();
+    c.set_channel(0);
+    int h_bad = 0;
+    CNHE_CUDA(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    CNHE_CUDA(cudaStreamSynchronize(c.stream));
+    if (h_bad) fail("value out of range");
+    return plain;
+}
+static void check_values(int n, uint64_t dim, double &scale) {
+    if (n < 1 || dim < 1) fail("bad arguments");
+    if (scale == 0) scale = 1; // AtomicSealBfvVector.cs:1120
+}
+// n dense vectors [n][dim] (device doubles) encrypted in one wave per channel into one slab per channel (GetEncryptedMatrix, IFactory.cs:353-380)
+static void encrypt_dense(Context &c, const double *values, int n, uint64_t dim, double scale, cnhe_vec **out) {
+    const size_t N = c.N;
+    const int bl = (int)((dim + N - 1) / N);
+    if ((uint64_t)n * bl >= (1ULL << 31)) fail("too many ciphertexts in one call");
+    const std::vector<u64 *> plain = encode_values(c, values, n, dim, scale, true);
+    std::vector<BufRef> big(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        big[ch] = c.alloc((size_t)n * bl * c.ct_words());
+        op_encrypt(c, ch, plain[ch], N, n * bl, (int)N, take_nonces(c, ch, (u64)n * bl), big[ch]->p);
+    }
+    c.set_channel(0);
+    for (int i = 0; i < n; i++) out[i] = slab_view(new_vec(c, dim, scale, CNHE_DENSE, true, bl), big, (size_t)i * bl);
+}
+// a sparse encrypted vector: one constant-polynomial plaintext per element (AtomicSealBfvVector.cs:1135-1138)
+static cnhe_vec *encrypt_sparse(Context &c, const double *values, uint64_t dim, double scale) {
+    if (dim >= (1ULL << 31)) fail("too many ciphertexts in one call");
+    const std::vector<u64 *> plain = encode_values(c, values, 1, dim, scale, false);
+    std::unique_ptr<cnhe_vec> out(new_vec(c, dim, scale, CNHE_SPARSE, true, (int)dim));
+    alloc_channels(out.get());
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        op_encrypt(c, ch, plain[ch], 1, (int)dim, 1, take_nonces(c, ch, dim), out->ptr(ch));
+    }
+    c.set_channel(0);
+    return out.release();
+}
+// a device copy of n * dim host doubles (stream 0)
+static const double *upload_values(Context &c, const double *v, size_t count) {
+    double *d = (double *)c.ws_alloc(count);
+    CNHE_CUDA(cudaMemcpyAsync(d, v, count * 8, cudaMemcpyHostToDevice, c.stream));
+    return d;
+}
+static const double *device_values(uint64_t addr) {
+    if (!addr) fail("null values");
+    return reinterpret_cast<const double *>((uintptr_t)addr);
+}
+
 extern "C" int cnhe_vec_encrypt(cnhe_ctx *h, const double *v, uint64_t dim, double scale, int format, cnhe_vec **out) {
     API_BEGIN(h)
-    not_recorded(c, "samples encryption randomness (a replay would reuse it for every input)");
-    *out = make_vector(c, v, dim, scale, format, true);
+    not_recorded(c, ENCRYPT_WHY);
+    if (!v || !out) fail("null values");
+    if (format != CNHE_DENSE && format != CNHE_SPARSE) fail("bad format");
+    check_values(1, dim, scale);
+    const double *d = upload_values(c, v, dim);
+    if (format == CNHE_DENSE) encrypt_dense(c, d, 1, dim, scale, out);
+    else *out = encrypt_sparse(c, d, dim, scale);
     API_END
 }
 // BigInteger entry points of the factory ("HE Wrapper/IFactory.cs:29,43" -> EncryptedSealBfvVector(IEnumerable<BigInteger>, ...),
@@ -910,7 +959,7 @@ extern "C" int cnhe_vec_from_residues(cnhe_ctx *h, const uint64_t *residues, uin
     API_BEGIN(h)
     if (!residues || !out || dim < 1) fail("bad arguments");
     if (format != CNHE_DENSE && format != CNHE_SPARSE) fail("bad format");
-    if (encrypt) not_recorded(c, "samples encryption randomness (a replay would reuse it for every input)");
+    if (encrypt) not_recorded(c, ENCRYPT_WHY);
     std::vector<std::vector<u64>> split(c.P, std::vector<u64>(dim));
     for (int ch = 0; ch < c.P; ch++)
         for (uint64_t j = 0; j < dim; j++) {
@@ -925,29 +974,20 @@ extern "C" int cnhe_vec_plain(cnhe_ctx *h, const double *v, uint64_t dim, double
     *out = make_vector(c, v, dim, scale, format, false);
     API_END
 }
-// n dense single-block-or-more vectors encrypted in one wave per channel (GetEncryptedMatrix, IFactory.cs:353-380)
 extern "C" int cnhe_vecs_encrypt(cnhe_ctx *h, const double *v, int n, uint64_t dim, double scale, cnhe_vec **out) {
     API_BEGIN(h)
-    not_recorded(c, "samples encryption randomness (a replay would reuse it for every input)");
-    if (n < 1 || !v || !out) fail("bad arguments");
-    if (scale == 0) scale = 1;
-    const size_t N = c.N;
-    const int bl = (int)((dim + N - 1) / N);
-    std::vector<std::vector<u64>> split;
-    split_values(c, v, (uint64_t)n * dim, scale, split);
-    std::vector<BufRef> big(c.P);
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        std::vector<u64> padded((size_t)n * bl * N, 0);
-        for (int i = 0; i < n; i++) memcpy(&padded[(size_t)i * bl * N], &split[ch][(size_t)i * dim], dim * 8);
-        u64 *dvals = c.ws_alloc(padded.size()), *plain = c.ws_alloc(padded.size());
-        CNHE_CUDA(cudaMemcpyAsync(dvals, padded.data(), padded.size() * 8, cudaMemcpyHostToDevice, c.stream));
-        op_encode(c, ch, dvals, n * bl, (int)N, plain);
-        big[ch] = c.alloc((size_t)n * bl * c.ct_words());
-        op_encrypt(c, ch, plain, N, n * bl, (int)N, take_nonces(c, ch, (u64)n * bl), big[ch]->p);
-        c.sync();
-    }
-    for (int i = 0; i < n; i++) out[i] = slab_view(new_vec(c, dim, scale, CNHE_DENSE, true, bl), big, (size_t)i * bl);
+    not_recorded(c, ENCRYPT_WHY);
+    if (!v || !out) fail("bad arguments");
+    check_values(n, dim, scale);
+    encrypt_dense(c, upload_values(c, v, (size_t)n * dim), n, dim, scale, out);
+    API_END
+}
+extern "C" int cnhe_vecs_encrypt_device(cnhe_ctx *h, uint64_t d_values, int n, uint64_t dim, double scale, cnhe_vec **out) {
+    API_BEGIN(h)
+    not_recorded(c, ENCRYPT_WHY);
+    if (!out) fail("bad arguments");
+    check_values(n, dim, scale);
+    encrypt_dense(c, device_values(d_values), n, dim, scale, out);
     API_END
 }
 
@@ -978,21 +1018,92 @@ static void decrypt_channel(Context &c, const cnhe_vec *v, int ch, std::vector<u
         memcpy(res.data(), hostv.data(), take * 8);
     }
 }
-// Decrypt of v's `dim` values: every channel's residues, joined
-static void decrypt_values(Context &c, const cnhe_vec *v, double *out) {
-    std::vector<std::vector<u64>> split(c.P);
+// out [n][dim] (device) = the first `dim` values of each vector (zero past its last block), stream-ordered on stream 0.  Per channel one
+// decryption wave over every encrypted block and one decode wave over every dense block; then one CRT join over all values on stream 0.
+static void decrypt_values(Context &c, const cnhe_vec *const *vecs, int n, uint64_t dim, double *out) {
+    if (n < 1 || !vecs) fail("bad arguments");
+    for (int i = 0; i < n; i++) {
+        same_ctx(c, vecs[i]);
+        if (vecs[i]->dim != dim) fail("all vectors must have the same dimension");
+        if (vecs[i]->enc && vecs[i]->key_slot() != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
+    }
+    const size_t N = c.N;
+    // per channel, the plaintexts in one buffer: [plain dense | encrypted dense | encrypted sparse] blocks; the decode covers the first two
+    std::vector<size_t> at(n); // vector i's first block within its group
+    size_t n_pd = 0, n_ed = 0, n_es = 0;
+    for (int i = 0; i < n; i++) {
+        const cnhe_vec *v = vecs[i];
+        if (!v->enc && v->format == CNHE_SPARSE) continue;
+        size_t &group = !v->enc ? n_pd : v->format == CNHE_DENSE ? n_ed : n_es;
+        at[i] = group;
+        group += v->blocks;
+    }
+    std::vector<JoinSrc> src((size_t)c.P * n);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
-        decrypt_channel(c, v, ch, split[ch]);
+        u64 *plain = c.ws_alloc((n_pd + n_ed + n_es) * N), *vals = c.ws_alloc((n_pd + n_ed) * N);
+        std::vector<const u64 *> cts(n_ed + n_es);
+        for (int i = 0; i < n; i++) {
+            const cnhe_vec *v = vecs[i];
+            if (v->enc)
+                for (int b = 0; b < v->blocks; b++) cts[(v->format == CNHE_DENSE ? 0 : n_ed) + at[i] + b] = v->block(ch, b);
+            else if (v->format == CNHE_DENSE)
+                CNHE_CUDA(cudaMemcpyAsync(plain + at[i] * N, v->ptr(ch), (size_t)v->blocks * N * 8, cudaMemcpyDeviceToDevice, c.stream));
+        }
+        if (!cts.empty()) op_decrypt_many(c, ch, cts, plain + n_pd * N);
+        if (n_pd + n_ed) op_decode(c, ch, plain, (int)(n_pd + n_ed), vals);
+        for (int i = 0; i < n; i++) {
+            const cnhe_vec *v = vecs[i];
+            JoinSrc &s = src[(size_t)ch * n + i];
+            s.scale = v->scale;
+            if (v->format == CNHE_DENSE) {
+                s.p = vals + ((v->enc ? n_pd : 0) + at[i]) * N;
+                s.stride = 1;
+                s.count = (u64)v->blocks * N;
+            } else if (v->enc) {
+                s.p = plain + (n_pd + n_ed + at[i]) * N;
+                s.stride = N;
+                s.count = (u64)v->blocks;
+            } else { // plain sparse: the host's residues
+                const std::vector<u64> &r = v->scalars[ch];
+                u64 *d = c.ws_alloc(r.size());
+                c.h2d(d, r.data(), r.size() * 8);
+                s.p = d;
+                s.stride = 1;
+                s.count = r.size();
+            }
+        }
     }
-    join_values(c, split, v->dim, v->scale, out);
+    c.join_streams();
+    c.set_channel(0);
+    JoinConst jc;
+    memset(&jc, 0, sizeof(jc));
+    jc.P = c.P;
+    jc.big_lo = (u64)c.big_factor;
+    jc.big_hi = (u64)(c.big_factor >> 64);
+    for (int ch = 0; ch < c.P; ch++) {
+        const u128 k = c.crt_coeff[ch] % c.big_factor;
+        jc.coeff_lo[ch] = (u64)k;
+        jc.coeff_hi[ch] = (u64)(k >> 64);
+    }
+    JoinSrc *d_src = (JoinSrc *)c.ws_alloc(src.size() * sizeof(JoinSrc) / 8);
+    c.h2d(d_src, src.data(), src.size() * sizeof(JoinSrc));
+    c.check(launch_crt_join(d_src, out, n, dim, jc, c.stream), "crt_join");
+    c.fork_streams(); // the channels' buffers the join reads are released on their streams
+}
+// the host entry points: one device buffer, one copy back
+static void decrypt_to_host(Context &c, const cnhe_vec *const *vecs, int n, uint64_t dim, double *out) {
+    double *d = (double *)c.ws_alloc((size_t)n * dim);
+    decrypt_values(c, vecs, n, dim, d);
+    if (n && dim) CNHE_CUDA(cudaMemcpyAsync(out, d, (size_t)n * dim * 8, cudaMemcpyDeviceToHost, c.stream));
+    c.sync();
 }
 extern "C" int cnhe_vec_decrypt(cnhe_ctx *h, const cnhe_vec *v, double *out, uint64_t cap) {
     API_BEGIN(h)
     not_recorded(c, "returns words to the host");
     same_ctx(c, v);
     if (cap < v->dim) fail("destination too small");
-    decrypt_values(c, v, out);
+    decrypt_to_host(c, &v, 1, v->dim, out);
     API_END
 }
 // DecryptFullPrecision ("EncryptedSealBfvVector.cs:343-348"): the residues of every channel, for the caller's BigInteger CRT join
@@ -1013,11 +1124,17 @@ extern "C" int cnhe_vec_decrypt_residues(cnhe_ctx *h, const cnhe_vec *v, uint64_
 extern "C" int cnhe_vecs_decrypt(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, double *out, uint64_t dim) {
     API_BEGIN(h)
     not_recorded(c, "returns words to the host");
-    for (int i = 0; i < n; i++) {
-        same_ctx(c, vecs[i]);
-        if (vecs[i]->dim != dim) fail("all vectors must have the same dimension");
-        decrypt_values(c, vecs[i], out + (size_t)i * dim);
-    }
+    if (n < 1) return CNHE_OK;
+    if (!out) fail("bad arguments");
+    decrypt_to_host(c, vecs, n, dim, out);
+    API_END
+}
+extern "C" int cnhe_vecs_decrypt_device(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t d_out, uint64_t dim) {
+    API_BEGIN(h)
+    not_recorded(c, "decrypts (the secret key's results are not part of a recorded inference)");
+    if (n < 1) return CNHE_OK;
+    if (!d_out) fail("bad arguments");
+    decrypt_values(c, vecs, n, dim, reinterpret_cast<double *>((uintptr_t)d_out));
     API_END
 }
 // New words for existing encrypted vectors (a graph's recorded inputs): dst[i] takes src[i]'s ciphertexts, device to device on each
@@ -1221,10 +1338,11 @@ static CompactHeader parse_compact(const Context &c, const uint8_t *src, size_t 
     if (len != hd.header_bytes + (size_t)c.P * hd.channel_words * 8) fail("compact blob: length does not match the header");
     return hd;
 }
-extern "C" int cnhe_vecs_encrypt_compact(cnhe_ctx *h, const double *v, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap, size_t *needed) {
-    API_BEGIN(h)
-    not_recorded(c, "samples encryption randomness (a replay would reuse it for every input)");
-    if (n < 1 || dim < 1 || !v || (!dst && !needed)) fail("bad arguments");
+// the compact blob of n dense vectors: `values` is called for the device doubles once the blob's size and the secret keys are checked
+template <class Values>
+static void encrypt_compact(Context &c, Values values, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap, size_t *needed) {
+    not_recorded(c, ENCRYPT_WHY);
+    if (n < 1 || dim < 1 || (!dst && !needed)) fail("bad arguments");
     if (scale == 0) scale = 1;
     const size_t N = c.N;
     const uint64_t bl = (dim + N - 1) / N, nct = (uint64_t)n * bl;
@@ -1232,26 +1350,21 @@ extern "C" int cnhe_vecs_encrypt_compact(cnhe_ctx *h, const double *v, int n, ui
     const CompactShape sh = compact_shape(c);
     const size_t hdr = compact_header_bytes(c.k, c.P), per_ch = (size_t)nct * sh.off[c.k] * 8, total = hdr + (size_t)c.P * per_ch;
     if (needed) *needed = total;
-    if (!dst) return CNHE_OK;
+    if (!dst) return;
     if (cap < total) fail("destination too small");
     for (int ch = 0; ch < c.P; ch++)
         if (!c.ch[ch].have_sk) throw Error(CNHE_ERR_STATE, "secret key is missing");
-    std::vector<std::vector<u64>> split;
-    split_values(c, v, (uint64_t)n * dim, scale, split);
+    const std::vector<u64 *> plain = encode_values(c, values(), n, dim, scale, true);
     std::vector<CompactKey> keys(c.P);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
-        std::vector<u64> padded((size_t)nct * N, 0);
-        for (int i = 0; i < n; i++) memcpy(&padded[(size_t)i * bl * N], &split[ch][(size_t)i * dim], dim * 8);
-        u64 *dvals = c.ws_alloc(padded.size()), *plain = c.ws_alloc(padded.size()), *packed = c.ws_alloc((size_t)nct * sh.off[c.k]);
-        CNHE_CUDA(cudaMemcpyAsync(dvals, padded.data(), padded.size() * 8, cudaMemcpyHostToDevice, c.stream));
-        op_encode(c, ch, dvals, (int)nct, (int)N, plain);
+        u64 *packed = c.ws_alloc((size_t)nct * sh.off[c.k]);
         const u64 nonce0 = take_nonces(c, ch, nct);
         keys[ch] = compact_key(c, ch, nonce0);
-        op_encrypt_compact(c, ch, plain, (int)nct, nonce0, keys[ch], packed);
+        op_encrypt_compact(c, ch, plain[ch], (int)nct, nonce0, keys[ch], packed);
         CNHE_CUDA(cudaMemcpyAsync(dst + hdr + ch * per_ch, packed, per_ch, cudaMemcpyDeviceToHost, c.stream));
-        c.sync();
     }
+    c.sync();
     auto wr32 = [&](size_t off, uint32_t x) { memcpy(dst + off, &x, 4); };
     auto wr64 = [&](size_t off, uint64_t x) { memcpy(dst + off, &x, 8); };
     memcpy(dst, "CNHC", 4);
@@ -1266,6 +1379,17 @@ extern "C" int cnhe_vecs_encrypt_compact(cnhe_ctx *h, const double *v, int n, ui
     for (int l = 0; l < c.k; l++) wr64(44 + 8 * (size_t)l, c.q[l]);
     for (int ch = 0; ch < c.P; ch++) wr64(44 + 8 * (size_t)c.k + 8 * (size_t)ch, c.t[ch]);
     for (int ch = 0; ch < c.P; ch++) memcpy(dst + 44 + 8 * (size_t)(c.k + c.P) + 32 * (size_t)ch, keys[ch].w, 32);
+}
+extern "C" int cnhe_vecs_encrypt_compact(cnhe_ctx *h, const double *v, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap, size_t *needed) {
+    API_BEGIN(h)
+    if (!v) fail("bad arguments");
+    encrypt_compact(c, [&] { return upload_values(c, v, (size_t)n * dim); }, n, dim, scale, dst, cap, needed);
+    API_END
+}
+extern "C" int cnhe_vecs_encrypt_compact_device(cnhe_ctx *h, uint64_t d_values, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap,
+                                                size_t *needed) {
+    API_BEGIN(h)
+    encrypt_compact(c, [&] { return device_values(d_values); }, n, dim, scale, dst, cap, needed);
     API_END
 }
 // Like cnhe_vecs_import_raw: the packed bytes go to a staging upload slot on the upload stream, k_compact_expand writes the ciphertexts

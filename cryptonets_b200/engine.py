@@ -3,6 +3,7 @@
 This is binding code only -- every method is one call into libcnhe.so.  The reference-shaped API (IFactory, IVector,
 IMatrix, layers) lives in he.py / layers.py on top of this."""
 import ctypes as C
+import sys
 import weakref
 
 import numpy as np
@@ -20,6 +21,12 @@ def _u64(a):
 
 def _p(a):
     return a.ctypes.data_as(U64P)
+
+
+def _cuda_tensor(x):
+    """True for a torch tensor in CUDA memory (torch is never imported here: a tensor means the caller already has it)."""
+    torch = sys.modules.get("torch")
+    return torch is not None and isinstance(x, torch.Tensor) and x.is_cuda
 
 
 def _vec_array(vecs):
@@ -476,7 +483,30 @@ class Engine:
     def plain(self, v, scale=1.0, fmt=DENSE):
         return self._new(self.L.cnhe_vec_plain, v, scale, fmt)
 
+    # ---- values in device memory (DESIGN 4.19): torch work is ordered with the library's channel-0 stream by events, never by a
+    # device-wide synchronise
+    def _library_stream(self, device):
+        import torch
+        return torch.cuda.ExternalStream(self.stream(0), device=device)
+
+    def _device_rows(self, rows):
+        """A CUDA tensor [n][dim] as contiguous float64 on its device, with the library's stream made to wait for the caller's current
+        stream (where the tensor, and its conversion, were queued)."""
+        import torch
+        if rows.dim() != 2:
+            raise ValueError("rows must be [n][dim]")
+        t = rows.to(torch.float64).contiguous()
+        self._library_stream(t.device).wait_stream(torch.cuda.current_stream(t.device))
+        return t  # the encrypt calls return once they have read it
+
     def encrypt_many(self, rows, scale=1.0):
+        """Encrypts the rows [n][dim] of a numpy array or a CUDA torch tensor (float64, or converted on its device) as n dense vectors."""
+        if _cuda_tensor(rows):
+            t = self._device_rows(rows)
+            n, dim = t.shape
+            out = (VECP * n)()
+            check(self.L.cnhe_vecs_encrypt_device(self.h, t.data_ptr(), n, dim, float(scale), out))
+            return [Vec(self, out[i]) for i in range(n)]
         a = np.ascontiguousarray(rows, dtype=np.float64)
         n, dim = a.shape
         out = (VECP * n)()
@@ -508,8 +538,19 @@ class Engine:
         for v in live:
             v.h = VECP(None)
 
-    def decrypt_many(self, vecs):
+    def decrypt_many(self, vecs, device=False):
+        """The vectors' values [n][dim] as a numpy array, or with device=True (or a torch device) as a float64 CUDA tensor on the current
+        CUDA device: ready for work queued on the caller's current stream afterwards, without a host wait."""
         dim = vecs[0].dim
+        if device is not False:
+            import torch
+            dev = torch.device("cuda", torch.cuda.current_device()) if device is True else torch.device(device)
+            out = torch.empty((len(vecs), dim), dtype=torch.float64, device=dev)
+            lib = self._library_stream(dev)
+            lib.wait_stream(torch.cuda.current_stream(dev))  # the allocation's stream order: the library writes after it
+            check(self.L.cnhe_vecs_decrypt_device(self.h, _vec_array(vecs), len(vecs), out.data_ptr(), dim))
+            torch.cuda.current_stream(dev).wait_stream(lib)
+            return out
         out = np.zeros((len(vecs), dim), np.float64)
         check(self.L.cnhe_vecs_decrypt(self.h, _vec_array(vecs), len(vecs), out.ctypes.data_as(DBLP), dim))
         return out
@@ -541,13 +582,19 @@ class Engine:
 
     def encrypt_compact(self, rows, scale=1.0):
         """Seeded secret-key encryption of n dense vectors (rows [n][dim]) into one compact blob (bytes): bit-packed c0 plus one ChaCha20
-        key per plaintext modulus from which import_compact regenerates c1 on the GPU.  Needs the secret key."""
-        a = np.ascontiguousarray(rows, dtype=np.float64)
-        n, dim = a.shape
+        key per plaintext modulus from which import_compact regenerates c1 on the GPU.  Needs the secret key.  rows: a numpy array or a
+        CUDA torch tensor, as for encrypt_many."""
+        if _cuda_tensor(rows):
+            t = self._device_rows(rows)
+            fn, src = self.L.cnhe_vecs_encrypt_compact_device, t.data_ptr()
+        else:
+            t = np.ascontiguousarray(rows, dtype=np.float64)
+            fn, src = self.L.cnhe_vecs_encrypt_compact, t.ctypes.data_as(DBLP)
+        n, dim = t.shape
         need = C.c_size_t()
-        check(self.L.cnhe_vecs_encrypt_compact(self.h, a.ctypes.data_as(DBLP), n, dim, float(scale), None, 0, C.byref(need)))
+        check(fn(self.h, src, n, dim, float(scale), None, 0, C.byref(need)))
         buf = (C.c_ubyte * need.value)()
-        check(self.L.cnhe_vecs_encrypt_compact(self.h, a.ctypes.data_as(DBLP), n, dim, float(scale), buf, need.value, C.byref(need)))
+        check(fn(self.h, src, n, dim, float(scale), buf, need.value, C.byref(need)))
         return bytes(buf)
 
     def import_compact(self, buf_or_ptr, length=None):

@@ -6,7 +6,7 @@ every method a call into libcnhe.so.  Vectors hold device handles instead of SEA
 Errors surface as Python exceptions carrying the reference's message (the reference throws System.Exception)."""
 import numpy as np
 
-from .engine import ALL_SLOTS, Engine, Vec
+from .engine import ALL_SLOTS, Engine, Vec, _cuda_tensor
 from .interfaces import EMatrixFormat, EVectorFormat, check_deferred_mul
 
 
@@ -54,7 +54,10 @@ class B200BfvVector:
     def RegisterDim(self, dim):
         self.vec.register_dim(dim)
 
-    def Decrypt(self, env=None):
+    def Decrypt(self, env=None, device=False):
+        """The values as numpy, or with device=True (or a torch device) as a CUDA tensor (Engine.decrypt_many)."""
+        if device is not False:
+            return self.eng.decrypt_many([self.vec], device=device)[0]
         return self.eng.decrypt(self.vec)
 
     def DecryptFullPrecision(self, env=None):
@@ -149,8 +152,9 @@ class B200BfvMatrix:
         for v in self.vectors:
             v.RegisterScale(scale)
 
-    def Decrypt(self, env=None):
-        rows = self.eng.decrypt_many([v.vec for v in self.vectors])
+    def Decrypt(self, env=None, device=False):
+        """The values as numpy, or with device=True (or a torch device) as a CUDA tensor in the same orientation (Engine.decrypt_many)."""
+        rows = self.eng.decrypt_many([v.vec for v in self.vectors], device=device)
         return rows if self.Format == EMatrixFormat.RowMajor else rows.T
 
     def MulRows(self, v, ForceDenseFormat, first_row, total_rows):
@@ -366,6 +370,9 @@ class B200BfvFactory:
         return B200BfvVector(self, self.engine.copy(v.vec))
 
     def _rows(self, m, fmt):
+        """The vectors of matrix m as rows [n][dim]: a CUDA torch tensor stays on its device (transposed and made contiguous there)."""
+        if _cuda_tensor(m):
+            return m.T.contiguous() if fmt == EMatrixFormat.ColumnMajor else m
         m = np.asarray(m, dtype=np.float64)
         return m.T if fmt == EMatrixFormat.ColumnMajor else m
 
@@ -374,14 +381,17 @@ class B200BfvFactory:
         return B200BfvMatrix(self, vecs, fmt, CopyVectors=False)
 
     def GetEncryptedMatrix(self, m, fmt, scale):
-        rows = np.ascontiguousarray(self._rows(m, fmt))
+        """m: a numpy-compatible matrix or a CUDA torch tensor (encrypted from device memory)."""
+        rows = self._rows(m, fmt)
+        rows = rows if _cuda_tensor(rows) else np.ascontiguousarray(rows)
         vecs = [B200BfvVector(self, v) for v in self.engine.encrypt_many(rows, scale)]
         return B200BfvMatrix(self, vecs, fmt, CopyVectors=False)
 
     def GetEncryptedMatrixCompact(self, m, fmt, scale):
         """The same encryption as GetEncryptedMatrix as one compact blob (bytes) for a server: bit-packed c0 and per-channel ChaCha20 keys
         for c1 (include/cnhe.h, cnhe_vecs_encrypt_compact).  Needs the secret key; the matrix format travels out of band."""
-        return self.engine.encrypt_compact(np.ascontiguousarray(self._rows(m, fmt)), scale)
+        rows = self._rows(m, fmt)
+        return self.engine.encrypt_compact(rows if _cuda_tensor(rows) else np.ascontiguousarray(rows), scale)
 
     def LoadCompactMatrix(self, data, fmt, slot=0):
         """The matrix of a compact blob (GetEncryptedMatrixCompact), expanded on the GPU; `fmt` is the format it was made with.  slot: the

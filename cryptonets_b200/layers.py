@@ -10,6 +10,7 @@ import numpy as np
 
 from .interfaces import EMatrixFormat, EVectorFormat
 from .raw import RawFactory, RawMatrix, poly_scale
+from .engine import _cuda_tensor
 
 
 class ConvolutionEngine:
@@ -178,11 +179,12 @@ class BaseLayer:
 
 class MatrixSource(BaseLayer):
     """Input layer over an in-memory feature matrix: the role of `BatchReader` (`BatchReader.cs:59-109`) with the TSV parsing
-    replaced by a synthetic / caller-supplied array (no dataset ships with the reference).  rows = images."""
+    replaced by a synthetic / caller-supplied array (no dataset ships with the reference).  rows = images.  features may be a CUDA torch
+    tensor: the matrices it yields then hold tensors on that device, and EncryptLayer encrypts them from device memory."""
 
     def __init__(self, features, Scale=1.0, NormalizationFactor=1.0, MaxSlots=None, labels=None):
         super().__init__()
-        self.features = np.asarray(features, dtype=np.float64)
+        self.features = features.double() if _cuda_tensor(features) else np.asarray(features, dtype=np.float64)
         self.Scale = Scale
         self.NormalizationFactor = NormalizationFactor
         self.MaxSlots = MaxSlots or len(self.features)
@@ -226,6 +228,12 @@ class LLConvReader(MatrixSource):
         f = self.features[self.pos] * self.NormalizationFactor
         self.pos += 1
         ce = self.ce
+        if _cuda_tensor(f):  # the same gather on the device: taps outside the image read the appended zero
+            import torch
+            idx = np.array([[ce.Location(corner, off, ce.InputShape) for off in ce.Offsets] for corner in ce.Corners], dtype=np.int64)
+            idx[idx < 0] = f.numel()
+            mat = torch.cat([f, f.new_zeros(1)])[torch.as_tensor(idx, device=f.device)]
+            return RawMatrix(mat, self.Scale, EMatrixFormat.ColumnMajor, 0)
         mat = np.zeros((len(ce.Corners), len(ce.Offsets)))
         for c, corner in enumerate(ce.Corners):
             for o, off in enumerate(ce.Offsets):

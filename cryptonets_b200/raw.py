@@ -6,6 +6,7 @@ result is compared with; it plays the same three roles here.  It is not a fallba
 import numpy as np
 
 from .interfaces import EMatrixFormat, EVectorFormat, check_deferred_mul
+from .engine import _cuda_tensor
 
 
 def _round(a):
@@ -147,16 +148,21 @@ class RawMatrix:
     Max = 0.0
 
     def __init__(self, m, scale, fmt, block_size):
-        m = np.asarray(m, dtype=np.float64)
+        """m: a numpy-compatible matrix, or a CUDA torch tensor (an input matrix that stays on its device: its Data is a tensor, which an
+        encrypting factory reads from device memory; the Raw backend's own operations take numpy matrices)"""
         self.Scale = scale
         self.Format = fmt
-        self.m = _round(m * scale)
+        if _cuda_tensor(m):
+            import torch
+            self.m = torch.round(m.to(torch.float64) * scale)  # ties to even, as np.rint
+        else:
+            self.m = _round(np.asarray(m, dtype=np.float64) * scale)
         self.BlockSize = block_size
         self.DataDisposedExternaly = False
 
     RowCount = property(lambda s: s.m.shape[0])
     ColumnCount = property(lambda s: s.m.shape[1])
-    Data = property(lambda s: s.m.copy())
+    Data = property(lambda s: s.m.clone() if _cuda_tensor(s.m) else s.m.copy())
     IsEncrypted = property(lambda s: False)
 
     def Dispose(self):

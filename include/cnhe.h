@@ -253,6 +253,18 @@ int cnhe_export_wait(cnhe_ctx *, int ticket);
  * asynchronous copy and must stay unchanged until the imported vectors have been consumed (e.g. their outputs exported). */
 int cnhe_vecs_encrypt_compact(cnhe_ctx *, const double *v, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap, size_t *needed);
 int cnhe_vecs_import_compact(cnhe_ctx *, const uint8_t *src, size_t len, cnhe_vec **out, int cap, int *n);
+/* Values in device memory (DESIGN 4.19).  d_values / d_out are device addresses of row-major [n][dim] doubles on the context's device.
+ * cnhe_vecs_encrypt_device / cnhe_vecs_encrypt_compact_device: the vectors, nonces and blob of cnhe_vecs_encrypt /
+ * cnhe_vecs_encrypt_compact, with the CRT split fused into the GPU encode.  d_values is read after the work already queued on the
+ * stream of channel 0 (cnhe_context_stream): a caller whose values come from another stream makes that stream wait first.  The calls
+ * return once d_values has been read.  An out-of-range value (NaN, infinity, |round(v scale)| >= 1.5e38) is CNHE_ERR_INVALID and takes no nonce.
+ * cnhe_vecs_decrypt_device: cnhe_vecs_decrypt into d_out, queued on channel 0's stream without waiting for it; work the caller queues
+ * on that stream afterwards sees the values, and the vectors may be destroyed once the call returns.  Vectors of another key slot are
+ * CNHE_ERR_STATE.  All three are refused while recording. */
+int cnhe_vecs_encrypt_device(cnhe_ctx *, uint64_t d_values, int n, uint64_t dim, double scale, cnhe_vec **out);
+int cnhe_vecs_encrypt_compact_device(cnhe_ctx *, uint64_t d_values, int n, uint64_t dim, double scale, uint8_t *dst, size_t cap,
+                                     size_t *needed);
+int cnhe_vecs_decrypt_device(cnhe_ctx *, const cnhe_vec *const *vecs, int n, uint64_t d_out, uint64_t dim);
 /* device pointer of a channel's ciphertext blocks (for NCCL gathers through torch; plumbing only) */
 int cnhe_vec_device_ptr(const cnhe_vec *, int channel, uint64_t *dptr, size_t *words);
 int cnhe_noise_budget(cnhe_ctx *, const cnhe_vec *, int channel, int block, int *bits); /* CryptoTracker.cs:41-52 */

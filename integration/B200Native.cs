@@ -78,6 +78,9 @@ namespace HEWrapper
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_export_wait(IntPtr a0, int ticket);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_encrypt_compact(IntPtr a0, double[] v, int n, ulong dim, double scale, byte[] dst, UIntPtr cap, out UIntPtr needed);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_import_compact(IntPtr a0, byte[] src, UIntPtr len, IntPtr[] @out, int cap, out int n);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_encrypt_device(IntPtr a0, ulong d_values, int n, ulong dim, double scale, IntPtr[] @out);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_encrypt_compact_device(IntPtr a0, ulong d_values, int n, ulong dim, double scale, byte[] dst, UIntPtr cap, out UIntPtr needed);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vecs_decrypt_device(IntPtr a0, IntPtr[] vecs, int n, ulong d_out, ulong dim);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_device_ptr(IntPtr a0, int channel, out ulong dptr, out UIntPtr words);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_noise_budget(IntPtr a0, IntPtr a1, int channel, int block, out int bits);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int cnhe_vec_add(IntPtr a0, IntPtr a, IntPtr b, out IntPtr @out);
