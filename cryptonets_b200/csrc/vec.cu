@@ -801,6 +801,8 @@ static std::vector<int> vec_slots(Context &c, const cnhe_vec *const *vs, int n, 
     return s;
 }
 // SplitBigNumbers ("EncryptedSealBfvVector.cs:352-365"): round(v*scale) -> +bigFactor if negative -> residues
+// On the host for plain vectors: they may be made while a graph records (the device split reads its range flag back), and plain sparse
+// vectors keep their residues on the host for MAC planning and the zero-plaintext checks.
 static void split_values(Context &c, const double *v, uint64_t n, double scale, std::vector<std::vector<u64>> &res) {
     res.assign(c.P, std::vector<u64>(n));
     for (uint64_t j = 0; j < n; j++) {
@@ -813,26 +815,15 @@ static void split_values(Context &c, const double *v, uint64_t n, double scale, 
         for (int i = 0; i < c.P; i++) res[i][j] = (u64)(z % c.t[i]);
     }
 }
-static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64>> &split, const double *v, uint64_t dim, double scale, int format,
-                                   bool encrypt);
-static cnhe_vec *make_vector(Context &c, const double *v, uint64_t dim, double scale, int format, bool encrypt) {
-    if (!v && dim) fail("null values");
-    if (format != CNHE_DENSE && format != CNHE_SPARSE) fail("bad format");
-    if (scale == 0) scale = 1; // AtomicSealBfvVector.cs:1120
-    std::vector<std::vector<u64>> split;
-    split_values(c, v, dim, scale, split);
-    return make_vector_split(c, split, v, dim, scale, format, encrypt);
-}
-// `split`: per plaintext modulus the residues of the (already scaled and rounded) values; `v` (may be null) only feeds the
-// all-slots-equal shortcut of plain dense vectors
-static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64>> &split, const double *v, uint64_t dim, double scale, int format,
-                                   bool encrypt) {
+// A plain vector.  `split`: per plaintext modulus the residues of the (already scaled and rounded) values; `v` (may be null) only feeds
+// the all-slots-equal shortcut of dense vectors
+static cnhe_vec *make_plain_vector(Context &c, const std::vector<std::vector<u64>> &split, const double *v, uint64_t dim, double scale, int format) {
     const size_t N = c.N;
     const int blocks = format == CNHE_DENSE ? (int)((dim + N - 1) / N) : (int)dim;
     if (blocks < 1) fail("empty vector");
-    cnhe_vec *out = new_vec(c, dim, scale, format, encrypt, blocks);
+    cnhe_vec *out = new_vec(c, dim, scale, format, false, blocks);
     std::unique_ptr<cnhe_vec> guard(out);
-    if (format == CNHE_SPARSE && !encrypt) {
+    if (format == CNHE_SPARSE) {
         out->scalars = split;
         for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
@@ -845,25 +836,15 @@ static cnhe_vec *make_vector_split(Context &c, const std::vector<std::vector<u64
     alloc_channels(out);
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
-        if (format == CNHE_DENSE) {
-            // BatchEncoder.Encode per N-slot chunk (AtomicSealBfvVector.cs:1123-1133); a short last chunk is zero padded
-            std::vector<u64> padded((size_t)blocks * N, 0);
-            memcpy(padded.data(), split[ch].data(), dim * 8);
-            u64 *dvals = c.ws_alloc((size_t)blocks * N);
-            c.upload(dvals, padded.data(), padded.size() * 8);
-            u64 *plain = encrypt ? c.ws_alloc((size_t)blocks * N) : out->ptr(ch);
-            op_encode(c, ch, dvals, blocks, (int)N, plain);
-            if (encrypt) {
-                op_encrypt(c, ch, plain, N, blocks, (int)N, take_nonces(c, ch, blocks), out->ptr(ch));
-            }
-        } else { // sparse encrypted: one constant-polynomial plaintext per element (AtomicSealBfvVector.cs:1135-1138)
-            u64 *dvals = c.ws_alloc(dim);
-            c.upload(dvals, split[ch].data(), dim * 8);
-            op_encrypt(c, ch, dvals, 1, blocks, 1, take_nonces(c, ch, blocks), out->ptr(ch));
-        }
+        // BatchEncoder.Encode per N-slot chunk (AtomicSealBfvVector.cs:1123-1133); a short last chunk is zero padded
+        std::vector<u64> padded((size_t)blocks * N, 0);
+        memcpy(padded.data(), split[ch].data(), dim * 8);
+        u64 *dvals = c.ws_alloc((size_t)blocks * N);
+        c.upload(dvals, padded.data(), padded.size() * 8);
+        op_encode(c, ch, dvals, blocks, (int)N, out->ptr(ch));
         c.host_fence(); // host staging buffers go out of scope
     }
-    if (v && !encrypt && format == CNHE_DENSE && dim % N == 0) { // every slot equal => every plaintext is the constant polynomial
+    if (v && dim % N == 0) { // every slot equal => every plaintext is the constant polynomial
         bool all_eq = true;
         for (uint64_t j = 1; j < dim && all_eq; j++) all_eq = v[j] == v[0];
         if (all_eq) {
@@ -903,33 +884,45 @@ static void check_values(int n, uint64_t dim, double &scale) {
     if (n < 1 || dim < 1) fail("bad arguments");
     if (scale == 0) scale = 1; // AtomicSealBfvVector.cs:1120
 }
+// encode_values' counterpart for residues [P][dim] the caller reduced: per channel uploaded and, dense, encoded (a short last block zero
+// padded) into the same layout
+static std::vector<u64 *> encode_residues(Context &c, const uint64_t *residues, uint64_t dim, bool dense) {
+    const size_t N = c.N, words = dense ? (dim + N - 1) / N * N : dim;
+    std::vector<u64 *> plain(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        u64 *vals = plain[ch] = c.ws_alloc(words);
+        if (dense) {
+            vals = c.ws_alloc(words);
+            CNHE_CUDA(cudaMemsetAsync(vals + dim, 0, (words - dim) * 8, c.stream));
+        }
+        c.h2d(vals, residues + (size_t)ch * dim, dim * 8);
+        if (dense) op_encode(c, ch, vals, (int)(words / N), (int)N, plain[ch]);
+    }
+    return plain;
+}
+// The encryption of every vector source: n vectors from per-channel plaintexts in encode_values' layout (sparse: n = 1, one
+// constant-polynomial plaintext per element, AtomicSealBfvVector.cs:1135-1138), in one wave per channel into one slab per channel
+static void encrypt_plain(Context &c, const std::vector<u64 *> &plain, int n, uint64_t dim, double scale, int format, cnhe_vec **out) {
+    const size_t N = c.N, coeffs = format == CNHE_DENSE ? N : 1;
+    const int bl = format == CNHE_DENSE ? (int)((dim + N - 1) / N) : (int)dim;
+    std::vector<BufRef> slab(c.P);
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        slab[ch] = c.alloc((size_t)n * bl * c.ct_words());
+        op_encrypt(c, ch, plain[ch], coeffs, n * bl, (int)coeffs, take_nonces(c, ch, (u64)n * bl), slab[ch]->p);
+    }
+    c.set_channel(0);
+    for (int i = 0; i < n; i++) out[i] = slab_view(new_vec(c, dim, scale, format, true, bl), slab, (size_t)i * bl);
+}
 // n dense vectors [n][dim] (device doubles) encrypted in one wave per channel into one slab per channel (GetEncryptedMatrix, IFactory.cs:353-380)
 static void encrypt_dense(Context &c, const double *values, int n, uint64_t dim, double scale, cnhe_vec **out) {
-    const size_t N = c.N;
-    const int bl = (int)((dim + N - 1) / N);
-    if ((uint64_t)n * bl >= (1ULL << 31)) fail("too many ciphertexts in one call");
-    const std::vector<u64 *> plain = encode_values(c, values, n, dim, scale, true);
-    std::vector<BufRef> big(c.P);
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        big[ch] = c.alloc((size_t)n * bl * c.ct_words());
-        op_encrypt(c, ch, plain[ch], N, n * bl, (int)N, take_nonces(c, ch, (u64)n * bl), big[ch]->p);
-    }
-    c.set_channel(0);
-    for (int i = 0; i < n; i++) out[i] = slab_view(new_vec(c, dim, scale, CNHE_DENSE, true, bl), big, (size_t)i * bl);
+    if ((uint64_t)n * ((dim + c.N - 1) / c.N) >= (1ULL << 31)) fail("too many ciphertexts in one call");
+    encrypt_plain(c, encode_values(c, values, n, dim, scale, true), n, dim, scale, CNHE_DENSE, out);
 }
-// a sparse encrypted vector: one constant-polynomial plaintext per element (AtomicSealBfvVector.cs:1135-1138)
-static cnhe_vec *encrypt_sparse(Context &c, const double *values, uint64_t dim, double scale) {
+static void encrypt_sparse(Context &c, const double *values, uint64_t dim, double scale, cnhe_vec **out) {
     if (dim >= (1ULL << 31)) fail("too many ciphertexts in one call");
-    const std::vector<u64 *> plain = encode_values(c, values, 1, dim, scale, false);
-    std::unique_ptr<cnhe_vec> out(new_vec(c, dim, scale, CNHE_SPARSE, true, (int)dim));
-    alloc_channels(out.get());
-    for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        op_encrypt(c, ch, plain[ch], 1, (int)dim, 1, take_nonces(c, ch, dim), out->ptr(ch));
-    }
-    c.set_channel(0);
-    return out.release();
+    encrypt_plain(c, encode_values(c, values, 1, dim, scale, false), 1, dim, scale, CNHE_SPARSE, out);
 }
 // a device copy of n * dim host doubles (stream 0)
 static const double *upload_values(Context &c, const double *v, size_t count) {
@@ -950,7 +943,7 @@ extern "C" int cnhe_vec_encrypt(cnhe_ctx *h, const double *v, uint64_t dim, doub
     check_values(1, dim, scale);
     const double *d = upload_values(c, v, dim);
     if (format == CNHE_DENSE) encrypt_dense(c, d, 1, dim, scale, out);
-    else *out = encrypt_sparse(c, d, dim, scale);
+    else encrypt_sparse(c, d, dim, scale, out);
     API_END
 }
 // BigInteger entry points of the factory ("HE Wrapper/IFactory.cs:29,43" -> EncryptedSealBfvVector(IEnumerable<BigInteger>, ...),
@@ -960,18 +953,27 @@ extern "C" int cnhe_vec_from_residues(cnhe_ctx *h, const uint64_t *residues, uin
     if (!residues || !out || dim < 1) fail("bad arguments");
     if (format != CNHE_DENSE && format != CNHE_SPARSE) fail("bad format");
     if (encrypt) not_recorded(c, ENCRYPT_WHY);
-    std::vector<std::vector<u64>> split(c.P, std::vector<u64>(dim));
+    if (scale == 0) scale = 1;
     for (int ch = 0; ch < c.P; ch++)
-        for (uint64_t j = 0; j < dim; j++) {
-            split[ch][j] = residues[(size_t)ch * dim + j];
-            if (split[ch][j] >= c.t[ch]) fail("residue not reduced modulo its plaintext prime");
-        }
-    *out = make_vector_split(c, split, nullptr, dim, scale == 0 ? 1 : scale, format, encrypt != 0);
+        for (uint64_t j = 0; j < dim; j++)
+            if (residues[(size_t)ch * dim + j] >= c.t[ch]) fail("residue not reduced modulo its plaintext prime");
+    if (encrypt) {
+        encrypt_plain(c, encode_residues(c, residues, dim, format == CNHE_DENSE), 1, dim, scale, format, out);
+    } else {
+        std::vector<std::vector<u64>> split(c.P);
+        for (int ch = 0; ch < c.P; ch++) split[ch].assign(residues + (size_t)ch * dim, residues + (size_t)(ch + 1) * dim);
+        *out = make_plain_vector(c, split, nullptr, dim, scale, format);
+    }
     API_END
 }
 extern "C" int cnhe_vec_plain(cnhe_ctx *h, const double *v, uint64_t dim, double scale, int format, cnhe_vec **out) {
     API_BEGIN(h)
-    *out = make_vector(c, v, dim, scale, format, false);
+    if (!v && dim) fail("null values");
+    if (format != CNHE_DENSE && format != CNHE_SPARSE) fail("bad format");
+    if (scale == 0) scale = 1; // AtomicSealBfvVector.cs:1120
+    std::vector<std::vector<u64>> split;
+    split_values(c, v, dim, scale, split);
+    *out = make_plain_vector(c, split, v, dim, scale, format);
     API_END
 }
 extern "C" int cnhe_vecs_encrypt(cnhe_ctx *h, const double *v, int n, uint64_t dim, double scale, cnhe_vec **out) {
@@ -991,36 +993,9 @@ extern "C" int cnhe_vecs_encrypt_device(cnhe_ctx *h, uint64_t d_values, int n, u
     API_END
 }
 
-// Decrypt of the blocks of one channel into residues (dense: first `dim` slots; sparse: constant coefficients)
-static void decrypt_channel(Context &c, const cnhe_vec *v, int ch, std::vector<u64> &res) {
-    const size_t N = c.N;
-    res.assign(v->dim, 0);
-    if (!v->enc && v->format == CNHE_SPARSE) { res = v->scalars[ch]; return; }
-    u64 *plain;
-    if (v->enc) {
-        if (v->key_slot() != 0) throw Error(CNHE_ERR_STATE, "the context holds no secret key of the vector's key slot");
-        plain = c.ws_alloc((size_t)v->blocks * N);
-        op_decrypt(c, ch, v->ptr(ch), v->blocks, plain);
-    } else plain = v->ptr(ch);
-    if (v->format == CNHE_DENSE) {
-        u64 *vals = c.ws_alloc((size_t)v->blocks * N);
-        op_decode(c, ch, plain, v->blocks, vals);
-        std::vector<u64> hostv((size_t)v->blocks * N);
-        CNHE_CUDA(cudaMemcpyAsync(hostv.data(), vals, hostv.size() * 8, cudaMemcpyDeviceToHost, c.stream));
-        c.sync();
-        const uint64_t take = std::min<uint64_t>(v->dim, hostv.size());
-        memcpy(res.data(), hostv.data(), take * 8);
-    } else {
-        std::vector<u64> hostv(v->blocks);
-        CNHE_CUDA(cudaMemcpy2DAsync(hostv.data(), 8, plain, N * 8, 8, v->blocks, cudaMemcpyDeviceToHost, c.stream));
-        c.sync();
-        const uint64_t take = std::min<uint64_t>(v->dim, hostv.size());
-        memcpy(res.data(), hostv.data(), take * 8);
-    }
-}
-// out [n][dim] (device) = the first `dim` values of each vector (zero past its last block), stream-ordered on stream 0.  Per channel one
-// decryption wave over every encrypted block and one decode wave over every dense block; then one CRT join over all values on stream 0.
-static void decrypt_values(Context &c, const cnhe_vec *const *vecs, int n, uint64_t dim, double *out) {
+// The residues of n vectors of dimension `dim`, stream-ordered on stream 0: per channel one decryption wave over every encrypted block and
+// one decode wave over every dense block.  src[ch * n + i] says where vector i's residues of channel ch are.
+static std::vector<JoinSrc> decrypt_channels(Context &c, const cnhe_vec *const *vecs, int n, uint64_t dim) {
     if (n < 1 || !vecs) fail("bad arguments");
     for (int i = 0; i < n; i++) {
         same_ctx(c, vecs[i]);
@@ -1076,6 +1051,12 @@ static void decrypt_values(Context &c, const cnhe_vec *const *vecs, int n, uint6
     }
     c.join_streams();
     c.set_channel(0);
+    return src;
+}
+// out [n][dim] (device) = the first `dim` values of each vector (zero past its last block), stream-ordered on stream 0: the residues of
+// decrypt_channels, then one CRT join over all values on stream 0.
+static void decrypt_values(Context &c, const cnhe_vec *const *vecs, int n, uint64_t dim, double *out) {
+    const std::vector<JoinSrc> src = decrypt_channels(c, vecs, n, dim);
     JoinConst jc;
     memset(&jc, 0, sizeof(jc));
     jc.P = c.P;
@@ -1113,12 +1094,14 @@ extern "C" int cnhe_vec_decrypt_residues(cnhe_ctx *h, const cnhe_vec *v, uint64_
     not_recorded(c, "returns words to the host");
     same_ctx(c, v);
     if (!out || cap < v->dim * (uint64_t)c.P) fail("destination too small");
+    const std::vector<JoinSrc> src = decrypt_channels(c, &v, 1, v->dim);
+    std::fill(out, out + (size_t)c.P * v->dim, 0); // zero past the last block
     for (int ch = 0; ch < c.P; ch++) {
-        c.set_channel(ch);
-        std::vector<u64> r;
-        decrypt_channel(c, v, ch, r);
-        memcpy(out + (size_t)ch * v->dim, r.data(), v->dim * 8);
+        const JoinSrc &s = src[ch];
+        CNHE_CUDA(cudaMemcpy2DAsync(out + (size_t)ch * v->dim, 8, s.p, s.stride * 8, 8, std::min<uint64_t>(v->dim, s.count), cudaMemcpyDeviceToHost,
+                                    c.stream));
     }
+    c.sync();
     API_END
 }
 extern "C" int cnhe_vecs_decrypt(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, double *out, uint64_t dim) {
@@ -1744,9 +1727,9 @@ extern "C" int cnhe_vecs_rotate(cnhe_ctx *h, const cnhe_vec *const *vecs, int n,
     rotate_vecs(c, vecs, n, amount, out);
     API_END
 }
-extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap) {
-    API_BEGIN(h)
-    not_recorded(c, "returns words to the host");
+// the checks and copies of cnhe_vecs_export_raw(_async): dst [P][n][blocks][2kN] from n encrypted vectors of equal block counts, queued on
+// each channel's stream.  The two entry points differ only in how they wait for the copies.
+static void queue_export(Context &c, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap) {
     if (n < 1 || !dst) fail("bad arguments");
     const int blocks = vecs[0]->blocks;
     const size_t per = (size_t)blocks * c.ct_words();
@@ -1754,25 +1737,25 @@ extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, in
     for (int i = 0; i < n; i++) {
         same_ctx(c, vecs[i]);
         if (!vecs[i]->enc || vecs[i]->blocks != blocks) fail("expecting encrypted vectors with equal block counts");
-        for (int ch = 0; ch < c.P; ch++) {
-            c.set_channel(ch);
-            CNHE_CUDA(cudaMemcpyAsync(dst + ((size_t)ch * n + i) * per, vecs[i]->ptr(ch), per * 8, cudaMemcpyDeviceToHost, c.stream));
-        }
     }
+    for (int ch = 0; ch < c.P; ch++) {
+        c.set_channel(ch);
+        for (int i = 0; i < n; i++)
+            CNHE_CUDA(cudaMemcpyAsync(dst + ((size_t)ch * n + i) * per, vecs[i]->ptr(ch), per * 8, cudaMemcpyDeviceToHost, c.stream));
+    }
+}
+extern "C" int cnhe_vecs_export_raw(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap) {
+    API_BEGIN(h)
+    not_recorded(c, "returns words to the host");
+    queue_export(c, vecs, n, dst, cap);
     c.sync();
     API_END
 }
 extern "C" int cnhe_vecs_export_raw_async(cnhe_ctx *h, const cnhe_vec *const *vecs, int n, uint64_t *dst, size_t cap, int *ticket) {
     API_BEGIN(h)
     not_recorded(c, "returns words to the host");
-    if (n < 1 || !dst || !ticket) fail("bad arguments");
-    const int blocks = vecs[0]->blocks;
-    const size_t per = (size_t)blocks * c.ct_words();
-    if (cap < (size_t)c.P * n * per) fail("destination too small");
-    for (int i = 0; i < n; i++) {
-        same_ctx(c, vecs[i]);
-        if (!vecs[i]->enc || vecs[i]->blocks != blocks) fail("expecting encrypted vectors with equal block counts");
-    }
+    if (!ticket) fail("bad arguments");
+    queue_export(c, vecs, n, dst, cap);
     if (c.ev_export.empty()) {
         c.ev_export.resize((size_t)8 * c.P);
         for (cudaEvent_t &e : c.ev_export) CNHE_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -1781,8 +1764,6 @@ extern "C" int cnhe_vecs_export_raw_async(cnhe_ctx *h, const cnhe_vec *const *ve
     c.export_next = (c.export_next + 1) & 7;
     for (int ch = 0; ch < c.P; ch++) {
         c.set_channel(ch);
-        for (int i = 0; i < n; i++)
-            CNHE_CUDA(cudaMemcpyAsync(dst + ((size_t)ch * n + i) * per, vecs[i]->ptr(ch), per * 8, cudaMemcpyDeviceToHost, c.stream));
         CNHE_CUDA(cudaEventRecord(c.ev_export[(size_t)t * c.P + ch], c.stream));
     }
     *ticket = t;
@@ -2009,13 +1990,9 @@ static cnhe_vec *sum_all_slots(Context &c, const cnhe_vec *a, uint64_t length, i
         len = sum_slots_batched(c, ch, sum, 1, length);
         if (force_column >= 0) { // one-hot mask (":936-945")
             if ((size_t)force_column >= N) fail("column out of range");
-            std::vector<u64> onehot(N, 0);
-            onehot[force_column] = 1;
-            u64 *dv = c.ws_alloc(N), *pl = c.ws_alloc(N);
-            c.upload(dv, onehot.data(), N * 8);
-            op_encode(c, ch, dv, 1, (int)N, pl);
+            u64 *pl = c.ws_alloc(N);
+            op_encode_onehot(c, ch, 1, force_column, pl);
             op_multiply_plain_dense(c, ch, sum, 1, pl, false, sum);
-            c.host_fence();
             len = 1;
         }
     }

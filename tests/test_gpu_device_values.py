@@ -50,7 +50,8 @@ def _words(eng, vecs):
 
 
 def _reference_vecs(eng, cfg, vals, scale):
-    """the vectors of the reference split, encrypted through cnhe_vec_from_residues (its own host path) from seed"""
+    """the vectors of the reference split, encrypted through cnhe_vec_from_residues from seed: its residues reach the plaintexts through
+    the encoder's scatter, not through the fused split-and-scatter under test"""
     eng.keygen(SEED)
     out = []
     for row in vals:
@@ -189,6 +190,60 @@ def test_decrypt_at_a_derived_level(setup):
         low.close()
 
 
+def _split(vals, scale, cfg):
+    return np.array(vr.split(vals.tolist(), scale, cfg["t"]), dtype=np.uint64)
+
+
+def test_decrypt_residues_every_kind(setup):
+    """cnhe_vec_decrypt_residues of every kind of vector: the residues of the reference split, exactly"""
+    eng, cfg = setup
+    N = cfg["N"]
+    eng.keygen(SEED)
+    kinds = {"plain dense": (DENSE, False, N + 7), "plain sparse": (SPARSE, False, 37), "encrypted dense, one block": (DENSE, True, N // 2 + 3),
+             "encrypted dense, three blocks": (DENSE, True, 2 * N + 5), "encrypted sparse": (SPARSE, True, 29)}
+    for seed, (name, (fmt, enc, dim)) in enumerate(kinds.items()):
+        vals = _edge_values(cfg, 1, dim, seed)[0]
+        v = eng.encrypt(vals, 2.0, fmt) if enc else eng.plain(vals, 2.0, fmt)
+        assert np.array_equal(eng.decrypt_residues(v), _split(vals, 2.0, cfg)), name
+    if cfg["dbc_r"] <= 16:  # wider digits: the context keeps no products pending
+        # a pending square: the size-3 ciphertext (c0, c1, 0) of a fresh encryption decrypts as that encryption does once relinearised
+        vals = _edge_values(cfg, 1, N, 11)[0]
+        fresh = eng.encrypt(vals, 2.0, DENSE)
+        zero = np.zeros(eng.ct_words // 2, np.uint64)
+        sq = eng.raw_import_products(np.stack([np.concatenate([fresh.export_raw(ch), zero]) for ch in range(eng.P)]), 1, N, 2.0)[0]
+        assert np.array_equal(eng.decrypt_residues(sq), _split(vals, 2.0, cfg))
+    if eng.k < 2:
+        return
+    low = eng.derive_level(eng.k - 1)
+    try:
+        vals = _edge_values(cfg, 1, 60, 12)[0]
+        v = eng.mod_switch(eng.encrypt_many(vals[None, :], 2.0), low)[0]
+        assert np.array_equal(low.decrypt_residues(v), _split(vals, 2.0, cfg))
+    finally:
+        low.close()
+
+
+def test_force_output_in_column(setup):
+    """sum_all_slots / dot_product with force_column at the first and last slot of each row: the full sum in that slot alone; column N
+    is refused"""
+    from cryptonets_b200._lib import CnheError
+    eng, cfg = setup
+    N = cfg["N"]
+    rng = np.random.default_rng(12)
+    a, b = rng.integers(-2, 3, N).astype(np.float64), rng.integers(-2, 3, N).astype(np.float64)
+    eng.keygen(SEED)
+    va, vb = eng.encrypt(a, 1.0, DENSE), eng.encrypt(b, 1.0, DENSE)
+    for col in (0, N // 2 - 1, N // 2, N - 1):
+        for out, total in ((eng.sum_all_slots(va, force_column=col), a.sum()), (eng.dot_product(va, vb, force_column=col), a @ b)):
+            want = np.zeros(N)
+            want[col] = total
+            assert np.array_equal(eng.decrypt(out), want), col
+    for f in (lambda: eng.sum_all_slots(va, force_column=N), lambda: eng.dot_product(va, vb, force_column=N)):
+        with pytest.raises(CnheError) as e:
+            f()
+        assert e.value.code == -1
+
+
 def test_one_wave_per_channel(setup):
     torch = _torch()
     eng, cfg = setup
@@ -236,7 +291,7 @@ def test_refusals_key_slot_and_recording(setup):
         slot = eng.add_client_compact(client.save_compact_keys(public=False, galois=[]))
         v = eng.encrypt_many(np.ones((1, 8)), 1.0)[0]
         v.set_key_slot(slot)
-        for f in (lambda: eng.decrypt_many([v]), lambda: eng.decrypt_many([v], device=True)):
+        for f in (lambda: eng.decrypt_many([v]), lambda: eng.decrypt_many([v], device=True), lambda: eng.decrypt_residues(v)):
             with pytest.raises(CnheError) as e:
                 f()
             assert e.value.code == -3
