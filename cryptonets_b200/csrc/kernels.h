@@ -71,12 +71,12 @@ cudaError_t launch_ntt_forward(const u64 *src, u64 *dst, int n_polys, int logn, 
 cudaError_t launch_ntt_inverse(const u64 *src, u64 *dst, int n_polys, int logn, const NttTab *tabs, int mod_base, int mod_count, int fp,
                                cudaStream_t s);
 // dst[((c*k + l)*D + d)] = NTT_l( digit d of target[c] )   target: [n_ct][k][N] coefficient form
-// ciphertext c's k-residue target polynomial starts at target + c * ct_stride (words)
+// ciphertext c's k-residue target polynomial starts at target + c * ct_stride (words); fp: 0, or NTT_FP | NTT_OUT_F (lazy doubles out)
 cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *dst, int n_ct, int k, const DigitMap &dm, int logn,
                                       const NttTab *tabs, int fp, cudaStream_t s);
 // Fused key switch (N = 4096 / 8192, FP64 path): out[c][p][l] = base_c[p][l] + INTT_l(sum_d NTT_l(digit d of target[c]) * key[d][p][l])
 // (mod q_l, canonical), key [D][2][k][N] canonical NTT form, base polynomial p of ciphertext c at base + c * base_stride + p * k * N, out
-// packed [n_ct][2][k][N] -- what launch_ntt_forward_digits, launch_ks_mac_fp(lazy) and launch_ntt_inverse_add compute, with no digit
+// packed [n_ct][2][k][N] -- what launch_ntt_forward_digits, launch_ks_mac_fp and launch_ntt_inverse_add compute, with no digit
 // buffer and no accumulator.  out must overlap neither the target nor the base words: other CTAs still read them while one writes.
 // key_packed: nullptr, or the copy of `key` made by launch_pack_keys48 (every q_l < 2^48), which the kernel then reads instead.
 // key_tab: nullptr, or a device table of n_ct key bases (ciphertext c reads key_tab[c] in place of key, or of key_packed when that is set)
@@ -132,7 +132,7 @@ struct BehzConstF {
     double q_mod_bsk[KBMAX], inv_q_mod_bsk[KBMAX], inv_mtilde_mod_bsk[KBMAX];
     double inv_bhat_mod_b[KBMAX], bhat_mod_q[KMAX][KBMAX], bhat_mod_msk[KBMAX];
     double inv_B_mod_msk, msk_half, B_mod_q[KMAX];
-    u64 q_u[KMAX], b_u[KBMAX]; // the moduli as integers (sign fix-up of canonical outputs on the integer pipe)
+    u64 q_u[KMAX]; // the coefficient moduli as integers (sign fix-up of canonical outputs on the integer pipe)
 };
 // Constants of the folded fast_floor / fastbconv_sk kernel (k_behz_floor_fold_fp), per plaintext modulus: every product by a constant
 // that SEAL applies in sequence (x t, x q-hat_i^-1, x q^-1, x B-hat_j^-1) is merged into the next conversion matrix on the host --
@@ -239,30 +239,26 @@ cudaError_t launch_behz_tensor(const u64 *a, const u64 *b, u64 *d, int n, int kt
 // mod q_l before the epilogue (the cubic activation's level 2, cnhe_layer_poly)
 cudaError_t launch_behz_floor(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConst *bc, cudaStream_t s, const FloorEpi *epi = nullptr,
                               bool pair = false);
-// lazy = 1: the buffers exchanged with the NTT kernels (lift output, tensor input/output, digit input, accumulator output) hold lazy
-// doubles (fparith.cuh) -- pair with NTT_IN_F / NTT_OUT_F on the transforms in between
-cudaError_t launch_behz_lift_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
+// FP64 (behz_fp.cu): the buffers exchanged with the NTT kernels (lift output, tensor input/output, digit input, accumulator output) hold
+// lazy doubles (fparith.cuh) -- pair with NTT_IN_F / NTT_OUT_F on the transforms in between
+cudaError_t launch_behz_lift_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, cudaStream_t s);
 // lazy Bsk residues only, out [n][2][kb][N]: the source of the fused square's residues l >= k
 cudaError_t launch_behz_lift_bsk_fp(const u64 *const *ct_ptrs, u64 *out, int n, int logn, const BehzConstF *f, cudaStream_t s);
 // Fused square (N = 4096 / 8192, ntt.cu): d [n][3][kt][N] lazy doubles, coefficient form, from ciphertexts ct_ptrs[c] ([2][k][N]) and
 // their lifted Bsk residues lift_bsk ([n][2][kb][N], launch_behz_lift_bsk_fp) -- what forward transforms, the square tensor and inverse
-// transforms compute on the output of launch_behz_lift_fp(lazy); needs split_ok on all kt moduli
+// transforms compute on the output of launch_behz_lift_fp; needs split_ok on all kt moduli
 cudaError_t launch_behz_square_fused(const u64 *const *ct_ptrs, const u64 *lift_bsk, u64 *d, int n_ct, int k, int kt, int logn, const NttTab *tabs,
                                      cudaStream_t s);
-cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConstF *f, int lazy, cudaStream_t s);
+cudaError_t launch_behz_tensor_fp(const u64 *a, const u64 *b, u64 *d, int n, int kt, int logn, const BehzConstF *f, cudaStream_t s);
 // sums of T tensor products per output: d[o] = sum_j a[o T + j] (x) b[j], a [n_out T][2][kt][N] and b [T][2][kt][N] in NTT form, d
-// [n_out][3][kt][N] as launch_behz_tensor writes one product (lazy: lazy doubles in and out, else canonical words)
-cudaError_t launch_behz_tensor_mac_fp(const u64 *a, const u64 *b, u64 *d, int n_out, int T, int kt, int logn, const BehzConstF *f, int lazy,
-                                      cudaStream_t s);
+// [n_out][3][kt][N] as launch_behz_tensor writes one product (integer: canonical words; FP64: lazy doubles in and out)
+cudaError_t launch_behz_tensor_mac_fp(const u64 *a, const u64 *b, u64 *d, int n_out, int T, int kt, int logn, const BehzConstF *f, cudaStream_t s);
 cudaError_t launch_behz_tensor_mac(const u64 *a, const u64 *b, u64 *d, int n_out, int T, int kt, int logn, const BehzConst *bc, cudaStream_t s);
-// canonical input; lazy input takes the folded kernel below
-cudaError_t launch_behz_floor_fp(const u64 *d, u64 *out3, int n, u64 t, int logn, const BehzConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr,
-                                bool pair = false);
-// folded constants + software-pipelined loads (lazy input only)
+// the floor of launch_behz_floor on lazy input, with folded constants
 cudaError_t launch_behz_floor_fold_fp(const u64 *d, u64 *out3, int n, int logn, const FloorConstF *f, cudaStream_t s, const FloorEpi *epi = nullptr,
                                      bool pair = false);
 cudaError_t launch_ks_mac_fp(const u64 *digits, const u64 *key, const u64 *const *key_tab, u64 *acc, int n, int D, int k, int logn,
-                             const BehzConstF *f, int lazy, cudaStream_t s, bool ref = false);
+                             const BehzConstF *f, cudaStream_t s, bool ref = false);
 // ---- K6: key-switch inner product. digits [n][D][k][N] (NTT), key [D][2][k][N] (NTT) -> acc [n][2][k][N] (NTT)
 // key_tab: nullptr, or a device table of n key bases (ciphertext c reads key_tab[c] in place of key); ref: key and the key_tab entries
 // are key references (key_base), as for the fused key switch

@@ -648,8 +648,8 @@ k_ntt_forward_fp(const u64 *src, u64 *dst, const NttTab *__restrict__ tabs, int 
     prefetch_next_poly<LOGN>(src, b, gridDim.x, tid);
     fwd_body_fp<LOGN, IN_F, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (size_t)b * N, tb, tid);
 }
-// target: ciphertext c's polynomial with `k` residues starts at target + c * ct_stride (words)
-template <int LOGN, bool OUT_F>
+// target: ciphertext c's polynomial with `k` residues starts at target + c * ct_stride (words); the output is lazy doubles
+template <int LOGN>
 __global__ void __launch_bounds__(fp_threads(LOGN), fp_min_blocks(LOGN))
 k_ntt_forward_digits_fp(const u64 *target, size_t ct_stride, u64 *dst, const NttTab *__restrict__ tabs, int k, DigitMap dm) {
     extern __shared__ __align__(16) u64 sm[];
@@ -663,7 +663,7 @@ k_ntt_forward_digits_fp(const u64 *target, size_t ct_stride, u64 *dst, const Ntt
     fs.shift = dm.shift[d];
     fs.mask = dm.mask;
     fs.need_reduce = dm.mask >= tb.mod.p;
-    fwd_body_fp<LOGN, false, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (((size_t)c * k + l) * dm.D + d) * N, tb, tid); // [c][l][d]
+    fwd_body_fp<LOGN, false, true>(reinterpret_cast<double *>(sm), fs, dst + (((size_t)c * k + l) * dm.D + d) * N, tb, tid); // [c][l][d]
 }
 
 // ---- inverse, FP64: stage U (0..3) on 16 consecutive coefficients; tw[i] is the twiddle of their i-th butterfly block (8 >> U of them)
@@ -985,7 +985,6 @@ k_ntt_forward_split(const u64 *src, u64 *dst, const NttTab *__restrict__ tabs, i
     fs.digit = false; fs.need_reduce = false; fs.shift = 0; fs.mask = 0;
     fwd_split_body<IN_F, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (size_t)b * (2 * SPLIT_H) + half * SPLIT_H, tb, half, tid);
 }
-template <bool OUT_F>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(SPLIT_THREADS, 2)
 k_ntt_forward_digits_split(const u64 *target, size_t ct_stride, u64 *dst, const NttTab *__restrict__ tabs, int k, DigitMap dm) {
     extern __shared__ __align__(16) u64 sm[];
@@ -998,7 +997,7 @@ k_ntt_forward_digits_split(const u64 *target, size_t ct_stride, u64 *dst, const 
     fs.shift = dm.shift[d];
     fs.mask = dm.mask;
     fs.need_reduce = dm.mask >= tb.mod.p;
-    fwd_split_body<false, OUT_F>(reinterpret_cast<double *>(sm), fs, dst + (((size_t)c * k + l) * dm.D + d) * (2 * SPLIT_H) + half * SPLIT_H, tb, half, tid);
+    fwd_split_body<false, true>(reinterpret_cast<double *>(sm), fs, dst + (((size_t)c * k + l) * dm.D + d) * (2 * SPLIT_H) + half * SPLIT_H, tb, half, tid);
 }
 // last in-half pass (stages 8 .. HLOGN-1) and the cross-half butterfly of NB polynomials (consecutive half buffers of sm; polynomial b goes to
 // dst + b * dst_stride and, with a base, adds base_add + b * dst_stride): own results go to shared memory for the partner, the partner's
@@ -1762,17 +1761,17 @@ static cudaError_t launch_fwd_fp(const u64 *src, u64 *dst, int n_polys, const Nt
     }
     return cudaGetLastError();
 }
-template <int L, bool OUT_F>
+template <int L>
 static cudaError_t launch_fwd_digits_fp(const u64 *target, size_t ct_stride, u64 *dst, int n_polys, int k, const DigitMap &dm, const NttTab *tabs,
                                         cudaStream_t s) {
     if constexpr (L == 14) {
-        cudaError_t e = split_prep(k_ntt_forward_digits_split<OUT_F>);
+        cudaError_t e = split_prep(k_ntt_forward_digits_split);
         if (e != cudaSuccess) return e;
-        k_ntt_forward_digits_split<OUT_F><<<2 * n_polys, SPLIT_THREADS, SPLIT_SMEM, s>>>(target, ct_stride, dst, tabs, k, dm);
+        k_ntt_forward_digits_split<<<2 * n_polys, SPLIT_THREADS, SPLIT_SMEM, s>>>(target, ct_stride, dst, tabs, k, dm);
     } else {
-        cudaError_t e = prep(k_ntt_forward_digits_fp<L, OUT_F>, L);
+        cudaError_t e = prep(k_ntt_forward_digits_fp<L>, L);
         if (e != cudaSuccess) return e;
-        k_ntt_forward_digits_fp<L, OUT_F><<<n_polys, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(target, ct_stride, dst, tabs, k, dm);
+        k_ntt_forward_digits_fp<L><<<n_polys, fp_threads(L), ntt_kernel_smem_bytes(L), s>>>(target, ct_stride, dst, tabs, k, dm);
     }
     return cudaGetLastError();
 }
@@ -1826,10 +1825,9 @@ cudaError_t launch_ntt_forward_digits(const u64 *target, size_t ct_stride, u64 *
                                       const NttTab *tabs, int fp, cudaStream_t s) {
     if (n_ct <= 0) return cudaSuccess;
     if (fp & NTT_FP) {
-        if (fp & NTT_IN_F) return cudaErrorInvalidValue; // digits are cut from canonical words
-        const int n_polys = n_ct * dm.D * k;
-        CNHE_DISPATCH_LOGN(logn, return (fp & NTT_OUT_F) ? launch_fwd_digits_fp<L, true>(target, ct_stride, dst, n_polys, k, dm, tabs, s)
-                                                         : launch_fwd_digits_fp<L, false>(target, ct_stride, dst, n_polys, k, dm, tabs, s));
+        // digits are cut from canonical words; only the lazy output (for launch_ks_mac_fp) is built
+        if (fp != (NTT_FP | NTT_OUT_F)) return cudaErrorInvalidValue;
+        CNHE_DISPATCH_LOGN(logn, return launch_fwd_digits_fp<L>(target, ct_stride, dst, n_ct * dm.D * k, k, dm, tabs, s));
     }
     CNHE_DISPATCH_LOGN(logn, {
         cudaError_t e = prep(k_ntt_forward_digits<L>, L);

@@ -845,7 +845,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
     bc.inv_B_mod_msk = hm::inv(hm::product_mod(B, -1, M_SK), M_SK);
     CNHE_CUDA(cudaMalloc((void **)&c.d_bc, sizeof(BehzConst)));
     CNHE_CUDA(cudaMemcpy(c.d_bc, &bc, sizeof(BehzConst), cudaMemcpyHostToDevice));
-    // FP64 twin of the constants (used when every q_i and Bsk prime is below 2^50)
+    // FP64 twin of the constants (used on the FP64 element-wise path: fp_elementwise)
     {
         BehzConstF &f = c.h_bf;
         memset(&f, 0, sizeof(f));
@@ -866,7 +866,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
         for (int j = 0; j < kb; j++) {
             const u64 p = c.bsk[j];
             c.fp_elementwise = c.fp_elementwise && hm::bit_length(p) <= 48;
-            f.bd[j] = (double)p; f.binv[j] = 1.0 / (double)p; f.b_u[j] = p;
+            f.bd[j] = (double)p; f.binv[j] = 1.0 / (double)p;
             for (int i = 0; i < k; i++) f.qhat_mod_bsk[j][i] = cen(bc.qhat_mod_bsk[j][i], p);
             f.q_mod_bsk[j] = cen(bc.q_mod_bsk[j], p);
             f.inv_q_mod_bsk[j] = cen(bc.inv_q_mod_bsk[j], p);
@@ -879,8 +879,7 @@ Context *context_create(const u64 *plain_primes, int P, uint32_t N, const u64 *c
         f.inv_B_mod_msk = cen(bc.inv_B_mod_msk, M_SK);
         f.msk_half = (double)(M_SK >> 1);
         // lazy-double intermediates between the kernels of a multiply / key switch: FP64 everywhere on the q and Bsk transforms
-        c.lazy = c.fp_elementwise && getenv("CNHE_NO_LAZY") == nullptr;
-        for (int i = 0; i < k + kb; i++) c.lazy = c.lazy && c.h_tabs[i].fp_ok;
+        for (int i = 0; i < k + kb; i++) c.fp_elementwise = c.fp_elementwise && c.h_tabs[i].fp_ok;
         CNHE_CUDA(cudaMalloc((void **)&c.d_bf, sizeof(BehzConstF)));
         CNHE_CUDA(cudaMemcpy(c.d_bf, &f, sizeof(BehzConstF), cudaMemcpyHostToDevice));
     }
@@ -996,7 +995,7 @@ constexpr int KS_FUSED_MIN = 64;
 // CNHE_KS_FUSED=0 / =1 forces the digit path / the fused path wherever it is built (read per call: tests compare both in one process)
 static bool ks_fused_built(const Context &c) {
     if (c.logN != 12 && c.logN != 13) return false;
-    if (!(c.lazy && c.fp_elementwise && fp_range(c, 0, c.k))) return false;
+    if (!c.fp_elementwise) return false;
     for (int i = 0; i < c.k; i++)
         if (!c.h_tabs[i].split_ok) return false;
     return true;
@@ -1104,8 +1103,8 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
     const int k = c.k;
     const u64 *key_packed = keys.per_ct() ? (keys.packs.empty() ? nullptr : keys.packs[0]) : keys.packed;
     const size_t N = c.N;
-    const int fpq = fp_range(c, 0, k);
-    const bool lazy = c.lazy && fpq;
+    // the FP64 path passes lazy doubles from the digit transforms to the product and from the product to the inverse transforms
+    const int fwd = c.fp_elementwise ? NTT_FP | NTT_OUT_F : 0, inv = c.fp_elementwise ? NTT_FP | NTT_IN_F : 0;
     // the fused kernel writes `out` while other CTAs still read target and base words, so it serves only calls whose output overlaps
     // neither; every internal caller passes scratch, an in-place cnhe_raw_relinearize (out2 inside in3) takes the digit path
     const size_t out_words = (size_t)n * 2 * k * N;
@@ -1135,17 +1134,17 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
             {
                 PROF(0, 16.0 * N * (double)m * dm.D * k); // SURVEY 8d: 16N bytes per transform (8N digit source read + 8N written)
                 c.check(launch_ntt_forward_digits(target + (size_t)c0 * target_stride, target_stride, digits, m, k, dm, c.logN, c.d_tabs,
-                                                  fpq | (lazy ? NTT_OUT_F : 0), c.stream),
+                                                  fwd, c.stream),
                         "ntt_forward_digits");
             }
             PROF(3, 8.0 * N * ((double)m * dm.D * k + (double)dm.D * 2 * k + (double)m * 2 * k));
             const u64 *key = key_arg(c, keys.key);
-            if (c.fp_elementwise) c.check(launch_ks_mac_fp(digits, key, key_tab, acc, m, dm.D, k, c.logN, &c.h_bf, lazy, c.stream, c.rec != nullptr), "ks_mac_fp");
+            if (c.fp_elementwise) c.check(launch_ks_mac_fp(digits, key, key_tab, acc, m, dm.D, k, c.logN, &c.h_bf, c.stream, c.rec != nullptr), "ks_mac_fp");
             else c.check(launch_ks_mac(digits, key, key_tab, acc, m, dm.D, k, c.logN, c.d_bc, c.stream, c.rec != nullptr), "ks_mac");
         }
         PROF(1, 24.0 * N * m * 2 * k);
         c.check(launch_ntt_inverse_add(acc, base + (size_t)c0 * base_stride, 2 * k, base_stride, out + (size_t)c0 * 2 * k * N, m * 2 * k, c.logN,
-                                       c.d_tabs, 0, k, fpq | (lazy ? NTT_IN_F : 0), c.stream),
+                                       c.d_tabs, 0, k, inv, c.stream),
                 "ntt_inverse_add");
     }
 }
@@ -1156,7 +1155,7 @@ void op_key_switch(Context &c, const u64 *target, size_t target_stride, int n, c
 static bool mul_fused(const Context &c, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b) {
     if (c.logN != 12 && c.logN != 13) return false;
     const int kt = c.k + c.kb;
-    if (!(c.lazy && c.fp_elementwise && fp_range(c, 0, kt))) return false;
+    if (!c.fp_elementwise) return false;
     for (int i = 0; i < kt; i++)
         if (!c.h_tabs[i].split_ok) return false;
     for (size_t i = 0; i < a.size(); i++)
@@ -1185,7 +1184,7 @@ FloorEpi floor_epi(const Context &c, int ch, u64 A, u64 B, u64 C) {
 }
 // epi: the call's FloorEpi, its x table (when the caller gave none: the squared operands, x_ptrs) and its c_poly table (one entry per
 // output of the call) still to be pointed at the wave, whose first output is o0.  m products; pair: they make m / 2 outputs (2i, 2i + 1)
-static void multiply_floor(Context &c, int ch, const u64 *D, int m, bool lazy, u64 *out3, const FloorEpi *epi = nullptr,
+static void multiply_floor(Context &c, int ch, const u64 *D, int m, u64 *out3, const FloorEpi *epi = nullptr,
                            const u64 *const *x_ptrs = nullptr, int o0 = 0, bool pair = false) {
     FloorEpi e;
     if (epi) {
@@ -1199,9 +1198,7 @@ static void multiply_floor(Context &c, int ch, const u64 *D, int m, bool lazy, u
     // parks the second product's floor in the output and reads it back
     PROF(2, 8.0 * c.N * m * 3 * (c.k + c.kb) + 8.0 * c.N * n_out * 3 * c.k + (epi ? 8.0 * c.N * n_out * 2 * c.k : 0.0) +
                 (pair ? 16.0 * c.N * n_out * 3 * c.k : 0.0));
-    if (c.fp_elementwise && lazy)
-        c.check(launch_behz_floor_fold_fp(D, out3, n_out, c.logN, &c.ch[ch].floor_f, c.stream, ep, pair), "behz_floor_fold_fp");
-    else if (c.fp_elementwise) c.check(launch_behz_floor_fp(D, out3, n_out, c.ch[ch].t, c.logN, &c.h_bf, c.stream, ep, pair), "behz_floor_fp");
+    if (c.fp_elementwise) c.check(launch_behz_floor_fold_fp(D, out3, n_out, c.logN, &c.ch[ch].floor_f, c.stream, ep, pair), "behz_floor_fold_fp");
     else c.check(launch_behz_floor(D, out3, n_out, c.ch[ch].t, c.logN, c.d_bc, c.stream, ep, pair), "behz_floor");
 }
 // products c0 .. c0 + m - 1 of a x b; with an epilogue, o0 is the wave's first output (c0, or c0 / 2 for pairs)
@@ -1222,7 +1219,7 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
             PROF(0, 8.0 * N * m * (2 * kt + 3 * kt));
             c.check(launch_behz_square_fused(ptrs, L, D, m, k, kt, c.logN, c.d_tabs, c.stream), "behz_square_fused");
         }
-        multiply_floor(c, ch, D, m, true, out3, epi, ptrs, o0, pair);
+        multiply_floor(c, ch, D, m, out3, epi, ptrs, o0, pair);
         return;
     }
     bool square = true;
@@ -1230,13 +1227,11 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
     if (epi && !square) throw Error(-1, "the activation epilogue applies to squares only");
     std::vector<const u64 *> pa(a.begin() + c0, a.begin() + c0 + m);
     u64 *A = c.ws_alloc((size_t)m * 2 * kt * N);
-    const int fpt = fp_range(c, 0, kt);
-    const int lazy = c.lazy && fpt ? 1 : 0;
-    const int fmt = fpt | (lazy ? NTT_IN_F | NTT_OUT_F : 0);
+    const int fmt = c.fp_elementwise ? NTT_FP | NTT_IN_F | NTT_OUT_F : 0;
     const u64 *const *pa_dev = upload_ptrs(c, pa);
     {
         PROF(2, 8.0 * N * m * 2 * (k + kt));
-        if (c.fp_elementwise) c.check(launch_behz_lift_fp(pa_dev, A, m, c.logN, &c.h_bf, lazy, c.stream), "behz_lift_fp");
+        if (c.fp_elementwise) c.check(launch_behz_lift_fp(pa_dev, A, m, c.logN, &c.h_bf, c.stream), "behz_lift_fp");
         else c.check(launch_behz_lift(pa_dev, A, m, c.logN, c.d_bc, c.stream), "behz_lift");
     }
     {
@@ -1247,21 +1242,21 @@ static void multiply_chunk(Context &c, int ch, const std::vector<const u64 *> &a
     if (!square) {
         std::vector<const u64 *> pb(b.begin() + c0, b.begin() + c0 + m);
         B = c.ws_alloc((size_t)m * 2 * kt * N);
-        if (c.fp_elementwise) c.check(launch_behz_lift_fp(upload_ptrs(c, pb), B, m, c.logN, &c.h_bf, lazy, c.stream), "behz_lift_fp");
+        if (c.fp_elementwise) c.check(launch_behz_lift_fp(upload_ptrs(c, pb), B, m, c.logN, &c.h_bf, c.stream), "behz_lift_fp");
         else c.check(launch_behz_lift(upload_ptrs(c, pb), B, m, c.logN, c.d_bc, c.stream), "behz_lift");
         c.check(launch_ntt_forward(B, B, m * 2 * kt, c.logN, c.d_tabs, 0, kt, fmt, c.stream), "ntt_forward");
     }
     u64 *D = c.ws_alloc((size_t)m * 3 * kt * N);
     {
         PROF(2, 8.0 * N * m * kt * (square ? 5 : 7));
-        if (c.fp_elementwise) c.check(launch_behz_tensor_fp(A, B, D, m, kt, c.logN, &c.h_bf, lazy, c.stream), "behz_tensor_fp");
+        if (c.fp_elementwise) c.check(launch_behz_tensor_fp(A, B, D, m, kt, c.logN, &c.h_bf, c.stream), "behz_tensor_fp");
         else c.check(launch_behz_tensor(A, B, D, m, kt, c.logN, c.d_bc, c.stream), "behz_tensor");
     }
     {
         PROF(1, 16.0 * N * m * 3 * kt);
         c.check(launch_ntt_inverse(D, D, m * 3 * kt, c.logN, c.d_tabs, 0, kt, fmt, c.stream), "ntt_inverse");
     }
-    multiply_floor(c, ch, D, m, lazy, out3, epi, pa_dev, o0, pair);
+    multiply_floor(c, ch, D, m, out3, epi, pa_dev, o0, pair);
 }
 void op_multiply(Context &c, int ch, const std::vector<const u64 *> &a, const std::vector<const u64 *> &b, u64 *out3, const FloorEpi *epi) {
     const int n = (int)a.size();
@@ -1290,16 +1285,14 @@ void op_multiply_sum(Context &c, int ch, const std::vector<const u64 *> &a, cons
     (void)relin_keys(c, ch, n_out, slots); // a missing key fails before any launch
     const int k = c.k, kt = k + c.kb;
     const size_t N = c.N, lifted = (size_t)2 * kt * N, s3 = (size_t)3 * k * N;
-    const int fpt = fp_range(c, 0, kt);
-    const int lazy = c.lazy && fpt ? 1 : 0;
-    const int fmt = fpt | (lazy ? NTT_IN_F | NTT_OUT_F : 0);
+    const int fmt = c.fp_elementwise ? NTT_FP | NTT_IN_F | NTT_OUT_F : 0;
     // BEHZ lift and forward transforms of n ciphertexts into [n][2][kt][N] (as multiply_chunk lifts its operands)
     auto lift = [&](const std::vector<const u64 *> &cts, u64 *dst) {
         const int n = (int)cts.size();
         const u64 *const *dev = upload_ptrs(c, cts);
         {
             PROF(2, 8.0 * N * n * 2 * (k + kt));
-            if (c.fp_elementwise) c.check(launch_behz_lift_fp(dev, dst, n, c.logN, &c.h_bf, lazy, c.stream), "behz_lift_fp");
+            if (c.fp_elementwise) c.check(launch_behz_lift_fp(dev, dst, n, c.logN, &c.h_bf, c.stream), "behz_lift_fp");
             else c.check(launch_behz_lift(dev, dst, n, c.logN, c.d_bc, c.stream), "behz_lift");
         }
         PROF(0, 16.0 * N * n * 2 * kt);
@@ -1322,7 +1315,7 @@ void op_multiply_sum(Context &c, int ch, const std::vector<const u64 *> &a, cons
             {
                 // HBM: every column word once, the shared words once (the outputs' CTAs of one tile read them out of L2), the sums written once
                 PROF(2, 8.0 * N * ((double)m * nt * 2 * kt + (double)nt * 2 * kt + (double)m * 3 * kt));
-                if (c.fp_elementwise) c.check(launch_behz_tensor_mac_fp(A, S, D, m, nt, kt, c.logN, &c.h_bf, lazy, c.stream), "behz_tensor_mac_fp");
+                if (c.fp_elementwise) c.check(launch_behz_tensor_mac_fp(A, S, D, m, nt, kt, c.logN, &c.h_bf, c.stream), "behz_tensor_mac_fp");
                 else c.check(launch_behz_tensor_mac(A, S, D, m, nt, kt, c.logN, c.d_bc, c.stream), "behz_tensor_mac");
             }
             {
@@ -1331,10 +1324,10 @@ void op_multiply_sum(Context &c, int ch, const std::vector<const u64 *> &a, cons
             }
             u64 *dst = Y + (size_t)o0 * s3;
             if (j0 == 0) {
-                multiply_floor(c, ch, D, m, lazy, dst);
+                multiply_floor(c, ch, D, m, dst);
             } else { // the chunk's floor added mod q to the earlier chunks' (the add kernel over the three polynomials)
                 u64 *F = c.ws_alloc((size_t)m * s3);
-                multiply_floor(c, ch, D, m, lazy, F);
+                multiply_floor(c, ch, D, m, F);
                 c.check(launch_ct_add(dst, F, dst, (size_t)m * s3, k, c.logN, c.d_bc, 0, c.stream), "ct_add");
             }
         }
@@ -1562,7 +1555,6 @@ void op_multiply_plain_dense_outer(Context &c, int ch, const std::vector<const u
     const size_t N = c.N, kN = (size_t)k * N, ctw = 2 * kN;
     if (B < 1 || R < 1) return;
     if (B == 1) return op_multiply_plain_dense_bcast(c, ch, cts[0], plains, R, out);
-    const bool fp = c.fp_elementwise && fpq;
     WsScope scope(c);
     u64 *ctn = c.ws_alloc((size_t)B * ctw);
     bool packed = true;
@@ -1579,7 +1571,7 @@ void op_multiply_plain_dense_outer(Context &c, int ch, const std::vector<const u
         u64 *lifted = c.ws_alloc((size_t)m * kN);
         c.check(launch_plain_lift(plains + (size_t)r0 * N, lifted, m, (int)N, k, c.logN, c.d_bc, c.ch[ch].pc, c.stream), "plain_lift");
         c.check(launch_ntt_forward(lifted, lifted, m * k, c.logN, c.d_tabs, 0, k, fpq, c.stream), "ntt_forward");
-        if (fp) c.check(launch_dyadic_outer(ctn, lifted, out + (size_t)r0 * ctw, B, m, R, k, c.logN, &c.h_bf, c.stream), "dyadic_outer");
+        if (c.fp_elementwise) c.check(launch_dyadic_outer(ctn, lifted, out + (size_t)r0 * ctw, B, m, R, k, c.logN, &c.h_bf, c.stream), "dyadic_outer");
         else
             for (int b = 0; b < B; b++)
                 c.check(launch_dyadic_bcast(ctn + (size_t)b * ctw, lifted, out + ((size_t)b * R + r0) * ctw, m, 2, 0, 1, k, c.logN, c.d_bc, c.stream),

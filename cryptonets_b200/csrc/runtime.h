@@ -136,8 +136,9 @@ struct Context {
     BehzConst *d_bc = nullptr;
     BehzConstF h_bf;
     BehzConstF *d_bf = nullptr;
-    bool fp_elementwise = false; // every q_i, Bsk prime small enough for the FP64 element-wise kernels
-    bool lazy = false;           // ... and for lazy-double intermediates between the kernels of a multiply / key switch
+    // the FP64 element-wise path: every q_i and Bsk prime small enough for the FP64 element-wise kernels, and every one of their transforms
+    // exact on FP64 butterflies (fp_ok), so that lazy doubles pass between the kernels of a multiply / key switch
+    bool fp_elementwise = false;
     std::vector<NttTab> h_tabs;
     NttTab *d_tabs = nullptr;
     u64 *d_table_mem = nullptr;

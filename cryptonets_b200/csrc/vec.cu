@@ -635,17 +635,14 @@ extern "C" int cnhe_raw_rotate_rows(cnhe_ctx *h, int channel, uint64_t in, int n
 }
 extern "C" int cnhe_raw_behz_lift(cnhe_ctx *h, uint64_t in_cts, int n, uint64_t out) {
     API_BEGIN(h)
-    if (c.fp_elementwise)
-        c.check(launch_behz_lift_fp(upload_ptrs(c, strided(in_cts, n, c.ct_words())), (u64 *)out, n, c.logN, &c.h_bf, 0, c.stream), "behz_lift_fp");
-    else c.check(launch_behz_lift(upload_ptrs(c, strided(in_cts, n, c.ct_words())), (u64 *)out, n, c.logN, c.d_bc, c.stream), "behz_lift");
+    c.check(launch_behz_lift(upload_ptrs(c, strided(in_cts, n, c.ct_words())), (u64 *)out, n, c.logN, c.d_bc, c.stream), "behz_lift");
     API_END
 }
 extern "C" int cnhe_raw_behz_floor(cnhe_ctx *h, int channel, uint64_t d, int n, uint64_t out3) {
     API_BEGIN(h)
     if (channel < 0 || channel >= c.P) fail("bad channel");
     c.set_channel(channel);
-    if (c.fp_elementwise) c.check(launch_behz_floor_fp((const u64 *)d, (u64 *)out3, n, c.ch[channel].t, c.logN, &c.h_bf, c.stream), "behz_floor_fp");
-    else c.check(launch_behz_floor((const u64 *)d, (u64 *)out3, n, c.ch[channel].t, c.logN, c.d_bc, c.stream), "behz_floor");
+    c.check(launch_behz_floor((const u64 *)d, (u64 *)out3, n, c.ch[channel].t, c.logN, c.d_bc, c.stream), "behz_floor");
     API_END
 }
 extern "C" int cnhe_dev_copy(cnhe_ctx *h, uint64_t dst, uint64_t src, size_t words) {
@@ -3894,9 +3891,6 @@ extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe
     }
     gstart.push_back(nd);
     const int ng = (int)gs.size();
-    bool fp = c.fp_elementwise;
-    for (int l = 0; l < k; l++) fp = fp && c.h_tabs[l].fp_ok;
-    const int fpq = fp ? 1 : 0;
     std::vector<std::unique_ptr<cnhe_vec>> outs(B);
     std::vector<BufRef> slab(c.P); // folded: the B outputs side by side, for the fold ladder and the mask
     for (int ch = 0; ch < c.P && d->fold; ch++) {
@@ -3932,7 +3926,7 @@ extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe
         op_ntt(c, X, X, nx * B * 2 * k, 0, k, false);
         u64 *acc = c.ws_alloc((size_t)ng * B * ctw); // [g][client], coefficient form once its wave is done
         const int *dxsel = nullptr;
-        if (fp) {
+        if (c.fp_elementwise) {
             int *p = reinterpret_cast<int *>(c.ws_alloc(((size_t)nd + 1) / 2));
             c.h2d(p, xsel.data(), (size_t)nd * sizeof(int));
             dxsel = p;
@@ -3954,7 +3948,7 @@ extern "C" int cnhe_mat_mul_diagonal(cnhe_ctx *h, const cnhe_diag *d, const cnhe
                 op_ntt(c, L, L, m * k, 0, k, false);
             }
             u64 *A = acc + (size_t)gi0 * B * ctw;
-            if (fp) {
+            if (c.fp_elementwise) {
                 std::vector<int> st(gw + 1);
                 for (int i = 0; i <= gw; i++) st[i] = gstart[gi0 + i] - j0;
                 int *dst = reinterpret_cast<int *>(c.ws_alloc(((size_t)gw + 2) / 2));

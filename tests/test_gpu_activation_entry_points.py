@@ -7,7 +7,7 @@ from cryptonets_b200.engine import DENSE, SPARSE, Engine
 
 pytestmark = pytest.mark.gpu
 
-KERNEL_ENV = ("CNHE_MAC_NO_UMMA", "CNHE_MAC_NO_IMMA", "CNHE_MAC_INT", "CNHE_MUL_FUSED", "CNHE_KS_FUSED", "CNHE_NO_LAZY")
+KERNEL_ENV = ("CNHE_MAC_NO_UMMA", "CNHE_MAC_NO_IMMA", "CNHE_MAC_INT", "CNHE_MUL_FUSED", "CNHE_KS_FUSED")
 
 
 def _engine(monkeypatch):

@@ -3,10 +3,10 @@ one BEHZ floor per chunk of at most K_c terms and one relinearisation per output
 
 Every output word must equal the CPU oracle's restatement, per plaintext prime and output block i:
     Y_i = sum over chunks (mod q) of floor(INTT(sum_{k in chunk} NTT(lift(cols[k]_i)) * NTT(lift(sparse_k)))),   out_i = relinearize(Y_i)
-with the oracle's own lift, transforms, floor and relinearisation, on the lazy FP64, canonical FP64 (CNHE_NO_LAZY) and integer
-(CNHE_NTT_INT, 53/56-bit moduli) paths, both m~ conventions, fast and SEAL Bsk, N = 4096 / 8192 / 16384, both key-switch paths.  K_c is
-checked against its derivation and pinned at the bound with constructed operands; the output decrypts to the existing call's values, the
-operation counts are the documented ones and every refusal leaves the output NULL."""
+with the oracle's own lift, transforms, floor and relinearisation, on the lazy FP64 and integer (CNHE_NTT_INT, 53/56-bit moduli) paths,
+both m~ conventions, fast and SEAL Bsk, N = 4096 / 8192 / 16384, both key-switch paths.  K_c is checked against its derivation and
+pinned at the bound with constructed operands; the output decrypts to the existing call's values, the operation counts are the documented
+ones and every refusal leaves the output NULL."""
 import ctypes as C
 
 import numpy as np
@@ -57,7 +57,7 @@ CONTEXTS = {
     "n16384": dict(t=[786433], N=16384, dbc=60, q=None),
     "n4096-q53": dict(t=[40961], N=4096, dbc=10, q=[_prime(53, 4096), _prime(56, 4096)]),
 }
-ENV = ("CNHE_AUX_BASE", "CNHE_NO_LAZY", "CNHE_NTT_INT", "CNHE_KS_FUSED", "CNHE_MUL_FUSED")
+ENV = ("CNHE_AUX_BASE", "CNHE_NTT_INT", "CNHE_KS_FUSED", "CNHE_MUL_FUSED")
 
 
 def _pair(name, monkeypatch, env=None):
@@ -161,7 +161,6 @@ def _check(eng, orcs, cols, sparse, out, blocks=None, mtilde=False):
 CASES = [  # (context, env, [(K, blocks)], m~ conventions)
     ("n4096", {}, [(1, 1), (2, 3), (100, 1)], (False, True)),
     ("n4096", {"CNHE_AUX_BASE": "seal"}, [(2, 3), (100, 1)], (False, True)),
-    ("n4096", {"CNHE_NO_LAZY": "1"}, [(2, 3), (30, 1)], (False,)),
     ("n4096", {"CNHE_NTT_INT": "1"}, [(2, 3), (30, 1)], (False, True)),
     ("n4096-q53", {}, [(2, 3), (30, 1)], (False,)),
     ("kc", {}, [(2, 1), ("Kc", 1), ("Kc+1", 1)], (False, True)),

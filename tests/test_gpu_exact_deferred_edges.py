@@ -17,7 +17,7 @@ from oracle.oracle_py import Oracle
 
 pytestmark = pytest.mark.gpu
 
-KERNEL_ENV = ("CNHE_MAC_NO_UMMA", "CNHE_MAC_NO_IMMA", "CNHE_MAC_INT", "CNHE_MUL_FUSED", "CNHE_KS_FUSED", "CNHE_NO_LAZY")
+KERNEL_ENV = ("CNHE_MAC_NO_UMMA", "CNHE_MAC_NO_IMMA", "CNHE_MAC_INT", "CNHE_MUL_FUSED", "CNHE_KS_FUSED")
 T = {4096: 40961, 8192: 786433}
 
 

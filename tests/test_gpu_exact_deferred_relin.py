@@ -18,7 +18,7 @@ CTX = {
     4096: dict(t=[40961], dbc=10),
     8192: dict(t=[549764251649, 549764284417], dbc=10),
 }
-KERNEL_ENV = ("CNHE_MAC_NO_UMMA", "CNHE_MAC_NO_IMMA", "CNHE_MAC_INT", "CNHE_MUL_FUSED", "CNHE_KS_FUSED", "CNHE_NO_LAZY")
+KERNEL_ENV = ("CNHE_MAC_NO_UMMA", "CNHE_MAC_NO_IMMA", "CNHE_MAC_INT", "CNHE_MUL_FUSED", "CNHE_KS_FUSED")
 
 
 def _engine(N, monkeypatch, dbc=None, t=None):

@@ -9,7 +9,7 @@ of 8), N = 4096 and 8192, the folded product at two fold widths, and the integer
 the profiler's launches of the diagonal MAC (family 4, FP64 path only).
 
 Summed tensor products: T = 8, 9, 33 and 255 identical terms on a 49-bit prime (K_c is unbounded there) and T = K_c = 256 on a 48-bit
-one, against the oracle restatement, on the lazy and canonical FP64 inputs and the integer k_behz_tensor_mac."""
+one, against the oracle restatement, on the lazy FP64 inputs and the integer k_behz_tensor_mac."""
 import numpy as np
 import pytest
 
@@ -21,7 +21,7 @@ pytestmark = pytest.mark.gpu
 T_PLAIN = 65537  # 1 mod 2N for N = 4096 and 8192
 WEIGHT = T_PLAIN - 3  # -3: w' = q - 3, so v w' / p is as large as v and fmodmul's rounding error is at its widest
 N1 = 64
-ENV = ("CNHE_AUX_BASE", "CNHE_NO_LAZY", "CNHE_NTT_INT", "CNHE_KS_FUSED", "CNHE_MUL_FUSED")
+ENV = ("CNHE_AUX_BASE", "CNHE_NTT_INT", "CNHE_KS_FUSED", "CNHE_MUL_FUSED")
 
 
 def _engine(monkeypatch, t, N, q, dbc=10, env=None, seed=31):
@@ -181,7 +181,7 @@ def test_integer_fallback_gives_the_same_words(mp):
 # ---------------------------------------------------------------- summed tensor products
 # "q49": one 49-bit prime, whose Bsk leaves K_c unbounded (2^31 - 1); "kc": one 48-bit prime and a 26-bit plaintext prime, K_c = 256
 TENSOR_CONTEXTS = {"q49": lambda N: W.primes(49, N, 1), "kc": lambda N: [_prime(48, N)]}
-TENSOR_ENV = {"lazy": {}, "canonical": {"CNHE_NO_LAZY": "1"}, "integer": {"CNHE_NTT_INT": "1"}}
+TENSOR_ENV = {"lazy": {}, "integer": {"CNHE_NTT_INT": "1"}}
 
 
 def _prime(bits, N):

@@ -167,15 +167,13 @@ def test_serve_batch_eight_clients_recorded_once_run_for_eight_others():
         f.Dispose()
 
 
-@pytest.mark.parametrize("form", ["fused", "digit", "nolazy", "int"])
+@pytest.mark.parametrize("form", ["fused", "digit", "int"])
 def test_every_key_reading_form(form, monkeypatch):
     """The fused key switch (packed relinearisation keys, u64 Galois keys), the digit path on lazy digits (one ciphertext per thread, the
-    copy-engine kernel's four per CTA, the per-ciphertext table of a two-client call) and on canonical digits (CNHE_NO_LAZY=1: one and four
-    ciphertexts per thread, the table), and the integer MAC (CNHE_NTT_INT=1), each word for word under a rebinding."""
+    copy-engine kernel's four per CTA, the per-ciphertext table of a two-client call), and the integer MAC (CNHE_NTT_INT=1), each word for
+    word under a rebinding."""
     from cryptonets_b200.networks import serve_batch
     monkeypatch.setenv("CNHE_KS_FUSED", "1" if form in ("fused", "int") else "0")
-    if form == "nolazy":
-        monkeypatch.setenv("CNHE_NO_LAZY", "1")
     if form == "int":
         monkeypatch.setenv("CNHE_NTT_INT", "1")
     f, (net, rd) = _factory("lola_small_rows", 1)
@@ -194,7 +192,7 @@ def test_every_key_reading_form(form, monkeypatch):
             for j in range(len(run)):
                 assert np.array_equal(_words(f, outs[j]), want[j]), (form, run, j)
             cap.Dispose()
-        if form in ("digit", "nolazy"):  # a key switch of at least 64 ciphertexts: four ciphertexts share each key load
+        if form == "digit":  # a key switch of at least 64 ciphertexts: four ciphertexts share each key load
             eng = f.engine
             a = eng.encrypt(np.arange(64 * eng.N, dtype=np.float64) % 7)
             a.set_key_slot(A)

@@ -1,6 +1,6 @@
 """The fused BEHZ square (forward transforms, tensor square and inverse transforms in one CTA-pair kernel, N = 4096 / 8192) against the
 separate kernels (CNHE_MUL_FUSED=0) bit for bit on every ciphertext and against the CPU oracle on sampled ones: size-3 products and
-multiply + relinearise.  Products of two different ciphertexts, CNHE_NO_LAZY and N = 16384 keep the separate kernels."""
+multiply + relinearise.  Products of two different ciphertexts, CNHE_NTT_INT and N = 16384 keep the separate kernels."""
 import os
 
 import numpy as np
@@ -122,7 +122,7 @@ def test_distinct_operands_keep_separate_kernels(pair, monkeypatch):
         eng.dev_free(p)
 
 
-@pytest.mark.parametrize("name,env", [("cryptonets8192", "CNHE_NO_LAZY"), ("default4096", "CNHE_NO_LAZY"), ("cifar16384", None)])
+@pytest.mark.parametrize("name,env", [("cryptonets8192", "CNHE_NTT_INT"), ("default4096", "CNHE_NTT_INT"), ("cifar16384", None)])
 def test_fallbacks_keep_separate_kernels(name, env, monkeypatch):
     cfg = dict(CONFIGS, cifar16384=dict(t=957181001729, N=16384, count=8, dbc_r=60, dbc_g=60))[name]
     if env:

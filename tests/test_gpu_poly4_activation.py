@@ -4,7 +4,7 @@ Every output word must equal the CPU oracle's composition, per plaintext prime, 
   quartic  q = poly2(x; 1, beta, gamma);  y = relin(A . q^2) + D' . x + E'
   cubic    u = relin(x^2);  q1 = u + x + gamma;  y = relin(lambda . (q1^2 - u^2)) + C' . x + D'
 (the size-3 difference formed here in numpy mod q_l; a term that is 0 mod the prime is skipped there), on every path the products take:
-fused square or separate kernels, fused or digit key switch, the lazy FP64, canonical FP64 and integer floors, N = 4096 / 8192 / 16384
+fused square or separate kernels, fused or digit key switch, the FP64 and integer floors, N = 4096 / 8192 / 16384
 and 53/56-bit moduli.  (1, 0, 0, 0, 0) is the square taken twice, the cubic relinearises once per output at its second level, mixed key
 slots give each client's words, and lola_small with its square replaced by a quartic or a cubic decrypts to the Raw backend."""
 import numpy as np
@@ -31,7 +31,6 @@ CONTEXTS = {
     "n8192-cryptonets": dict(t=[549764251649, 549764284417], N=8192, dbc=10, q=None, env={}),
     "n16384": dict(t=[786433], N=16384, dbc=60, q=None, env={}),
     "n8192-int": dict(t=[2277377, 2424833], N=8192, dbc=40, q=None, env={"CNHE_NTT_INT": "1"}),
-    "n8192-nolazy": dict(t=[549764251649], N=8192, dbc=10, q=None, env={"CNHE_NO_LAZY": "1"}),
     "n4096-q53": dict(t=[40961], N=4096, dbc=10, q=[_prime(53, 4096), _prime(56, 4096)], env={}),
 }
 PATHS = [dict(CNHE_MUL_FUSED="1", CNHE_KS_FUSED="1"), dict(CNHE_MUL_FUSED="0", CNHE_KS_FUSED="0"), dict(CNHE_MUL_FUSED="1", CNHE_KS_FUSED="0"),
@@ -42,8 +41,7 @@ def _pair(name, monkeypatch):
     from cryptonets_b200.engine import Engine
     from oracle.oracle_py import Oracle
     cfg = CONTEXTS[name]
-    for var in ("CNHE_NTT_INT", "CNHE_NO_LAZY"):
-        monkeypatch.delenv(var, raising=False)
+    monkeypatch.delenv("CNHE_NTT_INT", raising=False)
     for var, v in cfg["env"].items():
         monkeypatch.setenv(var, v)
     eng = Engine(cfg["t"], cfg["N"], cfg["dbc"], 20, -1, coeff_moduli=cfg["q"])

@@ -45,13 +45,12 @@ def _prime(bits, N):
 
 
 # name: plain primes, N, decomposition bit count, coefficient moduli (None: the default), environment at context creation (CNHE_NTT_INT:
-# the integer floor k_behz_floor; CNHE_NO_LAZY: canonical buffers between the product's kernels, so the FP64 floor k_behz_floor_fp)
+# the integer floor k_behz_floor)
 CONTEXTS = {
     "n4096": dict(t=[40961], N=4096, dbc=10, q=None, env={}),
     "n8192-cryptonets": dict(t=[549764251649, 549764284417], N=8192, dbc=10, q=None, env={}),
     "n16384": dict(t=[786433], N=16384, dbc=60, q=None, env={}),
     "n8192-int": dict(t=[2277377, 2424833], N=8192, dbc=40, q=None, env={"CNHE_NTT_INT": "1"}),
-    "n8192-nolazy": dict(t=[549764251649], N=8192, dbc=10, q=None, env={"CNHE_NO_LAZY": "1"}),
     "n4096-q53": dict(t=[40961], N=4096, dbc=10, q=[_prime(53, 4096), _prime(56, 4096)], env={}),
 }
 
@@ -60,8 +59,7 @@ def _pair(name, monkeypatch):
     from cryptonets_b200.engine import Engine
     from oracle.oracle_py import Oracle
     cfg = CONTEXTS[name]
-    for var in ("CNHE_NTT_INT", "CNHE_NO_LAZY"):
-        monkeypatch.delenv(var, raising=False)
+    monkeypatch.delenv("CNHE_NTT_INT", raising=False)
     for var, v in cfg["env"].items():
         monkeypatch.setenv(var, v)
     eng = Engine(cfg["t"], cfg["N"], cfg["dbc"], 20, -1, coeff_moduli=cfg["q"])

@@ -32,7 +32,7 @@ CONTEXTS = {
     "n2048-mixed": dict(t=40961, N=2048, q=_cp(61, 2048) + _cp(30, 2048) + _cp(57, 2048) + _cp(60, 2048), dbc=(10, 20), env={}),
     "n4096-61-seal": dict(t=40961, N=4096, q=_cp(61, 4096, 2), dbc=(10, 20), env={"CNHE_AUX_BASE": "seal"}),
 }
-ENV = ("CNHE_AUX_BASE", "CNHE_NO_LAZY", "CNHE_NTT_INT", "CNHE_KS_FUSED", "CNHE_MUL_FUSED")
+ENV = ("CNHE_AUX_BASE", "CNHE_NTT_INT", "CNHE_KS_FUSED", "CNHE_MUL_FUSED")
 SEED = 1234
 
 
